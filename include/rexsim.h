@@ -165,6 +165,9 @@ int rexsim_clear_errors(RexSim* sim, void* stream);          /* zeroes the aggre
 int rexsim_last_command(RexSim* sim, float** cmd);
 /* kernels launched by this handle since create (the bench reports it) */
 int64_t rexsim_launch_count(const RexSim* sim);
+/* which build of the step kernel the last rexsim_step / rexsim_step_host launched (all 0 before the first step): CTA size,
+ * resident CTAs per SM it is compiled for (1: 255 registers, 4: 128 registers), 1 if the sensor model is compiled in */
+int rexsim_last_step_build(const RexSim* sim, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor);
 /* the counter-based generator behind every reset draw (replaces Python's unseeded `random`,
  * walk_env.py:133-147, gallop_env.py:151, turn_env.py:138,147); host-callable so tests can pin it */
 uint32_t rexsim_rand_u32(uint64_t seed, uint32_t global_env, uint32_t reset_count, uint32_t slot);

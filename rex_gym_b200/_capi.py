@@ -40,7 +40,7 @@ AGENT_EXPORTS = ["rexagent_policy_floats", "rexagent_value_floats", "rexagent_cr
 
 EXPORTS = ["rexsim_obs_dim", "rexsim_action_dim", "rexsim_state_words", "rexsim_create", "rexsim_destroy",
            "rexsim_step", "rexsim_step_host", "rexsim_host_out_bytes", "rexsim_rebalance", "rexsim_reset", "rexsim_get_state", "rexsim_set_state", "rexsim_state_buffers",
-           "rexsim_error_flags", "rexsim_clear_errors", "rexsim_last_command", "rexsim_launch_count", "rexsim_last_error", "rexsim_rand_u32",
+           "rexsim_error_flags", "rexsim_clear_errors", "rexsim_last_command", "rexsim_launch_count", "rexsim_last_step_build", "rexsim_last_error", "rexsim_rand_u32",
            "rexsim_noise", "rexsim_history_depth", "rexsim_history_buffer"]
 
 _LIB = None
@@ -79,6 +79,7 @@ def load():
     L.rexsim_last_command.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
     L.rexsim_launch_count.argtypes = [C.c_void_p]
     L.rexsim_launch_count.restype = C.c_int64
+    L.rexsim_last_step_build.argtypes = [C.c_void_p] + [C.POINTER(C.c_int32)] * 3
     L.rexsim_last_error.restype = C.c_char_p
     L.rexsim_rand_u32.argtypes = [C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32]
     L.rexsim_rand_u32.restype = C.c_uint32

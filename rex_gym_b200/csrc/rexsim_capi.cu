@@ -37,6 +37,7 @@ struct RexSim {
     int A = 0, O = 0;
     int nsnap = 1;
     int64_t launches = 0;
+    int32_t launched[3] = {0, 0, 0};   // step_kernel instance of the last step launch: BLOCK, OCC, SENSOR
 };
 
 static thread_local char g_err[512] = "";
@@ -174,6 +175,7 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
     s->P.snap_f = s->d_snap_f; s->P.snap_i = s->d_snap_i; s->P.field_zoff = s->d_zoff;
     s->P.err = s->d_err; s->P.cmd_out = s->d_cmd;
     s->P.cost = s->d_cost; s->P.perm = nullptr;
+    s->P.launched = s->launched;
     // settled reset snapshots: Rex.Reset's 100 + 0.5/dt holding sub-steps (rex.py:314-323), once per field
     for (int f = 0; f < s->nsnap; f++) {
         s->P.settle_snapshot = f;
@@ -319,6 +321,11 @@ int rexsim_last_command(RexSim* s, float** cmd) {
     return REXSIM_OK;
 }
 int64_t rexsim_launch_count(const RexSim* s) { return s ? s->launches : 0; }
+int rexsim_last_step_build(const RexSim* s, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor) {
+    if (!s || !cta_threads || !ctas_per_sm || !sensor) return fail(REXSIM_ERR_INVALID, "null argument");
+    *cta_threads = s->launched[0]; *ctas_per_sm = s->launched[1]; *sensor = s->launched[2];
+    return REXSIM_OK;
+}
 uint32_t rexsim_rand_u32(uint64_t seed, uint32_t global_env, uint32_t reset_count, uint32_t slot) {
     return rand_u32(seed, global_env, reset_count, slot);
 }

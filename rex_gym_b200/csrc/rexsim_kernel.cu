@@ -1944,6 +1944,7 @@ static cudaError_t launch_step_variant(const Params& P, cudaStream_t st) {
         }
     }
     kern<<<blocks, BLOCK, smem, st>>>(P);
+    if (P.launched) { P.launched[0] = BLOCK; P.launched[1] = OCC; P.launched[2] = SENSOR; }
     return cudaGetLastError();
 }
 template <int TASK, int SIGNAL, int TERRAIN, bool ARM>

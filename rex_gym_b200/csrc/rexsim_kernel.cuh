@@ -71,6 +71,7 @@ struct Params {
     int32_t settle_snapshot;           // settle kernel: which snapshot this launch produces
     int32_t N;
     int32_t sm_count;                  // SMs of the device (kernel variant choice)
+    int32_t* launched;                 // host: {BLOCK, OCC, SENSOR} of the step_kernel instance the last step launched (never read on the device)
     const int32_t* __restrict__ perm;  // [N] slot -> env (null: identity); see rexsim_rebalance
     int32_t* __restrict__ cost;        // [N] solver iterations of the last control step
     // sensor model (control / PD latency, observation noise: rex.py:735-769); all unused when sensor_on == 0

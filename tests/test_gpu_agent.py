@@ -20,7 +20,8 @@ def _random_weights(rng, O, A, H1=200, H2=100):
     return w
 
 
-@pytest.mark.parametrize("O,A,n", [(4, 2, 4096), (16, 4, 1000), (4, 1, 77), (16, 2, 65536), (8, 3, 300), (4, 5, 129)])
+@pytest.mark.parametrize("O,A,n", [(4, 2, 4096), (16, 4, 1000), (4, 1, 77), (16, 2, 65536), (8, 3, 300), (4, 5, 129),
+                                   (4, 8, 1000), (16, 3, 333)])       # one case per compiled perform_tc_kernel<O, A> (A = 0: any width)
 def test_perform_on_the_tensor_cores(O, A, n):
     """tensor_cores=True: layer 2 as wgmma tf32 (operands rounded to 11 significant bits, fp32 accumulation in
     registers).  Against the fp64 oracle and against the fp32 kernel on the same inputs: mean (after tanh) and value within 5e-3
@@ -119,6 +120,60 @@ def test_experience_updates_both_filters_like_the_reference():
     g2 = net2.get_filters()
     np.testing.assert_array_equal(g2["observ_var_sum"], net.get_filters()["observ_var_sum"])
     net.close(); net2.close()
+
+
+def test_experience_in_partial_sums_matches_one_batch():
+    """The env-sharded form of experience (rexagent_experience_partial -> sum over the ranks -> rexagent_experience_finalize) on one
+    GPU: two half batches' partial sums, added on the device, finalised for the whole batch.  Partials leave the filters and
+    counters alone; the result matches the oracle and a single experience call on the whole batch; the perform noise step advances
+    once; a plain experience call afterwards still updates correctly."""
+    from rex_gym_b200 import _capi
+    from rex_gym_b200.agents import ForwardGaussianPolicy
+    rng = np.random.default_rng(8)
+    O, A, n = 16, 4, 5001
+    h = 2600                                          # unequal halves, both spread over several reduction blocks
+    a, b = ForwardGaussianPolicy(O, A, seed=1), ForwardGaussianPolicy(O, A, seed=1)
+    fo, fr = AO.StreamingNormalize((O,), True, True, 5), AO.StreamingNormalize((), False, True, 10)
+
+    def batch(m):
+        obs = rng.normal(0.5, 2.0, (m, O)).astype(np.float32); rew = rng.normal(0.1, 0.3, (m,)).astype(np.float32)
+        return obs, rew, torch.from_numpy(obs).cuda(), torch.from_numpy(rew).cuda()
+
+    def assert_filters(g, count):
+        assert g["observ_count"] == g["reward_count"] == fo.count == fr.count == count
+        np.testing.assert_allclose(g["observ_mean"], fo.mean, rtol=2e-5, atol=2e-6)
+        np.testing.assert_allclose(g["observ_var_sum"], fo.var_sum, rtol=5e-5, atol=1e-5)
+        np.testing.assert_allclose(g["reward_mean"], fr.mean, rtol=2e-5, atol=2e-6)
+        np.testing.assert_allclose(g["reward_var_sum"], fr.var_sum, rtol=5e-5, atol=1e-5)
+
+    obs, rew, x, r = batch(777)                       # a non-zero mean first: the partials are centred on it
+    a.experience(x, r); b.experience(x, r); fo.update(obs); fr.update(rew)
+    before, cnt_before = a.get_filters(), a._cnt.clone()
+    obs, rew, x, r = batch(n)
+    s = [torch.zeros((O + 1, 2), dtype=torch.float32, device="cuda") for _ in range(2)]
+    st = a._stream()
+    _capi.check(a._L.rexagent_experience_partial(a._h, x.data_ptr(), r.data_ptr(), h, s[0].data_ptr(), st))
+    _capi.check(a._L.rexagent_experience_partial(a._h, x[h:].data_ptr(), r[h:].data_ptr(), n - h, s[1].data_ptr(), st))
+    g = a.get_filters()
+    assert torch.equal(a._cnt, cnt_before)
+    for k in before:
+        np.testing.assert_array_equal(g[k], before[k])
+    total = s[0] + s[1]
+    _capi.check(a._L.rexagent_experience_finalize(a._h, total.data_ptr(), n, x.data_ptr(), r.data_ptr(), st))
+    b.experience(x, r); fo.update(obs); fr.update(rew)
+    ga, gb = a.get_filters(), b.get_filters()
+    assert_filters(ga, 777 + n)
+    for k in ("observ_mean", "observ_var_sum"):
+        np.testing.assert_allclose(ga[k], gb[k], rtol=1e-5, atol=1e-6)
+    assert int(a._cnt[2]) == int(b._cnt[2]) == 2 and int(a._cnt[3]) == 0
+    # the noise of the next perform is keyed on the step counter: the same draws as after the single call
+    pa, pb = a.perform(x[:300], training=True, seed=4), b.perform(x[:300], training=True, seed=4)
+    np.testing.assert_allclose((pa["action"] - pa["mean"]).cpu().numpy(), (pb["action"] - pb["mean"]).cpu().numpy(), atol=1e-6)
+    obs, rew, x, r = batch(4099)
+    a.experience(x, r); fo.update(obs); fr.update(rew)
+    assert_filters(a.get_filters(), 777 + n + 4099)
+    assert int(a._cnt[2]) == 3
+    a.close(); b.close()
 
 
 def test_scans_match_the_oracle_in_both_layouts():

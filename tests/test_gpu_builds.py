@@ -1,0 +1,341 @@
+"""GPU: every build of the step kernel the dispatcher can launch, against the fp64 oracle (called through the C ABI).
+
+`step_kernel<TASK, SIGNAL, TERRAIN, OCC, ARM, SENSOR, BLOCK>` (rex_gym_b200/csrc/rexsim_kernel.cu) exists in three builds for each
+(task, signal, terrain, arm); `launch_step_tsta` picks one on every step launch:
+
+  sensor  any control / PD latency or observation noise > 0        255 registers, 128-thread CTAs
+  big     no sensor model, no arm, and ceil(N / 32) > 2 x SMs on    128 registers (REXSIM_OCC_BIG), 256-thread CTAs
+          flat ground, > 4 x SMs on heightfields                    (REXSIM_BLOCK_BIG); on heightfields its 64 tiles per CTA
+          (H100 SXM, 132 SMs: N > 8448 / N > 16 896)                take 78 KB of shared memory through the opt-in
+  small   everything else                                           255 registers, 128-thread CTAs
+
+REXSIM_FORCE_BUILD=big|small replaces the size rule (arm batches stay on the small build); it is read on every step launch and
+does not touch the reset or settle kernels.
+
+INSTANCES is the table of reachable instances: 8 (task, signal) units x 2 terrains x 3 builds, plus the two arm units (walk-ik,
+standup) x 2 terrains x the small and sensor builds = 56 rows.  test_instance_against_the_oracle[<row id>] runs every row; the last
+column names the other tests of the suite that launch the same instance.
+"""
+import ctypes
+import os
+
+import numpy as np
+import pytest
+import torch
+
+import test_gpu_parity as P
+from test_gpu_parity import TOL_P, TOL_Q, _bound, _env, _oracle, _oracle_state, _toe_mask
+
+FR, HF, SA = "test_gpu_parity::test_free_running_rollout", "test_gpu_parity::test_heightfield_contact_parity", "test_gpu_parity::test_sensor_latency_and_noise"
+BL, WARP = "test_gpu_parity::test_baseline_size_batches_against_the_oracle", "test_gpu_parity::test_batches_that_do_not_fill_their_last_warp"
+REGROUP, HOST = ("test_gpu_parity::test_warp_regrouping_does_not_change_any_result_on_the_128_register_build",
+                 "test_gpu_parity::test_numpy_and_device_paths_agree_beyond_the_zero_copy_limit")
+NATURAL, SWITCH = "test_gpu_builds::test_heightfield_big_build_at_its_natural_size", "test_gpu_builds::test_the_dispatcher_switches_builds_at_its_thresholds"
+
+#  task      signal arm    terrain   build     also launched by
+INSTANCES = [
+    ("walk",    "ik", False, "plane",  "small",  (FR,)),
+    ("walk",    "ik", False, "plane",  "big",    (BL + "[C2]", REGROUP, HOST, SWITCH)),
+    ("walk",    "ik", False, "plane",  "sensor", (SA,)),
+    ("walk",    "ik", False, "random", "small",  (WARP,)),
+    ("walk",    "ik", False, "random", "big",    ()),
+    ("walk",    "ik", False, "random", "sensor", (SA,)),
+    ("walk",    "ol", False, "plane",  "small",  (FR,)),
+    ("walk",    "ol", False, "plane",  "big",    ()),
+    ("walk",    "ol", False, "plane",  "sensor", ()),
+    ("walk",    "ol", False, "random", "small",  ()),
+    ("walk",    "ol", False, "random", "big",    ()),
+    ("walk",    "ol", False, "random", "sensor", ()),
+    ("gallop",  "ik", False, "plane",  "small",  (FR,)),
+    ("gallop",  "ik", False, "plane",  "big",    ()),
+    ("gallop",  "ik", False, "plane",  "sensor", ()),
+    ("gallop",  "ik", False, "random", "small",  ()),
+    ("gallop",  "ik", False, "random", "big",    ()),
+    ("gallop",  "ik", False, "random", "sensor", ()),
+    ("gallop",  "ol", False, "plane",  "small",  (FR,)),
+    ("gallop",  "ol", False, "plane",  "big",    (BL + "[C3]",)),
+    ("gallop",  "ol", False, "plane",  "sensor", (SA,)),
+    ("gallop",  "ol", False, "random", "small",  ()),
+    ("gallop",  "ol", False, "random", "big",    ()),
+    ("gallop",  "ol", False, "random", "sensor", ()),
+    ("turn",    "ik", False, "plane",  "small",  (FR,)),
+    ("turn",    "ik", False, "plane",  "big",    ()),
+    ("turn",    "ik", False, "plane",  "sensor", (SA,)),
+    ("turn",    "ik", False, "random", "small",  (HF, BL + "[C4]")),
+    ("turn",    "ik", False, "random", "big",    (NATURAL, SWITCH)),
+    ("turn",    "ik", False, "random", "sensor", ()),
+    ("turn",    "ol", False, "plane",  "small",  (FR,)),
+    ("turn",    "ol", False, "plane",  "big",    ()),
+    ("turn",    "ol", False, "plane",  "sensor", ()),
+    ("turn",    "ol", False, "random", "small",  ()),
+    ("turn",    "ol", False, "random", "big",    ()),
+    ("turn",    "ol", False, "random", "sensor", ()),
+    ("standup", "ol", False, "plane",  "small",  (FR,)),
+    ("standup", "ol", False, "plane",  "big",    ()),
+    ("standup", "ol", False, "plane",  "sensor", ()),
+    ("standup", "ol", False, "random", "small",  ()),
+    ("standup", "ol", False, "random", "big",    ()),
+    ("standup", "ol", False, "random", "sensor", ()),
+    ("poses",   "ik", False, "plane",  "small",  (FR,)),
+    ("poses",   "ik", False, "plane",  "big",    ()),
+    ("poses",   "ik", False, "plane",  "sensor", (SA,)),
+    ("poses",   "ik", False, "random", "small",  ()),
+    ("poses",   "ik", False, "random", "big",    ()),
+    ("poses",   "ik", False, "random", "sensor", ()),
+    ("walk",    "ik", True,  "plane",  "small",  (FR,)),
+    ("walk",    "ik", True,  "plane",  "sensor", ()),
+    ("walk",    "ik", True,  "random", "small",  ()),
+    ("walk",    "ik", True,  "random", "sensor", ()),
+    ("standup", "ol", True,  "plane",  "small",  (FR, BL + "[C5]")),
+    ("standup", "ol", True,  "plane",  "sensor", (SA,)),
+    ("standup", "ol", True,  "random", "small",  ()),
+    ("standup", "ol", True,  "random", "sensor", ()),
+]
+UNITS = [("walk", "ik"), ("walk", "ol"), ("gallop", "ik"), ("gallop", "ol"), ("turn", "ik"), ("turn", "ol"), ("standup", "ol"), ("poses", "ik")]
+ARM_UNITS = [("walk", "ik"), ("standup", "ol")]          # launch_step_ts: HAS_ARM
+
+
+BUILDS = {"small": (128, 1, 0), "big": (256, 4, 0), "sensor": (128, 1, 1)}     # (CTA size, CTAs per SM, sensor) of each build
+
+
+def _row_id(row):
+    task, sig, arm, terrain, build, _ = row
+    return "-".join([task, sig] + (["arm"] if arm else []) + [terrain, build])
+
+
+def test_instance_table_lists_every_reachable_instance():
+    """CPU: the table above is the dispatch rule's whole image -- no instance missing, none listed twice, no arm row on the big
+    build -- and every test it names exists."""
+    want = {(t, s, arm, ter, b) for arm, units in ((False, UNITS), (True, ARM_UNITS)) for t, s in units
+            for ter in ("plane", "random") for b in (("small", "sensor") if arm else ("small", "big", "sensor"))}
+    got = [r[:5] for r in INSTANCES]
+    assert len(got) == len(set(got)) == len(want) == 56
+    assert set(got) == want
+    here = os.path.dirname(os.path.abspath(__file__))
+    for row in INSTANCES:
+        for ref in row[5]:
+            mod, name = ref.split("[")[0].split("::")
+            assert ("def %s(" % name) in open(os.path.join(here, mod + ".py")).read(), ref
+
+
+def _launched(env):
+    """(CTA size, CTAs per SM, sensor) of the step_kernel instance env's last step launched (rexsim_last_step_build)."""
+    v = [ctypes.c_int32() for _ in range(3)]
+    assert env._L.rexsim_last_step_build(env._h, *[ctypes.byref(x) for x in v]) == 0
+    return tuple(x.value for x in v)
+
+
+def _config(task, sig, arm, terrain, build):
+    kw = dict(signal_type=sig, seed=13, max_episode_steps=15)         # short episodes: every env runs the in-kernel reset twice
+    if arm:
+        kw["mark"] = "arm"
+    if (task, sig) == ("gallop", "ol"):
+        kw.update(motor_kp_range=(0.8, 1.2), motor_kd_range=(0.01, 0.03))
+    if terrain == "random":
+        kw.update(terrain_type="random", num_fields=4)
+    if build == "sensor":
+        kw["control_latency"] = 0.0125                                # a blend of two history rows, 12 sub-steps back
+    return kw
+
+
+def _sync_to_oracle(env, ora, idx):
+    """Overwrite the physical state of envs `idx` with the oracle's (the rest of the batch is written back unchanged)."""
+    st, so = env.get_state(), _oracle_state(ora, env.num_envs)
+    for k in ("pos", "quat", "linvel", "angvel", "q", "qd"):
+        st[k][idx] = so[k][idx]
+    env.set_state(st["pos"], st["quat"], st["linvel"], st["angvel"], st["q"], st["qd"])
+
+
+def _assert_bookkeeping(env, ora, sg, task, rough):
+    """Everything integer after a step, bit for bit: counters, resets, field ids, the draws of every reset."""
+    n = env.num_envs
+    E = [ora.env(i) for i in range(n)]
+    sf, si = env._state_f.cpu().numpy(), env._state_i.cpu().numpy()
+    np.testing.assert_array_equal(sg["step_counter"], [e.step_counter for e in E])
+    np.testing.assert_array_equal(sg["env_step_counter"], [e.env_step_counter for e in E])
+    np.testing.assert_array_equal(si[3], [e.reset_count for e in E])                                  # I_RESETCNT
+    if rough:
+        np.testing.assert_array_equal(si[4], [e.field_id for e in E])                                 # I_FIELD
+    tgt = [e.target_value if task == "poses" else e.target_position for e in E]
+    np.testing.assert_array_equal(sf[38], np.array(tgt, np.float32))                                  # F_TARGET
+    np.testing.assert_array_equal(sf[39], np.array([e.target_orient for e in E], np.float32))         # F_TORIENT
+    np.testing.assert_array_equal(sf[41], np.array([e.kp for e in E], np.float32))                    # F_KP
+    np.testing.assert_array_equal(sf[42], np.array([e.kd for e in E], np.float32))                    # F_KD
+    np.testing.assert_array_equal((si[2] >> 3) & 1, [e.backwards for e in E])
+    np.testing.assert_array_equal((si[2] >> 4) & 1, [e.clockwise for e in E])
+    if task == "poses":
+        np.testing.assert_array_equal((si[2] >> 26) & 7, [e.next_pose for e in E])                   # FL_POSE_SHIFT
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("row", INSTANCES, ids=[_row_id(r) for r in INSTANCES])
+def test_instance_against_the_oracle(monkeypatch, row):
+    """One instance, forced by REXSIM_FORCE_BUILD (the sensor build by its config; rexsim_last_step_build confirms which one ran
+    every step), against the oracle: 37 envs (padding lanes in
+    both CTA sizes), 40 control steps of random actions inside the task's bound, auto-reset after 15 steps.  Integer results bit
+    for bit after every step; continuous ones within the bounds the small build meets elsewhere in the suite:
+      flat-ground locomotion  test_free_running_rollout's strict window (90th percentile of the envs within 1e-3 rad / 1e-3 m,
+                              none beyond 5e-2 / 5e-3; motor commands 5e-4, rewards 5e-3);
+      standup, arm            its standup bounds (5e-3 / 2e-3 at the 90th percentile), from the oracle's settled state;
+      heightfields            test_heightfield_contact_parity's (1e-3 / 1e-3 at the 90th percentile, none beyond 2e-2 / 5e-3), from
+                              the oracle's settled state (toes creep on block edges while settling);
+    roll / pitch observations as in test_baseline_size_batches_against_the_oracle, toe contact masks in 98 % of the samples that
+    are not the first of an episode.
+    Where the state starts from the oracle's, every auto-reset lands within the settle bounds and is re-synchronised."""
+    task, sig, arm, terrain, build, _ = row
+    if build == "sensor":
+        monkeypatch.delenv("REXSIM_FORCE_BUILD", raising=False)
+    else:
+        monkeypatch.setenv("REXSIM_FORCE_BUILD", build)
+    n, steps = 37, 40
+    kw = _config(task, sig, arm, terrain, build)
+    env, ora = _env(task, n, auto_reset=True, **kw), _oracle(task, n, **kw)
+    env.reset(); ora.reset()
+    rough, standup = terrain == "random", task == "standup" or arm
+    resync = rough or standup
+    tol_q, tol_p = (5e-3, 2e-3) if standup else (TOL_Q, TOL_P)                     # test_free_running_rollout
+    max_q, max_p = (2e-2, 5e-3) if rough and not standup else (5e-2, 5e-3)
+    ta = 5e-3 if (rough or standup) else 1e-3                                      # roll / pitch observations
+    if resync:
+        _sync_to_oracle(env, ora, np.arange(n))
+    rng = np.random.default_rng(11)
+    b = _bound(task, sig)
+    err_rp, contact_total, contact_bad = [], 0, 0
+    for k in range(steps):
+        a = rng.uniform(-b, b, size=(n, env.action_dim)).astype(np.float32)
+        og, rg, dg, _ = env.step(a)
+        assert _launched(env) == BUILDS[build], _launched(env)
+        oc, rc, dc = ora.step(a)
+        np.testing.assert_array_equal(dg, dc, err_msg=f"done, step {k}")
+        cmd = env.last_command().cpu().numpy()[:12].T
+        ocmd = np.array([np.array(ora.env(i).cmd[:12]) for i in range(n)])
+        idx = np.nonzero(dc)[0]
+        if len(idx):
+            oc[idx] = ora.reset(idx)                      # the oracle has no auto-reset: the same semantics by hand
+        sg, so = env.get_state(), _oracle_state(ora, n)
+        _assert_bookkeeping(env, ora, sg, task, rough)
+        fresh = np.zeros(n, bool)
+        fresh[idx] = True
+        cmp = ~fresh if resync else np.ones(n, bool)
+        eq = np.abs(sg["q"] - so["q"]).max(axis=1)
+        ep = np.abs(sg["pos"] - so["pos"]).max(axis=1)
+        if not rough:
+            ep = np.maximum(ep, np.abs(sg["quat"] - so["quat"]).max(axis=1))
+        if resync and len(idx):
+            # the in-kernel reset restarts from the CUDA settle: test_reset_settle_and_draws' loosest bounds (standup with the arm)
+            assert eq[idx].max() < 3e-2 and ep[idx].max() < 2e-3, f"reset, step {k}: {eq[idx].max():.2e} {ep[idx].max():.2e}"
+        eq, ep = eq[cmp], ep[cmp]
+        if len(eq):
+            assert np.percentile(eq, 90) < tol_q and np.percentile(ep, 90) < tol_p, f"step {k}: {eq.max():.2e} {ep.max():.2e}"
+            assert eq.max() < max_q and ep.max() < max_p, f"step {k}: {eq.max():.2e} {ep.max():.2e}"
+            # a re-synchronised sensor build reads its own settle's history rows for the first 3 control steps of an episode
+            ocmp = cmp & (sg["env_step_counter"] >= 3) if (resync and build == "sensor") else cmp
+            err_rp.append(np.abs(og[ocmp, :2] - oc[ocmp, :2]).max(axis=1))
+        if not rough:
+            assert np.abs(cmd - ocmd).max() < 5e-4, f"cmd step {k}"     # the controller half: fp32 IK / Bezier vs fp64
+            rcmp = np.ones(n, bool)
+            if task == "standup":      # the standup reward jumps by 1 where the base crosses z = 0.21 or the L1 distance 0.1
+                l1 = np.abs(so["pos"][:, 0]) + np.abs(so["pos"][:, 1]) + np.abs(0.21 - so["pos"][:, 2])
+                rcmp &= (np.abs(so["pos"][:, 2] - 0.21) > 2e-3) & (np.abs(l1 - 0.1) > 2e-3) & ~fresh
+            np.testing.assert_allclose(rg[rcmp], rc[rcmp], atol=5e-3, err_msg=f"reward, step {k}")
+        # the mask of contacts in the last sub-step: after a reset the CUDA path reports none yet, the oracle its settle's last
+        cm = np.array([_toe_mask(ora, i) for i in range(n)])
+        contact_total += (~fresh).sum(); contact_bad += ((cm != sg["contact_mask"]) & ~fresh).sum()
+        if resync and len(idx):
+            _sync_to_oracle(env, ora, idx)
+    err_rp = np.concatenate(err_rp)
+    assert np.percentile(err_rp, 90) < ta / 5 and err_rp.max() < (2e-2 if rough else ta), (np.percentile(err_rp, 90), err_rp.max())
+    assert contact_bad <= 0.02 * max(contact_total, 1), (contact_bad, contact_total)
+    assert env.check_errors() == 0
+    env.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("build", ["small", "big"])
+@pytest.mark.parametrize("task,sig,kw,bound", [("walk", "ik", dict(target_position=2.0, backwards=False), 0.4),
+                                               ("standup", "ol", dict(), 0.1)], ids=["walk-ik", "standup-ol"])
+def test_one_step_is_tight_in_both_builds(monkeypatch, build, task, sig, kw, bound):
+    """test_one_step_is_tight (30 single control steps from an oracle-synchronised state) with the build forced: the big build
+    meets the same rounding-level bounds as the small one."""
+    monkeypatch.setenv("REXSIM_FORCE_BUILD", build)
+    P.test_one_step_is_tight(task, sig, kw, bound)
+
+
+@pytest.mark.gpu
+def test_heightfield_big_build_at_its_natural_size():
+    """test_baseline_size_batches_against_the_oracle's window on a heightfield batch large enough for the dispatcher to pick the big
+    build by itself (turn-ik, 64 fields, 32 768 envs: ceil(N / 32) = 1024 > 4 x SMs), so the 78 KB shared-memory opt-in and the
+    64-tile-per-CTA indexing run as a user's batch runs them.  48 consecutive envs from the middle of the batch are re-simulated by
+    the fp64 oracle (same global env ids): draws and done bit for bit; the window starts from the oracle's settled state, and its
+    base position and joint angles stay within test_heightfield_contact_parity's bounds, its roll / pitch observations within the
+    C4 bounds, over 40 control steps."""
+    n, w0, nw, steps = 32768, 32768 // 2 + 37, 48, 40
+    assert -(-n // 32) > 4 * torch.cuda.get_device_properties(0).multi_processor_count       # really above the switch
+    kw = dict(signal_type="ik", terrain_type="random", num_fields=64, normalize=True, seed=11)
+    env, ora = _env("turn", n, **kw), _oracle("turn", nw, env_offset=w0, **kw)
+    env.reset(); ora.reset()
+    sf, si = env._state_f.cpu().numpy()[:, w0:w0 + nw], env._state_i.cpu().numpy()[:, w0:w0 + nw]
+    np.testing.assert_array_equal(si[4], [ora.env(i).field_id for i in range(nw)])
+    np.testing.assert_array_equal(sf[39], np.array([ora.env(i).target_orient for i in range(nw)], np.float32))
+    np.testing.assert_array_equal((si[2] >> 4) & 1, [ora.env(i).clockwise for i in range(nw)])
+    st, so = env.get_state(), _oracle_state(ora, nw)
+    for k in ("pos", "quat", "linvel", "angvel", "q", "qd"):
+        st[k][w0:w0 + nw] = so[k]
+    env.set_state(st["pos"], st["quat"], st["linvel"], st["angvel"], st["q"], st["qd"])
+    g = torch.Generator(device="cuda"); g.manual_seed(5)
+    acts = torch.rand((steps, n, env.action_dim), device="cuda", generator=g) * 2 - 1
+    err, bad = [], 0
+    for k in range(steps):
+        o, r, d, _ = env.step(acts[k])
+        oc, rc, dc = ora.step(acts[k, w0:w0 + nw].cpu().numpy())
+        np.testing.assert_array_equal(d[w0:w0 + nw].cpu().numpy(), dc)
+        err.append(np.abs(o[w0:w0 + nw, :2].cpu().numpy() - oc[:, :2]).max(axis=1))
+        sg, so = env.get_state(), _oracle_state(ora, nw)
+        eq = np.abs(sg["q"][w0:w0 + nw] - so["q"]).max(1)
+        ep = np.abs(sg["pos"][w0:w0 + nw] - so["pos"]).max(1)
+        assert np.percentile(eq, 90) < TOL_Q and np.percentile(ep, 90) < TOL_P and eq.max() < 2e-2 and ep.max() < 5e-3, \
+            f"step {k}: {np.percentile(eq, 90):.2e} {np.percentile(ep, 90):.2e} {eq.max():.2e} {ep.max():.2e}"
+        bad += (np.array([_toe_mask(ora, i) for i in range(nw)]) != sg["contact_mask"][w0:w0 + nw]).sum()
+    err = np.concatenate(err) * (2 * np.pi + 0.01)                      # RangeNormalize'd -> radians
+    assert np.percentile(err, 90) < 1e-3 and err.max() < 2e-2, (np.percentile(err, 90), err.max())
+    assert bad <= 0.02 * steps * nw
+    assert (env.check_errors() & 1) == 0
+    env.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("terrain,per_sm", [("plane", 2), ("random", 4)])
+def test_the_dispatcher_switches_builds_at_its_thresholds(monkeypatch, terrain, per_sm):
+    """The size rule pinned where it switches: ceil(N / 32) > 2 x SMs on flat ground, > 4 x SMs on heightfields.  At the threshold
+    the unforced batch launches the same kernel as one forced onto the small build and is bit-identical to it over 12 steps (with
+    auto-resets); one env above it, the same holds with the big build.  The forced batches launch different instances (128-thread
+    CTAs at 1 CTA per SM, 256-thread CTAs at 4), so neither identity holds by accident: the two builds can agree bit for bit
+    (walk-ik and turn-ik do on an H100)."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    threshold = 32 * per_sm * sms                     # the largest N that stays on the small build
+    task = "walk" if terrain == "plane" else "turn"
+    kw = dict(signal_type="ik", auto_reset=True, max_episode_steps=10, normalize=True, seed=7)
+    if terrain == "random":
+        kw.update(terrain_type="random", num_fields=4)
+    for n, picked in ((threshold, "small"), (threshold + 1, "big")):
+        envs = {b: _env(task, n, **kw) for b in ("auto", "small", "big")}
+        for e in envs.values():
+            e.reset()
+        g = torch.Generator(device="cuda"); g.manual_seed(9)
+        launched = {}
+        for k in range(12):
+            act = torch.rand((n, 2), device="cuda", generator=g) * 2 - 1
+            out = {}
+            for b, e in envs.items():
+                if b == "auto":
+                    monkeypatch.delenv("REXSIM_FORCE_BUILD", raising=False)
+                else:
+                    monkeypatch.setenv("REXSIM_FORCE_BUILD", b)
+                out[b] = [t.clone() for t in e.step(act)[:3]]
+                launched.setdefault(b, set()).add(_launched(e))
+            assert all(torch.equal(x, y) for x, y in zip(out["auto"], out[picked])), (n, k)
+        assert launched["small"] == {(128, 1, 0)} and launched["big"] == {(256, 4, 0)} and launched["auto"] == launched[picked], (n, launched)
+        assert torch.equal(envs["auto"]._state_f, envs[picked]._state_f) and torch.equal(envs["auto"]._state_i, envs[picked]._state_i)
+        for e in envs.values():
+            assert (e.check_errors() & 1) == 0
+            e.close()

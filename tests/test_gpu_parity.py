@@ -403,7 +403,17 @@ def test_error_behaviour_matches_the_reference():
 
 
 def test_numpy_and_device_paths_agree_and_are_deterministic():
-    n = 256
+    _numpy_and_device_paths_agree(256)
+
+
+def test_numpy_and_device_paths_agree_beyond_the_zero_copy_limit():
+    """Above 16 384 envs rexsim_step_host stages the actions and results through device buffers instead of letting the kernel
+    address the pinned host block (zero-copy): the same bit-identity on that branch."""
+    _numpy_and_device_paths_agree(16385)
+
+
+def _numpy_and_device_paths_agree(n):
+    """numpy in / numpy out (rexsim_step_host) and CUDA tensors in / out give bit-identical results; state_dict round trip."""
     kw = dict(target_position=2.0, backwards=False, seed=5, auto_reset=True, max_episode_steps=50)
     e1, e2 = _env("walk", n, **kw), _env("walk", n, **kw)
     e1.reset(); e2.reset()
@@ -462,7 +472,9 @@ def test_baseline_size_batches_against_the_oracle(name, task, n, kw):
     """The BASELINE configurations at their per-GPU sizes, checked against the ORACLE (not only against themselves): a window
     of 48 consecutive envs from the middle of the batch is re-simulated by the fp64 oracle with the same global env ids
     (env_offset keys every reset draw) on the same actions.  Draws and episode bookkeeping bit-exact; observations / rewards within
-    the free-running tolerances over the first 40 control steps; the large batches run the 128-register 256-thread build."""
+    the free-running tolerances over the first 40 control steps.  On an H100 (132 SMs) C2 and C3 run the 128-register 256-thread
+    build; C4 (16 384 envs, below the heightfield switch at 16 896) and C5 (arm) run the 255-register 128-thread build
+    (tests/test_gpu_builds.py covers the rest)."""
     w0, nw, steps = n // 2 + 37, 48, 40
     common = dict(normalize=True, seed=11)
     env = _env(task, n, **common, **kw)
@@ -783,8 +795,17 @@ def test_error_flags_are_per_step_and_reset_indices_are_validated():
 
 def test_warp_regrouping_does_not_change_any_result():
     """rexsim_rebalance re-groups the envs over the warps by solver cost; each env's arithmetic is independent of where it
-    runs, so a de-synchronised batch stepped with re-grouping every step and one without give bit-identical outputs and state."""
-    n = 8192          # BatchedRexEnv only re-groups batches of >= 8192 envs (smaller ones fit a single wave)
+    runs, so a de-synchronised batch stepped with re-grouping every step and one without give bit-identical outputs and state.
+    BatchedRexEnv only re-groups batches of >= 8192 envs (smaller ones fit a single wave); 8192 envs run the 255-register build."""
+    _regrouping_is_bit_identical(8192)
+
+
+def test_warp_regrouping_does_not_change_any_result_on_the_128_register_build():
+    """The same at 16 384 envs, above the flat-ground switch: the 128-register 256-thread build (tests/test_gpu_builds.py)."""
+    _regrouping_is_bit_identical(16384)
+
+
+def _regrouping_is_bit_identical(n):
     kw = dict(signal_type="ik", normalize=True, auto_reset=True, max_episode_steps=60, seed=21)
     a, b = _env("walk", n, rebalance_every=1, **kw), _env("walk", n, rebalance_every=0, **kw)
     a.reset(); b.reset()
