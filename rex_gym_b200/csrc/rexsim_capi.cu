@@ -53,15 +53,8 @@ extern "C" {
 
 const char* rexsim_last_error(void) { return g_err; }
 
-int rexsim_obs_dim(int32_t task, int32_t num_motors) { return task == REXSIM_TASK_GALLOP ? 4 + num_motors : 4; }
-int rexsim_action_dim(int32_t task, int32_t signal) {
-    switch (task) {
-        case REXSIM_TASK_WALK: return signal == REXSIM_SIGNAL_IK ? 2 : 8;     /* walk_env.py:108-113 */
-        case REXSIM_TASK_GALLOP: return signal == REXSIM_SIGNAL_IK ? 2 : 4;   /* gallop_env.py:123-127 */
-        case REXSIM_TASK_TURN: return 2;                                      /* turn_env.py:104-108 */
-        default: return 1;                                                    /* standup_env.py:99, poses_env.py:118 */
-    }
-}
+int rexsim_obs_dim(int32_t task, int32_t num_motors) { return obs_dim(task, num_motors); }
+int rexsim_action_dim(int32_t task, int32_t signal) { return task_shape(task).act[signal == REXSIM_SIGNAL_IK ? 0 : 1]; }
 int rexsim_state_words(const RexSimConfig* cfg, int32_t* n_float, int32_t* n_int) {
     if (!cfg) return fail(REXSIM_ERR_INVALID, "null config");
     if (n_float) *n_float = NF;

@@ -7,10 +7,6 @@
 
 namespace rexsim {
 
-// resident CTAs per SM the step kernel is compiled for (register cap = 65536 / (128 * REXSIM_MIN_BLOCKS))
-#ifndef REXSIM_MIN_BLOCKS
-#define REXSIM_MIN_BLOCKS 1
-#endif
 // threads per CTA: small-batch (255-register) build / large-batch (128-register) build.  The warps of a CTA re-align at every
 // sub-step, so a larger CTA shares more of the instruction stream -- see REXSIM_SYNC_SUBSTEP below
 #ifndef REXSIM_BLOCK
@@ -110,6 +106,10 @@ __device__ __forceinline__ void euler_to_quat(const float* rpy, float* q) {     
 // deque's length is min(push, 100).  Every lane writes / reads the 9 words of its own leg; lane 0 writes the 7 base words
 // (and the arm's 18), which the other lanes read after a __syncwarp over the env's 4 lanes.
 struct Sensor { float* ring; int N, env, depth, words, push; uint32_t genv, rc; };
+template <bool ARM>
+__device__ __forceinline__ Sensor make_sensor(const Params& P, float* ring, int N, int env, uint32_t genv) {   // no rows pushed yet
+    return Sensor{ring, N, env, P.ring_depth, ARM ? HW_WORDS_ARM : HW_WORDS, 0, genv, 0u};
+}
 
 template <bool ARM>
 __device__ __forceinline__ void sensor_push(Sensor& S, int leg, const Lane& L, const Arm& AR, bool valid) {
@@ -1669,10 +1669,9 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
     // permutation (bit-identical results); the scattered state accesses stay in L2.
     const int env = P.perm ? P.perm[slot] : slot;
     const RexSimConfig& c = P.cfg;
-    constexpr int A = (TASK == REXSIM_TASK_WALK) ? (SIGNAL == REXSIM_SIGNAL_IK ? 2 : 8)
-                    : (TASK == REXSIM_TASK_GALLOP) ? (SIGNAL == REXSIM_SIGNAL_IK ? 2 : 4)
-                    : (TASK == REXSIM_TASK_TURN) ? 2 : 1;     // standup, poses: 1
-    const int O = (TASK == REXSIM_TASK_GALLOP) ? 4 + 12 : 4;
+    constexpr int A = task_shape(TASK).act[SIGNAL == REXSIM_SIGNAL_IK ? 0 : 1];
+    constexpr float bound = task_shape(TASK).bound[SIGNAL == REXSIM_SIGNAL_IK ? 0 : 1];
+    constexpr int O = obs_dim(TASK, 12);
 
     Lane L; Task K; Arm AR;
     load_lane(P.sf, P.si, N, env, leg, L);
@@ -1680,10 +1679,7 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
     if (ARM && leg == 0) load_arm(P.sf, P.si, N, env, AR);
     float kp = P.sf[F_KP * (size_t)N + env], kd = P.sf[F_KD * (size_t)N + env];
     int field = P.si[I_FIELD * (size_t)N + env];
-    Sensor S;
-    S.ring = P.ring; S.N = N; S.env = env; S.depth = P.ring_depth; S.words = ARM ? HW_WORDS_ARM : HW_WORDS;
-    S.genv = (uint32_t)env + (uint32_t)c.env_offset;
-    S.push = 0; S.rc = 0u;
+    Sensor S = make_sensor<ARM>(P, P.ring, N, env, (uint32_t)env + (uint32_t)c.env_offset);
     if (SENSOR) { S.push = P.si[I_HPUSH * (size_t)N + env]; S.rc = (uint32_t)P.si[I_RESETCNT * (size_t)N + env]; }
     Ground G;
     load_tile<TERRAIN>(P, field, L.pos, tiles + (TERRAIN == REXSIM_TERRAIN_RANDOM ? (threadIdx.x >> 2) * TILE_FLOATS : 0), G, leg);
@@ -1694,13 +1690,8 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
     for (int j = 0; j < A; j++) {
         float v = P.actions[(size_t)env * A + j];
         if (c.normalize) {
-            float b;
-            if (TASK == REXSIM_TASK_WALK) b = (SIGNAL == REXSIM_SIGNAL_IK) ? 0.4f : 0.01f;
-            else if (TASK == REXSIM_TASK_GALLOP) b = (SIGNAL == REXSIM_SIGNAL_IK) ? -0.4f : -0.3f;   // inverted Box: low=+b, high=-b
-            else if (TASK == REXSIM_TASK_TURN) b = 0.01f;
-            else b = 0.1f;
             v = fminf(fmaxf(v, -1.f), 1.f);
-            v = (v + 1.f) / 2.f * (2.f * b) + (-b);
+            v = (v + 1.f) / 2.f * (2.f * bound) + (-bound);
         }
         act[j] = v;
     }
@@ -1849,11 +1840,9 @@ __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_o
     const bool inrange = env >= 0 && env < P.N;
     if (!inrange) { if (valid && leg == 0) atomicOr(&P.err[P.N], REXSIM_FLAG_BAD_INDEX); env = 0; }
     const bool wr = valid && inrange;
-    const int O = (TASK == REXSIM_TASK_GALLOP) ? 4 + 12 : 4;
+    constexpr int O = obs_dim(TASK, 12);
     Lane L; Task K; Arm AR; float kp, kd; int field;
-    Sensor S;
-    S.ring = P.ring; S.N = P.N; S.env = env; S.depth = P.ring_depth; S.words = ARM ? HW_WORDS_ARM : HW_WORDS;
-    S.genv = (uint32_t)env + (uint32_t)P.cfg.env_offset; S.push = 0; S.rc = 0u;
+    Sensor S = make_sensor<ARM>(P, P.ring, P.N, env, (uint32_t)env + (uint32_t)P.cfg.env_offset);
     reset_from_snapshot<ARM>(P, env, leg, L, K, kp, kd, field, AR, wr, S);
     if (wr && obs_out) {
         if (P.sensor_on) write_obs<TASK, true>(P, env, leg, L, obs_out + (size_t)j * O, S, 0u);
@@ -1898,10 +1887,8 @@ __global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_
     // RexPosesEnv.reset -> RexGymEnv.reset(initial_motor_angles=None): Rex.Reset skips both holding phases (rex.py:307)
     // sensor history of the reset hold: _observation_history.clear() (rex.py:303), one ReceiveObservation before the hold
     // (:313), one per sub-step, one after it (:324).  The 8 replicas of the warp write identical rows to the same addresses.
-    Sensor S;
-    S.words = ARM ? HW_WORDS_ARM : HW_WORDS; S.depth = P.ring_depth;
-    S.ring = SENSOR ? P.snap_ring + (size_t)field * S.depth * S.words : nullptr;
-    S.N = 1; S.env = 0; S.push = 0; S.genv = 0u; S.rc = 0u;
+    Sensor S = make_sensor<ARM>(P, nullptr, 1, 0, 0u);
+    if (SENSOR) S.ring = P.snap_ring + (size_t)field * S.depth * S.words;
     const int n1 = (task == REXSIM_TASK_POSES) ? 0 : 100;
     if (SENSOR && n1) sensor_push<ARM>(S, leg, L, AR, true);
     for (int it = 0; it < n1; it++) apply_action_and_step<TERRAIN, ARM, SENSOR>(P, sm, L, leg, stand, P.cfg.motor_kp, P.cfg.motor_kd, G, AR, S, true);
@@ -1929,6 +1916,21 @@ __global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_
 // pair's step kernels are instantiated) and once with -DREXSIM_UNIT=100 (reset / settle / get / set kernels and the
 // dispatcher); rex_gym_b200/build.py runs the units in parallel.  Without REXSIM_UNIT everything is one unit.
 // -------------------------------------------------------------------------------------------------
+// unit k holds the step kernels of the (task, signal) pair c_units[k]: walk, gallop, turn with either signal, then standup, poses
+struct StepUnit { int task, signal; };
+constexpr StepUnit c_units[8] = {{REXSIM_TASK_WALK, REXSIM_SIGNAL_IK}, {REXSIM_TASK_WALK, REXSIM_SIGNAL_OL},
+                                 {REXSIM_TASK_GALLOP, REXSIM_SIGNAL_IK}, {REXSIM_TASK_GALLOP, REXSIM_SIGNAL_OL},
+                                 {REXSIM_TASK_TURN, REXSIM_SIGNAL_IK}, {REXSIM_TASK_TURN, REXSIM_SIGNAL_OL},
+                                 {REXSIM_TASK_STANDUP, REXSIM_SIGNAL_OL}, {REXSIM_TASK_POSES, REXSIM_SIGNAL_IK}};
+// the unit launch_step takes for a (task, signal) pair; standup and poses ignore the signal, an unknown task takes unit 6
+constexpr int unit_of(int task, int signal) {
+    return task == REXSIM_TASK_POSES ? 7 : (task >= 0 && task < REXSIM_TASK_STANDUP) ? 2 * task + (signal != REXSIM_SIGNAL_IK) : 6;
+}
+constexpr bool unit_of_inverts_c_units(int u = 0) {
+    return u == 8 || (unit_of(c_units[u].task, c_units[u].signal) == u && unit_of_inverts_c_units(u + 1));
+}
+static_assert(unit_of_inverts_c_units(), "unit_of must map every (task, signal) of c_units to its own unit");
+template <int U> cudaError_t launch_step_unit(const Params& P, cudaStream_t st);
 #if !defined(REXSIM_UNIT) || REXSIM_UNIT < 100
 template <int TASK, int SIGNAL, int TERRAIN, int OCC, bool ARM, bool SENSOR, int BLOCK>
 static cudaError_t launch_step_variant(const Params& P, cudaStream_t st) {
@@ -1974,33 +1976,11 @@ static cudaError_t launch_step_ts(const Params& P, cudaStream_t st) {
     }
     return launch_step_tsa<TASK, SIGNAL, false>(P, st);
 }
+template <int U>
+cudaError_t launch_step_unit(const Params& P, cudaStream_t st) { return launch_step_ts<c_units[U].task, c_units[U].signal>(P, st); }
+#ifdef REXSIM_UNIT
+template cudaError_t launch_step_unit<REXSIM_UNIT>(const Params&, cudaStream_t);
 #endif
-#define REXSIM_STEP_UNIT(k, T, S) \
-    cudaError_t launch_step_unit_##k(const Params& P, cudaStream_t st) { return launch_step_ts<T, S>(P, st); }
-#if !defined(REXSIM_UNIT) || REXSIM_UNIT == 0
-REXSIM_STEP_UNIT(0, REXSIM_TASK_WALK, REXSIM_SIGNAL_IK)
-#endif
-#if !defined(REXSIM_UNIT) || REXSIM_UNIT == 1
-REXSIM_STEP_UNIT(1, REXSIM_TASK_WALK, REXSIM_SIGNAL_OL)
-#endif
-#if !defined(REXSIM_UNIT) || REXSIM_UNIT == 2
-REXSIM_STEP_UNIT(2, REXSIM_TASK_GALLOP, REXSIM_SIGNAL_IK)
-#endif
-#if !defined(REXSIM_UNIT) || REXSIM_UNIT == 3
-REXSIM_STEP_UNIT(3, REXSIM_TASK_GALLOP, REXSIM_SIGNAL_OL)
-#endif
-#if !defined(REXSIM_UNIT) || REXSIM_UNIT == 4
-REXSIM_STEP_UNIT(4, REXSIM_TASK_TURN, REXSIM_SIGNAL_IK)
-#endif
-#if !defined(REXSIM_UNIT) || REXSIM_UNIT == 5
-REXSIM_STEP_UNIT(5, REXSIM_TASK_TURN, REXSIM_SIGNAL_OL)
-#endif
-#if !defined(REXSIM_UNIT) || REXSIM_UNIT == 6
-REXSIM_STEP_UNIT(6, REXSIM_TASK_STANDUP, REXSIM_SIGNAL_OL)
-#endif
-
-#if !defined(REXSIM_UNIT) || REXSIM_UNIT == 7
-REXSIM_STEP_UNIT(7, REXSIM_TASK_POSES, REXSIM_SIGNAL_IK)
 #endif
 
 #if !defined(REXSIM_UNIT) || REXSIM_UNIT == 100
@@ -2060,21 +2040,11 @@ cudaError_t launch_rebalance(const int32_t* cost, int n, int32_t* hist, int32_t*
     return cudaGetLastError();
 }
 
-cudaError_t launch_step_unit_0(const Params&, cudaStream_t);
-cudaError_t launch_step_unit_1(const Params&, cudaStream_t);
-cudaError_t launch_step_unit_2(const Params&, cudaStream_t);
-cudaError_t launch_step_unit_3(const Params&, cudaStream_t);
-cudaError_t launch_step_unit_4(const Params&, cudaStream_t);
-cudaError_t launch_step_unit_5(const Params&, cudaStream_t);
-cudaError_t launch_step_unit_6(const Params&, cudaStream_t);
-cudaError_t launch_step_unit_7(const Params&, cudaStream_t);
 cudaError_t launch_step(const Params& P, cudaStream_t st) {
-    const int t = P.cfg.task, s = P.cfg.signal;
-    if (t == REXSIM_TASK_WALK) return s == REXSIM_SIGNAL_IK ? launch_step_unit_0(P, st) : launch_step_unit_1(P, st);
-    if (t == REXSIM_TASK_GALLOP) return s == REXSIM_SIGNAL_IK ? launch_step_unit_2(P, st) : launch_step_unit_3(P, st);
-    if (t == REXSIM_TASK_TURN) return s == REXSIM_SIGNAL_IK ? launch_step_unit_4(P, st) : launch_step_unit_5(P, st);
-    if (t == REXSIM_TASK_POSES) return launch_step_unit_7(P, st);
-    return launch_step_unit_6(P, st);
+    static constexpr cudaError_t (*units[])(const Params&, cudaStream_t) = {
+        launch_step_unit<0>, launch_step_unit<1>, launch_step_unit<2>, launch_step_unit<3>,
+        launch_step_unit<4>, launch_step_unit<5>, launch_step_unit<6>, launch_step_unit<7>};
+    return units[unit_of(P.cfg.task, P.cfg.signal)](P, st);
 }
 cudaError_t launch_reset(const Params& P, float* obs_out, cudaStream_t st) {
     int k = P.reset_idx ? P.reset_k : P.N;

@@ -50,6 +50,17 @@ enum {
     FL_POSE_SHIFT = 26          // 3 bits: poses task, which base coordinate is staged (0 base_y, 1 base_z, 2 roll, 3 pitch, 4 yaw)
 };
 
+// ----- per-task action width [ik, ol signal], motor angles in the observation, RangeNormalize action bound [ik, ol] -----
+struct TaskShape { int act[2]; bool angles; float bound[2]; };
+__host__ __device__ constexpr TaskShape task_shape(int task) {
+    return task == REXSIM_TASK_WALK   ? TaskShape{{2, 8}, false, {0.4f, 0.01f}}       // walk_env.py:108-113
+         : task == REXSIM_TASK_GALLOP ? TaskShape{{2, 4}, true, {-0.4f, -0.3f}}       // gallop_env.py:123-127; inverted Box: low=+b, high=-b
+         : task == REXSIM_TASK_TURN   ? TaskShape{{2, 2}, false, {0.01f, 0.01f}}      // turn_env.py:104-108
+         : TaskShape{{1, 1}, false, {0.1f, 0.1f}};                                   // standup_env.py:99, poses_env.py:118
+}
+// observation width: base roll, pitch and their rates, then (gallop) the motor angles
+__host__ __device__ constexpr int obs_dim(int task, int num_motors) { return 4 + (task_shape(task).angles ? num_motors : 0); }
+
 struct Params {
     RexSimConfig cfg;
     const float* __restrict__ model;   // REXSIM_MT_FLOATS floats, 16-byte aligned
