@@ -55,15 +55,17 @@ int rexagent_get_params(RexAgent* a, float* host_params, int64_t n_floats);
 /* device pointer to the packed block (a learner updates it in place) */
 int rexagent_params_buffer(RexAgent* a, float** params);
 
-/* streaming normaliser state; host arrays.  observ: count, mean[O], var_sum[O]; reward: count, mean, var_sum */
-int rexagent_set_filters(RexAgent* a, int32_t observ_count, const float* observ_mean, const float* observ_var_sum,
-                         int32_t reward_count, float reward_mean, float reward_var_sum);
-int rexagent_get_filters(RexAgent* a, int32_t* counts /*[2]*/, float* observ_mean, float* observ_var_sum,
+/* streaming normaliser state; host arrays.  observ: count, mean[O], var_sum[O]; reward: count, mean, var_sum.
+ * The counts are 64-bit: every filter update adds the whole batch, so at 65 536 envs a 32-bit count would wrap after
+ * 32 768 control steps (the reference's int32 TF variable never gets near that at its 30 envs). */
+int rexagent_set_filters(RexAgent* a, int64_t observ_count, const float* observ_mean, const float* observ_var_sum,
+                         int64_t reward_count, float reward_mean, float reward_var_sum);
+int rexagent_get_filters(RexAgent* a, int64_t* counts /*[2]*/, float* observ_mean, float* observ_var_sum,
                          float* reward_mean_var /*[2]*/);
 
 /* raw device state for checkpoint / resume: filt dev [2*O + 2] f32 (observ mean[O], var_sum[O], reward mean, var_sum);
- * counters dev [4] i32 (observ count, reward count, step counter, internal ticket = 0 between launches) */
-int rexagent_state_buffers(RexAgent* a, float** filt, int32_t** counters);
+ * counters dev [4] i64 (observ count, reward count, step counter, internal ticket = 0 between launches) */
+int rexagent_state_buffers(RexAgent* a, float** filt, int64_t** counters);
 
 /* observ dev [n][O] -> action dev [n][A], mean dev [n][A], logprob dev [n], value dev [n]  (any output may be NULL).
  * training != 0: action = mean + exp(logstd) * eps, eps ~ N(0,1) from the counter-based generator keyed on

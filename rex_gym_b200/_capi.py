@@ -98,7 +98,7 @@ def load():
     L.rexagent_get_params.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
     L.rexagent_params_buffer.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
     L.rexagent_state_buffers.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    L.rexagent_set_filters.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_float]
+    L.rexagent_set_filters.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_float]
     L.rexagent_get_filters.argtypes = [C.c_void_p] * 5
     L.rexagent_perform.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_uint64, C.c_uint32, C.c_uint32] + [C.c_void_p] * 6
     L.rexagent_experience.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]

@@ -54,7 +54,7 @@ class ForwardGaussianPolicy(object):
         _capi.check(self._L.rexagent_state_buffers(self._h, C.byref(pf), C.byref(pc)))
         from ..envs.batched_env import _DevArray
         self._filt = torch.as_tensor(_DevArray(pf.value, (2 * self.O + 2,), "<f4", self), device=self.device)
-        self._cnt = torch.as_tensor(_DevArray(pc.value, (4,), "<i4", self), device=self.device)
+        self._cnt = torch.as_tensor(_DevArray(pc.value, (4,), "<i8", self), device=self.device)    # int64: counts pass 2^31
         self.observ_filter = StreamingNormalize(self, "observ")
         self.reward_filter = StreamingNormalize(self, "reward")
         # initialisers of networks.py:18-19 and tf.contrib.layers defaults: xavier-uniform hidden layers, zero biases,
@@ -129,7 +129,7 @@ class ForwardGaussianPolicy(object):
                                                      float(reward_mean), float(reward_var_sum)))
 
     def get_filters(self):
-        counts = np.zeros(2, np.int32); m = np.zeros(self.O, np.float32); v = np.zeros(self.O, np.float32); r = np.zeros(2, np.float32)
+        counts = np.zeros(2, np.int64); m = np.zeros(self.O, np.float32); v = np.zeros(self.O, np.float32); r = np.zeros(2, np.float32)
         with torch.cuda.device(self.device):
             _capi.check(self._L.rexagent_get_filters(self._h, counts.ctypes.data, m.ctypes.data, v.ctypes.data, r.ctypes.data))
         return dict(observ_count=int(counts[0]), observ_mean=m, observ_var_sum=v, reward_count=int(counts[1]),

@@ -22,7 +22,8 @@ struct AgentDev {
     const float* __restrict__ params;    // policy block | value block
     int pol_floats, val_floats;
     float* filt;                          // observ mean[O], var_sum[O], reward mean, var_sum
-    int32_t* cnt;                         // observ count, reward count, step counter, blocks-done ticket
+    int64_t* cnt;                         // observ count, reward count, step counter, blocks-done ticket
+                                          // (64-bit: at 65 536 envs a 32-bit count wraps after 32 768 control steps)
     float* partial;                       // [RED_BLOCKS][2 * (O + 1)]
 };
 
@@ -78,7 +79,7 @@ __global__ void __launch_bounds__(512, 1) perform_kernel(const PerformArgs P) {
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     if (tid < O) {   // StreamingNormalize.transform constants (normalize.py:57-66, _std :131-144)
-        const int cnt = P.D.cnt[0];
+        const int64_t cnt = P.D.cnt[0];
         float m = P.D.filt[tid], vs = P.D.filt[O + tid];
         float inv = 1.f;
         if (cnt > 1) inv = 1.f / (sqrtf(vs / (float)(cnt - 1) + 1e-4f) + 1e-8f);
@@ -275,7 +276,7 @@ __global__ void __launch_bounds__(tc::THREADS, 1) perform_tc_kernel(const Perfor
     const float* gW1 = G; const float* gb1 = gW1 + O * H1; const float* gW2 = gb1 + H1; const float* gb2 = gW2 + H1 * H2;
     const float* gW3 = gb2 + H2; const float* gb3 = gW3 + H2 * AO;
     if (tid < O) {   // StreamingNormalize.transform constants (normalize.py:57-66, _std :131-144)
-        const int cnt = P.D.cnt[0];
+        const int64_t cnt = P.D.cnt[0];
         float m = P.D.filt[tid], vs = P.D.filt[O + tid];
         float inv = 1.f;
         if (cnt > 1) inv = 1.f / (sqrtf(vs / (float)(cnt - 1) + 1e-4f) + 1e-8f);
@@ -444,7 +445,7 @@ struct ExperienceArgs { AgentDev D; const float* __restrict__ observ; const floa
 __device__ __forceinline__ void filters_finalize(const AgentDev& D, int col, float s1, float s2, int n_total, float first_value) {
     const int O = D.cfg.obs_dim;
     const int which = col < O ? 0 : 1;
-    const int cnt = D.cnt[which] + n_total;
+    const int64_t cnt = D.cnt[which] + n_total;
     const float step = (float)cnt;
     float* meanp = col < O ? &D.filt[col] : &D.filt[2 * O];
     float* varp = col < O ? &D.filt[O + col] : &D.filt[2 * O + 1];
@@ -483,7 +484,7 @@ __global__ void __launch_bounds__(256) experience_kernel(const ExperienceArgs P)
     }
     __threadfence();
     __syncthreads();
-    if (tid == 0) last = (atomicAdd(&P.D.cnt[3], 1) == (int)gridDim.x - 1);
+    if (tid == 0) last = (atomicAdd(reinterpret_cast<unsigned long long*>(&P.D.cnt[3]), 1ull) == (unsigned long long)gridDim.x - 1);
     __syncthreads();
     if (!last) return;
     __threadfence();
@@ -514,7 +515,7 @@ __global__ void experience_finalize_kernel(const AgentDev D, const float* __rest
 
 __global__ void transform_reward_kernel(const AgentDev D, const float* __restrict__ r, int n, float* __restrict__ out) {
     const int O = D.cfg.obs_dim;
-    const int cnt = D.cnt[1];
+    const int64_t cnt = D.cnt[1];
     float inv = 1.f;
     if (cnt > 1) inv = 1.f / (sqrtf(D.filt[2 * O + 1] / (float)(cnt - 1) + 1e-4f) + 1e-8f);
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
@@ -597,7 +598,7 @@ struct RexAgent {
     AgentDev D;
     float* d_params = nullptr;
     float* d_filt = nullptr;
-    int32_t* d_cnt = nullptr;
+    int64_t* d_cnt = nullptr;
     float* d_partial = nullptr;
     int sm_count = 132;
     int64_t launches = 0;
@@ -663,8 +664,8 @@ int rexagent_create(const RexAgentConfig* cfg, RexAgent** out) {
     ACK(cudaMemset(a->d_params, 0, np * sizeof(float)));
     ACK(cudaMalloc(&a->d_filt, (2 * O + 2) * sizeof(float)));
     ACK(cudaMemset(a->d_filt, 0, (2 * O + 2) * sizeof(float)));
-    ACK(cudaMalloc(&a->d_cnt, 4 * sizeof(int32_t)));
-    ACK(cudaMemset(a->d_cnt, 0, 4 * sizeof(int32_t)));
+    ACK(cudaMalloc(&a->d_cnt, 4 * sizeof(int64_t)));
+    ACK(cudaMemset(a->d_cnt, 0, 4 * sizeof(int64_t)));
     ACK(cudaMalloc(&a->d_partial, (size_t)RED_BLOCKS * 2 * (O + 1) * sizeof(float)));
     ACK(cudaFuncSetAttribute(perform_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)perform_smem_bytes(cfg, 64)));
     ACK(cudaFuncSetAttribute(perform_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)perform_smem_bytes(cfg, 128)));
@@ -708,28 +709,28 @@ int rexagent_params_buffer(RexAgent* a, float** p) {
     *p = a->d_params;
     return REXSIM_OK;
 }
-int rexagent_state_buffers(RexAgent* a, float** filt, int32_t** counters) {
+int rexagent_state_buffers(RexAgent* a, float** filt, int64_t** counters) {
     if (!a) return afail(REXSIM_ERR_INVALID, "null argument");
     if (filt) *filt = a->d_filt;
     if (counters) *counters = a->d_cnt;
     return REXSIM_OK;
 }
-int rexagent_set_filters(RexAgent* a, int32_t oc, const float* om, const float* ov, int32_t rc, float rm, float rv) {
+int rexagent_set_filters(RexAgent* a, int64_t oc, const float* om, const float* ov, int64_t rc, float rm, float rv) {
     if (!a || !om || !ov) return afail(REXSIM_ERR_INVALID, "null argument");
     const int O = a->D.cfg.obs_dim;
     std::vector<float> f(2 * O + 2);
     for (int i = 0; i < O; i++) { f[i] = om[i]; f[O + i] = ov[i]; }
     f[2 * O] = rm; f[2 * O + 1] = rv;
-    int32_t c[4] = {oc, rc, 0, 0};
+    int64_t c[4] = {oc, rc, 0, 0};
     ACK(cudaMemcpy(a->d_filt, f.data(), f.size() * sizeof(float), cudaMemcpyHostToDevice));
     ACK(cudaMemcpy(a->d_cnt, c, sizeof(c), cudaMemcpyHostToDevice));
     return REXSIM_OK;
 }
-int rexagent_get_filters(RexAgent* a, int32_t* counts, float* om, float* ov, float* rmv) {
+int rexagent_get_filters(RexAgent* a, int64_t* counts, float* om, float* ov, float* rmv) {
     if (!a || !counts || !om || !ov || !rmv) return afail(REXSIM_ERR_INVALID, "null argument");
     const int O = a->D.cfg.obs_dim;
     std::vector<float> f(2 * O + 2);
-    int32_t c[4];
+    int64_t c[4];
     ACK(cudaMemcpy(f.data(), a->d_filt, f.size() * sizeof(float), cudaMemcpyDeviceToHost));
     ACK(cudaMemcpy(c, a->d_cnt, sizeof(c), cudaMemcpyDeviceToHost));
     for (int i = 0; i < O; i++) { om[i] = f[i]; ov[i] = f[O + i]; }
