@@ -163,6 +163,9 @@ int rexsim_error_flags(RexSim* sim, int32_t** err_flags);
 int rexsim_clear_errors(RexSim* sim, void* stream);          /* zeroes the aggregate word (enqueued on stream) */
 /* last motor command of every env (info['action'], rex_gym_env.py:414): dev [nm][N] */
 int rexsim_last_command(RexSim* sim, float** cmd);
+/* solver cost of every env's last control step (what rexsim_rebalance sorts by): dev [N] int32, the PGS iterations of its sub-steps
+ * plus 64 per sub-step on the generic path */
+int rexsim_solver_cost(RexSim* sim, int32_t** cost);
 /* kernels launched by this handle since create (the bench reports it) */
 int64_t rexsim_launch_count(const RexSim* sim);
 /* which build of the step kernel the last rexsim_step / rexsim_step_host launched (all 0 before the first step): CTA size,

@@ -313,6 +313,11 @@ int rexsim_last_command(RexSim* s, float** cmd) {
     *cmd = s->d_cmd;
     return REXSIM_OK;
 }
+int rexsim_solver_cost(RexSim* s, int32_t** cost) {
+    if (!s || !cost) return fail(REXSIM_ERR_INVALID, "null argument");
+    *cost = s->d_cost;
+    return REXSIM_OK;
+}
 int64_t rexsim_launch_count(const RexSim* s) { return s ? s->launches : 0; }
 int rexsim_last_step_build(const RexSim* s, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor) {
     if (!s || !cta_threads || !ctas_per_sm || !sensor) return fail(REXSIM_ERR_INVALID, "null argument");

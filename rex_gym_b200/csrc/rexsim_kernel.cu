@@ -24,6 +24,21 @@ namespace rexsim {
 #ifndef REXSIM_SYNC_SUBSTEP
 #define REXSIM_SYNC_SUBSTEP 1
 #endif
+// 1: the 255-register builds on flat ground without the arm solve the 12 foot-contact rows replicated on the 4 lanes of an env
+// (one exchange per sub-step, no lane-to-lane traffic inside the PGS loop); 0: every build keeps the shuffle solver.
+// Bit-identical either way.
+#ifndef REXSIM_PGS_REPLICATED
+#define REXSIM_PGS_REPLICATED 1
+#endif
+// the replicated loop doubles the solver's instructions to cut its serial chain: worth it where each scheduler holds one or two
+// warps (the 255-register builds), not in the issue-bound 128-register build.  On heightfields the per-sub-step exchange and the
+// spills around the loop cost more than the shorter chain saves (C4 turn-ik, 4096 envs: 3.7 % slower on an H100 SXM)
+__host__ __device__ constexpr bool pgs_replicated(int occ, bool arm, int terrain) {
+    return REXSIM_PGS_REPLICATED && occ == 1 && !arm && terrain == REXSIM_TERRAIN_PLANE;
+}
+// per env, in dynamic shared memory after the heightfield tiles: the 12 pre-scaled Delassus rows (row-major), their running sums
+// and their denominators -- one exchange per sub-step
+#define PGS_ENV_FLOATS (12 * 12 + 12 + 12)
 #define PI_F 3.14159265358979323846f
 #define PI_D 3.14159265358979323846
 
@@ -334,9 +349,11 @@ __device__ __forceinline__ float clampv(float v, float lim) { return fminf(fmaxf
 // -------------------------------------------------------------------------------------------------
 // one pybullet.stepSimulation for the 4 lanes of an env (call site rex_gym/model/rex.py:161)
 // -------------------------------------------------------------------------------------------------
-template <int TERRAIN, bool ARM>
+// REPL: the 12-row fast path runs the replicated PGS loop (REXSIM_PGS_REPLICATED) instead of the shuffle loop, exchanging the
+// rows through the env's PGS_ENV_FLOATS floats of shared memory at `pgs`
+template <int TERRAIN, bool ARM, bool REPL>
 __device__ __forceinline__ void physics_substep(const Params& P, const float* __restrict__ sm, Lane& L, int leg,
-                                                const float* tau, Ground& G, Arm& AR, const float* tauA) {
+                                                const float* tau, Ground& G, Arm& AR, const float* tauA, float* pgs) {
     const float dt = (float)P.cfg.sim_dt_d;
     const float inv_dt = 1.0f / dt;
     const float* LB = sm + REXSIM_MT_LEG + leg * 48;
@@ -811,92 +828,173 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                 for (int cc = 0; cc < NC; cc++) Aarm[a][cc] *= -dinvA[a];
             }
         }
-        float denAll[4][NR];
+        if constexpr (REPL && !LIM && !ARM) {
+            // ---- replicated form: every lane of the env sweeps all 12 rows itself ------------------------------------
+            // A single warp per scheduler cannot hide the shuffle that hands each impulse change to the next row's owner, and
+            // that shuffle sits on the serial chain 8 times per iteration.  So exchange once per sub-step, through shared memory
+            // (a shuffle in this env-divergent branch is a collective of ~10 instructions): lane s publishes rows 3s..3s+2 (matrix
+            // row, running sum, denominator), every lane loads all 12 into registers, and each row then sees exactly the fmaf
+            // sequence lane s performs in the shuffle form below -- bit-identical impulses.  The normal row of a contact that does
+            // not touch is published as zeros (matrix row and sum), so its change is fmaxf(0, -0) = 0 with no select, and
+            // lam[n] > 0 alone gates its friction.
+            // The normal clamp (lam + dI < 0 ? -lam : dI) is fmaxf(dI, -lam): a rounded sum has the sign of the exact sum, so
+            // the two differ at most in the sign of a zero change, which leaves lam and the residual unchanged.
+            constexpr int NF = 12;
+            __syncwarp(env_mask());                     // the env's lanes are done reading the previous sub-step's rows
 #pragma unroll
-        for (int s = 0; s < 4; s++)
+            for (int d = 0; d < 3; d++) {
+                const bool keep = mine || d > 0;
+                float4* row = reinterpret_cast<float4*>(pgs + (3 * leg + d) * NF);
 #pragma unroll
-            for (int d = 0; d < NR; d++) denAll[s][d] = bcast4(den[d], s);
-        for (int it = 0; it < iters && running; it++) {
-            L.cost++;
-            float resid = 0.f;
-            // joint-limit rows first, in joint order (4 legs, then the arm), the direction alternating per iteration
-            // (btMultiBodyConstraintSolver::solveSingleIteration): even iterations descending, odd ascending
-            auto arm_round = [&](const int a) {
-                float dI = tA[a];
-                if (lamA[a] + dI < 0.f) dI = -lamA[a];
-                dI = (actA[a] && leg == 0) ? dI : 0.f;
-                lamA[a] += dI;
-                const float dl = bcast4(dI, 0);
-                const float rr = dl * denA[a]; resid = fmaxf(resid, rr * rr);
-#pragma unroll
-                for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][CA + a], dl, t[r]);
-#pragma unroll
-                for (int c2 = 0; c2 < ARM_KA; c2++) tA[c2] = fmaf(Aarm[c2][CA + a], dl, tA[c2]);
-            };
-            auto leg_round = [&](const int s) {
-                float dI = t[NR - 1];
-                if (lam[NR - 1] + dI < 0.f) dI = -lam[NR - 1];
-                dI = (hasL && leg == s) ? dI : 0.f;
-                lam[NR - 1] += dI;
-                const float dl = bcast4(dI, s);
-                const float rr = dl * denAll[s][NR - 1]; resid = fmaxf(resid, rr * rr);
-#pragma unroll
-                for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][CL + s], dl, t[r]);
-                if (ARM) {
-#pragma unroll
-                    for (int a = 0; a < ARM_KA; a++) tA[a] = fmaf(Aarm[a][CL + s], dl, tA[a]);
-                }
-            };
-            if (it & 1) {
-                if (LIM) { leg_round(0); leg_round(1); leg_round(2); leg_round(3); }
-                if (ARM) { arm_round(0); arm_round(1); arm_round(2); }
-            } else {
-                if (ARM) { arm_round(2); arm_round(1); arm_round(0); }
-                if (LIM) { leg_round(3); leg_round(2); leg_round(1); leg_round(0); }
+                for (int q = 0; q < NF / 4; q++)
+                    row[q] = keep ? make_float4(A[d][4 * q], A[d][4 * q + 1], A[d][4 * q + 2], A[d][4 * q + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
+                pgs[NF * NF + 3 * leg + d] = keep ? t[d] : 0.f;
+                pgs[NF * NF + NF + 3 * leg + d] = den[d];
             }
+            __syncwarp(env_mask());
+            float Af[NF][NF], T[NF], lamF[NF], denF[NF];
+            const float4* E = reinterpret_cast<const float4*>(pgs);
 #pragma unroll
-            for (int s = 0; s < 4; s++) {
-                float dI = t[0];
-                if (lam[0] + dI < 0.f) dI = -lam[0];
-                const bool upd = mine && (leg == s);
-                dI = upd ? dI : 0.f;
-                lam[0] += dI;
-                const float dl = bcast4(dI, s);
-                const float rr = dl * denAll[s][0]; resid = fmaxf(resid, rr * rr);
+            for (int j = 0; j < NF; j++) {
 #pragma unroll
-                for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][3 * s], dl, t[r]);
-                if (ARM) {
-#pragma unroll
-                    for (int a = 0; a < ARM_KA; a++) tA[a] = fmaf(Aarm[a][3 * s], dl, tA[a]);
+                for (int q = 0; q < NF / 4; q++) {
+                    const float4 v = E[j * (NF / 4) + q];
+                    Af[j][4 * q] = v.x; Af[j][4 * q + 1] = v.y; Af[j][4 * q + 2] = v.z; Af[j][4 * q + 3] = v.w;
                 }
             }
 #pragma unroll
-            for (int s = 0; s < 4; s++) {
-                // both friction rows of contact s belong to lane s: update t1, fold its change into the own t2 sum
-                // locally, update t2, then broadcast the two changes together (one communication round per contact)
-                const float lim = mu * lam[0];
-                const bool upd = mine && (leg == s) && (lam[0] > 0.f);
-                float dI1 = t[1];
-                const float sum1 = lam[1] + dI1;
-                if (sum1 < -lim) dI1 = -lim - lam[1]; else if (sum1 > lim) dI1 = lim - lam[1];
-                dI1 = upd ? dI1 : 0.f;
-                lam[1] += dI1;
-                float dI2 = fmaf(A[2][3 * s + 1], dI1, t[2]);            // own lane: column 3*leg+1 == 3*s+1 when upd
-                const float sum2 = lam[2] + dI2;
-                if (sum2 < -lim) dI2 = -lim - lam[2]; else if (sum2 > lim) dI2 = lim - lam[2];
-                dI2 = upd ? dI2 : 0.f;
-                lam[2] += dI2;
-                const float dl1 = bcast4(dI1, s), dl2 = bcast4(dI2, s);
-                const float r1 = dl1 * denAll[s][1], r2 = dl2 * denAll[s][2];
-                resid = fmaxf(resid, fmaxf(r1 * r1, r2 * r2));
-#pragma unroll
-                for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][3 * s + 2], dl2, fmaf(A[r][3 * s + 1], dl1, t[r]));
-                if (ARM) {
-#pragma unroll
-                    for (int a = 0; a < ARM_KA; a++) tA[a] = fmaf(Aarm[a][3 * s + 2], dl2, fmaf(Aarm[a][3 * s + 1], dl1, tA[a]));
-                }
+            for (int q = 0; q < NF / 4; q++) {
+                const float4 v = E[NF * NF / 4 + q], w = E[NF * NF / 4 + NF / 4 + q];
+                T[4 * q] = v.x; T[4 * q + 1] = v.y; T[4 * q + 2] = v.z; T[4 * q + 3] = v.w;
+                denF[4 * q] = w.x; denF[4 * q + 1] = w.y; denF[4 * q + 2] = w.z; denF[4 * q + 3] = w.w;
             }
-            if (resid <= thr) running = false;
+#pragma unroll
+            for (int j = 0; j < NF; j++) lamF[j] = 0.f;
+            for (int it = 0; it < iters && running; it++) {
+                L.cost++;
+                float resid = 0.f;
+#pragma unroll
+                for (int s = 0; s < 4; s++) {
+                    const int n = 3 * s;
+                    const float dI = fmaxf(T[n], -lamF[n]);
+                    lamF[n] += dI;
+                    const float rr = dI * denF[n]; resid = fmaxf(resid, rr * rr);
+#pragma unroll
+                    for (int j = 0; j < NF; j++) T[j] = fmaf(Af[j][n], dI, T[j]);
+                }
+#pragma unroll
+                for (int s = 0; s < 4; s++) {
+                    // the clamp bounds and the zero of a frozen pair are known before the row's sum: the chain is add, compare, 2 selects
+                    const int n = 3 * s, f1 = n + 1, f2 = n + 2;
+                    const float lim = mu * lamF[n];
+                    const bool upd = lamF[n] > 0.f;
+                    const float lo1 = upd ? -lim - lamF[f1] : 0.f, hi1 = upd ? lim - lamF[f1] : 0.f;
+                    const float sum1 = lamF[f1] + T[f1];
+                    const float dI1 = sum1 < -lim ? lo1 : (sum1 > lim ? hi1 : (upd ? T[f1] : 0.f));
+                    lamF[f1] += dI1;
+                    const float t2 = fmaf(Af[f2][f1], dI1, T[f2]);
+                    const float lo2 = upd ? -lim - lamF[f2] : 0.f, hi2 = upd ? lim - lamF[f2] : 0.f;
+                    const float sum2 = lamF[f2] + t2;
+                    const float dI2 = sum2 < -lim ? lo2 : (sum2 > lim ? hi2 : (upd ? t2 : 0.f));
+                    lamF[f2] += dI2;
+                    const float r1 = dI1 * denF[f1], r2 = dI2 * denF[f2];
+                    resid = fmaxf(resid, fmaxf(r1 * r1, r2 * r2));
+#pragma unroll
+                    for (int j = 0; j < NF; j++) T[j] = fmaf(Af[j][f2], dI2, fmaf(Af[j][f1], dI1, T[j]));
+                }
+                if (resid <= thr) running = false;
+            }
+#pragma unroll
+            for (int d = 0; d < 3; d++)
+                lam[d] = leg == 0 ? lamF[d] : (leg == 1 ? lamF[3 + d] : (leg == 2 ? lamF[6 + d] : lamF[9 + d]));
+        } else {
+            float denAll[4][NR];
+#pragma unroll
+            for (int s = 0; s < 4; s++)
+#pragma unroll
+                for (int d = 0; d < NR; d++) denAll[s][d] = bcast4(den[d], s);
+            for (int it = 0; it < iters && running; it++) {
+                L.cost++;
+                float resid = 0.f;
+                // joint-limit rows first, in joint order (4 legs, then the arm), the direction alternating per iteration
+                // (btMultiBodyConstraintSolver::solveSingleIteration): even iterations descending, odd ascending
+                auto arm_round = [&](const int a) {
+                    float dI = tA[a];
+                    if (lamA[a] + dI < 0.f) dI = -lamA[a];
+                    dI = (actA[a] && leg == 0) ? dI : 0.f;
+                    lamA[a] += dI;
+                    const float dl = bcast4(dI, 0);
+                    const float rr = dl * denA[a]; resid = fmaxf(resid, rr * rr);
+#pragma unroll
+                    for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][CA + a], dl, t[r]);
+#pragma unroll
+                    for (int c2 = 0; c2 < ARM_KA; c2++) tA[c2] = fmaf(Aarm[c2][CA + a], dl, tA[c2]);
+                };
+                auto leg_round = [&](const int s) {
+                    float dI = t[NR - 1];
+                    if (lam[NR - 1] + dI < 0.f) dI = -lam[NR - 1];
+                    dI = (hasL && leg == s) ? dI : 0.f;
+                    lam[NR - 1] += dI;
+                    const float dl = bcast4(dI, s);
+                    const float rr = dl * denAll[s][NR - 1]; resid = fmaxf(resid, rr * rr);
+#pragma unroll
+                    for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][CL + s], dl, t[r]);
+                    if (ARM) {
+#pragma unroll
+                        for (int a = 0; a < ARM_KA; a++) tA[a] = fmaf(Aarm[a][CL + s], dl, tA[a]);
+                    }
+                };
+                if (it & 1) {
+                    if (LIM) { leg_round(0); leg_round(1); leg_round(2); leg_round(3); }
+                    if (ARM) { arm_round(0); arm_round(1); arm_round(2); }
+                } else {
+                    if (ARM) { arm_round(2); arm_round(1); arm_round(0); }
+                    if (LIM) { leg_round(3); leg_round(2); leg_round(1); leg_round(0); }
+                }
+#pragma unroll
+                for (int s = 0; s < 4; s++) {
+                    float dI = t[0];
+                    if (lam[0] + dI < 0.f) dI = -lam[0];
+                    const bool upd = mine && (leg == s);
+                    dI = upd ? dI : 0.f;
+                    lam[0] += dI;
+                    const float dl = bcast4(dI, s);
+                    const float rr = dl * denAll[s][0]; resid = fmaxf(resid, rr * rr);
+#pragma unroll
+                    for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][3 * s], dl, t[r]);
+                    if (ARM) {
+#pragma unroll
+                        for (int a = 0; a < ARM_KA; a++) tA[a] = fmaf(Aarm[a][3 * s], dl, tA[a]);
+                    }
+                }
+#pragma unroll
+                for (int s = 0; s < 4; s++) {
+                    // both friction rows of contact s belong to lane s: update t1, fold its change into the own t2 sum
+                    // locally, update t2, then broadcast the two changes together (one communication round per contact)
+                    const float lim = mu * lam[0];
+                    const bool upd = mine && (leg == s) && (lam[0] > 0.f);
+                    float dI1 = t[1];
+                    const float sum1 = lam[1] + dI1;
+                    if (sum1 < -lim) dI1 = -lim - lam[1]; else if (sum1 > lim) dI1 = lim - lam[1];
+                    dI1 = upd ? dI1 : 0.f;
+                    lam[1] += dI1;
+                    float dI2 = fmaf(A[2][3 * s + 1], dI1, t[2]);            // own lane: column 3*leg+1 == 3*s+1 when upd
+                    const float sum2 = lam[2] + dI2;
+                    if (sum2 < -lim) dI2 = -lim - lam[2]; else if (sum2 > lim) dI2 = lim - lam[2];
+                    dI2 = upd ? dI2 : 0.f;
+                    lam[2] += dI2;
+                    const float dl1 = bcast4(dI1, s), dl2 = bcast4(dI2, s);
+                    const float r1 = dl1 * denAll[s][1], r2 = dl2 * denAll[s][2];
+                    resid = fmaxf(resid, fmaxf(r1 * r1, r2 * r2));
+#pragma unroll
+                    for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][3 * s + 2], dl2, fmaf(A[r][3 * s + 1], dl1, t[r]));
+                    if (ARM) {
+#pragma unroll
+                        for (int a = 0; a < ARM_KA; a++) tA[a] = fmaf(Aarm[a][3 * s + 2], dl2, fmaf(Aarm[a][3 * s + 1], dl1, tA[a]));
+                    }
+                }
+                if (resid <= thr) running = false;
+            }
         }
         // ---- apply the net impulse: one more response pass ---------------------------------------------------
         float e1 = 0.f, e2 = 0.f, e3 = 0.f;
@@ -1127,10 +1225,10 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
 // Rex.ApplyAction + stepSimulation (rex_gym/model/rex.py:158-163,568-641) for the own leg's three motors
 static __constant__ float c_arm_rest[6] = {-1.6f, -1.6f, 0.f, 0.f, 1.6f, 0.f};   // ARM_POSES['rest'] rex_constants.py:3-8
 
-template <int TERRAIN, bool ARM, bool SENSOR>
+template <int TERRAIN, bool ARM, bool SENSOR, bool REPL>
 __device__ __forceinline__ void apply_action_and_step(const Params& P, const float* sm, Lane& L, int leg,
                                                       const float* cmd, float kp, float kd, Ground& G, Arm& AR,
-                                                      Sensor& S, bool valid) {
+                                                      Sensor& S, bool valid, float* pgs) {
     float tau[3];
     float tauA[ARM_NJ];
     const bool pd_delayed = SENSOR && P.lat_pd > 0.f;        // _GetPDObservation (rex.py:755-759): q, qd as they were pd_latency ago
@@ -1174,7 +1272,7 @@ __device__ __forceinline__ void apply_action_and_step(const Params& P, const flo
         L.tau_obs[j] = to;
         tau[j] = ((L.enabled >> j) & 1u) ? ta : 0.f;
     }
-    physics_substep<TERRAIN, ARM>(P, sm, L, leg, tau, G, AR, tauA);
+    physics_substep<TERRAIN, ARM, REPL>(P, sm, L, leg, tau, G, AR, tauA, pgs);
     if (SENSOR) sensor_push<ARM>(S, leg, L, AR, valid);         // Rex.ReceiveObservation (rex.py:162,726-733)
 }
 
@@ -1650,12 +1748,14 @@ __device__ __forceinline__ bool write_obs(const Params& P, int env, int leg, con
 // 4 -> 128 registers (16 warps/SM hide the serial PGS / ABA chains, large batches)
 // SENSOR: the observation-history / latency / noise model of Rex (rex.py:726-769) is compiled in (any latency or noise > 0);
 // the default build reads the true state and keeps no history.
-extern __shared__ __align__(16) float dyn_smem[];      // heightfield tiles, (BLOCK / 4) x TILE_FLOATS floats (random terrain only)
+// heightfield tiles, (BLOCK / 4) x TILE_FLOATS floats (random terrain only), then (BLOCK / 4) x PGS_ENV_FLOATS (replicated PGS only)
+extern __shared__ __align__(16) float dyn_smem[];
 template <int TASK, int SIGNAL, int TERRAIN, int OCC, bool ARM, bool SENSOR, int BLOCK>
 __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const Params P) {
     __shared__ __align__(16) float sm[ARM ? REXSIM_MT_FLOATS_ARM : REXSIM_MT_FLOATS];
     __shared__ __align__(8) uint64_t bar;
     float* tiles = dyn_smem;
+    float* pgs = dyn_smem + (TERRAIN == REXSIM_TERRAIN_RANDOM ? (BLOCK / 4) * TILE_FLOATS : 0) + (threadIdx.x >> 2) * PGS_ENV_FLOATS;
     tma_load_tables(sm, P.model, (ARM ? REXSIM_MT_FLOATS_ARM : REXSIM_MT_FLOATS) * 4, &bar);
 
     const int N = P.N;
@@ -1672,6 +1772,7 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
     constexpr int A = task_shape(TASK).act[SIGNAL == REXSIM_SIGNAL_IK ? 0 : 1];
     constexpr float bound = task_shape(TASK).bound[SIGNAL == REXSIM_SIGNAL_IK ? 0 : 1];
     constexpr int O = obs_dim(TASK, 12);
+    constexpr bool REPL = pgs_replicated(OCC, ARM, TERRAIN);
 
     Lane L; Task K; Arm AR;
     load_lane(P.sf, P.si, N, env, leg, L);
@@ -1713,7 +1814,7 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
 #if REXSIM_SYNC_SUBSTEP
         __syncthreads();
 #endif
-        apply_action_and_step<TERRAIN, ARM, SENSOR>(P, sm, L, leg, cmd, kp, kd, G, AR, S, valid);
+        apply_action_and_step<TERRAIN, ARM, SENSOR, REPL>(P, sm, L, leg, cmd, kp, kd, G, AR, S, valid, pgs);
         K.step_counter += 1;
     }
     if (G.miss) L.err |= REXSIM_FLAG_TILE_MISS;
@@ -1891,9 +1992,9 @@ __global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_
     if (SENSOR) S.ring = P.snap_ring + (size_t)field * S.depth * S.words;
     const int n1 = (task == REXSIM_TASK_POSES) ? 0 : 100;
     if (SENSOR && n1) sensor_push<ARM>(S, leg, L, AR, true);
-    for (int it = 0; it < n1; it++) apply_action_and_step<TERRAIN, ARM, SENSOR>(P, sm, L, leg, stand, P.cfg.motor_kp, P.cfg.motor_kd, G, AR, S, true);
+    for (int it = 0; it < n1; it++) apply_action_and_step<TERRAIN, ARM, SENSOR, false>(P, sm, L, leg, stand, P.cfg.motor_kp, P.cfg.motor_kd, G, AR, S, true, nullptr);
     const int n2 = (task == REXSIM_TASK_POSES) ? 0 : (int)(0.5 / P.cfg.sim_dt_d);
-    for (int it = 0; it < n2; it++) apply_action_and_step<TERRAIN, ARM, SENSOR>(P, sm, L, leg, ip, P.cfg.motor_kp, P.cfg.motor_kd, G, AR, S, true);
+    for (int it = 0; it < n2; it++) apply_action_and_step<TERRAIN, ARM, SENSOR, false>(P, sm, L, leg, ip, P.cfg.motor_kp, P.cfg.motor_kd, G, AR, S, true, nullptr);
     if (SENSOR) sensor_push<ARM>(S, leg, L, AR, true);
     {
         float* qf = snap_f + (size_t)field * NF; int32_t* qi = snap_i + (size_t)field * NI;
@@ -1936,7 +2037,8 @@ template <int TASK, int SIGNAL, int TERRAIN, int OCC, bool ARM, bool SENSOR, int
 static cudaError_t launch_step_variant(const Params& P, cudaStream_t st) {
     auto kern = step_kernel<TASK, SIGNAL, TERRAIN, OCC, ARM, SENSOR, BLOCK>;
     const int blocks = (P.N * 4 + BLOCK - 1) / BLOCK;
-    const size_t smem = TERRAIN == REXSIM_TERRAIN_RANDOM ? (size_t)(BLOCK / 4) * TILE_FLOATS * sizeof(float) : 0;
+    const size_t smem = ((TERRAIN == REXSIM_TERRAIN_RANDOM ? (size_t)(BLOCK / 4) * TILE_FLOATS : 0) +
+                         (pgs_replicated(OCC, ARM, TERRAIN) ? (size_t)(BLOCK / 4) * PGS_ENV_FLOATS : 0)) * sizeof(float);
     if (smem > 48 * 1024) {        // opt in once per kernel (the attribute is sticky)
         static bool done = false;
         if (!done) {

@@ -6,7 +6,7 @@ import torch
 import rex_gym_b200 as R
 tag = os.environ.get("REXSIM_LIB", "default").split("/")[-1]
 for task, kw in (("walk", dict(target_position=2.0, backwards=False)), ("gallop", dict(signal_type="ol", target_position=2.0))):
-    for n in (4096, 65536):
+    for n in (4096, 8448, 65536):        # one wave of the 255-register build, the largest batch it takes, the 128-register build
         env = R.BatchedRexEnv(task=task, num_envs=n, normalize=True, auto_reset=True, max_episode_steps=2000, **kw)
         env.reset()
         acts = torch.rand((40, n, env.action_dim), device="cuda") * 2 - 1
