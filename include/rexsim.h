@@ -66,8 +66,12 @@ enum {
 #define REXSIM_MT_BASEBOX (16 + 192 + 384 + 288) /* [3 boxes][8][3] base + chassis boxes */
 #define REXSIM_MT_FLOATS (16 + 192 + 384 + 288 + 72)
 #define REXSIM_MT_ARM REXSIM_MT_FLOATS  /* mark 'arm' only: [6 bodies][32]: jpos[3], jrot[9] (child->parent, row-major), axis[3],
-                                         * mass, com[3], inertia[6], lower, upper, pad[5] */
-#define REXSIM_MT_FLOATS_ARM (REXSIM_MT_FLOATS + 192)
+                                         * mass, com[3], inertia[6], lower, upper, npts, start, reach (largest point
+                                         * distance from the body origin), pad[2] */
+#define REXSIM_MT_ARMPTS (REXSIM_MT_FLOATS + 192)   /* mark 'arm' only: [104][3] collision points of the six arm bodies, body frame
+                                                     * (16 per cylinder, 8 box corners), body by body; [start, start + npts) above */
+#define REXSIM_MT_ARMPTS_N 104
+#define REXSIM_MT_FLOATS_ARM (REXSIM_MT_ARMPTS + 3 * REXSIM_MT_ARMPTS_N)
 
 typedef struct {
     int32_t num_envs;
@@ -148,7 +152,7 @@ int rexsim_reset(RexSim* sim, const int32_t* idx, int32_t k, float* obs_out, voi
 /* Physical state of every env, SoA on device: out_f dev [13 + 2*nm][N] =
  *   pos[3], quat[4] (x,y,z,w), linvel[3], angvel[3], q[nm], qd[nm];  out_i dev [4][N] =
  *   step_counter, env_step_counter, flags, last-substep contact mask (bit 0: base group, bit 1+2l: shoulder/leg
- *   boxes of leg l, bit 2+2l: foot box + toe hull of leg l) */
+ *   boxes of leg l, bit 2+2l: foot box + toe hull of leg l, bits 9..14: arm bodies 0..5 of mark 'arm') */
 int rexsim_get_state(RexSim* sim, float* out_f, int32_t* out_i, void* stream);
 int rexsim_set_state(RexSim* sim, const float* in_f, void* stream);
 /* raw SoA state for checkpoint/resume: [n_float][N] f32 and [n_int][N] i32 device buffers */

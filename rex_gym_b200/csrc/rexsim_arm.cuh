@@ -15,6 +15,8 @@ namespace rexsim {
 #define ARM_NJ 6
 #define ARM_KA 3          // arm joint-limit rows the fast solver path carries (the rest pose violates exactly three: joints 0, 1, 4)
 // model-table layout of one arm body (REXSIM_MT_ARM + 32*j): jpos[3] jrot[9] axis[3] mass com[3] inertia[6] lower upper
+// npts start reach: its collision points are [start, start + npts) of the point block at REXSIM_MT_ARMPTS, at most reach from
+// the body origin
 #define ARM_STRIDE 32
 
 struct Arm {
@@ -23,6 +25,7 @@ struct Arm {
     uint32_t enabled;         // 6 bits
     // per sub-step working set
     float S[ARM_NJ][6], U[ARM_NJ][6], cJ[ARM_NJ][6], k[ARM_NJ], u[ARM_NJ], qs[ARM_NJ];
+    float R[ARM_NJ][9], p[ARM_NJ][3];     // body orientation (columns) and origin relative to the base position
 };
 
 __device__ __forceinline__ SV ld6(const float* p) { SV r; r.a = mk(p[0], p[1], p[2]); r.l = mk(p[3], p[4], p[5]); return r; }
@@ -70,6 +73,9 @@ static __device__ __noinline__ void arm_inward(const float* __restrict__ AT, con
         }
         IAb[j] = I; pAb[j] = pA;
         st6(A.S[j], S); st6(A.cJ[j], cJ);
+        A.R[j][0] = Rj.c0.x; A.R[j][1] = Rj.c0.y; A.R[j][2] = Rj.c0.z; A.R[j][3] = Rj.c1.x; A.R[j][4] = Rj.c1.y;
+        A.R[j][5] = Rj.c1.z; A.R[j][6] = Rj.c2.x; A.R[j][7] = Rj.c2.y; A.R[j][8] = Rj.c2.z;
+        A.p[j][0] = pj.x; A.p[j][1] = pj.y; A.p[j][2] = pj.z;
         Rp = Rj; pp = pj; vp = v;
     }
 #pragma unroll 1
@@ -115,6 +121,27 @@ static __device__ __noinline__ void arm_row(const Arm& A, int jl, float sg, SV& 
         if (j <= jl) pD = sfma(ud * A.k[j], ld6(A.U[j]), pD);
     }
     g = pD;
+    SV w; w.a = mk(0, 0, 0); w.l = mk(0, 0, 0);
+#pragma unroll 1
+    for (int j = 0; j < ARM_NJ; j++) {
+        float e = (uu[j] - sdot(ld6(A.U[j]), w)) * A.k[j];
+        ee[j] = e;
+        w = sfma(e, ld6(A.S[j]), w);
+    }
+}
+// one contact row on arm body jb (unit spatial force F about the base position): joint Jacobian jq[] (S_j . F for the joints
+// j <= jb that carry the body, 0 beyond), base bias g, fixed-base joint response ee[], inward joint terms uu[]
+static __device__ __noinline__ void arm_force_row(const Arm& A, int jb, SV F, SV& g, float* jq, float* ee, float* uu) {
+    SV pD; pD.a = mk(0, 0, 0); pD.l = mk(0, 0, 0);
+#pragma unroll 1
+    for (int j = ARM_NJ - 1; j >= 0; j--) {
+        const SV S = ld6(A.S[j]);
+        jq[j] = j <= jb ? sdot(S, F) : 0.f;
+        float ud = j <= jb ? jq[j] - sdot(S, pD) : 0.f;
+        uu[j] = ud;
+        if (j <= jb) pD = sfma(ud * A.k[j], ld6(A.U[j]), pD);
+    }
+    g = pD - F;
     SV w; w.a = mk(0, 0, 0); w.l = mk(0, 0, 0);
 #pragma unroll 1
     for (int j = 0; j < ARM_NJ; j++) {

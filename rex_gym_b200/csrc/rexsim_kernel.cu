@@ -307,9 +307,15 @@ __device__ __forceinline__ void plane_space(V3 n, V3& p, V3& q) {   // btPlaneSp
     }
 }
 
-// generic-path Gauss-Seidel order after the limit rows (rows 0..2 of a lane = its three joint limits): normals (base, then per leg upper, foot), then frictions
-static __constant__ int c_seq_owner[27] = {0, 0, 0, 1, 1, 2, 2, 3, 3, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3};
-static __constant__ int c_seq_row[27] = {3, 6, 9, 6, 9, 6, 9, 6, 9, 4, 5, 7, 8, 10, 11, 7, 8, 10, 11, 7, 8, 10, 11, 7, 8, 10, 11};
+// generic-path Gauss-Seidel order after the limit rows (rows 0..2 of a lane = its three joint limits), the oracle's contact-group
+// order: normals (base, then per leg upper, foot, then the six arm bodies), then frictions in the same order.  Owner 0..3 = the
+// lane whose rows 3..11 hold the row; owner 4 = arm contact row ri = 3 * body + direction (lane 0; builds without the arm never
+// have one)
+#define SEQ_N 45
+static __constant__ int c_seq_owner[SEQ_N] = {0, 0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 4, 4, 4, 4,
+                                              0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 4, 4, 4, 4, 4, 4, 4, 4, 4};
+static __constant__ int c_seq_row[SEQ_N] = {3, 6, 9, 6, 9, 6, 9, 6, 9, 0, 3, 6, 9, 12, 15,
+                                            4, 5, 7, 8, 10, 11, 7, 8, 10, 11, 7, 8, 10, 11, 7, 8, 10, 11, 1, 2, 4, 5, 7, 8, 10, 11, 13, 14, 16, 17};
 
 // motor model + overheat (rex_gym/model/motor.py:76-143, rex_gym/model/rex.py:601-623) for one joint
 // q, qd: what the PD loop sees (pd_latency ago, rex.py:755-759); qd_true: the motor's actual rate (back-EMF, motor.py:131)
@@ -610,6 +616,32 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
     const bool active = best <= brk;
     const bool activeU = bestU <= brk;
     const bool activeB = (leg == 0) && (bestB <= brk);
+    // arm groups (owned by lane 0): the deepest collision point of each arm body, points within 0.06 m of z = 0 only
+    unsigned armC = 0u; float bestA[ARM ? ARM_NJ : 1]; V3 rcA[ARM ? ARM_NJ : 1], nrmA[ARM ? ARM_NJ : 1];
+    if (ARM && leg == 0) {
+        const float* AP = sm + REXSIM_MT_ARMPTS;
+#pragma unroll 1
+        for (int k = 0; k < ARM_NJ; k++) {
+            const float* T = sm + REXSIM_MT_ARM + ARM_STRIDE * k;
+            bestA[k] = 1e30f;
+            // a body whose origin is higher than its reach (largest point distance) above 0.06 m has no point to test
+            if (AR.p[k][2] + L.pos.z - T[29] > 0.06f) continue;
+            const M3 Rk = {mk(AR.R[k][0], AR.R[k][1], AR.R[k][2]), mk(AR.R[k][3], AR.R[k][4], AR.R[k][5]), mk(AR.R[k][6], AR.R[k][7], AR.R[k][8])};
+            const V3 pk = mk(AR.p[k][0], AR.p[k][1], AR.p[k][2]);
+            float bk = 1e30f; V3 rk = mk(0.f, 0.f, 0.f), nk = mk(0.f, 0.f, 1.f);
+            const int p0 = (int)T[28], p1e = p0 + (int)T[27];
+#pragma unroll 1
+            for (int j = p0; j < p1e; j++) {
+                V3 r = pk + mul(Rk, mk(AP[3 * j], AP[3 * j + 1], AP[3 * j + 2]));
+                if (r.z + L.pos.z > 0.06f) continue;
+                float d; V3 n;
+                ground_query<TERRAIN>(G, mk(r.x + L.pos.x, r.y + L.pos.y, r.z + L.pos.z), d, n);
+                if (d < bk) { bk = d; rk = r; nk = n; }
+            }
+            bestA[k] = bk; rcA[k] = rk; nrmA[k] = nk;
+            if (bk <= brk) armC |= 1u << k;
+        }
+    }
     // joint limits (btMultiBodyJointLimitConstraint: a row only while the limit is violated).  One violated limit in the leg
     // rides in the fast solver path (limJ / limSg / limPen); two or three go to the generic path, one row per joint.
     int limJ = -1; float limSg = 0.f, limPen = 0.f; int nviolL = 0;
@@ -623,7 +655,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
             if (L.q[j] - lo <= 0.f) { limJ = j; limSg = 1.f; limPen = L.q[j] - lo; nviolL++; limSgJ[j] = 1.f; limPenJ[j] = limPen; }
         }
     }
-    L.contact = (active ? 1 : 0) | (activeU ? 2 : 0) | (activeB ? 4 : 0);
+    L.contact = (active ? 1 : 0) | (activeU ? 2 : 0) | (activeB ? 4 : 0) | (int)(armC << 3);
     // arm joint limits (lane 0): bit j set when joint j is outside [lower, upper]; sign +1 lower / -1 upper
     unsigned armLim = 0u; float armSg[ARM_NJ], armPen[ARM_NJ];
     if (ARM) {
@@ -638,10 +670,10 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
             }
         }
     }
-    // bit 0: a foot contact; bit 1: rows only the generic path solves (body contacts, two violated limits in one leg, more than
-    // ARM_KA arm limits); bit 2: arm joint limits, bit 3: a leg joint limit -- both ride along in the fast path
+    // bit 0: a foot contact; bit 1: rows only the generic path solves (body and arm contacts, two violated limits in one leg,
+    // more than ARM_KA arm limits); bit 2: arm joint limits, bit 3: a leg joint limit -- both ride along in the fast path
     const int nArmLim = ARM ? __popc(armLim) : 0;
-    const unsigned envf = or4((active ? 1u : 0u) | ((activeU || activeB || nviolL > 1 || nArmLim > ARM_KA) ? 2u : 0u) |
+    const unsigned envf = or4((active ? 1u : 0u) | ((activeU || activeB || armC || nviolL > 1 || nArmLim > ARM_KA) ? 2u : 0u) |
                               (nArmLim ? 4u : 0u) | (limJ >= 0 ? 8u : 0u));
     float dqA[ARM_NJ];
     if (ARM) {
@@ -1065,6 +1097,14 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
             actbits |= 1u << ri;
             return relv;
         };
+        // right-hand side of a contact normal row: speculative below the slop, Baumgarte inside it; with m_splitImpulse the
+        // positional term of a penetration deeper than 0.04 m goes to m_rhsPenetration, which the multibody solver never applies
+        auto contact_rhs = [&](float relv, float dist, float dinv) -> float {
+            float pen = dist + 1e-5f;
+            float poserr = 0.f, velerr = -relv;
+            if (pen > 0.f) velerr -= pen * inv_dt; else poserr = -pen * P.cfg.erp_contact * inv_dt;
+            return (pen > -0.04f) ? (poserr + velerr) * dinv : velerr * dinv;
+        };
         auto setup_contact = [&](int r0, V3 r, V3 n, int kb, float dist) {
             V3 t1, t2;
             if (TERRAIN == REXSIM_TERRAIN_PLANE) { t1 = mk(0.f, -1.f, 0.f); t2 = mk(1.f, 0.f, 0.f); }
@@ -1075,12 +1115,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                 SV F; F.a = cross(r, dir); F.l = dir;
                 float j0 = kb >= 1 ? sdot(S1, F) : 0.f, j1 = kb >= 2 ? sdot(S2, F) : 0.f, j2 = kb >= 3 ? sdot(S3v, F) : 0.f;
                 float relv = setup_row(r0 + d, F, j0, j1, j2);
-                if (d == 0) {
-                    float pen = dist + 1e-5f;
-                    float poserr = 0.f, velerr = -relv;
-                    if (pen > 0.f) velerr -= pen * inv_dt; else poserr = -pen * P.cfg.erp_contact * inv_dt;
-                    rhs_[r0] = (pen > -0.04f) ? (poserr + velerr) * dinv_[r0] : velerr * dinv_[r0];
-                } else rhs_[r0 + d] = -relv * dinv_[r0 + d];
+                rhs_[r0 + d] = d == 0 ? contact_rhs(relv, dist, dinv_[r0]) : -relv * dinv_[r0 + d];
             }
         };
 #pragma unroll 1
@@ -1116,27 +1151,56 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                 rhsA_[j] = (armPen[j] > -0.04f) ? (-armPen[j] * P.cfg.erp_joint * inv_dt - relv) * dinvA_[j] : -relv * dinvA_[j];
             }
         }
+        // arm contact rows (lane 0): rows 3k, 3k+1, 3k+2 = normal, t1, t2 of arm body k.  Only the rows of bodies in contact are
+        // written, and only those are read (by lane 0, in the sweep below)
+        constexpr int NCA = ARM ? 3 * ARM_NJ : 1;
+        float gC_[NCA][6], bC_[NCA][6], jqC_[NCA][ARM_NJ], eeC_[NCA][ARM_NJ], uuC_[NCA][ARM_NJ];
+        float rhsC_[NCA], dinvC_[NCA], denC_[NCA], lamC_[NCA];
+        if (ARM) {
+#pragma unroll 1
+            for (int k = 0; k < ARM_NJ; k++) {
+                if (!((armC >> k) & 1u)) continue;
+                V3 t1, t2;
+                if (TERRAIN == REXSIM_TERRAIN_PLANE) { t1 = mk(0.f, -1.f, 0.f); t2 = mk(1.f, 0.f, 0.f); }
+                else plane_space(nrmA[k], t1, t2);
+#pragma unroll 1
+                for (int d = 0; d < 3; d++) {
+                    const int r = 3 * k + d;
+                    V3 dir = d == 0 ? nrmA[k] : (d == 1 ? t1 : t2);
+                    SV F; F.a = cross(rcA[k], dir); F.l = dir;
+                    SV gg; arm_force_row(AR, k, F, gg, jqC_[r], eeC_[r], uuC_[r]);
+                    SV bb = neg_mul(Minv, gg);
+                    st6(gC_[r], gg); st6(bC_[r], bb);
+                    float dn = -sdot(gg, bb), relv = sdot(F, vs);
+#pragma unroll
+                    for (int j = 0; j < ARM_NJ; j++) { dn = fmaf(jqC_[r][j], eeC_[r][j], dn); relv = fmaf(jqC_[r][j], AR.qs[j], relv); }
+                    denC_[r] = dn; dinvC_[r] = 1.0f / dn; lamC_[r] = 0.f;
+                    rhsC_[r] = d == 0 ? contact_rhs(relv, bestA[k], dinvC_[r]) : -relv * dinvC_[r];
+                }
+            }
+        }
         SV beta; beta.a = mk(0, 0, 0); beta.l = mk(0, 0, 0);
         float eps0 = 0.f, eps1 = 0.f, eps2 = 0.f, us0 = 0.f, us1 = 0.f, us2 = 0.f;
         // compact the Gauss-Seidel sequence to the rows that exist in this env (env-uniform: built from shuffled bits)
         constexpr int NLIM = ARM ? 12 + ARM_NJ : 12;     // limit rows in joint order: 3 per leg (lane), then the arm
-        unsigned char llist[NLIM], clist[27];
+        unsigned char llist[NLIM], clist[SEQ_N];
         int nl = 0, nc = 0;
         {
             unsigned actAll[4];
 #pragma unroll
             for (int o = 0; o < 4; o++) actAll[o] = __shfl_sync(env_mask(), actbits, o, 4);
             const unsigned armAll = ARM ? __shfl_sync(env_mask(), armLim, 0, 4) : 0u;
+            const unsigned armCAll = ARM ? __shfl_sync(env_mask(), armC, 0, 4) : 0u;
 #pragma unroll
             for (int idx = 0; idx < NLIM; idx++) {
                 const bool a = idx < 12 ? ((actAll[idx < 12 ? idx / 3 : 0] >> (idx % 3)) & 1u) : ((armAll >> (idx - 12)) & 1u);
                 if (a) llist[nl++] = (unsigned char)idx;
             }
 #pragma unroll 1
-            for (int t = 0; t < 27; t++) {
+            for (int t = 0; t < SEQ_N; t++) {
                 const int o = c_seq_owner[t], ri = c_seq_row[t];
-                const unsigned a = o == 0 ? actAll[0] : (o == 1 ? actAll[1] : (o == 2 ? actAll[2] : actAll[3]));
-                if ((a >> ri) & 1u) clist[nc++] = (unsigned char)t;
+                const unsigned a = o == 0 ? actAll[0] : (o == 1 ? actAll[1] : (o == 2 ? actAll[2] : (o == 3 ? actAll[3] : armCAll)));
+                if ((o < 4 ? (a >> ri) : (a >> (ri / 3))) & 1u) clist[nc++] = (unsigned char)t;
             }
         }
         bool running = true;
@@ -1164,7 +1228,33 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                     }
                     o = idx / 3; ri = idx % 3;
                 }
-                else { const int t = clist[tt - nl]; o = c_seq_owner[t]; ri = c_seq_row[t]; }
+                else {
+                    const int t = clist[tt - nl]; o = c_seq_owner[t]; ri = c_seq_row[t];
+                    if (ARM && o == 4) {                            // an arm contact row, owned by lane 0
+                        SV dBC; dBC.a = mk(0.f, 0.f, 0.f); dBC.l = mk(0.f, 0.f, 0.f);
+                        if (leg == 0) {
+                            const int ph = ri % 3;
+                            float rsumC = -(gC_[ri][0] * beta.a.x + gC_[ri][1] * beta.a.y + gC_[ri][2] * beta.a.z + gC_[ri][3] * beta.l.x + gC_[ri][4] * beta.l.y + gC_[ri][5] * beta.l.z);
+#pragma unroll
+                            for (int c = 0; c < ARM_NJ; c++) rsumC = fmaf(jqC_[ri][c], epsA[c], rsumC);
+                            float dIC = rhsC_[ri] - rsumC * dinvC_[ri];
+                            const float lr = lamC_[ri];
+                            if (ph == 0) { if (lr + dIC < 0.f) dIC = -lr; }
+                            else {
+                                const float ln = lamC_[ri - ph], lim = mu * ln, sum = lr + dIC;
+                                if (sum < -lim) dIC = -lim - lr; else if (sum > lim) dIC = lim - lr;
+                                dIC = (ln > 0.f) ? dIC : 0.f;
+                            }
+                            lamC_[ri] = lr + dIC;
+                            float rrC = dIC * denC_[ri]; resid = fmaxf(resid, rrC * rrC);
+#pragma unroll
+                            for (int c = 0; c < ARM_NJ; c++) { epsA[c] = fmaf(dIC, eeC_[ri][c], epsA[c]); usA[c] = fmaf(dIC, uuC_[ri][c], usA[c]); }
+                            dBC.a = mk(dIC * bC_[ri][0], dIC * bC_[ri][1], dIC * bC_[ri][2]); dBC.l = mk(dIC * bC_[ri][3], dIC * bC_[ri][4], dIC * bC_[ri][5]);
+                        }
+                        beta = beta + bcast4(dBC, 0);
+                        continue;
+                    }
+                }
                 const int ph = (ri < 3) ? 0 : ri % 3;                   // 0: unilateral row (limit / normal), 1/2: friction row
                 float rsum = Jq_[ri][0] * eps0 + Jq_[ri][1] * eps1 + Jq_[ri][2] * eps2
                            - (g_[ri][0] * beta.a.x + g_[ri][1] * beta.a.y + g_[ri][2] * beta.a.z + g_[ri][3] * beta.l.x + g_[ri][4] * beta.l.y + g_[ri][5] * beta.l.z);
@@ -1566,8 +1656,10 @@ __device__ __forceinline__ void load_task(const float* sf, const int32_t* si, in
 __device__ __forceinline__ void store_lane(float* sf, int32_t* si, int N, int env, int leg, const Lane& L, const Task& K, bool valid) {
     // shuffles first (all lanes participate), stores predicated on `valid`
     uint32_t en = or4(L.enabled << (3 * leg));
-    // contact mask in the oracle's group numbering: bit 0 base, bit 1+2l upper group of leg l, bit 2+2l foot group
-    uint32_t ct = or4((((uint32_t)L.contact & 1u) << (2 + 2 * leg)) | ((((uint32_t)L.contact >> 1) & 1u) << (1 + 2 * leg)) | (((uint32_t)L.contact >> 2) & 1u));
+    // contact mask in the oracle's group numbering: bit 0 base, bit 1+2l upper group of leg l, bit 2+2l foot group, bits 9..14 the
+    // arm bodies (lane 0 only)
+    uint32_t ct = or4((((uint32_t)L.contact & 1u) << (2 + 2 * leg)) | ((((uint32_t)L.contact >> 1) & 1u) << (1 + 2 * leg)) | (((uint32_t)L.contact >> 2) & 1u) |
+                      (((uint32_t)L.contact >> 3) << 9));
     if (!valid) return;
 #pragma unroll
     for (int j = 0; j < 3; j++) {

@@ -8,7 +8,8 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 MT_BASE, MT_LEG, MT_TOE, MT_BOX, MT_BASEBOX, MT_FLOATS = 0, 16, 208, 592, 880, 952
-MT_ARM, ARM_STRIDE, MT_FLOATS_ARM = 952, 32, 952 + 192
+MT_ARM, ARM_STRIDE, MT_ARMPTS, ARMPTS_N = 952, 32, 952 + 192, 104
+MT_FLOATS_ARM = MT_ARMPTS + 3 * ARMPTS_N
 MAX_TOE_PTS = 96     # profile vertices of the toe prism ((x, z) pairs: 2 * 96 floats fit the 384-float toe block)
 # Margin added to the toe hull's reach.  Bullet's URDF importer puts 1 mm on convex hulls, but the PyBullet trajectories
 # recovered from the reference's checkpoints (25 episodes, identical free fall from z = 0.21) put the touchdown where the
@@ -111,6 +112,11 @@ def pack_model_tables(mark="base"):
                 elif n != npts or not np.allclose(prof, prof0, atol=1e-12) or abs(w - w0) > 1e-12:
                     raise ValueError("the four toe hulls must be identical in their foot frames")
     if arm:
+        # collision points of each arm body, in the order the oracle scans them (oracle.load_model: contact group 9 + k)
+        pts = [np.asarray(s["points"], dtype=np.float64).reshape(-1, 3) for k in range(6) for s in bodies[13 + k]["shapes"]]
+        if sum(len(p) for p in pts) != ARMPTS_N:
+            raise ValueError("expected %d arm collision points" % ARMPTS_N)
+        start = 0
         for k in range(6):
             b = bodies[13 + k]
             if b["parent"] != (0 if k == 0 else 12 + k):
@@ -123,6 +129,10 @@ def pack_model_tables(mark="base"):
             t[o + 16:o + 19] = b["com"]
             t[o + 19:o + 25] = _sym6(b["inertia"])
             t[o + 25], t[o + 26] = b["lower"], b["upper"]
+            p = np.concatenate([np.asarray(s["points"], dtype=np.float64).reshape(-1, 3) for s in b["shapes"]])
+            t[o + 27], t[o + 28], t[o + 29] = len(p), start, np.linalg.norm(p, axis=1).max()
+            t[MT_ARMPTS + 3 * start:MT_ARMPTS + 3 * (start + len(p))] = p.reshape(-1)
+            start += len(p)
     return t.astype(np.float32), int(npts)
 
 

@@ -121,6 +121,27 @@ def test_model_table_packer_layout():
     assert t[MT_BOX:MT_BASEBOX].reshape(4, 3, 8, 3).shape == (4, 3, 8, 3)
 
 
+def test_arm_collision_points_are_the_oracles():
+    """The arm's collision points (mark 'arm': six contact groups, 16 per cylinder + the 8 corners of arm_section_4's box) are
+    packed body by body in the order the oracle scans its contact groups 9-14, with each body's count, start and reach."""
+    from oracle.oracle import load_model
+    from rex_gym_b200.model_tables import pack_model_tables, MT_ARM, ARM_STRIDE, MT_ARMPTS, ARMPTS_N, MT_FLOATS_ARM
+    t, _ = pack_model_tables("arm")
+    assert t.shape == (MT_FLOATS_ARM,) and MT_FLOATS_ARM * 4 % 16 == 0 and ARMPTS_N == 104
+    m, _ = load_model("arm")
+    assert m.nshape == 15
+    for k in range(6):
+        o = MT_ARM + ARM_STRIDE * k
+        g = 9 + k
+        n, s = int(t[o + 27]), int(t[o + 28])
+        assert n == m.shape_npts[g] == (24 if k == 4 else 16)
+        ref = np.array([m.pts[m.shape_start[g] + v][:] for v in range(n)])
+        assert all(m.pt_body[m.shape_start[g] + v] == 13 + k for v in range(n))
+        np.testing.assert_array_equal(t[MT_ARMPTS + 3 * s:MT_ARMPTS + 3 * (s + n)].reshape(n, 3), ref.astype(np.float32))
+        assert abs(t[o + 29] - np.linalg.norm(ref, axis=1).max()) < 1e-6
+    assert int(t[MT_ARM + ARM_STRIDE * 5 + 28]) + int(t[MT_ARM + ARM_STRIDE * 5 + 27]) == ARMPTS_N
+
+
 def test_no_cpu_fallback():
     import torch
     import rex_gym_b200 as R
