@@ -161,7 +161,7 @@ struct RexoSim {
     int obs_dim, act_dim;
     double init_pose[REXO_MAXDOF];   /* task init pose incl. arm rest */
     double stand_pose[REXO_MAXDOF];  /* Rex.initial_pose = INIT_POSES['stand'] (+arm rest) */
-    double field_zoff[256];          /* (hmin+hmax)/2 per field */
+    double* field_zoff;              /* [nfields]: (hmin+hmax)/2 per field */
     /* sensor history: one ring per env, then one per reset snapshot; ctrl = the control observation of the last ReceiveObservation */
     struct Hist* hist;
     double (*ctrl)[REXO_OBSW];
@@ -1196,6 +1196,7 @@ RexoSim* rexo_create(const RexoModel* model, const RexoConfig* cfg) {
     else if (cfg->signal == REXO_SIGNAL_OL) ip = POSE_STAND_OL;
     for (int i = 0; i < 12; i++) { s->init_pose[i] = ip[i]; s->stand_pose[i] = POSE_STAND[i]; }
     for (int i = 12; i < model->nmotor; i++) { s->init_pose[i] = ARM_REST[i - 12]; s->stand_pose[i] = ARM_REST[i - 12]; }
+    s->field_zoff = (double*)calloc(cfg->nfields > 0 ? cfg->nfields : 1, sizeof(double));
     for (int f = 0; f < cfg->nfields && cfg->fields; f++) {
         float lo = 1e30f, hi = -1e30f;
         for (int a = 0; a < 65536; a++) { float h = cfg->fields[(size_t)f * 65536 + a]; if (h < lo) lo = h; if (h > hi) hi = h; }
@@ -1203,7 +1204,7 @@ RexoSim* rexo_create(const RexoModel* model, const RexoConfig* cfg) {
     }
     return s;
 }
-void rexo_destroy(RexoSim* s) { if (!s) return; free(s->env); free(s->snapshot); free(s->hist); free(s->ctrl); free(s); }
+void rexo_destroy(RexoSim* s) { if (!s) return; free(s->env); free(s->snapshot); free(s->hist); free(s->ctrl); free(s->field_zoff); free(s); }
 void rexo_sensor_clear(RexoSim* s, int i) { if (s->hist) { s->hist[i].len = 0; s->hist[i].head = REXO_HIST - 1; } }
 void rexo_sensor_push(RexoSim* s, int i, const double* obs) { if (s->hist) hist_push(&s->hist[i], obs, 3 * s->m.nmotor + 7); }
 void rexo_sensor_delayed(RexoSim* s, int i, double latency, double* out) {

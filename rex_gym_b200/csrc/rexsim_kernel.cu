@@ -248,8 +248,9 @@ __device__ __forceinline__ SV neg_mul(const Sym6& M, SV p) {   // -(M p)
 
 // ground query --------------------------------------------------------------------------------------
 // Random terrain (rex_gym/model/terrain.py:32-53): every env stages a 16x16-cell (0.8 m x 0.8 m) window of its
-// heightfield, centred on the base, in shared memory once per control step; all contact queries of the step's
-// sub-steps read that tile (4 heights per query) instead of the 256x256 field in L2.
+// heightfield in shared memory once per control step; all contact queries of the step's sub-steps read that tile
+// (4 heights per query) instead of the 256x256 field in L2.  The window's origin is the base's cell minus 8, clamped to
+// [0, 239]: it holds queries 7-8 cells (0.35-0.40 m) ahead of the base in +x / +y and 8-9 cells behind it.
 #define TILE_CELLS 16
 #define TILE_V (TILE_CELLS + 1)          // vertices per side
 #define TILE_STRIDE (TILE_V + 1)         // padded row
