@@ -127,7 +127,10 @@ int rexsim_action_dim(int32_t task, int32_t signal);
 int rexsim_state_words(const RexSimConfig* cfg, int32_t* n_float, int32_t* n_int);
 
 /* model_tables: HOST pointer to REXSIM_MT_FLOATS (12 motors) or REXSIM_MT_FLOATS_ARM (18 motors) floats.  Allocates device state, computes the settled
- * reset snapshot(s) (600 physics sub-steps, rex.py:314-323) and synchronises. */
+ * reset snapshot(s) (600 physics sub-steps, rex.py:314-323) and synchronises.
+ * Returns REXSIM_ERR_UNSUPPORTED when floor(1 / sim_dt_d) >= 1023: the overheat protection (rex.py:601-608) switches a motor off
+ * once it has been hot for more than floor(1 / sim_dt) sub-steps, and its per-motor counter is a 10-bit field that stops at 1023.
+ * Time steps of 1/1023 s and below are refused; every configuration of the reference (1 ms) is accepted. */
 int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_model_floats, RexSim** out);
 void rexsim_destroy(RexSim* sim);
 

@@ -69,6 +69,10 @@ static int validate(const RexSimConfig* c) {
     if (c->num_motors == 18 && !(c->task == REXSIM_TASK_STANDUP || (c->task == REXSIM_TASK_WALK && c->signal == REXSIM_SIGNAL_IK)))
         return fail(REXSIM_ERR_UNSUPPORTED, "mark='arm' is built for the standup and walk-ik tasks");
     if (c->action_repeat <= 0 || c->solver_iterations <= 0 || !(c->sim_dt_d > 0)) return fail(REXSIM_ERR_INVALID, "bad time stepping");
+    // the step kernel switches a motor off once its overheat count c > floor(1 / sim_dt) (rex.py:601-608); c is a 10-bit
+    // saturating field, so at floor(1 / sim_dt) >= 1023 the protection could never fire
+    if ((uint32_t)(1.0 / c->sim_dt_d) >= 1023u)
+        return fail(REXSIM_ERR_UNSUPPORTED, "sim_dt too small for the 10-bit overheat counter: needs floor(1 / sim_dt) <= 1022");
     if (c->terrain == REXSIM_TERRAIN_RANDOM && (c->nfields <= 0 || !c->fields)) return fail(REXSIM_ERR_INVALID, "random terrain needs a heightfield bank");
     if (c->terrain != REXSIM_TERRAIN_PLANE && c->terrain != REXSIM_TERRAIN_RANDOM) return fail(REXSIM_ERR_UNSUPPORTED, "terrain type");
     if (c->toe_npts <= 0 || c->toe_npts > REXSIM_MAX_TOE_PTS) return fail(REXSIM_ERR_MODEL, "toe_npts out of range");

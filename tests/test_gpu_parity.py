@@ -67,22 +67,52 @@ def _oracle_state(o, n):
     return {k: np.stack([s[k] for s in st]) for k in st[0]}
 
 
+# Packed overheat protection (rex.py:601-608) in the int SoA state: motor m's 10-bit saturating counter is field m % 3 of word
+# I_OVH + m // 3 for the legs (m < 12) and of word I_OVHA + (m - 12) // 3 for the arm; its enabled bit is bit 8 + m of I_FLAGS
+# (legs 8-19, arm 20-25).  The oracle counts in an int32 that goes on past 1023 while a switched-off motor stays hot.
+I_FLAGS, I_OVH, I_OVHA, FL_ENABLED_SHIFT = 2, 9, 14, 8
+
+
+def _protection_word(m):
+    return (I_OVH + m // 3) if m < 12 else (I_OVHA + (m - 12) // 3)
+
+
 def _sync_motor_protection(env, ora, n):
-    """Copy the oracle's overheat counters / motor-enabled bits (rex.py:601-608 state) into the raw SoA state: the
-    public set_state only carries the physical state, and a counter that is one sub-step off re-fires its event."""
+    """Copy the oracle's overheat counters / motor-enabled bits (rex.py:601-608 state, arm included) into the raw SoA state:
+    the public set_state only carries the physical state, and a counter that is one sub-step off re-fires its event."""
     si = env._state_i
-    host = si.cpu().numpy()
+    host = si.cpu().numpy().astype(np.int64) & 0xFFFFFFFF
+    nm = ora.nm
+    mask = (1 << (FL_ENABLED_SHIFT + nm)) - (1 << FL_ENABLED_SHIFT)
     for i in range(n):
         e = ora.env(i)
-        en = 0
-        for l in range(4):
-            w = 0
-            for j in range(3):
-                w |= min(int(e.overheat[3 * l + j]), 1023) << (10 * j)
-                en |= (1 if e.enabled[3 * l + j] else 0) << (3 * l + j)
-            host[9 + l, i] = w
-        host[2, i] = (host[2, i] & 0xFF) | (en << 8) | (host[2, i] & ~0xFFFFF)
-    si.copy_(torch.from_numpy(host).to(si.device))
+        en, words = 0, {}
+        for m in range(nm):
+            w = _protection_word(m)
+            words[w] = words.get(w, 0) | (min(int(e.overheat[m]), 1023) << (10 * (m % 3)))
+            en |= (1 if e.enabled[m] else 0) << (FL_ENABLED_SHIFT + m)
+        for w, v in words.items():
+            host[w, i] = v
+        host[I_FLAGS, i] = (host[I_FLAGS, i] & ~mask) | en
+    si.copy_(torch.from_numpy(host.astype(np.uint32).view(np.int32)).to(si.device))
+
+
+def _motor_protection(env, n=None):
+    """-> (counters [N][nm], enabled [N][nm] bool) read back from the raw SoA state of the first n envs."""
+    n = env.num_envs if n is None else n
+    si = env._state_i[:, :n].cpu().numpy().astype(np.int64) & 0xFFFFFFFF
+    nm = env.num_motors
+    cnt = np.stack([(si[_protection_word(m)] >> (10 * (m % 3))) & 1023 for m in range(nm)], 1)
+    en = np.stack([(si[I_FLAGS] >> (FL_ENABLED_SHIFT + m)) & 1 for m in range(nm)], 1).astype(bool)
+    return cnt, en
+
+
+def _oracle_protection(ora, n=None):
+    """-> the oracle's (min(counter, 1023) [N][nm], enabled [N][nm] bool): what the kernel's saturating fields must hold."""
+    n = ora.N if n is None else n
+    cnt = np.array([[min(int(ora.env(i).overheat[m]), 1023) for m in range(ora.nm)] for i in range(n)])
+    en = np.array([[bool(ora.env(i).enabled[m]) for m in range(ora.nm)] for i in range(n)])
+    return cnt, en
 
 
 def _toe_mask(o, i):
@@ -118,9 +148,14 @@ def test_loaded_library_is_the_in_tree_cuda_build():
     assert "librexsim.so" in maps
 
 
-@pytest.mark.parametrize("task,sig,kw", CASES)
+# the settle runs once per field of the bank: standup's hold leaves its foot motors counting on every field
+RESET_CASES = CASES + [("standup", "ol", dict(terrain_type="random", num_fields=4))]
+
+
+@pytest.mark.parametrize("task,sig,kw", RESET_CASES)
 def test_reset_settle_and_draws(task, sig, kw):
-    """Rex.Reset's 600 settle sub-steps run on the GPU; task draws are bit-exact."""
+    """Rex.Reset's 600 settle sub-steps run on the GPU; task draws are bit-exact, and so are the overheat counters and
+    motor-enabled bits the hold leaves (standup: its four foot motors are still hot when the hold ends)."""
     n = 16
     env, ora = _env(task, n, signal_type=sig, seed=77, **kw), _oracle(task, n, signal_type=sig, seed=77, **kw)
     og, oc = env.reset(), ora.reset()
@@ -154,6 +189,15 @@ def test_reset_settle_and_draws(task, sig, kw):
     flags = si[2]
     np.testing.assert_array_equal((flags >> 3) & 1, [ora.env(i).backwards for i in range(n)])
     np.testing.assert_array_equal((flags >> 4) & 1, [ora.env(i).clockwise for i in range(n)])
+    cnt, en = _motor_protection(env)
+    ocnt, oen = _oracle_protection(ora)
+    np.testing.assert_array_equal(cnt, ocnt)
+    np.testing.assert_array_equal(en, oen)
+    assert en.all()
+    if task == "standup":
+        # the feet are past 2.45 N m over the hold's last 500 sub-steps (flat ground; some fields of the bank hold them longer)
+        feet = cnt[:, [2, 5, 8, 11]]
+        assert (feet == 500).all() if "terrain_type" not in kw else (feet >= 500).all(), feet
     assert env.check_errors() == 0
     env.close()
 
