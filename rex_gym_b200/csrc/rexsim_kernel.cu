@@ -903,40 +903,47 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
             }
 #pragma unroll
             for (int j = 0; j < NF; j++) lamF[j] = 0.f;
-            for (int it = 0; it < iters && running; it++) {
-                L.cost++;
+            // One warp per scheduler issues about one instruction per cycle here, so the loop's length is its instruction count.
+            // The residual is the largest |dI * den|, squared once at the test: fl(x * x) is monotone in |x|, so the early-out
+            // decision is the one the per-row squares give.  The iteration count goes to L.cost after the loop.
+            int it = 0;
+            for (; it < iters && running; it++) {
                 float resid = 0.f;
 #pragma unroll
                 for (int s = 0; s < 4; s++) {
                     const int n = 3 * s;
                     const float dI = fmaxf(T[n], -lamF[n]);
                     lamF[n] += dI;
-                    const float rr = dI * denF[n]; resid = fmaxf(resid, rr * rr);
+                    resid = fmaxf(resid, fabsf(dI * denF[n]));
 #pragma unroll
                     for (int j = 0; j < NF; j++) T[j] = fmaf(Af[j][n], dI, T[j]);
                 }
 #pragma unroll
                 for (int s = 0; s < 4; s++) {
-                    // the clamp bounds and the zero of a frozen pair are known before the row's sum: the chain is add, compare, 2 selects
+                    // friction clamp: the change is the sum when inside [-lim, lim], else the bound minus the impulse (the lower
+                    // bound wins, as in the shuffle form), and zero while the normal impulse is zero.  Written as overrides under
+                    // predicates, a row is one add, two compares folding in `upd`, one select and two predicated adds
                     const int n = 3 * s, f1 = n + 1, f2 = n + 2;
                     const float lim = mu * lamF[n];
                     const bool upd = lamF[n] > 0.f;
-                    const float lo1 = upd ? -lim - lamF[f1] : 0.f, hi1 = upd ? lim - lamF[f1] : 0.f;
                     const float sum1 = lamF[f1] + T[f1];
-                    const float dI1 = sum1 < -lim ? lo1 : (sum1 > lim ? hi1 : (upd ? T[f1] : 0.f));
+                    float dI1 = upd ? T[f1] : 0.f;
+                    if (upd && sum1 > lim) dI1 = lim - lamF[f1];
+                    if (upd && sum1 < -lim) dI1 = -lim - lamF[f1];
                     lamF[f1] += dI1;
                     const float t2 = fmaf(Af[f2][f1], dI1, T[f2]);
-                    const float lo2 = upd ? -lim - lamF[f2] : 0.f, hi2 = upd ? lim - lamF[f2] : 0.f;
                     const float sum2 = lamF[f2] + t2;
-                    const float dI2 = sum2 < -lim ? lo2 : (sum2 > lim ? hi2 : (upd ? t2 : 0.f));
+                    float dI2 = upd ? t2 : 0.f;
+                    if (upd && sum2 > lim) dI2 = lim - lamF[f2];
+                    if (upd && sum2 < -lim) dI2 = -lim - lamF[f2];
                     lamF[f2] += dI2;
-                    const float r1 = dI1 * denF[f1], r2 = dI2 * denF[f2];
-                    resid = fmaxf(resid, fmaxf(r1 * r1, r2 * r2));
+                    resid = fmaxf(resid, fmaxf(fabsf(dI1 * denF[f1]), fabsf(dI2 * denF[f2])));
 #pragma unroll
                     for (int j = 0; j < NF; j++) T[j] = fmaf(Af[j][f2], dI2, fmaf(Af[j][f1], dI1, T[j]));
                 }
-                if (resid <= thr) running = false;
+                if (resid * resid <= thr) running = false;
             }
+            L.cost += it;
 #pragma unroll
             for (int d = 0; d < 3; d++)
                 lam[d] = leg == 0 ? lamF[d] : (leg == 1 ? lamF[3 + d] : (leg == 2 ? lamF[6 + d] : lamF[9 + d]));
@@ -946,8 +953,9 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
             for (int s = 0; s < 4; s++)
 #pragma unroll
                 for (int d = 0; d < NR; d++) denAll[s][d] = bcast4(den[d], s);
-            for (int it = 0; it < iters && running; it++) {
-                L.cost++;
+            // residual and iteration count as in the replicated form: the largest |dI * den| squared once at the test
+            int it = 0;
+            for (; it < iters && running; it++) {
                 float resid = 0.f;
                 // joint-limit rows first, in joint order (4 legs, then the arm), the direction alternating per iteration
                 // (btMultiBodyConstraintSolver::solveSingleIteration): even iterations descending, odd ascending
@@ -957,7 +965,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                     dI = (actA[a] && leg == 0) ? dI : 0.f;
                     lamA[a] += dI;
                     const float dl = bcast4(dI, 0);
-                    const float rr = dl * denA[a]; resid = fmaxf(resid, rr * rr);
+                    resid = fmaxf(resid, fabsf(dl * denA[a]));
 #pragma unroll
                     for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][CA + a], dl, t[r]);
 #pragma unroll
@@ -969,7 +977,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                     dI = (hasL && leg == s) ? dI : 0.f;
                     lam[NR - 1] += dI;
                     const float dl = bcast4(dI, s);
-                    const float rr = dl * denAll[s][NR - 1]; resid = fmaxf(resid, rr * rr);
+                    resid = fmaxf(resid, fabsf(dl * denAll[s][NR - 1]));
 #pragma unroll
                     for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][CL + s], dl, t[r]);
                     if (ARM) {
@@ -992,7 +1000,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                     dI = upd ? dI : 0.f;
                     lam[0] += dI;
                     const float dl = bcast4(dI, s);
-                    const float rr = dl * denAll[s][0]; resid = fmaxf(resid, rr * rr);
+                    resid = fmaxf(resid, fabsf(dl * denAll[s][0]));
 #pragma unroll
                     for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][3 * s], dl, t[r]);
                     if (ARM) {
@@ -1006,19 +1014,19 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                     // locally, update t2, then broadcast the two changes together (one communication round per contact)
                     const float lim = mu * lam[0];
                     const bool upd = mine && (leg == s) && (lam[0] > 0.f);
-                    float dI1 = t[1];
-                    const float sum1 = lam[1] + dI1;
-                    if (sum1 < -lim) dI1 = -lim - lam[1]; else if (sum1 > lim) dI1 = lim - lam[1];
-                    dI1 = upd ? dI1 : 0.f;
+                    const float sum1 = lam[1] + t[1];
+                    float dI1 = upd ? t[1] : 0.f;
+                    if (upd && sum1 > lim) dI1 = lim - lam[1];
+                    if (upd && sum1 < -lim) dI1 = -lim - lam[1];
                     lam[1] += dI1;
-                    float dI2 = fmaf(A[2][3 * s + 1], dI1, t[2]);            // own lane: column 3*leg+1 == 3*s+1 when upd
-                    const float sum2 = lam[2] + dI2;
-                    if (sum2 < -lim) dI2 = -lim - lam[2]; else if (sum2 > lim) dI2 = lim - lam[2];
-                    dI2 = upd ? dI2 : 0.f;
+                    const float t2 = fmaf(A[2][3 * s + 1], dI1, t[2]);      // own lane: column 3*leg+1 == 3*s+1 when upd
+                    const float sum2 = lam[2] + t2;
+                    float dI2 = upd ? t2 : 0.f;
+                    if (upd && sum2 > lim) dI2 = lim - lam[2];
+                    if (upd && sum2 < -lim) dI2 = -lim - lam[2];
                     lam[2] += dI2;
                     const float dl1 = bcast4(dI1, s), dl2 = bcast4(dI2, s);
-                    const float r1 = dl1 * denAll[s][1], r2 = dl2 * denAll[s][2];
-                    resid = fmaxf(resid, fmaxf(r1 * r1, r2 * r2));
+                    resid = fmaxf(resid, fmaxf(fabsf(dl1 * denAll[s][1]), fabsf(dl2 * denAll[s][2])));
 #pragma unroll
                     for (int r = 0; r < NR; r++) t[r] = fmaf(A[r][3 * s + 2], dl2, fmaf(A[r][3 * s + 1], dl1, t[r]));
                     if (ARM) {
@@ -1026,8 +1034,9 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                         for (int a = 0; a < ARM_KA; a++) tA[a] = fmaf(Aarm[a][3 * s + 2], dl2, fmaf(Aarm[a][3 * s + 1], dl1, tA[a]));
                     }
                 }
-                if (resid <= thr) running = false;
+                if (resid * resid <= thr) running = false;
             }
+            L.cost += it;
         }
         // ---- apply the net impulse: one more response pass ---------------------------------------------------
         float e1 = 0.f, e2 = 0.f, e3 = 0.f;
