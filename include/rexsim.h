@@ -73,6 +73,19 @@ enum {
 #define REXSIM_MT_ARMPTS_N 104
 #define REXSIM_MT_FLOATS_ARM (REXSIM_MT_ARMPTS + 3 * REXSIM_MT_ARMPTS_N)
 
+/* float offsets inside the render table (rex_gym_b200/model_tables.py pack_render_tables): everything visual */
+#define REXSIM_RT_NSHAPES 26        /* 3 base boxes, 12 leg boxes (leg-major: shoulder, leg, foot), 4 toes, 6 arm cylinders, arm box */
+#define REXSIM_RT_LIGHT 0           /* unit direction towards the light [3], ambient, diffuse weight (Lambert + ambient) */
+#define REXSIM_RT_SKY 5             /* rgb of misses and of hits outside [near, far] */
+#define REXSIM_RT_CHECK 8           /* ground checker: two rgb tones, square size [m] */
+#define REXSIM_RT_CAM 15            /* vertical field of view [deg], near, far */
+#define REXSIM_RT_COLOR 18          /* [REXSIM_RT_NSHAPES][3] rgb: URDF visual material of each shape's link */
+#define REXSIM_RT_TOE 96            /* [toe_npts <= REXSIM_MAX_TOE_PTS][3] edge planes (nx, nz, d) of the toe profile, foot frame */
+#define REXSIM_RT_TOESPH 384        /* bounding sphere of the toe prism in the foot frame: centre x, centre z, radius, pad */
+#define REXSIM_RT_CYL 388           /* mark 'arm': [6 arm bodies][8] cylinder centre[3], axis[3], radius, half length, body frame */
+#define REXSIM_RT_ARMBOX 436        /* mark 'arm': arm body index of the box, then its [8][3] corners in that body's frame */
+#define REXSIM_RT_FLOATS 464
+
 typedef struct {
     int32_t num_envs;
     int32_t task, signal, terrain;
@@ -173,6 +186,15 @@ int rexsim_last_command(RexSim* sim, float** cmd);
 /* solver cost of every env's last control step (what rexsim_rebalance sorts by): dev [N] int32, the PGS iterations of its sub-steps
  * plus 64 per sub-step on the generic path */
 int rexsim_solver_cost(RexSim* sim, int32_t** cost);
+/* Render table (REXSIM_RT_FLOATS floats, HOST pointer): copied into the buffer rexsim_create allocated for it; synchronous.
+ * Kept out of RexSimConfig so that the configuration the step kernels receive stays as it is. */
+int rexsim_set_render_tables(RexSim* sim, const float* render_tables, int32_t n_floats);
+/* RexGymEnv.render(mode="rgb_array") (rex_gym_env.py:416-439) for k envs at once: idx dev [k] int32, rgb dev [k][height][width][3]
+ * uint8, row 0 at the top.  Ray-casts the collision geometry of each env from its state through the reference's follow camera
+ * (target = base position; distance [m], yaw and pitch [deg]; the lens of the render table).  Reads the state only.  Sizes
+ * 1..4096 per side, k >= 0.  An index outside [0, N) gives a sky image and sets REXSIM_FLAG_BAD_INDEX in the aggregate word. */
+int rexsim_render(RexSim* sim, const int32_t* idx, int32_t k, int32_t width, int32_t height, float distance, float yaw_deg,
+                  float pitch_deg, uint8_t* rgb, void* stream);
 /* kernels launched by this handle since create (the bench reports it) */
 int64_t rexsim_launch_count(const RexSim* sim);
 /* which build of the step kernel the last rexsim_step / rexsim_step_host launched (all 0 before the first step): CTA size,

@@ -41,7 +41,7 @@ AGENT_EXPORTS = ["rexagent_policy_floats", "rexagent_value_floats", "rexagent_cr
 EXPORTS = ["rexsim_obs_dim", "rexsim_action_dim", "rexsim_state_words", "rexsim_create", "rexsim_destroy",
            "rexsim_step", "rexsim_step_host", "rexsim_host_out_bytes", "rexsim_rebalance", "rexsim_reset", "rexsim_get_state", "rexsim_set_state", "rexsim_state_buffers",
            "rexsim_error_flags", "rexsim_clear_errors", "rexsim_last_command", "rexsim_solver_cost", "rexsim_launch_count", "rexsim_last_step_build", "rexsim_last_error", "rexsim_rand_u32",
-           "rexsim_noise", "rexsim_history_depth", "rexsim_history_buffer"]
+           "rexsim_noise", "rexsim_history_depth", "rexsim_history_buffer", "rexsim_set_render_tables", "rexsim_render"]
 
 _LIB = None
 
@@ -88,6 +88,9 @@ def load():
     L.rexsim_noise.restype = C.c_float
     L.rexsim_history_depth.argtypes = [C.POINTER(RexSimConfig)]
     L.rexsim_history_buffer.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
+    L.rexsim_set_render_tables.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
+    L.rexsim_render.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_float,
+                                C.c_void_p, C.c_void_p]
     # include/rexsim_agent.h
     cfgp = C.POINTER(RexAgentConfig)
     L.rexagent_policy_floats.argtypes = [cfgp]; L.rexagent_policy_floats.restype = C.c_int64

@@ -12,6 +12,8 @@ cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, cudaS
 cudaError_t launch_get_state(const Params& P, float* out_f, int32_t* out_i, cudaStream_t st);
 cudaError_t launch_set_state(const Params& P, const float* in_f, cudaStream_t st);
 cudaError_t launch_rebalance(const int32_t* cost, int n, int32_t* hist, int32_t* perm, cudaStream_t st);
+cudaError_t launch_render(const Params& P, const float* rt, const float* zrange, const int32_t* idx, int k, int W, int H,
+                          float distance, float yaw_deg, float pitch_deg, uint8_t* rgb, cudaStream_t st, int64_t* launches);
 }  // namespace rexsim
 
 using namespace rexsim;
@@ -24,6 +26,9 @@ struct RexSim {
     float* d_snap_f = nullptr;
     int32_t* d_snap_i = nullptr;
     float* d_zoff = nullptr;
+    float* d_zrange = nullptr;         // [nfields][2] lowest / highest centred height of each field (renderer)
+    float* d_rt = nullptr;             // render table (rexsim_set_render_tables)
+    bool rt_set = false;
     int32_t* d_err = nullptr;
     float* d_cmd = nullptr;
     int32_t* d_perm = nullptr;         // slot -> env, sorted by solver cost (rexsim_rebalance)
@@ -136,6 +141,7 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
     CK(cudaMalloc(&s->d_cost, (size_t)N * sizeof(int32_t)));
     CK(cudaMemset(s->d_cost, 0, (size_t)N * sizeof(int32_t)));
     CK(cudaMalloc(&s->d_hist, 256 * sizeof(int32_t)));
+    CK(cudaMalloc(&s->d_rt, REXSIM_RT_FLOATS * sizeof(float)));
     if (sensor_on(cfg)) {
         Params& P = s->P;
         const double dt = cfg->sim_dt_d;
@@ -158,15 +164,18 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
     CK(cudaMemset(s->d_out, 0, (size_t)rexsim_host_out_bytes(s)));
     if (cfg->terrain == REXSIM_TERRAIN_RANDOM) {
         // vertical centring of each field: btHeightfieldTerrainShape local origin = (min+max)/2
-        std::vector<float> h((size_t)65536), zo(cfg->nfields);
+        std::vector<float> h((size_t)65536), zo(cfg->nfields), zr(2 * (size_t)cfg->nfields);
         for (int f = 0; f < cfg->nfields; f++) {
             CK(cudaMemcpy(h.data(), cfg->fields + (size_t)f * 65536, 65536 * sizeof(float), cudaMemcpyDeviceToHost));
             float lo = 1e30f, hi = -1e30f;
             for (float v : h) { lo = fminf(lo, v); hi = fmaxf(hi, v); }
             zo[f] = (float)(0.5 * ((double)lo + (double)hi));
+            zr[2 * f] = lo - zo[f]; zr[2 * f + 1] = hi - zo[f];
         }
         CK(cudaMalloc(&s->d_zoff, cfg->nfields * sizeof(float)));
         CK(cudaMemcpy(s->d_zoff, zo.data(), cfg->nfields * sizeof(float), cudaMemcpyHostToDevice));
+        CK(cudaMalloc(&s->d_zrange, 2 * cfg->nfields * sizeof(float)));
+        CK(cudaMemcpy(s->d_zrange, zr.data(), 2 * cfg->nfields * sizeof(float), cudaMemcpyHostToDevice));
     }
     s->P.model = s->d_model; s->P.sf = s->d_sf; s->P.si = s->d_si;
     s->P.snap_f = s->d_snap_f; s->P.snap_i = s->d_snap_i; s->P.field_zoff = s->d_zoff;
@@ -191,6 +200,7 @@ void rexsim_destroy(RexSim* s) {
     cudaFree(s->d_model); cudaFree(s->d_sf); cudaFree(s->d_si); cudaFree(s->d_snap_f); cudaFree(s->d_snap_i);
     cudaFree(s->d_ring); cudaFree(s->d_snap_ring);
     cudaFree(s->d_zoff); cudaFree(s->d_err); cudaFree(s->d_cmd); cudaFree(s->d_act); cudaFree(s->d_out); cudaFree(s->d_perm); cudaFree(s->d_cost); cudaFree(s->d_hist);
+    cudaFree(s->d_zrange); cudaFree(s->d_rt);
     delete s;
 }
 
@@ -320,6 +330,26 @@ int rexsim_last_command(RexSim* s, float** cmd) {
 int rexsim_solver_cost(RexSim* s, int32_t** cost) {
     if (!s || !cost) return fail(REXSIM_ERR_INVALID, "null argument");
     *cost = s->d_cost;
+    return REXSIM_OK;
+}
+int rexsim_set_render_tables(RexSim* s, const float* rt, int32_t n_floats) {
+    if (!s || !rt) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (n_floats != REXSIM_RT_FLOATS) return fail(REXSIM_ERR_MODEL, "render table size mismatch");
+    CK(cudaMemcpy(s->d_rt, rt, REXSIM_RT_FLOATS * sizeof(float), cudaMemcpyHostToDevice));
+    s->rt_set = true;
+    return REXSIM_OK;
+}
+int rexsim_render(RexSim* s, const int32_t* idx, int32_t k, int32_t width, int32_t height, float distance, float yaw_deg,
+                  float pitch_deg, uint8_t* rgb, void* stream) {
+    if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
+    if (k < 0) return fail(REXSIM_ERR_INVALID, "negative count");
+    if (width < 1 || width > 4096 || height < 1 || height > 4096) return fail(REXSIM_ERR_INVALID, "image sides must be 1..4096");
+    if (!s->rt_set) return fail(REXSIM_ERR_INVALID, "render tables not set (rexsim_set_render_tables)");
+    if (k == 0) return REXSIM_OK;
+    if (!idx || !rgb) return fail(REXSIM_ERR_INVALID, "null argument");
+    cudaError_t e = launch_render(s->P, s->d_rt, s->d_zrange, idx, k, width, height, distance, yaw_deg, pitch_deg, rgb,
+                                  (cudaStream_t)stream, &s->launches);
+    if (e != cudaSuccess) return cuda_fail(e, "render launch");
     return REXSIM_OK;
 }
 int64_t rexsim_launch_count(const RexSim* s) { return s ? s->launches : 0; }

@@ -1,0 +1,417 @@
+// rexsim_render.cu -- rgb_array frames of chosen environments, ray-cast on the device from the SoA state
+// (RexGymEnv.render(mode="rgb_array"), rex_gym/envs/rex_gym_env.py:416-439).
+//
+// What is drawn is the collision geometry the contact model collides with, not the URDF visual meshes: the base and
+// chassis boxes, the 12 leg boxes, the four toe prisms, with mark 'arm' the six arm cylinders and arm_section_4's box, and
+// the ground (plane z = 0, or the env's heightfield).  Each shape takes its link's URDF visual colour from the render table
+// (include/rexsim.h REXSIM_RT_*, packed by rex_gym_b200/model_tables.py pack_render_tables), which also holds the light,
+// the checker tones of the ground and the sky.
+//
+// Grid: one CTA of 16 x 16 threads per 16 x 16 pixel tile of one image, blockIdx.x = tile, blockIdx.y = image.  Warp 0
+// poses the robot (forward kinematics over the model table, 19 bodies: cheap enough to redo per CTA, and it keeps the
+// library free of allocations after rexsim_create), writes every shape as world-space geometry + bounding sphere into
+// shared memory, and culls the spheres against the tile's frustum.  Then every thread casts its pixel's ray against
+// the surviving shapes and the ground.  The kernel only reads the state.
+#include "rexsim_kernel.cuh"
+
+namespace rexsim {
+
+struct RenderArgs {
+    const float* __restrict__ sf;       // [NF][N]
+    const int32_t* __restrict__ si;     // [NI][N]
+    const float* __restrict__ model;    // model table
+    const float* __restrict__ rt;       // render table, REXSIM_RT_FLOATS
+    const float* __restrict__ fields;   // [nfields][256*256] (terrain RANDOM)
+    const float* __restrict__ zoff;     // [nfields] vertical centring of each field
+    const float* __restrict__ zrange;   // [nfields][2] lowest / highest centred height
+    const int32_t* __restrict__ idx;    // [k] env of each image
+    uint8_t* __restrict__ rgb;          // [k][H][W][3]
+    int32_t* __restrict__ err;          // [N + 1]: word N = aggregate error bits
+    int N, terrain, arm, toe_npts;
+    int W, H, tiles_x, image0;
+    float dist, yaw, pitch;             // radians
+};
+
+enum { RT_TILE = 16, SHAPE_FLOATS = 20, MAX_SHAPES = REXSIM_RT_NSHAPES };
+// shape record: [0..2] centre (box, cylinder) or body origin (toe); [3..11] three unit axes (box axes, foot frame columns,
+// cylinder axis in [9..11]); [12..14] half extents (box) or radius, half length (cylinder); [15..17] bounding sphere centre, [18] radius
+enum { SH_C = 0, SH_A0 = 3, SH_A1 = 6, SH_A2 = 9, SH_H = 12, SH_S = 15, SH_R = 18 };
+
+// Bullet's computeViewMatrixFromYawPitchRoll (up axis z) followed by computeViewMatrixFromPositions (gluLookAt) and
+// computeProjectionMatrixFOV (pybullet client API, the calls of rex_gym_env.py:420-436): R = Rz(yaw) Rx(pitch),
+// eye = target + R (0, -d, 0), up = R (0, 0, 1); f = normalize(target - eye), s = normalize(f x up), u = s x f.
+// The ray of pixel (row, col) is f + x tan(fov/2) (W/H) s + y tan(fov/2) u with x = (2 col + 1)/W - 1, y = 1 - (2 row + 1)/H;
+// its f component is 1, so the ray parameter of a hit is its depth along the view axis (what near / far clip).
+struct Camera { V3 eye, f, s, u; };
+__device__ __forceinline__ Camera make_camera(V3 target, float d, float yaw, float pitch, float tan_half, float aspect) {
+    float sy, cy, sp, cp;
+    sincosf(yaw, &sy, &cy); sincosf(pitch, &sp, &cp);
+    // Rx(pitch) (0, -d, 0) = (0, -d cp, -d sp); Rz(yaw) of that
+    V3 off = mk(d * cp * sy, -d * cp * cy, -d * sp);
+    V3 up = mk(sp * sy, -sp * cy, cp);
+    Camera C;
+    C.eye = target + off;
+    V3 f = mk(-off.x, -off.y, -off.z);
+    f = rsqrtf(dot(f, f)) * f;
+    V3 s = cross(f, up);
+    s = rsqrtf(dot(s, s)) * s;
+    C.u = (tan_half) * cross(s, f);
+    C.s = (tan_half * aspect) * s;
+    C.f = f;
+    return C;
+}
+__device__ __forceinline__ V3 pixel_ray(const Camera& C, float x, float y) { return fma3(x, C.s, fma3(y, C.u, C.f)); }
+
+// box from its 8 body-frame corners (index 4 ix + 2 iy + iz, tools/compile_urdf.py shape_points) placed by (R, p)
+__device__ void write_box(float* rec, const float* corners, const M3& R, V3 p) {
+    V3 c0 = mk(corners[0], corners[1], corners[2]);
+    V3 ex = 0.5f * (mk(corners[12], corners[13], corners[14]) - c0);
+    V3 ey = 0.5f * (mk(corners[6], corners[7], corners[8]) - c0);
+    V3 ez = 0.5f * (mk(corners[3], corners[4], corners[5]) - c0);
+    V3 c = p + mul(R, c0 + ex + ey + ez);
+    float hx = sqrtf(dot(ex, ex)), hy = sqrtf(dot(ey, ey)), hz = sqrtf(dot(ez, ez));
+    V3 ax = mul(R, (1.f / hx) * ex), ay = mul(R, (1.f / hy) * ey), az = mul(R, (1.f / hz) * ez);
+    rec[SH_C] = c.x; rec[SH_C + 1] = c.y; rec[SH_C + 2] = c.z;
+    rec[SH_A0] = ax.x; rec[SH_A0 + 1] = ax.y; rec[SH_A0 + 2] = ax.z;
+    rec[SH_A1] = ay.x; rec[SH_A1 + 1] = ay.y; rec[SH_A1 + 2] = ay.z;
+    rec[SH_A2] = az.x; rec[SH_A2 + 1] = az.y; rec[SH_A2 + 2] = az.z;
+    rec[SH_H] = hx; rec[SH_H + 1] = hy; rec[SH_H + 2] = hz;
+    rec[SH_S] = c.x; rec[SH_S + 1] = c.y; rec[SH_S + 2] = c.z; rec[SH_R] = sqrtf(hx * hx + hy * hy + hz * hz);
+}
+__device__ void write_frame(float* rec, const M3& R, V3 p) {
+    rec[SH_C] = p.x; rec[SH_C + 1] = p.y; rec[SH_C + 2] = p.z;
+    rec[SH_A0] = R.c0.x; rec[SH_A0 + 1] = R.c0.y; rec[SH_A0 + 2] = R.c0.z;
+    rec[SH_A1] = R.c1.x; rec[SH_A1 + 1] = R.c1.y; rec[SH_A1 + 2] = R.c1.z;
+    rec[SH_A2] = R.c2.x; rec[SH_A2 + 1] = R.c2.y; rec[SH_A2 + 2] = R.c2.z;
+}
+__device__ __forceinline__ void write_sphere(float* rec, V3 c, float r) {
+    rec[SH_S] = c.x; rec[SH_S + 1] = c.y; rec[SH_S + 2] = c.z; rec[SH_R] = r;
+}
+__device__ __forceinline__ V3 ld3(const float* p) { return mk(p[0], p[1], p[2]); }
+
+// btMatrix3x3::setRotation, written as rexsim_kernel.cu's quat_to_mat (which stays there: moving it into the shared header
+// reorders the step kernels' stack slots)
+__device__ __forceinline__ M3 quat_rotation(float x, float y, float z, float w) {
+    float d = x * x + y * y + z * z + w * w;
+    float s = 2.0f / d;
+    float xs = x * s, ys = y * s, zs = z * s;
+    float wx = w * xs, wy = w * ys, wz = w * zs, xx = x * xs, xy = x * ys, xz = x * zs, yy = y * ys, yz = y * zs, zz = z * zs;
+    M3 R;
+    R.c0 = mk(1.f - (yy + zz), xy + wz, xz - wy);
+    R.c1 = mk(xy - wz, 1.f - (xx + zz), yz + wx);
+    R.c2 = mk(xz + wy, yz - wx, 1.f - (xx + yy));
+    return R;
+}
+// Rodrigues rotation about unit axis a (columns), and A B
+__device__ __forceinline__ M3 rot_axis(V3 a, float q) {
+    float s, c; sincosf(q, &s, &c); float t = 1.f - c;
+    M3 R;
+    R.c0 = mk(t * a.x * a.x + c, t * a.x * a.y + s * a.z, t * a.x * a.z - s * a.y);
+    R.c1 = mk(t * a.x * a.y - s * a.z, t * a.y * a.y + c, t * a.y * a.z + s * a.x);
+    R.c2 = mk(t * a.x * a.z + s * a.y, t * a.y * a.z - s * a.x, t * a.z * a.z + c);
+    return R;
+}
+__device__ __forceinline__ M3 mulMM(const M3& A, const M3& B) { M3 r; r.c0 = mul(A, B.c0); r.c1 = mul(A, B.c1); r.c2 = mul(A, B.c2); return r; }
+
+// warp 0: pose every shape of env `env` into `shapes` (world frame)
+__device__ void pose_shapes(const RenderArgs& A, int env, float* shapes, int lane) {
+    const size_t N = A.N;
+    const float* sf = A.sf;
+    const V3 pos = mk(sf[(F_POS + 0) * N + env], sf[(F_POS + 1) * N + env], sf[(F_POS + 2) * N + env]);
+    const M3 R0 = quat_rotation(sf[(F_QUAT + 0) * N + env], sf[(F_QUAT + 1) * N + env], sf[(F_QUAT + 2) * N + env],
+                                sf[(F_QUAT + 3) * N + env]);
+    const float* mt = A.model;
+    if (lane < 4) {            // leg `lane`: shoulder about x, leg and foot about y, unrotated joint frames (model_tables.py)
+        const int leg = lane;
+        const float* LB = mt + REXSIM_MT_LEG + leg * 48;
+        float s1, c1, s2, c2, s3, c3;
+        sincosf(sf[(F_Q + 3 * leg + 0) * N + env], &s1, &c1);
+        sincosf(sf[(F_Q + 3 * leg + 1) * N + env], &s2, &c2);
+        sincosf(sf[(F_Q + 3 * leg + 2) * N + env], &s3, &c3);
+        M3 R1; R1.c0 = R0.c0; R1.c1 = fma3(c1, R0.c1, s1 * R0.c2); R1.c2 = fma3(-s1, R0.c1, c1 * R0.c2);
+        M3 R2; R2.c0 = fma3(c2, R1.c0, -s2 * R1.c2); R2.c1 = R1.c1; R2.c2 = fma3(s2, R1.c0, c2 * R1.c2);
+        M3 R3; R3.c0 = fma3(c3, R2.c0, -s3 * R2.c2); R3.c1 = R2.c1; R3.c2 = fma3(s3, R2.c0, c3 * R2.c2);
+        V3 p1 = pos + mul(R0, ld3(LB));
+        V3 p2 = p1 + mul(R1, ld3(LB + 16));
+        V3 p3 = p2 + mul(R2, ld3(LB + 32));
+        const float* BX = mt + REXSIM_MT_BOX + leg * 72;
+        write_box(shapes + (3 + 3 * leg + 0) * SHAPE_FLOATS, BX, R1, p1);
+        write_box(shapes + (3 + 3 * leg + 1) * SHAPE_FLOATS, BX + 24, R2, p2);
+        write_box(shapes + (3 + 3 * leg + 2) * SHAPE_FLOATS, BX + 48, R3, p3);
+        float* toe = shapes + (15 + leg) * SHAPE_FLOATS;
+        write_frame(toe, R3, p3);
+        const float* ts = A.rt + REXSIM_RT_TOESPH;
+        write_sphere(toe, p3 + mul(R3, mk(ts[0], 0.f, ts[1])), ts[2]);
+    } else if (lane < 7) {     // base and chassis boxes
+        write_box(shapes + (lane - 4) * SHAPE_FLOATS, mt + REXSIM_MT_BASEBOX + 24 * (lane - 4), R0, pos);
+    } else if (lane == 7 && A.arm) {   // the arm: one serial chain with general joint frames (rexsim_arm.cuh layout)
+        M3 Rp = R0; V3 pp = pos;
+        for (int j = 0; j < 6; j++) {
+            const float* T = mt + REXSIM_MT_ARM + 32 * j;
+            M3 Jr; Jr.c0 = mk(T[3], T[6], T[9]); Jr.c1 = mk(T[4], T[7], T[10]); Jr.c2 = mk(T[5], T[8], T[11]);
+            M3 Rj = mulMM(mulMM(Rp, Jr), rot_axis(ld3(T + 12), sf[(F_AQ + j) * N + env]));
+            V3 pj = pp + mul(Rp, ld3(T));
+            const float* cy = A.rt + REXSIM_RT_CYL + 8 * j;
+            float* rec = shapes + (19 + j) * SHAPE_FLOATS;
+            V3 c = pj + mul(Rj, ld3(cy)), ax = mul(Rj, ld3(cy + 3));
+            rec[SH_C] = c.x; rec[SH_C + 1] = c.y; rec[SH_C + 2] = c.z;
+            rec[SH_A2] = ax.x; rec[SH_A2 + 1] = ax.y; rec[SH_A2 + 2] = ax.z;
+            rec[SH_H] = cy[6]; rec[SH_H + 1] = cy[7];
+            write_sphere(rec, c, sqrtf(cy[6] * cy[6] + cy[7] * cy[7]));
+            if (j == (int)A.rt[REXSIM_RT_ARMBOX]) write_box(shapes + 25 * SHAPE_FLOATS, A.rt + REXSIM_RT_ARMBOX + 1, Rj, pj);
+            Rp = Rj; pp = pj;
+        }
+    }
+}
+
+// entering parameter of the ray o + t r into the slab |a . (p - c)| <= h: clips [t0, t1], remembers the entering face
+__device__ __forceinline__ void clip_plane(float denom, float dist, float& t0, float& t1, int& face, int f) {
+    // inside where denom t <= dist
+    if (denom < 0.f) { float t = dist / denom; if (t > t0) { t0 = t; face = f; } }
+    else if (denom > 0.f) { float t = dist / denom; t1 = fminf(t1, t); }
+    else if (dist < 0.f) t1 = -1.f;
+}
+
+// ray against one posed shape; on a nearer hit updates best t and the outward normal
+__device__ __forceinline__ void hit_box(const float* rec, V3 o, V3 r, float& best, V3& nrm) {
+    V3 w = o - ld3(rec + SH_C);
+    float t0 = 0.f, t1 = best; int face = -1;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        V3 a = ld3(rec + SH_A0 + 3 * k);
+        float h = rec[SH_H + k], ow = dot(a, w), ra = dot(a, r);
+        clip_plane(ra, h - ow, t0, t1, face, 2 * k + 1);
+        clip_plane(-ra, h + ow, t0, t1, face, 2 * k);
+    }
+    if (face >= 0 && t0 <= t1) {
+        best = t0;
+        V3 a = ld3(rec + SH_A0 + 3 * (face >> 1));
+        nrm = (face & 1) ? a : mk(-a.x, -a.y, -a.z);
+    }
+}
+// toe prism: the convex (x, z) profile of the foot frame extruded over y in [-w, w] (REXSIM_MT_TOE); planes n . (x, z) <= d
+__device__ __forceinline__ void hit_toe(const float* rec, const float* planes, int np, float w, V3 o, V3 r, float& best, V3& nrm) {
+    V3 dw = o - ld3(rec + SH_C);
+    V3 a0 = ld3(rec + SH_A0), a1 = ld3(rec + SH_A1), a2 = ld3(rec + SH_A2);
+    float ox = dot(a0, dw), oy = dot(a1, dw), oz = dot(a2, dw);
+    float rx = dot(a0, r), ry = dot(a1, r), rz = dot(a2, r);
+    float t0 = 0.f, t1 = best; int face = -1;
+    clip_plane(ry, w - oy, t0, t1, face, np + 1);
+    clip_plane(-ry, w + oy, t0, t1, face, np);
+    for (int e = 0; e < np && t0 <= t1; e++) {
+        const float* P = planes + 3 * e;
+        clip_plane(fmaf(P[0], rx, P[1] * rz), P[2] - fmaf(P[0], ox, P[1] * oz), t0, t1, face, e);
+    }
+    if (face >= 0 && t0 <= t1) {
+        best = t0;
+        nrm = face == np ? mk(-a1.x, -a1.y, -a1.z) : face == np + 1 ? a1 : fma3(planes[3 * face], a0, planes[3 * face + 1] * a2);
+    }
+}
+// capped cylinder: the slab |axial| <= half length intersected with the infinite cylinder of the radius
+__device__ __forceinline__ void hit_cylinder(const float* rec, V3 o, V3 r, float& best, V3& nrm) {
+    V3 ax = ld3(rec + SH_A2);
+    V3 w = o - ld3(rec + SH_C);
+    float R = rec[SH_H], h = rec[SH_H + 1];
+    float oa = dot(ax, w), ra = dot(ax, r);
+    float t0 = 0.f, t1 = best; int face = -1;
+    clip_plane(ra, h - oa, t0, t1, face, 1);
+    clip_plane(-ra, h + oa, t0, t1, face, 0);
+    V3 wp = fma3(-oa, ax, w), rp = fma3(-ra, ax, r);
+    float a = dot(rp, rp), b = dot(wp, rp), c = dot(wp, wp) - R * R;
+    if (a > 0.f) {
+        float disc = b * b - a * c;
+        if (disc < 0.f) return;
+        float sq = sqrtf(disc), te = (-b - sq) / a, tx = (-b + sq) / a;
+        if (te > t0) { t0 = te; face = 2; }
+        t1 = fminf(t1, tx);
+    } else if (c > 0.f) return;
+    if (face >= 0 && t0 <= t1) {
+        best = t0;
+        if (face == 2) { V3 q = fma3(t0, rp, wp); nrm = rsqrtf(dot(q, q)) * q; }
+        else nrm = face ? ax : mk(-ax.x, -ax.y, -ax.z);
+    }
+}
+
+// ground: the plane z = 0, or the env's heightfield (rexsim_kernel.cu ground_query: vertex (ix, iy) at x = (ix - 127.5) * 0.05,
+// height h[iy][ix] - zoff, cell split v >= u).  The ray is marched cell by cell (2-D DDA) over the part of it that lies inside
+// the field's square and inside the slab of the field's heights.  Outside the square the ground is the horizontal plane at
+// the field's lowest centred height (the physics clamps its queries to the border cells instead; DESIGN.md section 5).
+__device__ __forceinline__ void hit_ground(const RenderArgs& A, const float* h, float zoff, float zlo, float zhi, V3 o, V3 r,
+                                           float& best, V3& nrm) {
+    if (A.terrain != REXSIM_TERRAIN_RANDOM) {
+        if (r.z < 0.f) { float t = -o.z / r.z; if (t > 0.f && t < best) { best = t; nrm = mk(0.f, 0.f, 1.f); } }
+        return;
+    }
+    const float gx0 = fmaf(o.x, 20.f, 127.5f), gy0 = fmaf(o.y, 20.f, 127.5f), dgx = r.x * 20.f, dgy = r.y * 20.f;
+    if (r.z < 0.f) {           // the plane outside the square
+        float t = (zlo - o.z) / r.z;
+        float gx = fmaf(t, dgx, gx0), gy = fmaf(t, dgy, gy0);
+        if (t > 0.f && t < best && (gx < 0.f || gx > 255.f || gy < 0.f || gy > 255.f)) { best = t; nrm = mk(0.f, 0.f, 1.f); }
+    }
+    float ta = 0.f, tb = best; int dummy = 0;
+    clip_plane(r.z, zhi - o.z, ta, tb, dummy, 0);
+    clip_plane(-r.z, o.z - zlo, ta, tb, dummy, 0);
+    clip_plane(dgx, 255.f - gx0, ta, tb, dummy, 0);
+    clip_plane(-dgx, gx0, ta, tb, dummy, 0);
+    clip_plane(dgy, 255.f - gy0, ta, tb, dummy, 0);
+    clip_plane(-dgy, gy0, ta, tb, dummy, 0);
+    if (!(ta <= tb)) return;
+    int ix = min(max((int)floorf(fmaf(ta, dgx, gx0)), 0), 254), iy = min(max((int)floorf(fmaf(ta, dgy, gy0)), 0), 254);
+    const int sx = dgx > 0.f ? 1 : -1, sy = dgy > 0.f ? 1 : -1;
+    const float ez = o.z + zoff;          // heights are compared uncentred
+    float t = ta;
+    for (;;) {
+        const float tx = dgx != 0.f ? ((float)(ix + (sx > 0)) - gx0) / dgx : INFINITY;
+        const float ty = dgy != 0.f ? ((float)(iy + (sy > 0)) - gy0) / dgy : INFINITY;
+        const float tn = fminf(fminf(tx, ty), tb);
+        const float* c = h + iy * 256 + ix;
+        const float h00 = __ldg(c), h10 = __ldg(c + 1), h01 = __ldg(c + 256), h11 = __ldg(c + 257);
+        const float u0 = gx0 - (float)ix, v0 = gy0 - (float)iy;
+        float th = INFINITY, hx = 0.f, hy = 0.f;
+#pragma unroll
+        for (int tri = 0; tri < 2; tri++) {
+            // tri 0: v >= u, z = h00 + (h11 - h01) u + (h01 - h00) v;  tri 1: v < u, z = h00 + (h10 - h00) u + (h11 - h10) v
+            const float a = tri == 0 ? h11 - h01 : h10 - h00, b = tri == 0 ? h01 - h00 : h11 - h10;
+            const float f0 = ez - h00 - a * u0 - b * v0, f1 = r.z - a * dgx - b * dgy;
+            if (f1 == 0.f) continue;
+            const float tt = -f0 / f1;
+            if (tt < t || tt > tn || tt >= th) continue;
+            const float u = fmaf(tt, dgx, u0), v = fmaf(tt, dgy, v0);
+            if ((v >= u) != (tri == 0)) continue;
+            th = tt; hx = a; hy = b;
+        }
+        if (th < INFINITY) {
+            best = th;
+            float nx = -hx * 20.f, ny = -hy * 20.f, inv = rsqrtf(nx * nx + ny * ny + 1.f);
+            nrm = mk(nx * inv, ny * inv, inv);
+            return;
+        }
+        if (tn >= tb) return;
+        t = tn;
+        if (tx <= ty) ix += sx; else iy += sy;
+        if (ix < 0 || ix > 254 || iy < 0 || iy > 254) return;
+    }
+}
+
+__global__ void __launch_bounds__(RT_TILE * RT_TILE) render_kernel(const RenderArgs A) {
+    __shared__ float rt[REXSIM_RT_FLOATS];
+    __shared__ float shapes[MAX_SHAPES * SHAPE_FLOATS];
+    __shared__ unsigned live;
+    const int tid = threadIdx.y * RT_TILE + threadIdx.x;
+    const int img = A.image0 + blockIdx.y;
+    const int env = A.idx[img];
+    const bool valid = env >= 0 && env < A.N;
+    for (int i = tid; i < REXSIM_RT_FLOATS; i += RT_TILE * RT_TILE) rt[i] = A.rt[i];
+    const int tile = blockIdx.x, c0 = (tile % A.tiles_x) * RT_TILE, r0 = (tile / A.tiles_x) * RT_TILE;
+    const float tan_half = tanf(0.5f * A.rt[REXSIM_RT_CAM] * (3.14159265358979323846f / 180.f)), aspect = (float)A.W / (float)A.H;
+    const float inv_w = 1.f / (float)A.W, inv_h = 1.f / (float)A.H;
+    const int nshapes = A.arm ? REXSIM_RT_NSHAPES : 19;
+    Camera C;
+    if (valid) C = make_camera(mk(A.sf[(F_POS + 0) * (size_t)A.N + env], A.sf[(F_POS + 1) * (size_t)A.N + env],
+                                  A.sf[(F_POS + 2) * (size_t)A.N + env]), A.dist, A.yaw, A.pitch, tan_half, aspect);
+    if (tid < 32) {
+        if (valid) {
+            pose_shapes(A, env, shapes, tid);
+            __syncwarp();
+            // frustum of the tile: the four planes through the eye spanned by its extreme pixel rays
+            const int c1 = min(c0 + RT_TILE, A.W) - 1, r1 = min(r0 + RT_TILE, A.H) - 1;
+            const float xl = (2 * c0 + 1) * inv_w - 1.f, xr = (2 * c1 + 1) * inv_w - 1.f;
+            const float yt = 1.f - (2 * r0 + 1) * inv_h, yb = 1.f - (2 * r1 + 1) * inv_h;
+            const V3 tl = pixel_ray(C, xl, yt), tr = pixel_ray(C, xr, yt), bl = pixel_ray(C, xl, yb), br = pixel_ray(C, xr, yb);
+            const V3 mid = pixel_ray(C, 0.5f * (xl + xr), 0.5f * (yt + yb));
+            bool keep = tid < nshapes;
+            if (keep) {
+                const float* rec = shapes + tid * SHAPE_FLOATS;
+                const V3 d = ld3(rec + SH_S) - C.eye;
+                const float rad = rec[SH_R];
+                const V3 edges[4][2] = {{bl, tl}, {tl, tr}, {tr, br}, {br, bl}};
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    V3 n = cross(edges[k][0], edges[k][1]);
+                    const float nn = dot(n, n);
+                    if (!(nn > 1e-20f)) continue;         // a one-pixel-wide tile: no plane on that side
+                    n = rsqrtf(nn) * n;
+                    if (dot(n, mid) < 0.f) n = mk(-n.x, -n.y, -n.z);
+                    if (dot(n, d) < -rad) keep = false;
+                }
+            }
+            const unsigned m = __ballot_sync(0xffffffffu, keep);
+            if (tid == 0) live = m;
+        } else if (tid == 0) {
+            live = 0;
+            if (blockIdx.x == 0) atomicOr(A.err + A.N, REXSIM_FLAG_BAD_INDEX);
+        }
+    }
+    __syncthreads();
+    const int col = c0 + threadIdx.x, row = r0 + threadIdx.y;
+    if (col >= A.W || row >= A.H) return;
+    float rgbf[3] = {rt[REXSIM_RT_SKY], rt[REXSIM_RT_SKY + 1], rt[REXSIM_RT_SKY + 2]};
+    if (valid) {
+        const V3 r = pixel_ray(C, (2 * col + 1) * inv_w - 1.f, 1.f - (2 * row + 1) * inv_h);
+        const V3 o = C.eye;
+        const float rr = dot(r, r);
+        float best = INFINITY; V3 nrm = mk(0.f, 0.f, 1.f); int who = -1;
+        for (unsigned m = live; m; m &= m - 1) {
+            const int s = __ffs(m) - 1;
+            const float* rec = shapes + s * SHAPE_FLOATS;
+            const V3 d = ld3(rec + SH_S) - o;                 // bounding sphere first
+            const float tc = dot(d, r), rad = rec[SH_R];
+            if (dot(d, d) * rr - tc * tc > rad * rad * rr) continue;
+            const float prev = best;
+            if (s < 15 || s == 25) hit_box(rec, o, r, best, nrm);
+            else if (s < 19) hit_toe(rec, rt + REXSIM_RT_TOE, A.toe_npts, A.model[REXSIM_MT_BASE + 15], o, r, best, nrm);
+            else hit_cylinder(rec, o, r, best, nrm);
+            if (best < prev) who = s;
+        }
+        if (A.terrain == REXSIM_TERRAIN_RANDOM) {
+            const int field = A.si[I_FIELD * (size_t)A.N + env];
+            const float prev = best;
+            hit_ground(A, A.fields + (size_t)field * 65536, A.zoff[field], A.zrange[2 * field], A.zrange[2 * field + 1], o, r, best, nrm);
+            if (best < prev) who = -2;
+        } else {
+            const float prev = best;
+            hit_ground(A, nullptr, 0.f, 0.f, 0.f, o, r, best, nrm);
+            if (best < prev) who = -2;
+        }
+        if (who != -1 && best >= rt[REXSIM_RT_CAM + 1] && best <= rt[REXSIM_RT_CAM + 2]) {
+            const float* col3;
+            if (who == -2) {
+                const V3 p = fma3(best, r, o);
+                const float inv_sq = 1.f / rt[REXSIM_RT_CHECK + 6];
+                const int parity = ((int)floorf(p.x * inv_sq) + (int)floorf(p.y * inv_sq)) & 1;
+                col3 = rt + REXSIM_RT_CHECK + 3 * parity;
+            } else {
+                col3 = rt + REXSIM_RT_COLOR + 3 * who;
+            }
+            const float lam = fmaxf(0.f, dot(nrm, mk(rt[REXSIM_RT_LIGHT], rt[REXSIM_RT_LIGHT + 1], rt[REXSIM_RT_LIGHT + 2])));
+            const float shade = fmaf(rt[REXSIM_RT_LIGHT + 4], lam, rt[REXSIM_RT_LIGHT + 3]);
+            rgbf[0] = col3[0] * shade; rgbf[1] = col3[1] * shade; rgbf[2] = col3[2] * shade;
+        }
+    }
+    uint8_t* out = A.rgb + (((size_t)blockIdx.y * A.H + row) * A.W + col) * 3;
+#pragma unroll
+    for (int c = 0; c < 3; c++) out[c] = (uint8_t)fminf(fmaxf(rgbf[c] * 255.f + 0.5f, 0.f), 255.f);
+}
+
+cudaError_t launch_render(const Params& P, const float* rt, const float* zrange, const int32_t* idx, int k, int W, int H,
+                          float distance, float yaw_deg, float pitch_deg, uint8_t* rgb, cudaStream_t st, int64_t* launches) {
+    RenderArgs A;
+    A.sf = P.sf; A.si = P.si; A.model = P.model; A.rt = rt; A.fields = P.cfg.fields; A.zoff = P.field_zoff; A.zrange = zrange;
+    A.idx = idx; A.err = P.err; A.N = P.N; A.terrain = P.cfg.terrain; A.arm = P.cfg.num_motors == 18; A.toe_npts = P.cfg.toe_npts;
+    A.W = W; A.H = H; A.dist = distance;
+    A.yaw = yaw_deg * (float)(3.14159265358979323846 / 180.0); A.pitch = pitch_deg * (float)(3.14159265358979323846 / 180.0);
+    const int tiles_y = (H + RT_TILE - 1) / RT_TILE;
+    A.tiles_x = (W + RT_TILE - 1) / RT_TILE;
+    for (int i0 = 0; i0 < k; i0 += 65535) {          // gridDim.y <= 65535 images per launch
+        const int n = min(k - i0, 65535);
+        A.image0 = i0;
+        A.rgb = rgb + (size_t)i0 * H * W * 3;
+        render_kernel<<<dim3(A.tiles_x * tiles_y, n), dim3(RT_TILE, RT_TILE), 0, st>>>(A);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        ++*launches;
+    }
+    return cudaSuccess;
+}
+
+}  // namespace rexsim

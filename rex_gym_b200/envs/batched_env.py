@@ -14,7 +14,7 @@ import numpy as np
 import torch
 
 from .. import _capi
-from ..model_tables import (pack_model_tables, contact_breaking_distance, TOE_MARGIN, LINK_DAMPING,
+from ..model_tables import (pack_model_tables, pack_render_tables, contact_breaking_distance, TOE_MARGIN, LINK_DAMPING,
                             MAX_COORDINATE_VELOCITY)
 from ..terrain import make_random_fields
 from .spaces import Box
@@ -74,6 +74,12 @@ class _EnvView(object):
     @property
     def env_step_counter(self):
         return int(self._b.get_state()["env_step_counter"][self.index])
+
+    def render(self, mode="rgb_array", close=False):
+        """This env's frame (RexGymEnv.render, rex_gym_env.py:416-439)."""
+        if mode != "rgb_array":
+            return np.array([])
+        return self._b.render_batch([self.index])[0].cpu().numpy()
 
 
 class BatchedRexEnv(object):
@@ -158,6 +164,9 @@ class BatchedRexEnv(object):
             tb = np.ascontiguousarray(tables)
             _capi.check(self._L.rexsim_create(C.byref(c), tb.ctypes.data, tb.size, C.byref(h)))
         self._h = h
+        rt = np.ascontiguousarray(pack_render_tables(mark))
+        with torch.cuda.device(self.device):
+            _capi.check(self._L.rexsim_set_render_tables(self._h, rt.ctypes.data, rt.size))
         self.obs_dim = self._L.rexsim_obs_dim(c.task, c.num_motors)
         self.action_dim = self._L.rexsim_action_dim(c.task, c.signal)
         N, O, A = self.num_envs, self.obs_dim, self.action_dim
@@ -376,7 +385,34 @@ class BatchedRexEnv(object):
         return [seed]
 
     def render(self, mode="rgb_array", close=False):
-        return np.array([])
+        """RexGymEnv.render as BatchEnv forwards it (batch_env.py:52-61: to env 0): a (360, 480, 3) uint8 frame of env 0 through
+        the reference's follow camera for mode 'rgb_array', an empty array for any other mode (rex_gym_env.py:416-418)."""
+        if mode != "rgb_array":
+            return np.array([])
+        return self.render_batch([0])[0].cpu().numpy()
+
+    def render_batch(self, indices, width=480, height=360, distance=1.0, yaw=0.0, pitch=-30.0):
+        """Frames of the envs `indices` as a CUDA uint8 tensor [k, height, width, 3] (row 0 at the top), ray-cast from the
+        device state on the current stream without synchronising.  The camera follows each env's base the way the reference's
+        does (rex_gym_env.py:214-216,420-436): distance [m], yaw and pitch [deg].  What is drawn is the collision geometry.
+        Host indices outside the batch raise IndexError; device indices are not inspected (an out-of-range one gives a sky
+        image and check_errors() raises IndexError), as in reset()."""
+        if not (1 <= int(width) <= 4096 and 1 <= int(height) <= 4096):
+            raise ValueError("image sides must be 1..4096")
+        with torch.cuda.device(self.device):
+            if isinstance(indices, torch.Tensor):
+                idx = indices.to(device=self.device, dtype=torch.int32).reshape(-1).contiguous()
+            else:
+                ia = np.asarray(indices, dtype=np.int64).reshape(-1)
+                if ia.size and (ia.min() < 0 or ia.max() >= self.num_envs):
+                    raise IndexError("render index out of range")
+                idx = torch.from_numpy(ia.astype(np.int32)).to(self.device)
+            k = int(idx.numel())
+            out = torch.empty((k, int(height), int(width), 3), dtype=torch.uint8, device=self.device)
+            if k > 0:
+                _capi.check(self._L.rexsim_render(self._h, idx.data_ptr(), k, int(width), int(height), float(distance), float(yaw),
+                                                  float(pitch), out.data_ptr(), self._stream()))
+            return out
 
 
 class RexWalkBatchEnv(BatchedRexEnv):

@@ -36,7 +36,8 @@ class SingleRexEnv(_Base):
         return obs[0], float(reward[0]), bool(done[0]), info[0]
 
     def render(self, mode="rgb_array", close=False):
-        return np.array([])                       # rex_gym_env.py:416-418 returns an empty array for non-rgb modes too
+        """(360, 480, 3) uint8 frame for 'rgb_array'; rex_gym_env.py:416-418 returns an empty array for the other modes."""
+        return self._batch.render(mode, close)
 
     def seed(self, seed=None):
         return [seed]

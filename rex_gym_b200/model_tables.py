@@ -10,6 +10,18 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 MT_BASE, MT_LEG, MT_TOE, MT_BOX, MT_BASEBOX, MT_FLOATS = 0, 16, 208, 592, 880, 952
 MT_ARM, ARM_STRIDE, MT_ARMPTS, ARMPTS_N = 952, 32, 952 + 192, 104
 MT_FLOATS_ARM = MT_ARMPTS + 3 * ARMPTS_N
+# render table (include/rexsim.h REXSIM_RT_*): light, sky, ground checker, camera lens, shape colours and the fixed geometry the
+# renderer needs beyond the model table
+RT_LIGHT, RT_SKY, RT_CHECK, RT_CAM, RT_COLOR, RT_TOE, RT_TOESPH, RT_CYL, RT_ARMBOX, RT_FLOATS = 0, 5, 8, 15, 18, 96, 384, 388, 436, 464
+RT_NSHAPES = 26
+# What is not URDF data: a light from above, behind the default camera's left shoulder; Lambert + ambient weights; a grey 1 m
+# checker on the ground; a pale sky.  The camera lens is the reference's (rex_gym_env.py:428-431: fov 60, near 0.1, far 100).
+LIGHT_DIR = (-0.4, -0.6, 1.0)
+AMBIENT, DIFFUSE = 0.35, 0.65
+SKY_RGB = (0.62, 0.76, 0.92)
+CHECKER_RGB = ((0.80, 0.80, 0.80), (0.55, 0.55, 0.55))
+CHECKER_SIZE = 1.0
+CAMERA_FOV_DEG, CAMERA_NEAR, CAMERA_FAR = 60.0, 0.1, 100.0
 MAX_TOE_PTS = 96     # profile vertices of the toe prism ((x, z) pairs: 2 * 96 floats fit the 384-float toe block)
 # Margin added to the toe hull's reach.  Bullet's URDF importer puts 1 mm on convex hulls, but the PyBullet trajectories
 # recovered from the reference's checkpoints (25 episodes, identical free fall from z = 0.21) put the touchdown where the
@@ -153,3 +165,84 @@ def contact_breaking_distance(mark="base"):
     half_w = np.abs(R) @ half                                                               # btTransformAabb
     centre_w = R @ centre + t
     return float((np.linalg.norm(centre_w) + np.linalg.norm(half_w)) * 0.02)
+
+
+def toe_profile_planes(profile):
+    """Edge planes of the convex toe profile ((x, z) vertices in order along its boundary, closed by the chord from the last to
+    the first): [n][3] rows (nx, nz, d), outward unit normal and offset, inside where nx x + nz z <= d."""
+    P = np.asarray(profile, dtype=np.float64)
+    c = P.mean(0)
+    out = []
+    for i in range(len(P)):
+        a, b = P[i], P[(i + 1) % len(P)]
+        n = np.array([b[1] - a[1], a[0] - b[0]])
+        n /= np.linalg.norm(n)
+        if n @ (a - c) < 0:
+            n = -n
+        out.append([n[0], n[1], n @ a])
+    out = np.array(out)
+    if np.any(P @ out[:, :2].T - out[:, 2] > 1e-9):
+        raise ValueError("toe profile is not convex in its stored order")
+    return out
+
+
+def render_shape_colors(mark="base"):
+    """[26][3] rgb of the rendered shapes (URDF visual material of each shape's link), in the renderer's shape order: base +
+    two chassis boxes, the 12 leg boxes (leg-major: shoulder, leg, foot), the four toes, the six arm cylinders, arm box."""
+    j = load_model_json(mark)
+    bodies = j["bodies"]
+    cols = np.zeros((RT_NSHAPES, 3))
+
+    def col(b, kind):
+        shapes = [s for s in b["shapes"] if s["kind"] == kind]
+        rgba = b["link_rgba"][shapes[0]["link"]]
+        if rgba is None:
+            raise ValueError("link %s has no visual material" % shapes[0]["link"])
+        return rgba[:3]
+    cols[0:3] = [b["link_rgba"][s["link"]][:3] for b in bodies[:1] for s in b["shapes"] if s["kind"] == "box"]
+    for leg in range(4):
+        for bi in range(3):
+            cols[3 + 3 * leg + bi] = col(bodies[1 + 3 * leg + bi], "box")
+        cols[15 + leg] = col(bodies[3 + 3 * leg], "hull")
+    if mark == "arm":
+        for k in range(6):
+            cols[19 + k] = col(bodies[13 + k], "cylinder")
+        cols[25] = col(bodies[17], "box")
+    return cols
+
+
+def pack_render_tables(mark="base"):
+    """float32[RT_FLOATS] render table of `mark` (layout: include/rexsim.h REXSIM_RT_*), uploaded by rexsim_set_render_tables."""
+    j = load_model_json(mark)
+    bodies = j["bodies"]
+    mt, npts = pack_model_tables(mark)
+    t = np.zeros(RT_FLOATS, dtype=np.float64)
+    L = np.asarray(LIGHT_DIR, dtype=np.float64)
+    t[RT_LIGHT:RT_LIGHT + 3] = L / np.linalg.norm(L)
+    t[RT_LIGHT + 3], t[RT_LIGHT + 4] = AMBIENT, DIFFUSE
+    t[RT_SKY:RT_SKY + 3] = SKY_RGB
+    t[RT_CHECK:RT_CHECK + 6] = np.asarray(CHECKER_RGB).reshape(-1)
+    t[RT_CHECK + 6] = CHECKER_SIZE
+    t[RT_CAM:RT_CAM + 3] = CAMERA_FOV_DEG, CAMERA_NEAR, CAMERA_FAR
+    t[RT_COLOR:RT_COLOR + 3 * RT_NSHAPES] = render_shape_colors(mark).reshape(-1)
+    prof = mt[MT_TOE:MT_TOE + 2 * npts].astype(np.float64).reshape(-1, 2)
+    t[RT_TOE:RT_TOE + 3 * npts] = toe_profile_planes(prof).reshape(-1)
+    w = float(mt[MT_BASE + 15])
+    c = 0.5 * (prof.min(0) + prof.max(0))
+    t[RT_TOESPH:RT_TOESPH + 3] = c[0], c[1], np.sqrt(((prof - c) ** 2).sum(1).max() + w * w) * (1 + 1e-5)
+    if mark == "arm":
+        for k in range(6):
+            cyl = [s for s in bodies[13 + k]["shapes"] if s["kind"] == "cylinder"]
+            if len(cyl) != 1:
+                raise ValueError("expected one cylinder per arm body")
+            s = cyl[0]
+            o = RT_CYL + 8 * k
+            t[o:o + 3] = s["origin_xyz"]
+            t[o + 3:o + 6] = np.asarray(s["origin_rot"])[:, 2]          # cylinder axis = z of its origin frame
+            t[o + 6], t[o + 7] = s["radius"], 0.5 * s["length"]
+        boxes = [(k, s) for k in range(6) for s in bodies[13 + k]["shapes"] if s["kind"] == "box"]
+        if len(boxes) != 1:
+            raise ValueError("expected one arm box")
+        t[RT_ARMBOX] = boxes[0][0]
+        t[RT_ARMBOX + 1:RT_ARMBOX + 25] = np.asarray(boxes[0][1]["points"]).reshape(-1)
+    return t.astype(np.float32)

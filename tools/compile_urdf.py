@@ -75,10 +75,16 @@ def support_polytope(verts):
 
 def parse_urdf(path, stl_dir):
     root = ET.parse(path).getroot()
+    materials = {m.get("name"): vec(m.find("color").get("rgba")) for m in root.findall("material") if m.find("color") is not None}
     links = {}
     for ln in root.findall("link"):
         name = ln.get("name")
         mass = float(ln.find("inertial/mass").get("value"))
+        # visual material: a named robot-level material or an inline colour; None for a link without a visual
+        rgba = None
+        mat = ln.find("visual/material")
+        if mat is not None:
+            rgba = vec(mat.find("color").get("rgba")) if mat.find("color") is not None else materials.get(mat.get("name"))
         shapes = []
         for col in ln.findall("collision"):
             org = col.find("origin")
@@ -95,7 +101,7 @@ def parse_urdf(path, stl_dir):
                     fn = os.path.join(stl_dir, os.path.basename(g.get("filename")))
                     sc = vec(g.get("scale"), (1, 1, 1))[0]
                     shapes.append(dict(kind="hull", verts=load_stl_vertices(fn, sc), xyz=xyz, rpy=rpy))
-        links[name] = dict(name=name, mass=mass, shapes=shapes)
+        links[name] = dict(name=name, mass=mass, shapes=shapes, rgba=None if rgba is None else rgba.tolist())
     joints = []
     for jn in root.findall("joint"):
         org = jn.find("origin")
@@ -191,8 +197,12 @@ def compile_model(urdf_path, stl_dir, motor_names):
                                    points=(shape_points(sh) @ R.T + t).tolist()))
                 if sh["kind"] == "hull":     # prism: first half = profile on the y_min face, second half = y_max face
                     shapes[-1]["prism_profile_points"] = len(shapes[-1]["points"]) // 2
+                if sh["kind"] == "cylinder":  # the renderer draws true capped cylinders: axis = z of the origin frame
+                    shapes[-1].update(radius=sh["radius"], length=sh["length"], origin_xyz=(R @ sh["xyz"] + t).tolist(),
+                                      origin_rot=(R @ rpy_to_mat(sh["rpy"])).tolist())
         b = dict(name=link_name, parent=parent_body, mass=mass, com=com.tolist(), inertia=I.tolist(),
                  shapes=shapes, links=[p[0]["name"] for p in parts])
+        b["link_rgba"] = {p[0]["name"]: p[0]["rgba"] for p in parts}      # URDF visual material of every merged link
         if joint is not None:
             b.update(joint=joint["name"], joint_xyz=joint["xyz"].tolist(), joint_rpy=joint["rpy"].tolist(),
                      axis=joint["axis"].tolist(), lower=joint["lower"], upper=joint["upper"])
