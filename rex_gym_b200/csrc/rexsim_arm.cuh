@@ -39,6 +39,13 @@ __device__ __forceinline__ M3 axis_angle(V3 a, float q) {   // Rodrigues, column
     R.c2 = mk(t * a.x * a.z + s * a.y, t * a.y * a.z - s * a.x, t * a.z * a.z + c);
     return R;
 }
+// frame Rj and origin pj of arm body j from its model table T (REXSIM_MT_ARM + ARM_STRIDE * j), its joint angle q and the
+// frame (Rp, pp) of its parent
+__device__ __forceinline__ void arm_joint_frame(const float* T, const M3& Rp, V3 pp, float q, M3& Rj, V3& pj) {
+    M3 Jr; Jr.c0 = mk(T[3], T[6], T[9]); Jr.c1 = mk(T[4], T[7], T[10]); Jr.c2 = mk(T[5], T[8], T[11]);   // row-major -> columns
+    Rj = mulM(mulM(Rp, Jr), axis_angle(mk(T[12], T[13], T[14]), q));
+    pj = pp + mul(Rp, mk(T[0], T[1], T[2]));
+}
 
 // ABA passes 1 and 2 over the arm: kinematics, bias terms, inward reduction.  Returns the arm's articulated inertia and
 // bias force as seen by the base (to be added to the base sums), fills A.S/U/k/u/cJ.
@@ -46,31 +53,18 @@ static __device__ __noinline__ void arm_inward(const float* __restrict__ AT, con
                                         AI& IaOut, SV& paOut, float kdamp) {
     AI IAb[ARM_NJ]; SV pAb[ARM_NJ];
     M3 Rp = R0; V3 pp = mk(0.f, 0.f, 0.f); SV vp = v0;
-    const float gz = -10.0f;
 #pragma unroll 1
     for (int j = 0; j < ARM_NJ; j++) {
         const float* T = AT + ARM_STRIDE * j;
-        M3 Jr; Jr.c0 = mk(T[3], T[6], T[9]); Jr.c1 = mk(T[4], T[7], T[10]); Jr.c2 = mk(T[5], T[8], T[11]);   // row-major -> columns
-        V3 ax = mk(T[12], T[13], T[14]);
-        M3 Rj = mulM(mulM(Rp, Jr), axis_angle(ax, A.q[j]));
-        V3 pj = pp + mul(Rp, mk(T[0], T[1], T[2]));
-        SV S; S.a = mul(Rj, ax); S.l = cross(pj, S.a);
+        M3 Rj; V3 pj;
+        arm_joint_frame(T, Rp, pp, A.q[j], Rj, pj);
+        SV S; S.a = mul(Rj, mk(T[12], T[13], T[14])); S.l = cross(pj, S.a);
         SV vj = A.qd[j] * S;
         SV v = vp + vj;
         SV cJ = crm(v, vj);
-        float m = T[15]; V3 cw = pj + mul(Rj, mk(T[16], T[17], T[18]));
         S3 Ib = {T[19], T[20], T[21], T[22], T[23], T[24]};
-        const S3 Iw = rotate_inertia(Rj, Ib);
-        AI I = rigid_inertia(m, cw, Iw);
-        SV pA = crf(v, mul(I, v));
-        pA.a = pA.a - mk(cw.y * m * gz, -cw.x * m * gz, 0.f); pA.l.z -= m * gz;
-        {   // link damping (same term as the legs: rexsim_kernel.cu link_damping)
-            V3 vo = v.l + cross(v.a, pj);
-            float wn = sqrtf(dot(v.a, v.a)), vn = sqrtf(dot(vo, vo));
-            V3 f = (m * fmaf(kdamp, vn, kdamp)) * vo;
-            pA.a = pA.a + fmaf(kdamp, wn, kdamp) * mul(Iw, v.a) + cross(pj, f);
-            pA.l = pA.l + f;
-        }
+        AI I; SV pA;
+        link_terms(T[15], pj + mul(Rj, mk(T[16], T[17], T[18])), rotate_inertia(Rj, Ib), pj, v, kdamp, I, pA);
         IAb[j] = I; pAb[j] = pA;
         st6(A.S[j], S); st6(A.cJ[j], cJ);
         A.R[j][0] = Rj.c0.x; A.R[j][1] = Rj.c0.y; A.R[j][2] = Rj.c0.z; A.R[j][3] = Rj.c1.x; A.R[j][4] = Rj.c1.y;
@@ -109,6 +103,16 @@ static __device__ __noinline__ void arm_apply(Arm& A, SV b, const float* us, flo
         b = sfma(dq[j], ld6(A.S[j]), b);
     }
 }
+// fixed-base joint response ee[] of the arm to the inward joint terms uu[] of a row
+__device__ __forceinline__ void arm_fixed_response(const Arm& A, const float* uu, float* ee) {
+    SV w; w.a = mk(0, 0, 0); w.l = mk(0, 0, 0);
+#pragma unroll 1
+    for (int j = 0; j < ARM_NJ; j++) {
+        float e = (uu[j] - sdot(ld6(A.U[j]), w)) * A.k[j];
+        ee[j] = e;
+        w = sfma(e, ld6(A.S[j]), w);
+    }
+}
 // one joint-limit row of the arm (unit generalized force sg on joint jl): base bias g, fixed-base joint response ee[],
 // inward joint terms uu[]
 static __device__ __noinline__ void arm_row(const Arm& A, int jl, float sg, SV& g, float* ee, float* uu) {
@@ -121,13 +125,7 @@ static __device__ __noinline__ void arm_row(const Arm& A, int jl, float sg, SV& 
         if (j <= jl) pD = sfma(ud * A.k[j], ld6(A.U[j]), pD);
     }
     g = pD;
-    SV w; w.a = mk(0, 0, 0); w.l = mk(0, 0, 0);
-#pragma unroll 1
-    for (int j = 0; j < ARM_NJ; j++) {
-        float e = (uu[j] - sdot(ld6(A.U[j]), w)) * A.k[j];
-        ee[j] = e;
-        w = sfma(e, ld6(A.S[j]), w);
-    }
+    arm_fixed_response(A, uu, ee);
 }
 // one contact row on arm body jb (unit spatial force F about the base position): joint Jacobian jq[] (S_j . F for the joints
 // j <= jb that carry the body, 0 beyond), base bias g, fixed-base joint response ee[], inward joint terms uu[]
@@ -142,13 +140,7 @@ static __device__ __noinline__ void arm_force_row(const Arm& A, int jb, SV F, SV
         if (j <= jb) pD = sfma(ud * A.k[j], ld6(A.U[j]), pD);
     }
     g = pD - F;
-    SV w; w.a = mk(0, 0, 0); w.l = mk(0, 0, 0);
-#pragma unroll 1
-    for (int j = 0; j < ARM_NJ; j++) {
-        float e = (uu[j] - sdot(ld6(A.U[j]), w)) * A.k[j];
-        ee[j] = e;
-        w = sfma(e, ld6(A.S[j]), w);
-    }
+    arm_fixed_response(A, uu, ee);
 }
 
 }  // namespace rexsim

@@ -81,17 +81,6 @@ struct Lane {
     int cost;              // solver iterations spent this control step (drives the warp re-grouping, rexsim_rebalance)
 };
 
-__device__ __forceinline__ M3 quat_to_mat(float x, float y, float z, float w) {   // btMatrix3x3::setRotation
-    float d = x * x + y * y + z * z + w * w;
-    float s = 2.0f / d;
-    float xs = x * s, ys = y * s, zs = z * s;
-    float wx = w * xs, wy = w * ys, wz = w * zs, xx = x * xs, xy = x * ys, xz = x * zs, yy = y * ys, yz = y * zs, zz = z * zs;
-    M3 R;
-    R.c0 = mk(1.f - (yy + zz), xy + wz, xz - wy);
-    R.c1 = mk(xy - wz, 1.f - (xx + zz), yz + wx);
-    R.c2 = mk(xz + wy, yz - wx, 1.f - (xx + yy));
-    return R;
-}
 __device__ __forceinline__ void quat_to_euler(float x, float y, float z, float w, float* rpy) {   // pybullet getEulerFromQuaternion
     float sqx = x * x, sqy = y * y, sqz = z * z, squ = w * w;
     float sarg = -2.f * (x * z - w * y);
@@ -307,6 +296,26 @@ __device__ __forceinline__ void plane_space(V3 n, V3& p, V3& q) {   // btPlaneSp
         q = mk(-n.z * p.y, n.z * p.x, a * k);
     }
 }
+// friction directions of a contact with normal n: fixed on flat ground, else btPlaneSpace1 of n
+__device__ __forceinline__ void contact_tangents(bool plane, V3 n, V3& t1, V3& t2) {
+    if (plane) { t1 = mk(0.f, -1.f, 0.f); t2 = mk(1.f, 0.f, 0.f); }
+    else plane_space(n, t1, t2);
+}
+// right-hand sides of the unilateral rows (btMultiBodyConstraintSolver::setupMultiBodyContactConstraint,
+// btMultiBodyJointLimitConstraint), scaled by the inverse denominator dinv of the row.  With m_splitImpulse the positional term of
+// a penetration deeper than 0.04 goes to m_rhsPenetration, which the multibody solver never applies (the row only stops further
+// motion).  Each branch scales on its own: that is the instruction stream the fast path is tuned for.
+// Contact normal at distance `dist`: speculative below the slop, Baumgarte inside it.
+__device__ __forceinline__ float contact_rhs(const Params& P, float relv, float dist, float inv_dt, float dinv) {
+    float pen = dist + 1e-5f;
+    float poserr = 0.f, velerr = -relv;
+    if (pen > 0.f) velerr -= pen * inv_dt; else poserr = -pen * P.cfg.erp_contact * inv_dt;
+    return (pen > -0.04f) ? (poserr + velerr) * dinv : velerr * dinv;
+}
+// joint limit violated by pen <= 0 (the fast path's own leg-limit row divides by its denominator instead, and is written there)
+__device__ __forceinline__ float limit_rhs(const Params& P, float relv, float pen, float inv_dt, float dinv) {
+    return (pen > -0.04f) ? (-pen * P.cfg.erp_joint * inv_dt - relv) * dinv : -relv * dinv;
+}
 
 // generic-path Gauss-Seidel order after the limit rows (rows 0..2 of a lane = its three joint limits), the oracle's contact-group
 // order: normals (base, then per leg upper, foot, then the six arm bodies), then frictions in the same order.  Owner 0..3 = the
@@ -339,17 +348,40 @@ __device__ __forceinline__ float motor_torque(float cmd, float q, float qd, floa
     else t = 0.1f * mag;
     return copysignf(t, cur) * (cur != 0.f ? 1.f : 0.f);
 }
+// one motor of Rex.ApplyAction (rex.py:568-641): the torque from the PD observation (q, qd, or sensor words wq, wqd as they were
+// pd_latency ago), then the overheat counter (10 bits at `shift` of `ovh`): past `limit` consecutive sub-steps above 2.45 N m
+// the motor's bit of `enabled` clears for good.  Returns the applied torque.
+__device__ __forceinline__ float motor_step(const Params& P, const Sensor& S, bool pd_delayed, int wq, int wqd, float cmd, float q,
+                                            float qd, float kp, float kd, uint32_t limit, uint32_t& ovh, int shift,
+                                            uint32_t& enabled, int bit, float& tau_obs) {
+    float qo = q, qdo = qd;
+    if (pd_delayed) {
+        qo = sensor_delayed(S, P.lat_pd, P.n_pd, P.a_pd, wq);
+        qdo = sensor_delayed(S, P.lat_pd, P.n_pd, P.a_pd, wqd);
+    }
+    const float ta = motor_torque(cmd, qo, qdo, qd, kp, kd, tau_obs);
+    uint32_t c = (ovh >> shift) & 1023u;
+    c = (fabsf(ta) > 2.45f) ? min(c + 1u, 1023u) : 0u;
+    if (c > limit) enabled &= ~(1u << bit);
+    ovh = (ovh & ~(1023u << shift)) | (c << shift);
+    return ((enabled >> bit) & 1u) ? ta : 0.f;
+}
 
-// btMultiBody::computeAccelerationsArticulatedBodyAlgorithmMultiDof adds the damping term of the base to EVERY link too
-// (m_linearDamping = m_angularDamping = 0.04, K1 = K2): torque I w (k + k|w|) about the link origin and force
-// m v_o (k + k|v_o|) at it, v_o = velocity of the link origin.  Expressed about the common-frame origin (the base position).
-__device__ __forceinline__ void link_damping(float k, float m, const S3& Iw, V3 p, const SV& v, SV& pA) {
-    V3 vo = v.l + cross(v.a, p);
-    float wn = sqrtf(dot(v.a, v.a)), vn = sqrtf(dot(vo, vo));
-    V3 f = (m * fmaf(k, vn, k)) * vo;
-    V3 n = fmaf(k, wn, k) * mul(Iw, v.a);
-    pA.a = pA.a + n + cross(p, f);
-    pA.l = pA.l + f;
+// link_terms of the leg body whose model table (REXSIM_MT_LEG) is T, with frame R
+__device__ __forceinline__ void leg_link_terms(const float* T, const M3& R, V3 p, const SV& v, float k, AI& IA, SV& pA) {
+    link_terms(T[3], p + mul(R, mk(T[4], T[5], T[6])), world_inertia(R, T + 8, T[15]), p, v, k, IA, pA);
+}
+// generic-path sweep: g . beta of a row's base bias g (6 floats) and the base velocity change beta
+__device__ __forceinline__ float dot6(const float* g, const SV& beta) {
+    return g[0] * beta.a.x + g[1] * beta.a.y + g[2] * beta.a.z + g[3] * beta.l.x + g[4] * beta.l.y + g[5] * beta.l.z;
+}
+// response of a leg's joint rates to a base velocity change b plus joint impulses e1..e3 through its inward terms (arm_apply
+// of the leg)
+__device__ __forceinline__ void leg_apply(SV b, float e1, float e2, float e3, const SV& S1, const SV& S2, const SV& U1, const SV& U2,
+                                          const SV& U3, float k1, float k2, float k3, float& dq1, float& dq2, float& dq3) {
+    dq1 = (e1 - sdot(U1, b)) * k1; b = sfma(dq1, S1, b);
+    dq2 = (e2 - sdot(U2, b)) * k2; b = sfma(dq2, S2, b);
+    dq3 = (e3 - sdot(U3, b)) * k3;
 }
 __device__ __forceinline__ float clampv(float v, float lim) { return fminf(fmaxf(v, -lim), lim); }
 
@@ -366,14 +398,8 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
     const float* LB = sm + REXSIM_MT_LEG + leg * 48;
     // ---- forward kinematics, world-aligned frame with origin at the base position -------------------
     M3 R0 = quat_to_mat(L.qx, L.qy, L.qz, L.qw);
-    float s1, c1, s2, c2, s3, c3;
-    sincosf(L.q[0], &s1, &c1); sincosf(L.q[1], &s2, &c2); sincosf(L.q[2], &s3, &c3);
-    M3 R1; R1.c0 = R0.c0; R1.c1 = fma3(c1, R0.c1, s1 * R0.c2); R1.c2 = fma3(-s1, R0.c1, c1 * R0.c2);
-    M3 R2; R2.c0 = fma3(c2, R1.c0, -s2 * R1.c2); R2.c1 = R1.c1; R2.c2 = fma3(s2, R1.c0, c2 * R1.c2);
-    M3 R3; R3.c0 = fma3(c3, R2.c0, -s3 * R2.c2); R3.c1 = R2.c1; R3.c2 = fma3(s3, R2.c0, c3 * R2.c2);
-    V3 p1 = mul(R0, mk(LB[0], LB[1], LB[2]));
-    V3 p2 = p1 + mul(R1, mk(LB[16], LB[17], LB[18]));
-    V3 p3 = p2 + mul(R2, mk(LB[32], LB[33], LB[34]));
+    M3 R1, R2, R3; V3 p1, p2, p3;
+    leg_frames(R0, LB, L.q, R1, R2, R3, p1, p2, p3);
     SV S1, S2, S3v;
     S1.a = R0.c0; S1.l = cross(p1, S1.a);
     S2.a = R1.c1; S2.l = cross(p2, S2.a);
@@ -383,35 +409,10 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
     SV vj1 = L.qd[0] * S1, vj2 = L.qd[1] * S2, vj3 = L.qd[2] * S3v;
     SV v1 = v0 + vj1, v2 = v1 + vj2, v3 = v2 + vj3;
     SV cJ1 = crm(v1, vj1), cJ2 = crm(v2, vj2), cJ3 = crm(v3, vj3);
-    const float gz = -10.0f;   // setGravity(0,0,-10) rex_gym_env.py:314
     AI IA1, IA2, IA3; SV pA1, pA2, pA3;
-    {
-        float m = LB[3]; V3 cw = p1 + mul(R1, mk(LB[4], LB[5], LB[6]));
-        S3 Ib = {LB[8], LB[9], LB[10], LB[11], LB[12], LB[13]};
-        const S3 Iw = (LB[15] != 0.f ? rotate_inertia_diag(R1, Ib.xx, Ib.yy, Ib.zz) : rotate_inertia(R1, Ib));
-        IA1 = rigid_inertia(m, cw, Iw);
-        pA1 = crf(v1, mul(IA1, v1));
-        pA1.a = pA1.a - mk(cw.y * m * gz, -cw.x * m * gz, 0.f); pA1.l.z -= m * gz;
-        link_damping(P.cfg.link_damping, m, Iw, p1, v1, pA1);
-    }
-    {
-        float m = LB[16 + 3]; V3 cw = p2 + mul(R2, mk(LB[16 + 4], LB[16 + 5], LB[16 + 6]));
-        S3 Ib = {LB[16 + 8], LB[16 + 9], LB[16 + 10], LB[16 + 11], LB[16 + 12], LB[16 + 13]};
-        const S3 Iw = (LB[16 + 15] != 0.f ? rotate_inertia_diag(R2, Ib.xx, Ib.yy, Ib.zz) : rotate_inertia(R2, Ib));
-        IA2 = rigid_inertia(m, cw, Iw);
-        pA2 = crf(v2, mul(IA2, v2));
-        pA2.a = pA2.a - mk(cw.y * m * gz, -cw.x * m * gz, 0.f); pA2.l.z -= m * gz;
-        link_damping(P.cfg.link_damping, m, Iw, p2, v2, pA2);
-    }
-    {
-        float m = LB[32 + 3]; V3 cw = p3 + mul(R3, mk(LB[32 + 4], LB[32 + 5], LB[32 + 6]));
-        S3 Ib = {LB[32 + 8], LB[32 + 9], LB[32 + 10], LB[32 + 11], LB[32 + 12], LB[32 + 13]};
-        const S3 Iw = (LB[32 + 15] != 0.f ? rotate_inertia_diag(R3, Ib.xx, Ib.yy, Ib.zz) : rotate_inertia(R3, Ib));
-        IA3 = rigid_inertia(m, cw, Iw);
-        pA3 = crf(v3, mul(IA3, v3));
-        pA3.a = pA3.a - mk(cw.y * m * gz, -cw.x * m * gz, 0.f); pA3.l.z -= m * gz;
-        link_damping(P.cfg.link_damping, m, Iw, p3, v3, pA3);
-    }
+    leg_link_terms(LB, R1, p1, v1, P.cfg.link_damping, IA1, pA1);
+    leg_link_terms(LB + 16, R2, p2, v2, P.cfg.link_damping, IA2, pA2);
+    leg_link_terms(LB + 32, R3, p3, v3, P.cfg.link_damping, IA3, pA3);
     // ---- ABA inward pass over the own leg ------------------------------------------------------------
     SV U3 = mul(IA3, S3v); float k3 = 1.0f / sdot(S3v, U3); float u3 = tau[2] - sdot(S3v, pA3);
     rank1_sub(IA3, U3, k3);
@@ -434,10 +435,9 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
     {
         const float* B = sm + REXSIM_MT_BASE;
         float m = B[0]; V3 cw = mul(R0, mk(B[1], B[2], B[3]));
-        S3 Ib = {B[4], B[5], B[6], B[7], B[8], B[9]};
-        IA0 = rigid_inertia(m, cw, B[14] != 0.f ? rotate_inertia_diag(R0, Ib.xx, Ib.yy, Ib.zz) : rotate_inertia(R0, Ib));
+        IA0 = rigid_inertia(m, cw, world_inertia(R0, B + 4, B[14]));
         pA0 = crf(v0, mul(IA0, v0));
-        pA0.a = pA0.a - mk(cw.y * m * gz, -cw.x * m * gz, 0.f); pA0.l.z -= m * gz;
+        gravity_bias(m, cw, pA0);
         // Bullet default base damping 0.04 (K1 = K2) with the un-merged root link's mass / inertia
         const float kd = 0.04f;
         V3 wb = mk(dot(R0.c0, L.w), dot(R0.c1, L.w), dot(R0.c2, L.w));
@@ -695,8 +695,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
         constexpr int NR = LIM ? 4 : 3;                         // own rows: n, t1, t2 (, limit)
         // ---- constraint rows of the own contact: n, t1, t2 ----------------------------------------------
         V3 t1, t2;
-        if (TERRAIN == REXSIM_TERRAIN_PLANE) { t1 = mk(0.f, -1.f, 0.f); t2 = mk(1.f, 0.f, 0.f); }
-        else plane_space(nrm, t1, t2);
+        contact_tangents(TERRAIN == REXSIM_TERRAIN_PLANE, nrm, t1, t2);
         SV F[3];
         F[0].a = cross(rc, nrm); F[0].l = nrm;
         F[1].a = cross(rc, t1); F[1].l = t1;
@@ -738,7 +737,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
             ownLL = j0 * e1 + j1 * e2 + j2 * e3;
             denL = hasL ? ownLL - sdot(g[3], dvb[3]) : 1.f;
             const float relL = j0 * qs1 + j1 * qs2 + j2 * qs3;
-            // m_splitImpulse: beyond the -0.04 threshold the positional term goes to m_rhsPenetration, which is never applied
+            // limit_rhs, but divided by denL: one multiply by 1 / denL rounds differently
             rhsL = hasL ? ((limPen > -0.04f) ? (-limPen * P.cfg.erp_joint * inv_dt - relL) : -relL) / denL : 0.f;
         }
         // ARM builds: up to ARM_KA violated arm joint limits ride along as extra rows owned by lane 0 (slot a = a-th violated
@@ -773,8 +772,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                     sgA[a] = sg;
                     denA[a] = -sdot(gA[a], bbA[a]) + sg * eeA[a][j];
                     dinvA[a] = 1.0f / denA[a];
-                    const float relvA = sg * AR.qs[j];
-                    rhsA[a] = (armPen[j] > -0.04f) ? (-armPen[j] * P.cfg.erp_joint * inv_dt - relvA) * dinvA[a] : -relvA * dinvA[a];
+                    rhsA[a] = limit_rhs(P, sg * AR.qs[j], armPen[j], inv_dt, dinvA[a]);
                 }
             }
             // arm x arm block: velocity of slot a's joint per unit impulse of slot c = sg_a * ee_c[j_a] - g_a . b_c
@@ -826,15 +824,9 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
         float den[NR], dinv[NR], rhs[NR];
 #pragma unroll
         for (int d = 0; d < 3; d++) { den[d] = Dd[d][d] - sdot(g[d], dvb[d]); dinv[d] = 1.0f / den[d]; }
-        {
-            const float slop = 1e-5f;
-            float pen = best + slop;
-            float poserr = 0.f, velerr = -relv[0];
-            if (pen > 0.f) velerr -= pen * inv_dt; else poserr = -pen * P.cfg.erp_contact * inv_dt;
-            rhs[0] = (pen > -0.04f) ? (poserr + velerr) * dinv[0] : velerr * dinv[0];
-            rhs[1] = -relv[1] * dinv[1];
-            rhs[2] = -relv[2] * dinv[2];
-        }
+        rhs[0] = contact_rhs(P, relv[0], best, inv_dt, dinv[0]);
+        rhs[1] = -relv[1] * dinv[1];
+        rhs[2] = -relv[2] * dinv[2];
         if (LIM) { den[3] = denL; dinv[3] = 1.0f / denL; rhs[3] = rhsL; }
         // ---- PGS in impulse space, Bullet row order: joint-limit rows (legs, arm), normals 0..3, then (t1,t2) of contacts 0..3 ----
         // Each lane keeps only its own impulses and the PRE-SCALED running row sums t[d] = rhs[d] - dinv[d] * sum_j A[d][j] lambda_j:
@@ -1060,10 +1052,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
             }
         }
         dv0 = sum4(own_b);
-        SV b = dv0;
-        dq1 = (e1 - sdot(U1, b)) * k1; b = sfma(dq1, S1, b);
-        dq2 = (e2 - sdot(U2, b)) * k2; b = sfma(dq2, S2, b);
-        dq3 = (e3 - sdot(U3, b)) * k3;
+        leg_apply(dv0, e1, e2, e3, S1, S2, U1, U2, U3, k1, k2, k3, dq1, dq2, dq3);
         if (ARM && leg == 0) arm_apply(AR, dv0, usA, dqA);
     };
     if (envf != 0u && !(envf & 2u)) {
@@ -1107,25 +1096,16 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
             actbits |= 1u << ri;
             return relv;
         };
-        // right-hand side of a contact normal row: speculative below the slop, Baumgarte inside it; with m_splitImpulse the
-        // positional term of a penetration deeper than 0.04 m goes to m_rhsPenetration, which the multibody solver never applies
-        auto contact_rhs = [&](float relv, float dist, float dinv) -> float {
-            float pen = dist + 1e-5f;
-            float poserr = 0.f, velerr = -relv;
-            if (pen > 0.f) velerr -= pen * inv_dt; else poserr = -pen * P.cfg.erp_contact * inv_dt;
-            return (pen > -0.04f) ? (poserr + velerr) * dinv : velerr * dinv;
-        };
         auto setup_contact = [&](int r0, V3 r, V3 n, int kb, float dist) {
             V3 t1, t2;
-            if (TERRAIN == REXSIM_TERRAIN_PLANE) { t1 = mk(0.f, -1.f, 0.f); t2 = mk(1.f, 0.f, 0.f); }
-            else plane_space(n, t1, t2);
+            contact_tangents(TERRAIN == REXSIM_TERRAIN_PLANE, n, t1, t2);
 #pragma unroll 1
             for (int d = 0; d < 3; d++) {
                 V3 dir = d == 0 ? n : (d == 1 ? t1 : t2);
                 SV F; F.a = cross(r, dir); F.l = dir;
                 float j0 = kb >= 1 ? sdot(S1, F) : 0.f, j1 = kb >= 2 ? sdot(S2, F) : 0.f, j2 = kb >= 3 ? sdot(S3v, F) : 0.f;
                 float relv = setup_row(r0 + d, F, j0, j1, j2);
-                rhs_[r0 + d] = d == 0 ? contact_rhs(relv, dist, dinv_[r0]) : -relv * dinv_[r0 + d];
+                rhs_[r0 + d] = d == 0 ? contact_rhs(P, relv, dist, inv_dt, dinv_[r0]) : -relv * dinv_[r0 + d];
             }
         };
 #pragma unroll 1
@@ -1135,14 +1115,13 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
             const float pen = j == 0 ? limPenJ[0] : (j == 1 ? limPenJ[1] : limPenJ[2]);
             SV z; z.a = mk(0, 0, 0); z.l = mk(0, 0, 0);
             float relv = setup_row(j, z, j == 0 ? sg : 0.f, j == 1 ? sg : 0.f, j == 2 ? sg : 0.f);
-            // btMultiBodyJointLimitConstraint with m_splitImpulse: beyond the -0.04 threshold the positional term goes to
-            // m_rhsPenetration, which the multibody solver never applies (the row only stops further motion)
-            rhs_[j] = (pen > -0.04f) ? (-pen * P.cfg.erp_joint * inv_dt - relv) * dinv_[j] : -relv * dinv_[j];
+            rhs_[j] = limit_rhs(P, relv, pen, inv_dt, dinv_[j]);
         }
         if (activeB) setup_contact(3, rcB, nrmB, 0, bestB);
         if (activeU) setup_contact(6, rcU, nrmU, kU, bestU);
         if (active) setup_contact(9, rc, nrm, 3, best);
-        // arm joint-limit rows (lane 0)
+        // arm joint-limit rows (lane 0).  They stay apart from the arm contact rows below: stored as rows of that table (joint
+        // Jacobian sg e_j), they spill more in the arm builds
         float gA_[ARM ? ARM_NJ : 1][6], bA_[ARM ? ARM_NJ : 1][6], eeA_[ARM ? ARM_NJ : 1][ARM_NJ], uuA_[ARM ? ARM_NJ : 1][ARM_NJ];
         float rhsA_[ARM_NJ], dinvA_[ARM_NJ], denA_[ARM_NJ], lamA_[ARM_NJ], epsA[ARM_NJ], usA[ARM_NJ];
         if (ARM) {
@@ -1157,8 +1136,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                 st6(gA_[j], gg); st6(bA_[j], bb);
                 float dn = -sdot(gg, bb) + armSg[j] * eeA_[j][j];
                 denA_[j] = dn; dinvA_[j] = 1.0f / dn;
-                float relv = armSg[j] * AR.qs[j];
-                rhsA_[j] = (armPen[j] > -0.04f) ? (-armPen[j] * P.cfg.erp_joint * inv_dt - relv) * dinvA_[j] : -relv * dinvA_[j];
+                rhsA_[j] = limit_rhs(P, armSg[j] * AR.qs[j], armPen[j], inv_dt, dinvA_[j]);
             }
         }
         // arm contact rows (lane 0): rows 3k, 3k+1, 3k+2 = normal, t1, t2 of arm body k.  Only the rows of bodies in contact are
@@ -1171,8 +1149,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
             for (int k = 0; k < ARM_NJ; k++) {
                 if (!((armC >> k) & 1u)) continue;
                 V3 t1, t2;
-                if (TERRAIN == REXSIM_TERRAIN_PLANE) { t1 = mk(0.f, -1.f, 0.f); t2 = mk(1.f, 0.f, 0.f); }
-                else plane_space(nrmA[k], t1, t2);
+                contact_tangents(TERRAIN == REXSIM_TERRAIN_PLANE, nrmA[k], t1, t2);
 #pragma unroll 1
                 for (int d = 0; d < 3; d++) {
                     const int r = 3 * k + d;
@@ -1185,7 +1162,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
 #pragma unroll
                     for (int j = 0; j < ARM_NJ; j++) { dn = fmaf(jqC_[r][j], eeC_[r][j], dn); relv = fmaf(jqC_[r][j], AR.qs[j], relv); }
                     denC_[r] = dn; dinvC_[r] = 1.0f / dn; lamC_[r] = 0.f;
-                    rhsC_[r] = d == 0 ? contact_rhs(relv, bestA[k], dinvC_[r]) : -relv * dinvC_[r];
+                    rhsC_[r] = d == 0 ? contact_rhs(P, relv, bestA[k], inv_dt, dinvC_[r]) : -relv * dinvC_[r];
                 }
             }
         }
@@ -1224,7 +1201,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                     const int idx = llist[(it & 1) ? tt : nl - 1 - tt];
                     if (ARM && idx >= 12) {                         // an arm joint-limit row, owned by lane 0
                         const int j = idx - 12;
-                        float rsumA = armSg[j] * epsA[j] - (gA_[j][0] * beta.a.x + gA_[j][1] * beta.a.y + gA_[j][2] * beta.a.z + gA_[j][3] * beta.l.x + gA_[j][4] * beta.l.y + gA_[j][5] * beta.l.z);
+                        float rsumA = armSg[j] * epsA[j] - dot6(gA_[j], beta);
                         float dIA = rhsA_[j] - rsumA * dinvA_[j];
                         if (lamA_[j] + dIA < 0.f) dIA = -lamA_[j];
                         dIA = (((armLim >> j) & 1u) && leg == 0) ? dIA : 0.f;
@@ -1244,9 +1221,10 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                         SV dBC; dBC.a = mk(0.f, 0.f, 0.f); dBC.l = mk(0.f, 0.f, 0.f);
                         if (leg == 0) {
                             const int ph = ri % 3;
-                            float rsumC = -(gC_[ri][0] * beta.a.x + gC_[ri][1] * beta.a.y + gC_[ri][2] * beta.a.z + gC_[ri][3] * beta.l.x + gC_[ri][4] * beta.l.y + gC_[ri][5] * beta.l.z);
+                            float rsumC = -dot6(gC_[ri], beta);
 #pragma unroll
                             for (int c = 0; c < ARM_NJ; c++) rsumC = fmaf(jqC_[ri][c], epsA[c], rsumC);
+                            // the clamp of the leg rows below, written twice: one shared form lengthens the leg rows' code
                             float dIC = rhsC_[ri] - rsumC * dinvC_[ri];
                             const float lr = lamC_[ri];
                             if (ph == 0) { if (lr + dIC < 0.f) dIC = -lr; }
@@ -1266,8 +1244,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
                     }
                 }
                 const int ph = (ri < 3) ? 0 : ri % 3;                   // 0: unilateral row (limit / normal), 1/2: friction row
-                float rsum = Jq_[ri][0] * eps0 + Jq_[ri][1] * eps1 + Jq_[ri][2] * eps2
-                           - (g_[ri][0] * beta.a.x + g_[ri][1] * beta.a.y + g_[ri][2] * beta.a.z + g_[ri][3] * beta.l.x + g_[ri][4] * beta.l.y + g_[ri][5] * beta.l.z);
+                float rsum = Jq_[ri][0] * eps0 + Jq_[ri][1] * eps1 + Jq_[ri][2] * eps2 - dot6(g_[ri], beta);
                 float dI = rhs_[ri] - rsum * dinv_[ri];
                 const float lr = lam_[ri];
                 bool ok = ((actbits >> ri) & 1u) && (leg == o);
@@ -1289,10 +1266,7 @@ __device__ __forceinline__ void physics_substep(const Params& P, const float* __
             if (resid <= thr) running = false;
         }
         dv0 = beta;
-        SV b = dv0;
-        dq1 = (us0 - sdot(U1, b)) * k1; b = sfma(dq1, S1, b);
-        dq2 = (us1 - sdot(U2, b)) * k2; b = sfma(dq2, S2, b);
-        dq3 = (us2 - sdot(U3, b)) * k3;
+        leg_apply(dv0, us0, us1, us2, S1, S2, U1, U2, U3, k1, k2, k3, dq1, dq2, dq3);
         if (ARM && leg == 0) arm_apply(AR, dv0, usA, dqA);
     }
     // ---- integrate (btMultiBody::stepPositionsMultiDof) --------------------------------------------------
@@ -1332,46 +1306,21 @@ __device__ __forceinline__ void apply_action_and_step(const Params& P, const flo
     float tau[3];
     float tauA[ARM_NJ];
     const bool pd_delayed = SENSOR && P.lat_pd > 0.f;        // _GetPDObservation (rex.py:755-759): q, qd as they were pd_latency ago
+    const uint32_t limit = (uint32_t)(1.0 / P.cfg.sim_dt_d);   // OVERHEAT_SHUTDOWN_TIME / time_step
     if (ARM) {
 #pragma unroll
         for (int j = 0; j < ARM_NJ; j++) tauA[j] = 0.f;
         if (leg == 0) {
-            const uint32_t limitA = (uint32_t)(1.0 / P.cfg.sim_dt_d);
 #pragma unroll
-            for (int j = 0; j < ARM_NJ; j++) {
-                float to;
-                float qo = AR.q[j], qdo = AR.qd[j];
-                if (pd_delayed) {
-                    qo = sensor_delayed(S, P.lat_pd, P.n_pd, P.a_pd, HW_ARM + j);
-                    qdo = sensor_delayed(S, P.lat_pd, P.n_pd, P.a_pd, HW_ARM + 6 + j);
-                }
-                float ta = motor_torque(c_arm_rest[j], qo, qdo, AR.qd[j], kp, kd, to);
-                uint32_t w = AR.ovh[j / 3], c = (w >> (10 * (j % 3))) & 1023u;
-                c = (fabsf(ta) > 2.45f) ? min(c + 1u, 1023u) : 0u;
-                if (c > limitA) AR.enabled &= ~(1u << j);
-                AR.ovh[j / 3] = (w & ~(1023u << (10 * (j % 3)))) | (c << (10 * (j % 3)));
-                AR.tau_obs[j] = to;
-                tauA[j] = ((AR.enabled >> j) & 1u) ? ta : 0.f;
-            }
+            for (int j = 0; j < ARM_NJ; j++)
+                tauA[j] = motor_step(P, S, pd_delayed, HW_ARM + j, HW_ARM + 6 + j, c_arm_rest[j], AR.q[j], AR.qd[j], kp, kd, limit,
+                                     AR.ovh[j / 3], 10 * (j % 3), AR.enabled, j, AR.tau_obs[j]);
         }
     }
-    const uint32_t limit = (uint32_t)(1.0 / P.cfg.sim_dt_d);   // OVERHEAT_SHUTDOWN_TIME / time_step
 #pragma unroll
-    for (int j = 0; j < 3; j++) {
-        float to;
-        float qo = L.q[j], qdo = L.qd[j];
-        if (pd_delayed) {
-            qo = sensor_delayed(S, P.lat_pd, P.n_pd, P.a_pd, 9 * leg + j);
-            qdo = sensor_delayed(S, P.lat_pd, P.n_pd, P.a_pd, 9 * leg + 3 + j);
-        }
-        float ta = motor_torque(cmd[j], qo, qdo, L.qd[j], kp, kd, to);
-        uint32_t c = (L.ovh >> (10 * j)) & 1023u;
-        c = (fabsf(ta) > 2.45f) ? min(c + 1u, 1023u) : 0u;
-        if (c > limit) L.enabled &= ~(1u << j);
-        L.ovh = (L.ovh & ~(1023u << (10 * j))) | (c << (10 * j));
-        L.tau_obs[j] = to;
-        tau[j] = ((L.enabled >> j) & 1u) ? ta : 0.f;
-    }
+    for (int j = 0; j < 3; j++)
+        tau[j] = motor_step(P, S, pd_delayed, 9 * leg + j, 9 * leg + 3 + j, cmd[j], L.q[j], L.qd[j], kp, kd, limit, L.ovh, 10 * j,
+                            L.enabled, j, L.tau_obs[j]);
     physics_substep<TERRAIN, ARM, REPL>(P, sm, L, leg, tau, G, AR, tauA, pgs);
     if (SENSOR) sensor_push<ARM>(S, leg, L, AR, valid);         // Rex.ReceiveObservation (rex.py:162,726-733)
 }

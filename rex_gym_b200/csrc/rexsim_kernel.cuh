@@ -181,6 +181,61 @@ __device__ __forceinline__ S3 rotate_inertia_diag(const M3& R, float dx, float d
 __device__ __forceinline__ SV crm(SV v, SV m) { SV r; r.a = cross(v.a, m.a); r.l = cross(v.a, m.l) + cross(v.l, m.a); return r; }
 __device__ __forceinline__ SV crf(SV v, SV f) { SV r; r.a = cross(v.a, f.a) + cross(v.l, f.l); r.l = cross(v.a, f.l); return r; }
 
+// ----- body geometry and per-link terms, in the world-aligned frame with origin at the base position ----------------------
+__device__ __forceinline__ M3 quat_to_mat(float x, float y, float z, float w) {   // btMatrix3x3::setRotation
+    float d = x * x + y * y + z * z + w * w;
+    float s = 2.0f / d;
+    float xs = x * s, ys = y * s, zs = z * s;
+    float wx = w * xs, wy = w * ys, wz = w * zs, xx = x * xs, xy = x * ys, xz = x * zs, yy = y * ys, yz = y * zs, zz = z * zs;
+    M3 R;
+    R.c0 = mk(1.f - (yy + zz), xy + wz, xz - wy);
+    R.c1 = mk(xy - wz, 1.f - (xx + zz), yz + wx);
+    R.c2 = mk(xz + wy, yz - wx, 1.f - (xx + yy));
+    return R;
+}
+// frames of a leg's three bodies and their origins relative to the base position, from the base frame R0, the leg's model
+// table LB (REXSIM_MT_LEG) and its joint angles q: shoulder about x, leg and foot about y, unrotated joint frames
+__device__ __forceinline__ void leg_frames(const M3& R0, const float* LB, const float* q, M3& R1, M3& R2, M3& R3, V3& p1, V3& p2,
+                                           V3& p3) {
+    float s1, c1, s2, c2, s3, c3;
+    sincosf(q[0], &s1, &c1); sincosf(q[1], &s2, &c2); sincosf(q[2], &s3, &c3);
+    R1.c0 = R0.c0; R1.c1 = fma3(c1, R0.c1, s1 * R0.c2); R1.c2 = fma3(-s1, R0.c1, c1 * R0.c2);
+    R2.c0 = fma3(c2, R1.c0, -s2 * R1.c2); R2.c1 = R1.c1; R2.c2 = fma3(s2, R1.c0, c2 * R1.c2);
+    R3.c0 = fma3(c3, R2.c0, -s3 * R2.c2); R3.c1 = R2.c1; R3.c2 = fma3(s3, R2.c0, c3 * R2.c2);
+    p1 = mul(R0, mk(LB[0], LB[1], LB[2]));
+    p2 = p1 + mul(R1, mk(LB[16], LB[17], LB[18]));
+    p3 = p2 + mul(R2, mk(LB[32], LB[33], LB[34]));
+}
+// world inertia R I R^T of a body whose model table holds I = (xx, yy, zz, xy, xz, yz) and a flag that I is diagonal
+__device__ __forceinline__ S3 world_inertia(const M3& R, const float* I, float diag) {
+    const S3 Ib = {I[0], I[1], I[2], I[3], I[4], I[5]};
+    return diag != 0.f ? rotate_inertia_diag(R, Ib.xx, Ib.yy, Ib.zz) : rotate_inertia(R, Ib);
+}
+// gravity on mass m with its centre of mass at c, as a bias force (setGravity(0,0,-10) rex_gym_env.py:314)
+__device__ __forceinline__ void gravity_bias(float m, V3 c, SV& pA) {
+    const float gz = -10.0f;
+    pA.a = pA.a - mk(c.y * m * gz, -c.x * m * gz, 0.f); pA.l.z -= m * gz;
+}
+// btMultiBody::computeAccelerationsArticulatedBodyAlgorithmMultiDof adds the damping term of the base to EVERY link too
+// (m_linearDamping = m_angularDamping = 0.04, K1 = K2): torque I w (k + k|w|) about the link origin and force
+// m v_o (k + k|v_o|) at it, v_o = velocity of the link origin.  Expressed about the common-frame origin (the base position).
+__device__ __forceinline__ void link_damping(float k, float m, const S3& Iw, V3 p, const SV& v, SV& pA) {
+    V3 vo = v.l + cross(v.a, p);
+    float wn = sqrtf(dot(v.a, v.a)), vn = sqrtf(dot(vo, vo));
+    V3 f = (m * fmaf(k, vn, k)) * vo;
+    V3 n = fmaf(k, wn, k) * mul(Iw, v.a);
+    pA.a = pA.a + n + cross(p, f);
+    pA.l = pA.l + f;
+}
+// ABA pass 1 for one link of a limb (origin p, velocity v, mass m, centre of mass cw, world inertia Iw): its spatial inertia and
+// its bias force (velocity product, gravity, link damping k)
+__device__ __forceinline__ void link_terms(float m, V3 cw, const S3& Iw, V3 p, const SV& v, float k, AI& IA, SV& pA) {
+    IA = rigid_inertia(m, cw, Iw);
+    pA = crf(v, mul(IA, v));
+    gravity_bias(m, cw, pA);
+    link_damping(k, m, Iw, p, v, pA);
+}
+
 // ----- width-4 (one env) shuffles -------------------------------------------------------------------
 // The member mask names only the 4 lanes of the env: different envs of a warp may diverge (stay-still
 // early-outs, auto-reset, converged solvers) without deadlocking each other's shuffles.

@@ -13,6 +13,7 @@
 // shared memory, and culls the spheres against the tile's frustum.  Then every thread casts its pixel's ray against
 // the surviving shapes and the ground.  The kernel only reads the state.
 #include "rexsim_kernel.cuh"
+#include "rexsim_arm.cuh"
 
 namespace rexsim {
 
@@ -89,51 +90,20 @@ __device__ __forceinline__ void write_sphere(float* rec, V3 c, float r) {
 }
 __device__ __forceinline__ V3 ld3(const float* p) { return mk(p[0], p[1], p[2]); }
 
-// btMatrix3x3::setRotation, written as rexsim_kernel.cu's quat_to_mat (which stays there: moving it into the shared header
-// reorders the step kernels' stack slots)
-__device__ __forceinline__ M3 quat_rotation(float x, float y, float z, float w) {
-    float d = x * x + y * y + z * z + w * w;
-    float s = 2.0f / d;
-    float xs = x * s, ys = y * s, zs = z * s;
-    float wx = w * xs, wy = w * ys, wz = w * zs, xx = x * xs, xy = x * ys, xz = x * zs, yy = y * ys, yz = y * zs, zz = z * zs;
-    M3 R;
-    R.c0 = mk(1.f - (yy + zz), xy + wz, xz - wy);
-    R.c1 = mk(xy - wz, 1.f - (xx + zz), yz + wx);
-    R.c2 = mk(xz + wy, yz - wx, 1.f - (xx + yy));
-    return R;
-}
-// Rodrigues rotation about unit axis a (columns), and A B
-__device__ __forceinline__ M3 rot_axis(V3 a, float q) {
-    float s, c; sincosf(q, &s, &c); float t = 1.f - c;
-    M3 R;
-    R.c0 = mk(t * a.x * a.x + c, t * a.x * a.y + s * a.z, t * a.x * a.z - s * a.y);
-    R.c1 = mk(t * a.x * a.y - s * a.z, t * a.y * a.y + c, t * a.y * a.z + s * a.x);
-    R.c2 = mk(t * a.x * a.z + s * a.y, t * a.y * a.z - s * a.x, t * a.z * a.z + c);
-    return R;
-}
-__device__ __forceinline__ M3 mulMM(const M3& A, const M3& B) { M3 r; r.c0 = mul(A, B.c0); r.c1 = mul(A, B.c1); r.c2 = mul(A, B.c2); return r; }
-
 // warp 0: pose every shape of env `env` into `shapes` (world frame)
 __device__ void pose_shapes(const RenderArgs& A, int env, float* shapes, int lane) {
     const size_t N = A.N;
     const float* sf = A.sf;
     const V3 pos = mk(sf[(F_POS + 0) * N + env], sf[(F_POS + 1) * N + env], sf[(F_POS + 2) * N + env]);
-    const M3 R0 = quat_rotation(sf[(F_QUAT + 0) * N + env], sf[(F_QUAT + 1) * N + env], sf[(F_QUAT + 2) * N + env],
-                                sf[(F_QUAT + 3) * N + env]);
+    const M3 R0 = quat_to_mat(sf[(F_QUAT + 0) * N + env], sf[(F_QUAT + 1) * N + env], sf[(F_QUAT + 2) * N + env],
+                              sf[(F_QUAT + 3) * N + env]);
     const float* mt = A.model;
-    if (lane < 4) {            // leg `lane`: shoulder about x, leg and foot about y, unrotated joint frames (model_tables.py)
+    if (lane < 4) {            // leg `lane`: the step kernel's frames, origins moved from the base position to the world's
         const int leg = lane;
-        const float* LB = mt + REXSIM_MT_LEG + leg * 48;
-        float s1, c1, s2, c2, s3, c3;
-        sincosf(sf[(F_Q + 3 * leg + 0) * N + env], &s1, &c1);
-        sincosf(sf[(F_Q + 3 * leg + 1) * N + env], &s2, &c2);
-        sincosf(sf[(F_Q + 3 * leg + 2) * N + env], &s3, &c3);
-        M3 R1; R1.c0 = R0.c0; R1.c1 = fma3(c1, R0.c1, s1 * R0.c2); R1.c2 = fma3(-s1, R0.c1, c1 * R0.c2);
-        M3 R2; R2.c0 = fma3(c2, R1.c0, -s2 * R1.c2); R2.c1 = R1.c1; R2.c2 = fma3(s2, R1.c0, c2 * R1.c2);
-        M3 R3; R3.c0 = fma3(c3, R2.c0, -s3 * R2.c2); R3.c1 = R2.c1; R3.c2 = fma3(s3, R2.c0, c3 * R2.c2);
-        V3 p1 = pos + mul(R0, ld3(LB));
-        V3 p2 = p1 + mul(R1, ld3(LB + 16));
-        V3 p3 = p2 + mul(R2, ld3(LB + 32));
+        const float q[3] = {sf[(F_Q + 3 * leg + 0) * N + env], sf[(F_Q + 3 * leg + 1) * N + env], sf[(F_Q + 3 * leg + 2) * N + env]};
+        M3 R1, R2, R3; V3 p1, p2, p3;
+        leg_frames(R0, mt + REXSIM_MT_LEG + leg * 48, q, R1, R2, R3, p1, p2, p3);
+        p1 = pos + p1; p2 = pos + p2; p3 = pos + p3;
         const float* BX = mt + REXSIM_MT_BOX + leg * 72;
         write_box(shapes + (3 + 3 * leg + 0) * SHAPE_FLOATS, BX, R1, p1);
         write_box(shapes + (3 + 3 * leg + 1) * SHAPE_FLOATS, BX + 24, R2, p2);
@@ -146,11 +116,9 @@ __device__ void pose_shapes(const RenderArgs& A, int env, float* shapes, int lan
         write_box(shapes + (lane - 4) * SHAPE_FLOATS, mt + REXSIM_MT_BASEBOX + 24 * (lane - 4), R0, pos);
     } else if (lane == 7 && A.arm) {   // the arm: one serial chain with general joint frames (rexsim_arm.cuh layout)
         M3 Rp = R0; V3 pp = pos;
-        for (int j = 0; j < 6; j++) {
-            const float* T = mt + REXSIM_MT_ARM + 32 * j;
-            M3 Jr; Jr.c0 = mk(T[3], T[6], T[9]); Jr.c1 = mk(T[4], T[7], T[10]); Jr.c2 = mk(T[5], T[8], T[11]);
-            M3 Rj = mulMM(mulMM(Rp, Jr), rot_axis(ld3(T + 12), sf[(F_AQ + j) * N + env]));
-            V3 pj = pp + mul(Rp, ld3(T));
+        for (int j = 0; j < ARM_NJ; j++) {
+            M3 Rj; V3 pj;
+            arm_joint_frame(mt + REXSIM_MT_ARM + ARM_STRIDE * j, Rp, pp, sf[(F_AQ + j) * N + env], Rj, pj);
             const float* cy = A.rt + REXSIM_RT_CYL + 8 * j;
             float* rec = shapes + (19 + j) * SHAPE_FLOATS;
             V3 c = pj + mul(Rj, ld3(cy)), ax = mul(Rj, ld3(cy + 3));

@@ -7,7 +7,12 @@ Runs every step-kernel instance of tests/test_gpu_builds.INSTANCES (forced build
 auto-reset after 15 steps), walk-ik on flat ground at 8449 and 65 536 envs and turn-ik on heightfields at 16 897 envs (the
 big build, warp re-grouping on) once per library, each library in its own process (REXSIM_LIB).  After every step it hashes
 obs, reward, done, last_command, the error words, the whole SoA state and the sensor ring; then bench.py --dump-outputs.
-Every later library is compared with the first: each array that is not bit-identical is reported."""
+Random actions from reset rarely reach the generic solver path, so every configuration of tests/test_gpu_generic_path.CONFIGS
+also runs from that test's start states (body, arm and multi-limit contacts): 4 single sub-steps, then 4 control steps of the
+task configuration, hashing rexsim_solver_cost as well.  Last, render_batch frames of a few envs of walk-ik on flat ground,
+turn-ik on the random heightfields and standup with the arm, with the default camera and at 97 x 61.
+Every later library is compared with the first: each array that is not bit-identical is reported, and for a frame the number
+of pixels that differ."""
 import hashlib
 import json
 import os
@@ -36,37 +41,95 @@ def digest(a):
     return hashlib.sha256(str((a.dtype.str, a.shape)).encode() + a.tobytes()).hexdigest()
 
 
+def _force_build(build):
+    if build:
+        os.environ["REXSIM_FORCE_BUILD"] = build
+    else:
+        os.environ.pop("REXSIM_FORCE_BUILD", None)
+
+
+def _record(env, rec, k, ret, cost=False):
+    """Hash what step `k` returned (`ret`) and left in the library's buffers into `rec`."""
+    o, r, d = ret[:3]
+    arrs = dict(obs=o, reward=r, done=d, cmd=env.last_command(), err=env._err, sf=env._state_f, si=env._state_i)
+    if env._ring is not None:
+        arrs["ring"] = env._ring
+    for name, v in arrs.items():
+        rec[f"{k:02d}_{name}"] = digest(v if isinstance(v, np.ndarray) else v.cpu().numpy())
+    if cost:
+        import test_gpu_generic_path as G
+        rec[f"{k:02d}_cost"] = digest(G._cost(env))
+
+
+def generic_cases(R, res):
+    """tests/test_gpu_generic_path start states, every CONFIGS entry: single sub-steps, then control steps."""
+    import test_gpu_generic_path as G
+    for mark, terrain, build in G.CONFIGS:
+        ids, st = G._batch(mark, terrain)
+        for sub, steps in ((True, 4), (False, 4)):
+            _force_build(None if build == "sensor" else build)
+            kw = dict(G.SUB) if sub else {}
+            if build == "sensor":
+                kw["observation_noise_stdev"] = G.NOISE
+            env = R.BatchedRexEnv(task="walk", num_envs=G.N, signal_type="ik", terrain_type=terrain, num_fields=4, mark=mark,
+                                  seed=21, target_position=2.0, backwards=False, **kw)
+            env.reset()
+            G._set(env, st)
+            rng = np.random.default_rng(7)
+            rec = res[f"generic-{mark}-{terrain}-{build}-{'substep' if sub else 'control'}"] = {}
+            for k in range(steps):
+                ret = env.step(rng.uniform(-0.4, 0.4, size=(G.N, env.action_dim)).astype(np.float32))
+                _record(env, rec, k, ret, cost=True)
+            env.close()
+
+
+def render_cases(R, res, frames):
+    """render_batch of a few stepped envs: default camera and an odd size."""
+    import torch
+    _force_build(None)
+    for cid, task, kw in (("render-walk-ik-plane", "walk", dict(signal_type="ik")),
+                          ("render-turn-ik-random", "turn", dict(signal_type="ik", terrain_type="random", num_fields=4)),
+                          ("render-standup-ol-arm", "standup", dict(signal_type="ol", mark="arm"))):
+        env = R.BatchedRexEnv(task=task, num_envs=8, seed=5, **kw)
+        env.reset()
+        rng = np.random.default_rng(2)
+        for _ in range(30):
+            env.step(rng.uniform(-0.1, 0.1, size=(8, env.action_dim)).astype(np.float32))
+        for size, (w, h) in (("480x360", (480, 360)), ("97x61", (97, 61))):
+            img = env.render_batch(torch.arange(4, device="cuda"), width=w, height=h).cpu().numpy()
+            res[f"{cid}-{size}"] = {"frames": digest(img)}
+            frames[f"{cid}-{size}"] = img
+        env.close()
+
+
 def run(out):
-    """Child process: every case with the library REXSIM_LIB names; {case: {step_array: sha256}} to `out`."""
+    """Child process: every case with the library REXSIM_LIB names; {case: {step_array: sha256}} to `out`, the render frames
+    beside it (frames.npz)."""
     import torch
     import rex_gym_b200 as R
     from rex_gym_b200.envs.batched_env import ACTION_BOUND
     res = {}
     for cid, task, build, n, kw in cases():
-        if build:
-            os.environ["REXSIM_FORCE_BUILD"] = build
-        else:
-            os.environ.pop("REXSIM_FORCE_BUILD", None)
+        _force_build(build)
         env = R.BatchedRexEnv(task=task, num_envs=n, auto_reset=True, **kw)
         env.reset()
         rng = np.random.default_rng(11)
         b = ACTION_BOUND[(task, kw["signal_type"])]
         rec = res[cid] = {}
         for k in range(40):
-            a = torch.as_tensor(rng.uniform(-b, b, size=(n, env.action_dim)).astype(np.float32), device="cuda")
-            o, r, d = env.step(a)[:3]
-            arrs = dict(obs=o, reward=r, done=d, cmd=env.last_command(), err=env._err, sf=env._state_f, si=env._state_i)
-            if env._ring is not None:
-                arrs["ring"] = env._ring
-            for name, v in arrs.items():
-                rec[f"{k:02d}_{name}"] = digest(v.cpu().numpy())
+            ret = env.step(torch.as_tensor(rng.uniform(-b, b, size=(n, env.action_dim)).astype(np.float32), device="cuda"))
+            _record(env, rec, k, ret)
         env.close()
+    generic_cases(R, res)
+    frames = {}
+    render_cases(R, res, frames)
     with open(out, "w") as f:
         json.dump(res, f)
+    np.savez(os.path.join(os.path.dirname(out), "frames.npz"), **frames)
 
 
 def outputs(lib):
-    """{case: {step_array: sha256}} of every case and of bench.py --dump-outputs with library `lib`."""
+    """{case: {step_array: sha256}} of every case and of bench.py --dump-outputs with library `lib`, and the render frames."""
     env = dict(os.environ, REXSIM_LIB=os.path.abspath(lib))
     with tempfile.TemporaryDirectory(prefix="ab_outputs_") as d:
         subprocess.run([sys.executable, os.path.abspath(__file__), "--child", os.path.join(d, "steps.json")], env=env,
@@ -77,20 +140,26 @@ def outputs(lib):
             steps = json.load(f)
         for f in sorted(os.listdir(os.path.join(d, "bench"))):
             steps["bench " + f] = {"array": digest(np.load(os.path.join(d, "bench", f)))}
-    return steps
+        with np.load(os.path.join(d, "frames.npz")) as z:
+            frames = {k: z[k] for k in z.files}
+    return steps, frames
 
 
 def main(libs):
     runs = [outputs(lib) for lib in libs]
-    status = 0
-    for lib, other in zip(libs[1:], runs[1:]):
+    (ref_steps, ref_frames), status = runs[0], 0
+    for lib, (other, frames) in zip(libs[1:], runs[1:]):
         print(f"== {libs[0]} vs {lib}")
         nbad = 0
-        for cid, ref in runs[0].items():
+        for cid, ref in ref_steps.items():
             bad = [k for k in ref if other.get(cid, {}).get(k) != ref[k]]
             nbad += bool(bad)
-            print(f"{cid:32s} {'identical' if not bad else 'DIFFERS in %d arrays, first %s' % (len(bad), bad[0])}")
-        print(f"{len(runs[0]) - nbad} of {len(runs[0])} runs bit-identical\n")
+            what = "identical" if not bad else "DIFFERS in %d arrays, first %s" % (len(bad), bad[0])
+            if bad and cid in ref_frames:
+                px = (ref_frames[cid] != frames[cid]).any(-1).reshape(len(ref_frames[cid]), -1).sum(1)
+                what += f", differing pixels per image {px.tolist()} of {ref_frames[cid][0, ..., 0].size}"
+            print(f"{cid:40s} {what}")
+        print(f"{len(ref_steps) - nbad} of {len(ref_steps)} runs bit-identical\n")
         status |= nbad > 0
     return status
 
