@@ -335,6 +335,17 @@ class OracleSim:
         return dict(pos=np.array(e.pos), quat=np.array(e.quat), linvel=np.array(e.linvel), angvel=np.array(e.angvel),
                     q=np.array(e.q[:nd]), qd=np.array(e.qd[:nd]))
 
+    def states(self):
+        """state() of every env, batched: {key: [N][...]}."""
+        st = [self.state(i) for i in range(self.N)]
+        return {k: np.stack([s[k] for s in st]) for k in st[0]}
+
+    def set_state(self, i, st):
+        """Write a physical state (the keys of state()) into env i."""
+        e = self.env(i)
+        for k in ("pos", "quat", "linvel", "angvel", "q", "qd"):
+            getattr(e, k)[:len(st[k])] = [float(x) for x in st[k]]
+
     def mass_matrix_inv(self, i=0):
         nd = 6 + self.model.ndof
         M = np.zeros((nd, nd))

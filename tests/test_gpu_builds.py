@@ -9,22 +9,20 @@
           (H100 SXM, 132 SMs: N > 8448 / N > 16 896)                take 78 KB of shared memory through the opt-in
   small   everything else                                           255 registers, 128-thread CTAs
 
-REXSIM_FORCE_BUILD=big|small replaces the size rule (arm batches stay on the small build); it is read on every step launch and
-does not touch the reset or settle kernels.
+twin.force_build(monkeypatch, "big" | "small") replaces the size rule (arm batches stay on the small build); the forced build is
+read on every step launch and does not touch the reset or settle kernels.
 
 INSTANCES is the table of reachable instances: 8 (task, signal) units x 2 terrains x 3 builds, plus the two arm units (walk-ik,
 standup) x 2 terrains x the small and sensor builds = 56 rows.  test_instance_against_the_oracle[<row id>] runs every row; the last
 column names the other tests of the suite that launch the same instance.
 """
-import ctypes
 import os
 
 import numpy as np
 import pytest
 import torch
-
-import test_gpu_parity as P
-from test_gpu_parity import TOL_P, TOL_Q, _bound, _env, _oracle, _oracle_state, _toe_mask
+from twin import (BUILDS, STATE_KEYS, TOL_P, TOL_Q, assert_draws, bound, force_build, launched, make_env, make_oracle,
+                  one_step_is_tight, state_errors, sync, toe_masks)
 
 FR, HF, SA = "test_gpu_parity::test_free_running_rollout", "test_gpu_parity::test_heightfield_contact_parity", "test_gpu_parity::test_sensor_latency_and_noise"
 BL, WARP = "test_gpu_parity::test_baseline_size_batches_against_the_oracle", "test_gpu_parity::test_batches_that_do_not_fill_their_last_warp"
@@ -95,9 +93,6 @@ UNITS = [("walk", "ik"), ("walk", "ol"), ("gallop", "ik"), ("gallop", "ol"), ("t
 ARM_UNITS = [("walk", "ik"), ("standup", "ol")]          # launch_step_ts: HAS_ARM
 
 
-BUILDS = {"small": (128, 1, 0), "big": (256, 4, 0), "sensor": (128, 1, 1)}     # (CTA size, CTAs per SM, sensor) of each build
-
-
 def _row_id(row):
     task, sig, arm, terrain, build, _ = row
     return "-".join([task, sig] + (["arm"] if arm else []) + [terrain, build])
@@ -118,13 +113,6 @@ def test_instance_table_lists_every_reachable_instance():
             assert ("def %s(" % name) in open(os.path.join(here, mod + ".py")).read(), ref
 
 
-def _launched(env):
-    """(CTA size, CTAs per SM, sensor) of the step_kernel instance env's last step launched (rexsim_last_step_build)."""
-    v = [ctypes.c_int32() for _ in range(3)]
-    assert env._L.rexsim_last_step_build(env._h, *[ctypes.byref(x) for x in v]) == 0
-    return tuple(x.value for x in v)
-
-
 def _config(task, sig, arm, terrain, build):
     kw = dict(signal_type=sig, seed=13, max_episode_steps=15)         # short episodes: every env runs the in-kernel reset twice
     if arm:
@@ -138,39 +126,10 @@ def _config(task, sig, arm, terrain, build):
     return kw
 
 
-def _sync_to_oracle(env, ora, idx):
-    """Overwrite the physical state of envs `idx` with the oracle's (the rest of the batch is written back unchanged)."""
-    st, so = env.get_state(), _oracle_state(ora, env.num_envs)
-    for k in ("pos", "quat", "linvel", "angvel", "q", "qd"):
-        st[k][idx] = so[k][idx]
-    env.set_state(st["pos"], st["quat"], st["linvel"], st["angvel"], st["q"], st["qd"])
-
-
-def _assert_bookkeeping(env, ora, sg, task, rough):
-    """Everything integer after a step, bit for bit: counters, resets, field ids, the draws of every reset."""
-    n = env.num_envs
-    E = [ora.env(i) for i in range(n)]
-    sf, si = env._state_f.cpu().numpy(), env._state_i.cpu().numpy()
-    np.testing.assert_array_equal(sg["step_counter"], [e.step_counter for e in E])
-    np.testing.assert_array_equal(sg["env_step_counter"], [e.env_step_counter for e in E])
-    np.testing.assert_array_equal(si[3], [e.reset_count for e in E])                                  # I_RESETCNT
-    if rough:
-        np.testing.assert_array_equal(si[4], [e.field_id for e in E])                                 # I_FIELD
-    tgt = [e.target_value if task == "poses" else e.target_position for e in E]
-    np.testing.assert_array_equal(sf[38], np.array(tgt, np.float32))                                  # F_TARGET
-    np.testing.assert_array_equal(sf[39], np.array([e.target_orient for e in E], np.float32))         # F_TORIENT
-    np.testing.assert_array_equal(sf[41], np.array([e.kp for e in E], np.float32))                    # F_KP
-    np.testing.assert_array_equal(sf[42], np.array([e.kd for e in E], np.float32))                    # F_KD
-    np.testing.assert_array_equal((si[2] >> 3) & 1, [e.backwards for e in E])
-    np.testing.assert_array_equal((si[2] >> 4) & 1, [e.clockwise for e in E])
-    if task == "poses":
-        np.testing.assert_array_equal((si[2] >> 26) & 7, [e.next_pose for e in E])                   # FL_POSE_SHIFT
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("row", INSTANCES, ids=[_row_id(r) for r in INSTANCES])
 def test_instance_against_the_oracle(monkeypatch, row):
-    """One instance, forced by REXSIM_FORCE_BUILD (the sensor build by its config; rexsim_last_step_build confirms which one ran
+    """One instance, forced by force_build (the sensor build by its config; rexsim_last_step_build confirms which one ran
     every step), against the oracle: 37 envs (padding lanes in
     both CTA sizes), 40 control steps of random actions inside the task's bound, auto-reset after 15 steps.  Integer results bit
     for bit after every step; continuous ones within the bounds the small build meets elsewhere in the suite:
@@ -183,13 +142,10 @@ def test_instance_against_the_oracle(monkeypatch, row):
     are not the first of an episode.
     Where the state starts from the oracle's, every auto-reset lands within the settle bounds and is re-synchronised."""
     task, sig, arm, terrain, build, _ = row
-    if build == "sensor":
-        monkeypatch.delenv("REXSIM_FORCE_BUILD", raising=False)
-    else:
-        monkeypatch.setenv("REXSIM_FORCE_BUILD", build)
+    force_build(monkeypatch, build)
     n, steps = 37, 40
     kw = _config(task, sig, arm, terrain, build)
-    env, ora = _env(task, n, auto_reset=True, **kw), _oracle(task, n, **kw)
+    env, ora = make_env(task, n, auto_reset=True, **kw), make_oracle(task, n, **kw)
     env.reset(); ora.reset()
     rough, standup = terrain == "random", task == "standup" or arm
     resync = rough or standup
@@ -197,14 +153,14 @@ def test_instance_against_the_oracle(monkeypatch, row):
     max_q, max_p = (2e-2, 5e-3) if rough and not standup else (5e-2, 5e-3)
     ta = 5e-3 if (rough or standup) else 1e-3                                      # roll / pitch observations
     if resync:
-        _sync_to_oracle(env, ora, np.arange(n))
+        sync(env, ora)
     rng = np.random.default_rng(11)
-    b = _bound(task, sig)
+    b = bound(task, sig)
     err_rp, contact_total, contact_bad = [], 0, 0
     for k in range(steps):
         a = rng.uniform(-b, b, size=(n, env.action_dim)).astype(np.float32)
         og, rg, dg, _ = env.step(a)
-        assert _launched(env) == BUILDS[build], _launched(env)
+        assert launched(env) == BUILDS[build], launched(env)
         oc, rc, dc = ora.step(a)
         np.testing.assert_array_equal(dg, dc, err_msg=f"done, step {k}")
         cmd = env.last_command().cpu().numpy()[:12].T
@@ -212,13 +168,12 @@ def test_instance_against_the_oracle(monkeypatch, row):
         idx = np.nonzero(dc)[0]
         if len(idx):
             oc[idx] = ora.reset(idx)                      # the oracle has no auto-reset: the same semantics by hand
-        sg, so = env.get_state(), _oracle_state(ora, n)
-        _assert_bookkeeping(env, ora, sg, task, rough)
+        sg, so = env.get_state(), ora.states()
+        assert_draws(env, ora, task)
         fresh = np.zeros(n, bool)
         fresh[idx] = True
         cmp = ~fresh if resync else np.ones(n, bool)
-        eq = np.abs(sg["q"] - so["q"]).max(axis=1)
-        ep = np.abs(sg["pos"] - so["pos"]).max(axis=1)
+        eq, ep = state_errors(env, ora)
         if not rough:
             ep = np.maximum(ep, np.abs(sg["quat"] - so["quat"]).max(axis=1))
         if resync and len(idx):
@@ -239,10 +194,9 @@ def test_instance_against_the_oracle(monkeypatch, row):
                 rcmp &= (np.abs(so["pos"][:, 2] - 0.21) > 2e-3) & (np.abs(l1 - 0.1) > 2e-3) & ~fresh
             np.testing.assert_allclose(rg[rcmp], rc[rcmp], atol=5e-3, err_msg=f"reward, step {k}")
         # the mask of contacts in the last sub-step: after a reset the CUDA path reports none yet, the oracle its settle's last
-        cm = np.array([_toe_mask(ora, i) for i in range(n)])
-        contact_total += (~fresh).sum(); contact_bad += ((cm != sg["contact_mask"]) & ~fresh).sum()
+        contact_total += (~fresh).sum(); contact_bad += ((toe_masks(ora) != sg["contact_mask"]) & ~fresh).sum()
         if resync and len(idx):
-            _sync_to_oracle(env, ora, idx)
+            sync(env, ora, idx)
     err_rp = np.concatenate(err_rp)
     assert np.percentile(err_rp, 90) < ta / 5 and err_rp.max() < (2e-2 if rough else ta), (np.percentile(err_rp, 90), err_rp.max())
     assert contact_bad <= 0.02 * max(contact_total, 1), (contact_bad, contact_total)
@@ -257,8 +211,8 @@ def test_instance_against_the_oracle(monkeypatch, row):
 def test_one_step_is_tight_in_both_builds(monkeypatch, build, task, sig, kw, bound):
     """test_one_step_is_tight (30 single control steps from an oracle-synchronised state) with the build forced: the big build
     meets the same rounding-level bounds as the small one."""
-    monkeypatch.setenv("REXSIM_FORCE_BUILD", build)
-    P.test_one_step_is_tight(task, sig, kw, bound)
+    force_build(monkeypatch, build)
+    one_step_is_tight(task, sig, kw, bound)
 
 
 @pytest.mark.gpu
@@ -272,16 +226,13 @@ def test_heightfield_big_build_at_its_natural_size():
     n, w0, nw, steps = 32768, 32768 // 2 + 37, 48, 40
     assert -(-n // 32) > 4 * torch.cuda.get_device_properties(0).multi_processor_count       # really above the switch
     kw = dict(signal_type="ik", terrain_type="random", num_fields=64, normalize=True, seed=11)
-    env, ora = _env("turn", n, **kw), _oracle("turn", nw, env_offset=w0, **kw)
+    env, ora = make_env("turn", n, **kw), make_oracle("turn", nw, env_offset=w0, **kw)
     env.reset(); ora.reset()
-    sf, si = env._state_f.cpu().numpy()[:, w0:w0 + nw], env._state_i.cpu().numpy()[:, w0:w0 + nw]
-    np.testing.assert_array_equal(si[4], [ora.env(i).field_id for i in range(nw)])
-    np.testing.assert_array_equal(sf[39], np.array([ora.env(i).target_orient for i in range(nw)], np.float32))
-    np.testing.assert_array_equal((si[2] >> 4) & 1, [ora.env(i).clockwise for i in range(nw)])
-    st, so = env.get_state(), _oracle_state(ora, nw)
-    for k in ("pos", "quat", "linvel", "angvel", "q", "qd"):
+    assert_draws(env, ora, "turn", window=w0)
+    st, so = env.get_state(), ora.states()
+    for k in STATE_KEYS:
         st[k][w0:w0 + nw] = so[k]
-    env.set_state(st["pos"], st["quat"], st["linvel"], st["angvel"], st["q"], st["qd"])
+    env.set_state(*(st[k] for k in STATE_KEYS))
     g = torch.Generator(device="cuda"); g.manual_seed(5)
     acts = torch.rand((steps, n, env.action_dim), device="cuda", generator=g) * 2 - 1
     err, bad = [], 0
@@ -290,12 +241,10 @@ def test_heightfield_big_build_at_its_natural_size():
         oc, rc, dc = ora.step(acts[k, w0:w0 + nw].cpu().numpy())
         np.testing.assert_array_equal(d[w0:w0 + nw].cpu().numpy(), dc)
         err.append(np.abs(o[w0:w0 + nw, :2].cpu().numpy() - oc[:, :2]).max(axis=1))
-        sg, so = env.get_state(), _oracle_state(ora, nw)
-        eq = np.abs(sg["q"][w0:w0 + nw] - so["q"]).max(1)
-        ep = np.abs(sg["pos"][w0:w0 + nw] - so["pos"]).max(1)
+        eq, ep = state_errors(env, ora, window=w0)
         assert np.percentile(eq, 90) < TOL_Q and np.percentile(ep, 90) < TOL_P and eq.max() < 2e-2 and ep.max() < 5e-3, \
             f"step {k}: {np.percentile(eq, 90):.2e} {np.percentile(ep, 90):.2e} {eq.max():.2e} {ep.max():.2e}"
-        bad += (np.array([_toe_mask(ora, i) for i in range(nw)]) != sg["contact_mask"][w0:w0 + nw]).sum()
+        bad += (toe_masks(ora) != env.get_state()["contact_mask"][w0:w0 + nw]).sum()
     err = np.concatenate(err) * (2 * np.pi + 0.01)                      # RangeNormalize'd -> radians
     assert np.percentile(err, 90) < 1e-3 and err.max() < 2e-2, (np.percentile(err, 90), err.max())
     assert bad <= 0.02 * steps * nw
@@ -318,23 +267,20 @@ def test_the_dispatcher_switches_builds_at_its_thresholds(monkeypatch, terrain, 
     if terrain == "random":
         kw.update(terrain_type="random", num_fields=4)
     for n, picked in ((threshold, "small"), (threshold + 1, "big")):
-        envs = {b: _env(task, n, **kw) for b in ("auto", "small", "big")}
+        envs = {b: make_env(task, n, **kw) for b in ("auto", "small", "big")}
         for e in envs.values():
             e.reset()
         g = torch.Generator(device="cuda"); g.manual_seed(9)
-        launched = {}
+        ran = {}
         for k in range(12):
             act = torch.rand((n, 2), device="cuda", generator=g) * 2 - 1
             out = {}
             for b, e in envs.items():
-                if b == "auto":
-                    monkeypatch.delenv("REXSIM_FORCE_BUILD", raising=False)
-                else:
-                    monkeypatch.setenv("REXSIM_FORCE_BUILD", b)
+                force_build(monkeypatch, None if b == "auto" else b)
                 out[b] = [t.clone() for t in e.step(act)[:3]]
-                launched.setdefault(b, set()).add(_launched(e))
+                ran.setdefault(b, set()).add(launched(e))
             assert all(torch.equal(x, y) for x, y in zip(out["auto"], out[picked])), (n, k)
-        assert launched["small"] == {(128, 1, 0)} and launched["big"] == {(256, 4, 0)} and launched["auto"] == launched[picked], (n, launched)
+        assert ran["small"] == {(128, 1, 0)} and ran["big"] == {(256, 4, 0)} and ran["auto"] == ran[picked], (n, ran)
         assert torch.equal(envs["auto"]._state_f, envs[picked]._state_f) and torch.equal(envs["auto"]._state_i, envs[picked]._state_i)
         for e in envs.values():
             assert (e.check_errors() & 1) == 0

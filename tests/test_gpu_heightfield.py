@@ -37,16 +37,14 @@ import math
 import numpy as np
 import pytest
 
-from test_gpu_builds import BUILDS, _launched
-from test_gpu_generic_path import HOLD, NOISE, SUB, WANT, _cost, _generic, _ostate, _quat, _set, _start, _violated, _write
+from twin import (BODY_BITS, BUILDS, FOLDED, LAYOUT, NOISE, STATE_KEYS, SUB, TOE_BITS, UPPER_BITS, IterationBand,
+                  compare_control_steps, compare_substeps, force_build, launched, make_env, make_oracle, qmul, quat, rot,
+                  state_errors, sync)
 
 CELL = 0.05
 EDGE = 127.5 * CELL                                     # vertex 0 / 255 of a field: its borders at x, y = -+6.375 m
-TOE_BITS = (1 << 2) | (1 << 4) | (1 << 6) | (1 << 8)
-UPPER_BITS = (1 << 1) | (1 << 3) | (1 << 5) | (1 << 7)
 TILE_MISS = 8                                           # REXSIM_FLAG_TILE_MISS
 BANKS = {"default": (64, 0), "big": (300, 255), "slopes": (7, 0)}   # (fields, env_offset): env i starts on (i + offset + 1) % fields
-FOLDED = np.array([-0.42, -1.51, 2.70, 0.42, -1.51, 2.70, -0.44, -1.49, 2.69, 0.44, -1.49, 2.69])
 CLEAR = 0.015                                           # drop height above the local ground
 STRETCH_CLEAR = 4e-4                                    # the stretched poses' lowest point: inside the 0.81 mm breaking distance
 
@@ -126,13 +124,6 @@ def _model():
     return _MODEL
 
 
-def _rot(q):
-    x, y, z, w = q
-    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)],
-                     [2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)],
-                     [2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)]])
-
-
 def _axis_angle(a, t):
     a = np.asarray(a, float)
     K = np.array([[0, -a[2], a[1]], [a[2], 0, -a[0]], [-a[1], a[0], 0]])
@@ -142,7 +133,7 @@ def _axis_angle(a, t):
 def _points(s):
     """World positions [P][3] and contact groups [P] of the points the heightfield contact samples, in state s."""
     M = _model()
-    Rw, pw = [_rot(s["quat"])], [np.asarray(s["pos"], float)]
+    Rw, pw = [rot(s["quat"])], [np.asarray(s["pos"], float)]
     for i in range(1, len(M["parent"])):
         p = M["parent"][i]
         Rw.append(Rw[p] @ M["jrot"][i] @ _axis_angle(M["axis"][i], s["q"][i - 1]))
@@ -174,13 +165,6 @@ def _window_origin(px):
 
 
 # ---- placements ------------------------------------------------------------------------------------------------------
-def _qmul(a, b):
-    ax, ay, az, aw = a
-    bx, by, bz, bw = b
-    return np.array([aw * bx + ax * bw + ay * bz - az * by, aw * by - ax * bz + ay * bw + az * bx,
-                     aw * bz + ax * by - ay * bx + az * bw, aw * bw - ax * bx - ay * by - az * bz])
-
-
 def _at(frac, cell=0):
     """World coordinate of cell fraction `frac` of the cell `cell` cells above the middle one."""
     return (127 + cell + frac - 127.5) * CELL
@@ -220,23 +204,30 @@ FALLEN = {"back": (math.pi + 0.04, 0.03), "side": (math.pi / 2 + 0.05, 0.02), "n
 def _want(pose, m, bank):
     """The contacts a placement is dropped until: standing, all four toes on the slopes and three on the random blocks (10 cm
     blocks up to 5 cm apart in height rarely carry all four feet at once); a shoulder or leg box on the knees; else the fallen
-    scenario's groups of test_gpu_generic_path.WANT."""
+    scenario's groups of test_gpu_generic_path.WANT (back: the base box; side: a shoulder or leg box; nose: either)."""
     if pose == "stand":
         return bin(m & TOE_BITS).count("1") >= (4 if bank == "slopes" else 3)
     if pose == "knees":
         return bool(m & UPPER_BITS)
     if pose.startswith("stretch"):
         return m != 0
-    return bool(WANT[pose](m, None))
+    return bool(m & {"back": 1, "side": UPPER_BITS, "nose": BODY_BITS}[pose])
 
 
-def _oracle(bank, n, sub=True, **kw):
-    from oracle.oracle import OracleSim
+def _kw(bank, sub=True, build=None):
+    """The keywords of a placement batch, the same for the GPU env and its oracle; the sensor build: observation noise only."""
+    nf, off = BANKS[bank]
+    kw = dict(signal_type="ik", terrain_type="random", num_fields=nf, env_offset=off, mark="base", seed=21, target_position=2.0,
+              backwards=False)
     if sub:
         kw.update(SUB)
-    nf, off = BANKS[bank]
-    return OracleSim(n, "walk", "ik", terrain="random", fields=_fields(bank), env_offset=off, mark="base", seed=21,
-                     target_position=2.0, backwards=False, **kw)
+    if build == "sensor":
+        kw["observation_noise_stdev"] = NOISE
+    return kw
+
+
+def _oracle(bank, n, sub=True, build=None, **extra):
+    return make_oracle("walk", n, fields=_fields(bank), **_kw(bank, sub, build), **extra)
 
 
 _CACHE = {}
@@ -264,7 +255,7 @@ def _batch(bank):
         for i in pending:
             if attempt == 0 or lay[i][1] == "stand":
                 st[i] = _place(bank, lay[i], settled[i], F[fid[i]], 0.5 * attempt)
-                _write(o, i, st[i])
+                o.set_state(i, st[i])
         for _ in range(150):
             prev = {i: o.state(i) for i in pending}
             o.step(np.zeros((n, o.A), np.float32))
@@ -293,7 +284,7 @@ def _place(bank, where, settled, f, turn, clear=CLEAR):
     kind, pose, x, y, yaw = where
     zo = _zoff(f)
     s = {k: np.array(v, np.float64) for k, v in settled.items()}
-    qy = _quat(0, 0, yaw + turn)
+    qy = quat(0, 0, yaw + turn)
     s["linvel"], s["angvel"], s["qd"] = np.zeros(3), np.zeros(3), np.zeros_like(s["qd"])
     if pose == "stand":                                 # upright with the settled joints (some fields settle the robot fallen)
         s["quat"] = qy
@@ -303,10 +294,10 @@ def _place(bank, where, settled, f, turn, clear=CLEAR):
             if np.linalg.norm(ax) > 1e-12:
                 a = math.acos(nrm[2]) / 2
                 t = ax / np.linalg.norm(ax) * math.sin(a)
-                s["quat"] = _qmul([t[0], t[1], t[2], math.cos(a)], s["quat"])
+                s["quat"] = qmul([t[0], t[1], t[2], math.cos(a)], s["quat"])
     else:
         r, p = FALLEN[pose.split("-")[-1]]
-        s["quat"] = _qmul(qy, _quat(r, p, 0.0))
+        s["quat"] = qmul(qy, quat(r, p, 0.0))
         if pose == "knees":
             s["q"][:12] = FOLDED
         if kind == "stretch":
@@ -350,7 +341,7 @@ def test_oracle_takes_banks_beyond_256_fields():
         s = {k: v.copy() for k, v in got[3].items()}
         s["pos"][2] -= _zoff(F[fid]) - _zoff(F[3])
         o.env(i).field_id = fid
-        _write(o, i, s)
+        o.set_state(i, s)
     for _ in range(50):
         o.step(a)
     s0 = o.state(0)
@@ -374,7 +365,8 @@ def test_placements_reach_their_contacts(bank):
         assert min(fid) >= 256
     o = _oracle(bank, n)
     o.reset()
-    _start(o, st)
+    for i in range(n):
+        o.set_state(i, {k: v[i] for k, v in st.items()})
     o.step(np.zeros((n, o.A), np.float32))
     for i, (kind, pose, *_r) in enumerate(lay):
         assert _want(pose, o.env(i).contact_mask, bank), (i, kind, pose, bin(o.env(i).contact_mask))
@@ -411,22 +403,11 @@ def test_placements_reach_their_contacts(bank):
 
 # ---- GPU ---------------------------------------------------------------------------------------------------------------
 def _gpu_env(bank, build, monkeypatch, n, sub=True):
-    import rex_gym_b200 as R
     from rex_gym_b200.envs import batched_env
     F = _fields(bank)
-    nf, off = BANKS[bank]
     monkeypatch.setattr(batched_env, "make_random_fields", lambda k, seed=10: F[:k].copy())
-    if build == "sensor":
-        monkeypatch.delenv("REXSIM_FORCE_BUILD", raising=False)
-    else:
-        monkeypatch.setenv("REXSIM_FORCE_BUILD", build)
-    kw = dict(SUB) if sub else {}
-    if build == "sensor":
-        kw["observation_noise_stdev"] = NOISE
-    env = R.BatchedRexEnv(task="walk", num_envs=n, signal_type="ik", terrain_type="random", num_fields=nf, env_offset=off,
-                          mark="base", seed=21, target_position=2.0, backwards=False, **kw)
-    okw = {"observation_noise_stdev": NOISE} if build == "sensor" else {}
-    return env, okw
+    force_build(monkeypatch, build)
+    return make_env("walk", n, **_kw(bank, sub, build))
 
 
 def _mask_exception(s, i, groups, f, zoff, breaking):
@@ -468,50 +449,16 @@ def test_heightfield_substeps_against_the_oracle(monkeypatch, bank, build):
     lay, st, fid = _batch(bank)
     n = len(lay)
     F = _fields(bank)
-    env, okw = _gpu_env(bank, build, monkeypatch, n)
-    ora = _oracle(bank, n, **okw)
-    band = [_oracle(bank, n, residual_threshold=t, f32=f, **okw) for t in HOLD for f in (False, True)]
-    env.reset(); ora.reset()
-    for b in band:
-        b.reset()
-    np.testing.assert_array_equal(env._state_i.cpu().numpy()[4], fid)            # I_FIELD
-    _start(ora, st)
+    env, ora = _gpu_env(bank, build, monkeypatch, n), _oracle(bank, n, build=build)
+    band = IterationBand(lambda **b: _oracle(bank, n, build=build, **b))
+    env.reset(); ora.reset(); band.reset()
+    np.testing.assert_array_equal(env._state_i.cpu().numpy()[LAYOUT.I_FIELD], fid)
     breaking = contact_breaking_distance("base")
-    rng = np.random.default_rng(7)
-    eq, ep, off_band, excused, generic_steps = [], [], 0, 0, 0
-    for k in range(30):
-        so = _ostate(ora)
-        _set(env, so)
-        for b in band:
-            _start(b, so)
-        viol = _violated(so["q"], "base")
-        a = rng.uniform(-0.4, 0.4, size=(n, env.action_dim)).astype(np.float32)
-        env.step(a)
-        assert _launched(env) == BUILDS[build], _launched(env)
-        ora.step(a)
-        its = []
-        for b in band:
-            b.step(a)
-            its.append([b.env(i).solver_iters for i in range(n)])
-        cost, sg = _cost(env), env.get_state()
-        flags = env.error_flags().cpu().numpy()
-        assert not (flags & TILE_MISS).any(), ("TILE_MISS", k, [lay[i][:2] for i in np.nonzero(flags & TILE_MISS)[0]])
-        mask = np.array([ora.env(i).contact_mask for i in range(n)]) & 0x1FF
-        gm = sg["contact_mask"] & 0x1FF
-        same = gm == mask
-        for i in np.nonzero(~same)[0]:
-            groups = [g for g in range(9) if ((gm[i] ^ mask[i]) >> g) & 1]
-            assert _mask_exception(so, i, groups, F[fid[i]], _zoff(F[fid[i]]), breaking), \
-                f"contact mask, sub-step {k}, env {i} {lay[i][:2]}: {bin(gm[i])} vs {bin(mask[i])}"
-            excused += 1
-        gen = _generic(mask, viol)
-        np.testing.assert_array_equal((cost >= 64)[same], gen[same], err_msg=f"solver path, sub-step {k}")
-        generic_steps += gen.sum()
-        lo_it, hi_it = np.min(its, 0), np.max(its, 0)
-        off_band += (((cost % 64 < lo_it) | (cost % 64 > hi_it)) & same).sum()
-        s2 = _ostate(ora)
-        eq.append(np.abs(sg["q"] - s2["q"]).max(1)); ep.append(np.abs(sg["pos"] - s2["pos"]).max(1))
-    eq, ep = np.concatenate(eq), np.concatenate(ep)
+    eq, ep, off_band, generic_steps, excused, flags = compare_substeps(
+        env, ora, band, st, build, [w[:2] for w in lay],
+        exception=lambda so, i, groups: _mask_exception(so, i, groups, F[fid[i]], _zoff(F[fid[i]]), breaking))
+    miss = np.argwhere(flags & TILE_MISS)
+    assert not len(miss), ("TILE_MISS", [(k, lay[i][:2]) for k, i in miss])
     stats = (np.median(eq), np.percentile(eq, 90), eq.max(), np.median(ep), np.percentile(ep, 90), ep.max(), off_band, excused)
     print("heightfield sub-steps q (median, p90, max), pos (median, p90, max), iterations off the band, mask exceptions:", stats)
     assert generic_steps >= 30 * 8 * 0.5, generic_steps
@@ -531,28 +478,10 @@ def test_heightfield_control_steps_against_the_oracle(monkeypatch, bank, build):
       default 9.4e-7 / 3.8e-6 / 2.8e-4, 1.9e-6;  big 7.5e-7 / 4.1e-6 / 3.4e-4, 1.9e-6;  slopes 1.2e-6 / 4.6e-6 / 9.4e-4, 5.1e-5."""
     lay, st, fid = _batch(bank)
     n = len(lay)
-    env, okw = _gpu_env(bank, build, monkeypatch, n, sub=False)
-    ora = _oracle(bank, n, sub=False, **okw)
+    env, ora = _gpu_env(bank, build, monkeypatch, n, sub=False), _oracle(bank, n, sub=False, build=build)
     env.reset(); ora.reset()
-    _start(ora, st)
-    rng = np.random.default_rng(9)
-    eqs, eps_ = [], []
-    for k in range(20):
-        if k % 5 == 0:
-            _set(env, _ostate(ora))
-        a = rng.uniform(-0.4, 0.4, size=(n, env.action_dim)).astype(np.float32)
-        og, rg, _, _ = env.step(a)
-        assert _launched(env) == BUILDS[build], _launched(env)
-        ora.step(a)
-        assert np.isfinite(og).all() and np.isfinite(rg).all()
-        assert not env.error_flags().cpu().numpy().any(), (k, env.error_flags().cpu().numpy())
-        sg, so = env.get_state(), _ostate(ora)
-        eq = np.abs(sg["q"] - so["q"]).max(1)
-        ep = np.abs(sg["pos"] - so["pos"]).max(1)
-        eqs.append(eq); eps_.append(ep)
-        assert np.percentile(eq, 90) < 1e-3 and np.percentile(ep, 90) < 1e-3, f"step {k}: {np.percentile(eq, 90):.2e} {np.percentile(ep, 90):.2e}"
-        assert eq.max() < 5e-2 and ep.max() < 5e-3, f"step {k}: {eq.max():.2e} {ep.max():.2e} in {lay[int(np.argmax(eq))][:2]}"
-    eqs, eps_ = np.concatenate(eqs), np.concatenate(eps_)
+    eqs, eps_, flags = compare_control_steps(env, ora, st, build, [w[:2] for w in lay], q90=1e-3, p90=1e-3, qmax=5e-2, pmax=5e-3)
+    assert not flags.any(), np.argwhere(flags)
     print("heightfield control steps q (median, p90, max), pos (median, p90, max):",
           (np.median(eqs), np.percentile(eqs, 90), eqs.max(), np.median(eps_), np.percentile(eps_, 90), eps_.max()))
     assert env.check_errors() == 0
@@ -569,32 +498,26 @@ def test_tile_miss_flags_exactly_the_envs_that_leave_the_window(monkeypatch, bui
     on the oracle), at 0, 1 m/s (2 cm per step) and 40 m/s (0.8 m per step) in +-x and +-y.  The 40 m/s envs leave the window
     staged at the start of the step and raise TILE_MISS, the others do not; with no contact the states still match the oracle.
     After set_state with zero velocity, the next step clears the per-env word."""
-    import rex_gym_b200 as R
     from rex_gym_b200.envs import batched_env
     n = len(FLY)
     F = np.zeros((1, 256, 256), np.float32)
     monkeypatch.setattr(batched_env, "make_random_fields", lambda k, seed=10: F.copy())
+    force_build(monkeypatch, build)
+    kw = dict(signal_type="ik", terrain_type="random", num_fields=1, seed=21, target_position=2.0, backwards=False,
+              control_time_step=0.02, action_repeat=20)
     if build == "sensor":
-        monkeypatch.delenv("REXSIM_FORCE_BUILD", raising=False)
-    else:
-        monkeypatch.setenv("REXSIM_FORCE_BUILD", build)
-    kw = dict(control_time_step=0.02, action_repeat=20)
-    noise = {"observation_noise_stdev": NOISE} if build == "sensor" else {}
-    env = R.BatchedRexEnv(task="walk", num_envs=n, signal_type="ik", terrain_type="random", num_fields=1, seed=21,
-                          target_position=2.0, backwards=False, **kw, **noise)
-    from oracle.oracle import OracleSim
-    ora = OracleSim(n, "walk", "ik", terrain="random", fields=F, seed=21, target_position=2.0, backwards=False, **kw, **noise)
-    env.reset(); ora.reset()
-    so = _ostate(ora)
+        kw["observation_noise_stdev"] = NOISE
+    env, ora, chk = make_env("walk", n, **kw), make_oracle("walk", n, fields=F, **kw), make_oracle("walk", n, fields=F, **kw)
+    env.reset(); ora.reset(); chk.reset()
+    so = ora.states()
     so["pos"][:, 2] += 0.035
     so["linvel"][:, :2] = FLY
     so["linvel"][:, 2] = 0.0
-    _start(ora, so)
-    _set(env, so)
+    for i in range(n):
+        ora.set_state(i, {k: v[i] for k, v in so.items()})
+        chk.set_state(i, {k: v[i] for k, v in so.items()})
+    sync(env, ora)
     a = np.zeros((n, env.action_dim), np.float32)
-    chk = OracleSim(n, "walk", "ik", terrain="random", fields=F, seed=21, target_position=2.0, backwards=False, **kw, **noise)
-    chk.reset()
-    _start(chk, so)
     for i in range(n):                                  # the same control step, sub-step by sub-step: no contact anywhere
         cmd = chk.transform_action(a[i], i)
         for _ in range(20):
@@ -602,19 +525,19 @@ def test_tile_miss_flags_exactly_the_envs_that_leave_the_window(monkeypatch, bui
             assert chk.env(i).contact_mask == 0, (i, FLY[i])
     ora.step(a)
     env.step(a)
-    assert _launched(env) == BUILDS[build], _launched(env)
+    assert launched(env) == BUILDS[build], launched(env)
     flags = env.error_flags().cpu().numpy()
     fast = np.array([math.hypot(*v) > 10 for v in FLY])
     np.testing.assert_array_equal((flags & TILE_MISS) != 0, fast)
     assert not (flags & ~TILE_MISS).any(), flags
-    sg, s2 = env.get_state(), _ostate(ora)
-    assert (sg["contact_mask"] == 0).all() and all(ora.env(i).contact_mask == 0 for i in range(n))
-    assert np.abs(sg["q"] - s2["q"]).max() < 1e-4 and np.abs(sg["pos"] - s2["pos"]).max() < 1e-5
+    assert (env.get_state()["contact_mask"] == 0).all() and all(ora.env(i).contact_mask == 0 for i in range(n))
+    eq, ep = state_errors(env, ora)
+    assert eq.max() < 1e-4 and ep.max() < 1e-5
     assert env.check_errors() == TILE_MISS
-    s2 = _ostate(ora)
+    s2 = ora.states()
     for k in ("linvel", "angvel", "qd"):
         s2[k][:] = 0.0
-    _set(env, s2)
+    env.set_state(*(s2[k] for k in STATE_KEYS))
     env.step(a)
     assert not env.error_flags().cpu().numpy().any()
     assert env.check_errors() == 0

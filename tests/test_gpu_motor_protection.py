@@ -17,15 +17,13 @@ import ctypes
 import numpy as np
 import pytest
 
-from test_gpu_builds import BUILDS, _launched
-from test_gpu_parity import _bound, _motor_protection, _oracle, _oracle_protection, _oracle_state, _sync_motor_protection
+from twin import (BUILDS, NOISE, SUB, bound, force_build, launched, make_env, make_oracle, oracle_protection, protection,
+                  state_errors, sync)
 
 N = 37
 SEEDED = np.array([i % 3 != 1 for i in range(N)])              # envs 0, 2, 3, 5, ..., 36 seeded; 1, 4, ..., 34 not
 FEET = [2, 5, 8, 11]
-SUB = dict(control_time_step=0.001, action_repeat=1, solver_iterations=60)      # test_gpu_generic_path.SUB: one sub-step per step
 EDGE = dict(control_time_step=0.00489, action_repeat=5)        # 1 / dt = 1022.49: the largest floor(1 / dt) the counters serve
-NOISE = (0.01, 0.05, 0.1, 0.02, 0.1)                           # the sensor build, with zero latencies
 
 # scenario: (task, signal, mark, control steps of random actions before the seeding, extra kwargs)
 SCENARIOS = {
@@ -71,12 +69,12 @@ def _prepare(name, terrain, env=None, **extra):
     """Oracle (and, if given, the GPU env) reset and stepped to the seeding point on the same actions; the oracle seeded on the
     SEEDED envs.  -> (oracle, rng for the actions that follow)."""
     task, kw = _okw(name, terrain, **extra)
-    ora = _oracle(task, N, **kw)
+    ora = make_oracle(task, N, **kw)
     ora.reset()
     if env is not None:
         env.reset()
     rng = np.random.default_rng(5)
-    b = _bound(task, SCENARIOS[name][1])
+    b = bound(task, SCENARIOS[name][1])
     for k in range(SCENARIOS[name][3]):
         a = rng.uniform(-b, b, size=(N, ora.A)).astype(np.float32)
         ora.step(a)
@@ -87,22 +85,12 @@ def _prepare(name, terrain, env=None, **extra):
     return ora, rng
 
 
-def _sync(env, ora):
-    """The GPU env's physical state and protection words := the oracle's."""
-    so = _oracle_state(ora, N)
-    env.set_state(so["pos"], so["quat"], so["linvel"], so["angvel"], so["q"], so["qd"])
-    _sync_motor_protection(env, ora, N)
-
-
 def _gpu_env(name, terrain, build, monkeypatch, **extra):
-    import rex_gym_b200 as R
-    if build == "sensor":
-        monkeypatch.delenv("REXSIM_FORCE_BUILD", raising=False)
+    force_build(monkeypatch, build)
+    if build == "sensor":                                      # the sensor build, with zero latencies
         extra.setdefault("observation_noise_stdev", NOISE)
-    else:
-        monkeypatch.setenv("REXSIM_FORCE_BUILD", build)
     task, kw = _okw(name, terrain, **extra)
-    return R.BatchedRexEnv(task=task, num_envs=N, **kw), extra
+    return make_env(task, N, **kw), extra
 
 
 # ---------------------------------------------------------------------------------------------------------------- CPU
@@ -116,10 +104,10 @@ def test_scenarios_switch_motors_off(terrain):
     for name in LEG_SCENARIOS + ARM_SCENARIOS:
         ora, rng = _prepare(name, terrain)
         task, sig = SCENARIOS[name][:2]
-        b = _bound(task, sig)
+        b = bound(task, sig)
         for k in range(15):
             ora.step(rng.uniform(-b, b, size=(N, ora.A)).astype(np.float32))
-        _, en = _oracle_protection(ora)
+        _, en = oracle_protection(ora)
         off = ~en
         assert not off[~SEEDED].any(), (name, np.nonzero(off[~SEEDED]))
         assert off.any(), name
@@ -153,20 +141,20 @@ def test_create_refuses_time_steps_the_counters_cannot_count():
 def test_oracle_switches_off_on_count_1023_at_the_largest_accepted_rate():
     """CPU: at 1 / dt = 1022.49 the oracle switches a motor off on its 1023rd consecutive hot sub-step -- the top value of the
     kernel's 10-bit field -- and standup's hold leaves 511 on the feet (it holds them hot for its last 0.5 s)."""
-    ora = _oracle("standup", 4, signal_type="ol", **EDGE)
+    ora = make_oracle("standup", 4, signal_type="ol", **EDGE)
     ora.reset()
-    cnt, en = _oracle_protection(ora)
+    cnt, en = oracle_protection(ora)
     assert (cnt[:, FEET] == 511).all() and en.all()
     for i, v in enumerate((1018, 1017, 1016, None)):           # 5 hot sub-steps per control step
         for m in FEET:
             if v is not None:
                 ora.env(i).overheat[m] = v
     ora.step(np.zeros((4, 1), np.float32))
-    cnt, en = _oracle_protection(ora)
+    cnt, en = oracle_protection(ora)
     assert (cnt[:, FEET] == [[1023], [1022], [1021], [516]]).all(), cnt[:, FEET]
     np.testing.assert_array_equal(en[:, FEET].all(1), [False, True, True, True])
     ora.step(np.zeros((4, 1), np.float32))
-    cnt, en = _oracle_protection(ora)
+    cnt, en = oracle_protection(ora)
     np.testing.assert_array_equal(en[:, FEET].any(1), [False, False, False, True])
 
 
@@ -182,8 +170,8 @@ EXACT_IDS = ["-".join(c) for c in EXACT_CONFIGS]
 
 def _assert_protection(env, ora, what, budget=0):
     """Enabled bits equal the oracle's; at most `budget` counters differ.  -> (counters, enabled, differing counters)."""
-    cnt, en = _motor_protection(env)
-    ocnt, oen = _oracle_protection(ora)
+    cnt, en = protection(env)
+    ocnt, oen = oracle_protection(ora)
     np.testing.assert_array_equal(en, oen, err_msg=f"enabled bits, {what}")
     bad = int((cnt != ocnt).sum())
     assert bad <= budget, (what, bad, np.argwhere(cnt != ocnt)[:8], cnt[cnt != ocnt][:8], ocnt[cnt != ocnt][:8])
@@ -208,20 +196,19 @@ def test_shutdown_on_the_exact_substep(monkeypatch, name, terrain, build):
     for i in np.nonzero(SEEDED)[0]:
         for m in motors:
             ora.env(i).overheat[m] = 1000 - (i % 5)
-    _sync(env, ora)
-    b = _bound(task, sig)
+    sync(env, ora, protection=True)
+    b = bound(task, sig)
     eq, ep, offs = [], [], []
     for k in range(8):
-        so = _oracle_state(ora, N)
-        env.set_state(so["pos"], so["quat"], so["linvel"], so["angvel"], so["q"], so["qd"])
+        sync(env, ora)
         a = rng.uniform(-b, b, size=(N, env.action_dim)).astype(np.float32)
         env.step(a)
-        assert _launched(env) == BUILDS[build], _launched(env)
+        assert launched(env) == BUILDS[build], launched(env)
         ora.step(a)
         _, en, _ = _assert_protection(env, ora, f"sub-step {k}")
         offs.append((~en).sum())
-        sg, s2 = env.get_state(), _oracle_state(ora, N)
-        eq.append(np.abs(sg["q"] - s2["q"]).max(1)); ep.append(np.abs(sg["pos"] - s2["pos"]).max(1))
+        q, p = state_errors(env, ora)
+        eq.append(q); ep.append(p)
     eq, ep = np.concatenate(eq), np.concatenate(ep)
     print("exact sub-step: motors off after each sub-step", offs, "q (p90, max)", np.percentile(eq, 90), eq.max(),
           "pos (p90, max)", np.percentile(ep, 90), ep.max())
@@ -247,13 +234,13 @@ def test_shutdowns_in_the_task_configuration(monkeypatch, name, terrain, build):
     env, extra = _gpu_env(name, terrain, build, monkeypatch)
     task, sig = SCENARIOS[name][:2]
     ora, rng = _prepare(name, terrain, env, **extra)
-    b = _bound(task, sig)
+    b = bound(task, sig)
     saturated = relieved = ties = 0
     for k in range(15):
-        _sync(env, ora)
+        sync(env, ora, protection=True)
         a = rng.uniform(-b, b, size=(N, env.action_dim)).astype(np.float32)
         _, _, dg, _ = env.step(a)
-        assert _launched(env) == BUILDS[build], _launched(env)
+        assert launched(env) == BUILDS[build], launched(env)
         _, _, dc = ora.step(a)
         np.testing.assert_array_equal(dg, dc, err_msg=f"done, step {k}")
         cnt, en, bad = _assert_protection(env, ora, f"step {k}", TIES - ties)
@@ -287,25 +274,25 @@ def test_edge_rate_switches_off_on_count_1023(monkeypatch, build):
     top of the 10-bit field -- on the last sub-step of the first control step and switch off there; feet seeded at 1017 / 1016 one
     and two sub-steps into the second.  After every step the GPU's enabled bits and counters equal the oracle's."""
     env, extra = _gpu_env("standup", "plane", build, monkeypatch, **EDGE)
-    ora = _oracle("standup", N, **_okw("standup", "plane", **extra)[1])
+    ora = make_oracle("standup", N, **_okw("standup", "plane", **extra)[1])
     env.reset(); ora.reset()
     _assert_protection(env, ora, "reset")
-    assert (_motor_protection(env)[0][:, FEET] == 511).all()
+    assert (protection(env)[0][:, FEET] == 511).all()
     for i in range(N):
         if i % 4 != 3:                                         # every fourth env unseeded
             for m in FEET:
                 ora.env(i).overheat[m] = 1016 + i % 3
-    _sync(env, ora)
+    sync(env, ora, protection=True)
     rng = np.random.default_rng(3)
     offs = []
     for k in range(4):
         a = rng.uniform(-0.1, 0.1, size=(N, 1)).astype(np.float32)
         env.step(a)
-        assert _launched(env) == BUILDS[build], _launched(env)
+        assert launched(env) == BUILDS[build], launched(env)
         ora.step(a)
         _, en, _ = _assert_protection(env, ora, f"step {k}")
         offs.append(int((~en[:, FEET]).any(1).sum()))
-        _sync(env, ora)                                        # the next step from the oracle's state (protection words included)
+        sync(env, ora, protection=True)                        # the next step from the oracle's state (protection words included)
     seeded = sum(i % 4 != 3 for i in range(N))
     assert offs == [sum(i % 4 != 3 and i % 3 == 2 for i in range(N))] + [seeded] * 3, offs
     env.close()
@@ -320,21 +307,20 @@ def test_reset_restores_the_snapshot_protection(monkeypatch, build):
     env, extra = _gpu_env("standup", "plane", build, monkeypatch, max_episode_steps=6, auto_reset=True)
     extra.pop("auto_reset")
     ora, rng = _prepare("standup", "plane", env, **extra)
-    b = _bound("standup", "ol")
+    b = bound("standup", "ol")
     half = np.arange(0, N, 2)
     for k in range(11):
         if k == 0:
-            _sync(env, ora)
+            sync(env, ora, protection=True)
         if k == 3:
-            before = _motor_protection(env)
+            before = protection(env)
             assert (~before[1]).any()
             env.reset(half); ora.reset(half)
             cnt, en, _ = _assert_protection(env, ora, "rexsim_reset")
             assert (cnt[half][:, FEET] == 500).all() and (np.delete(cnt[half], FEET, 1) == 0).all() and en[half].all()
             keep = np.setdiff1d(np.arange(N), half)
             np.testing.assert_array_equal(cnt[keep], before[0][keep]); np.testing.assert_array_equal(en[keep], before[1][keep])
-            so = _oracle_state(ora, N)                       # the reset envs restart from the oracle's settle (chaotic fold-down)
-            env.set_state(so["pos"], so["quat"], so["linvel"], so["angvel"], so["q"], so["qd"])
+            sync(env, ora)                                   # the reset envs restart from the oracle's settle (chaotic fold-down)
         a = rng.uniform(-b, b, size=(N, 1)).astype(np.float32)
         _, _, dg, _ = env.step(a)
         _, _, dc = ora.step(a)
@@ -346,8 +332,7 @@ def test_reset_restores_the_snapshot_protection(monkeypatch, build):
                 assert set(idx) >= set(np.setdiff1d(np.arange(N), half))       # the auto-reset half
             cnt, en, _ = _assert_protection(env, ora, f"auto-reset, step {k}")
             assert en[idx].all() and (cnt[idx][:, FEET] == 500).all()
-            so = _oracle_state(ora, N)
-            env.set_state(so["pos"], so["quat"], so["linvel"], so["angvel"], so["q"], so["qd"])
+            sync(env, ora)
         else:
             _assert_protection(env, ora, f"step {k}")
     assert (env.check_errors() & 1) == 0
@@ -365,18 +350,17 @@ def test_natural_counting(task, sig, kw):
     each step the counters and enabled bits equal the oracle's, except (env, motor, step) samples where the applied torque sits on
     the 2.45 N m threshold within the fp32 / fp64 difference (budgeted like contact masks at 0.1 %).  Measured on an H100: no sample
     of the 13 320 per task differs; turn-ik, standup-ol and gallop-ol have 580, 3010 and 2610 hot samples, walk-ik none."""
-    from test_gpu_parity import _env
-    env, ora = _env(task, N, signal_type=sig, seed=7, **kw), _oracle(task, N, signal_type=sig, seed=7, **kw)
+    env, ora = make_env(task, N, signal_type=sig, seed=7, **kw), make_oracle(task, N, signal_type=sig, seed=7, **kw)
     env.reset(); ora.reset()
     rng = np.random.default_rng(8)
-    b = _bound(task, sig)
+    b = bound(task, sig)
     bad = total = hot = 0
     for k in range(30):
-        _sync(env, ora)
+        sync(env, ora, protection=True)
         a = rng.uniform(-b, b, size=(N, env.action_dim)).astype(np.float32)
         env.step(a); ora.step(a)
-        cnt, en = _motor_protection(env)
-        ocnt, oen = _oracle_protection(ora)
+        cnt, en = protection(env)
+        ocnt, oen = oracle_protection(ora)
         np.testing.assert_array_equal(en, oen)
         bad += int((cnt != ocnt).sum()); total += cnt.size; hot += int((ocnt > 0).sum())
     print(f"natural counting {task}-{sig}: {bad} of {total} samples differ, {hot} hot")
@@ -390,23 +374,22 @@ def test_standup_shutdown_with_pd_latency():
     newest history rows.  Standup at reset, feet seeded at 996: 10 control steps, each from the oracle's physical state and
     protection words (the history ring is each side's own), enabled bits and counters equal the oracle's after every step, and
     every seeded foot is off at the end.  Measured on an H100: q p90 5.2e-7, max 2.1e-6 rad; bounded here at 2e-5."""
-    import rex_gym_b200 as R
     kw = dict(signal_type="ol", seed=31, pd_latency=0.0005)
-    env, ora = R.BatchedRexEnv(task="standup", num_envs=N, **kw), _oracle("standup", N, **kw)
+    env, ora = make_env("standup", N, **kw), make_oracle("standup", N, **kw)
     env.reset(); ora.reset()
     _seed(ora, "standup", [996 if s else None for s in SEEDED])
     rng = np.random.default_rng(4)
     eq = []
     for k in range(10):
-        _sync(env, ora)
+        sync(env, ora, protection=True)
         a = rng.uniform(-0.1, 0.1, size=(N, 1)).astype(np.float32)
         env.step(a)
-        assert _launched(env) == BUILDS["sensor"]
+        assert launched(env) == BUILDS["sensor"]
         ora.step(a)
         _assert_protection(env, ora, f"step {k}")
-        eq.append(np.abs(env.get_state()["q"] - _oracle_state(ora, N)["q"]).max(1))
+        eq.append(state_errors(env, ora)[0])
     eq = np.concatenate(eq)
     print("pd latency: q (p90, max)", np.percentile(eq, 90), eq.max())
     assert eq.max() < 2e-5, eq.max()
-    assert (~_motor_protection(env)[1][SEEDED][:, FEET]).all()
+    assert (~protection(env)[1][SEEDED][:, FEET]).all()
     env.close()

@@ -14,114 +14,29 @@ import numpy as np
 import pybullet_memory
 import pytest
 import torch
+from twin import (LAYOUT, NOISE, STATE_KEYS, TOL_P, TOL_Q, IterationBand, assert_draws, bound, make_env, make_oracle,
+                  one_step_is_tight, oracle_protection, protection, solver_cost, state_errors, sync, toe_masks)
 
 pytestmark = pytest.mark.gpu
-
-TOL_Q, TOL_P = 1e-3, 1e-3
-TOES = (2, 4, 6, 8)          # oracle contact-group ids of the four feet (foot box + toe hull)
-
-
-def _env(task="walk", n=8, **kw):
-    import rex_gym_b200 as R
-    return R.BatchedRexEnv(task=task, num_envs=n, **kw)
-
-
-def _oracle(task="walk", n=8, **kw):
-    from oracle.oracle import OracleSim
-    kw = dict(kw)
-    sig = kw.pop("signal_type", "ik")
-    ter = kw.pop("terrain_type", "plane")
-    nf = kw.pop("num_fields", 0)
-    kr, dr = kw.pop("motor_kp_range", None), kw.pop("motor_kd_range", None)
-    kw.pop("auto_reset", None)
-    return OracleSim(n, task, sig, terrain=ter, nfields=nf, kp_range=kr, kd_range=dr, **kw)
 
 
 # Base rates at the end of Rex.Reset's 0.6 s hold.  Two of the settled configurations still rock when the hold ends: the walk
 # with the arm (its three limit rows pressed by their motors) and field 3 of the heightfield bank used below (a robot creeping on
 # a slope).  There the sampled rate depends on which PGS iteration first meets the 1e-7 early-out, and a single fp64 oracle run
 # is one sample of a spread wider than the tolerance the other configurations keep: for those two only, the CUDA path is held
-# to the range the oracle spans over early-outs within 20 % of 1e-7 in its fp64 and fp32 builds, within 2e-3 rad/s.
-HOLD_THRESHOLDS = (0.8e-7, 0.9e-7, 1e-7, 1.1e-7, 1.2e-7)
-
-
+# to the range the oracle spans over early-outs within 20 % of 1e-7 (HOLD_THRESHOLDS) in its fp64 and fp32 builds, within
+# 2e-3 rad/s.
 def _hold_rate_band(task, n, cols, **kw):
     """-> (lo, hi, field ids): per env, the range of reset-observation columns `cols` over HOLD_THRESHOLDS x (fp64, fp32)."""
-    runs, fields = [], None
-    for thr in HOLD_THRESHOLDS:
-        for f32 in (False, True):
-            o = _oracle(task, n, residual_threshold=thr, f32=f32, **kw)
-            runs.append(o.reset()[:, cols])
-            fields = [o.env(i).field_id for i in range(n)]
-    return np.min(runs, 0), np.max(runs, 0), fields
+    oracles = IterationBand(lambda **b: make_oracle(task, n, **b, **kw)).oracles
+    runs = [o.reset()[:, cols] for o in oracles]
+    return np.min(runs, 0), np.max(runs, 0), [oracles[-1].env(i).field_id for i in range(n)]
 
 
 def _assert_in_band(g, lo, hi, tol):
     lo, hi = np.broadcast_to(lo, g.shape), np.broadcast_to(hi, g.shape)
     bad = (g < lo - tol) | (g > hi + tol)
     assert not bad.any(), ("outside the oracle's band", g[bad], lo[bad], hi[bad])
-
-
-def _oracle_state(o, n):
-    st = [o.state(i) for i in range(n)]
-    return {k: np.stack([s[k] for s in st]) for k in st[0]}
-
-
-# Packed overheat protection (rex.py:601-608) in the int SoA state: motor m's 10-bit saturating counter is field m % 3 of word
-# I_OVH + m // 3 for the legs (m < 12) and of word I_OVHA + (m - 12) // 3 for the arm; its enabled bit is bit 8 + m of I_FLAGS
-# (legs 8-19, arm 20-25).  The oracle counts in an int32 that goes on past 1023 while a switched-off motor stays hot.
-I_FLAGS, I_OVH, I_OVHA, FL_ENABLED_SHIFT = 2, 9, 14, 8
-
-
-def _protection_word(m):
-    return (I_OVH + m // 3) if m < 12 else (I_OVHA + (m - 12) // 3)
-
-
-def _sync_motor_protection(env, ora, n):
-    """Copy the oracle's overheat counters / motor-enabled bits (rex.py:601-608 state, arm included) into the raw SoA state:
-    the public set_state only carries the physical state, and a counter that is one sub-step off re-fires its event."""
-    si = env._state_i
-    host = si.cpu().numpy().astype(np.int64) & 0xFFFFFFFF
-    nm = ora.nm
-    mask = (1 << (FL_ENABLED_SHIFT + nm)) - (1 << FL_ENABLED_SHIFT)
-    for i in range(n):
-        e = ora.env(i)
-        en, words = 0, {}
-        for m in range(nm):
-            w = _protection_word(m)
-            words[w] = words.get(w, 0) | (min(int(e.overheat[m]), 1023) << (10 * (m % 3)))
-            en |= (1 if e.enabled[m] else 0) << (FL_ENABLED_SHIFT + m)
-        for w, v in words.items():
-            host[w, i] = v
-        host[I_FLAGS, i] = (host[I_FLAGS, i] & ~mask) | en
-    si.copy_(torch.from_numpy(host.astype(np.uint32).view(np.int32)).to(si.device))
-
-
-def _motor_protection(env, n=None):
-    """-> (counters [N][nm], enabled [N][nm] bool) read back from the raw SoA state of the first n envs."""
-    n = env.num_envs if n is None else n
-    si = env._state_i[:, :n].cpu().numpy().astype(np.int64) & 0xFFFFFFFF
-    nm = env.num_motors
-    cnt = np.stack([(si[_protection_word(m)] >> (10 * (m % 3))) & 1023 for m in range(nm)], 1)
-    en = np.stack([(si[I_FLAGS] >> (FL_ENABLED_SHIFT + m)) & 1 for m in range(nm)], 1).astype(bool)
-    return cnt, en
-
-
-def _oracle_protection(ora, n=None):
-    """-> the oracle's (min(counter, 1023) [N][nm], enabled [N][nm] bool): what the kernel's saturating fields must hold."""
-    n = ora.N if n is None else n
-    cnt = np.array([[min(int(ora.env(i).overheat[m]), 1023) for m in range(ora.nm)] for i in range(n)])
-    en = np.array([[bool(ora.env(i).enabled[m]) for m in range(ora.nm)] for i in range(n)])
-    return cnt, en
-
-
-def _toe_mask(o, i):
-    return o.env(i).contact_mask & 0x1FF       # 9 contact groups, same bit layout on both sides
-
-
-def _bound(task, sig):
-    from rex_gym_b200.envs.batched_env import ACTION_BOUND
-    return ACTION_BOUND[(task, sig)]
 
 
 CASES = [("walk", "ik", dict(target_position=2.0, backwards=False)),
@@ -157,9 +72,9 @@ def test_reset_settle_and_draws(task, sig, kw):
     """Rex.Reset's 600 settle sub-steps run on the GPU; task draws are bit-exact, and so are the overheat counters and
     motor-enabled bits the hold leaves (standup: its four foot motors are still hot when the hold ends)."""
     n = 16
-    env, ora = _env(task, n, signal_type=sig, seed=77, **kw), _oracle(task, n, signal_type=sig, seed=77, **kw)
+    env, ora = make_env(task, n, signal_type=sig, seed=77, **kw), make_oracle(task, n, signal_type=sig, seed=77, **kw)
     og, oc = env.reset(), ora.reset()
-    sg, so = env.get_state(), _oracle_state(ora, n)
+    sg, so = env.get_state(), ora.states()
     # standup settles by folding the legs onto the foot joint limits and dropping the base 15 cm: a violent transient
     tq, tp = (5e-3, 2e-3) if task == "standup" else ((2e-4, 2e-5) if kw.get("mark") == "arm" else (2e-5, 2e-6))
     if task == "standup" and kw.get("mark") == "arm":
@@ -178,19 +93,9 @@ def test_reset_settle_and_draws(task, sig, kw):
         np.testing.assert_allclose(og[:, 2:4], oc[:, 2:4], atol=1e-2 if kw.get("mark") == "arm" else 10 * tq)
     if og.shape[1] > 4:
         np.testing.assert_allclose(og[:, 4:], oc[:, 4:], atol=10 * tq)
-    sf, si = env._state_f.cpu().numpy(), env._state_i.cpu().numpy()
-    tp = np.array([ora.env(i).target_value if task == "poses" else ora.env(i).target_position for i in range(n)], np.float32)
-    np.testing.assert_array_equal(sf[38], tp)                                         # F_TARGET
-    if task == "poses":
-        np.testing.assert_array_equal((si[2] >> 26) & 7, [ora.env(i).next_pose for i in range(n)])   # FL_POSE_SHIFT
-    np.testing.assert_array_equal(sf[41], np.array([ora.env(i).kp for i in range(n)], np.float32))
-    np.testing.assert_array_equal(sf[42], np.array([ora.env(i).kd for i in range(n)], np.float32))
-    np.testing.assert_array_equal(si[3], [ora.env(i).reset_count for i in range(n)])  # I_RESETCNT
-    flags = si[2]
-    np.testing.assert_array_equal((flags >> 3) & 1, [ora.env(i).backwards for i in range(n)])
-    np.testing.assert_array_equal((flags >> 4) & 1, [ora.env(i).clockwise for i in range(n)])
-    cnt, en = _motor_protection(env)
-    ocnt, oen = _oracle_protection(ora)
+    assert_draws(env, ora, task)
+    cnt, en = protection(env)
+    ocnt, oen = oracle_protection(ora)
     np.testing.assert_array_equal(cnt, ocnt)
     np.testing.assert_array_equal(en, oen)
     assert en.all()
@@ -216,25 +121,24 @@ def test_free_running_rollout(task, sig, kw):
         steps = 150        # RexPosesEnv.reset does not settle: the 5 mm drop onto the feet is part of the episode (chaos starts earlier)
     if task == "gallop" and sig == "ik":
         steps = 110        # every env follows the same hopping trajectory (the action only shifts ramp timings): common-mode chaos
-    env, ora = _env(task, n, signal_type=sig, seed=3, **kw), _oracle(task, n, signal_type=sig, seed=3, **kw)
+    env, ora = make_env(task, n, signal_type=sig, seed=3, **kw), make_oracle(task, n, signal_type=sig, seed=3, **kw)
     env.reset(); ora.reset()
     if task == "standup" or kw.get("mark") == "arm":      # start both from the oracle's settled state (see test_reset_settle_and_draws)
-        so = _oracle_state(ora, n)
-        env.set_state(so["pos"], so["quat"], so["linvel"], so["angvel"], so["q"], so["qd"])
+        sync(env, ora)
     rng = np.random.default_rng(11)
-    b = _bound(task, sig)
+    b = bound(task, sig)
     alive = np.ones(n, bool)
     contact_total = contact_bad = 0
     for k in range(steps):
         a = rng.uniform(-b, b, size=(n, env.action_dim)).astype(np.float32)
         og, rg, dg, info = env.step(a)
         oc, rc, dc = ora.step(a)
-        sg, so = env.get_state(), _oracle_state(ora, n)
+        sg, so = env.get_state(), ora.states()
         cmp = alive.copy()
         if not cmp.any():
             break
-        eq = np.abs(sg["q"] - so["q"]).max(axis=1)[cmp]
-        ep = np.maximum(np.abs(sg["pos"] - so["pos"]).max(axis=1), np.abs(sg["quat"] - so["quat"]).max(axis=1))[cmp]
+        eq, ep = state_errors(env, ora)
+        eq, ep = eq[cmp], np.maximum(ep, np.abs(sg["quat"] - so["quat"]).max(axis=1))[cmp]
         if k < strict:
             # every env inside the tolerance, except isolated touchdown events: a foot landing one 1 ms sub-step earlier
             # on one side (fp32 vs fp64 height) gives a transient of a few mrad in that env; allow 10 % such envs, bounded
@@ -252,8 +156,7 @@ def test_free_running_rollout(task, sig, kw):
             assert np.median(eq) < 2 * tol_q and np.median(ep) < 2 * tol_p, f"step {k}"
             assert (eq < 2 * tol_q).mean() >= 0.6 and (ep < 2 * tol_p).mean() >= 0.6, f"step {k}"
         np.testing.assert_array_equal(sg["step_counter"], [ora.env(i).step_counter for i in range(n)])
-        cm = np.array([_toe_mask(ora, i) for i in range(n)])
-        contact_total += cmp.sum(); contact_bad += ((cm != sg["contact_mask"]) & cmp).sum()
+        contact_total += cmp.sum(); contact_bad += ((toe_masks(ora) != sg["contact_mask"]) & cmp).sum()
         alive &= ~(dg | dc)
         if not alive.any():
             break
@@ -271,25 +174,22 @@ def test_shadowing_1000_steps_walk():
     median 6e-7 rad, 90th percentile 4e-6, max 4e-4 rad."""
     n, steps, window = 8, 1000, 25
     kw = dict(target_position=3.0, backwards=True)         # the backwards gait walks for the whole horizon
-    env, ora = _env("walk", n, **kw), _oracle("walk", n, **kw)
+    env, ora = make_env("walk", n, **kw), make_oracle("walk", n, **kw)
     env.reset(); ora.reset()
     rng = np.random.default_rng(5)
     eqs, eps_, erp = [], [], []
     mism = tot = 0
     for k in range(steps):
         if k % window == 0:
-            so = _oracle_state(ora, n)
-            env.set_state(so["pos"], so["quat"], so["linvel"], so["angvel"], so["q"], so["qd"])
-            _sync_motor_protection(env, ora, n)
+            sync(env, ora, protection=True)
         a = rng.uniform(-0.4, 0.4, size=(n, 2)).astype(np.float32)
         og, rg, dg, _ = env.step(a)
         oc, rc, dc = ora.step(a)
         assert not dg.any() and not dc.any()
-        sg, so = env.get_state(), _oracle_state(ora, n)
-        eqs.append(np.abs(sg["q"] - so["q"]).max(axis=1)); eps_.append(np.abs(sg["pos"] - so["pos"]).max(axis=1))
+        eq, ep = state_errors(env, ora)
+        eqs.append(eq); eps_.append(ep)
         erp.append(np.abs(og[:, :2] - oc[:, :2]).max(axis=1))
-        cm = np.array([_toe_mask(ora, i) for i in range(n)])
-        mism += (cm != sg["contact_mask"]).sum(); tot += n
+        mism += (toe_masks(ora) != env.get_state()["contact_mask"]).sum(); tot += n
     eqs, eps_, erp = np.concatenate(eqs), np.concatenate(eps_), np.concatenate(erp)
     stats = [(np.percentile(e, 50), np.percentile(e, 90), e.max()) for e in (eqs, eps_, erp)]
     print("shadowing (median, p90, max) q/pos/roll-pitch:", stats)
@@ -312,28 +212,7 @@ def test_shadowing_1000_steps_walk():
 def test_one_step_is_tight(task, sig, kw, bound):
     """A single control step from a synchronised state agrees far below the rollout tolerance (standup exercises
     the joint-limit rows and the generic solver path from the first sub-step on)."""
-    n = 32
-    env, ora = _env(task, n, signal_type=sig, **kw), _oracle(task, n, signal_type=sig, **kw)
-    env.reset(); ora.reset()
-    rng = np.random.default_rng(2)
-    bad = 0
-    for k in range(30):
-        a = rng.uniform(-bound, bound, size=(n, env.action_dim)).astype(np.float32)
-        so = _oracle_state(ora, n)
-        env.set_state(so["pos"], so["quat"], so["linvel"], so["angvel"], so["q"], so["qd"])
-        env.step(a); ora.step(a)
-        sg, so = env.get_state(), _oracle_state(ora, n)
-        dq = np.abs(sg["q"] - so["q"]).max(axis=1)
-        # 5 sub-steps from identical states: rounding level, except envs where a discrete event (a contact or limit row
-        # switching on one sub-step apart) falls inside the step
-        # the arm's three limit rows sit exactly on their activation boundary (q hovers at the limit under the PD
-        # pull), so whether a row exists in a given sub-step is itself rounding-sensitive: 2e-3 there
-        t90 = 2e-3 if kw.get("mark") == "arm" else 2e-5
-        assert np.percentile(dq, 90) < t90 and dq.max() < 3e-3, (np.percentile(dq, 90), dq.max())
-        assert np.percentile(np.abs(sg["pos"] - so["pos"]).max(axis=1), 90) < (2e-4 if kw.get("mark") == "arm" else 2e-6)
-        bad += (sg["contact_mask"] != np.array([_toe_mask(ora, i) for i in range(n)])).sum()
-    assert bad <= 0.01 * 30 * n
-    env.close()
+    one_step_is_tight(task, sig, kw, bound)
 
 
 @pytest.mark.parametrize("in_air", [True, False])
@@ -344,11 +223,11 @@ def test_several_joint_limits_in_one_leg(in_air):
     foot contacts), and one control step is compared with the oracle."""
     n = 32
     kw = dict(target_position=2.0, backwards=False)
-    env, ora = _env("walk", n, **kw), _oracle("walk", n, **kw)
+    env, ora = make_env("walk", n, **kw), make_oracle("walk", n, **kw)
     env.reset(); ora.reset()
     rng = np.random.default_rng(3)
-    so = _oracle_state(ora, n)
-    q, qd, pos = so["q"].copy(), so["qd"].copy(), so["pos"].copy()
+    so = ora.states()
+    q, qd, pos = so["q"], so["qd"], so["pos"]
     for i in range(n):
         legs = rng.choice(4, size=1 + i % 3, replace=False)
         for l in legs:
@@ -360,29 +239,21 @@ def test_several_joint_limits_in_one_leg(in_air):
             qd[i, 3 * l:3 * l + 3] = rng.uniform(-1.0, 1.0, 3)
         if in_air:
             pos[i, 2] = 0.4
-    for i in range(n):                                 # the oracle has no set_state: write the struct
-        e = ora.env(i)
-        for j in range(12):
-            e.q[j], e.qd[j] = q[i, j], qd[i, j]
-        for a in range(3):
-            e.pos[a] = pos[i, a]
-    env.set_state(pos, so["quat"], so["linvel"], so["angvel"], q, qd)
+    for i in range(n):
+        ora.set_state(i, {k: v[i] for k, v in so.items()})
+    sync(env, ora)
     a = np.zeros((n, 2), np.float32)
     env.step(a); ora.step(a)
-    # the generic path ran (rexsim_solver_cost adds 64 per generic sub-step) exactly where a leg holds two or more violated limits
-    p = C.c_void_p()
-    assert env._L.rexsim_solver_cost(env._h, C.byref(p)) == 0
-    from rex_gym_b200.envs.batched_env import _DevArray
-    cost = torch.as_tensor(_DevArray(p.value, (n,), "<i4", env), device="cuda").cpu().numpy()
+    # the generic path ran (the solver cost adds 64 per generic sub-step) exactly where a leg holds two or more violated limits
+    cost = solver_cost(env)
     lo, hi = np.float32([-1.0, -2.17, -0.1]), np.float32([1.0, 0.97, 2.59])       # rex.urdf limits of shoulder, leg, foot
     qf = q.astype(np.float32).reshape(n, 4, 3)
     several = (((qf - lo) <= 0) | ((hi - qf) <= 0)).sum(2).max(1) >= 2
     np.testing.assert_array_equal(cost >= 64, several)
     assert several.all()                               # every env was given a leg with two or three violated limits
-    sg, s2 = env.get_state(), _oracle_state(ora, n)
-    dq = np.abs(sg["q"] - s2["q"]).max(axis=1)
+    dq, dp = state_errors(env, ora)
     assert np.percentile(dq, 90) < 5e-5 and dq.max() < 3e-3, (np.percentile(dq, 90), dq.max())
-    assert np.abs(sg["pos"] - s2["pos"]).max() < 2e-4
+    assert dp.max() < 2e-4
     assert (env.check_errors() & 3) == 0              # neither non-finite nor the (retired) joint-limit flag
     env.close()
 
@@ -390,23 +261,21 @@ def test_several_joint_limits_in_one_leg(in_air):
 def test_heightfield_contact_parity():
     n = 16
     kw = dict(signal_type="ik", terrain_type="random", num_fields=4, seed=9)
-    env, ora = _env("turn", n, **kw), _oracle("turn", n, **kw)
+    env, ora = make_env("turn", n, **kw), make_oracle("turn", n, **kw)
     env.reset(); ora.reset()
-    np.testing.assert_array_equal(env._state_i.cpu().numpy()[4], [ora.env(i).field_id for i in range(n)])
-    sg, so = env.get_state(), _oracle_state(ora, n)
-    assert np.abs(sg["q"] - so["q"]).max() < 5e-3          # settle on bumps: toes creep on the 45-degree block edges
-    env.set_state(so["pos"], so["quat"], so["linvel"], so["angvel"], so["q"], so["qd"])
+    assert_draws(env, ora, "turn")
+    assert state_errors(env, ora)[0].max() < 5e-3          # settle on bumps: toes creep on the 45-degree block edges
+    sync(env, ora)
     rng = np.random.default_rng(1)
     bad = 0
     for k in range(60):
         a = rng.uniform(-0.01, 0.01, size=(n, 2)).astype(np.float32)
         env.step(a); ora.step(a)
-        sg, so = env.get_state(), _oracle_state(ora, n)
         # a toe vertex handing over to its neighbour across a crease of the field happens a sub-step apart in fp32 and fp64:
         # 90 % of the envs inside the north-star tolerance at every step, the rest bounded
-        eq, ep = np.abs(sg["q"] - so["q"]).max(1), np.abs(sg["pos"] - so["pos"]).max(1)
+        eq, ep = state_errors(env, ora)
         assert np.percentile(eq, 90) < TOL_Q and np.percentile(ep, 90) < TOL_P and eq.max() < 2e-2 and ep.max() < 5e-3, f"step {k}: {eq.max():.2e}"
-        bad += (np.array([_toe_mask(ora, i) for i in range(n)]) != sg["contact_mask"]).sum()
+        bad += (toe_masks(ora) != env.get_state()["contact_mask"]).sum()
     assert bad <= 0.02 * 60 * n and env.check_errors() == 0
     env.close()
 
@@ -415,7 +284,7 @@ def test_wrappers_autoreset_and_limit():
     """ClipAction + RangeNormalize + LimitDuration fused (wrappers.py:183-291) and the in-kernel auto-reset."""
     n = 64
     kw = dict(target_position=2.0, backwards=False, normalize=True, max_episode_steps=7)
-    env, ora = _env("walk", n, auto_reset=True, **kw), _oracle("walk", n, **kw)
+    env, ora = make_env("walk", n, auto_reset=True, **kw), make_oracle("walk", n, **kw)
     o0 = env.reset(); ora.reset()
     assert np.abs(o0).max() <= 1.0
     rng = np.random.default_rng(0)
@@ -436,7 +305,7 @@ def test_wrappers_autoreset_and_limit():
 
 
 def test_error_behaviour_matches_the_reference():
-    env = _env("walk", 4, target_position=2.0, backwards=False)
+    env = make_env("walk", 4, target_position=2.0, backwards=False)
     env.reset()
     with pytest.raises(ValueError):
         env.step(np.zeros((4, 3), np.float32))               # batch_env.py:77-79 Invalid action
@@ -466,7 +335,7 @@ def test_numpy_and_device_paths_agree_beyond_the_zero_copy_limit():
 def _numpy_and_device_paths_agree(n):
     """numpy in / numpy out (rexsim_step_host) and CUDA tensors in / out give bit-identical results; state_dict round trip."""
     kw = dict(target_position=2.0, backwards=False, seed=5, auto_reset=True, max_episode_steps=50)
-    e1, e2 = _env("walk", n, **kw), _env("walk", n, **kw)
+    e1, e2 = make_env("walk", n, **kw), make_env("walk", n, **kw)
     e1.reset(); e2.reset()
     g = torch.Generator(device="cuda"); g.manual_seed(0)
     acts = (torch.rand((80, n, 2), device="cuda", generator=g) * 2 - 1) * 0.4
@@ -491,7 +360,7 @@ def test_full_size_properties_65536():
     (3) the result is finite and no unsupported-condition flag fires on flat ground."""
     N = 65536
     kw = dict(target_position=2.0, backwards=False, normalize=True, max_episode_steps=2000, auto_reset=True, seed=42)
-    big = _env("walk", N, **kw)
+    big = make_env("walk", N, **kw)
     big.reset()
     g = torch.Generator(device="cuda"); g.manual_seed(1)
     row = torch.rand((40, 1, 2), device="cuda", generator=g) * 2 - 1
@@ -502,9 +371,9 @@ def test_full_size_properties_65536():
     assert big.check_errors() == 0
     big.close()
     kw2 = dict(normalize=True, max_episode_steps=30, auto_reset=True, seed=42)      # random targets / directions
-    big = _env("walk", N, **kw2)
+    big = make_env("walk", N, **kw2)
     off, ns = 32768, 32768      # same kernel variant on both sides (the 255- and 128-register builds round differently)
-    shard = _env("walk", ns, env_offset=off, **kw2)
+    shard = make_env("walk", ns, env_offset=off, **kw2)
     big.reset(); shard.reset()
     acts = torch.rand((45, N, 2), device="cuda", generator=g) * 2 - 1
     for k in range(45):
@@ -528,22 +397,18 @@ def test_baseline_size_batches_against_the_oracle(name, task, n, kw):
     (tests/test_gpu_builds.py covers the rest)."""
     w0, nw, steps = n // 2 + 37, 48, 40
     common = dict(normalize=True, seed=11)
-    env = _env(task, n, **common, **kw)
-    ora = _oracle(task, nw, env_offset=w0, **common, **kw)
+    env = make_env(task, n, **common, **kw)
+    ora = make_oracle(task, nw, env_offset=w0, **common, **kw)
     og = env.reset()[w0:w0 + nw]
     oc = ora.reset()
     rough, arm = kw.get("terrain_type") == "random", kw.get("mark") == "arm"
     np.testing.assert_allclose(og[:, :2], oc[:, :2], atol=2e-5 if not (rough or arm) else 2e-4)      # RangeNormalize'd roll / pitch
-    sf = env._state_f.cpu().numpy()[:, w0:w0 + nw]
-    np.testing.assert_array_equal(sf[38], np.array([ora.env(i).target_position for i in range(nw)], np.float32))
-    np.testing.assert_array_equal(sf[41], np.array([ora.env(i).kp for i in range(nw)], np.float32))
-    np.testing.assert_array_equal(sf[39], np.array([ora.env(i).target_orient for i in range(nw)], np.float32))
+    assert_draws(env, ora, task, window=w0)
     if arm:            # start both from the oracle's settled state (chaotic fold-down, see test_reset_settle_and_draws)
-        st = env.get_state()
-        so = _oracle_state(ora, nw)
-        for k in ("pos", "quat", "linvel", "angvel", "q", "qd"):
+        st, so = env.get_state(), ora.states()
+        for k in STATE_KEYS:
             st[k][w0:w0 + nw] = so[k]
-        env.set_state(st["pos"], st["quat"], st["linvel"], st["angvel"], st["q"], st["qd"])
+        env.set_state(*(st[k] for k in STATE_KEYS))
     g = torch.Generator(device="cuda"); g.manual_seed(5)
     acts = torch.rand((steps, n, env.action_dim), device="cuda", generator=g) * 2 - 1
     err = []
@@ -600,7 +465,7 @@ def test_cuda_path_tracks_pybullet_goldens(task):
     n, steps = 25, 600
     ac, ref = G[task + "_ol_action"][:n], denorm(G[task + "_ol_observ"][:n])
     kw = dict(target_position=3.0) if task == "gallop" else dict(target_position=3.0, backwards=False)
-    env = _env(task, n, signal_type="ol", normalize=True, **kw)
+    env = make_env(task, n, signal_type="ol", normalize=True, **kw)
     env.reset()
     ol = np.array([0.15192765, -0.90412283, 1.48156545])
     q0 = np.tile(np.concatenate([ol * [s, 1, 1] for s in (1, -1, 1, -1)]), (n, 1))
@@ -640,7 +505,7 @@ def test_cuda_standup_hop_tracks_pybullet_goldens():
     ua = 2 * math.pi + 0.01
     n, steps = 25, 30
     ac, ref, rw = G["standup_ol_action"][:n], G["standup_ol_observ"][:n].astype(np.float64) * ua, G["standup_ol_reward"][:n]
-    env = _env("standup", n, signal_type="ol", normalize=True)
+    env = make_env("standup", n, signal_type="ol", normalize=True)
     env.reset()
     st = env.get_state()
     assert 2.62 < st["q"][0, 2] < 2.80 and 2.62 < st["q"][0, 8] < 2.80 and -0.09 < st["angvel"][0, 1] < -0.02
@@ -663,7 +528,7 @@ def test_walk_ik_reaches_its_target_at_the_readme_demo_clock():
     seconds per simulated second; 4.0 here): 32 envs, half zero and half random actions, forward to the 2 m target without a
     single `done`, every env latching its goal at |x| >= 1.85 and braking to a stop (walk_env.py:207-290, rex_gym_env.py:490-495)."""
     n = 32
-    env = _env("walk", n, signal_type="ik", target_position=2.0, backwards=False, gait_clock_scale=4.0)
+    env = make_env("walk", n, signal_type="ik", target_position=2.0, backwards=False, gait_clock_scale=4.0)
     env.reset()
     rng = np.random.default_rng(5)
     done_any = np.zeros(n, bool)
@@ -692,7 +557,7 @@ def test_batches_that_do_not_fill_their_last_warp(n):
     short episodes exercise reset bookkeeping (reset counter, field id, gains) on exactly those lanes; everything integer is
     compared bit-exactly with the oracle after every step."""
     kw = dict(signal_type="ik", terrain_type="random", num_fields=4, seed=9, max_episode_steps=7)
-    env, ora = _env("walk", n, auto_reset=True, **kw), _oracle("walk", n, **kw)
+    env, ora = make_env("walk", n, auto_reset=True, **kw), make_oracle("walk", n, **kw)
     og, oc = env.reset(), ora.reset()
     # settled angles agree to 1e-4; the residual base rates of a robot still creeping on a slope of the field are only as exact
     # as the solver's 1e-7 (squared) early-out: 2e-2 rad/s -- except on ROCKING_FIELD, which still rocks when the hold ends (see
@@ -713,9 +578,7 @@ def test_batches_that_do_not_fill_their_last_warp(n):
         idx = np.nonzero(dc)[0]
         if len(idx):
             oc[idx] = ora.reset(idx)                   # the oracle has no auto-reset: same semantics by hand
-        si = env._state_i.cpu().numpy()
-        np.testing.assert_array_equal(si[3], [ora.env(i).reset_count for i in range(n)])      # I_RESETCNT
-        np.testing.assert_array_equal(si[4], [ora.env(i).field_id for i in range(n)])         # I_FIELD
+        assert_draws(env, ora, "walk")
         np.testing.assert_allclose(o[:, :2], oc[:, :2], atol=2e-3)          # roll, pitch
         np.testing.assert_allclose(o[:, 2:], oc[:, 2:], atol=0.3)           # base angular rates on heightfield contact: chaotic at the 0.1 rad/s level
     rs, rso = env.reset(np.array([n - 1])), ora.reset(np.array([n - 1]))
@@ -724,12 +587,11 @@ def test_batches_that_do_not_fill_their_last_warp(n):
         _assert_in_band(rs[:, 2:], rock_lo, rock_hi, 2e-3)
     else:
         np.testing.assert_allclose(rs[:, 2:], rso[:, 2:], atol=2e-2)
-    assert int(env._state_i[3, n - 1]) == ora.env(n - 1).reset_count
+    assert int(env._state_i[LAYOUT.I_RESETCNT, n - 1]) == ora.env(n - 1).reset_count
     env.check_errors()
     env.close()
 
 
-NOISE = (0.01, 0.05, 0.1, 0.02, 0.1)       # motor angle, motor velocity, motor torque, base rpy, base rpy rate (SENSOR_NOISE_STDDEV order)
 # PD latencies: half a sub-step (a blend of the two newest rows).  From 1 ms on the delayed kp = 1 / kd = 0.02 loop rings
 # (walk-ik: 1e-6 agreement for 25 steps at 1 ms, chaotic from the reset hold on at 3 ms -- tools/dev_sensor.py), which leaves
 # nothing to compare; the history indexing itself is exercised by the control latencies (12.5 / 20 / 30 / 105 sub-steps back).
@@ -748,17 +610,16 @@ def test_sensor_latency_and_noise(task, sig, n, kw):
     Gaussian noise.  The kernel keeps the history as a ring in HBM; compared with the oracle (itself pinned to goldens generated
     from rex.py, tests/test_sensor_golden.py) over the reset observation and 40 control steps incl. auto-resets."""
     steps = 40
-    env, ora = _env(task, n, signal_type=sig, seed=5, **kw), _oracle(task, n, signal_type=sig, seed=5, **kw)
+    env, ora = make_env(task, n, signal_type=sig, seed=5, **kw), make_oracle(task, n, signal_type=sig, seed=5, **kw)
     og, oc = env.reset(), ora.reset()
     rough = kw.get("terrain_type") == "random"      # field 3 of the bank leaves the robot creeping down a slope after the hold
     rate_tol = 3e-2 if rough else (5e-3 if task == "standup" else 5e-4)
     np.testing.assert_allclose(og[:, :2], oc[:, :2], atol=5e-4 if task == "standup" else 2e-4)
     np.testing.assert_allclose(og[:, 2:4], oc[:, 2:4], atol=rate_tol)
     if task == "standup":
-        so = _oracle_state(ora, n)        # chaotic fold-down during the settle (test_reset_settle_and_draws): start from the oracle's
-        env.set_state(so["pos"], so["quat"], so["linvel"], so["angvel"], so["q"], so["qd"])
+        sync(env, ora)        # chaotic fold-down during the settle (test_reset_settle_and_draws): start from the oracle's
     rng = np.random.default_rng(4)
-    b = _bound(task, sig)
+    b = bound(task, sig)
     e_ang, e_rate, e_rew = [], [], []
     for k in range(steps):
         a = rng.uniform(-b, b, size=(n, env.action_dim)).astype(np.float32)
@@ -790,7 +651,7 @@ def test_checkpoint_resume_is_exact_with_the_sensor_model():
     """state_dict() carries the SoA state and, with the sensor model on, the history ring: a batch restored into a fresh handle
     continues bit for bit (the reference never checkpoints env state, SURVEY section 5)."""
     kw = dict(target_position=2.0, backwards=False, control_latency=0.012, observation_noise_stdev=NOISE, auto_reset=True, max_episode_steps=25, seed=3)
-    a, b = _env("walk", 64, **kw), _env("walk", 64, **kw)
+    a, b = make_env("walk", 64, **kw), make_env("walk", 64, **kw)
     a.reset(); b.reset()
     g = torch.Generator(device="cuda"); g.manual_seed(2)
     acts = torch.rand((40, 64, 2), device="cuda", generator=g) * 0.8 - 0.4
@@ -807,18 +668,18 @@ def test_checkpoint_resume_is_exact_with_the_sensor_model():
 def test_sensor_model_off_is_the_reference_default():
     """control_latency = pd_latency = 0 and zero noise (rex_gym_env.py:61,70-71 defaults): no history is allocated and the kernels
     read the true state -- the same launches as before the sensor model existed."""
-    env = _env("walk", 64, target_position=2.0, backwards=False)
+    env = make_env("walk", 64, target_position=2.0, backwards=False)
     assert env._L.rexsim_history_depth(C.byref(env._cfg)) == 0
     env.close()
     with pytest.raises(ValueError):
-        _env("walk", 8, control_latency=-0.01)
+        make_env("walk", 8, control_latency=-0.01)
 
 
 def test_error_flags_are_per_step_and_reset_indices_are_validated():
     """ADVICE r1: (a) a non-finite event raises for the step it happens in, not for the life of the handle
     (ConvertTo32Bit, wrappers.py:522-523,542-543); (b) a reset index outside the batch never touches state."""
     n = 8
-    env = _env("walk", n, signal_type="ik", target_position=2.0, backwards=False, auto_reset=True)
+    env = make_env("walk", n, signal_type="ik", target_position=2.0, backwards=False, auto_reset=True)
     env.reset()
     a = np.zeros((n, 2), np.float32)
     env.step(a)
@@ -835,9 +696,9 @@ def test_error_flags_are_per_step_and_reset_indices_are_validated():
     env.reset(idx)
     with pytest.raises(IndexError):
         env.check_errors()
-    after = env._state_i
-    assert int(after[3, 2]) == int(before[3, 2]) + 1                       # the valid index was reset once
-    assert torch.equal(after[3, [0, 1, 3, 4, 5, 6, 7]], before[3, [0, 1, 3, 4, 5, 6, 7]])
+    after, rc = env._state_i, LAYOUT.I_RESETCNT
+    assert int(after[rc, 2]) == int(before[rc, 2]) + 1                     # the valid index was reset once
+    assert torch.equal(after[rc, [0, 1, 3, 4, 5, 6, 7]], before[rc, [0, 1, 3, 4, 5, 6, 7]])
     assert env.check_errors() == 0
     with pytest.raises(IndexError):
         env.reset(np.array([n]))
@@ -858,7 +719,7 @@ def test_warp_regrouping_does_not_change_any_result_on_the_128_register_build():
 
 def _regrouping_is_bit_identical(n):
     kw = dict(signal_type="ik", normalize=True, auto_reset=True, max_episode_steps=60, seed=21)
-    a, b = _env("walk", n, rebalance_every=1, **kw), _env("walk", n, rebalance_every=0, **kw)
+    a, b = make_env("walk", n, rebalance_every=1, **kw), make_env("walk", n, rebalance_every=0, **kw)
     a.reset(); b.reset()
     gen = torch.Generator(device="cuda").manual_seed(3)
     for k in range(90):

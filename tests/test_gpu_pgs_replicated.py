@@ -8,14 +8,9 @@ walk-ik and turn-ik already agreed bit for bit between the two builds before the
 on everything a step writes: obs, reward, done, the whole SoA state and the per-env solver cost (PGS iterations), which also pins
 that both loops leave at the same iteration.
 """
-import ctypes
-
 import pytest
 import torch
-
-from rex_gym_b200.envs.batched_env import _DevArray
-from test_gpu_builds import _launched
-from test_gpu_parity import _env
+from twin import BUILDS, force_build, launched, make_env, solver_cost
 
 CASES = [  # (envs, solver_iterations): None = the task's default, int(300 / action_repeat)
     (8449, None),      # 265 CTAs of the small build: more than one wave, one env in the last CTA
@@ -25,19 +20,13 @@ CASES = [  # (envs, solver_iterations): None = the task's default, int(300 / act
 ]
 
 
-def _cost(env):
-    p = ctypes.c_void_p()
-    assert env._L.rexsim_solver_cost(env._h, ctypes.byref(p)) == 0
-    return torch.as_tensor(_DevArray(p.value, (env.num_envs,), "<i4", env), device="cuda").clone()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("n,iters", CASES, ids=["n8449", "n1003", "n1003-iters1", "n1003-iters60"])
 @pytest.mark.parametrize("task", ["walk", "turn"])
 def test_replicated_and_shuffle_solvers_agree_bit_for_bit(monkeypatch, task, n, iters):
     """60 auto-resetting control steps with episode phases staggered by partial resets; the two builds alternate step by step."""
     kw = dict(signal_type="ik", normalize=True, auto_reset=True, max_episode_steps=25, seed=17, solver_iterations=iters)
-    envs = {b: _env(task, n, **kw) for b in ("small", "big")}
+    envs = {b: make_env(task, n, **kw) for b in ("small", "big")}
     for e in envs.values():
         e.reset()
     gen = torch.Generator(device="cuda").manual_seed(5)
@@ -50,9 +39,9 @@ def test_replicated_and_shuffle_solvers_agree_bit_for_bit(monkeypatch, task, n, 
                 e.reset(idx)
         out = {}
         for b, e in envs.items():
-            monkeypatch.setenv("REXSIM_FORCE_BUILD", b)
-            out[b] = [t.clone() for t in e.step(act)[:3]] + [_cost(e), e._state_f.clone(), e._state_i.clone()]
-        assert _launched(envs["small"]) == (128, 1, 0) and _launched(envs["big"]) == (256, 4, 0)
+            force_build(monkeypatch, b)
+            out[b] = [t.clone() for t in e.step(act)[:3]] + [torch.from_numpy(solver_cost(e)), e._state_f.clone(), e._state_i.clone()]
+        assert launched(envs["small"]) == BUILDS["small"] and launched(envs["big"]) == BUILDS["big"]
         for name, x, y in zip(("obs", "reward", "done", "cost", "state_f", "state_i"), out["small"], out["big"]):
             assert torch.equal(x, y), f"{name} differs at step {k}"
         iterations.update(out["small"][3].unique().tolist())

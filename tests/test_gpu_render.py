@@ -2,10 +2,9 @@
 independent of the other images of a call, free of side effects, index checks."""
 import numpy as np
 import pytest
+from twin import LAYOUT
 
 pytestmark = pytest.mark.gpu
-
-I_FIELD = 4     # int state word of the env's heightfield (rexsim_kernel.cuh)
 
 
 def assert_frames_match(got, ref, ids, what=""):
@@ -30,7 +29,7 @@ def oracle_frame(env, i, width=480, height=360, distance=1.0, yaw=0.0, pitch=-30
     st = st or env.get_state()
     heights = None
     if env.terrain_type == "random":
-        field = int(env.state_dict()["state_i"][I_FIELD, i].item())
+        field = int(env.state_dict()["state_i"][LAYOUT.I_FIELD, i].item())
         heights = env._fields[field].cpu().numpy().reshape(256, 256)
     return RO.render(env.mark, st["pos"][i].astype(np.float64), st["quat"][i].astype(np.float64), st["q"][i].astype(np.float64),
                      width, height, distance, yaw, pitch, env.terrain_type, heights, draw_robot=draw_robot)

@@ -9,7 +9,7 @@ big build, warp re-grouping on) once per library, each library in its own proces
 obs, reward, done, last_command, the error words, the whole SoA state and the sensor ring; then bench.py --dump-outputs.
 Random actions from reset rarely reach the generic solver path, so every configuration of tests/test_gpu_generic_path.CONFIGS
 also runs from that test's start states (body, arm and multi-limit contacts): 4 single sub-steps, then 4 control steps of the
-task configuration, hashing rexsim_solver_cost as well.  Last, render_batch frames of a few envs of walk-ik on flat ground,
+task configuration, hashing the solver cost as well.  Last, render_batch frames of a few envs of walk-ik on flat ground,
 turn-ik on the random heightfields and standup with the arm, with the default camera and at 97 x 61.
 Every later library is compared with the first: each array that is not bit-identical is reported, and for a frame the number
 of pixels that differ."""
@@ -42,10 +42,9 @@ def digest(a):
 
 
 def _force_build(build):
-    if build:
-        os.environ["REXSIM_FORCE_BUILD"] = build
-    else:
-        os.environ.pop("REXSIM_FORCE_BUILD", None)
+    import pytest
+    import twin
+    twin.force_build(pytest.MonkeyPatch(), build)
 
 
 def _record(env, rec, k, ret, cost=False):
@@ -57,24 +56,21 @@ def _record(env, rec, k, ret, cost=False):
     for name, v in arrs.items():
         rec[f"{k:02d}_{name}"] = digest(v if isinstance(v, np.ndarray) else v.cpu().numpy())
     if cost:
-        import test_gpu_generic_path as G
-        rec[f"{k:02d}_cost"] = digest(G._cost(env))
+        import twin
+        rec[f"{k:02d}_cost"] = digest(twin.solver_cost(env))
 
 
-def generic_cases(R, res):
+def generic_cases(res):
     """tests/test_gpu_generic_path start states, every CONFIGS entry: single sub-steps, then control steps."""
     import test_gpu_generic_path as G
+    import twin
     for mark, terrain, build in G.CONFIGS:
         ids, st = G._batch(mark, terrain)
         for sub, steps in ((True, 4), (False, 4)):
-            _force_build(None if build == "sensor" else build)
-            kw = dict(G.SUB) if sub else {}
-            if build == "sensor":
-                kw["observation_noise_stdev"] = G.NOISE
-            env = R.BatchedRexEnv(task="walk", num_envs=G.N, signal_type="ik", terrain_type=terrain, num_fields=4, mark=mark,
-                                  seed=21, target_position=2.0, backwards=False, **kw)
+            _force_build(build)
+            env = twin.make_env("walk", G.N, **G._kw(mark, terrain, sub, build))
             env.reset()
-            G._set(env, st)
+            env.set_state(*(st[k] for k in twin.STATE_KEYS))
             rng = np.random.default_rng(7)
             rec = res[f"generic-{mark}-{terrain}-{build}-{'substep' if sub else 'control'}"] = {}
             for k in range(steps):
@@ -120,7 +116,7 @@ def run(out):
             ret = env.step(torch.as_tensor(rng.uniform(-b, b, size=(n, env.action_dim)).astype(np.float32), device="cuda"))
             _record(env, rec, k, ret)
         env.close()
-    generic_cases(R, res)
+    generic_cases(res)
     frames = {}
     render_cases(R, res, frames)
     with open(out, "w") as f:
