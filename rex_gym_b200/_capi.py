@@ -3,6 +3,8 @@ missing or CUDA is unavailable the product path raises."""
 import ctypes as C
 import os
 
+import torch
+
 from . import build as _build
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -33,15 +35,61 @@ class RexAgentConfig(C.Structure):
                 ("observ_clip", C.c_float), ("reward_clip", C.c_float)]
 
 
-AGENT_EXPORTS = ["rexagent_policy_floats", "rexagent_value_floats", "rexagent_create", "rexagent_destroy", "rexagent_set_precision", "rexagent_set_params",
-                 "rexagent_get_params", "rexagent_params_buffer", "rexagent_state_buffers", "rexagent_set_filters", "rexagent_get_filters",
-                 "rexagent_perform", "rexagent_experience", "rexagent_experience_partial", "rexagent_experience_finalize", "rexagent_transform_reward", "rexagent_discounted_return",
-                 "rexagent_lambda_advantage", "rexagent_gae_segments", "rexagent_launch_count"]
+_i32, _i64, _u32, _u64, _f32, _ptr = C.c_int32, C.c_int64, C.c_uint32, C.c_uint64, C.c_float, C.c_void_p
+_out, _sim_cfg, _agent_cfg = C.POINTER, C.POINTER(RexSimConfig), C.POINTER(RexAgentConfig)
 
-EXPORTS = ["rexsim_obs_dim", "rexsim_action_dim", "rexsim_state_words", "rexsim_create", "rexsim_destroy",
-           "rexsim_step", "rexsim_step_host", "rexsim_host_out_bytes", "rexsim_rebalance", "rexsim_reset", "rexsim_get_state", "rexsim_set_state", "rexsim_state_buffers",
-           "rexsim_error_flags", "rexsim_clear_errors", "rexsim_last_command", "rexsim_solver_cost", "rexsim_launch_count", "rexsim_last_step_build", "rexsim_last_error", "rexsim_rand_u32",
-           "rexsim_noise", "rexsim_history_depth", "rexsim_history_buffer", "rexsim_set_render_tables", "rexsim_render"]
+# name: (restype, argtypes) of every function of include/rexsim.h and include/rexsim_agent.h.  load() declares exactly these,
+# and the export lists below are its keys: a function ctypes has no signature for would get C ints and truncated pointers.
+SIGNATURES = {
+    "rexsim_obs_dim": (C.c_int, [_i32, _i32]),
+    "rexsim_action_dim": (C.c_int, [_i32, _i32]),
+    "rexsim_state_words": (C.c_int, [_sim_cfg, _out(_i32), _out(_i32)]),
+    "rexsim_create": (C.c_int, [_sim_cfg, _ptr, _i32, _out(_ptr)]),
+    "rexsim_destroy": (None, [_ptr]),
+    "rexsim_step": (C.c_int, [_ptr] * 6),
+    "rexsim_step_host": (C.c_int, [_ptr] * 4),
+    "rexsim_host_out_bytes": (_i64, [_ptr]),
+    "rexsim_rebalance": (C.c_int, [_ptr, _ptr]),
+    "rexsim_reset": (C.c_int, [_ptr, _ptr, _i32, _ptr, _ptr]),
+    "rexsim_get_state": (C.c_int, [_ptr] * 4),
+    "rexsim_set_state": (C.c_int, [_ptr] * 3),
+    "rexsim_state_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_ptr)]),
+    "rexsim_error_flags": (C.c_int, [_ptr, _out(_ptr)]),
+    "rexsim_clear_errors": (C.c_int, [_ptr, _ptr]),
+    "rexsim_last_command": (C.c_int, [_ptr, _out(_ptr)]),
+    "rexsim_solver_cost": (C.c_int, [_ptr, _out(_ptr)]),
+    "rexsim_launch_count": (_i64, [_ptr]),
+    "rexsim_last_step_build": (C.c_int, [_ptr] + [_out(_i32)] * 3),
+    "rexsim_last_error": (C.c_char_p, []),
+    "rexsim_rand_u32": (_u32, [_u64, _u32, _u32, _u32]),
+    "rexsim_noise": (_f32, [_u64] + [_u32] * 5),
+    "rexsim_history_depth": (C.c_int, [_sim_cfg]),
+    "rexsim_history_buffer": (C.c_int, [_ptr, _out(_ptr), _out(_i64)]),
+    "rexsim_set_render_tables": (C.c_int, [_ptr, _ptr, _i32]),
+    "rexsim_render": (C.c_int, [_ptr, _ptr, _i32, _i32, _i32, _f32, _f32, _f32, _ptr, _ptr]),
+    "rexagent_policy_floats": (_i64, [_agent_cfg]),
+    "rexagent_value_floats": (_i64, [_agent_cfg]),
+    "rexagent_create": (C.c_int, [_agent_cfg, _out(_ptr)]),
+    "rexagent_destroy": (None, [_ptr]),
+    "rexagent_set_precision": (C.c_int, [_ptr, _i32]),
+    "rexagent_set_params": (C.c_int, [_ptr, _ptr, _i64]),
+    "rexagent_get_params": (C.c_int, [_ptr, _ptr, _i64]),
+    "rexagent_params_buffer": (C.c_int, [_ptr, _out(_ptr)]),
+    "rexagent_state_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_ptr)]),
+    "rexagent_set_filters": (C.c_int, [_ptr, _i64, _ptr, _ptr, _i64, _f32, _f32]),
+    "rexagent_get_filters": (C.c_int, [_ptr] * 5),
+    "rexagent_perform": (C.c_int, [_ptr, _ptr, _i32, _i32, _u64, _u32, _u32] + [_ptr] * 6),
+    "rexagent_experience": (C.c_int, [_ptr, _ptr, _ptr, _i32, _ptr]),
+    "rexagent_experience_partial": (C.c_int, [_ptr, _ptr, _ptr, _i32, _ptr, _ptr]),
+    "rexagent_experience_finalize": (C.c_int, [_ptr, _ptr, _i32, _ptr, _ptr, _ptr]),
+    "rexagent_transform_reward": (C.c_int, [_ptr, _ptr, _i32, _ptr, _ptr]),
+    "rexagent_discounted_return": (C.c_int, [_ptr, _ptr, _i32, _i32, _i64, _i64, _f32, _ptr, _ptr]),
+    "rexagent_lambda_advantage": (C.c_int, [_ptr, _ptr, _ptr, _i32, _i32, _i64, _i64, _f32, _ptr, _ptr]),
+    "rexagent_gae_segments": (C.c_int, [_ptr, _ptr, _ptr, _i32, _i32, _f32, _f32, _ptr, _ptr, _ptr]),
+    "rexagent_launch_count": (_i64, [_ptr]),
+}
+EXPORTS = [n for n in SIGNATURES if n.startswith("rexsim_")]
+AGENT_EXPORTS = [n for n in SIGNATURES if n.startswith("rexagent_")]
 
 _LIB = None
 
@@ -59,60 +107,9 @@ def load():
     if not os.environ.get("REXSIM_LIB") and _build.needs_build():
         _build.build()
     L = C.CDLL(lib_path())
-    L.rexsim_obs_dim.argtypes = [C.c_int32, C.c_int32]
-    L.rexsim_action_dim.argtypes = [C.c_int32, C.c_int32]
-    L.rexsim_state_words.argtypes = [C.POINTER(RexSimConfig), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
-    L.rexsim_create.argtypes = [C.POINTER(RexSimConfig), C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]
-    L.rexsim_destroy.argtypes = [C.c_void_p]
-    L.rexsim_destroy.restype = None
-    L.rexsim_step.argtypes = [C.c_void_p] * 6
-    L.rexsim_step_host.argtypes = [C.c_void_p] * 4
-    L.rexsim_host_out_bytes.argtypes = [C.c_void_p]
-    L.rexsim_host_out_bytes.restype = C.c_int64
-    L.rexsim_rebalance.argtypes = [C.c_void_p, C.c_void_p]
-    L.rexsim_reset.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
-    L.rexsim_get_state.argtypes = [C.c_void_p] * 4
-    L.rexsim_set_state.argtypes = [C.c_void_p] * 3
-    L.rexsim_state_buffers.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    L.rexsim_error_flags.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-    L.rexsim_clear_errors.argtypes = [C.c_void_p, C.c_void_p]
-    L.rexsim_last_command.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-    L.rexsim_solver_cost.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-    L.rexsim_launch_count.argtypes = [C.c_void_p]
-    L.rexsim_launch_count.restype = C.c_int64
-    L.rexsim_last_step_build.argtypes = [C.c_void_p] + [C.POINTER(C.c_int32)] * 3
-    L.rexsim_last_error.restype = C.c_char_p
-    L.rexsim_rand_u32.argtypes = [C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32]
-    L.rexsim_rand_u32.restype = C.c_uint32
-    L.rexsim_noise.argtypes = [C.c_uint64] + [C.c_uint32] * 5
-    L.rexsim_noise.restype = C.c_float
-    L.rexsim_history_depth.argtypes = [C.POINTER(RexSimConfig)]
-    L.rexsim_history_buffer.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
-    L.rexsim_set_render_tables.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
-    L.rexsim_render.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_float,
-                                C.c_void_p, C.c_void_p]
-    # include/rexsim_agent.h
-    cfgp = C.POINTER(RexAgentConfig)
-    L.rexagent_policy_floats.argtypes = [cfgp]; L.rexagent_policy_floats.restype = C.c_int64
-    L.rexagent_value_floats.argtypes = [cfgp]; L.rexagent_value_floats.restype = C.c_int64
-    L.rexagent_create.argtypes = [cfgp, C.POINTER(C.c_void_p)]
-    L.rexagent_destroy.argtypes = [C.c_void_p]; L.rexagent_destroy.restype = None
-    L.rexagent_set_precision.argtypes = [C.c_void_p, C.c_int32]
-    L.rexagent_set_params.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
-    L.rexagent_get_params.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
-    L.rexagent_params_buffer.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-    L.rexagent_state_buffers.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    L.rexagent_set_filters.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_float]
-    L.rexagent_get_filters.argtypes = [C.c_void_p] * 5
-    L.rexagent_perform.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_uint64, C.c_uint32, C.c_uint32] + [C.c_void_p] * 6
-    L.rexagent_experience.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
-    L.rexagent_experience_partial.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
-    L.rexagent_experience_finalize.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.rexagent_transform_reward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
-    L.rexagent_discounted_return.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_float, C.c_void_p, C.c_void_p]
-    L.rexagent_lambda_advantage.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_float, C.c_void_p, C.c_void_p]
-    L.rexagent_gae_segments.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.rexagent_launch_count.argtypes = [C.c_void_p]; L.rexagent_launch_count.restype = C.c_int64
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _LIB = L
     return L
 
@@ -124,3 +121,33 @@ def check(rc):
     if rc in (-1, -2, -4):
         raise ValueError(f"rexsim: {msg} (status {rc})")
     raise RuntimeError(f"rexsim: {msg} (status {rc})")
+
+
+class DevArray(object):
+    """Expose a raw device pointer to torch through __cuda_array_interface__ (no copy, no ownership)."""
+
+    def __init__(self, ptr, shape, typestr, owner):
+        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (int(ptr), False), "version": 2}
+        self._owner = owner
+
+
+def device_view(ptr, shape, typestr, owner, device):
+    """torch tensor over raw device memory of a handle; the view keeps `owner` alive."""
+    return torch.as_tensor(DevArray(ptr, shape, typestr, owner), device=device)
+
+
+def stream_ptr(device):
+    """The current torch stream of `device`, as the `void* stream` argument of the C ABI."""
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+def call(index, fn, *args, stream=True):
+    """fn(*args[, current stream]) with CUDA device `index` current, raising on a non-zero status.  The device is only
+    entered when it is not the current one already, which is what a step costs least."""
+    if torch.cuda.current_device() == index:
+        rc = fn(*args, torch.cuda.current_stream().cuda_stream) if stream else fn(*args)
+    else:
+        with torch.cuda.device(index):
+            rc = fn(*args, torch.cuda.current_stream().cuda_stream) if stream else fn(*args)
+    if rc:
+        check(rc)

@@ -2,6 +2,7 @@
 vector, value MLP) fused with PPOAlgorithm.perform's observation filter and sampling (agents/ppo/algorithm.py:105-135) in
 one CUDA kernel (csrc/rexsim_agent.cu, C ABI include/rexsim_agent.h).  There is no CPU fallback."""
 import ctypes as C
+import functools
 import os
 
 import numpy as np
@@ -40,21 +41,21 @@ class ForwardGaussianPolicy(object):
         self._cfg = c
         self.n_policy = int(self._L.rexagent_policy_floats(C.byref(c)))
         self.n_value = int(self._L.rexagent_value_floats(C.byref(c)))
+        index = self.device.index if self.device.index is not None else torch.cuda.current_device()
+        # every library call: on this network's device and torch's current stream there, a non-zero status raised
+        self._call = functools.partial(_capi.call, index)
         h = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _capi.check(self._L.rexagent_create(C.byref(c), C.byref(h)))
+        self._call(self._L.rexagent_create, C.byref(c), C.byref(h), stream=False)
         self._h = h
         # tensor_cores=True: layer 2 (97 % of the flops) as wgmma tf32 with fp32 accumulation in registers; operands keep 11
         # significant bits (error vs the fp32 kernel: DESIGN.md section 5).  False (default): fp32 on the CUDA cores.
         self.tensor_cores = bool(tensor_cores)
         if self.tensor_cores:
-            with torch.cuda.device(self.device):
-                _capi.check(self._L.rexagent_set_precision(self._h, 1))
+            self._call(self._L.rexagent_set_precision, self._h, 1, stream=False)
         pf, pc = C.c_void_p(), C.c_void_p()
         _capi.check(self._L.rexagent_state_buffers(self._h, C.byref(pf), C.byref(pc)))
-        from ..envs.batched_env import _DevArray
-        self._filt = torch.as_tensor(_DevArray(pf.value, (2 * self.O + 2,), "<f4", self), device=self.device)
-        self._cnt = torch.as_tensor(_DevArray(pc.value, (4,), "<i8", self), device=self.device)    # int64: counts pass 2^31
+        self._filt = _capi.device_view(pf.value, (2 * self.O + 2,), "<f4", self, self.device)
+        self._cnt = _capi.device_view(pc.value, (4,), "<i8", self, self.device)                    # int64: counts pass 2^31
         self.observ_filter = StreamingNormalize(self, "observ")
         self.reward_filter = StreamingNormalize(self, "reward")
         # initialisers of networks.py:18-19 and tf.contrib.layers defaults: xavier-uniform hidden layers, zero biases,
@@ -92,13 +93,11 @@ class ForwardGaussianPolicy(object):
             if a.shape != shapes[k]:
                 raise ValueError("weight %s has shape %s, expected %s" % (k, a.shape, shapes[k]))
             block[o:o + a.size] = a.reshape(-1); o += a.size
-        with torch.cuda.device(self.device):
-            _capi.check(self._L.rexagent_set_params(self._h, block.ctypes.data, block.size))
+        self._call(self._L.rexagent_set_params, self._h, block.ctypes.data, block.size, stream=False)
 
     def get_weights(self):
         block = np.zeros(self.n_policy + self.n_value, np.float32)
-        with torch.cuda.device(self.device):
-            _capi.check(self._L.rexagent_get_params(self._h, block.ctypes.data, block.size))
+        self._call(self._L.rexagent_get_params, self._h, block.ctypes.data, block.size, stream=False)
         out, o = {}, 0
         shapes = self._shapes()
         for k in ("pW1", "pb1", "pW2", "pb2", "pW3", "pb3", "logstd"):
@@ -124,20 +123,18 @@ class ForwardGaussianPolicy(object):
         m = np.ascontiguousarray(observ_mean, np.float32); v = np.ascontiguousarray(observ_var_sum, np.float32)
         if m.shape != (self.O,) or v.shape != (self.O,):
             raise ValueError("filter statistics must have shape (%d,)" % self.O)
-        with torch.cuda.device(self.device):
-            _capi.check(self._L.rexagent_set_filters(self._h, int(observ_count), m.ctypes.data, v.ctypes.data, int(reward_count),
-                                                     float(reward_mean), float(reward_var_sum)))
+        self._call(self._L.rexagent_set_filters, self._h, int(observ_count), m.ctypes.data, v.ctypes.data, int(reward_count),
+                   float(reward_mean), float(reward_var_sum), stream=False)
 
     def get_filters(self):
         counts = np.zeros(2, np.int64); m = np.zeros(self.O, np.float32); v = np.zeros(self.O, np.float32); r = np.zeros(2, np.float32)
-        with torch.cuda.device(self.device):
-            _capi.check(self._L.rexagent_get_filters(self._h, counts.ctypes.data, m.ctypes.data, v.ctypes.data, r.ctypes.data))
+        self._call(self._L.rexagent_get_filters, self._h, counts.ctypes.data, m.ctypes.data, v.ctypes.data, r.ctypes.data, stream=False)
         return dict(observ_count=int(counts[0]), observ_mean=m, observ_var_sum=v, reward_count=int(counts[1]),
                     reward_mean=float(r[0]), reward_var_sum=float(r[1]))
 
     # ---- PPOAlgorithm.perform / experience -----------------------------------------------------------------------------
     def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        return _capi.stream_ptr(self.device)
 
     def perform(self, observ, training=False, seed=0, step=0, env_offset=0, out=None, observ_copy=None):
         """observ: CUDA float32 [n][O].  Returns dict(action [n][A], mean [n][A], logprob [n], value [n]) of CUDA tensors
@@ -152,10 +149,8 @@ class ForwardGaussianPolicy(object):
             out = dict(action=torch.empty((n, self.A), device=dev), mean=torch.empty((n, self.A), device=dev),
                        logprob=torch.empty((n,), device=dev), value=torch.empty((n,), device=dev))
         ptr = lambda t: None if t is None else t.data_ptr()
-        with torch.cuda.device(self.device):
-            _capi.check(self._L.rexagent_perform(self._h, observ.data_ptr(), n, int(bool(training)), int(seed), int(step), int(env_offset),
-                                                 ptr(out.get("action")), ptr(out.get("mean")), ptr(out.get("logprob")), ptr(out.get("value")),
-                                                 ptr(observ_copy), self._stream()))
+        self._call(self._L.rexagent_perform, self._h, observ.data_ptr(), n, int(bool(training)), int(seed), int(step), int(env_offset),
+                   ptr(out.get("action")), ptr(out.get("mean")), ptr(out.get("logprob")), ptr(out.get("value")), ptr(observ_copy))
         return out
 
     def experience(self, observ, reward, group=None):
@@ -166,21 +161,20 @@ class ForwardGaussianPolicy(object):
         import torch.distributed as dist
         n = observ.shape[0]
         sharded = dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1
+        if not sharded:
+            self._call(self._L.rexagent_experience, self._h, observ.data_ptr(), reward.data_ptr(), n)
+            return
+        if getattr(self, "_sums", None) is None:
+            self._sums = torch.zeros((self.O + 1, 2), dtype=torch.float32, device=self.device)
+        self._call(self._L.rexagent_experience_partial, self._h, observ.data_ptr(), reward.data_ptr(), n, self._sums.data_ptr())
         with torch.cuda.device(self.device):
-            if not sharded:
-                _capi.check(self._L.rexagent_experience(self._h, observ.data_ptr(), reward.data_ptr(), n, self._stream()))
-                return
-            if getattr(self, "_sums", None) is None:
-                self._sums = torch.zeros((self.O + 1, 2), dtype=torch.float32, device=self.device)
-            _capi.check(self._L.rexagent_experience_partial(self._h, observ.data_ptr(), reward.data_ptr(), n, self._sums.data_ptr(), self._stream()))
             dist.all_reduce(self._sums, op=dist.ReduceOp.SUM, group=group)
-            _capi.check(self._L.rexagent_experience_finalize(self._h, self._sums.data_ptr(), n * dist.get_world_size(group),
-                                                              observ.data_ptr(), reward.data_ptr(), self._stream()))
+        self._call(self._L.rexagent_experience_finalize, self._h, self._sums.data_ptr(), n * dist.get_world_size(group),
+                   observ.data_ptr(), reward.data_ptr())
 
     def transform_reward(self, reward, out=None):
         out = torch.empty_like(reward) if out is None else out
-        with torch.cuda.device(self.device):
-            _capi.check(self._L.rexagent_transform_reward(self._h, reward.data_ptr(), reward.numel(), out.data_ptr(), self._stream()))
+        self._call(self._L.rexagent_transform_reward, self._h, reward.data_ptr(), reward.numel(), out.data_ptr())
         return out
 
     def state_dict(self):

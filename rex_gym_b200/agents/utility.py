@@ -1,8 +1,6 @@
 """discounted_return / lambda_advantage (rex_gym/agents/ppo/utility.py:72-82,112-124) as CUDA scans; tensors stay on
 the device.  Rows are episodes ([E][L] like the reference's EpisodeMemory) in any strided layout -- pass a transposed view of
 a time-major buffer and the kernel reads it coalesced."""
-import ctypes as C
-
 import torch
 
 from .. import _capi
@@ -13,10 +11,6 @@ def _check(t, name):
         raise ValueError("%s must be a 2-D CUDA float32 tensor" % name)
 
 
-def _stream(t):
-    return C.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
-
-
 def discounted_return(reward, length, discount):
     _check(reward, "reward")
     E, L = reward.shape
@@ -24,7 +18,7 @@ def discounted_return(reward, length, discount):
     out = torch.empty_strided(reward.shape, reward.stride(), dtype=torch.float32, device=reward.device)
     with torch.cuda.device(reward.device):
         _capi.check(_capi.load().rexagent_discounted_return(reward.data_ptr(), length.data_ptr(), E, L, reward.stride(0), reward.stride(1),
-                                                            float(discount), out.data_ptr(), _stream(reward)))
+                                                            float(discount), out.data_ptr(), _capi.stream_ptr(reward.device)))
     return out
 
 
@@ -37,7 +31,7 @@ def lambda_advantage(reward, value, length, discount):
     out = torch.empty_strided(reward.shape, reward.stride(), dtype=torch.float32, device=reward.device)
     with torch.cuda.device(reward.device):
         _capi.check(_capi.load().rexagent_lambda_advantage(reward.data_ptr(), value.data_ptr(), length.data_ptr(), E, L, reward.stride(0),
-                                                           reward.stride(1), float(discount), out.data_ptr(), _stream(reward)))
+                                                           reward.stride(1), float(discount), out.data_ptr(), _capi.stream_ptr(reward.device)))
     return out
 
 
@@ -51,5 +45,5 @@ def gae_segments(reward, value, done, discount, lam=1.0):
     ret, adv = torch.empty_like(reward), torch.empty_like(reward)
     with torch.cuda.device(reward.device):
         _capi.check(_capi.load().rexagent_gae_segments(reward.data_ptr(), value.data_ptr(), d8.data_ptr(), T, n, float(discount), float(lam),
-                                                       ret.data_ptr(), adv.data_ptr(), _stream(reward)))
+                                                       ret.data_ptr(), adv.data_ptr(), _capi.stream_ptr(reward.device)))
     return ret, adv

@@ -5,14 +5,13 @@
 // fp32 throughout (the reference's TF graph is fp32): the MLP is computed on the CUDA cores with a register-tiled
 // shared-memory GEMM so results match an fp32 reference to rounding; see DESIGN.md for the roofline of each kernel.
 #include "rexsim_kernel.cuh"
+#include "rexsim_host.h"
 #include "../../include/rexsim_agent.h"
-#include <cstdio>
 #include <cstring>
 #include <vector>
 #include <type_traits>
 
 namespace rexsim {
-void set_error(const char* msg);   // rexsim_capi.cu (message returned by rexsim_last_error)
 
 constexpr int AG_MAX_O = 32, AG_MAX_A = 8, AG_MAX_H1 = 256, AG_MAX_H2 = 128;
 constexpr int RED_BLOCKS = 256;    // partial blocks of the filter update
@@ -595,11 +594,9 @@ __global__ void __launch_bounds__(256) gae_segments_kernel(const float* __restri
 using namespace rexsim;
 
 struct RexAgent {
-    AgentDev D;
-    float* d_params = nullptr;
-    float* d_filt = nullptr;
-    int64_t* d_cnt = nullptr;
-    float* d_partial = nullptr;
+    AgentDev D;                        // filt, cnt and partial are allocated from `mem` in place
+    DeviceBuffers mem;
+    float* params = nullptr;           // what D.params reads (the kernels' pointer is to const)
     int sm_count = 132;
     int64_t launches = 0;
     int precision = 0;                 // 0: fp32 on the CUDA cores (parity default); 1: layer 2 on the tensor cores in TF32
@@ -614,16 +611,34 @@ static PerformTcKernel perform_tc_pick(const RexAgentConfig* c) {
     return perform_tc_kernel<0, 0>;
 }
 
-static int afail(int code, const char* msg) { set_error(msg); return code; }
-#define ACK(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { char b[256]; snprintf(b, sizeof(b), "%s: %s", #x, cudaGetErrorString(_e)); set_error(b); return REXSIM_ERR_CUDA; } } while (0)
-
 static int64_t pad4(int64_t n) { return (n + 3) & ~(int64_t)3; }
 static int check_cfg(const RexAgentConfig* c) {
-    if (!c) return afail(REXSIM_ERR_INVALID, "null agent config");
+    if (!c) return fail(REXSIM_ERR_INVALID, "null agent config");
     if (c->obs_dim <= 0 || c->obs_dim > AG_MAX_O || c->action_dim <= 0 || c->action_dim > AG_MAX_A)
-        return afail(REXSIM_ERR_INVALID, "agent: obs_dim must be 1..32 and action_dim 1..8");
+        return fail(REXSIM_ERR_INVALID, "agent: obs_dim must be 1..32 and action_dim 1..8");
     if (c->hidden1 <= 0 || c->hidden1 > AG_MAX_H1 || c->hidden2 <= 0 || c->hidden2 > AG_MAX_H2 || (c->hidden1 & 3) || (c->hidden2 & 3))
-        return afail(REXSIM_ERR_UNSUPPORTED, "agent: hidden1 <= 256, hidden2 <= 128, both multiples of 4");
+        return fail(REXSIM_ERR_UNSUPPORTED, "agent: hidden1 <= 256, hidden2 <= 128, both multiples of 4");
+    return REXSIM_OK;
+}
+
+// StreamingNormalize.update of one batch; sums_out null: into the filters, else this rank's partial sums for the sharded path
+static int experience(RexAgent* a, const float* observ, const float* reward, int32_t n, float* sums_out, void* stream) {
+    if (n <= 0) return fail(REXSIM_ERR_INVALID, "agent: n must be positive");
+    ExperienceArgs P; P.D = a->D; P.observ = observ; P.reward = reward; P.n = n; P.sums_out = sums_out;
+    int blocks = (n + 255) / 256;
+    if (blocks > RED_BLOCKS) blocks = RED_BLOCKS;
+    experience_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(P);
+    return enqueue(a, cudaGetLastError(), "experience launch");
+}
+
+// discounted_return (ADV = false, no values) / lambda_advantage; the scans have no handle, so they count no launch
+template <bool ADV>
+static int row_scan(const float* reward, const float* value, const int32_t* length, int32_t episodes, int32_t L, int64_t se,
+                    int64_t st, float discount, float* out, void* stream) {
+    if (!reward || (ADV && !value) || !length || !out) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (episodes <= 0 || L <= 0) return fail(REXSIM_ERR_INVALID, "agent: empty scan");
+    row_scan_kernel<ADV><<<(episodes + 255) / 256, 256, 0, (cudaStream_t)stream>>>(reward, value, length, episodes, L, se, st, discount, out);
+    CK(cudaGetLastError());
     return REXSIM_OK;
 }
 
@@ -648,9 +663,9 @@ static size_t perform_smem_bytes(const RexAgentConfig* c, int tm) {
 int rexagent_create(const RexAgentConfig* cfg, RexAgent** out) {
     int rc = check_cfg(cfg);
     if (rc) return rc;
-    if (!out) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (perform_smem_bytes(cfg, 128) > 227 * 1024) return afail(REXSIM_ERR_UNSUPPORTED, "agent: network does not fit the 227 KB of shared memory");
-    if (cfg->action_dim * (cfg->hidden2 / 4) > cfg->hidden1) return afail(REXSIM_ERR_UNSUPPORTED, "agent: action_dim * hidden2 / 4 must not exceed hidden1");
+    if (!out) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (perform_smem_bytes(cfg, 128) > 227 * 1024) return fail(REXSIM_ERR_UNSUPPORTED, "agent: network does not fit the 227 KB of shared memory");
+    if (cfg->action_dim * (cfg->hidden2 / 4) > cfg->hidden1) return fail(REXSIM_ERR_UNSUPPORTED, "agent: action_dim * hidden2 / 4 must not exceed hidden1");
     RexAgent* a = new RexAgent();
     struct Guard { RexAgent* a; ~Guard() { if (a) rexagent_destroy(a); } } guard{a};  // frees everything on an early return
     a->D.cfg = *cfg;
@@ -658,81 +673,77 @@ int rexagent_create(const RexAgentConfig* cfg, RexAgent** out) {
     const size_t np = (size_t)a->D.pol_floats + a->D.val_floats;
     const int O = cfg->obs_dim;
     int dev = 0;
-    ACK(cudaGetDevice(&dev));
-    ACK(cudaDeviceGetAttribute(&a->sm_count, cudaDevAttrMultiProcessorCount, dev));
-    ACK(cudaMalloc(&a->d_params, np * sizeof(float)));
-    ACK(cudaMemset(a->d_params, 0, np * sizeof(float)));
-    ACK(cudaMalloc(&a->d_filt, (2 * O + 2) * sizeof(float)));
-    ACK(cudaMemset(a->d_filt, 0, (2 * O + 2) * sizeof(float)));
-    ACK(cudaMalloc(&a->d_cnt, 4 * sizeof(int64_t)));
-    ACK(cudaMemset(a->d_cnt, 0, 4 * sizeof(int64_t)));
-    ACK(cudaMalloc(&a->d_partial, (size_t)RED_BLOCKS * 2 * (O + 1) * sizeof(float)));
-    ACK(cudaFuncSetAttribute(perform_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)perform_smem_bytes(cfg, 64)));
-    ACK(cudaFuncSetAttribute(perform_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)perform_smem_bytes(cfg, 128)));
-    a->D.params = a->d_params; a->D.filt = a->d_filt; a->D.cnt = a->d_cnt; a->D.partial = a->d_partial;
-    ACK(cudaDeviceSynchronize());
+    CK(cudaGetDevice(&dev));
+    CK(cudaDeviceGetAttribute(&a->sm_count, cudaDevAttrMultiProcessorCount, dev));
+    if (a->mem.zeroed(&a->params, np) || a->mem.zeroed(&a->D.filt, 2 * O + 2) || a->mem.zeroed(&a->D.cnt, 4) ||
+        a->mem.zeroed(&a->D.partial, (size_t)RED_BLOCKS * 2 * (O + 1)))
+        return REXSIM_ERR_CUDA;
+    a->D.params = a->params;
+    CK(cudaFuncSetAttribute(perform_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)perform_smem_bytes(cfg, 64)));
+    CK(cudaFuncSetAttribute(perform_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)perform_smem_bytes(cfg, 128)));
+    CK(cudaDeviceSynchronize());
     guard.a = nullptr;
     *out = a;
     return REXSIM_OK;
 }
 void rexagent_destroy(RexAgent* a) {
     if (!a) return;
-    cudaFree(a->d_params); cudaFree(a->d_filt); cudaFree(a->d_cnt); cudaFree(a->d_partial);
+    a->mem.release();
     delete a;
 }
 int rexagent_set_precision(RexAgent* a, int32_t mode) {
-    if (!a) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (mode != 0 && mode != 1) return afail(REXSIM_ERR_INVALID, "agent: precision must be 0 (fp32) or 1 (tf32 tensor cores)");
+    if (!a) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (mode != 0 && mode != 1) return fail(REXSIM_ERR_INVALID, "agent: precision must be 0 (fp32) or 1 (tf32 tensor cores)");
     if (mode == 1) {
         const RexAgentConfig* c = &a->D.cfg;
         if ((c->hidden1 & 7) || c->obs_dim > 16 || perform_tc_smem_bytes(c) > 227 * 1024)
-            return afail(REXSIM_ERR_UNSUPPORTED, "agent: the tensor-core path needs hidden1 % 8 == 0, obs_dim <= 16 and operands that fit 227 KB of shared memory");
-        ACK(cudaFuncSetAttribute(perform_tc_pick(c), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)perform_tc_smem_bytes(c)));
+            return fail(REXSIM_ERR_UNSUPPORTED, "agent: the tensor-core path needs hidden1 % 8 == 0, obs_dim <= 16 and operands that fit 227 KB of shared memory");
+        CK(cudaFuncSetAttribute(perform_tc_pick(c), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)perform_tc_smem_bytes(c)));
     }
     a->precision = mode;
     return REXSIM_OK;
 }
 int rexagent_set_params(RexAgent* a, const float* h, int64_t n) {
-    if (!a || !h) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (n != (int64_t)a->D.pol_floats + a->D.val_floats) return afail(REXSIM_ERR_INVALID, "agent: parameter block size mismatch");
-    ACK(cudaMemcpy(a->d_params, h, n * sizeof(float), cudaMemcpyHostToDevice));
+    if (!a || !h) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (n != (int64_t)a->D.pol_floats + a->D.val_floats) return fail(REXSIM_ERR_INVALID, "agent: parameter block size mismatch");
+    CK(cudaMemcpy(a->params, h, n * sizeof(float), cudaMemcpyHostToDevice));
     return REXSIM_OK;
 }
 int rexagent_get_params(RexAgent* a, float* h, int64_t n) {
-    if (!a || !h) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (n != (int64_t)a->D.pol_floats + a->D.val_floats) return afail(REXSIM_ERR_INVALID, "agent: parameter block size mismatch");
-    ACK(cudaMemcpy(h, a->d_params, n * sizeof(float), cudaMemcpyDeviceToHost));
+    if (!a || !h) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (n != (int64_t)a->D.pol_floats + a->D.val_floats) return fail(REXSIM_ERR_INVALID, "agent: parameter block size mismatch");
+    CK(cudaMemcpy(h, a->params, n * sizeof(float), cudaMemcpyDeviceToHost));
     return REXSIM_OK;
 }
 int rexagent_params_buffer(RexAgent* a, float** p) {
-    if (!a || !p) return afail(REXSIM_ERR_INVALID, "null argument");
-    *p = a->d_params;
+    if (!a || !p) return fail(REXSIM_ERR_INVALID, "null argument");
+    *p = a->params;
     return REXSIM_OK;
 }
 int rexagent_state_buffers(RexAgent* a, float** filt, int64_t** counters) {
-    if (!a) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (filt) *filt = a->d_filt;
-    if (counters) *counters = a->d_cnt;
+    if (!a) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (filt) *filt = a->D.filt;
+    if (counters) *counters = a->D.cnt;
     return REXSIM_OK;
 }
 int rexagent_set_filters(RexAgent* a, int64_t oc, const float* om, const float* ov, int64_t rc, float rm, float rv) {
-    if (!a || !om || !ov) return afail(REXSIM_ERR_INVALID, "null argument");
+    if (!a || !om || !ov) return fail(REXSIM_ERR_INVALID, "null argument");
     const int O = a->D.cfg.obs_dim;
     std::vector<float> f(2 * O + 2);
     for (int i = 0; i < O; i++) { f[i] = om[i]; f[O + i] = ov[i]; }
     f[2 * O] = rm; f[2 * O + 1] = rv;
     int64_t c[4] = {oc, rc, 0, 0};
-    ACK(cudaMemcpy(a->d_filt, f.data(), f.size() * sizeof(float), cudaMemcpyHostToDevice));
-    ACK(cudaMemcpy(a->d_cnt, c, sizeof(c), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(a->D.filt, f.data(), f.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(a->D.cnt, c, sizeof(c), cudaMemcpyHostToDevice));
     return REXSIM_OK;
 }
 int rexagent_get_filters(RexAgent* a, int64_t* counts, float* om, float* ov, float* rmv) {
-    if (!a || !counts || !om || !ov || !rmv) return afail(REXSIM_ERR_INVALID, "null argument");
+    if (!a || !counts || !om || !ov || !rmv) return fail(REXSIM_ERR_INVALID, "null argument");
     const int O = a->D.cfg.obs_dim;
     std::vector<float> f(2 * O + 2);
     int64_t c[4];
-    ACK(cudaMemcpy(f.data(), a->d_filt, f.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    ACK(cudaMemcpy(c, a->d_cnt, sizeof(c), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(f.data(), a->D.filt, f.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(c, a->D.cnt, sizeof(c), cudaMemcpyDeviceToHost));
     for (int i = 0; i < O; i++) { om[i] = f[i]; ov[i] = f[O + i]; }
     rmv[0] = f[2 * O]; rmv[1] = f[2 * O + 1];
     counts[0] = c[0]; counts[1] = c[1];
@@ -742,8 +753,8 @@ int rexagent_get_filters(RexAgent* a, int64_t* counts, float* om, float* ov, flo
 int rexagent_perform(RexAgent* a, const float* observ, int32_t n, int32_t training, uint64_t seed, uint32_t step,
                      uint32_t env_offset, float* action, float* mean, float* logprob, float* value, float* observ_copy,
                      void* stream) {
-    if (!a || !observ) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (n <= 0) return afail(REXSIM_ERR_INVALID, "agent: n must be positive");
+    if (!a || !observ) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (n <= 0) return fail(REXSIM_ERR_INVALID, "agent: n must be positive");
     PerformArgs P;
     P.D = a->D; P.observ = observ; P.n = n; P.training = training; P.seed = seed; P.step = step; P.env_offset = env_offset;
     P.action = action; P.mean = mean; P.logprob = logprob; P.value = value; P.observ_copy = observ_copy;
@@ -752,9 +763,7 @@ int rexagent_perform(RexAgent* a, const float* observ, int32_t n, int32_t traini
         const int nt = (n + tc::TM - 1) / tc::TM;
         dim3 grid_tc(nt < half_tc ? nt : half_tc, 2);
         perform_tc_pick(&a->D.cfg)<<<grid_tc, tc::THREADS, perform_tc_smem_bytes(&a->D.cfg), (cudaStream_t)stream>>>(P);
-        ACK(cudaGetLastError());
-        a->launches++;
-        return REXSIM_OK;
+        return enqueue(a, cudaGetLastError(), "perform launch");
     }
     // one CTA per SM (the weights fill most of the shared memory); the two networks run in different CTAs (blockIdx.y).
     // Small batches use 64-env tiles so that more SMs get a tile, large ones 128-env tiles (8 x 4 register tile per thread).
@@ -767,72 +776,44 @@ int rexagent_perform(RexAgent* a, const float* observ, int32_t n, int32_t traini
     if (threads < tm) threads = tm;
     if (big) perform_kernel<128><<<grid, threads, perform_smem_bytes(&a->D.cfg, 128), (cudaStream_t)stream>>>(P);
     else perform_kernel<64><<<grid, threads, perform_smem_bytes(&a->D.cfg, 64), (cudaStream_t)stream>>>(P);
-    ACK(cudaGetLastError());
-    a->launches++;
-    return REXSIM_OK;
+    return enqueue(a, cudaGetLastError(), "perform launch");
 }
 int rexagent_experience(RexAgent* a, const float* observ, const float* reward, int32_t n, void* stream) {
-    if (!a || !observ || !reward) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (n <= 0) return afail(REXSIM_ERR_INVALID, "agent: n must be positive");
-    ExperienceArgs P; P.D = a->D; P.observ = observ; P.reward = reward; P.n = n; P.sums_out = nullptr;
-    int blocks = (n + 255) / 256;
-    if (blocks > RED_BLOCKS) blocks = RED_BLOCKS;
-    experience_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(P);
-    ACK(cudaGetLastError());
-    a->launches++;
-    return REXSIM_OK;
+    if (!a || !observ || !reward) return fail(REXSIM_ERR_INVALID, "null argument");
+    return experience(a, observ, reward, n, nullptr, stream);
 }
 int rexagent_experience_partial(RexAgent* a, const float* observ, const float* reward, int32_t n, float* sums, void* stream) {
-    if (!a || !observ || !reward || !sums) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (n <= 0) return afail(REXSIM_ERR_INVALID, "agent: n must be positive");
-    ExperienceArgs P; P.D = a->D; P.observ = observ; P.reward = reward; P.n = n; P.sums_out = sums;
-    int blocks = (n + 255) / 256;
-    if (blocks > RED_BLOCKS) blocks = RED_BLOCKS;
-    experience_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(P);
-    ACK(cudaGetLastError());
-    a->launches++;
-    return REXSIM_OK;
+    if (!a || !observ || !reward || !sums) return fail(REXSIM_ERR_INVALID, "null argument");
+    return experience(a, observ, reward, n, sums, stream);
 }
 int rexagent_experience_finalize(RexAgent* a, const float* sums, int32_t n_total, const float* observ, const float* reward, void* stream) {
-    if (!a || !sums || !observ || !reward) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (n_total <= 0) return afail(REXSIM_ERR_INVALID, "agent: n_total must be positive");
+    if (!a || !sums || !observ || !reward) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (n_total <= 0) return fail(REXSIM_ERR_INVALID, "agent: n_total must be positive");
     experience_finalize_kernel<<<1, 64, 0, (cudaStream_t)stream>>>(a->D, sums, n_total, observ, reward);
-    ACK(cudaGetLastError());
-    a->launches++;
-    return REXSIM_OK;
+    return enqueue(a, cudaGetLastError(), "experience_finalize launch");
 }
 int rexagent_transform_reward(RexAgent* a, const float* reward, int32_t n, float* out, void* stream) {
-    if (!a || !reward || !out) return afail(REXSIM_ERR_INVALID, "null argument");
+    if (!a || !reward || !out) return fail(REXSIM_ERR_INVALID, "null argument");
     if (n <= 0) return REXSIM_OK;
     int blocks = (n + 255) / 256;
     if (blocks > 1184) blocks = 1184;
     transform_reward_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a->D, reward, n, out);
-    ACK(cudaGetLastError());
-    a->launches++;
-    return REXSIM_OK;
+    return enqueue(a, cudaGetLastError(), "transform_reward launch");
 }
 int rexagent_discounted_return(const float* reward, const int32_t* length, int32_t episodes, int32_t L, int64_t se, int64_t st,
                                float discount, float* out, void* stream) {
-    if (!reward || !length || !out) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (episodes <= 0 || L <= 0) return afail(REXSIM_ERR_INVALID, "agent: empty scan");
-    row_scan_kernel<false><<<(episodes + 255) / 256, 256, 0, (cudaStream_t)stream>>>(reward, nullptr, length, episodes, L, se, st, discount, out);
-    ACK(cudaGetLastError());
-    return REXSIM_OK;
+    return row_scan<false>(reward, nullptr, length, episodes, L, se, st, discount, out, stream);
 }
 int rexagent_lambda_advantage(const float* reward, const float* value, const int32_t* length, int32_t episodes, int32_t L,
                               int64_t se, int64_t st, float discount, float* out, void* stream) {
-    if (!reward || !value || !length || !out) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (episodes <= 0 || L <= 0) return afail(REXSIM_ERR_INVALID, "agent: empty scan");
-    row_scan_kernel<true><<<(episodes + 255) / 256, 256, 0, (cudaStream_t)stream>>>(reward, value, length, episodes, L, se, st, discount, out);
-    ACK(cudaGetLastError());
-    return REXSIM_OK;
+    return row_scan<true>(reward, value, length, episodes, L, se, st, discount, out, stream);
 }
 int rexagent_gae_segments(const float* reward, const float* value, const uint8_t* done, int32_t T, int32_t n, float discount,
                           float lambda, float* out_return, float* out_advantage, void* stream) {
-    if (!reward || !value || !done) return afail(REXSIM_ERR_INVALID, "null argument");
-    if (T <= 0 || n <= 0) return afail(REXSIM_ERR_INVALID, "agent: empty scan");
+    if (!reward || !value || !done) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (T <= 0 || n <= 0) return fail(REXSIM_ERR_INVALID, "agent: empty scan");
     gae_segments_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(reward, value, done, T, n, discount, lambda, out_return, out_advantage);
-    ACK(cudaGetLastError());
+    CK(cudaGetLastError());
     return REXSIM_OK;
 }
 int64_t rexagent_launch_count(const RexAgent* a) { return a ? a->launches : 0; }

@@ -1,6 +1,6 @@
 // rexsim_capi.cu -- the C ABI declared in include/rexsim.h (plain pointers and sizes, no torch types).
 #include "rexsim_kernel.cuh"
-#include <cstdio>
+#include "rexsim_host.h"
 #include <cstring>
 #include <cmath>
 #include <vector>
@@ -13,46 +13,56 @@ cudaError_t launch_get_state(const Params& P, float* out_f, int32_t* out_i, cuda
 cudaError_t launch_set_state(const Params& P, const float* in_f, cudaStream_t st);
 cudaError_t launch_rebalance(const int32_t* cost, int n, int32_t* hist, int32_t* perm, cudaStream_t st);
 cudaError_t launch_render(const Params& P, const float* rt, const float* zrange, const int32_t* idx, int k, int W, int H,
-                          float distance, float yaw_deg, float pitch_deg, uint8_t* rgb, cudaStream_t st, int64_t* launches);
+                          float distance, float yaw_deg, float pitch_deg, uint8_t* rgb, cudaStream_t st, int* launches);
 }  // namespace rexsim
 
 using namespace rexsim;
 
 struct RexSim {
-    Params P;
-    float* d_model = nullptr;
-    float* d_sf = nullptr;
-    int32_t* d_si = nullptr;
-    float* d_snap_f = nullptr;
-    int32_t* d_snap_i = nullptr;
-    float* d_zoff = nullptr;
-    float* d_zrange = nullptr;         // [nfields][2] lowest / highest centred height of each field (renderer)
-    float* d_rt = nullptr;             // render table (rexsim_set_render_tables)
+    Params P;                          // the handle's buffers are P's pointer fields, allocated from `mem`
+    DeviceBuffers mem;
+    float* zrange = nullptr;           // [nfields][2] lowest / highest centred height of each field (renderer)
+    float* rt = nullptr;               // render table (rexsim_set_render_tables)
     bool rt_set = false;
-    int32_t* d_err = nullptr;
-    float* d_cmd = nullptr;
-    int32_t* d_perm = nullptr;         // slot -> env, sorted by solver cost (rexsim_rebalance)
-    int32_t* d_cost = nullptr;
-    int32_t* d_hist = nullptr;
-    bool perm_valid = false;
-    float* d_ring = nullptr;           // sensor history [D][words][N] (sensor model only)
-    float* d_snap_ring = nullptr;      // [nsnap][D][words]
-    float* d_act = nullptr;            // staging for rexsim_step_host
-    uint8_t* d_out = nullptr;          // obs | reward | done (same layout as the host block)
+    int32_t* perm = nullptr;           // slot -> env, sorted by solver cost; P.perm points here after rexsim_rebalance
+    int32_t* hist = nullptr;
+    float* act = nullptr;              // staging for rexsim_step_host
+    uint8_t* out = nullptr;            // obs | reward | done (same layout as the host block)
     int A = 0, O = 0;
     int nsnap = 1;
     int64_t launches = 0;
     int32_t launched[3] = {0, 0, 0};   // step_kernel instance of the last step launch: BLOCK, OCC, SENSOR
 };
 
-static thread_local char g_err[512] = "";
-namespace rexsim { void set_error(const char* msg) { snprintf(g_err, sizeof(g_err), "%s", msg); } }   // shared with rexsim_agent.cu
-static int fail(int code, const char* msg) { snprintf(g_err, sizeof(g_err), "%s", msg); return code; }
-static int cuda_fail(cudaError_t e, const char* where) {
-    snprintf(g_err, sizeof(g_err), "%s: %s", where, cudaGetErrorString(e));
-    return REXSIM_ERR_CUDA;
+// byte offsets of the block rexsim_step_host fills: obs [N][O] at 0 | reward [N] | done [N] | pad to 4 | int32 error bits |
+// 8 flag bytes the kernel sets directly on the zero-copy path
+struct HostBlock { size_t reward, done, err, bytes; };
+static HostBlock host_block(size_t N, size_t O) {
+    HostBlock b;
+    b.reward = N * O * sizeof(float);
+    b.done = b.reward + N * sizeof(float);
+    b.err = (b.done + N + 3) & ~(size_t)3;
+    b.bytes = b.err + sizeof(int32_t) + 8;
+    return b;
 }
-#define CK(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) return cuda_fail(_e, #x); } while (0)
+
+// the sensor model a config asks for (all zero but `words` when it is off)
+struct SensorCfg { int on, depth, n_ctl, n_pd; float a_ctl, a_pd; int words; };
+static SensorCfg sensor_cfg(const RexSimConfig* c) {
+    SensorCfg sc = {};
+    sc.words = c->num_motors == 18 ? HW_WORDS_ARM : HW_WORDS;
+    sc.on = c->control_latency > 0 || c->pd_latency > 0;
+    for (int k = 0; k < 5; k++) sc.on = sc.on || c->noise_stdev[k] > 0;
+    if (!sc.on) return sc;
+    // Rex._GetDelayedObservation reads history[n] and history[n + 1], n = int(latency / dt); once n + 1 reaches the deque's
+    // length (maxlen 100, rex.py:122) it reads the oldest row instead
+    const double dt = c->sim_dt_d;
+    sc.n_ctl = (int)(c->control_latency / dt); sc.n_pd = (int)(c->pd_latency / dt);
+    sc.a_ctl = (float)((c->control_latency - sc.n_ctl * dt) / dt); sc.a_pd = (float)((c->pd_latency - sc.n_pd * dt) / dt);
+    const int n = sc.n_ctl > sc.n_pd ? sc.n_ctl : sc.n_pd;
+    sc.depth = n + 1 >= HIST_MAXLEN ? (int)HIST_MAXLEN : n + 2;
+    return sc;
+}
 
 extern "C" {
 
@@ -86,19 +96,7 @@ static int validate(const RexSimConfig* c) {
     for (int k = 0; k < 5; k++) if (!(c->noise_stdev[k] >= 0)) return fail(REXSIM_ERR_INVALID, "noise_stdev must be >= 0");
     return REXSIM_OK;
 }
-static bool sensor_on(const RexSimConfig* c) {
-    bool on = c->control_latency > 0 || c->pd_latency > 0;
-    for (int k = 0; k < 5; k++) on = on || c->noise_stdev[k] > 0;
-    return on;
-}
-int rexsim_history_depth(const RexSimConfig* c) {
-    if (!c || !sensor_on(c)) return 0;
-    // Rex._GetDelayedObservation reads history[n] and history[n + 1], n = int(latency / dt); once n + 1 reaches the deque's
-    // length (maxlen 100, rex.py:122) it reads the oldest row instead
-    const int n_ctl = (int)(c->control_latency / c->sim_dt_d), n_pd = (int)(c->pd_latency / c->sim_dt_d);
-    const int n = n_ctl > n_pd ? n_ctl : n_pd;
-    return n + 1 >= HIST_MAXLEN ? (int)HIST_MAXLEN : n + 2;
-}
+int rexsim_history_depth(const RexSimConfig* c) { return c ? sensor_cfg(c).depth : 0; }
 float rexsim_noise(uint64_t seed, uint32_t global_env, uint32_t reset_count, uint32_t control_step, uint32_t site, uint32_t comp) {
     return noise_unit(seed, global_env, reset_count, control_step, site, comp);
 }
@@ -111,57 +109,42 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
     if (n_model_floats != mt_floats) return fail(REXSIM_ERR_MODEL, "model table size mismatch");
     RexSim* s = new RexSim();
     struct Guard { RexSim* s; ~Guard() { if (s) rexsim_destroy(s); } } guard{s};      // frees everything on an early return
-    memset(&s->P, 0, sizeof(Params));
-    s->P.cfg = *cfg;
-    s->P.cfg.sim_dt = (float)cfg->sim_dt_d;
-    const int N = cfg->num_envs;
-    s->P.N = N;
+    Params& P = s->P;
+    DeviceBuffers& mem = s->mem;
+    memset(&P, 0, sizeof(Params));
+    P.cfg = *cfg;
+    P.cfg.sim_dt = (float)cfg->sim_dt_d;
+    const size_t N = cfg->num_envs;
+    P.N = cfg->num_envs;
     {
         int dev = 0, sms = 132;
         CK(cudaGetDevice(&dev));
         CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        s->P.sm_count = sms;
+        P.sm_count = sms;
     }
     s->nsnap = cfg->terrain == REXSIM_TERRAIN_RANDOM ? cfg->nfields : 1;
-    CK(cudaMalloc(&s->d_model, mt_floats * sizeof(float)));
-    CK(cudaMemcpy(s->d_model, model_tables, mt_floats * sizeof(float), cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&s->d_sf, (size_t)NF * N * sizeof(float)));
-    CK(cudaMalloc(&s->d_si, (size_t)NI * N * sizeof(int32_t)));
-    CK(cudaMemset(s->d_sf, 0, (size_t)NF * N * sizeof(float)));
-    CK(cudaMemset(s->d_si, 0, (size_t)NI * N * sizeof(int32_t)));
-    CK(cudaMalloc(&s->d_snap_f, (size_t)NF * s->nsnap * sizeof(float)));
-    CK(cudaMalloc(&s->d_snap_i, (size_t)NI * s->nsnap * sizeof(int32_t)));
-    CK(cudaMemset(s->d_snap_f, 0, (size_t)NF * s->nsnap * sizeof(float)));
-    CK(cudaMemset(s->d_snap_i, 0, (size_t)NI * s->nsnap * sizeof(int32_t)));
-    CK(cudaMalloc(&s->d_err, (size_t)(N + 1) * sizeof(int32_t)));   /* [N] per-env bits + 1 word: OR of all */
-    CK(cudaMemset(s->d_err, 0, (size_t)(N + 1) * sizeof(int32_t)));
-    CK(cudaMalloc(&s->d_cmd, (size_t)cfg->num_motors * N * sizeof(float)));
-    CK(cudaMemset(s->d_cmd, 0, (size_t)cfg->num_motors * N * sizeof(float)));
-    CK(cudaMalloc(&s->d_perm, (size_t)N * sizeof(int32_t)));
-    CK(cudaMalloc(&s->d_cost, (size_t)N * sizeof(int32_t)));
-    CK(cudaMemset(s->d_cost, 0, (size_t)N * sizeof(int32_t)));
-    CK(cudaMalloc(&s->d_hist, 256 * sizeof(int32_t)));
-    CK(cudaMalloc(&s->d_rt, REXSIM_RT_FLOATS * sizeof(float)));
-    if (sensor_on(cfg)) {
-        Params& P = s->P;
-        const double dt = cfg->sim_dt_d;
+    s->A = rexsim_action_dim(cfg->task, cfg->signal); s->O = rexsim_obs_dim(cfg->task, cfg->num_motors);
+    // the kernels read these through pointers to const; create fills them
+    float *model = nullptr, *snap_f = nullptr, *zoff = nullptr;
+    int32_t* snap_i = nullptr;
+    if (mem.zeroed(&model, mt_floats) || mem.zeroed(&P.sf, NF * N) || mem.zeroed(&P.si, NI * N) ||
+        mem.zeroed(&snap_f, (size_t)NF * s->nsnap) || mem.zeroed(&snap_i, (size_t)NI * s->nsnap) ||
+        mem.zeroed(&P.err, N + 1) ||                                    // [N] per-env bits + 1 word: OR of all
+        mem.zeroed(&P.cmd_out, cfg->num_motors * N) || mem.zeroed(&P.cost, N) || mem.zeroed(&s->perm, N) ||
+        mem.zeroed(&s->hist, 256) || mem.zeroed(&s->rt, REXSIM_RT_FLOATS) || mem.zeroed(&s->act, N * s->A) ||
+        mem.zeroed(&s->out, host_block(N, s->O).bytes))
+        return REXSIM_ERR_CUDA;
+    CK(cudaMemcpy(model, model_tables, mt_floats * sizeof(float), cudaMemcpyHostToDevice));
+    const SensorCfg sc = sensor_cfg(cfg);
+    if (sc.on) {
         P.sensor_on = 1;
-        P.ring_depth = rexsim_history_depth(cfg);
-        P.n_ctl = (int)(cfg->control_latency / dt); P.n_pd = (int)(cfg->pd_latency / dt);
-        P.a_ctl = (float)((cfg->control_latency - P.n_ctl * dt) / dt); P.a_pd = (float)((cfg->pd_latency - P.n_pd * dt) / dt);
+        P.ring_depth = sc.depth;
+        P.n_ctl = sc.n_ctl; P.n_pd = sc.n_pd; P.a_ctl = sc.a_ctl; P.a_pd = sc.a_pd;
         P.lat_ctl = (float)cfg->control_latency; P.lat_pd = (float)cfg->pd_latency;
         for (int k = 0; k < 5; k++) P.noise_sd[k] = (float)cfg->noise_stdev[k];
-        const size_t words = cfg->num_motors == 18 ? HW_WORDS_ARM : HW_WORDS;
-        CK(cudaMalloc(&s->d_ring, (size_t)P.ring_depth * words * N * sizeof(float)));
-        CK(cudaMemset(s->d_ring, 0, (size_t)P.ring_depth * words * N * sizeof(float)));
-        CK(cudaMalloc(&s->d_snap_ring, (size_t)s->nsnap * P.ring_depth * words * sizeof(float)));
-        CK(cudaMemset(s->d_snap_ring, 0, (size_t)s->nsnap * P.ring_depth * words * sizeof(float)));
-        P.ring = s->d_ring; P.snap_ring = s->d_snap_ring;
+        if (mem.zeroed(&P.ring, (size_t)sc.depth * sc.words * N) || mem.zeroed(&P.snap_ring, (size_t)s->nsnap * sc.depth * sc.words))
+            return REXSIM_ERR_CUDA;
     }
-    s->A = rexsim_action_dim(cfg->task, cfg->signal); s->O = rexsim_obs_dim(cfg->task, cfg->num_motors);
-    CK(cudaMalloc(&s->d_act, (size_t)N * s->A * sizeof(float)));
-    CK(cudaMalloc(&s->d_out, (size_t)rexsim_host_out_bytes(s)));
-    CK(cudaMemset(s->d_out, 0, (size_t)rexsim_host_out_bytes(s)));
     if (cfg->terrain == REXSIM_TERRAIN_RANDOM) {
         // vertical centring of each field: btHeightfieldTerrainShape local origin = (min+max)/2
         std::vector<float> h((size_t)65536), zo(cfg->nfields), zr(2 * (size_t)cfg->nfields);
@@ -172,22 +155,16 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
             zo[f] = (float)(0.5 * ((double)lo + (double)hi));
             zr[2 * f] = lo - zo[f]; zr[2 * f + 1] = hi - zo[f];
         }
-        CK(cudaMalloc(&s->d_zoff, cfg->nfields * sizeof(float)));
-        CK(cudaMemcpy(s->d_zoff, zo.data(), cfg->nfields * sizeof(float), cudaMemcpyHostToDevice));
-        CK(cudaMalloc(&s->d_zrange, 2 * cfg->nfields * sizeof(float)));
-        CK(cudaMemcpy(s->d_zrange, zr.data(), 2 * cfg->nfields * sizeof(float), cudaMemcpyHostToDevice));
+        if (mem.zeroed(&zoff, zo.size()) || mem.zeroed(&s->zrange, zr.size())) return REXSIM_ERR_CUDA;
+        CK(cudaMemcpy(zoff, zo.data(), zo.size() * sizeof(float), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(s->zrange, zr.data(), zr.size() * sizeof(float), cudaMemcpyHostToDevice));
     }
-    s->P.model = s->d_model; s->P.sf = s->d_sf; s->P.si = s->d_si;
-    s->P.snap_f = s->d_snap_f; s->P.snap_i = s->d_snap_i; s->P.field_zoff = s->d_zoff;
-    s->P.err = s->d_err; s->P.cmd_out = s->d_cmd;
-    s->P.cost = s->d_cost; s->P.perm = nullptr;
-    s->P.launched = s->launched;
+    P.model = model; P.snap_f = snap_f; P.snap_i = snap_i; P.field_zoff = zoff;
+    P.launched = s->launched;
     // settled reset snapshots: Rex.Reset's 100 + 0.5/dt holding sub-steps (rex.py:314-323), once per field
     for (int f = 0; f < s->nsnap; f++) {
-        s->P.settle_snapshot = f;
-        cudaError_t e = launch_settle(s->P, s->d_snap_f, s->d_snap_i, 0);
-        if (e != cudaSuccess) return cuda_fail(e, "settle launch");
-        s->launches++;
+        P.settle_snapshot = f;
+        if ((rc = enqueue(s, launch_settle(P, snap_f, snap_i, 0), "settle launch"))) return rc;
     }
     CK(cudaDeviceSynchronize());
     guard.s = nullptr;
@@ -197,10 +174,7 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
 
 void rexsim_destroy(RexSim* s) {
     if (!s) return;
-    cudaFree(s->d_model); cudaFree(s->d_sf); cudaFree(s->d_si); cudaFree(s->d_snap_f); cudaFree(s->d_snap_i);
-    cudaFree(s->d_ring); cudaFree(s->d_snap_ring);
-    cudaFree(s->d_zoff); cudaFree(s->d_err); cudaFree(s->d_cmd); cudaFree(s->d_act); cudaFree(s->d_out); cudaFree(s->d_perm); cudaFree(s->d_cost); cudaFree(s->d_hist);
-    cudaFree(s->d_zrange); cudaFree(s->d_rt);
+    s->mem.release();
     delete s;
 }
 
@@ -208,18 +182,10 @@ int rexsim_step(RexSim* s, const float* actions, float* obs, float* reward, uint
     if (!s || !actions || !obs || !reward || !done) return fail(REXSIM_ERR_INVALID, "null argument");
     Params P = s->P;
     P.actions = actions; P.obs = obs; P.reward = reward; P.done = done;
-    cudaError_t e = launch_step(P, (cudaStream_t)stream);
-    if (e != cudaSuccess) return cuda_fail(e, "step launch");
-    s->launches++;
-    return REXSIM_OK;
+    return enqueue(s, launch_step(P, (cudaStream_t)stream), "step launch");
 }
 
-static size_t out_done_offset(const RexSim* s) { return ((size_t)s->P.N * s->O + s->P.N) * sizeof(float); }
-static size_t out_err_offset(const RexSim* s) { return (out_done_offset(s) + (size_t)s->P.N + 3) & ~(size_t)3; }
-int64_t rexsim_host_out_bytes(const RexSim* s) {
-    if (!s) return 0;
-    return (int64_t)(out_err_offset(s) + sizeof(int32_t) + 8);      // + 8 flag bytes the kernel sets directly on the zero-copy path
-}
+int64_t rexsim_host_out_bytes(const RexSim* s) { return s ? (int64_t)host_block(s->P.N, s->O).bytes : 0; }
 // true when p is page-locked host memory the device can address directly (UVA: same pointer value on both sides)
 static bool device_can_address(const void* p) {
     cudaPointerAttributes at;
@@ -230,32 +196,31 @@ int rexsim_step_host(RexSim* s, const float* h_actions, void* h_out, void* strea
     if (!s || !h_actions || !h_out) return fail(REXSIM_ERR_INVALID, "null argument");
     cudaStream_t st = (cudaStream_t)stream;
     const size_t N = s->P.N;
+    const HostBlock hb = host_block(N, s->O);
     Params P = s->P;
     // Small batches with pinned buffers: the kernel reads the actions from, and writes its results into, the host block
     // directly (zero-copy over PCIe) -- no DMA launches at all: the error bits travel as flag bytes the kernel sets in the
     // block, the device-side aggregate is cleared BEFORE the kernel.  Large batches stage through device buffers so the kernel
     // never waits on PCIe.
     const bool zero_copy = N <= 16384 && device_can_address(h_actions) && device_can_address(h_out);   // queried per call (~1 us)
-    int32_t* h_err = reinterpret_cast<int32_t*>((char*)h_out + out_err_offset(s));
+    int32_t* h_err = reinterpret_cast<int32_t*>((char*)h_out + hb.err);
     uint8_t* h_flags = reinterpret_cast<uint8_t*>(h_err + 1);
     if (zero_copy) {
         memset(h_flags, 0, 8);
-        CK(cudaMemsetAsync(s->d_err + N, 0, sizeof(int32_t), st));    // the aggregate is per step on the host path
+        CK(cudaMemsetAsync(P.err + N, 0, sizeof(int32_t), st));       // the aggregate is per step on the host path
         P.actions = h_actions;
-        P.obs = (float*)h_out; P.reward = (float*)h_out + N * s->O; P.done = (uint8_t*)h_out + out_done_offset(s);
         P.err_host = h_flags;
     } else {
-        CK(cudaMemcpyAsync(s->d_act, h_actions, N * s->A * sizeof(float), cudaMemcpyHostToDevice, st));
-        P.actions = s->d_act;
-        P.obs = (float*)s->d_out; P.reward = (float*)s->d_out + N * s->O; P.done = s->d_out + out_done_offset(s);
+        CK(cudaMemcpyAsync(s->act, h_actions, N * s->A * sizeof(float), cudaMemcpyHostToDevice, st));
+        P.actions = s->act;
     }
-    cudaError_t e = launch_step(P, st);
-    if (e != cudaSuccess) return cuda_fail(e, "step launch");
-    s->launches++;
+    uint8_t* block = zero_copy ? (uint8_t*)h_out : s->out;
+    P.obs = (float*)block; P.reward = (float*)(block + hb.reward); P.done = block + hb.done;
+    if (int rc = enqueue(s, launch_step(P, st), "step launch")) return rc;
     if (!zero_copy) {
-        CK(cudaMemcpyAsync(h_out, s->d_out, out_err_offset(s), cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(h_err, s->d_err + N, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        CK(cudaMemsetAsync(s->d_err + N, 0, sizeof(int32_t), st));
+        CK(cudaMemcpyAsync(h_out, s->out, hb.err, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(h_err, P.err + N, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemsetAsync(P.err + N, 0, sizeof(int32_t), st));
     }
     CK(cudaStreamSynchronize(st));
     if (zero_copy) {
@@ -268,11 +233,9 @@ int rexsim_step_host(RexSim* s, const float* h_actions, void* h_out, void* strea
 
 int rexsim_rebalance(RexSim* s, void* stream) {
     if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
-    cudaError_t e = launch_rebalance(s->d_cost, s->P.N, s->d_hist, s->d_perm, (cudaStream_t)stream);
-    if (e != cudaSuccess) return cuda_fail(e, "rebalance launch");
-    s->launches += 3;
-    s->P.perm = s->d_perm;              // steps enqueued after this call use the new grouping
-    return REXSIM_OK;
+    const int rc = enqueue(s, launch_rebalance(s->P.cost, s->P.N, s->hist, s->perm, (cudaStream_t)stream), "rebalance launch", 3);
+    if (rc == REXSIM_OK) s->P.perm = s->perm;   // steps enqueued after this call use the new grouping
+    return rc;
 }
 
 int rexsim_reset(RexSim* s, const int32_t* idx, int32_t k, float* obs_out, void* stream) {
@@ -280,62 +243,54 @@ int rexsim_reset(RexSim* s, const int32_t* idx, int32_t k, float* obs_out, void*
     if (idx && k < 0) return fail(REXSIM_ERR_INVALID, "negative count");
     Params P = s->P;
     P.reset_idx = idx; P.reset_k = k;
-    cudaError_t e = launch_reset(P, obs_out, (cudaStream_t)stream);
-    if (e != cudaSuccess) return cuda_fail(e, "reset launch");
-    if (!idx || k > 0) s->launches++;
-    return REXSIM_OK;
+    return enqueue(s, launch_reset(P, obs_out, (cudaStream_t)stream), "reset launch", !idx || k > 0);
 }
 
 int rexsim_get_state(RexSim* s, float* out_f, int32_t* out_i, void* stream) {
     if (!s || !out_f || !out_i) return fail(REXSIM_ERR_INVALID, "null argument");
-    cudaError_t e = launch_get_state(s->P, out_f, out_i, (cudaStream_t)stream);
-    if (e != cudaSuccess) return cuda_fail(e, "get_state launch");
-    s->launches++;
-    return REXSIM_OK;
+    return enqueue(s, launch_get_state(s->P, out_f, out_i, (cudaStream_t)stream), "get_state launch");
 }
 int rexsim_set_state(RexSim* s, const float* in_f, void* stream) {
     if (!s || !in_f) return fail(REXSIM_ERR_INVALID, "null argument");
-    cudaError_t e = launch_set_state(s->P, in_f, (cudaStream_t)stream);
-    if (e != cudaSuccess) return cuda_fail(e, "set_state launch");
-    s->launches++;
-    return REXSIM_OK;
+    return enqueue(s, launch_set_state(s->P, in_f, (cudaStream_t)stream), "set_state launch");
 }
 int rexsim_state_buffers(RexSim* s, float** state_f, int32_t** state_i) {
     if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
-    if (state_f) *state_f = s->d_sf;
-    if (state_i) *state_i = s->d_si;
+    if (state_f) *state_f = s->P.sf;
+    if (state_i) *state_i = s->P.si;
     return REXSIM_OK;
 }
 int rexsim_history_buffer(RexSim* s, float** ring, int64_t* n_floats) {
     if (!s || !ring || !n_floats) return fail(REXSIM_ERR_INVALID, "null argument");
-    *ring = s->d_ring;
-    *n_floats = s->d_ring ? (int64_t)s->P.ring_depth * (s->P.cfg.num_motors == 18 ? HW_WORDS_ARM : HW_WORDS) * s->P.N : 0;
+    const SensorCfg sc = sensor_cfg(&s->P.cfg);
+    *ring = s->P.ring;
+    *n_floats = (int64_t)sc.depth * sc.words * s->P.N;       // depth 0: the sensor model is off
     return REXSIM_OK;
 }
 int rexsim_error_flags(RexSim* s, int32_t** err_flags) {
     if (!s || !err_flags) return fail(REXSIM_ERR_INVALID, "null argument");
-    *err_flags = s->d_err;
+    *err_flags = s->P.err;
     return REXSIM_OK;
 }
 int rexsim_clear_errors(RexSim* s, void* stream) {
     if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
-    CK(cudaMemsetAsync(s->d_err + s->P.N, 0, sizeof(int32_t), (cudaStream_t)stream));
+    CK(cudaMemsetAsync(s->P.err + s->P.N, 0, sizeof(int32_t), (cudaStream_t)stream));
     return REXSIM_OK;
 }
 int rexsim_last_command(RexSim* s, float** cmd) {
     if (!s || !cmd) return fail(REXSIM_ERR_INVALID, "null argument");
-    *cmd = s->d_cmd;
+    *cmd = s->P.cmd_out;
     return REXSIM_OK;
 }
 int rexsim_solver_cost(RexSim* s, int32_t** cost) {
     if (!s || !cost) return fail(REXSIM_ERR_INVALID, "null argument");
-    *cost = s->d_cost;
+    *cost = s->P.cost;
     return REXSIM_OK;
 }
 int rexsim_set_render_tables(RexSim* s, const float* rt, int32_t n_floats) {
     if (!s || !rt) return fail(REXSIM_ERR_INVALID, "null argument");
     if (n_floats != REXSIM_RT_FLOATS) return fail(REXSIM_ERR_MODEL, "render table size mismatch");
-    CK(cudaMemcpy(s->d_rt, rt, REXSIM_RT_FLOATS * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(s->rt, rt, REXSIM_RT_FLOATS * sizeof(float), cudaMemcpyHostToDevice));
     s->rt_set = true;
     return REXSIM_OK;
 }
@@ -347,10 +302,10 @@ int rexsim_render(RexSim* s, const int32_t* idx, int32_t k, int32_t width, int32
     if (!s->rt_set) return fail(REXSIM_ERR_INVALID, "render tables not set (rexsim_set_render_tables)");
     if (k == 0) return REXSIM_OK;
     if (!idx || !rgb) return fail(REXSIM_ERR_INVALID, "null argument");
-    cudaError_t e = launch_render(s->P, s->d_rt, s->d_zrange, idx, k, width, height, distance, yaw_deg, pitch_deg, rgb,
-                                  (cudaStream_t)stream, &s->launches);
-    if (e != cudaSuccess) return cuda_fail(e, "render launch");
-    return REXSIM_OK;
+    int launches = 0;
+    const cudaError_t e = launch_render(s->P, s->rt, s->zrange, idx, k, width, height, distance, yaw_deg, pitch_deg, rgb,
+                                        (cudaStream_t)stream, &launches);
+    return enqueue(s, e, "render launch", launches);
 }
 int64_t rexsim_launch_count(const RexSim* s) { return s ? s->launches : 0; }
 int rexsim_last_step_build(const RexSim* s, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor) {

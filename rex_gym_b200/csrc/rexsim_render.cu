@@ -362,7 +362,7 @@ __global__ void __launch_bounds__(RT_TILE * RT_TILE) render_kernel(const RenderA
 }
 
 cudaError_t launch_render(const Params& P, const float* rt, const float* zrange, const int32_t* idx, int k, int W, int H,
-                          float distance, float yaw_deg, float pitch_deg, uint8_t* rgb, cudaStream_t st, int64_t* launches) {
+                          float distance, float yaw_deg, float pitch_deg, uint8_t* rgb, cudaStream_t st, int* launches) {
     RenderArgs A;
     A.sf = P.sf; A.si = P.si; A.model = P.model; A.rt = rt; A.fields = P.cfg.fields; A.zoff = P.field_zoff; A.zrange = zrange;
     A.idx = idx; A.err = P.err; A.N = P.N; A.terrain = P.cfg.terrain; A.arm = P.cfg.num_motors == 18; A.toe_npts = P.cfg.toe_npts;

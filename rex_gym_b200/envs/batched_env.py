@@ -8,6 +8,7 @@ Reference interface mirrored (same names, argument meaning, error behaviour):
 One call = one kernel launch for all N environments; there is no CPU fallback.
 """
 import ctypes as C
+import functools
 import math
 
 import numpy as np
@@ -32,12 +33,20 @@ ERR_NONFINITE, ERR_JOINT_LIMIT, ERR_BODY_CONTACT, ERR_TILE_MISS, ERR_BAD_INDEX =
 SENSOR_NOISE_STDDEV = (0.0, 0.0, 0.0, 0.0, 0.0)      # rex_gym/model/rex.py:22, default of rex_gym_env.py:61
 
 
-class _DevArray(object):
-    """Expose a raw device pointer to torch through __cuda_array_interface__ (no copy, no ownership)."""
+_DevArray = _capi.DevArray       # the name tests/twin.py wraps the solver-cost buffer with
 
-    def __init__(self, ptr, shape, typestr, owner):
-        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (int(ptr), False), "version": 2}
-        self._owner = owner
+
+def _host_block_views(block, N, O):
+    """numpy views of the block rexsim_step_host fills (include/rexsim.h): obs [N][O] f32 | reward [N] f32 | done [N] u8 | pad to
+    4 bytes | int32 OR of the step's error bits | 8 scratch bytes."""
+    views, at = [], 0
+    for count, dtype in ((N * O, np.float32), (N, np.float32), (N, np.bool_), (1, np.int32)):
+        at = (at + 3) & ~3
+        nbytes = count * np.dtype(dtype).itemsize
+        views.append(block[at:at + nbytes].view(dtype))
+        at += nbytes
+    assert at + 8 == block.size, "host block layout differs from rexsim_host_out_bytes()"
+    return views[0].reshape(N, O), views[1], views[2], views[3]
 
 
 class _Info(object):
@@ -164,9 +173,11 @@ class BatchedRexEnv(object):
             tb = np.ascontiguousarray(tables)
             _capi.check(self._L.rexsim_create(C.byref(c), tb.ctypes.data, tb.size, C.byref(h)))
         self._h = h
+        self._dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
+        # every library call: on this env's device and torch's current stream there, a non-zero status raised (_capi.call)
+        self._call = functools.partial(_capi.call, self._dev_index)
         rt = np.ascontiguousarray(pack_render_tables(mark))
-        with torch.cuda.device(self.device):
-            _capi.check(self._L.rexsim_set_render_tables(self._h, rt.ctypes.data, rt.size))
+        self._call(self._L.rexsim_set_render_tables, self._h, rt.ctypes.data, rt.size, stream=False)
         self.obs_dim = self._L.rexsim_obs_dim(c.task, c.num_motors)
         self.action_dim = self._L.rexsim_action_dim(c.task, c.signal)
         N, O, A = self.num_envs, self.obs_dim, self.action_dim
@@ -177,32 +188,26 @@ class BatchedRexEnv(object):
         self._done_u8 = torch.zeros((N,), dtype=torch.uint8, device=dev)
         self._done = self._done_u8.view(torch.bool)
         # host path (numpy in / numpy out): ONE pinned block each way, filled by rexsim_step_host in one C call
-        nb_obs, nb_rew = N * O * 4, N * 4
-        nb_out = int(self._L.rexsim_host_out_bytes(self._h))
         self._h_act = torch.zeros((N, A), dtype=torch.float32).pin_memory()
-        self._h_out = torch.zeros((nb_out,), dtype=torch.uint8).pin_memory()
+        self._h_out = torch.zeros((int(self._L.rexsim_host_out_bytes(self._h)),), dtype=torch.uint8).pin_memory()
         self._h_act_np = self._h_act.numpy()
         self._h_act_ptr, self._h_out_ptr = self._h_act.data_ptr(), self._h_out.data_ptr()
-        ho = self._h_out.numpy()
-        self._h_obs = ho[:nb_obs].view(np.float32).reshape(N, O)
-        self._h_reward = ho[nb_obs:nb_obs + nb_rew].view(np.float32)
-        self._h_done = ho[nb_obs + nb_rew:nb_obs + nb_rew + N].view(np.bool_)
-        self._h_err = ho[nb_out - 12:nb_out - 8].view(np.int32)      # int32 OR of the step's error bits (8 scratch bytes follow)
-        self._dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        p = C.c_void_p()
+        self._h_obs, self._h_reward, self._h_done, self._h_err = _host_block_views(self._h_out.numpy(), N, O)
+
+        def view(p, shape, typestr):
+            return _capi.device_view(p.value, shape, typestr, self, dev)
+        p, q = C.c_void_p(), C.c_void_p()
         _capi.check(self._L.rexsim_error_flags(self._h, C.byref(p)))
-        self._err = torch.as_tensor(_DevArray(p.value, (N + 1,), "<i4", self), device=dev)
+        self._err = view(p, (N + 1,), "<i4")
         _capi.check(self._L.rexsim_last_command(self._h, C.byref(p)))
-        self._cmd = torch.as_tensor(_DevArray(p.value, (self.num_motors, N), "<f4", self), device=dev)
+        self._cmd = view(p, (self.num_motors, N), "<f4")
         nf, ni = C.c_int32(), C.c_int32()
         _capi.check(self._L.rexsim_state_words(C.byref(c), C.byref(nf), C.byref(ni)))
-        pf, pi = C.c_void_p(), C.c_void_p()
-        _capi.check(self._L.rexsim_state_buffers(self._h, C.byref(pf), C.byref(pi)))
-        self._state_f = torch.as_tensor(_DevArray(pf.value, (nf.value, N), "<f4", self), device=dev)
-        self._state_i = torch.as_tensor(_DevArray(pi.value, (ni.value, N), "<i4", self), device=dev)
-        pr, nr = C.c_void_p(), C.c_int64()
-        _capi.check(self._L.rexsim_history_buffer(self._h, C.byref(pr), C.byref(nr)))          # sensor history ring (None: model off)
-        self._ring = torch.as_tensor(_DevArray(pr.value, (nr.value,), "<f4", self), device=dev) if nr.value else None
+        _capi.check(self._L.rexsim_state_buffers(self._h, C.byref(p), C.byref(q)))
+        self._state_f, self._state_i = view(p, (nf.value, N), "<f4"), view(q, (ni.value, N), "<i4")
+        nr = C.c_int64()
+        _capi.check(self._L.rexsim_history_buffer(self._h, C.byref(p), C.byref(nr)))           # sensor history ring (None: model off)
+        self._ring = view(p, (nr.value,), "<f4") if nr.value else None
         # spaces: raw task spaces, or the wrapper-visible ones when the training wrappers are fused in
         b = ACTION_BOUND[(task, signal_type)]
         if normalize:
@@ -230,14 +235,10 @@ class BatchedRexEnv(object):
             raise IndexError(index)
         return _EnvView(self, index % self.num_envs)
 
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
     def _maybe_rebalance(self):
         self._nsteps += 1
         if self._rebalance_every and self._nsteps % self._rebalance_every == 0:
-            with torch.cuda.device(self.device):
-                _capi.check(self._L.rexsim_rebalance(self._h, self._stream()))
+            self._call(self._L.rexsim_rebalance, self._h)
 
     def step(self, action):
         """BatchEnv.step (batch_env.py:63-90).  numpy in -> numpy out (host buffers: one rexsim_step_host call = H2D copy,
@@ -248,15 +249,8 @@ class BatchedRexEnv(object):
                 raise ValueError("Invalid action shape %s, expected %s" % (tuple(action.shape), (N, A)))
             if action.dtype != torch.float32 or not action.is_contiguous():
                 action = action.to(torch.float32).contiguous()
-            if torch.cuda.current_device() != self._dev_index:
-                with torch.cuda.device(self.device):
-                    rc = self._L.rexsim_step(self._h, action.data_ptr(), self._obs.data_ptr(), self._reward.data_ptr(),
-                                             self._done_u8.data_ptr(), self._stream())
-            else:
-                rc = self._L.rexsim_step(self._h, action.data_ptr(), self._obs.data_ptr(), self._reward.data_ptr(),
-                                         self._done_u8.data_ptr(), torch.cuda.current_stream().cuda_stream)
-            if rc:
-                _capi.check(rc)
+            self._call(self._L.rexsim_step, self._h, action.data_ptr(), self._obs.data_ptr(), self._reward.data_ptr(),
+                       self._done_u8.data_ptr())
             self._maybe_rebalance()
             return self._obs, self._reward, self._done, _Info(self)
         a = np.asarray(action, dtype=np.float32)
@@ -265,13 +259,7 @@ class BatchedRexEnv(object):
         if not np.isfinite(a).all():
             raise ValueError("Invalid action: non-finite values")
         np.copyto(self._h_act_np, a)
-        if torch.cuda.current_device() != self._dev_index:
-            with torch.cuda.device(self.device):
-                rc = self._L.rexsim_step_host(self._h, self._h_act_ptr, self._h_out_ptr, self._stream())
-        else:
-            rc = self._L.rexsim_step_host(self._h, self._h_act_ptr, self._h_out_ptr, torch.cuda.current_stream().cuda_stream)
-        if rc:
-            _capi.check(rc)
+        self._call(self._L.rexsim_step_host, self._h, self._h_act_ptr, self._h_out_ptr)
         self._maybe_rebalance()
         if self._h_err[0] & ERR_NONFINITE:        # the aggregate word is per step on this path (rexsim_step_host clears it)
             raise ValueError("Infinite observation encountered.")          # ConvertTo32Bit wrappers.py:522-523,542-543
@@ -280,34 +268,35 @@ class BatchedRexEnv(object):
     def step_into(self, action, obs, reward, done_u8):
         """Raw device form of step(): CUDA float32 action [N][A] in; obs [N][O], reward [N] (float32) and done [N] (uint8) are
         written into the caller's contiguous CUDA buffers (e.g. slices of a rollout).  One asynchronous kernel launch."""
-        with torch.cuda.device(self.device):
-            _capi.check(self._L.rexsim_step(self._h, action.data_ptr(), obs.data_ptr(), reward.data_ptr(), done_u8.data_ptr(), self._stream()))
+        self._call(self._L.rexsim_step, self._h, action.data_ptr(), obs.data_ptr(), reward.data_ptr(), done_u8.data_ptr())
         self._maybe_rebalance()
+
+    def _indices(self, indices, what):
+        """Host or device indices -> int32 CUDA tensor [k].  Host indices outside the batch raise IndexError here.  Device indices
+        are not inspected on the host: the kernels skip any index outside [0, N) and raise REXSIM_FLAG_BAD_INDEX in the aggregate
+        error word (check_errors() -> IndexError)."""
+        if isinstance(indices, torch.Tensor):
+            return indices.to(device=self.device, dtype=torch.int32).reshape(-1).contiguous()
+        ia = np.asarray(indices, dtype=np.int64).reshape(-1)
+        if ia.size and (ia.min() < 0 or ia.max() >= self.num_envs):
+            raise IndexError("%s index out of range" % what)
+        return torch.from_numpy(ia.astype(np.int32)).to(self.device)
 
     def reset(self, indices=None):
         """BatchEnv.reset (batch_env.py:92-109): observations of the reset environments."""
-        with torch.cuda.device(self.device):
-            if indices is None:
-                k, idx_ptr = self.num_envs, None
-            else:
-                if isinstance(indices, torch.Tensor):
-                    # device indices are not inspected on the host: the kernel skips any index outside [0, N) and raises
-                    # REXSIM_FLAG_BAD_INDEX in the aggregate error word (check_errors() -> IndexError); debug=True checks here
-                    idx = indices.to(device=self.device, dtype=torch.int32).contiguous()
-                    if self._debug and idx.numel() and (int(idx.min()) < 0 or int(idx.max()) >= self.num_envs):
-                        raise IndexError("reset index out of range")
-                else:
-                    ia = np.asarray(indices, dtype=np.int64).reshape(-1)
-                    if ia.size and (ia.min() < 0 or ia.max() >= self.num_envs):
-                        raise IndexError("reset index out of range")
-                    idx = torch.from_numpy(ia.astype(np.int32)).to(self.device)
-                k, idx_ptr = int(idx.numel()), idx.data_ptr()
-            out = torch.zeros((k, self.obs_dim), dtype=torch.float32, device=self.device)
-            if k > 0:
-                _capi.check(self._L.rexsim_reset(self._h, idx_ptr, k, out.data_ptr(), self._stream()))
-            if isinstance(indices, torch.Tensor):
-                return out
-            return out.cpu().numpy()
+        if indices is None:
+            k, idx_ptr = self.num_envs, None
+        else:
+            idx = self._indices(indices, "reset")
+            if self._debug and idx.numel() and (int(idx.min()) < 0 or int(idx.max()) >= self.num_envs):
+                raise IndexError("reset index out of range")       # debug=True inspects device indices too (one sync)
+            k, idx_ptr = int(idx.numel()), idx.data_ptr()
+        out = torch.zeros((k, self.obs_dim), dtype=torch.float32, device=self.device)
+        if k > 0:
+            self._call(self._L.rexsim_reset, self._h, idx_ptr, k, out.data_ptr())
+        if isinstance(indices, torch.Tensor):
+            return out
+        return out.cpu().numpy()
 
     def close(self):
         if not self._closed:
@@ -328,8 +317,7 @@ class BatchedRexEnv(object):
         N, nm = self.num_envs, self.num_motors
         f = torch.zeros((13 + 2 * nm, N), dtype=torch.float32, device=self.device)
         i = torch.zeros((4, N), dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            _capi.check(self._L.rexsim_get_state(self._h, f.data_ptr(), i.data_ptr(), self._stream()))
+        self._call(self._L.rexsim_get_state, self._h, f.data_ptr(), i.data_ptr())
         f, i = f.cpu().numpy(), i.cpu().numpy()
         return dict(pos=f[0:3].T.copy(), quat=f[3:7].T.copy(), linvel=f[7:10].T.copy(), angvel=f[10:13].T.copy(),
                     q=f[13:13 + nm].T.copy(), qd=f[13 + nm:13 + 2 * nm].T.copy(),
@@ -339,9 +327,8 @@ class BatchedRexEnv(object):
         N, nm = self.num_envs, self.num_motors
         f = np.concatenate([np.asarray(x, np.float32).reshape(N, -1).T for x in (pos, quat, linvel, angvel, q, qd)], axis=0)
         t = torch.from_numpy(np.ascontiguousarray(f)).to(self.device)
-        with torch.cuda.device(self.device):
-            _capi.check(self._L.rexsim_set_state(self._h, t.data_ptr(), self._stream()))
-            torch.cuda.current_stream(self.device).synchronize()
+        self._call(self._L.rexsim_set_state, self._h, t.data_ptr())
+        torch.cuda.current_stream(self.device).synchronize()
 
     def last_command(self):
         """[num_motors, N] motor commands of the last step (info['action'], rex_gym_env.py:414)."""
@@ -356,8 +343,7 @@ class BatchedRexEnv(object):
         reset index outside the batch; returns the remaining (informational) bits."""
         e = int(self._err[self.num_envs].item())
         if e:
-            with torch.cuda.device(self.device):
-                _capi.check(self._L.rexsim_clear_errors(self._h, self._stream()))
+            self._call(self._L.rexsim_clear_errors, self._h)
         if e & ERR_NONFINITE:
             raise ValueError("Infinite observation encountered.")
         if e & ERR_BAD_INDEX:
@@ -399,20 +385,13 @@ class BatchedRexEnv(object):
         image and check_errors() raises IndexError), as in reset()."""
         if not (1 <= int(width) <= 4096 and 1 <= int(height) <= 4096):
             raise ValueError("image sides must be 1..4096")
-        with torch.cuda.device(self.device):
-            if isinstance(indices, torch.Tensor):
-                idx = indices.to(device=self.device, dtype=torch.int32).reshape(-1).contiguous()
-            else:
-                ia = np.asarray(indices, dtype=np.int64).reshape(-1)
-                if ia.size and (ia.min() < 0 or ia.max() >= self.num_envs):
-                    raise IndexError("render index out of range")
-                idx = torch.from_numpy(ia.astype(np.int32)).to(self.device)
-            k = int(idx.numel())
-            out = torch.empty((k, int(height), int(width), 3), dtype=torch.uint8, device=self.device)
-            if k > 0:
-                _capi.check(self._L.rexsim_render(self._h, idx.data_ptr(), k, int(width), int(height), float(distance), float(yaw),
-                                                  float(pitch), out.data_ptr(), self._stream()))
-            return out
+        idx = self._indices(indices, "render")
+        k = int(idx.numel())
+        out = torch.empty((k, int(height), int(width), 3), dtype=torch.uint8, device=self.device)
+        if k > 0:
+            self._call(self._L.rexsim_render, self._h, idx.data_ptr(), k, int(width), int(height), float(distance), float(yaw),
+                       float(pitch), out.data_ptr())
+        return out
 
 
 class RexWalkBatchEnv(BatchedRexEnv):
