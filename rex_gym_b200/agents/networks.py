@@ -13,16 +13,23 @@ from . import tf_checkpoint as tfc
 from .normalize import StreamingNormalize
 
 _TF = "network/rnn/"
-_TF_NAMES = (("pW1", "policy/fully_connected/weights"), ("pb1", "policy/fully_connected/biases"),
-             ("pW2", "policy/fully_connected_1/weights"), ("pb2", "policy/fully_connected_1/biases"),
-             ("pW3", "policy/fully_connected_2/weights"), ("pb3", "policy/fully_connected_2/biases"), ("logstd", "policy/logstd"),
-             ("vW1", "value/fully_connected/weights"), ("vb1", "value/fully_connected/biases"),
-             ("vW2", "value/fully_connected_1/weights"), ("vb2", "value/fully_connected_1/biases"),
-             ("vW3", "value/fully_connected_2/weights"), ("vb3", "value/fully_connected_2/biases"))
-
-
-def _pad4(n):
-    return (n + 3) & ~3
+POLICY, VALUE = 0, 1
+# the parameter block in its order (include/rexsim_agent.h): key, block, TF variable name under _TF, shape from (O, A, H1, H2)
+_PARAMS = (
+    ("pW1", POLICY, "policy/fully_connected/weights", lambda O, A, H1, H2: (O, H1)),
+    ("pb1", POLICY, "policy/fully_connected/biases", lambda O, A, H1, H2: (H1,)),
+    ("pW2", POLICY, "policy/fully_connected_1/weights", lambda O, A, H1, H2: (H1, H2)),
+    ("pb2", POLICY, "policy/fully_connected_1/biases", lambda O, A, H1, H2: (H2,)),
+    ("pW3", POLICY, "policy/fully_connected_2/weights", lambda O, A, H1, H2: (H2, A)),
+    ("pb3", POLICY, "policy/fully_connected_2/biases", lambda O, A, H1, H2: (A,)),
+    ("logstd", POLICY, "policy/logstd", lambda O, A, H1, H2: (A,)),
+    ("vW1", VALUE, "value/fully_connected/weights", lambda O, A, H1, H2: (O, H1)),
+    ("vb1", VALUE, "value/fully_connected/biases", lambda O, A, H1, H2: (H1,)),
+    ("vW2", VALUE, "value/fully_connected_1/weights", lambda O, A, H1, H2: (H1, H2)),
+    ("vb2", VALUE, "value/fully_connected_1/biases", lambda O, A, H1, H2: (H2,)),
+    ("vW3", VALUE, "value/fully_connected_2/weights", lambda O, A, H1, H2: (H2, 1)),
+    ("vb3", VALUE, "value/fully_connected_2/biases", lambda O, A, H1, H2: (1,)),
+)
 
 
 class ForwardGaussianPolicy(object):
@@ -73,39 +80,27 @@ class ForwardGaussianPolicy(object):
             vW3=xavier(H2, 1), vb3=np.zeros(1)))
 
     # ---- parameters ----------------------------------------------------------------------------------------------
-    def _shapes(self):
-        O, A, H1, H2 = self.O, self.A, self.H1, self.H2
-        return dict(pW1=(O, H1), pb1=(H1,), pW2=(H1, H2), pb2=(H2,), pW3=(H2, A), pb3=(A,), logstd=(A,),
-                    vW1=(O, H1), vb1=(H1,), vW2=(H1, H2), vb2=(H2,), vW3=(H2, 1), vb3=(1,))
+    def _layout(self):
+        """(key, shape, offset) of every parameter in the block: the policy's from 0, the value network's from n_policy."""
+        o = [0, self.n_policy]
+        for k, block, _, shape in _PARAMS:
+            s = shape(self.O, self.A, self.H1, self.H2)
+            yield k, s, o[block]
+            o[block] += int(np.prod(s))
 
     def set_weights(self, w):
-        shapes = self._shapes()
         block = np.zeros(self.n_policy + self.n_value, np.float32)
-        o = 0
-        for k in ("pW1", "pb1", "pW2", "pb2", "pW3", "pb3", "logstd"):
+        for k, s, o in self._layout():
             a = np.asarray(w[k], np.float32)
-            if a.shape != shapes[k]:
-                raise ValueError("weight %s has shape %s, expected %s" % (k, a.shape, shapes[k]))
-            block[o:o + a.size] = a.reshape(-1); o += a.size
-        o = self.n_policy
-        for k in ("vW1", "vb1", "vW2", "vb2", "vW3", "vb3"):
-            a = np.asarray(w[k], np.float32)
-            if a.shape != shapes[k]:
-                raise ValueError("weight %s has shape %s, expected %s" % (k, a.shape, shapes[k]))
-            block[o:o + a.size] = a.reshape(-1); o += a.size
+            if a.shape != s:
+                raise ValueError("weight %s has shape %s, expected %s" % (k, a.shape, s))
+            block[o:o + a.size] = a.reshape(-1)
         self._call(self._L.rexagent_set_params, self._h, block.ctypes.data, block.size, stream=False)
 
     def get_weights(self):
         block = np.zeros(self.n_policy + self.n_value, np.float32)
         self._call(self._L.rexagent_get_params, self._h, block.ctypes.data, block.size, stream=False)
-        out, o = {}, 0
-        shapes = self._shapes()
-        for k in ("pW1", "pb1", "pW2", "pb2", "pW3", "pb3", "logstd"):
-            n = int(np.prod(shapes[k])); out[k] = block[o:o + n].reshape(shapes[k]).copy(); o += n
-        o = self.n_policy
-        for k in ("vW1", "vb1", "vW2", "vb2", "vW3", "vb3"):
-            n = int(np.prod(shapes[k])); out[k] = block[o:o + n].reshape(shapes[k]).copy(); o += n
-        return out
+        return {k: block[o:o + int(np.prod(s))].reshape(s).copy() for k, s, o in self._layout()}
 
     @classmethod
     def from_tf_checkpoint(cls, directory_or_prefix, device="cuda:0"):
@@ -204,13 +199,13 @@ class ForwardGaussianPolicy(object):
 def read_tf_policy(directory_or_prefix):
     """(weights dict, (observ_count, observ_mean, observ_var_sum, reward_count, reward_mean, reward_var_sum)) from a TF checkpoint."""
     prefix = tfc.latest_checkpoint(directory_or_prefix) if os.path.isdir(directory_or_prefix) else directory_or_prefix
-    names = [_TF + n for _, n in _TF_NAMES] + ["normalize_observ/Variable", "normalize_observ/Variable_1", "normalize_observ/Variable_2",
+    names = [_TF + n for _, _, n, _ in _PARAMS] + ["normalize_observ/Variable", "normalize_observ/Variable_1", "normalize_observ/Variable_2",
                                                "normalize_reward/Variable", "normalize_reward/Variable_1", "normalize_reward/Variable_2"]
     v = tfc.load_variables(prefix, names)
     missing = [n for n in names if n not in v]
     if missing:
         raise ValueError("checkpoint %s is not a ForwardGaussianPolicy PPO checkpoint (missing %s)" % (prefix, missing[:3]))
-    w = {k: v[_TF + n] for k, n in _TF_NAMES}
+    w = {k: v[_TF + n] for k, _, n, _ in _PARAMS}
     filt = (int(v["normalize_observ/Variable"]), v["normalize_observ/Variable_1"], v["normalize_observ/Variable_2"],
             int(v["normalize_reward/Variable"]), float(v["normalize_reward/Variable_1"]), float(v["normalize_reward/Variable_2"]))
     return w, filt

@@ -16,9 +16,8 @@ def discounted_return(reward, length, discount):
     E, L = reward.shape
     length = length.to(device=reward.device, dtype=torch.int32).contiguous()
     out = torch.empty_strided(reward.shape, reward.stride(), dtype=torch.float32, device=reward.device)
-    with torch.cuda.device(reward.device):
-        _capi.check(_capi.load().rexagent_discounted_return(reward.data_ptr(), length.data_ptr(), E, L, reward.stride(0), reward.stride(1),
-                                                            float(discount), out.data_ptr(), _capi.stream_ptr(reward.device)))
+    _capi.call(reward.device.index, _capi.load().rexagent_discounted_return, reward.data_ptr(), length.data_ptr(), E, L,
+               reward.stride(0), reward.stride(1), float(discount), out.data_ptr())
     return out
 
 
@@ -29,9 +28,8 @@ def lambda_advantage(reward, value, length, discount):
     E, L = reward.shape
     length = length.to(device=reward.device, dtype=torch.int32).contiguous()
     out = torch.empty_strided(reward.shape, reward.stride(), dtype=torch.float32, device=reward.device)
-    with torch.cuda.device(reward.device):
-        _capi.check(_capi.load().rexagent_lambda_advantage(reward.data_ptr(), value.data_ptr(), length.data_ptr(), E, L, reward.stride(0),
-                                                           reward.stride(1), float(discount), out.data_ptr(), _capi.stream_ptr(reward.device)))
+    _capi.call(reward.device.index, _capi.load().rexagent_lambda_advantage, reward.data_ptr(), value.data_ptr(), length.data_ptr(),
+               E, L, reward.stride(0), reward.stride(1), float(discount), out.data_ptr())
     return out
 
 
@@ -43,7 +41,6 @@ def gae_segments(reward, value, done, discount, lam=1.0):
     reward, value = reward.contiguous(), value.contiguous()
     d8 = done.contiguous().view(torch.uint8) if done.dtype == torch.bool else done.to(torch.uint8).contiguous()
     ret, adv = torch.empty_like(reward), torch.empty_like(reward)
-    with torch.cuda.device(reward.device):
-        _capi.check(_capi.load().rexagent_gae_segments(reward.data_ptr(), value.data_ptr(), d8.data_ptr(), T, n, float(discount), float(lam),
-                                                       ret.data_ptr(), adv.data_ptr(), _capi.stream_ptr(reward.device)))
+    _capi.call(reward.device.index, _capi.load().rexagent_gae_segments, reward.data_ptr(), value.data_ptr(), d8.data_ptr(), T, n,
+               float(discount), float(lam), ret.data_ptr(), adv.data_ptr())
     return ret, adv

@@ -28,22 +28,29 @@ struct AgentDev {
 
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
-// one 1-D TMA bulk copy global -> shared (weights of one network), completion on an mbarrier with explicit parity
-__device__ __forceinline__ void tma_bulk_load(float* smem_dst, const float* gsrc, uint32_t bytes, uint64_t* bar, uint32_t parity) {
-    uint32_t bar_a = (uint32_t)__cvta_generic_to_shared(bar);
-    uint32_t dst_a = (uint32_t)__cvta_generic_to_shared(smem_dst);
-    if (threadIdx.x == 0) {
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // earlier generic-proxy reads of the buffer vs the async write
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"(bytes) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     ::"r"(dst_a), "l"(gsrc), "r"(bytes), "r"(bar_a) : "memory");
-    }
-    uint32_t ok = 0;
-    while (!ok) {
-        asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
-                     : "=r"(ok) : "r"(bar_a), "r"(parity) : "memory");
-    }
+// One network's packed parameter block (include/rexsim_agent.h), offsets in floats: W1 [O][H1], b1 [H1], W2 [H1][H2], b2 [H2],
+// W3 [H2][AO], b3 [AO], then the policy's logstd [A]; AO = A for the policy, 1 for the value network; padded to 4 floats.
+// I: the index type of the caller's address arithmetic -- int64_t in perform_kernel and the exported sizes, int in
+// perform_tc_kernel (the type that keeps each kernel's registers and instruction count at or below the hand-chained form).
+template <typename I> struct ParamLayout { I W1, b1, W2, b2, W3, b3, logstd, floats; };
+template <typename I>
+__host__ __device__ constexpr ParamLayout<I> param_layout(I O, I A, I H1, I H2, bool policy) {
+    const I AO = policy ? A : 1, b1 = O * H1, W2 = b1 + H1, b2 = W2 + H1 * H2, W3 = b2 + H2, b3 = W3 + H2 * AO, ls = b3 + AO;
+    return {0, b1, W2, b2, W3, b3, ls, (ls + (policy ? A : 0) + 3) & ~(I)3};
 }
+
+// filt = [observ mean O | observ var_sum O | reward mean | reward var_sum]: column j < O is observation j, column O the reward
+__device__ __forceinline__ float* filt_mean(float* filt, int O, int col) { return col < O ? &filt[col] : &filt[2 * O]; }
+__device__ __forceinline__ float* filt_var_sum(float* filt, int O, int col) { return col < O ? &filt[O + col] : &filt[2 * O + 1]; }
+// StreamingNormalize's 1 / (std + 1e-8), std = sqrt(var_sum / (count - 1) + 1e-4) (normalize.py:57-66, _std :131-144); 1 until
+// the count passes 1
+__device__ __forceinline__ float filter_inv_std(float var_sum, int64_t count) {
+    float inv = 1.f;
+    if (count > 1) inv = 1.f / (sqrtf(var_sum / (float)(count - 1) + 1e-4f) + 1e-8f);
+    return inv;
+}
+// after a filter update over n rows: both counts advance by n, the step counter by one (the next perform draws fresh noise)
+__device__ __forceinline__ void advance_counts(const AgentDev& D, int64_t n) { D.cnt[0] += n; D.cnt[1] += n; D.cnt[2] += 1; }
 
 struct PerformArgs {
     AgentDev D;
@@ -53,6 +60,73 @@ struct PerformArgs {
     uint32_t step, env_offset;
     float* action; float* mean; float* logprob; float* value; float* observ_copy;
 };
+
+// StreamingNormalize.transform constants of the O observation columns -> nrm = [mean O | 1 / (std + 1e-8) O]
+__device__ __forceinline__ void load_normaliser(const AgentDev& D, int O, float* nrm, int tid) {
+    if (tid < O) {
+        const int64_t cnt = D.cnt[0];
+        const float m = *filt_mean(D.filt, O, tid), vs = *filt_var_sum(D.filt, O, tid);
+        nrm[tid] = m; nrm[O + tid] = filter_inv_std(vs, cnt);
+    }
+}
+
+// normalised, clipped observations of the TM-env tile starting at env e0 -> xs [O][TM] (zeros past n), threads tid, tid + nt, ..
+// reading the [TM][O] block coalesced; the policy CTAs (net 0) copy the raw rows to observ_copy on the way
+template <int TM>
+__device__ __forceinline__ void load_obs_tile(const PerformArgs& P, int O, int net, const float* nrm, float* xs, int e0, int tid,
+                                              int nt) {
+    for (int i = tid; i < TM * O; i += nt) {
+        const int e = i / O, o = i - e * O;
+        float v = 0.f;
+        if (e0 + e < P.n) {
+            v = P.observ[(size_t)(e0 + e) * O + o];
+            if (net == 0 && P.observ_copy) P.observ_copy[(size_t)(e0 + e) * O + o] = v;
+        }
+        v = (v - nrm[o]) * nrm[O + o];
+        v = fminf(fmaxf(v, -P.D.cfg.observ_clip), P.D.cfg.observ_clip);
+        xs[o * TM + e] = v;
+    }
+}
+
+// one env's outputs from its head sums s (b3 included): the value (net 1), or per action tanh -> mean, the sample of
+// network.policy.sample (algorithm.py:116) when training, and the diag-normal log-density (net 0).  AC: the head width at
+// compile time; 0 = the first A of s[AG_MAX_A].
+template <int AC, int AU>
+__device__ __forceinline__ void head_outputs(const PerformArgs& P, int net, int A, int env, uint32_t step, const float (&s)[AU],
+                                             const float* logstd) {
+    if (net == 1) {
+        if (P.value) P.value[env] = s[0];
+    } else {
+        float lp = 0.f;
+#pragma unroll
+        for (int a = 0; a < AU; a++) {
+            if (AC || a < A) {
+                const float mu = tanhf(s[a]);
+                const float ls = logstd[a];
+                float act = mu, z = 0.f;
+                if (P.training) {
+                    const uint32_t genv = P.env_offset + (uint32_t)env;
+                    const float u1 = ((float)(rand_u32(P.seed, genv, step, 2 * a) >> 8) + 0.5f) * (1.0f / 16777216.0f);
+                    const float u2 = ((float)(rand_u32(P.seed, genv, step, 2 * a + 1) >> 8) + 0.5f) * (1.0f / 16777216.0f);
+                    z = sqrtf(-2.f * logf(u1)) * cospif(2.f * u2);
+                    act = fmaf(expf(ls), z, mu);
+                }
+                lp += -0.5f * z * z - ls - 0.9189385332046727f;
+                if (P.action) P.action[(size_t)env * A + a] = act;
+                if (P.mean) P.mean[(size_t)env * A + a] = mu;
+            }
+        }
+        if (P.logprob) P.logprob[env] = lp;
+    }
+}
+
+// dynamic shared memory of perform_kernel<TM>, offsets in floats after the weights of the larger network (wmax floats):
+// xs [AG_MAX_O][TM], h1 [H1][TM] (reused for the head partials [H2/4][TM][AO]), nrm [2][AG_MAX_O]
+struct PerformSmem { size_t xs, h1, nrm, bytes; };
+__host__ __device__ constexpr PerformSmem perform_smem(int wmax, int H1, int tm) {
+    const size_t xs = wmax, h1 = xs + (size_t)AG_MAX_O * tm, nrm = h1 + (size_t)H1 * tm;
+    return {xs, h1, nrm, (nrm + 2 * AG_MAX_O) * sizeof(float)};
+}
 
 // Persistent CTAs, blockIdx.y = network (0 policy, 1 value): weights -> shared memory once (TMA bulk copy), then for every
 // tile of TM envs:  normalise -> layer 1 (O x H1) -> layer 2 (H1 x H2: TM/16 envs x 4 outputs per thread, register tile) ->
@@ -67,23 +141,13 @@ __global__ void __launch_bounds__(512, 1) perform_kernel(const PerformArgs P) {
     const int O = c.obs_dim, A = c.action_dim, H1 = c.hidden1, H2 = c.hidden2;
     const int nt = blockDim.x, tid = threadIdx.x;
     const int net = blockIdx.y;
-    const int wmax = max(P.D.pol_floats, P.D.val_floats);
+    const PerformSmem S = perform_smem(max(P.D.pol_floats, P.D.val_floats), H1, TM);
     float* W = smem;                          // weights of this CTA's network
-    float* xs = W + wmax;                     // [O][TM] normalised observations
-    float* h1 = xs + AG_MAX_O * TM;           // [H1][TM]; reused for the head partials [H2/4][TM][AO]
-    float* nrm = h1 + (size_t)H1 * TM;        // [2][O] mean, 1/(std + 1e-8)
-    if (tid == 0) {
-        uint32_t bar_a = (uint32_t)__cvta_generic_to_shared(&bar);
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (tid < O) {   // StreamingNormalize.transform constants (normalize.py:57-66, _std :131-144)
-        const int64_t cnt = P.D.cnt[0];
-        float m = P.D.filt[tid], vs = P.D.filt[O + tid];
-        float inv = 1.f;
-        if (cnt > 1) inv = 1.f / (sqrtf(vs / (float)(cnt - 1) + 1e-4f) + 1e-8f);
-        nrm[tid] = m; nrm[O + tid] = inv;
-    }
+    float* xs = smem + S.xs;
+    float* h1 = smem + S.h1;
+    float* nrm = smem + S.nrm;
+    mbar_init(&bar);
+    load_normaliser(P.D, O, nrm, tid);
     __syncthreads();
     const int ntiles = (P.n + TM - 1) / TM;
     const uint32_t step = P.step + (uint32_t)P.D.cnt[2];
@@ -92,25 +156,16 @@ __global__ void __launch_bounds__(512, 1) perform_kernel(const PerformArgs P) {
     const bool l2_active = og < ngroups;              // the launch rounds the block up to TM threads for tiny networks
     const int AO = net == 0 ? A : 1;
     const int wfloats = net == 0 ? P.D.pol_floats : P.D.val_floats;
+    // no proxy fence before the copy: nothing in this CTA has touched W through the generic proxy yet
     tma_bulk_load(W, P.D.params + (net == 0 ? 0 : P.D.pol_floats), (uint32_t)wfloats * 4u, &bar, 0u);
-    const float* W1 = W; const float* b1 = W1 + O * H1;
-    const float* W2 = b1 + H1; const float* b2 = W2 + H1 * H2;
-    const float* W3 = b2 + H2; const float* b3 = W3 + H2 * AO;
-    const float* logstd = b3 + AO;                      // policy block only
+    const ParamLayout<int64_t> L = param_layout<int64_t>(O, A, H1, H2, net == 0);
+    const float* W1 = W + L.W1; const float* b1 = W + L.b1;
+    const float* W2 = W + L.W2; const float* b2 = W + L.b2;
+    const float* W3 = W + L.W3; const float* b3 = W + L.b3;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int e0 = tile * TM;
         __syncthreads();                                // previous tile's head is done with h1
-        for (int i = tid; i < TM * O; i += nt) {        // coalesced read of the [TM][O] block
-            const int e = i / O, o = i - e * O;
-            float v = 0.f;
-            if (e0 + e < P.n) {
-                v = P.observ[(size_t)(e0 + e) * O + o];
-                if (net == 0 && P.observ_copy) P.observ_copy[(size_t)(e0 + e) * O + o] = v;
-            }
-            v = (v - nrm[o]) * nrm[O + o];
-            v = fminf(fmaxf(v, -c.observ_clip), c.observ_clip);
-            xs[o * TM + e] = v;
-        }
+        load_obs_tile<TM>(P, O, net, nrm, xs, e0, tid, nt);
         __syncthreads();
         for (int i = tid; i < H1 * TM; i += nt) {       // layer 1
             const int k = i / TM, e = i - k * TM;
@@ -174,30 +229,7 @@ __global__ void __launch_bounds__(512, 1) perform_kernel(const PerformArgs P) {
 #pragma unroll
                 for (int a = 0; a < AG_MAX_A; a++) if (a < AO) s[a] += src[a];
             }
-            if (net == 1) {
-                if (P.value) P.value[env] = s[0];
-            } else {
-                float lp = 0.f;
-#pragma unroll
-                for (int a = 0; a < AG_MAX_A; a++) {
-                    if (a < A) {
-                        const float mu = tanhf(s[a]);
-                        const float ls = logstd[a];
-                        float act = mu, z = 0.f;
-                        if (P.training) {               // network.policy.sample (algorithm.py:116)
-                            const uint32_t genv = P.env_offset + (uint32_t)env;
-                            const float u1 = ((float)(rand_u32(P.seed, genv, step, 2 * a) >> 8) + 0.5f) * (1.0f / 16777216.0f);
-                            const float u2 = ((float)(rand_u32(P.seed, genv, step, 2 * a + 1) >> 8) + 0.5f) * (1.0f / 16777216.0f);
-                            z = sqrtf(-2.f * logf(u1)) * cospif(2.f * u2);
-                            act = fmaf(expf(ls), z, mu);
-                        }
-                        lp += -0.5f * z * z - ls - 0.9189385332046727f;     // diag-normal log-density
-                        if (P.action) P.action[(size_t)env * A + a] = act;
-                        if (P.mean) P.mean[(size_t)env * A + a] = mu;
-                    }
-                }
-                if (P.logprob) P.logprob[env] = lp;
-            }
+            head_outputs<0>(P, net, A, env, step, s, W + L.logstd);
         }
     }
 }
@@ -272,15 +304,10 @@ __global__ void __launch_bounds__(tc::THREADS, 1) perform_tc_kernel(const Perfor
     float* xs = b3 + 2 * AG_MAX_A;                          // [O][TM]
     float* nrm = xs + O * TM;                               // [2][O]
     const float* G = P.D.params + (net == 0 ? 0 : P.D.pol_floats);
-    const float* gW1 = G; const float* gb1 = gW1 + O * H1; const float* gW2 = gb1 + H1; const float* gb2 = gW2 + H1 * H2;
-    const float* gW3 = gb2 + H2; const float* gb3 = gW3 + H2 * AO;
-    if (tid < O) {   // StreamingNormalize.transform constants (normalize.py:57-66, _std :131-144)
-        const int64_t cnt = P.D.cnt[0];
-        float m = P.D.filt[tid], vs = P.D.filt[O + tid];
-        float inv = 1.f;
-        if (cnt > 1) inv = 1.f / (sqrtf(vs / (float)(cnt - 1) + 1e-4f) + 1e-8f);
-        nrm[tid] = m; nrm[O + tid] = inv;
-    }
+    const ParamLayout<int> L = param_layout(O, A, H1, H2, net == 0);
+    const float* gW1 = G + L.W1; const float* gb1 = G + L.b1; const float* gW2 = G + L.W2; const float* gb2 = G + L.b2;
+    const float* gW3 = G + L.W3; const float* gb3 = G + L.b3;
+    load_normaliser(P.D, O, nrm, tid);
     // weights: the small layers as they are, W2 transposed into the B operand form (rounded to tf32, zero rows up to NP)
     for (int i = tid; i < O * H1; i += THREADS) W1[i] = gW1[i];
     for (int i = tid; i < H1; i += THREADS) b1[i] = gb1[i];
@@ -306,22 +333,9 @@ __global__ void __launch_bounds__(tc::THREADS, 1) perform_tc_kernel(const Perfor
     const uint32_t a_addr = smem_u32(Asm) + (uint32_t)wg * 1024u, b_addr = smem_u32(Bsm);
     const int ntiles = (P.n + TM - 1) / TM;
     const uint32_t step = P.step + (uint32_t)P.D.cnt[2];
-    // normalised observations of a tile -> xs (coalesced read of the [TM][O] block).  Issued for the first tile here and for
-    // tile t + 1 right after the MMAs of tile t are issued, so the global loads are in flight while the tensor cores run.
-    auto load_obs = [&](int tile) {
-        const int e0 = tile * TM;
-        for (int i = tid; i < TM * O; i += THREADS) {
-            const int e = i / O, o = i - e * O;
-            float v = 0.f;
-            if (e0 + e < P.n) {
-                v = P.observ[(size_t)(e0 + e) * O + o];
-                if (net == 0 && P.observ_copy) P.observ_copy[(size_t)(e0 + e) * O + o] = v;
-            }
-            v = (v - nrm[o]) * nrm[O + o];
-            v = fminf(fmaxf(v, -c.observ_clip), c.observ_clip);
-            xs[o * TM + e] = v;
-        }
-    };
+    // a tile's observations -> xs: issued for the first tile here and for tile t + 1 right after the MMAs of tile t are issued,
+    // so the global loads are in flight while the tensor cores run
+    auto load_obs = [&](int tile) { load_obs_tile<TM>(P, O, net, nrm, xs, tile * TM, tid, THREADS); };
     if ((int)blockIdx.x < ntiles) load_obs(blockIdx.x);
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int e0 = tile * TM;
@@ -403,30 +417,7 @@ __global__ void __launch_bounds__(tc::THREADS, 1) perform_tc_kernel(const Perfor
                 float sh[AU];
 #pragma unroll
                 for (int a = 0; a < AU; a++) sh[a] = (AC || a < AO) ? b3[a] + (r ? s[1][a] : s[0][a]) : 0.f;
-                if (net == 1) {
-                    if (P.value) P.value[env] = sh[0];
-                } else {
-                    float lp = 0.f;
-#pragma unroll
-                    for (int a = 0; a < AU; a++) {
-                        if (AC || a < A) {
-                            const float mu = tanhf(sh[a]);
-                            const float ls = b3[AO + a];
-                            float act = mu, z = 0.f;
-                            if (P.training) {               // network.policy.sample (algorithm.py:116)
-                                const uint32_t genv = P.env_offset + (uint32_t)env;
-                                const float u1 = ((float)(rand_u32(P.seed, genv, step, 2 * a) >> 8) + 0.5f) * (1.0f / 16777216.0f);
-                                const float u2 = ((float)(rand_u32(P.seed, genv, step, 2 * a + 1) >> 8) + 0.5f) * (1.0f / 16777216.0f);
-                                z = sqrtf(-2.f * logf(u1)) * cospif(2.f * u2);
-                                act = fmaf(expf(ls), z, mu);
-                            }
-                            lp += -0.5f * z * z - ls - 0.9189385332046727f;     // diag-normal log-density
-                            if (P.action) P.action[(size_t)env * A + a] = act;
-                            if (P.mean) P.mean[(size_t)env * A + a] = mu;
-                        }
-                    }
-                    if (P.logprob) P.logprob[env] = lp;
-                }
+                head_outputs<AC>(P, net, A, env, step, sh, b3 + AO);
             }
         };
         if (net == 1) epilogue(std::integral_constant<int, 1>{});
@@ -446,8 +437,8 @@ __device__ __forceinline__ void filters_finalize(const AgentDev& D, int col, flo
     const int which = col < O ? 0 : 1;
     const int64_t cnt = D.cnt[which] + n_total;
     const float step = (float)cnt;
-    float* meanp = col < O ? &D.filt[col] : &D.filt[2 * O];
-    float* varp = col < O ? &D.filt[O + col] : &D.filt[2 * O + 1];
+    float* meanp = filt_mean(D.filt, O, col);
+    float* varp = filt_var_sum(D.filt, O, col);
     float new_mean = *meanp + s1 / step;
     if (cnt <= 1) new_mean = first_value;                                   // tf.cond(count > 1, new_mean, value[0])
     *varp += s2 - s1 * (s1 / step);
@@ -460,7 +451,7 @@ __global__ void __launch_bounds__(256) experience_kernel(const ExperienceArgs P)
     __shared__ float mean_s[AG_MAX_O + 1];
     __shared__ int last;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid < C) mean_s[tid] = tid < O ? P.D.filt[tid] : P.D.filt[2 * O];
+    if (tid < C) mean_s[tid] = *filt_mean(P.D.filt, O, tid);
     __syncthreads();
     // each thread walks rows with a fixed stride; column sums kept per thread for its own column set
     for (int cidx = 0; cidx < C; cidx++) {
@@ -498,7 +489,7 @@ __global__ void __launch_bounds__(256) experience_kernel(const ExperienceArgs P)
     }
     __syncthreads();
     if (tid == 0) {
-        if (!P.sums_out) { P.D.cnt[0] += P.n; P.D.cnt[1] += P.n; P.D.cnt[2] += 1; }     // step counter: the next perform draws fresh noise
+        if (!P.sums_out) advance_counts(P.D, P.n);
         P.D.cnt[3] = 0;
     }
 }
@@ -509,14 +500,11 @@ __global__ void experience_finalize_kernel(const AgentDev D, const float* __rest
     const int O = D.cfg.obs_dim, tid = threadIdx.x;
     if (tid <= O) filters_finalize(D, tid, sums[2 * tid], sums[2 * tid + 1], n_total, tid < O ? observ[tid] : reward[0]);
     __syncthreads();
-    if (tid == 0) { D.cnt[0] += n_total; D.cnt[1] += n_total; D.cnt[2] += 1; }
+    if (tid == 0) advance_counts(D, n_total);
 }
 
 __global__ void transform_reward_kernel(const AgentDev D, const float* __restrict__ r, int n, float* __restrict__ out) {
-    const int O = D.cfg.obs_dim;
-    const int64_t cnt = D.cnt[1];
-    float inv = 1.f;
-    if (cnt > 1) inv = 1.f / (sqrtf(D.filt[2 * O + 1] / (float)(cnt - 1) + 1e-4f) + 1e-8f);
+    const float inv = filter_inv_std(*filt_var_sum(D.filt, D.cfg.obs_dim, D.cfg.obs_dim), D.cnt[1]);
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
         out[i] = fminf(fmaxf(r[i] * inv, -D.cfg.reward_clip), D.cfg.reward_clip);      // center=False, scale=True, clip=10
 }
@@ -611,7 +599,6 @@ static PerformTcKernel perform_tc_pick(const RexAgentConfig* c) {
     return perform_tc_kernel<0, 0>;
 }
 
-static int64_t pad4(int64_t n) { return (n + 3) & ~(int64_t)3; }
 static int check_cfg(const RexAgentConfig* c) {
     if (!c) return fail(REXSIM_ERR_INVALID, "null agent config");
     if (c->obs_dim <= 0 || c->obs_dim > AG_MAX_O || c->action_dim <= 0 || c->action_dim > AG_MAX_A)
@@ -645,19 +632,15 @@ static int row_scan(const float* reward, const float* value, const int32_t* leng
 extern "C" {
 
 int64_t rexagent_policy_floats(const RexAgentConfig* c) {
-    if (!c) return 0;
-    const int64_t O = c->obs_dim, A = c->action_dim, H1 = c->hidden1, H2 = c->hidden2;
-    return pad4(O * H1 + H1 + H1 * H2 + H2 + H2 * A + A + A);
+    return c ? param_layout(c->obs_dim, c->action_dim, c->hidden1, c->hidden2, true).floats : 0;
 }
 int64_t rexagent_value_floats(const RexAgentConfig* c) {
-    if (!c) return 0;
-    const int64_t O = c->obs_dim, H1 = c->hidden1, H2 = c->hidden2;
-    return pad4(O * H1 + H1 + H1 * H2 + H2 + H2 + 1);
+    return c ? param_layout(c->obs_dim, c->action_dim, c->hidden1, c->hidden2, false).floats : 0;
 }
 
 static size_t perform_smem_bytes(const RexAgentConfig* c, int tm) {
-    const size_t wmax = (size_t)(rexagent_policy_floats(c) > rexagent_value_floats(c) ? rexagent_policy_floats(c) : rexagent_value_floats(c));
-    return (wmax + (size_t)AG_MAX_O * tm + (size_t)c->hidden1 * tm + 2 * AG_MAX_O) * sizeof(float);
+    const int64_t p = rexagent_policy_floats(c), v = rexagent_value_floats(c);
+    return perform_smem((int)(p > v ? p : v), c->hidden1, tm).bytes;
 }
 
 int rexagent_create(const RexAgentConfig* cfg, RexAgent** out) {
@@ -758,24 +741,22 @@ int rexagent_perform(RexAgent* a, const float* observ, int32_t n, int32_t traini
     PerformArgs P;
     P.D = a->D; P.observ = observ; P.n = n; P.training = training; P.seed = seed; P.step = step; P.env_offset = env_offset;
     P.action = action; P.mean = mean; P.logprob = logprob; P.value = value; P.observ_copy = observ_copy;
-    if (a->precision == 1) {          // wgmma path: 128-env tiles, one CTA per SM, networks in different CTAs (blockIdx.y)
-        const int half_tc = a->sm_count / 2 > 0 ? a->sm_count / 2 : 1;
-        const int nt = (n + tc::TM - 1) / tc::TM;
-        dim3 grid_tc(nt < half_tc ? nt : half_tc, 2);
-        perform_tc_pick(&a->D.cfg)<<<grid_tc, tc::THREADS, perform_tc_smem_bytes(&a->D.cfg), (cudaStream_t)stream>>>(P);
-        return enqueue(a, cudaGetLastError(), "perform launch");
-    }
     // one CTA per SM (the weights fill most of the shared memory); the two networks run in different CTAs (blockIdx.y).
-    // Small batches use 64-env tiles so that more SMs get a tile, large ones 128-env tiles (8 x 4 register tile per thread).
+    // The wgmma path always uses 128-env tiles; the fp32 kernel uses 64-env tiles on small batches so that more SMs get a
+    // tile, 128-env tiles (8 x 4 register tile per thread) on large ones.
     const int half = a->sm_count / 2 > 0 ? a->sm_count / 2 : 1;
-    const bool big = (n + 127) / 128 >= half;
-    const int tm = big ? 128 : 64;
+    const bool tc_path = a->precision == 1;
+    const int tm = tc_path || (n + 127) / 128 >= half ? 128 : 64;
     const int ntiles = (n + tm - 1) / tm;
-    dim3 grid(ntiles < half ? ntiles : half, 2);
-    int threads = 16 * (a->D.cfg.hidden2 / 4);
-    if (threads < tm) threads = tm;
-    if (big) perform_kernel<128><<<grid, threads, perform_smem_bytes(&a->D.cfg, 128), (cudaStream_t)stream>>>(P);
-    else perform_kernel<64><<<grid, threads, perform_smem_bytes(&a->D.cfg, 64), (cudaStream_t)stream>>>(P);
+    const dim3 grid(ntiles < half ? ntiles : half, 2);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (tc_path) {
+        perform_tc_pick(&a->D.cfg)<<<grid, tc::THREADS, perform_tc_smem_bytes(&a->D.cfg), st>>>(P);
+    } else {
+        const int threads = 16 * (a->D.cfg.hidden2 / 4) > tm ? 16 * (a->D.cfg.hidden2 / 4) : tm;
+        if (tm == 128) perform_kernel<128><<<grid, threads, perform_smem_bytes(&a->D.cfg, 128), st>>>(P);
+        else perform_kernel<64><<<grid, threads, perform_smem_bytes(&a->D.cfg, 64), st>>>(P);
+    }
     return enqueue(a, cudaGetLastError(), "perform launch");
 }
 int rexagent_experience(RexAgent* a, const float* observ, const float* reward, int32_t n, void* stream) {

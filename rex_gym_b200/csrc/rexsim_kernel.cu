@@ -46,23 +46,9 @@ __host__ __device__ constexpr bool pgs_replicated(int occ, bool arm, int terrain
 // model tables: one 1-D TMA bulk copy global -> shared per CTA (cp.async.bulk + mbarrier)
 // -------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_load_tables(float* smem_dst, const float* gsrc, uint32_t bytes, uint64_t* bar) {
-    uint32_t bar_a = (uint32_t)__cvta_generic_to_shared(bar);
-    uint32_t dst_a = (uint32_t)__cvta_generic_to_shared(smem_dst);
-    if (threadIdx.x == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    mbar_init(bar);
     __syncthreads();
-    if (threadIdx.x == 0) {
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"(bytes) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     ::"r"(dst_a), "l"(gsrc), "r"(bytes), "r"(bar_a) : "memory");
-    }
-    uint32_t ok = 0;
-    while (!ok) {
-        asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
-                     : "=r"(ok) : "r"(bar_a), "r"(0u) : "memory");
-    }
+    tma_bulk_load(smem_dst, gsrc, bytes, bar, 0u);
 }
 
 // -------------------------------------------------------------------------------------------------

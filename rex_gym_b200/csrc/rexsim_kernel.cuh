@@ -288,4 +288,28 @@ __device__ __forceinline__ double rand_uniform(uint64_t seed, uint32_t env, uint
     return a + (b - a) * u;
 }
 
+// ----- 1-D TMA bulk copy global -> shared, completion on an mbarrier ------------------------------------------
+// thread 0 initialises the barrier for one arrival; the CTA syncs before any thread waits on it
+__device__ __forceinline__ void mbar_init(uint64_t* bar) {
+    if (threadIdx.x == 0) {
+        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"((uint32_t)__cvta_generic_to_shared(bar)));
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+}
+// thread 0 arms the barrier with `bytes` and issues the copy; every thread waits for the phase with `parity` to complete
+__device__ __forceinline__ void tma_bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar, uint32_t parity) {
+    const uint32_t bar_a = (uint32_t)__cvta_generic_to_shared(bar);
+    const uint32_t dst_a = (uint32_t)__cvta_generic_to_shared(smem_dst);
+    if (threadIdx.x == 0) {
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"(bytes) : "memory");
+        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                     ::"r"(dst_a), "l"(gsrc), "r"(bytes), "r"(bar_a) : "memory");
+    }
+    uint32_t ok = 0;
+    while (!ok) {
+        asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
+                     : "=r"(ok) : "r"(bar_a), "r"(parity) : "memory");
+    }
+}
+
 }  // namespace rexsim

@@ -10,7 +10,10 @@ obs, reward, done, last_command, the error words, the whole SoA state and the se
 Random actions from reset rarely reach the generic solver path, so every configuration of tests/test_gpu_generic_path.CONFIGS
 also runs from that test's start states (body, arm and multi-limit contacts): 4 single sub-steps, then 4 control steps of the
 task configuration, hashing the solver cost as well.  Last, render_batch frames of a few envs of walk-ik on flat ground,
-turn-ik on the random heightfields and standup with the arm, with the default camera and at 97 x 61.
+turn-ik on the random heightfields and standup with the arm, with the default camera and at 97 x 61.  Then the agent kernels:
+every network of tests/test_gpu_agent_shapes.ROWS in its precision at that test's batch sizes (perform's four outputs, noise-free
+and sampled), the filter update (whole batch and partial + finalize: filter state and counters) and the reward transform, and
+the three scans on seeded inputs.
 Every later library is compared with the first: each array that is not bit-identical is reported, and for a frame the number
 of pixels that differ."""
 import hashlib
@@ -98,6 +101,44 @@ def render_cases(R, res, frames):
         env.close()
 
 
+def agent_cases(res):
+    """perform, experience, transform_reward of every tests/test_gpu_agent_shapes row; the three scans."""
+    import torch
+    import test_gpu_agent_shapes as S
+    from rex_gym_b200.agents import utility
+    sizes = S.batch_sizes(S._half())
+    for row in S.ROWS:
+        _, _, obs, nets = S._setup(row, max(sizes))
+        net = nets[-1]
+        x_all = torch.from_numpy(obs).cuda()
+        rew_all = torch.from_numpy(np.random.default_rng(3).normal(0.1, 0.5, max(sizes)).astype(np.float32)).cuda()
+        rec = res["agent-" + S.row_id(row)] = {}
+        for n in sizes:
+            for training in (False, True):
+                out = net.perform(x_all[:n], training=training, seed=S.SEED, step=S.STEP, env_offset=S.OFFSET)
+                for k, t in out.items():
+                    rec[f"n{n}_{'sampled' if training else 'mean'}_{k}"] = digest(t.cpu().numpy())
+        for n in sizes:
+            net.experience(x_all[:n], rew_all[:n])
+            rec[f"n{n}_experience"] = digest(np.r_[net._filt.cpu().numpy().view(np.int32), net._cnt.cpu().numpy().view(np.int32)])
+            S._experience_split(net, x_all[:n], rew_all[:n])
+            rec[f"n{n}_partial_finalize"] = digest(np.r_[net._filt.cpu().numpy().view(np.int32), net._cnt.cpu().numpy().view(np.int32)])
+            rec[f"n{n}_transform_reward"] = digest(net.transform_reward(rew_all[:n]).cpu().numpy())
+        for nt in nets:
+            nt.close()
+    rng = np.random.default_rng(17)
+    rec = res["agent-scans"] = {}
+    for L in S.SCAN_LENGTHS:
+        r, v = (torch.from_numpy(rng.normal(size=(300, L)).astype(np.float32)).cuda() for _ in range(2))
+        length = torch.from_numpy(rng.integers(0, L + 1, 300).astype(np.int32)).cuda()
+        rec[f"L{L}_return"] = digest(utility.discounted_return(r, length, 0.985).cpu().numpy())
+        rec[f"L{L}_advantage"] = digest(utility.lambda_advantage(r, v, length, 0.985).cpu().numpy())
+        v1 = torch.from_numpy(rng.normal(size=(L + 1, 300)).astype(np.float32)).cuda()
+        done = torch.from_numpy(rng.random((L, 300)) < 0.05).cuda()
+        ret, adv = utility.gae_segments(r.t().contiguous(), v1, done, 0.985, 0.95)
+        rec[f"L{L}_gae"] = digest(np.r_[ret.cpu().numpy(), adv.cpu().numpy()])
+
+
 def run(out):
     """Child process: every case with the library REXSIM_LIB names; {case: {step_array: sha256}} to `out`, the render frames
     beside it (frames.npz)."""
@@ -119,6 +160,7 @@ def run(out):
     generic_cases(res)
     frames = {}
     render_cases(R, res, frames)
+    agent_cases(res)
     with open(out, "w") as f:
         json.dump(res, f)
     np.savez(os.path.join(os.path.dirname(out), "frames.npz"), **frames)

@@ -26,7 +26,7 @@ CHECKPOINTS = ["gallop/ik", "gallop/ol", "standup/ol", "turn/ik", "turn/ol", "wa
 MEM_STEPS = 96
 FILTERS = ["global_step", "normalize_observ/Variable", "normalize_observ/Variable_1", "normalize_observ/Variable_2",
            "normalize_reward/Variable", "normalize_reward/Variable_1", "normalize_reward/Variable_2"]
-POLICY = [networks._TF + n for k, n in networks._TF_NAMES if not k.startswith("v")]
+POLICY = [networks._TF + n for _, block, n, _ in networks._PARAMS if block == networks.POLICY]
 
 
 def main():
