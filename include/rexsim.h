@@ -89,7 +89,8 @@ enum {
 typedef struct {
     int32_t num_envs;
     int32_t task, signal, terrain;
-    int32_t num_motors;               /* 12 (mark 'base') or 18 (mark 'arm': model table has REXSIM_MT_FLOATS_ARM floats) */
+    int32_t num_motors;               /* 12 (mark 'base') or 18 (mark 'arm': model table has REXSIM_MT_FLOATS_ARM floats; every
+                                         task but gallop, whose observation would carry the 18 motor angles) */
     int32_t action_repeat;
     int32_t solver_iterations;        /* int(300 / action_repeat) (rex_gym_env.py:25,184) */
     float sim_dt;                     /* control_time_step / action_repeat (unused: sim_dt_d is authoritative) */

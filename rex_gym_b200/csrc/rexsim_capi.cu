@@ -81,8 +81,8 @@ static int validate(const RexSimConfig* c) {
     if (c->num_envs <= 0) return fail(REXSIM_ERR_INVALID, "num_envs must be positive");
     if (c->task < 0 || c->task > 4 || c->signal < 0 || c->signal > 1) return fail(REXSIM_ERR_INVALID, "bad task/signal");
     if (c->num_motors != 12 && c->num_motors != 18) return fail(REXSIM_ERR_INVALID, "num_motors must be 12 (base) or 18 (arm)");
-    if (c->num_motors == 18 && !(c->task == REXSIM_TASK_STANDUP || (c->task == REXSIM_TASK_WALK && c->signal == REXSIM_SIGNAL_IK)))
-        return fail(REXSIM_ERR_UNSUPPORTED, "mark='arm' is built for the standup and walk-ik tasks");
+    if (c->num_motors == 18 && c->task == REXSIM_TASK_GALLOP)
+        return fail(REXSIM_ERR_UNSUPPORTED, "mark='arm' is built for every task but gallop (its observation would carry the 18 motor angles)");
     if (c->action_repeat <= 0 || c->solver_iterations <= 0 || !(c->sim_dt_d > 0)) return fail(REXSIM_ERR_INVALID, "bad time stepping");
     // the step kernel switches a motor off once its overheat count c > floor(1 / sim_dt) (rex.py:601-608); c is a 10-bit
     // saturating field, so at floor(1 / sim_dt) >= 1023 the protection could never fire

@@ -2107,8 +2107,9 @@ static cudaError_t launch_step_tsa(const Params& P, cudaStream_t st) {
 }
 template <int TASK, int SIGNAL>
 static cudaError_t launch_step_ts(const Params& P, cudaStream_t st) {
-    // the arm (mark='arm') is built for the standup task (BASELINE config 5) and the walk-ik task
-    constexpr bool HAS_ARM = (TASK == REXSIM_TASK_STANDUP || (TASK == REXSIM_TASK_WALK && SIGNAL == REXSIM_SIGNAL_IK));
+    // the arm (mark='arm') is built for every task but gallop: the reference's gallop observes all 18 motor angles, and the
+    // step and reset kernels fix the observation at obs_dim(TASK, 12)
+    constexpr bool HAS_ARM = TASK != REXSIM_TASK_GALLOP;
     if (P.cfg.num_motors == 18) {
         if (HAS_ARM) return launch_step_tsa<TASK, SIGNAL, HAS_ARM>(P, st);
         return cudaErrorNotSupported;

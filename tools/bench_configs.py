@@ -15,6 +15,9 @@ CONFIGS = [
     ("C4' turn-ik heightfield 65536 on one GPU", dict(task="turn", num_envs=65536, signal_type="ik", terrain_type="random", num_fields=64)),
     ("standup (base mark) 16384", dict(task="standup", num_envs=16384, signal_type="ol")),
     ("C5 standup arm (18-DOF) 16384 (per-GPU share of 131072 on 8)", dict(task="standup", num_envs=16384, signal_type="ol", mark="arm")),
+    ("turn-ik heightfield arm (18-DOF) 16384", dict(task="turn", num_envs=16384, signal_type="ik", terrain_type="random", num_fields=64, mark="arm")),
+    ("walk-ol flat arm (18-DOF) 16384", dict(task="walk", num_envs=16384, signal_type="ol", target_position=2.0, backwards=False, mark="arm")),
+    ("poses arm (18-DOF) 16384", dict(task="poses", num_envs=16384, signal_type="ik", mark="arm")),
 ]
 
 def main():
