@@ -105,6 +105,7 @@ def lib(f32=False):
         L.rexo_sensor_clear.argtypes = [C.c_void_p, C.c_int]
         L.rexo_sensor_push.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         L.rexo_sensor_delayed.argtypes = [C.c_void_p, C.c_int, C.c_double, C.c_void_p]
+        L.rexo_sensor_row.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         L.rexo_noise.restype = C.c_double
         L.rexo_noise.argtypes = [C.c_uint64] + [C.c_uint32] * 5
         L.rexo_mass_matrix.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
@@ -320,6 +321,16 @@ class OracleSim:
         obs = np.zeros(4 + MAXDOF)
         self.L.rexo_reward_done_obs(C.c_void_p(self.h), i, C.byref(r), C.byref(d), obs.ctypes.data_as(C.c_void_p))
         return r.value, bool(d.value), obs[:self.O]
+
+    def sensor_history(self, i):
+        """-> [len][3 nm + 7] env i's observation history, newest row first (rex.py:726-733 deque; q, qd, torque, quat, rpy rate)."""
+        w = 3 * self.nm + 7
+        row = np.zeros(w)
+        n = self.L.rexo_sensor_row(self.h, i, 0, row.ctypes.data)
+        out = np.zeros((n, w))
+        for k in range(n):
+            self.L.rexo_sensor_row(self.h, i, k, out[k].ctypes.data)
+        return out
 
     def substep(self, i, cmd):
         c = np.ascontiguousarray(cmd, np.float64)

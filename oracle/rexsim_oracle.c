@@ -1210,6 +1210,11 @@ void rexo_sensor_push(RexoSim* s, int i, const double* obs) { if (s->hist) hist_
 void rexo_sensor_delayed(RexoSim* s, int i, double latency, double* out) {
     if (s->hist) hist_delayed(&s->hist[i], latency, s->c.sim_dt, 3 * s->m.nmotor + 7, out);
 }
+int rexo_sensor_row(RexoSim* s, int i, int k, double* out) {
+    if (!s->hist) return 0;
+    if (k >= 0 && k < s->hist[i].len) memcpy(out, hist_at(&s->hist[i], k), sizeof(double) * (3 * s->m.nmotor + 7));
+    return s->hist[i].len;
+}
 int rexo_obs_dim(const RexoSim* s) { return s->obs_dim; }
 int rexo_action_dim(const RexoSim* s) { return s->act_dim; }
 RexoEnv* rexo_env(RexoSim* s, int i) { return &s->env[i]; }
