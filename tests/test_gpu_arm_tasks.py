@@ -4,187 +4,32 @@ The arm is a fifth limb on lane 0 of each env (rex_gym_b200/csrc/rexsim_arm.cuh)
 (rex_gym_env.py:363-367): the 12 leg commands come from the task, the 6 arm commands are the rest pose.  Gallop stays refused:
 the reference's gallop observes all 18 motor angles, and the step and reset kernels fix the observation at the 12 legs.
 
-ARM_INSTANCES is the arm half of the step kernel's dispatch image: 6 (task, signal) units x 2 terrains x the small and sensor
-builds (arm batches never take the 128-register build) = 24 rows.  The 8 rows of walk-ik and standup are run by
-test_gpu_builds::test_instance_against_the_oracle; test_arm_instance_against_the_oracle runs the other 16 here.
+The arm's step-kernel instances are rows of the dispatch image twin.INSTANCES: test_gpu_builds::test_instance_against_the_oracle
+runs them against the oracle with the rest of the image.
 """
-import json
-import os
-
 import numpy as np
 import pytest
-import torch
-from twin import (BUILDS, LAYOUT, STATE_KEYS, IterationBand, assert_draws, bound, force_build, launched, make_env, make_oracle,
-                  oracle_protection, protection, state_errors, sync)
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ARM_REST = np.array(json.load(open(os.path.join(HERE, "golden", "constants_golden.json")))["arm_poses"]["rest"], np.float32)
-UNITS = [("walk", "ik"), ("walk", "ol"), ("gallop", "ik"), ("gallop", "ol"), ("turn", "ik"), ("turn", "ol"), ("standup", "ol"), ("poses", "ik")]
-ALL_GROUPS = 0x7FFF                   # contact groups 0-8 of the legged robot and 9-14 of the arm links
-BUILDS_TEST = "test_gpu_builds::test_instance_against_the_oracle"
-
-#  task      signal terrain   build     run by
-ARM_INSTANCES = [
-    ("walk",    "ik", "plane",  "small",  BUILDS_TEST),
-    ("walk",    "ik", "plane",  "sensor", BUILDS_TEST),
-    ("walk",    "ik", "random", "small",  BUILDS_TEST),
-    ("walk",    "ik", "random", "sensor", BUILDS_TEST),
-    ("walk",    "ol", "plane",  "small",  None),
-    ("walk",    "ol", "plane",  "sensor", None),
-    ("walk",    "ol", "random", "small",  None),
-    ("walk",    "ol", "random", "sensor", None),
-    ("turn",    "ik", "plane",  "small",  None),
-    ("turn",    "ik", "plane",  "sensor", None),
-    ("turn",    "ik", "random", "small",  None),
-    ("turn",    "ik", "random", "sensor", None),
-    ("turn",    "ol", "plane",  "small",  None),
-    ("turn",    "ol", "plane",  "sensor", None),
-    ("turn",    "ol", "random", "small",  None),
-    ("turn",    "ol", "random", "sensor", None),
-    ("standup", "ol", "plane",  "small",  BUILDS_TEST),
-    ("standup", "ol", "plane",  "sensor", BUILDS_TEST),
-    ("standup", "ol", "random", "small",  BUILDS_TEST),
-    ("standup", "ol", "random", "sensor", BUILDS_TEST),
-    ("poses",   "ik", "plane",  "small",  None),
-    ("poses",   "ik", "plane",  "sensor", None),
-    ("poses",   "ik", "random", "small",  None),
-    ("poses",   "ik", "random", "sensor", None),
-]
-NEW = [r[:4] for r in ARM_INSTANCES if r[4] is None]
-NEW_PAIRS = [("walk", "ol"), ("turn", "ik"), ("turn", "ol"), ("poses", "ik")]
+from twin import (ARM_REST, ARM_UNITS, BUILDS, LAYOUT, STATE_KEYS, IterationBand, assert_draws, bound, create_status, launched,
+                  make_env, make_oracle, oracle_protection, protection, state_errors, window_twin)
 
 
-def _row_id(row):
-    task, sig, terrain, build = row[:4]
-    return "-".join([task, sig, "arm", terrain, build])
-
-
-def _create_status(task, sig):
-    """rexsim_create's status for an 18-motor config of (task, sig) handed a base-sized (952-float) model table: -2 once the
-    config is accepted (the table size is checked after validation and before any CUDA call), -4 when the arm is refused."""
-    import ctypes as C
-    from rex_gym_b200 import _capi
-    from rex_gym_b200.envs.batched_env import SIGNALS, TASKS
-    L = _capi.load()
-    cfg = _capi.RexSimConfig()
-    cfg.num_envs, cfg.task, cfg.signal, cfg.num_motors = 8, TASKS[task], SIGNALS[sig], 18
-    cfg.action_repeat, cfg.solver_iterations, cfg.sim_dt_d, cfg.toe_npts, cfg.gait_clock_scale = 5, 60, 0.001, 27, 1.0
-    h = C.c_void_p()
-    tb = np.zeros(952, np.float32)
-    return L.rexsim_create(C.byref(cfg), tb.ctypes.data, 952, C.byref(h)), L.rexsim_last_error()
-
-
-@pytest.mark.parametrize("task,sig", [u for u in UNITS if u[0] != "gallop"] + [("standup", "ik"), ("poses", "ol")])
+@pytest.mark.parametrize("task,sig", ARM_UNITS + [("standup", "ik"), ("poses", "ol")])
 def test_create_accepts_the_arm_for_every_task_but_gallop(task, sig):
     """CPU: an 18-motor config of any task but gallop passes validation (it fails on the model table size, -2)."""
-    rc, msg = _create_status(task, sig)
+    rc, msg = create_status(task, sig)
     assert rc == -2 and b"model table" in msg, (rc, msg)
 
 
 @pytest.mark.parametrize("sig", ["ik", "ol"])
 def test_create_still_refuses_gallop_with_the_arm(sig):
     """CPU: gallop with the arm is refused before any CUDA call, with the arm and gallop named in the message."""
-    rc, msg = _create_status("gallop", sig)
+    rc, msg = create_status("gallop", sig)
     assert rc == -4 and b"arm" in msg and b"gallop" in msg, (rc, msg)
 
 
-def test_arm_instance_table_is_the_arm_half_of_the_dispatch_image():
-    """CPU: the table above lists each arm instance once, for exactly the units the library accepts the arm for, on both
-    terrains and in the small and sensor builds; the rows this file does not run name an existing test."""
-    arm_units = [(t, s) for t, s in UNITS if _create_status(t, s)[0] == -2]
-    want = {(t, s, ter, b) for t, s in arm_units for ter in ("plane", "random") for b in ("small", "sensor")}
-    got = [r[:4] for r in ARM_INSTANCES]
-    assert len(got) == len(set(got)) == len(want) == 24
-    assert set(got) == want
-    assert len(NEW) == 16 and {(t, s) for t, s, _, _ in NEW} == set(NEW_PAIRS)
-    for row in ARM_INSTANCES:
-        if row[4] is not None:
-            mod, name = row[4].split("::")
-            assert ("def %s(" % name) in open(os.path.join(HERE, mod + ".py")).read(), row
-
-
-def _config(task, sig, terrain, build):
-    kw = dict(signal_type=sig, seed=13, max_episode_steps=15, mark="arm")    # short episodes: two in-kernel resets per env
-    if terrain == "random":
-        kw.update(terrain_type="random", num_fields=4)
-    if build == "sensor":
-        kw["control_latency"] = 0.0125                                      # a blend of two history rows, 12 sub-steps back
-    return kw
-
-
-def _masks(ora):
-    return np.array([ora.env(i).contact_mask & ALL_GROUPS for i in range(ora.N)])
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("row", NEW, ids=[_row_id(r) for r in NEW])
-def test_arm_instance_against_the_oracle(monkeypatch, row):
-    """One new arm instance, forced by force_build (the sensor build by its config; rexsim_last_step_build confirms which one ran
-    every step), against the oracle: 37 envs, 40 control steps of random actions inside the task's bound, auto-reset after 15
-    steps.  Done, draws and counters bit for bit after every step.  The state starts from the oracle's settled state and is
-    re-synchronised at each reset; between resets it stays within the bounds the walk-ik and standup arm rows meet
-    (5e-3 rad / 2e-3 m at the 90th percentile of the envs, none beyond 5e-2 / 5e-3), and every auto-reset lands within
-    test_reset_settle_and_draws' loosest bounds.  Every step's command block has 18 rows, the last six ARM_POSES['rest']; on flat
-    ground the 12 leg commands are within 5e-4 of the oracle's and the rewards within 5e-3.  Roll / pitch observations and the
-    contact masks of all 15 groups (arm links included) as in test_instance_against_the_oracle."""
-    task, sig, terrain, build = row
-    force_build(monkeypatch, build)
-    n, steps = 37, 40
-    kw = _config(task, sig, terrain, build)
-    env, ora = make_env(task, n, auto_reset=True, **kw), make_oracle(task, n, **kw)
-    env.reset(); ora.reset()
-    rough = terrain == "random"
-    sync(env, ora)
-    rng = np.random.default_rng(11)
-    b = bound(task, sig)
-    err_rp, contact_total, contact_bad = [], 0, 0
-    for k in range(steps):
-        a = rng.uniform(-b, b, size=(n, env.action_dim)).astype(np.float32)
-        og, rg, dg, info = env.step(a)
-        assert launched(env) == BUILDS[build], launched(env)
-        assert info[n - 1]["action"].shape == (18,)
-        np.testing.assert_array_equal(info[n - 1]["action"][12:], ARM_REST)
-        oc, rc, dc = ora.step(a)
-        np.testing.assert_array_equal(dg, dc, err_msg=f"done, step {k}")
-        cmd = env.last_command().cpu().numpy().T
-        np.testing.assert_array_equal(cmd[:, 12:], np.broadcast_to(ARM_REST, (n, 6)))
-        ocmd = np.array([np.array(ora.env(i).cmd[:12]) for i in range(n)])
-        idx = np.nonzero(dc)[0]
-        if len(idx):
-            oc[idx] = ora.reset(idx)                      # the oracle has no auto-reset: the same semantics by hand
-        sg, so = env.get_state(), ora.states()
-        assert_draws(env, ora, task)
-        fresh = np.zeros(n, bool)
-        fresh[idx] = True
-        eq, ep = state_errors(env, ora)
-        if not rough:
-            ep = np.maximum(ep, np.abs(sg["quat"] - so["quat"]).max(axis=1))
-        if len(idx):
-            # the in-kernel reset restarts from the CUDA settle: test_reset_settle_and_draws' loosest bounds (standup with the arm)
-            assert eq[idx].max() < 3e-2 and ep[idx].max() < 2e-3, f"reset, step {k}: {eq[idx].max():.2e} {ep[idx].max():.2e}"
-        eq, ep = eq[~fresh], ep[~fresh]
-        if len(eq):
-            assert np.percentile(eq, 90) < 5e-3 and np.percentile(ep, 90) < 2e-3, f"step {k}: {eq.max():.2e} {ep.max():.2e}"
-            assert eq.max() < 5e-2 and ep.max() < 5e-3, f"step {k}: {eq.max():.2e} {ep.max():.2e}"
-            # a re-synchronised sensor build reads its own settle's history rows for the first 3 control steps of an episode
-            ocmp = ~fresh & (sg["env_step_counter"] >= 3) if build == "sensor" else ~fresh
-            err_rp.append(np.abs(og[ocmp, :2] - oc[ocmp, :2]).max(axis=1))
-        if not rough:
-            assert np.abs(cmd[:, :12] - ocmd).max() < 5e-4, f"cmd step {k}"     # the controller half: fp32 IK / Bezier vs fp64
-            np.testing.assert_allclose(rg, rc, atol=5e-3, err_msg=f"reward, step {k}")
-        # the mask of contacts in the last sub-step: after a reset the CUDA path reports none yet, the oracle its settle's last
-        contact_total += (~fresh).sum()
-        contact_bad += ((_masks(ora) != (sg["contact_mask"] & ALL_GROUPS)) & ~fresh).sum()
-        if len(idx):
-            sync(env, ora, idx)
-    err_rp = np.concatenate(err_rp)
-    assert np.percentile(err_rp, 90) < 1e-3 and err_rp.max() < (2e-2 if rough else 5e-3), (np.percentile(err_rp, 90), err_rp.max())
-    assert contact_bad <= 0.02 * max(contact_total, 1), (contact_bad, contact_total)
-    assert env.check_errors() == 0
-    env.close()
-
-
-RESET_CASES = [(t, s, "plane") for t, s in NEW_PAIRS] + [("turn", "ik", "random")]
+# the arm units test_gpu_parity::test_reset_settle_and_draws does not reset (it has walk-ik and standup), and turn-ik on the bank
+RESET_CASES = [("walk", "ol", "plane"), ("turn", "ik", "plane"), ("turn", "ol", "plane"), ("poses", "ik", "plane"),
+               ("turn", "ik", "random")]
 
 
 @pytest.mark.gpu
@@ -260,18 +105,9 @@ def test_turn_ik_arm_heightfield_batch_against_the_oracle():
     other env and on that one until it leaves."""
     n, nw, steps = 16384, 48, 40
     w0 = n // 2 + 37
-    kw = dict(signal_type="ik", terrain_type="random", num_fields=64, mark="arm", normalize=True, seed=11)
-    env, ora = make_env("turn", n, **kw), make_oracle("turn", nw, env_offset=w0, **kw)
-    og = env.reset()[w0:w0 + nw]
-    oc = ora.reset()
+    env, ora, og, oc, acts = window_twin("turn", n, w0, nw, steps, settled=True, signal_type="ik", terrain_type="random",
+                                         num_fields=64, mark="arm", normalize=True, seed=11)
     np.testing.assert_allclose(og[:, :2], oc[:, :2], atol=2e-4)          # RangeNormalize'd roll / pitch
-    assert_draws(env, ora, "turn", window=w0)
-    st, so = env.get_state(), ora.states()
-    for k in STATE_KEYS:
-        st[k][w0:w0 + nw] = so[k]
-    env.set_state(*(st[k] for k in STATE_KEYS))
-    g = torch.Generator(device="cuda"); g.manual_seed(5)
-    acts = torch.rand((steps, n, env.action_dim), device="cuda", generator=g) * 2 - 1
     err, left = [], np.zeros(nw, bool)
     for k in range(steps):
         o, r, d, _ = env.step(acts[k])

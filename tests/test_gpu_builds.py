@@ -12,17 +12,18 @@
 twin.force_build(monkeypatch, "big" | "small") replaces the size rule (arm batches stay on the small build); the forced build is
 read on every step launch and does not touch the reset or settle kernels.
 
-INSTANCES is the table of reachable instances: 8 (task, signal) units x 2 terrains x 3 builds, plus the two arm units (walk-ik,
-standup) x 2 terrains x the small and sensor builds = 56 rows.  test_instance_against_the_oracle[<row id>] runs every row; the last
-column names the other tests of the suite that launch the same instance.
+twin.INSTANCES is the dispatch rule's whole image: 8 (task, signal) units x 2 terrains x 3 builds, plus the 6 arm units (every
+task but gallop) x 2 terrains x the small and sensor builds = 72 rows.  test_instance_against_the_oracle[<row id>] runs every row;
+ALSO names the other tests of the suite that launch the same instance.
 """
 import os
 
 import numpy as np
 import pytest
 import torch
-from twin import (BUILDS, STATE_KEYS, TOL_P, TOL_Q, assert_draws, bound, force_build, launched, make_env, make_oracle,
-                  one_step_is_tight, state_errors, sync, toe_masks)
+from twin import (ARM_REST, ARM_UNITS, BUILDS, BUILDS_OF, INSTANCES, TOL_P, TOL_Q, UNITS, assert_draws, bound, create_status,
+                  force_build, instance_config, launched, make_env, make_oracle, one_step_is_tight, row_id, state_errors, sync,
+                  toe_masks, window_twin)
 
 FR, HF, SA = "test_gpu_parity::test_free_running_rollout", "test_gpu_parity::test_heightfield_contact_parity", "test_gpu_parity::test_sensor_latency_and_noise"
 BL, WARP = "test_gpu_parity::test_baseline_size_batches_against_the_oracle", "test_gpu_parity::test_batches_that_do_not_fill_their_last_warp"
@@ -30,104 +31,40 @@ REGROUP, HOST = ("test_gpu_parity::test_warp_regrouping_does_not_change_any_resu
                  "test_gpu_parity::test_numpy_and_device_paths_agree_beyond_the_zero_copy_limit")
 NATURAL, SWITCH = "test_gpu_builds::test_heightfield_big_build_at_its_natural_size", "test_gpu_builds::test_the_dispatcher_switches_builds_at_its_thresholds"
 
-#  task      signal arm    terrain   build     also launched by
-INSTANCES = [
-    ("walk",    "ik", False, "plane",  "small",  (FR,)),
-    ("walk",    "ik", False, "plane",  "big",    (BL + "[C2]", REGROUP, HOST, SWITCH)),
-    ("walk",    "ik", False, "plane",  "sensor", (SA,)),
-    ("walk",    "ik", False, "random", "small",  (WARP,)),
-    ("walk",    "ik", False, "random", "big",    ()),
-    ("walk",    "ik", False, "random", "sensor", (SA,)),
-    ("walk",    "ol", False, "plane",  "small",  (FR,)),
-    ("walk",    "ol", False, "plane",  "big",    ()),
-    ("walk",    "ol", False, "plane",  "sensor", ()),
-    ("walk",    "ol", False, "random", "small",  ()),
-    ("walk",    "ol", False, "random", "big",    ()),
-    ("walk",    "ol", False, "random", "sensor", ()),
-    ("gallop",  "ik", False, "plane",  "small",  (FR,)),
-    ("gallop",  "ik", False, "plane",  "big",    ()),
-    ("gallop",  "ik", False, "plane",  "sensor", ()),
-    ("gallop",  "ik", False, "random", "small",  ()),
-    ("gallop",  "ik", False, "random", "big",    ()),
-    ("gallop",  "ik", False, "random", "sensor", ()),
-    ("gallop",  "ol", False, "plane",  "small",  (FR,)),
-    ("gallop",  "ol", False, "plane",  "big",    (BL + "[C3]",)),
-    ("gallop",  "ol", False, "plane",  "sensor", (SA,)),
-    ("gallop",  "ol", False, "random", "small",  ()),
-    ("gallop",  "ol", False, "random", "big",    ()),
-    ("gallop",  "ol", False, "random", "sensor", ()),
-    ("turn",    "ik", False, "plane",  "small",  (FR,)),
-    ("turn",    "ik", False, "plane",  "big",    ()),
-    ("turn",    "ik", False, "plane",  "sensor", (SA,)),
-    ("turn",    "ik", False, "random", "small",  (HF, BL + "[C4]")),
-    ("turn",    "ik", False, "random", "big",    (NATURAL, SWITCH)),
-    ("turn",    "ik", False, "random", "sensor", ()),
-    ("turn",    "ol", False, "plane",  "small",  (FR,)),
-    ("turn",    "ol", False, "plane",  "big",    ()),
-    ("turn",    "ol", False, "plane",  "sensor", ()),
-    ("turn",    "ol", False, "random", "small",  ()),
-    ("turn",    "ol", False, "random", "big",    ()),
-    ("turn",    "ol", False, "random", "sensor", ()),
-    ("standup", "ol", False, "plane",  "small",  (FR,)),
-    ("standup", "ol", False, "plane",  "big",    ()),
-    ("standup", "ol", False, "plane",  "sensor", ()),
-    ("standup", "ol", False, "random", "small",  ()),
-    ("standup", "ol", False, "random", "big",    ()),
-    ("standup", "ol", False, "random", "sensor", ()),
-    ("poses",   "ik", False, "plane",  "small",  (FR,)),
-    ("poses",   "ik", False, "plane",  "big",    ()),
-    ("poses",   "ik", False, "plane",  "sensor", (SA,)),
-    ("poses",   "ik", False, "random", "small",  ()),
-    ("poses",   "ik", False, "random", "big",    ()),
-    ("poses",   "ik", False, "random", "sensor", ()),
-    ("walk",    "ik", True,  "plane",  "small",  (FR,)),
-    ("walk",    "ik", True,  "plane",  "sensor", ()),
-    ("walk",    "ik", True,  "random", "small",  ()),
-    ("walk",    "ik", True,  "random", "sensor", ()),
-    ("standup", "ol", True,  "plane",  "small",  (FR, BL + "[C5]")),
-    ("standup", "ol", True,  "plane",  "sensor", (SA,)),
-    ("standup", "ol", True,  "random", "small",  ()),
-    ("standup", "ol", True,  "random", "sensor", ()),
-]
-UNITS = [("walk", "ik"), ("walk", "ol"), ("gallop", "ik"), ("gallop", "ol"), ("turn", "ik"), ("turn", "ol"), ("standup", "ol"), ("poses", "ik")]
-ARM_UNITS = [("walk", "ik"), ("standup", "ol")]          # launch_step_ts: HAS_ARM
-
-
-def _row_id(row):
-    task, sig, arm, terrain, build, _ = row
-    return "-".join([task, sig] + (["arm"] if arm else []) + [terrain, build])
+# the other tests of the suite that launch an instance
+ALSO = {
+    "walk-ik-plane-small": (FR,), "walk-ik-plane-big": (BL + "[C2]", REGROUP, HOST, SWITCH), "walk-ik-plane-sensor": (SA,),
+    "walk-ik-random-small": (WARP,), "walk-ik-random-sensor": (SA,),
+    "walk-ol-plane-small": (FR,),
+    "gallop-ik-plane-small": (FR,),
+    "gallop-ol-plane-small": (FR,), "gallop-ol-plane-big": (BL + "[C3]",), "gallop-ol-plane-sensor": (SA,),
+    "turn-ik-plane-small": (FR,), "turn-ik-plane-sensor": (SA,), "turn-ik-random-small": (HF, BL + "[C4]"),
+    "turn-ik-random-big": (NATURAL, SWITCH),
+    "turn-ol-plane-small": (FR,),
+    "standup-ol-plane-small": (FR,),
+    "poses-ik-plane-small": (FR,), "poses-ik-plane-sensor": (SA,),
+    "walk-ik-arm-plane-small": (FR,),
+    "standup-ol-arm-plane-small": (FR, BL + "[C5]"), "standup-ol-arm-plane-sensor": (SA,),
+}
 
 
 def test_instance_table_lists_every_reachable_instance():
-    """CPU: the table above is the dispatch rule's whole image -- no instance missing, none listed twice, no arm row on the big
-    build -- and every test it names exists."""
-    want = {(t, s, arm, ter, b) for arm, units in ((False, UNITS), (True, ARM_UNITS)) for t, s in units
-            for ter in ("plane", "random") for b in (("small", "sensor") if arm else ("small", "big", "sensor"))}
-    got = [r[:5] for r in INSTANCES]
-    assert len(got) == len(set(got)) == len(want) == 56
-    assert set(got) == want
+    """CPU: the dispatch image lists each instance once; its arm half covers exactly the units the library accepts the arm for
+    (rexsim_create, before any CUDA call); every row's build is one of its mark's; every test ALSO names exists."""
+    assert len(INSTANCES) == len(set(INSTANCES)) == 72
+    assert {(t, s) for t, s, arm, _, _ in INSTANCES if arm} == {u for u in UNITS if create_status(*u)[0] == -2} == set(ARM_UNITS)
+    assert all(b in BUILDS_OF["arm" if arm else "base"] for _, _, arm, _, b in INSTANCES)
+    ids = {row_id(r) for r in INSTANCES}
     here = os.path.dirname(os.path.abspath(__file__))
-    for row in INSTANCES:
-        for ref in row[5]:
+    for rid, refs in ALSO.items():
+        assert rid in ids, rid
+        for ref in refs:
             mod, name = ref.split("[")[0].split("::")
             assert ("def %s(" % name) in open(os.path.join(here, mod + ".py")).read(), ref
 
 
-def _config(task, sig, arm, terrain, build):
-    kw = dict(signal_type=sig, seed=13, max_episode_steps=15)         # short episodes: every env runs the in-kernel reset twice
-    if arm:
-        kw["mark"] = "arm"
-    if (task, sig) == ("gallop", "ol"):
-        kw.update(motor_kp_range=(0.8, 1.2), motor_kd_range=(0.01, 0.03))
-    if terrain == "random":
-        kw.update(terrain_type="random", num_fields=4)
-    if build == "sensor":
-        kw["control_latency"] = 0.0125                                # a blend of two history rows, 12 sub-steps back
-    return kw
-
-
 @pytest.mark.gpu
-@pytest.mark.parametrize("row", INSTANCES, ids=[_row_id(r) for r in INSTANCES])
+@pytest.mark.parametrize("row", INSTANCES, ids=[row_id(r) for r in INSTANCES])
 def test_instance_against_the_oracle(monkeypatch, row):
     """One instance, forced by force_build (the sensor build by its config; rexsim_last_step_build confirms which one ran
     every step), against the oracle: 37 envs (padding lanes in
@@ -138,13 +75,15 @@ def test_instance_against_the_oracle(monkeypatch, row):
       standup, arm            its standup bounds (5e-3 / 2e-3 at the 90th percentile), from the oracle's settled state;
       heightfields            test_heightfield_contact_parity's (1e-3 / 1e-3 at the 90th percentile, none beyond 2e-2 / 5e-3), from
                               the oracle's settled state (toes creep on block edges while settling);
-    roll / pitch observations as in test_baseline_size_batches_against_the_oracle, toe contact masks in 98 % of the samples that
-    are not the first of an episode.
-    Where the state starts from the oracle's, every auto-reset lands within the settle bounds and is re-synchronised."""
-    task, sig, arm, terrain, build, _ = row
+    roll / pitch observations as in test_baseline_size_batches_against_the_oracle, contact masks (the 9 groups of the legged
+    robot, all 15 with the arm) in 98 % of the samples that are not the first of an episode.
+    Where the state starts from the oracle's, every auto-reset lands within the settle bounds and is re-synchronised.
+    With the arm, every step's command block has 18 rows, the last six ARM_POSES['rest'] (rex_gym_env.py:363-367), and so
+    has info['action']."""
+    task, sig, arm, terrain, build = row
     force_build(monkeypatch, build)
     n, steps = 37, 40
-    kw = _config(task, sig, arm, terrain, build)
+    kw = instance_config(row)
     env, ora = make_env(task, n, auto_reset=True, **kw), make_oracle(task, n, **kw)
     env.reset(); ora.reset()
     rough, standup = terrain == "random", task == "standup" or arm
@@ -152,6 +91,7 @@ def test_instance_against_the_oracle(monkeypatch, row):
     tol_q, tol_p = (5e-3, 2e-3) if standup else (TOL_Q, TOL_P)                     # test_free_running_rollout
     max_q, max_p = (2e-2, 5e-3) if rough and not standup else (5e-2, 5e-3)
     ta = 5e-3 if (rough or standup) else 1e-3                                      # roll / pitch observations
+    groups = 0x7FFF if arm else 0x1FF                                              # contact groups 0-8, 9-14 the arm links
     if resync:
         sync(env, ora)
     rng = np.random.default_rng(11)
@@ -159,11 +99,15 @@ def test_instance_against_the_oracle(monkeypatch, row):
     err_rp, contact_total, contact_bad = [], 0, 0
     for k in range(steps):
         a = rng.uniform(-b, b, size=(n, env.action_dim)).astype(np.float32)
-        og, rg, dg, _ = env.step(a)
+        og, rg, dg, info = env.step(a)
         assert launched(env) == BUILDS[build], launched(env)
         oc, rc, dc = ora.step(a)
         np.testing.assert_array_equal(dg, dc, err_msg=f"done, step {k}")
-        cmd = env.last_command().cpu().numpy()[:12].T
+        cmd = env.last_command().cpu().numpy().T
+        if arm:
+            assert info[n - 1]["action"].shape == (18,)
+            np.testing.assert_array_equal(info[n - 1]["action"][12:], ARM_REST)
+            np.testing.assert_array_equal(cmd[:, 12:], np.broadcast_to(ARM_REST, (n, 6)))
         ocmd = np.array([np.array(ora.env(i).cmd[:12]) for i in range(n)])
         idx = np.nonzero(dc)[0]
         if len(idx):
@@ -187,14 +131,15 @@ def test_instance_against_the_oracle(monkeypatch, row):
             ocmp = cmp & (sg["env_step_counter"] >= 3) if (resync and build == "sensor") else cmp
             err_rp.append(np.abs(og[ocmp, :2] - oc[ocmp, :2]).max(axis=1))
         if not rough:
-            assert np.abs(cmd - ocmd).max() < 5e-4, f"cmd step {k}"     # the controller half: fp32 IK / Bezier vs fp64
+            assert np.abs(cmd[:, :12] - ocmd).max() < 5e-4, f"cmd step {k}"     # the controller half: fp32 IK / Bezier vs fp64
             rcmp = np.ones(n, bool)
             if task == "standup":      # the standup reward jumps by 1 where the base crosses z = 0.21 or the L1 distance 0.1
                 l1 = np.abs(so["pos"][:, 0]) + np.abs(so["pos"][:, 1]) + np.abs(0.21 - so["pos"][:, 2])
                 rcmp &= (np.abs(so["pos"][:, 2] - 0.21) > 2e-3) & (np.abs(l1 - 0.1) > 2e-3) & ~fresh
             np.testing.assert_allclose(rg[rcmp], rc[rcmp], atol=5e-3, err_msg=f"reward, step {k}")
         # the mask of contacts in the last sub-step: after a reset the CUDA path reports none yet, the oracle its settle's last
-        contact_total += (~fresh).sum(); contact_bad += ((toe_masks(ora) != sg["contact_mask"]) & ~fresh).sum()
+        omask = np.array([ora.env(i).contact_mask for i in range(n)]) & groups
+        contact_total += (~fresh).sum(); contact_bad += ((omask != sg["contact_mask"]) & ~fresh).sum()
         if resync and len(idx):
             sync(env, ora, idx)
     err_rp = np.concatenate(err_rp)
@@ -225,16 +170,8 @@ def test_heightfield_big_build_at_its_natural_size():
     C4 bounds, over 40 control steps."""
     n, w0, nw, steps = 32768, 32768 // 2 + 37, 48, 40
     assert -(-n // 32) > 4 * torch.cuda.get_device_properties(0).multi_processor_count       # really above the switch
-    kw = dict(signal_type="ik", terrain_type="random", num_fields=64, normalize=True, seed=11)
-    env, ora = make_env("turn", n, **kw), make_oracle("turn", nw, env_offset=w0, **kw)
-    env.reset(); ora.reset()
-    assert_draws(env, ora, "turn", window=w0)
-    st, so = env.get_state(), ora.states()
-    for k in STATE_KEYS:
-        st[k][w0:w0 + nw] = so[k]
-    env.set_state(*(st[k] for k in STATE_KEYS))
-    g = torch.Generator(device="cuda"); g.manual_seed(5)
-    acts = torch.rand((steps, n, env.action_dim), device="cuda", generator=g) * 2 - 1
+    env, ora, _, _, acts = window_twin("turn", n, w0, nw, steps, settled=True, signal_type="ik", terrain_type="random",
+                                       num_fields=64, normalize=True, seed=11)
     err, bad = [], 0
     for k in range(steps):
         o, r, d, _ = env.step(acts[k])

@@ -16,8 +16,8 @@ import math
 
 import numpy as np
 import pytest
-from twin import (ARM_MASK, BODY_BITS, FOLDED, NOISE, SUB, UPPER_BITS, IterationBand, compare_control_steps, compare_substeps,
-                  force_build, generic_path, limits, make_env, make_oracle, quat, rot, violated)
+from twin import (ARM_MASK, BODY_BITS, BUILDS_OF, FOLDED, NOISE, SUB, UPPER_BITS, IterationBand, compare_control_steps,
+                  compare_substeps, force_build, generic_path, limits, make_env, make_oracle, quat, rot, violated)
 
 N = 37
 
@@ -159,8 +159,7 @@ def test_scenarios_reach_the_generic_rows(mark, terrain):
     assert len(set(ids)) == (12 if mark == "arm" else 9)
 
 
-CONFIGS = [(m, t, b) for m, builds in (("base", ("small", "big", "sensor")), ("arm", ("small", "sensor")))
-           for t in ("plane", "random") for b in builds]
+CONFIGS = [(m, t, b) for m in ("base", "arm") for t in ("plane", "random") for b in BUILDS_OF[m]]
 
 
 @pytest.mark.gpu

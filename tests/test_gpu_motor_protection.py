@@ -17,8 +17,8 @@ import ctypes
 import numpy as np
 import pytest
 
-from twin import (BUILDS, NOISE, SUB, bound, force_build, launched, make_env, make_oracle, oracle_protection, protection,
-                  state_errors, sync)
+from twin import (BUILDS, BUILDS_OF, NOISE, SUB, bound, force_build, launched, make_env, make_oracle, oracle_protection,
+                  protection, state_errors, sync)
 
 N = 37
 SEEDED = np.array([i % 3 != 1 for i in range(N)])              # envs 0, 2, 3, 5, ..., 36 seeded; 1, 4, ..., 34 not
@@ -159,8 +159,8 @@ def test_oracle_switches_off_on_count_1023_at_the_largest_accepted_rate():
 
 
 # ---------------------------------------------------------------------------------------------------------------- GPU
-LEG_CONFIGS = [(s, t, b) for s in LEG_SCENARIOS for t in ("plane", "random") for b in ("small", "big", "sensor")]
-ARM_CONFIGS = [(s, t, b) for s in ARM_SCENARIOS for t in ("plane", "random") for b in ("small", "sensor")]
+LEG_CONFIGS = [(s, t, b) for s in LEG_SCENARIOS for t in ("plane", "random") for b in BUILDS_OF["base"]]
+ARM_CONFIGS = [(s, t, b) for s in ARM_SCENARIOS for t in ("plane", "random") for b in BUILDS_OF["arm"]]
 CONFIGS = LEG_CONFIGS + ARM_CONFIGS
 IDS = ["-".join(c) for c in CONFIGS]
 TIES = 2

@@ -14,8 +14,8 @@ import numpy as np
 import pybullet_memory
 import pytest
 import torch
-from twin import (LAYOUT, NOISE, STATE_KEYS, TOL_P, TOL_Q, IterationBand, assert_draws, bound, make_env, make_oracle,
-                  one_step_is_tight, oracle_protection, protection, solver_cost, state_errors, sync, toe_masks)
+from twin import (LAYOUT, NOISE, TOL_P, TOL_Q, IterationBand, assert_draws, bound, make_env, make_oracle, one_step_is_tight,
+                  oracle_protection, protection, solver_cost, state_errors, sync, toe_masks, window_twin)
 
 pytestmark = pytest.mark.gpu
 
@@ -396,21 +396,10 @@ def test_baseline_size_batches_against_the_oracle(name, task, n, kw):
     build; C4 (16 384 envs, below the heightfield switch at 16 896) and C5 (arm) run the 255-register 128-thread build
     (tests/test_gpu_builds.py covers the rest)."""
     w0, nw, steps = n // 2 + 37, 48, 40
-    common = dict(normalize=True, seed=11)
-    env = make_env(task, n, **common, **kw)
-    ora = make_oracle(task, nw, env_offset=w0, **common, **kw)
-    og = env.reset()[w0:w0 + nw]
-    oc = ora.reset()
     rough, arm = kw.get("terrain_type") == "random", kw.get("mark") == "arm"
+    # the arm starts both from the oracle's settled state (chaotic fold-down, see test_reset_settle_and_draws)
+    env, ora, og, oc, acts = window_twin(task, n, w0, nw, steps, settled=arm, normalize=True, seed=11, **kw)
     np.testing.assert_allclose(og[:, :2], oc[:, :2], atol=2e-5 if not (rough or arm) else 2e-4)      # RangeNormalize'd roll / pitch
-    assert_draws(env, ora, task, window=w0)
-    if arm:            # start both from the oracle's settled state (chaotic fold-down, see test_reset_settle_and_draws)
-        st, so = env.get_state(), ora.states()
-        for k in STATE_KEYS:
-            st[k][w0:w0 + nw] = so[k]
-        env.set_state(*(st[k] for k in STATE_KEYS))
-    g = torch.Generator(device="cuda"); g.manual_seed(5)
-    acts = torch.rand((steps, n, env.action_dim), device="cuda", generator=g) * 2 - 1
     err = []
     for k in range(steps):
         o, r, d, _ = env.step(acts[k])

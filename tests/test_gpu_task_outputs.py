@@ -7,7 +7,7 @@ the kernel's own SoA words and sensor-history ring, so no divergence enters the 
 
 CPU: the restatement reproduces what the fp64 oracle's step returned (and its reward_done_obs), from the oracle's own state, for
 every task and signal, both marks, normalize on and off, and the sensor configurations of test_gpu_parity.
-GPU: every step-kernel instance the dispatcher can launch (test_gpu_builds.INSTANCES and test_gpu_arm_tasks' arm rows), 300
+GPU: every step-kernel instance the dispatcher can launch (twin.INSTANCES), 300
 control steps of 37 envs without auto-reset, each output against the restatement of the kernel's words after every step, and
 every motor command against the oracle's controller fed the kernel's pre-step task words.
 """
@@ -17,11 +17,9 @@ import numpy as np
 import pytest
 import task_outputs as T
 import twin
-from twin import BUILDS, LAYOUT, NOISE, bound, force_build, launched, make_env, make_oracle
+from twin import ARM_UNITS, BUILDS, INSTANCES, LAYOUT, NOISE, UNITS, bound, force_build, launched, make_env, make_oracle, row_id
 
 EPS32 = float(np.finfo(np.float32).eps)
-UNITS = [("walk", "ik"), ("walk", "ol"), ("gallop", "ik"), ("gallop", "ol"), ("turn", "ik"), ("turn", "ol"), ("standup", "ol"), ("poses", "ik")]
-ARM_UNITS = [("walk", "ik"), ("walk", "ol"), ("turn", "ik"), ("turn", "ol"), ("standup", "ol"), ("poses", "ik")]
 MARGIN = 1e-5          # envs this close to a threshold of their termination or a jump of their reward: counted, not compared
 
 
@@ -106,19 +104,11 @@ def test_restatement_reproduces_the_oracle_with_the_sensor_model(case):
 
 
 # ---- GPU sweep ---------------------------------------------------------------------------------------------------------------
-def _sweep_rows():
-    from test_gpu_arm_tasks import NEW
-    from test_gpu_builds import INSTANCES
-    rows = [r[:5] for r in INSTANCES] + [(t, s, True, ter, b) for t, s, ter, b in NEW]
-    return [r + (k % 2 == 1,) for k, r in enumerate(rows)]        # every other row: normalize=True, actions beyond +-1
-
-
-SWEEP = _sweep_rows()
+SWEEP = [r + (k % 2 == 1,) for k, r in enumerate(INSTANCES)]        # every other row: normalize=True, actions beyond +-1
 
 
 def _row_id(row):
-    task, sig, arm, terrain, build, norm = row
-    return "-".join([task, sig] + (["arm"] if arm else []) + [terrain, build] + (["norm"] if norm else []))
+    return row_id(row[:5]) + ("-norm" if row[5] else "")
 
 
 def _sweep_config(task, sig, arm, terrain, build, norm):

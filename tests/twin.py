@@ -3,6 +3,7 @@
 Not collected by pytest (like render_oracle.py): the tests import what they need from here, and each keeps its own scenario,
 its own bounds and its own asserts.
 """
+import json
 import math
 import os
 import re
@@ -14,6 +15,8 @@ TOL_Q, TOL_P = 1e-3, 1e-3             # north star: joint angles 1e-3 rad, base 
 SUB = dict(control_time_step=0.001, action_repeat=1, solver_iterations=60)    # one control step = one physics sub-step
 NOISE = (0.01, 0.05, 0.1, 0.02, 0.1)  # motor angle, velocity, torque, base rpy, rpy rate (SENSOR_NOISE_STDDEV order)
 FOLDED = np.array([-0.42, -1.51, 2.70, 0.42, -1.51, 2.70, -0.44, -1.49, 2.69, 0.44, -1.49, 2.69])   # standup's settled legs
+HERE = os.path.dirname(os.path.abspath(__file__))
+ARM_REST = np.array(json.load(open(os.path.join(HERE, "golden", "constants_golden.json")))["arm_poses"]["rest"], np.float32)
 
 # oracle contact groups, the same bits in the kernel's contact mask: 0 base / chassis; per leg 1 + 2l shoulder and leg boxes,
 # 2 + 2l foot box and toe hull; 9-14 the arm links
@@ -29,11 +32,56 @@ STATE_KEYS = ("pos", "quat", "linvel", "angvel", "q", "qd")       # what Batched
 
 # step_kernel instance (CTA size, CTAs per SM, sensor) of each build the dispatcher can launch
 BUILDS = {"small": (128, 1, 0), "big": (256, 4, 0), "sensor": (128, 1, 1)}
+BUILDS_OF = {"base": ("small", "big", "sensor"), "arm": ("small", "sensor")}     # arm batches never take the big build
+
+# ---- the step kernel's dispatch image --------------------------------------------------------------------------------
+# (task, signal) of each compilation unit, in the order of c_units in rex_gym_b200/csrc/rexsim_kernel.cu
+UNITS = [("walk", "ik"), ("walk", "ol"), ("gallop", "ik"), ("gallop", "ol"), ("turn", "ik"), ("turn", "ol"), ("standup", "ol"), ("poses", "ik")]
+ARM_UNITS = [u for u in UNITS if u[0] != "gallop"]              # launch_step_ts: HAS_ARM
+# every step_kernel instance the dispatcher can launch: (task, signal, arm, terrain, build), 8 x 2 x 3 + 6 x 2 x 2 = 72 rows
+INSTANCES = [(t, s, arm, ter, b) for arm, mark, units in ((False, "base", UNITS), (True, "arm", ARM_UNITS)) for t, s in units
+             for ter in ("plane", "random") for b in BUILDS_OF[mark]]
+
+
+def row_id(row):
+    """walk-ik-plane-small, standup-ol-arm-random-sensor."""
+    task, sig, arm, terrain, build = row
+    return "-".join([task, sig] + (["arm"] if arm else []) + [terrain, build])
+
+
+def instance_config(row):
+    """BatchedRexEnv / oracle keywords that reach the instance `row` (with force_build for the small and big builds)."""
+    task, sig, arm, terrain, build = row
+    kw = dict(signal_type=sig, seed=13, max_episode_steps=15)         # short episodes: every env runs the in-kernel reset twice
+    if arm:
+        kw["mark"] = "arm"
+    if (task, sig) == ("gallop", "ol"):
+        kw.update(motor_kp_range=(0.8, 1.2), motor_kd_range=(0.01, 0.03))
+    if terrain == "random":
+        kw.update(terrain_type="random", num_fields=4)
+    if build == "sensor":
+        kw["control_latency"] = 0.0125                                # a blend of two history rows, 12 sub-steps back
+    return kw
+
+
+def create_status(task, sig):
+    """rexsim_create's status for an 18-motor config of (task, sig) handed a base-sized (952-float) model table: -2 once the
+    config is accepted (the table size is checked after validation and before any CUDA call), -4 when the arm is refused."""
+    import ctypes as C
+    from rex_gym_b200 import _capi
+    from rex_gym_b200.envs.batched_env import SIGNALS, TASKS
+    L = _capi.load()
+    cfg = _capi.RexSimConfig()
+    cfg.num_envs, cfg.task, cfg.signal, cfg.num_motors = 8, TASKS[task], SIGNALS[sig], 18
+    cfg.action_repeat, cfg.solver_iterations, cfg.sim_dt_d, cfg.toe_npts, cfg.gait_clock_scale = 5, 60, 0.001, 27, 1.0
+    h = C.c_void_p()
+    tb = np.zeros(952, np.float32)
+    return L.rexsim_create(C.byref(cfg), tb.ctypes.data, 952, C.byref(h)), L.rexsim_last_error()
 
 
 def _read_layout():
     """The SoA state word indices and flag bits (F_*, I_*, FL_*, NF, NI) of the step kernel's header."""
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "rex_gym_b200", "csrc", "rexsim_kernel.cuh")
+    path = os.path.join(HERE, "..", "rex_gym_b200", "csrc", "rexsim_kernel.cuh")
     src = re.sub(r"//[^\n]*|/\*.*?\*/", "", open(path).read(), flags=re.S)
     words = {k: int(v) for block in re.findall(r"\benum\s*\{(.*?)\}", src, re.S)
              for k, v in re.findall(r"\b((?:F|I|FL)_\w+|NF|NI)\s*=\s*(\d+)", block)}
@@ -95,19 +143,36 @@ def solver_cost(env):
     return torch.as_tensor(_DevArray(p.value, (env.num_envs,), "<i4", env), device="cuda").cpu().numpy().copy()
 
 
-def sync(env, ora, idx=None, protection=False):
+def sync(env, ora, idx=None, protection=False, window=None):
     """Set the physical state of envs `idx` (default: all) to the oracle's; the rest of the batch is written back unchanged.
-    protection=True also copies every env's overheat counters and motor-enabled bits, which set_state does not carry: a counter
-    one sub-step off re-fires its event."""
+    With `window`, oracle env i is batch env window + i (and `idx` counts oracle envs).  protection=True (whole batches only)
+    also copies every env's overheat counters and motor-enabled bits, which set_state does not carry: a counter one sub-step
+    off re-fires its event."""
     so = ora.states()
-    if idx is not None:
+    if idx is not None or window is not None:
+        idx = np.arange(ora.N) if idx is None else np.asarray(idx)
         st = env.get_state()
         for k in STATE_KEYS:
-            st[k][idx] = so[k][idx]
+            st[k][idx + (window or 0)] = so[k][idx]
         so = st
     env.set_state(*(so[k] for k in STATE_KEYS))
     if protection:
         _sync_protection(env, ora)
+
+
+def window_twin(task, n, w0, nw, steps, settled=False, **kw):
+    """A batch of n envs and the oracle of its nw envs from w0 on (same global env ids: env_offset keys every reset draw), both
+    reset, the window's draws checked bit for bit; settled=True starts the window from the oracle's settled state.
+    -> (env, oracle, the window's reset observations from the batch and from the oracle, [steps][n][action_dim] seeded
+        uniform actions in [-1, 1) on the device)."""
+    import torch
+    env, ora = make_env(task, n, **kw), make_oracle(task, nw, env_offset=w0, **kw)
+    og, oc = env.reset()[w0:w0 + nw], ora.reset()
+    assert_draws(env, ora, task, window=w0)
+    if settled:
+        sync(env, ora, window=w0)
+    g = torch.Generator(device="cuda"); g.manual_seed(5)
+    return env, ora, og, oc, torch.rand((steps, n, env.action_dim), device="cuda", generator=g) * 2 - 1
 
 
 # ---- state words --------------------------------------------------------------------------------------------------------

@@ -3,7 +3,7 @@
 
     python tools/dev_ab_outputs.py rex_gym_b200/librexsim_parent.so rex_gym_b200/librexsim.so [more.so ...]
 
-Runs every step-kernel instance of tests/test_gpu_builds.INSTANCES (forced build, 37 envs, 40 steps of seeded random actions,
+Runs all 72 step-kernel instances of tests/twin.INSTANCES (forced build, 37 envs, 40 steps of seeded random actions,
 auto-reset after 15 steps), walk-ik on flat ground at 8449 and 65 536 envs and turn-ik on heightfields at 16 897 envs (the
 big build, warp re-grouping on) once per library, each library in its own process (REXSIM_LIB).  After every step it hashes
 obs, reward, done, last_command, the error words, the whole SoA state and the sensor ring; then bench.py --dump-outputs.
@@ -30,8 +30,8 @@ sys.path[:0] = [os.path.join(ROOT, "tests"), os.path.join(ROOT, "tests", "golden
 
 
 def cases():
-    from test_gpu_builds import INSTANCES, _config, _row_id
-    out = [(_row_id(r), r[0], None if r[4] == "sensor" else r[4], 37, _config(*r[:5])) for r in INSTANCES]
+    from twin import INSTANCES, instance_config, row_id
+    out = [(row_id(r), r[0], None if r[4] == "sensor" else r[4], 37, instance_config(r)) for r in INSTANCES]
     for n in (8449, 65536):
         out.append((f"walk-ik-plane-n{n}", "walk", None, n, dict(signal_type="ik", seed=13, max_episode_steps=15)))
     out.append(("turn-ik-random-n16897", "turn", None, 16897,
