@@ -185,6 +185,7 @@ def test_generic_substeps_against_the_oracle(monkeypatch, mark, terrain, build):
     eq, ep, off_band, generic_steps, _, _ = compare_substeps(env, ora, band, st, build, ids)
     stats = (np.median(eq), np.percentile(eq, 90), eq.max(), np.median(ep), np.percentile(ep, 90), ep.max(), off_band)
     print("generic sub-steps q (median, p90, max), pos (median, p90, max), iterations off the band:", stats)
+    print("generic sub-steps q (p95, p99), samples beyond 1e-4 rad:", np.percentile(eq, 95), np.percentile(eq, 99), (eq > 1e-4).sum())
     assert generic_steps >= 30 * (N - 3) * 0.5, generic_steps
     assert off_band <= 3, stats
     assert np.percentile(eq, 90) < 2e-5 and np.percentile(ep, 90) < 2e-6 and eq.max() < 3e-3 and ep.max() < 3e-3, stats

@@ -123,6 +123,7 @@ def test_free_running_rollout(task, sig, kw):
         steps = 110        # every env follows the same hopping trajectory (the action only shifts ramp timings): common-mode chaos
     env, ora = make_env(task, n, signal_type=sig, seed=3, **kw), make_oracle(task, n, signal_type=sig, seed=3, **kw)
     env.reset(); ora.reset()
+    print(f"{task}-{sig} reset max|dq|, max|dpos|:", *(e.max() for e in state_errors(env, ora)))
     if task == "standup" or kw.get("mark") == "arm":      # start both from the oracle's settled state (see test_reset_settle_and_draws)
         sync(env, ora)
     rng = np.random.default_rng(11)
@@ -139,6 +140,9 @@ def test_free_running_rollout(task, sig, kw):
             break
         eq, ep = state_errors(env, ora)
         eq, ep = eq[cmp], np.maximum(ep, np.abs(sg["quat"] - so["quat"]).max(axis=1))[cmp]
+        if k % 25 == 0 or k == steps - 1:
+            print(f"{task}-{sig} step {k:3d} alive {cmp.sum():2d} max|dq| {eq.max():.2e} max|dpos,dquat| {ep.max():.2e} |dobs| "
+                  f"{np.abs(og - oc)[cmp].max():.2e} |drew| {np.abs(rg - rc)[cmp].max():.2e} done g/c {dg.sum()}/{dc.sum()}")
         if k < strict:
             # every env inside the tolerance, except isolated touchdown events: a foot landing one 1 ms sub-step earlier
             # on one side (fp32 vs fp64 height) gives a transient of a few mrad in that env; allow 10 % such envs, bounded
@@ -160,6 +164,7 @@ def test_free_running_rollout(task, sig, kw):
         alive &= ~(dg | dc)
         if not alive.any():
             break
+    print(f"{task}-{sig} toe contact-mask mismatches {contact_bad} of {contact_total}, error word {int(env._err[n])}")
     assert contact_bad <= 0.02 * max(contact_total, 1)          # toe contact-pair masks after each control step
     assert (env.check_errors() & 1) == 0
     env.close()
@@ -193,6 +198,7 @@ def test_shadowing_1000_steps_walk():
     eqs, eps_, erp = np.concatenate(eqs), np.concatenate(eps_), np.concatenate(erp)
     stats = [(np.percentile(e, 50), np.percentile(e, 90), e.max()) for e in (eqs, eps_, erp)]
     print("shadowing (median, p90, max) q/pos/roll-pitch:", stats)
+    print(f"shadowing q samples beyond {TOL_Q}: {(eqs >= TOL_Q).sum()} of {eqs.size}; toe contact-mask mismatches {mism} of {tot}")
     assert stats[0][0] < 1e-5 and stats[1][0] < 1e-5, stats
     assert stats[0][1] < 1e-4 and stats[1][1] < 1e-4 and stats[2][1] < 1e-4, stats
     # every sample of base pose and roll/pitch inside the north-star 1e-3; joint angles: 99.9 % of the (step, env) samples inside

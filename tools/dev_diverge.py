@@ -1,31 +1,24 @@
 #!/usr/bin/env python3
 """Find the first env/step where GPU and oracle part ways and print what happened around it."""
 import sys, os
-sys.path.insert(0, os.path.join(os.path.dirname(__file__), ".."))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 import numpy as np
-from oracle.oracle import OracleSim
-import rex_gym_b200 as R
-from rex_gym_b200.envs.batched_env import ACTION_BOUND
+from twin import bound, make_env, make_oracle, state_errors, toe_masks
 
 def run(task, sig, n, steps, seed, thr=2e-4, **kw):
-    env = R.BatchedRexEnv(task=task, num_envs=n, signal_type=sig, seed=seed, **kw)
-    okw = dict(kw); kr, dr = okw.pop("motor_kp_range", None), okw.pop("motor_kd_range", None)
-    ter = okw.pop("terrain_type", "plane"); nf = okw.pop("num_fields", 0)
-    ora = OracleSim(n, task, sig, seed=seed, kp_range=kr, kd_range=dr, terrain=ter, nfields=nf, **okw)
+    env, ora = make_env(task, n, signal_type=sig, seed=seed, **kw), make_oracle(task, n, signal_type=sig, seed=seed, **kw)
     env.reset(); ora.reset()
-    sg = env.get_state()
-    print(f"[{task}-{sig}] reset dq {max(np.abs(sg['q'][i]-ora.state(i)['q']).max() for i in range(n)):.2e}")
-    rng = np.random.default_rng(11); b = ACTION_BOUND[(task, sig)]
+    print(f"[{task}-{sig}] reset dq {state_errors(env, ora)[0].max():.2e}")
+    rng = np.random.default_rng(11); b = bound(task, sig)
     hist = []
     for k in range(steps):
         a = rng.uniform(-b, b, size=(n, env.action_dim)).astype(np.float32)
         env.step(a); ora.step(a)
-        sg = env.get_state()
-        eq = np.array([np.abs(sg['q'][i] - ora.state(i)['q']).max() for i in range(n)])
-        cm = np.array([ora.env(i).contact_mask & 0x1FF for i in range(n)])
+        eq = state_errors(env, ora)[0]
         lim = np.array([ora.env(i).limit_rows for i in range(n)])
         it = np.array([ora.env(i).solver_iters for i in range(n)])
-        hist.append((eq, cm, sg['contact_mask'].copy(), lim, it))
+        hist.append((eq, toe_masks(ora), env.get_state()['contact_mask'].copy(), lim, it))
         bad = np.nonzero(eq > thr)[0]
         if len(bad):
             i = bad[0]
