@@ -18,6 +18,10 @@
  *                   <- getBasePositionAndOrientation / getBaseVelocity / getJointState /
  *                      resetBasePositionAndOrientation / resetJointState (rex_gym/model/rex.py:297-299,
  *                      360-372,416,451,545) -- used for golden comparison and checkpoint/resume
+ *   rexsim_episode_summary
+ *                   <- simulate()'s score / length bookkeeping and its StreamingMeans (rex_gym/agents/tools/simulate.py:57-113,
+ *                      streaming_mean.py), RexGymEnv.get_objectives (rex_gym_env.py:538-547); kept by rexsim_step when
+ *                      RexSimConfig.episode_stats is set
  *   rexsim_destroy  <- RexGymEnv.close (rex_gym/envs/rex_gym_env.py:287-291)
  *
  * Conventions: plain C, no exceptions; every function returns 0 or a negative RexSimStatus.
@@ -130,6 +134,13 @@ typedef struct {
      * rexsim_noise is the same generator host-side. */
     double control_latency, pd_latency;   /* seconds */
     double noise_stdev[5];                /* SENSOR_NOISE_STDDEV order (rex.py:22): motor angle, velocity, torque, base rpy, rpy rate */
+    /* 1: keep simulate()'s episode bookkeeping on the device (rex_gym/agents/tools/simulate.py:57-113): every step adds its
+     * reward to the env's score and counts its length; a step that returns done submits the episode to per-env accumulators
+     * (episode count, score sum, length sum) and restarts both, with or without auto_reset.  An episode ending on a step that
+     * raises REXSIM_FLAG_NONFINITE is counted apart and not submitted.  Walk and gallop also record the unweighted objectives
+     * [forward, energy, drift, shake] of every step (RexGymEnv._reward, rex_gym_env.py:501-555).  See rexsim_episode_buffers /
+     * rexsim_episode_summary.  0: nothing is allocated and every output is what it is without the switch. */
+    int32_t episode_stats;
 } RexSimConfig;
 
 typedef struct RexSim RexSim;
@@ -196,6 +207,24 @@ int rexsim_set_render_tables(RexSim* sim, const float* render_tables, int32_t n_
  * 1..4096 per side, k >= 0.  An index outside [0, N) gives a sky image and sets REXSIM_FLAG_BAD_INDEX in the aggregate word. */
 int rexsim_render(RexSim* sim, const int32_t* idx, int32_t k, int32_t width, int32_t height, float distance, float yaw_deg,
                   float pitch_deg, uint8_t* rgb, void* stream);
+/* Episode statistics (RexSimConfig.episode_stats = 1), device pointers owned by the handle:
+ *   score dev [N] f32, length dev [N] int32: the running episode of every env (rexsim_reset zeroes those of the envs it resets
+ *     and submits nothing, as simulate(reset=True) does);
+ *   objectives dev [4][N] f32: forward, energy, drift, shake of every env's last step, before the task's weights (walk and
+ *     gallop; NULL for turn, standup and poses, whose reward has no objectives);
+ *   summary dev [4] f64: count, nonfinite, sum of scores, sum of lengths, written by rexsim_episode_summary;
+ *   block / block_bytes: the one allocation behind score and length and the per-env accumulators, indexed by env:
+ *     sum_score f64 [N] | sum_length i64 [N] | score f32 [N] | length i32 [N] | count i32 [N] | nonfinite i32 [N].
+ *     Part of an exact checkpoint together with the state buffers.
+ * REXSIM_ERR_INVALID when the switch is off. */
+int rexsim_episode_buffers(RexSim* sim, float** score, int32_t** length, float** objectives, double** summary, void** block,
+                           int64_t* block_bytes);
+/* StreamingMean.submit's totals (simulate.py:90-106, streaming_mean.py:45-60) over the whole batch into the summary block: episodes submitted, episodes
+ * ended non-finite, score sum, length sum (sums, not means, so that shards can add them).  The reduction order is fixed (one CTA,
+ * thread t sums envs t, t + 1024, ... in order, then a fixed tree): repeated runs give bit-identical sums whatever the device,
+ * the rebalancing or the launch history.  clear != 0 also zeroes the accumulators (StreamingMean.clear); running episodes go
+ * on.  One launch on `stream`; REXSIM_ERR_INVALID when the switch is off. */
+int rexsim_episode_summary(RexSim* sim, int32_t clear, void* stream);
 /* kernels launched by this handle since create (the bench reports it) */
 int64_t rexsim_launch_count(const RexSim* sim);
 /* which build of the step kernel the last rexsim_step / rexsim_step_host launched (all 0 before the first step): CTA size,

@@ -27,6 +27,7 @@ class RexSimConfig(C.Structure):
         ("contact_breaking", C.c_float), ("link_damping", C.c_float), ("max_coordinate_velocity", C.c_float), ("env_offset", C.c_int32),
         ("gait_clock_scale", C.c_double), ("pose_values", C.c_float * 5),
         ("control_latency", C.c_double), ("pd_latency", C.c_double), ("noise_stdev", C.c_double * 5),
+        ("episode_stats", C.c_int32),
     ]
 
 
@@ -67,6 +68,8 @@ SIGNATURES = {
     "rexsim_history_buffer": (C.c_int, [_ptr, _out(_ptr), _out(_i64)]),
     "rexsim_set_render_tables": (C.c_int, [_ptr, _ptr, _i32]),
     "rexsim_render": (C.c_int, [_ptr, _ptr, _i32, _i32, _i32, _f32, _f32, _f32, _ptr, _ptr]),
+    "rexsim_episode_buffers": (C.c_int, [_ptr] + [_out(_ptr)] * 5 + [_out(_i64)]),
+    "rexsim_episode_summary": (C.c_int, [_ptr, _i32, _ptr]),
     "rexagent_policy_floats": (_i64, [_agent_cfg]),
     "rexagent_value_floats": (_i64, [_agent_cfg]),
     "rexagent_create": (C.c_int, [_agent_cfg, _out(_ptr)]),

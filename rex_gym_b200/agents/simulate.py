@@ -79,6 +79,12 @@ class Rollout(object):
         return dict(observ=self.observ, action=self.action, mean=self.mean, logprob=self.logprob, value=self.value,
                     reward=self.reward, done=self.done.view(torch.bool))
 
+    def summary(self, clear=True):
+        """simulate()'s mean_score / mean_length (simulate.py:95-106) over the episodes that ended since the last clear: the step
+        kernel keeps the bookkeeping of an env created with episode_statistics=True, inside the captured graph as well
+        (BatchedRexEnv.episode_summary)."""
+        return self.env.episode_summary(clear)
+
     def returns_and_advantages(self, discount, lam=1.0):
         """Done-aware discounted return and GAE over the last rollout (utility.gae_segments)."""
         return utility.gae_segments(self.reward, self.value, self.done, discount, lam)

@@ -12,6 +12,7 @@ cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, cudaS
 cudaError_t launch_get_state(const Params& P, float* out_f, int32_t* out_i, cudaStream_t st);
 cudaError_t launch_set_state(const Params& P, const float* in_f, cudaStream_t st);
 cudaError_t launch_rebalance(const int32_t* cost, int n, int32_t* hist, int32_t* perm, cudaStream_t st);
+cudaError_t launch_episode_summary(const Params& P, int clear, double* out, cudaStream_t st);
 cudaError_t launch_render(const Params& P, const float* rt, const float* zrange, const int32_t* idx, int k, int W, int H,
                           float distance, float yaw_deg, float pitch_deg, uint8_t* rgb, cudaStream_t st, int* launches);
 }  // namespace rexsim
@@ -23,6 +24,8 @@ struct RexSim {
     DeviceBuffers mem;
     float* zrange = nullptr;           // [nfields][2] lowest / highest centred height of each field (renderer)
     float* rt = nullptr;               // render table (rexsim_set_render_tables)
+    uint8_t* ep_block = nullptr;       // episode statistics: the per-env block behind P.ep (episode_block_bytes)
+    double* ep_summary = nullptr;      // [4] count, nonfinite, sum of scores, sum of lengths (rexsim_episode_summary)
     bool rt_set = false;
     int32_t* perm = nullptr;           // slot -> env, sorted by solver cost; P.perm points here after rexsim_rebalance
     int32_t* hist = nullptr;
@@ -94,6 +97,7 @@ static int validate(const RexSimConfig* c) {
     if (!(c->gait_clock_scale > 0)) return fail(REXSIM_ERR_INVALID, "gait_clock_scale must be positive (1 = simulation clock)");
     if (!(c->control_latency >= 0) || !(c->pd_latency >= 0)) return fail(REXSIM_ERR_INVALID, "latencies must be >= 0");
     for (int k = 0; k < 5; k++) if (!(c->noise_stdev[k] >= 0)) return fail(REXSIM_ERR_INVALID, "noise_stdev must be >= 0");
+    if (c->episode_stats != 0 && c->episode_stats != 1) return fail(REXSIM_ERR_INVALID, "episode_stats must be 0 or 1");
     return REXSIM_OK;
 }
 int rexsim_history_depth(const RexSimConfig* c) { return c ? sensor_cfg(c).depth : 0; }
@@ -143,6 +147,20 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
         P.lat_ctl = (float)cfg->control_latency; P.lat_pd = (float)cfg->pd_latency;
         for (int k = 0; k < 5; k++) P.noise_sd[k] = (float)cfg->noise_stdev[k];
         if (mem.zeroed(&P.ring, (size_t)sc.depth * sc.words * N) || mem.zeroed(&P.snap_ring, (size_t)s->nsnap * sc.depth * sc.words))
+            return REXSIM_ERR_CUDA;
+    }
+    if (cfg->episode_stats) {
+        if (mem.zeroed(&s->ep_block, episode_block_bytes(N)) || mem.zeroed(&s->ep_summary, 4)) return REXSIM_ERR_CUDA;
+        EpisodeStats& E = P.ep;
+        E.sum_score = reinterpret_cast<double*>(s->ep_block);
+        E.sum_length = reinterpret_cast<int64_t*>(E.sum_score + N);
+        E.score = reinterpret_cast<float*>(E.sum_length + N);
+        E.length = reinterpret_cast<int32_t*>(E.score + N);
+        E.count = E.length + N;
+        E.nonfinite = E.count + N;
+        // RexGymEnv._reward's objectives: turn, standup and poses override _reward and record none (turn_env.py:362-367,
+        // standup_env.py:151-167, poses_env.py:256-258)
+        if ((cfg->task == REXSIM_TASK_WALK || cfg->task == REXSIM_TASK_GALLOP) && mem.zeroed(&E.objectives, 4 * N))
             return REXSIM_ERR_CUDA;
     }
     if (cfg->terrain == REXSIM_TERRAIN_RANDOM) {
@@ -306,6 +324,19 @@ int rexsim_render(RexSim* s, const int32_t* idx, int32_t k, int32_t width, int32
     const cudaError_t e = launch_render(s->P, s->rt, s->zrange, idx, k, width, height, distance, yaw_deg, pitch_deg, rgb,
                                         (cudaStream_t)stream, &launches);
     return enqueue(s, e, "render launch", launches);
+}
+int rexsim_episode_buffers(RexSim* s, float** score, int32_t** length, float** objectives, double** summary, void** block,
+                           int64_t* block_bytes) {
+    if (!s || !score || !length || !objectives || !summary || !block || !block_bytes) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (!s->ep_block) return fail(REXSIM_ERR_INVALID, "episode statistics are off (RexSimConfig.episode_stats)");
+    *score = s->P.ep.score; *length = s->P.ep.length; *objectives = s->P.ep.objectives; *summary = s->ep_summary;
+    *block = s->ep_block; *block_bytes = (int64_t)episode_block_bytes(s->P.N);
+    return REXSIM_OK;
+}
+int rexsim_episode_summary(RexSim* s, int32_t clear, void* stream) {
+    if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
+    if (!s->ep_block) return fail(REXSIM_ERR_INVALID, "episode statistics are off (RexSimConfig.episode_stats)");
+    return enqueue(s, launch_episode_summary(s->P, clear != 0, s->ep_summary, (cudaStream_t)stream), "episode summary launch");
 }
 int64_t rexsim_launch_count(const RexSim* s) { return s ? s->launches : 0; }
 int rexsim_last_step_build(const RexSim* s, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor) {

@@ -1909,6 +1909,10 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
         }
         float energy = -fabsf(sum4(e)) * (float)c.sim_dt_d;
         reward = fwd * c.w_distance + energy * c.w_energy + drift * c.w_drift + shake * c.w_shake;
+        if (P.ep.objectives && valid && leg == 0) {     // RexGymEnv._objectives.append(objectives) (rex_gym_env.py:538-541)
+            float* o = P.ep.objectives + env;
+            o[0] = fwd; o[(size_t)N] = energy; o[2 * (size_t)N] = drift; o[3 * (size_t)N] = shake;
+        }
     }
     // ---- termination ----------------------------------------------------------------------------------------
     bool done;
@@ -1950,6 +1954,18 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
                 for (int b = 0; b < 8; b++) if ((err >> b) & 1) P.err_host[b] = 1;
             }
         }
+        // simulate(): score.assign_add(reward), length += 1 (simulate.py:71-72); a done step ends the episode -- submitted to the
+        // accumulators (_define_end_episode, :90-91) unless it is non-finite -- and the next one starts at 0 (:51-52)
+        if (P.ep.score) {
+            float score = P.ep.score[env] + reward;
+            int32_t length = P.ep.length[env] + 1;
+            if (done) {
+                if (finite) { P.ep.count[env] += 1; P.ep.sum_score[env] += (double)score; P.ep.sum_length[env] += length; }
+                else P.ep.nonfinite[env] += 1;
+                score = 0.f; length = 0;
+            }
+            P.ep.score[env] = score; P.ep.length[env] = length;
+        }
     }
     // ---- auto reset: done envs restart from the settled snapshot; obs = first observation of the new episode --
     if (c.auto_reset && done) {
@@ -1986,7 +2002,10 @@ __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_o
         if (P.sensor_on) write_obs<TASK, true>(P, env, leg, L, obs_out + (size_t)j * O, S, 0u);
         else write_obs<TASK, false>(P, env, leg, L, obs_out + (size_t)j * O, S, 0u);
     }
-    if (wr && leg == 0) P.err[env] = 0;
+    if (wr && leg == 0) {
+        P.err[env] = 0;
+        if (P.ep.score) { P.ep.score[env] = 0.f; P.ep.length[env] = 0; }   // _define_begin_episode (simulate.py:51-52): nothing submitted
+    }
     store_lane(P.sf, P.si, P.N, env, leg, L, K, wr);
     if (ARM && wr && leg == 0) store_arm(P.sf, P.si, P.N, env, AR);
 }
@@ -2177,6 +2196,42 @@ cudaError_t launch_rebalance(const int32_t* cost, int n, int32_t* hist, int32_t*
     rebalance_hist_kernel<<<(n + 255) / 256, 256, 0, st>>>(cost, n, hist);
     rebalance_scan_kernel<<<1, 256, 0, st>>>(hist);
     rebalance_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(cost, n, hist, perm);
+    return cudaGetLastError();
+}
+
+// ---- episode summary: the per-env accumulators reduced in a fixed order (one CTA whatever the device or the batch history) ----
+constexpr int SUMMARY_THREADS = 1024;
+__global__ void __launch_bounds__(SUMMARY_THREADS) episode_summary_kernel(const EpisodeStats E, int n, int clear, double* __restrict__ out) {
+    __shared__ double s_score[SUMMARY_THREADS / 32];
+    __shared__ long long s_count[SUMMARY_THREADS / 32], s_nonfinite[SUMMARY_THREADS / 32], s_length[SUMMARY_THREADS / 32];
+    const int t = threadIdx.x;
+    double score = 0.0;
+    long long count = 0, nonfinite = 0, length = 0;
+    for (int e = t; e < n; e += SUMMARY_THREADS) {
+        score += E.sum_score[e]; length += E.sum_length[e]; count += E.count[e]; nonfinite += E.nonfinite[e];
+        if (clear) { E.sum_score[e] = 0.0; E.sum_length[e] = 0; E.count[e] = 0; E.nonfinite[e] = 0; }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        score += __shfl_down_sync(0xFFFFFFFFu, score, o);
+        count += __shfl_down_sync(0xFFFFFFFFu, count, o);
+        nonfinite += __shfl_down_sync(0xFFFFFFFFu, nonfinite, o);
+        length += __shfl_down_sync(0xFFFFFFFFu, length, o);
+    }
+    if ((t & 31) == 0) { s_score[t >> 5] = score; s_count[t >> 5] = count; s_nonfinite[t >> 5] = nonfinite; s_length[t >> 5] = length; }
+    __syncthreads();
+    if (t < 32) {
+        score = s_score[t]; count = s_count[t]; nonfinite = s_nonfinite[t]; length = s_length[t];
+        for (int o = 16; o > 0; o >>= 1) {
+            score += __shfl_down_sync(0xFFFFFFFFu, score, o);
+            count += __shfl_down_sync(0xFFFFFFFFu, count, o);
+            nonfinite += __shfl_down_sync(0xFFFFFFFFu, nonfinite, o);
+            length += __shfl_down_sync(0xFFFFFFFFu, length, o);
+        }
+        if (t == 0) { out[0] = (double)count; out[1] = (double)nonfinite; out[2] = score; out[3] = (double)length; }
+    }
+}
+cudaError_t launch_episode_summary(const Params& P, int clear, double* out, cudaStream_t st) {
+    episode_summary_kernel<<<1, SUMMARY_THREADS, 0, st>>>(P.ep, P.N, clear, out);
     return cudaGetLastError();
 }
 

@@ -61,8 +61,24 @@ __host__ __device__ constexpr TaskShape task_shape(int task) {
 // observation width: base roll, pitch and their rates, then (gallop) the motor angles
 __host__ __device__ constexpr int obs_dim(int task, int num_motors) { return 4 + (task_shape(task).angles ? num_motors : 0); }
 
+// Episode statistics (RexSimConfig.episode_stats; every pointer is null when it is off): simulate()'s per-env score and length
+// (rex_gym/agents/tools/simulate.py:57-105) and what its StreamingMeans were handed by the episodes that ended, per env (not per
+// slot, so rexsim_rebalance cannot move them).  score, length and the four accumulators live in one allocation, `block`.
+struct EpisodeStats {
+    double* __restrict__ sum_score;    // [N] scores of the submitted episodes, summed
+    int64_t* __restrict__ sum_length;  // [N] their lengths, summed
+    float* __restrict__ score;         // [N] reward summed since the env's episode began
+    int32_t* __restrict__ length;      // [N] control steps since the env's episode began
+    int32_t* __restrict__ count;       // [N] episodes submitted
+    int32_t* __restrict__ nonfinite;   // [N] episodes that ended on a step raising REXSIM_FLAG_NONFINITE (never submitted)
+    float* __restrict__ objectives;    // [4][N] forward, energy, drift, shake of the last step, unweighted (walk and gallop only)
+};
+// bytes of the per-env block behind EpisodeStats: sum_score | sum_length | score | length | count | nonfinite
+__host__ __device__ constexpr size_t episode_block_bytes(size_t n) { return n * (2 * sizeof(double) + 4 * sizeof(int32_t)); }
+
 struct Params {
     RexSimConfig cfg;
+    EpisodeStats ep;
     const float* __restrict__ model;   // REXSIM_MT_FLOATS floats, 16-byte aligned
     float* __restrict__ sf;            // [NF][N]
     int32_t* __restrict__ si;          // [NI][N]

@@ -49,6 +49,15 @@ def _host_block_views(block, N, O):
     return views[0].reshape(N, O), views[1], views[2], views[3]
 
 
+def summarize_episodes(totals):
+    """Episode totals [4] (BatchedRexEnv.episode_totals, or their sum over shards) -> the summary simulate() logs (one copy to
+    the host).  The reference writes no summary when no episode ended (simulate.py:101-106): the means are None then."""
+    count, nonfinite, score, length = totals.cpu().tolist()
+    count = int(count)
+    return dict(count=count, nonfinite=int(nonfinite), mean_score=score / count if count else None,
+                mean_length=length / count if count else None)
+
+
 class _Info(object):
     """Stand-in for BatchEnv's `tuple(infos)`: info[i] == {'action': motor command of env i} of THE STEP THAT RETURNED IT
     (rex_gym_env.py:414).  The command block lives on the device and is overwritten by the next step, so the host copy is taken
@@ -102,7 +111,7 @@ class BatchedRexEnv(object):
                  normalize=False, max_episode_steps=0, auto_reset=False, seed=1234,
                  motor_kp_range=None, motor_kd_range=None, num_fields=64, solver_iterations=None, env_offset=0,
                  base_y=None, base_z=None, base_roll=None, base_pitch=None, base_yaw=None, gait_clock_scale=1.0,
-                 rebalance_every=8, observation_noise_stdev=SENSOR_NOISE_STDDEV):
+                 rebalance_every=8, observation_noise_stdev=SENSOR_NOISE_STDDEV, episode_statistics=False):
         if urdf_version is not None and urdf_version != DEFAULT_URDF_VERSION:
             raise ValueError("%s is not a supported urdf_version." % urdf_version)     # rex_gym_env.py:317-318
         if task not in TASKS or signal_type not in SIGNALS:
@@ -154,6 +163,7 @@ class BatchedRexEnv(object):
         c.control_latency, c.pd_latency = float(control_latency), float(pd_latency)
         for k, v in enumerate(observation_noise_stdev):
             c.noise_stdev[k] = float(v)
+        c.episode_stats = int(bool(episode_statistics))       # simulate()'s score / length bookkeeping on the device
         self._fields = None
         with torch.cuda.device(self.device):
             if terrain_type == "random":
@@ -208,6 +218,13 @@ class BatchedRexEnv(object):
         nr = C.c_int64()
         _capi.check(self._L.rexsim_history_buffer(self._h, C.byref(p), C.byref(nr)))           # sensor history ring (None: model off)
         self._ring = view(p, (nr.value,), "<f4") if nr.value else None
+        self._episode = None
+        if episode_statistics:
+            o, sm, blk, nb = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int64()
+            _capi.check(self._L.rexsim_episode_buffers(self._h, *(C.byref(x) for x in (p, q, o, sm, blk, nb))))
+            self._episode = dict(score=view(p, (N,), "<f4"), length=view(q, (N,), "<i4"), summary=view(sm, (4,), "<f8"),
+                                 block=view(blk, (nb.value,), "|u1"),
+                                 objectives=view(o, (4, N), "<f4") if o.value else None)
         # spaces: raw task spaces, or the wrapper-visible ones when the training wrappers are fused in
         b = ACTION_BOUND[(task, signal_type)]
         if normalize:
@@ -355,6 +372,8 @@ class BatchedRexEnv(object):
         sd = {"state_f": self._state_f.clone(), "state_i": self._state_i.clone()}
         if self._ring is not None:
             sd["sensor_history"] = self._ring.clone()
+        if self._episode is not None:
+            sd["episode_statistics"] = self._episode["block"].clone()
         return sd
 
     def load_state_dict(self, sd):
@@ -362,6 +381,49 @@ class BatchedRexEnv(object):
         self._state_i.copy_(sd["state_i"])
         if self._ring is not None:
             self._ring.copy_(sd["sensor_history"])
+        if self._episode is not None:
+            self._episode["block"].copy_(sd["episode_statistics"])
+
+    # ---- episode statistics (episode_statistics=True) ------------------------------------------------
+    def _episode_buffer(self, name):
+        if self._episode is None:
+            raise ValueError("episode statistics are off: create the env with episode_statistics=True")
+        return self._episode[name]
+
+    @property
+    def objective_weights(self):
+        """RexGymEnv.objective_weights (rex_gym_env.py:547-556): weights of forward, energy, drift and shake in the reward."""
+        c = self._cfg
+        return (c.w_distance, c.w_energy, c.w_drift, c.w_shake)
+
+    def objectives(self):
+        """RexGymEnv.get_objectives of the last step for every env: CUDA view [N, 4] of forward, energy, drift, shake before
+        the weights, overwritten by the next step.  Walk and gallop only: the other tasks' rewards have no objectives."""
+        o = self._episode_buffer("objectives")
+        if o is None:
+            raise ValueError("the %s task records no objectives (its _reward replaces RexGymEnv's)" % self.task)
+        return o.t()
+
+    def episode_score(self):
+        """simulate()'s `score`: CUDA view [N] of the reward summed over each env's running episode."""
+        return self._episode_buffer("score")
+
+    def episode_length(self):
+        """simulate()'s `length`: CUDA view [N] (int32) of the control steps of each env's running episode."""
+        return self._episode_buffer("length")
+
+    def episode_totals(self, clear=True):
+        """Enqueue the batch's episode totals on the current stream (no sync): CUDA view [4] float64 of episodes submitted,
+        episodes ended non-finite, their score sum and length sum.  The next call overwrites it.  clear=True starts the next
+        totals from zero (StreamingMean.clear); running episodes go on."""
+        self._episode_buffer("summary")
+        self._call(self._L.rexsim_episode_summary, self._h, int(bool(clear)))
+        return self._episode["summary"]
+
+    def episode_summary(self, clear=True):
+        """What simulate() logs (simulate.py:95-106): {'count', 'nonfinite', 'mean_score', 'mean_length'} over the episodes
+        that ended since the last clear; the means are None when none did.  One device sync."""
+        return summarize_episodes(self.episode_totals(clear))
 
     @property
     def launch_count(self):

@@ -5,7 +5,7 @@ no data-path collective.  Reset draws key on the GLOBAL env id (RexSimConfig.env
 produces exactly the trajectories of the single-GPU run.  The one optional collective is an all-gather
 of the packed per-rank outputs [n, O + 2] = (obs | reward | done) for a learner that wants the whole batch on
 every rank; it is a single NCCL call on the step stream (torch.distributed, backend nccl on GPUs, gloo in the
-CPU tests)."""
+CPU tests).  The other is an all-reduce of the four episode totals (episode_summary) when the summary is logged."""
 import torch
 import torch.distributed as dist
 
@@ -36,6 +36,16 @@ def all_gather_outputs(obs, reward, done, group=None):
     out = torch.empty((world * packed.shape[0], packed.shape[1]), dtype=packed.dtype, device=packed.device)
     dist.all_gather_into_tensor(out, packed, group=group)
     return unpack_outputs(out)
+
+
+def episode_summary(env, group=None, clear=True):
+    """simulate()'s episode summary over every rank's shard: one all-reduce (sum) of the shards' episode totals, then the
+    means of the whole batch on every rank (BatchedRexEnv.episode_summary of a single-GPU run)."""
+    from .envs.batched_env import summarize_episodes
+    totals = env.episode_totals(clear).clone()
+    if dist.is_initialized() and dist.get_world_size(group) > 1:
+        dist.all_reduce(totals, op=dist.ReduceOp.SUM, group=group)
+    return summarize_episodes(totals)
 
 
 def make_sharded_env(global_envs, rank=None, world=None, **kwargs):
