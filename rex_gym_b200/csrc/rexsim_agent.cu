@@ -250,8 +250,8 @@ __global__ void __launch_bounds__(512, 1) perform_kernel(const PerformArgs P) {
 // two core matrices one instruction reads along K are LBO bytes apart, 8-row groups SBO = 128 bytes apart:
 //   byte(row, k) = (k / 4) * LBO + (row / 8) * 128 + (row % 8) * 16 + (k % 4) * 4,   LBO = rows * 16.
 // Layer 1 writes A directly in that form (one 16-byte store per (env, 4 hidden units)).
-// TF32 keeps 11 significant bits: tests/test_gpu_agent.py bounds the error against the fp32 kernel, which stays the
-// parity default.
+// TF32 keeps 11 significant bits: tests/test_gpu_agent_rounding.py holds exact networks bit for bit and realistic ones to a
+// bound propagated from the tensor cores' accumulation model; the fp32 kernel stays the parity default.
 // -------------------------------------------------------------------------------------------------------------------
 namespace tc {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }

@@ -201,8 +201,13 @@ def test_scans_match_the_oracle_in_both_layouts():
 
 
 def test_rollout_graph_equals_the_step_by_step_loop():
+    rollout_graph_equals_the_step_by_step_loop(tensor_cores=False)
+
+
+def rollout_graph_equals_the_step_by_step_loop(tensor_cores):
     """simulate(): T control steps of perform -> env.step -> experience captured as one CUDA graph; same buffers as the
-    unrolled loop on twin environments, and consistent with stepping the env by hand with the recorded actions."""
+    unrolled loop on twin environments, and consistent with stepping the env by hand with the recorded actions.  With
+    tensor_cores=True (test_gpu_agent_rounding.py) the networks run perform_tc_kernel."""
     import rex_gym_b200 as R
     from rex_gym_b200.agents import ForwardGaussianPolicy, Rollout
     n, T = 512, 16
@@ -210,7 +215,7 @@ def test_rollout_graph_equals_the_step_by_step_loop():
     outs = []
     for use_graph in (False, True):
         env = R.BatchedRexEnv(**kw)
-        net = ForwardGaussianPolicy(env.obs_dim, env.action_dim, seed=3)
+        net = ForwardGaussianPolicy(env.obs_dim, env.action_dim, seed=3, tensor_cores=tensor_cores)
         ro = Rollout(env, net, T, seed=17, training=True, use_graph=use_graph)
         a = {k: v.clone() for k, v in ro.collect().items()}
         b = {k: v.clone() for k, v in ro.collect().items()}               # second window: continues the episodes
