@@ -36,10 +36,17 @@ class RexAgentConfig(C.Structure):
                 ("observ_clip", C.c_float), ("reward_clip", C.c_float)]
 
 
+class RexRnnConfig(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("hidden1", C.c_int32), ("cell", C.c_int32), ("num_envs", C.c_int32)]
+
+
+REXRNN_GRU, REXRNN_LINEAR = 0, 1
+
 _i32, _i64, _u32, _u64, _f32, _ptr = C.c_int32, C.c_int64, C.c_uint32, C.c_uint64, C.c_float, C.c_void_p
 _out, _sim_cfg, _agent_cfg = C.POINTER, C.POINTER(RexSimConfig), C.POINTER(RexAgentConfig)
+_rnn_cfg = C.POINTER(RexRnnConfig)
 
-# name: (restype, argtypes) of every function of include/rexsim.h and include/rexsim_agent.h.  load() declares exactly these,
+# name: (restype, argtypes) of every function of include/rexsim.h, include/rexsim_agent.h and include/rexsim_recurrent.h.  load() declares exactly these,
 # and the export lists below are its keys: a function ctypes has no signature for would get C ints and truncated pointers.
 SIGNATURES = {
     "rexsim_obs_dim": (C.c_int, [_i32, _i32]),
@@ -90,9 +97,19 @@ SIGNATURES = {
     "rexagent_lambda_advantage": (C.c_int, [_ptr, _ptr, _ptr, _i32, _i32, _i64, _i64, _f32, _ptr, _ptr]),
     "rexagent_gae_segments": (C.c_int, [_ptr, _ptr, _ptr, _i32, _i32, _f32, _f32, _ptr, _ptr, _ptr]),
     "rexagent_launch_count": (_i64, [_ptr]),
+    "rexrnn_policy_floats": (_i64, [_agent_cfg, _rnn_cfg]),
+    "rexrnn_check": (C.c_int, [_agent_cfg, _rnn_cfg]),
+    "rexrnn_create": (C.c_int, [_ptr, _rnn_cfg, _out(_ptr)]),
+    "rexrnn_destroy": (None, [_ptr]),
+    "rexrnn_set_params": (C.c_int, [_ptr, _ptr, _i64]),
+    "rexrnn_get_params": (C.c_int, [_ptr, _ptr, _i64]),
+    "rexrnn_state_buffer": (C.c_int, [_ptr, _out(_ptr)]),
+    "rexrnn_perform": (C.c_int, [_ptr, _ptr, _ptr, _i32, _i32, _u64, _u32, _u32] + [_ptr] * 6),
+    "rexrnn_launch_count": (_i64, [_ptr]),
 }
 EXPORTS = [n for n in SIGNATURES if n.startswith("rexsim_")]
 AGENT_EXPORTS = [n for n in SIGNATURES if n.startswith("rexagent_")]
+RNN_EXPORTS = [n for n in SIGNATURES if n.startswith("rexrnn_")]
 
 _LIB = None
 

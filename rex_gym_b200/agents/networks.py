@@ -134,11 +134,7 @@ class ForwardGaussianPolicy(object):
     def perform(self, observ, training=False, seed=0, step=0, env_offset=0, out=None, observ_copy=None):
         """observ: CUDA float32 [n][O].  Returns dict(action [n][A], mean [n][A], logprob [n], value [n]) of CUDA tensors
         (pass `out` to reuse buffers, e.g. slices of a rollout)."""
-        if not (isinstance(observ, torch.Tensor) and observ.is_cuda and observ.dtype == torch.float32 and observ.is_contiguous()):
-            raise ValueError("observ must be a contiguous CUDA float32 tensor")
-        n = observ.shape[0]
-        if observ.dim() != 2 or observ.shape[1] != self.O:
-            raise ValueError("Invalid observation shape %s, expected (n, %d)" % (tuple(observ.shape), self.O))
+        n = check_observ(observ, self.O)
         if out is None:
             dev = observ.device
             out = dict(action=torch.empty((n, self.A), device=dev), mean=torch.empty((n, self.A), device=dev),
@@ -194,6 +190,15 @@ class ForwardGaussianPolicy(object):
             self.close()
         except Exception:
             pass
+
+
+def check_observ(observ, O):
+    """The batch size of a perform call's observations; raises unless they are a contiguous CUDA float32 [n][O] tensor."""
+    if not (isinstance(observ, torch.Tensor) and observ.is_cuda and observ.dtype == torch.float32 and observ.is_contiguous()):
+        raise ValueError("observ must be a contiguous CUDA float32 tensor")
+    if observ.dim() != 2 or observ.shape[1] != O:
+        raise ValueError("Invalid observation shape %s, expected (n, %d)" % (tuple(observ.shape), O))
+    return observ.shape[0]
 
 
 def read_tf_policy(directory_or_prefix):

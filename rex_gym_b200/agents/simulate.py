@@ -7,6 +7,9 @@
 
 Environments that finish are restarted inside the step kernel (auto_reset), which is what simulate() does at the top of
 the next iteration (`begin_episode`, :117-120): the observation stored after a `done` is the first one of the new episode.
+A recurrent network (RecurrentGaussianPolicy) gets the matching episode-start mask with every perform: all ones after
+reset(), else the `done` row of the previous control step -- for the first step of a collect, the last row of the previous
+one, kept in a buffer the captured graph owns.
 The whole T-step loop is captured once into a CUDA graph and replayed: no host round trip per step (SURVEY.md 8(f) row 1).
 """
 import torch
@@ -20,6 +23,8 @@ class Rollout(object):
             raise ValueError("Rollout needs an env created with auto_reset=True")
         if network.O != env.obs_dim or network.A != env.action_dim:
             raise ValueError("network (%d -> %d) does not fit the env (%d -> %d)" % (network.O, network.A, env.obs_dim, env.action_dim))
+        if getattr(network, "recurrent", False) and network.num_envs < env.num_envs:
+            raise ValueError("the network keeps cell state for %d envs, the env has %d" % (network.num_envs, env.num_envs))
         self.env, self.net, self.T, self.seed, self.training = env, network, int(horizon), int(seed), bool(training)
         N, O, A, T, dev = env.num_envs, env.obs_dim, env.action_dim, self.T, env.device
         f32 = dict(dtype=torch.float32, device=dev)
@@ -31,6 +36,8 @@ class Rollout(object):
         self.reward = torch.zeros((T, N), **f32)
         self.done = torch.zeros((T, N), dtype=torch.uint8, device=dev)
         self._cur = torch.zeros((N, O), **f32)             # observation the next action is computed from
+        self._recurrent = bool(getattr(network, "recurrent", False))
+        self._begin = torch.ones((N,), dtype=torch.uint8, device=dev) if self._recurrent else None    # episode starts of step 0
         self._graph = None
         import torch.distributed as dist
         if use_graph and dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
@@ -42,17 +49,24 @@ class Rollout(object):
         """simulate(reset=True): restart every environment."""
         idx = torch.arange(self.env.num_envs, device=self.env.device, dtype=torch.int32)
         self._cur.copy_(self.env.reset(idx))
+        if self._recurrent:
+            self._begin.fill_(1)
 
     def _loop(self):
         env, net, T = self.env, self.net, self.T
         for t in range(T):
-            net.perform(self._cur, training=self.training, seed=self.seed, step=0, env_offset=env._cfg.env_offset,
+            step = dict(training=self.training, seed=self.seed, step=0, env_offset=env._cfg.env_offset,
                         out=dict(action=self.action[t], mean=self.mean[t], logprob=self.logprob[t], value=self.value[t]),
                         observ_copy=self.observ[t])
+            if self._recurrent:
+                step["begin"] = self._begin if t == 0 else self.done[t - 1]
+            net.perform(self._cur, **step)
             env.step_into(self.action[t], self._cur, self.reward[t], self.done[t])
             if self.training:
                 net.experience(self.observ[t], self.reward[t])
         net.perform(self._cur, training=False, out=dict(value=self.value[T]))       # bootstrap value of the last observation
+        if self._recurrent:
+            self._begin.copy_(self.done[T - 1])
 
     def collect(self):
         """Run T control steps for every env; returns views of the rollout buffers (valid until the next collect)."""
@@ -65,12 +79,15 @@ class Rollout(object):
                 side.wait_stream(torch.cuda.current_stream(self.env.device))
                 # warm-up outside capture (lazy kernel loading must not happen while capturing); the warm-up advances the
                 # environments and the filters, so everything is snapshotted first and put back afterwards
-                snap = (self.env.state_dict(), self.net.state_dict(), self._cur.clone())
+                snap = (self.env.state_dict(), self.net.state_dict(), self._cur.clone(),
+                        None if self._begin is None else self._begin.clone())
                 with torch.cuda.stream(side):
                     self._loop()
                 torch.cuda.current_stream(self.env.device).wait_stream(side)
                 torch.cuda.synchronize(self.env.device)
                 self.env.load_state_dict(snap[0]); self.net.load_state_dict(snap[1]); self._cur.copy_(snap[2])
+                if self._begin is not None:
+                    self._begin.copy_(snap[3])
                 torch.cuda.synchronize(self.env.device)
                 self._graph = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(self._graph):

@@ -17,7 +17,7 @@ STAMP = os.path.join(HERE, "librexsim.srchash")
 KERNEL_UNITS = [0, 1, 2, 3, 4, 5, 6, 7, 100]           # see the tail of rexsim_kernel.cu
 OTHER_SOURCES = ["rexsim_capi.cu", "rexsim_agent.cu", "rexsim_render.cu"]
 HEADERS = ["rexsim_kernel.cuh", "rexsim_arm.cuh", "rexsim_host.h", os.path.join("..", "..", "include", "rexsim.h"),
-           os.path.join("..", "..", "include", "rexsim_agent.h")]
+           os.path.join("..", "..", "include", "rexsim_agent.h"), os.path.join("..", "..", "include", "rexsim_recurrent.h")]
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17"]
 NVCC_FLAGS = ARCH_FLAGS + ["-Xcompiler", "-fPIC"]
 

@@ -1,5 +1,6 @@
 // rexsim_agent.cu -- device-side agent glue around the step kernel (include/rexsim_agent.h):
 //   perform     : StreamingNormalize.transform + ForwardGaussianPolicy (policy MLP, value MLP) + sampling, one fused kernel
+//   rexrnn_*    : the RecurrentGaussianPolicy (GRU) and LinearGaussianPolicy policies of include/rexsim_recurrent.h
 //   experience  : StreamingNormalize.update for observations and rewards, one deterministic reduction kernel
 //   scans       : discounted_return / lambda_advantage (reference row semantics) and the done-aware time-major GAE
 // fp32 throughout (the reference's TF graph is fp32): the MLP is computed on the CUDA cores with a register-tiled
@@ -7,6 +8,7 @@
 #include "rexsim_kernel.cuh"
 #include "rexsim_host.h"
 #include "../../include/rexsim_agent.h"
+#include "../../include/rexsim_recurrent.h"
 #include <cstring>
 #include <vector>
 #include <type_traits>
@@ -56,6 +58,7 @@ struct PerformArgs {
     AgentDev D;
     const float* __restrict__ observ;
     int n, training;
+    int net_base;                         // perform_kernel: network of blockIdx.y = 0 (1: the value network alone)
     uint64_t seed;
     uint32_t step, env_offset;
     float* action; float* mean; float* logprob; float* value; float* observ_copy;
@@ -140,7 +143,7 @@ __global__ void __launch_bounds__(512, 1) perform_kernel(const PerformArgs P) {
     const RexAgentConfig& c = P.D.cfg;
     const int O = c.obs_dim, A = c.action_dim, H1 = c.hidden1, H2 = c.hidden2;
     const int nt = blockDim.x, tid = threadIdx.x;
-    const int net = blockIdx.y;
+    const int net = blockIdx.y + P.net_base;
     const PerformSmem S = perform_smem(max(P.D.pol_floats, P.D.val_floats), H1, TM);
     float* W = smem;                          // weights of this CTA's network
     float* xs = smem + S.xs;
@@ -232,6 +235,204 @@ __global__ void __launch_bounds__(512, 1) perform_kernel(const PerformArgs P) {
             head_outputs<0>(P, net, A, env, step, s, W + L.logstd);
         }
     }
+}
+
+// -------------------------------------------------------------------------------------------------------------------
+// RecurrentGaussianPolicy / LinearGaussianPolicy policies (include/rexsim_recurrent.h).  The value network is the agent's
+// perform_kernel on the value block alone (net_base = 1); normalisation, sampling and log-density are load_obs_tile and
+// head_outputs above, so one (seed, env_offset + env, step) draws the same noise as ForwardGaussianPolicy.
+// -------------------------------------------------------------------------------------------------------------------
+constexpr int RNN_MAX_H1 = 256, RNN_MAX_G = 128;
+constexpr int RNN_TM = 64;          // envs per tile: 4 per thread x 16 env groups
+constexpr int RNN_KC = 16;          // weight rows per streamed chunk
+
+// the GRU policy block (include/rexsim_recurrent.h), offsets in floats; every array starts on a 16-byte boundary (H1, G
+// multiples of 4)
+template <typename I> struct RnnLayout { I W1, b1, w_ru, b_ru, w_c, b_c, W3, b3, logstd, floats; };
+template <typename I>
+__host__ __device__ constexpr RnnLayout<I> rnn_layout(I O, I A, I H1, I G) {
+    const I b1 = O * H1, wru = b1 + H1, bru = wru + (H1 + G) * 2 * G, wc = bru + 2 * G, bc = wc + (H1 + G) * G, W3 = bc + G,
+            b3 = W3 + G * A, ls = b3 + A;
+    return {0, b1, wru, bru, wc, bc, W3, b3, ls, (ls + A + 3) & ~(I)3};
+}
+// the linear policy block: W [O][A] at 0, b [A] at O * A, logstd [A] after it
+__host__ __device__ constexpr int64_t linear_floats(int64_t O, int64_t A) { return (O * A + 2 * A + 3) & ~(int64_t)3; }
+
+struct RnnArgs {
+    PerformArgs P;                        // observations, filters, sampling keys, outputs (P.value is the value pass's)
+    const float* __restrict__ params;     // the policy block
+    float* state;                         // [num_envs][G]
+    const uint8_t* __restrict__ begin;    // [n] or null
+    int H1, G;
+};
+
+// dynamic shared memory of gru_policy_kernel, offsets in floats: xs [O][TM], a1 [H1][TM] (dense layer), h [G][TM] (state, then
+// the new state), rh [G][TM] (r * h), w [2][KC][2G] (streamed weight chunks), head [TM][AG_MAX_A], nrm [2][AG_MAX_O]
+struct RnnSmem { size_t xs, a1, h, rh, w, head, nrm, bytes; };
+__host__ __device__ constexpr RnnSmem rnn_smem(int O, int H1, int G) {
+    const size_t a1 = (size_t)O * RNN_TM, h = a1 + (size_t)H1 * RNN_TM, rh = h + (size_t)G * RNN_TM, w = rh + (size_t)G * RNN_TM,
+                 head = w + 2 * (size_t)RNN_KC * 2 * G, nrm = head + (size_t)RNN_TM * AG_MAX_A;
+    return {0, a1, h, rh, w, head, nrm, (nrm + 2 * AG_MAX_O) * sizeof(float)};
+}
+
+__device__ __forceinline__ void cp_async16(float* dst, const float* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ float sigmoidf(float x) { return 1.f / (1.f + expf(-x)); }
+
+// acc[s][i][j] += sum_k in[k][env 4 eg + i] * Wg[k][s G + 4 og + j] over the K = H1 + G rows of the cell input [x, hx]: rows
+// k < H1 from a1, the rest from hx.  Wg [K][S G] is streamed from global memory (L2) in KC-row chunks through the two halves of
+// wbuf, cp.async double-buffered: chunk c + 1 is in flight while chunk c is used.  Every thread calls this (it syncs); threads
+// past the G / 4 column groups only help with the copies.  Per row: one LDS.128 of activations and S of weights feed 16 S FFMAs.
+template <int S>
+__device__ __forceinline__ void gru_gemm(const float* __restrict__ Wg, int H1, int G, const float* a1, const float* hx, float* wbuf,
+                                         bool active, int eg, int og, int tid, int nt, float (&acc)[S][4][4]) {
+    const int K = H1 + G, NC = S * G, nchunks = (K + RNN_KC - 1) / RNN_KC;
+    const int half = RNN_KC * 2 * G;
+    auto stage = [&](int c) {
+        const int k0 = c * RNN_KC, rows = min(RNN_KC, K - k0);
+        float* dst = wbuf + (c & 1) * half;
+        const float* src = Wg + (size_t)k0 * NC;
+        for (int i = 4 * tid; i < rows * NC; i += 4 * nt) cp_async16(dst + i, src + i);
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+    stage(0);
+    for (int c = 0; c < nchunks; c++) {
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        __syncthreads();                                // chunk c is in; every thread is done with chunk c - 1's half
+        if (c + 1 < nchunks) stage(c + 1);
+        if (!active) continue;
+        const float* wb = wbuf + (c & 1) * half + 4 * og;
+        const int k0 = c * RNN_KC, rows = min(RNN_KC, K - k0);
+#pragma unroll 4
+        for (int kk = 0; kk < rows; kk++) {
+            const int k = k0 + kk;
+            const float4 x = ld4((k < H1 ? a1 + (size_t)k * RNN_TM : hx + (size_t)(k - H1) * RNN_TM) + 4 * eg);
+            const float xv[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+            for (int s = 0; s < S; s++) {
+                const float4 w = ld4(wb + kk * NC + s * G);
+#pragma unroll
+                for (int i = 0; i < 4; i++) {
+                    acc[s][i][0] = fmaf(xv[i], w.x, acc[s][i][0]); acc[s][i][1] = fmaf(xv[i], w.y, acc[s][i][1]);
+                    acc[s][i][2] = fmaf(xv[i], w.z, acc[s][i][2]); acc[s][i][3] = fmaf(xv[i], w.w, acc[s][i][3]);
+                }
+            }
+        }
+    }
+}
+
+// Persistent CTAs over 64-env tiles, one CTA per SM; per tile: normalise -> dense H1 ReLU -> gates [r | u] (register tile:
+// 4 envs x 4 units of r and the same 4 units of u per thread) -> r * h -> candidate c (same tile) -> h' = u h + (1 - u) c in
+// place of h -> state write-back -> head (one thread per (env, action)) -> tanh / sampling.  blockDim.x = max(16 G / 4, 128).
+__global__ void __launch_bounds__(512, 1) gru_policy_kernel(const RnnArgs R) {
+    const PerformArgs& P = R.P;
+    extern __shared__ __align__(16) float smem[];
+    const int O = P.D.cfg.obs_dim, A = P.D.cfg.action_dim, H1 = R.H1, G = R.G;
+    const int nt = blockDim.x, tid = threadIdx.x, eg = tid & 15, og = tid >> 4;
+    const bool active = og < G / 4;
+    const RnnSmem S = rnn_smem(O, H1, G);
+    float* xs = smem + S.xs; float* a1 = smem + S.a1; float* h = smem + S.h; float* rh = smem + S.rh;
+    float* wbuf = smem + S.w; float* head = smem + S.head; float* nrm = smem + S.nrm;
+    const RnnLayout<int64_t> L = rnn_layout<int64_t>(O, A, H1, G);
+    const float* W = R.params;
+    load_normaliser(P.D, O, nrm, tid);
+    __syncthreads();
+    const int ntiles = (P.n + RNN_TM - 1) / RNN_TM;
+    const uint32_t step = P.step + (uint32_t)P.D.cnt[2];
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const int e0 = tile * RNN_TM;
+        __syncthreads();                                // previous tile's head is done with h and head
+        load_obs_tile<RNN_TM>(P, O, 0, nrm, xs, e0, tid, nt);
+        for (int i = tid; i < G * RNN_TM; i += nt) {    // the state rows, coalesced; zero where an episode begins and past n
+            const int e = i / G, j = i - e * G, env = e0 + e;
+            h[j * RNN_TM + e] = env < P.n && !(R.begin && R.begin[env]) ? R.state[(size_t)env * G + j] : 0.f;
+        }
+        __syncthreads();
+        for (int i = tid; i < H1 * RNN_TM; i += nt) {   // dense layer
+            const int k = i / RNN_TM, e = i - k * RNN_TM;
+            float s = W[L.b1 + k];
+            for (int o = 0; o < O; o++) s = fmaf(xs[o * RNN_TM + e], W[L.W1 + o * H1 + k], s);
+            a1[i] = fmaxf(s, 0.f);
+        }
+        float ru[2][4][4], cc[1][4][4];
+        if (active) {
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                const float br = W[L.b_ru + 4 * og + j], bu = W[L.b_ru + G + 4 * og + j], bc = W[L.b_c + 4 * og + j];
+#pragma unroll
+                for (int i = 0; i < 4; i++) { ru[0][i][j] = br; ru[1][i][j] = bu; cc[0][i][j] = bc; }
+            }
+        }
+        gru_gemm<2>(W + L.w_ru, H1, G, a1, h, wbuf, active, eg, og, tid, nt, ru);      // its first sync covers a1
+        if (active) {                                   // r * h for the candidate; u stays in ru[1]
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+#pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    const int idx = (4 * og + j) * RNN_TM + 4 * eg + i;
+                    rh[idx] = sigmoidf(ru[0][i][j]) * h[idx];
+                    ru[1][i][j] = sigmoidf(ru[1][i][j]);
+                }
+        }
+        __syncthreads();                                // rh complete; the weight halves are free again
+        gru_gemm<1>(W + L.w_c, H1, G, a1, rh, wbuf, active, eg, og, tid, nt, cc);
+        if (active) {                                   // nothing reads h any more but the thread that owns each element
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+#pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    const int idx = (4 * og + j) * RNN_TM + 4 * eg + i;
+                    const float u = ru[1][i][j];
+                    h[idx] = fmaf(u, h[idx], (1.f - u) * tanhf(cc[0][i][j]));
+                }
+        }
+        __syncthreads();
+        for (int i = tid; i < G * RNN_TM; i += nt) {    // the new state, coalesced
+            const int e = i / G, j = i - e * G, env = e0 + e;
+            if (env < P.n) R.state[(size_t)env * G + j] = h[j * RNN_TM + e];
+        }
+        for (int i = tid; i < RNN_TM * A; i += nt) {    // head sums, one thread per (env, action), b3 first then the units in order
+            const int e = i / A, a = i - e * A;
+            float s = W[L.b3 + a];
+            for (int j = 0; j < G; j++) s = fmaf(h[j * RNN_TM + e], W[L.W3 + j * A + a], s);
+            head[e * AG_MAX_A + a] = s;
+        }
+        __syncthreads();
+        if (tid < RNN_TM && e0 + tid < P.n) {
+            float s[AG_MAX_A];
+#pragma unroll
+            for (int a = 0; a < AG_MAX_A; a++) s[a] = a < A ? head[tid * AG_MAX_A + a] : 0.f;
+            head_outputs<0>(P, 0, A, e0 + tid, step, s, W + L.logstd);
+        }
+    }
+}
+
+// LinearGaussianPolicy: one CTA per 128-env tile, one thread per env: s = b + x . W, then head_outputs
+constexpr int LIN_TM = 128;
+__global__ void __launch_bounds__(LIN_TM) linear_policy_kernel(const RnnArgs R) {
+    const PerformArgs& P = R.P;
+    __shared__ __align__(16) float xs[AG_MAX_O * LIN_TM];
+    __shared__ float nrm[2 * AG_MAX_O];
+    const int O = P.D.cfg.obs_dim, A = P.D.cfg.action_dim, tid = threadIdx.x, e0 = blockIdx.x * LIN_TM;
+    const float* W = R.params;
+    load_normaliser(P.D, O, nrm, tid);
+    __syncthreads();
+    load_obs_tile<LIN_TM>(P, O, 0, nrm, xs, e0, tid, LIN_TM);
+    __syncthreads();
+    if (e0 + tid >= P.n) return;
+    float s[AG_MAX_A];
+#pragma unroll
+    for (int a = 0; a < AG_MAX_A; a++) {
+        if (a < A) {
+            float v = W[O * A + a];
+            for (int o = 0; o < O; o++) v = fmaf(xs[o * LIN_TM + tid], W[o * A + a], v);
+            s[a] = v;
+        } else {
+            s[a] = 0.f;
+        }
+    }
+    head_outputs<0>(P, 0, A, e0 + tid, P.step + (uint32_t)P.D.cnt[2], s, W + O * A + A);
 }
 
 
@@ -590,6 +791,16 @@ struct RexAgent {
     int precision = 0;                 // 0: fp32 on the CUDA cores (parity default); 1: layer 2 on the tensor cores in TF32
 };
 
+struct RexRnn {
+    RexAgent* agent;                   // filters, step counter and value network
+    RexRnnConfig cfg;
+    DeviceBuffers mem;
+    float* params = nullptr;           // the policy block
+    float* state = nullptr;            // GRU: [num_envs][cell]
+    int64_t floats = 0;
+    int64_t launches = 0;
+};
+
 // the instance compiled for this network's input / output widths (the reference's tasks: 4 or 16 observations, 1-8 actions)
 typedef void (*PerformTcKernel)(const PerformArgs);
 static PerformTcKernel perform_tc_pick(const RexAgentConfig* c) {
@@ -733,29 +944,41 @@ int rexagent_get_filters(RexAgent* a, int64_t* counts, float* om, float* ov, flo
     return REXSIM_OK;
 }
 
+// the arguments of one perform call (net_base 0: perform_kernel's blockIdx.y picks the network)
+static PerformArgs perform_args(const RexAgent* a, const float* observ, int32_t n, int32_t training, uint64_t seed, uint32_t step,
+                                uint32_t env_offset, float* action, float* mean, float* logprob, float* value, float* observ_copy) {
+    PerformArgs P;
+    P.D = a->D; P.observ = observ; P.n = n; P.training = training; P.net_base = 0; P.seed = seed; P.step = step;
+    P.env_offset = env_offset; P.action = action; P.mean = mean; P.logprob = logprob; P.value = value; P.observ_copy = observ_copy;
+    return P;
+}
+
+// perform_kernel on `nets` networks from P.net_base, at most `ctas` persistent CTAs per network: 64-env tiles while there are
+// fewer 128-env tiles than CTAs, so that more SMs get a tile, 128-env tiles (8 x 4 register tile per thread) above
+static void perform_fp32_launch(const RexAgent* a, const PerformArgs& P, int ctas, int nets, cudaStream_t st) {
+    const int tm = (P.n + 127) / 128 >= ctas ? 128 : 64;
+    const int ntiles = (P.n + tm - 1) / tm;
+    const dim3 grid(ntiles < ctas ? ntiles : ctas, nets);
+    const int threads = 16 * (a->D.cfg.hidden2 / 4) > tm ? 16 * (a->D.cfg.hidden2 / 4) : tm;
+    if (tm == 128) perform_kernel<128><<<grid, threads, perform_smem_bytes(&a->D.cfg, 128), st>>>(P);
+    else perform_kernel<64><<<grid, threads, perform_smem_bytes(&a->D.cfg, 64), st>>>(P);
+}
+
 int rexagent_perform(RexAgent* a, const float* observ, int32_t n, int32_t training, uint64_t seed, uint32_t step,
                      uint32_t env_offset, float* action, float* mean, float* logprob, float* value, float* observ_copy,
                      void* stream) {
     if (!a || !observ) return fail(REXSIM_ERR_INVALID, "null argument");
     if (n <= 0) return fail(REXSIM_ERR_INVALID, "agent: n must be positive");
-    PerformArgs P;
-    P.D = a->D; P.observ = observ; P.n = n; P.training = training; P.seed = seed; P.step = step; P.env_offset = env_offset;
-    P.action = action; P.mean = mean; P.logprob = logprob; P.value = value; P.observ_copy = observ_copy;
-    // one CTA per SM (the weights fill most of the shared memory); the two networks run in different CTAs (blockIdx.y).
-    // The wgmma path always uses 128-env tiles; the fp32 kernel uses 64-env tiles on small batches so that more SMs get a
-    // tile, 128-env tiles (8 x 4 register tile per thread) on large ones.
+    const PerformArgs P = perform_args(a, observ, n, training, seed, step, env_offset, action, mean, logprob, value, observ_copy);
+    // one CTA per SM (the weights fill most of the shared memory); the two networks run in different CTAs (blockIdx.y), on
+    // half the SMs each.  The wgmma path always uses 128-env tiles.
     const int half = a->sm_count / 2 > 0 ? a->sm_count / 2 : 1;
-    const bool tc_path = a->precision == 1;
-    const int tm = tc_path || (n + 127) / 128 >= half ? 128 : 64;
-    const int ntiles = (n + tm - 1) / tm;
-    const dim3 grid(ntiles < half ? ntiles : half, 2);
     const cudaStream_t st = (cudaStream_t)stream;
-    if (tc_path) {
-        perform_tc_pick(&a->D.cfg)<<<grid, tc::THREADS, perform_tc_smem_bytes(&a->D.cfg), st>>>(P);
+    if (a->precision == 1) {
+        const int ntiles = (n + 127) / 128;
+        perform_tc_pick(&a->D.cfg)<<<dim3(ntiles < half ? ntiles : half, 2), tc::THREADS, perform_tc_smem_bytes(&a->D.cfg), st>>>(P);
     } else {
-        const int threads = 16 * (a->D.cfg.hidden2 / 4) > tm ? 16 * (a->D.cfg.hidden2 / 4) : tm;
-        if (tm == 128) perform_kernel<128><<<grid, threads, perform_smem_bytes(&a->D.cfg, 128), st>>>(P);
-        else perform_kernel<64><<<grid, threads, perform_smem_bytes(&a->D.cfg, 64), st>>>(P);
+        perform_fp32_launch(a, P, half, 2, st);
     }
     return enqueue(a, cudaGetLastError(), "perform launch");
 }
@@ -798,5 +1021,100 @@ int rexagent_gae_segments(const float* reward, const float* value, const uint8_t
     return REXSIM_OK;
 }
 int64_t rexagent_launch_count(const RexAgent* a) { return a ? a->launches : 0; }
+
+// ---- include/rexsim_recurrent.h ------------------------------------------------------------------------------------------
+int64_t rexrnn_policy_floats(const RexAgentConfig* c, const RexRnnConfig* r) {
+    if (!c || !r) return 0;
+    if (r->kind == REXRNN_LINEAR) return linear_floats(c->obs_dim, c->action_dim);
+    return rnn_layout<int64_t>(c->obs_dim, c->action_dim, r->hidden1, r->cell).floats;
+}
+int rexrnn_check(const RexAgentConfig* c, const RexRnnConfig* r) {
+    int rc = check_cfg(c);
+    if (rc) return rc;
+    if (!r) return fail(REXSIM_ERR_INVALID, "null recurrent config");
+    if (r->kind != REXRNN_GRU && r->kind != REXRNN_LINEAR) return fail(REXSIM_ERR_INVALID, "rnn: kind must be REXRNN_GRU or REXRNN_LINEAR");
+    if (r->num_envs <= 0) return fail(REXSIM_ERR_INVALID, "rnn: num_envs must be positive");
+    if (r->kind == REXRNN_GRU) {
+        if (r->hidden1 <= 0 || r->hidden1 > RNN_MAX_H1 || r->cell <= 0 || r->cell > RNN_MAX_G || (r->hidden1 & 3) || (r->cell & 3))
+            return fail(REXSIM_ERR_UNSUPPORTED, "rnn: hidden1 <= 256, cell <= 128, both multiples of 4");
+        if (rnn_smem(c->obs_dim, r->hidden1, r->cell).bytes > 227 * 1024)       // 174 KB at the largest accepted shape
+            return fail(REXSIM_ERR_UNSUPPORTED, "rnn: the cell's tile does not fit the 227 KB of shared memory");
+    }
+    return REXSIM_OK;
+}
+int rexrnn_create(RexAgent* a, const RexRnnConfig* cfg, RexRnn** out) {
+    if (!a || !out) return fail(REXSIM_ERR_INVALID, "null argument");
+    int rc = rexrnn_check(&a->D.cfg, cfg);
+    if (rc) return rc;
+    RexRnn* r = new RexRnn();
+    struct Guard { RexRnn* r; ~Guard() { if (r) rexrnn_destroy(r); } } guard{r};
+    r->agent = a; r->cfg = *cfg;
+    r->floats = rexrnn_policy_floats(&a->D.cfg, cfg);
+    if (r->mem.zeroed(&r->params, (size_t)r->floats)) return REXSIM_ERR_CUDA;
+    if (cfg->kind == REXRNN_GRU) {
+        if (r->mem.zeroed(&r->state, (size_t)cfg->num_envs * cfg->cell)) return REXSIM_ERR_CUDA;
+        CK(cudaFuncSetAttribute(gru_policy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)rnn_smem(a->D.cfg.obs_dim, cfg->hidden1, cfg->cell).bytes));
+    }
+    CK(cudaDeviceSynchronize());
+    guard.r = nullptr;
+    *out = r;
+    return REXSIM_OK;
+}
+void rexrnn_destroy(RexRnn* r) {
+    if (!r) return;
+    r->mem.release();
+    delete r;
+}
+int rexrnn_set_params(RexRnn* r, const float* h, int64_t n) {
+    if (!r || !h) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (n != r->floats) return fail(REXSIM_ERR_INVALID, "rnn: parameter block size mismatch");
+    CK(cudaMemcpy(r->params, h, n * sizeof(float), cudaMemcpyHostToDevice));
+    return REXSIM_OK;
+}
+int rexrnn_get_params(RexRnn* r, float* h, int64_t n) {
+    if (!r || !h) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (n != r->floats) return fail(REXSIM_ERR_INVALID, "rnn: parameter block size mismatch");
+    CK(cudaMemcpy(h, r->params, n * sizeof(float), cudaMemcpyDeviceToHost));
+    return REXSIM_OK;
+}
+int rexrnn_state_buffer(RexRnn* r, float** state) {
+    if (!r || !state) return fail(REXSIM_ERR_INVALID, "null argument");
+    *state = r->state;
+    return REXSIM_OK;
+}
+int rexrnn_perform(RexRnn* r, const float* observ, const uint8_t* begin, int32_t n, int32_t training, uint64_t seed, uint32_t step,
+                   uint32_t env_offset, float* action, float* mean, float* logprob, float* value, float* observ_copy, void* stream) {
+    if (!r || !observ) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (n <= 0 || n > r->cfg.num_envs) return fail(REXSIM_ERR_INVALID, "rnn: n must be 1..num_envs");
+    const bool policy = action || mean || logprob;
+    if (observ_copy && !policy) return fail(REXSIM_ERR_INVALID, "rnn: observ_copy is written by the policy pass only");
+    const RexAgent* a = r->agent;
+    const cudaStream_t st = (cudaStream_t)stream;
+    int launches = 0;
+    if (policy) {
+        RnnArgs R;
+        R.P = perform_args(a, observ, n, training, seed, step, env_offset, action, mean, logprob, nullptr, observ_copy);
+        R.params = r->params; R.state = r->state; R.begin = begin; R.H1 = r->cfg.hidden1; R.G = r->cfg.cell;
+        if (r->cfg.kind == REXRNN_GRU) {
+            const int ntiles = (n + RNN_TM - 1) / RNN_TM, threads = 4 * R.G > 128 ? 4 * R.G : 128;
+            gru_policy_kernel<<<ntiles < a->sm_count ? ntiles : a->sm_count, threads,
+                                rnn_smem(a->D.cfg.obs_dim, R.H1, R.G).bytes, st>>>(R);
+        } else {
+            linear_policy_kernel<<<(n + LIN_TM - 1) / LIN_TM, LIN_TM, 0, st>>>(R);
+        }
+        launches++;
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return cuda_fail(e, "rnn policy launch");
+    }
+    if (value) {                       // the agent's value network alone, on every SM
+        PerformArgs P = perform_args(a, observ, n, training, seed, step, env_offset, nullptr, nullptr, nullptr, value, nullptr);
+        P.net_base = 1;
+        perform_fp32_launch(a, P, a->sm_count, 1, st);
+        launches++;
+    }
+    return enqueue(r, cudaGetLastError(), "rnn value launch", launches);
+}
+int64_t rexrnn_launch_count(const RexRnn* r) { return r ? r->launches : 0; }
 
 }  // extern "C"
