@@ -111,9 +111,14 @@ def rand_u32(seed, env, counter, slot):
     return (z >> 32) & 0xFFFFFFFF
 
 
+def uniform_pair(seed, env, step, a):
+    """The sampler's (u1, u2) of action a (rexsim_agent.cu head_outputs): (k + 1/2) / 2^23 for the top 23 bits k of a draw,
+    which the kernel computes exactly in fp32."""
+    return tuple(((rand_u32(seed, env, step, 2 * a + i) >> 9) + 0.5) / 8388608.0 for i in (0, 1))
+
+
 def normal_noise(seed, env, step, a):
-    u1 = ((rand_u32(seed, env, step, 2 * a) >> 8) + 0.5) / 16777216.0
-    u2 = ((rand_u32(seed, env, step, 2 * a + 1) >> 8) + 0.5) / 16777216.0
+    u1, u2 = uniform_pair(seed, env, step, a)
     return math.sqrt(-2.0 * math.log(u1)) * math.cos(2.0 * math.pi * u2)
 
 

@@ -108,9 +108,11 @@ __device__ __forceinline__ void head_outputs(const PerformArgs& P, int net, int 
                 const float ls = logstd[a];
                 float act = mu, z = 0.f;
                 if (P.training) {
+                    // u = (k + 1/2) 2^-23 for the top 23 bits k: k + 0.5 has at most 24 significant bits, so u is exact in fp32
+                    // and lies in [2^-24, 1 - 2^-24] (never 1, where logf would give z = 0)
                     const uint32_t genv = P.env_offset + (uint32_t)env;
-                    const float u1 = ((float)(rand_u32(P.seed, genv, step, 2 * a) >> 8) + 0.5f) * (1.0f / 16777216.0f);
-                    const float u2 = ((float)(rand_u32(P.seed, genv, step, 2 * a + 1) >> 8) + 0.5f) * (1.0f / 16777216.0f);
+                    const float u1 = ((float)(rand_u32(P.seed, genv, step, 2 * a) >> 9) + 0.5f) * 0x1p-23f;
+                    const float u2 = ((float)(rand_u32(P.seed, genv, step, 2 * a + 1) >> 9) + 0.5f) * 0x1p-23f;
                     z = sqrtf(-2.f * logf(u1)) * cospif(2.f * u2);
                     act = fmaf(expf(ls), z, mu);
                 }

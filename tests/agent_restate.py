@@ -9,7 +9,11 @@ Not collected by pytest (like task_outputs.py).  The restatement follows the ker
   is in an order fixed by the code, so the head sums (the value, and the argument of the mean's tanhf) come out bit for bit;
 * perform_tc_kernel<O, A> (tf32): layer 2's operands rounded with cvt.rna.tf32.f32, then D_n = sum_k a_k b_kn and
   S_n = sum_k |a_k b_kn| in fp64 (the products are exact there, and fp64 summation error is about 2^-30 of the accumulation
-  model below, so it is negligible); the head in fp64 from D with a forward error bound for every output.
+  model below, so it is negligible); the head in fp64 from D with a forward error bound for every output;
+* gru_policy_kernel and linear_policy_kernel: every GEMM of the cell, the blend and both heads are fmaf chains in an order
+  the code fixes (fma_chain; the cp.async chunking of gru_gemm does not reorder the rows), so what reaches sigmoidf / tanhf
+  comes out bit for bit; sigmoidf, tanhf and the sampler (head_outputs) are held to error bounds built from the library's
+  documented maximum ulp errors.
 
 fmaf32 is a correctly rounded fp32 fused multiply-add, vectorised; the tests check it against the C library's fmaf.
 """
@@ -23,6 +27,14 @@ OBSERV_CLIP, REWARD_CLIP = 5.0, 10.0          # the clips ForwardGaussianPolicy 
 # CUDA's tanhf: at most 2 ulp from the exact tanh over the whole range (CUDA C++ Programming Guide, maximum ulp errors of
 # the single-precision mathematical functions); the library is built without fast-math, so this is the tanhf that runs
 TANHF_ULP = 2
+# the same table for the other functions the agent kernels call; sqrtf and fp32 division are correctly rounded (0 ulp) in a
+# build without fast-math (nvcc's -prec-sqrt and -prec-div default to true)
+EXPF_ULP, LOGF_ULP, COSPIF_ULP = 2, 1, 1
+# sigmoidf(x) = 1 / (1 + expf(-x)) is exactly 1 for x >= SIGMOID_ONE (expf(-24) < 2^-25 even with expf's error, so 1 + E
+# rounds to 1) and exactly 0 for x <= SIGMOID_ZERO (expf(96) overflows to inf); tests/test_gpu_recurrent_rounding.py asserts both
+SIGMOID_ONE, SIGMOID_ZERO = 24.0, -96.0
+FLT_MAX = float(np.finfo(F32).max)
+LOGPROB_C = F32(0.9189385332046727)           # head_outputs' 0.5 log(2 pi), as the fp32 constant the kernel uses
 
 
 # ---- fp32 arithmetic --------------------------------------------------------------------------------------------------
@@ -189,3 +201,152 @@ def tanh_bound(z, bz):
     z = np.asarray(z, np.float64)
     t = np.tanh(z)
     return bz / np.cosh(np.maximum(np.abs(z) - bz, 0)) ** 2 + TANHF_ULP * ulp32(np.abs(t) + bz)
+
+
+# ---- the transcendental functions and their bounds -------------------------------------------------------------------------
+def sigmoid_bound(x):
+    """Bound on |sigmoidf(x) - sigmoid(x)| for float32 x: expf's error on E = exp(-x), the rounding of 1 + E, its effect on
+    1 / D (|1/D' - 1/D| <= |D' - D| / (D (D - |D' - D|))) and the correctly rounded division.  Where expf(-x) may overflow to
+    inf in fp32, sigmoidf gives 0 and sigmoid(x) itself is added."""
+    x = np.asarray(x, np.float64)
+    with np.errstate(over="ignore"):
+        E = np.exp(-x)
+    E = np.minimum(E, 2.0 ** 200)                          # beyond fp32's range the formula only needs to stay finite
+    dE = EXPF_ULP * ulp32(E)
+    D = 1.0 + E
+    dD = dE + 0.5 * ulp32(D + dE)
+    s = 1.0 / D
+    di = dD / (D * (D - dD))
+    return di + 0.5 * ulp32(s + di) + np.where(E * (1 + 2.0 ** -21) >= FLT_MAX, s, 0.0)
+
+
+def sigmoid(x):
+    with np.errstate(over="ignore"):
+        return 1.0 / (1.0 + np.exp(-np.asarray(x, np.float64)))
+
+
+def uniforms(r):
+    """head_outputs' uniform of a 32-bit draw r: ((float)(r >> 9) + 0.5f) * 2^-23, in float32 operations."""
+    k = (np.asarray(r, np.uint64) >> np.uint64(9)).astype(F32)
+    return (k + F32(0.5)) * F32(2.0 ** -23)
+
+
+def normal_bound(u1, u2):
+    """z = sqrtf(-2 logf(u1)) * cospif(2 u2) for float32 u1, u2 (exact): the exact z and a bound on the kernel's error.
+    logf within LOGF_ULP; -2 logf and 2 u2 are exact scalings; sqrtf correctly rounded; cospif within COSPIF_ULP; the
+    product rounded once."""
+    u1, u2 = np.asarray(u1, np.float64), np.asarray(u2, np.float64)
+    L = np.log(u1)
+    dT = 2 * LOGF_ULP * ulp32(L)
+    T = -2.0 * L
+    S = np.sqrt(T)
+    dS = dT / (np.sqrt(np.maximum(T - dT, 0.0)) + S)
+    dS = dS + 0.5 * ulp32(S + dS)
+    Cs = np.cos(2.0 * np.pi * u2)
+    dC = COSPIF_ULP * ulp32(Cs)
+    Z = S * Cs
+    dZ = S * dC + np.abs(Cs) * dS + dS * dC
+    return Z, dZ + 0.5 * ulp32(np.abs(Z) + dZ)
+
+
+def action_bound(z, dz, logstd, mean):
+    """act = fmaf(expf(ls), z', mu) against mean + exp(ls) z: (the exact value, bound); mean is the kernel's own mu."""
+    E = np.exp(np.asarray(logstd, np.float64))
+    dE = EXPF_ULP * ulp32(E)
+    act = np.asarray(mean, np.float64) + E * z
+    d = E * dz + np.abs(z) * dE + dE * dz
+    return act, d + 0.5 * ulp32(np.abs(act) + d)
+
+
+def logprob_bound(z, dz, logstd):
+    """lp = sum over a of -0.5f * z * z - ls - c (c = LOGPROB_C) against the same sum of the exact z, in fp64: (value, bound).
+    The bound covers the code as written and every FMA contraction nvcc may apply under its default --fmad=true: each of
+    the at most 4 A roundings (the product by z, the two subtractions, the accumulation) is at most u times the largest
+    intermediate, which is below M = sum (0.5 (|z| + dz)^2 + |ls| + c); a contraction only removes roundings.  z's own
+    error enters through |z'^2 - z^2| / 2 <= dz (2 |z| + dz) / 2."""
+    z, dz = np.asarray(z, np.float64), np.asarray(dz, np.float64)
+    ls = np.asarray(logstd, np.float64)
+    c = float(LOGPROB_C)
+    lp = (-0.5 * z * z - ls - c).sum(-1)
+    M = (0.5 * (np.abs(z) + dz) ** 2 + np.abs(ls) + c).sum(-1)
+    k = 4 * z.shape[-1]
+    return lp, (dz * (2 * np.abs(z) + dz) / 2).sum(-1) + k * U32 / (1 - k * U32) * M
+
+
+# ---- gru_policy_kernel / linear_policy_kernel ------------------------------------------------------------------------------
+def fma_chain(x, W, b):
+    """b[j], then one fmaf(x[:, k], W[k, j], .) per row k = 0 .. K-1 in order: float32 [R][C].  This is gru_gemm (x = [a1, h]
+    or [a1, r h], rows below H1 from a1; the 16-row chunks are consumed in order, each from its first row), the GRU head
+    (x = h', W = W3, b = b3), the linear policy (x = the normalised observation, W = pW, b = pb) and layer1 before the ReLU."""
+    x, W = np.asarray(x, F32), np.asarray(W, F32)
+    acc = np.broadcast_to(np.asarray(b, F32), (x.shape[0], W.shape[1]))
+    for k in range(W.shape[0]):
+        acc = fmaf32(x[:, k:k + 1], W[k][None, :], acc)
+    return acc
+
+
+def gru_blend(u, h, t):
+    """h' = fmaf(u, h, (1 - u) * t) with t = tanhf(c): 1 - u and the product each rounded in fp32."""
+    u, h, t = (np.asarray(v, F32) for v in (u, h, t))
+    return fmaf32(u, h, (F32(1) - u) * t)
+
+
+def gru_gate_sums(a1, h, w):
+    """The pre-activations [r | u] of the cell, bit for bit: b_ru, then the rows of w_ru over [a1, h] in order."""
+    return fma_chain(np.concatenate([a1, h], 1), w["w_ru"], w["b_ru"])
+
+
+def chain_bound(x, dx, W, b):
+    """Two fmaf chains over the same W and b, the reference on float32 inputs x, the other on inputs within dx of them:
+    (the reference's float32 result, a bound on the distance of the two).  Per row k the bound grows by |W[k]| dx[k] and,
+    once the two chains differ, by half an ulp of each chain's partial sum.  Identical inputs into identical partial
+    sums give identical results, so the bound stays 0 until the first row with dx > 0."""
+    x, W = np.asarray(x, F32), np.asarray(W, F32)
+    dx = np.asarray(dx, np.float64)
+    aW = np.abs(W.astype(np.float64))
+    acc = np.broadcast_to(np.asarray(b, F32), (x.shape[0], W.shape[1]))
+    e = np.zeros(acc.shape)
+    for k in range(W.shape[0]):
+        acc = fmaf32(x[:, k:k + 1], W[k][None, :], acc)
+        grow = e + dx[:, k:k + 1] * aW[k][None, :]
+        a = np.abs(acc.astype(np.float64))
+        e = np.where(grow > 0, grow + 0.5 * ulp32(a + ulp32(a) + grow) + 0.5 * ulp32(a), 0.0)
+    return acc, e
+
+
+def gru_step_bound(w, a1, h):
+    """One step of gru_policy_kernel from its dense activations a1 and state h (float32, begin rows already zero), against
+    the GRU cell applied to the kernel's own gate sums: (h' reference, bound, head sums s, bound on s).
+
+    The gate sums are the kernel's bit for bit (gru_gate_sums).  From there: r and u within sigmoid_bound of sigmoid;
+    r h rounded once, so |rh - F32(sigmoid(r) h)| <= sb_r |h| + half an ulp of each; the candidate chain over [a1, rh]
+    within chain_bound of the reference chain over F32(sigmoid(r) h); tanhf within tanh_bound; then 1 - u (one
+    rounding), the product (one rounding) and the fmaf blend (one rounding) each add their operands' bounds times the
+    other operand and half an ulp.  h' is compared with u h + (1 - u) tanh(c) in fp64 (c: the reference chain).  The head
+    is chain_bound over F32(h'), its inputs within the bound on h' plus that rounding; the mean is then within
+    tanh_bound(s, bound on s) of tanh(s)."""
+    a1, h = np.asarray(a1, F32), np.asarray(h, F32)
+    G = h.shape[1]
+    pre = gru_gate_sums(a1, h, w).astype(np.float64)
+    r, u = sigmoid(pre[:, :G]), sigmoid(pre[:, G:])
+    sb = sigmoid_bound(pre)
+    sr, su = sb[:, :G], sb[:, G:]
+    h64 = h.astype(np.float64)
+    rh_ex = r * h64
+    rh = rh_ex.astype(F32)
+    drh = sr * np.abs(h64) + 0.5 * ulp32(np.abs(rh_ex) + sr * np.abs(h64)) + np.abs(rh.astype(np.float64) - rh_ex)
+    dx = np.concatenate([np.zeros(a1.shape), drh], 1)
+    c, ec = chain_bound(np.concatenate([a1, rh], 1), dx, w["w_c"], w["b_c"])
+    c = c.astype(np.float64)
+    t, dt = np.tanh(c), tanh_bound(c, ec)
+    om = 1.0 - u
+    dom = su + 0.5 * ulp32(om + su)
+    q = om * t
+    dq = dom * np.abs(t) + om * dt + dom * dt
+    dq = dq + 0.5 * ulp32(np.abs(q) + dq)
+    hp = u * h64 + q
+    dh = su * np.abs(h64) + dq
+    dh = dh + 0.5 * ulp32(np.abs(hp) + dh)
+    h32 = hp.astype(F32)
+    s, es = chain_bound(h32, dh + np.abs(h32.astype(np.float64) - hp), w["pW3"], w["pb3"])
+    return hp, dh, s, es
