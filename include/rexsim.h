@@ -159,7 +159,7 @@ int rexsim_state_words(const RexSimConfig* cfg, int32_t* n_float, int32_t* n_int
 int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_model_floats, RexSim** out);
 void rexsim_destroy(RexSim* sim);
 
-/* actions dev [N][A] f32; obs dev [N][O] f32; reward dev [N] f32; done dev [N] u8 */
+/* actions dev [N][A] f32; obs dev [N][O] f32 (O = rexsim_out_dim); reward dev [N] f32; done dev [N] u8 */
 int rexsim_step(RexSim* sim, const float* actions, float* obs, float* reward, uint8_t* done, void* stream);
 /* Host-buffer form of rexsim_step -- BatchEnv.step with numpy arrays (batch_env.py:63-90): h_actions HOST [N][A] f32,
  * h_out HOST block of rexsim_host_out_bytes() bytes laid out as obs [N][O] f32 | reward [N] f32 | done [N] u8 | pad to 4 |
@@ -174,7 +174,7 @@ int rexsim_step_host(RexSim* sim, const float* h_actions, void* h_out, void* str
  * Purely a scheduling hint: every env's results are bit-identical with and without it.  Call every few steps (the
  * Python mirror does it every 8 for batches of >= 8192 envs; a batch that fits one wave gains nothing). */
 int rexsim_rebalance(RexSim* sim, void* stream);
-/* idx dev [k] int32 (NULL: all envs, k ignored); obs_out dev [k][O] or NULL */
+/* idx dev [k] int32 (NULL: all envs, k ignored); obs_out dev [k][O] (O = rexsim_out_dim) or NULL */
 int rexsim_reset(RexSim* sim, const int32_t* idx, int32_t k, float* obs_out, void* stream);
 
 /* Physical state of every env, SoA on device: out_f dev [13 + 2*nm][N] =
@@ -225,6 +225,25 @@ int rexsim_episode_buffers(RexSim* sim, float** score, int32_t** length, float**
  * the rebalancing or the launch history.  clear != 0 also zeroes the accumulators (StreamingMean.clear); running episodes go
  * on.  One launch on `stream`; REXSIM_ERR_INVALID when the switch is off. */
 int rexsim_episode_summary(RexSim* sim, int32_t clear, void* stream);
+/* Frame wrappers (rex_gym/agents/tools/wrappers.py:93-181), fused into rexsim_step and rexsim_reset as
+ *   ConvertTo32Bit(FrameHistory(FrameDelta(ClipAction(RangeNormalize(LimitDuration(env))))))
+ * (RangeNormalize and ClipAction only with RexSimConfig.normalize).  Off by default; accepted only before the handle's first
+ * rexsim_reset / rexsim_step / rexsim_step_host and only once, REXSIM_ERR_INVALID otherwise.
+ *   delta = 1 (FrameDelta): a reset returns the observation itself and keeps it as `last`; a step returns obs - last (fp32
+ *     subtraction) and keeps obs.  An auto-reset step therefore returns the new episode's first observation.
+ *   count > 0 (FrameHistory, flatten=True): past_indices HOST [count], 1..16 values in 0..64 that include 0, capacity C = their
+ *     maximum (> 0).  A reset fills all C slots with the (delta) observation; step t (LimitDuration's counter, 1 after the first
+ *     step of an episode) writes slot t % C and returns the slots (t - i) mod C for each index i in order, concatenated, so the
+ *     observation row widens to count x obs_dim.  Duplicates and any order are allowed; an index equal to C reads slot t % C,
+ *     the current frame, as the reference's ring does.
+ * REXSIM_FLAG_NONFINITE keeps its meaning: the observation the step produced (before the wrappers) is non-finite. */
+int rexsim_set_frames(RexSim* sim, const int32_t* past_indices, int32_t count, int32_t delta);
+/* words per env of the observation rows rexsim_step, rexsim_step_host and rexsim_reset write: rexsim_obs_dim, times the number of
+ * past indices when FrameHistory is on */
+int rexsim_out_dim(const RexSim* sim);
+/* the frame wrappers' device buffers, part of an exact checkpoint together with the state buffers: ring dev [C][obs_dim][N] f32
+ * (FrameHistory, NULL and 0 floats when off), last dev [obs_dim][N] f32 (FrameDelta, NULL and 0 floats when off) */
+int rexsim_frame_buffers(RexSim* sim, float** ring, int64_t* ring_floats, float** last, int64_t* last_floats);
 /* kernels launched by this handle since create (the bench reports it) */
 int64_t rexsim_launch_count(const RexSim* sim);
 /* which build of the step kernel the last rexsim_step / rexsim_step_host launched (all 0 before the first step): CTA size,

@@ -77,6 +77,9 @@ SIGNATURES = {
     "rexsim_render": (C.c_int, [_ptr, _ptr, _i32, _i32, _i32, _f32, _f32, _f32, _ptr, _ptr]),
     "rexsim_episode_buffers": (C.c_int, [_ptr] + [_out(_ptr)] * 5 + [_out(_i64)]),
     "rexsim_episode_summary": (C.c_int, [_ptr, _i32, _ptr]),
+    "rexsim_set_frames": (C.c_int, [_ptr, _ptr, _i32, _i32]),
+    "rexsim_out_dim": (C.c_int, [_ptr]),
+    "rexsim_frame_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_i64), _out(_ptr), _out(_i64)]),
     "rexagent_policy_floats": (_i64, [_agent_cfg]),
     "rexagent_value_floats": (_i64, [_agent_cfg]),
     "rexagent_create": (C.c_int, [_agent_cfg, _out(_ptr)]),

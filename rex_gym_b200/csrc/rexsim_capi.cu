@@ -31,7 +31,8 @@ struct RexSim {
     int32_t* hist = nullptr;
     float* act = nullptr;              // staging for rexsim_step_host
     uint8_t* out = nullptr;            // obs | reward | done (same layout as the host block)
-    int A = 0, O = 0;
+    int A = 0;
+    bool started = false;              // a reset or step has been enqueued: the frame wrappers can no longer be switched on
     int nsnap = 1;
     int64_t launches = 0;
     int32_t launched[3] = {0, 0, 0};   // step_kernel instance of the last step launch: BLOCK, OCC, SENSOR
@@ -127,7 +128,8 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
         P.sm_count = sms;
     }
     s->nsnap = cfg->terrain == REXSIM_TERRAIN_RANDOM ? cfg->nfields : 1;
-    s->A = rexsim_action_dim(cfg->task, cfg->signal); s->O = rexsim_obs_dim(cfg->task, cfg->num_motors);
+    s->A = rexsim_action_dim(cfg->task, cfg->signal);
+    P.out_dim = out_dim(cfg->task, cfg->num_motors, 0);
     // the kernels read these through pointers to const; create fills them
     float *model = nullptr, *snap_f = nullptr, *zoff = nullptr;
     int32_t* snap_i = nullptr;
@@ -136,7 +138,7 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
         mem.zeroed(&P.err, N + 1) ||                                    // [N] per-env bits + 1 word: OR of all
         mem.zeroed(&P.cmd_out, cfg->num_motors * N) || mem.zeroed(&P.cost, N) || mem.zeroed(&s->perm, N) ||
         mem.zeroed(&s->hist, 256) || mem.zeroed(&s->rt, REXSIM_RT_FLOATS) || mem.zeroed(&s->act, N * s->A) ||
-        mem.zeroed(&s->out, host_block(N, s->O).bytes))
+        mem.zeroed(&s->out, host_block(N, P.out_dim).bytes))
         return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(model, model_tables, mt_floats * sizeof(float), cudaMemcpyHostToDevice));
     const SensorCfg sc = sensor_cfg(cfg);
@@ -200,10 +202,12 @@ int rexsim_step(RexSim* s, const float* actions, float* obs, float* reward, uint
     if (!s || !actions || !obs || !reward || !done) return fail(REXSIM_ERR_INVALID, "null argument");
     Params P = s->P;
     P.actions = actions; P.obs = obs; P.reward = reward; P.done = done;
+    s->started = true;
     return enqueue(s, launch_step(P, (cudaStream_t)stream), "step launch");
 }
 
-int64_t rexsim_host_out_bytes(const RexSim* s) { return s ? (int64_t)host_block(s->P.N, s->O).bytes : 0; }
+int64_t rexsim_host_out_bytes(const RexSim* s) { return s ? (int64_t)host_block(s->P.N, s->P.out_dim).bytes : 0; }
+int rexsim_out_dim(const RexSim* s) { return s ? s->P.out_dim : 0; }
 // true when p is page-locked host memory the device can address directly (UVA: same pointer value on both sides)
 static bool device_can_address(const void* p) {
     cudaPointerAttributes at;
@@ -214,8 +218,9 @@ int rexsim_step_host(RexSim* s, const float* h_actions, void* h_out, void* strea
     if (!s || !h_actions || !h_out) return fail(REXSIM_ERR_INVALID, "null argument");
     cudaStream_t st = (cudaStream_t)stream;
     const size_t N = s->P.N;
-    const HostBlock hb = host_block(N, s->O);
+    const HostBlock hb = host_block(N, s->P.out_dim);
     Params P = s->P;
+    s->started = true;
     // Small batches with pinned buffers: the kernel reads the actions from, and writes its results into, the host block
     // directly (zero-copy over PCIe) -- no DMA launches at all: the error bits travel as flag bytes the kernel sets in the
     // block, the device-side aggregate is cleared BEFORE the kernel.  Large batches stage through device buffers so the kernel
@@ -261,6 +266,7 @@ int rexsim_reset(RexSim* s, const int32_t* idx, int32_t k, float* obs_out, void*
     if (idx && k < 0) return fail(REXSIM_ERR_INVALID, "negative count");
     Params P = s->P;
     P.reset_idx = idx; P.reset_k = k;
+    s->started = true;
     return enqueue(s, launch_reset(P, obs_out, (cudaStream_t)stream), "reset launch", !idx || k > 0);
 }
 
@@ -337,6 +343,47 @@ int rexsim_episode_summary(RexSim* s, int32_t clear, void* stream) {
     if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
     if (!s->ep_block) return fail(REXSIM_ERR_INVALID, "episode statistics are off (RexSimConfig.episode_stats)");
     return enqueue(s, launch_episode_summary(s->P, clear != 0, s->ep_summary, (cudaStream_t)stream), "episode summary launch");
+}
+int rexsim_set_frames(RexSim* s, const int32_t* past_indices, int32_t count, int32_t delta) {
+    if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
+    if (s->started) return fail(REXSIM_ERR_INVALID, "frame wrappers must be set before the first reset or step");
+    if (s->P.fr.ring || s->P.fr.last) return fail(REXSIM_ERR_INVALID, "frame wrappers are already set");
+    if (delta != 0 && delta != 1) return fail(REXSIM_ERR_INVALID, "delta must be 0 or 1");
+    if (count < 0 || count > FRAMES_MAX_INDICES) return fail(REXSIM_ERR_INVALID, "frame history takes 0 to 16 past indices");
+    if (count > 0 && !past_indices) return fail(REXSIM_ERR_INVALID, "null past_indices");
+    int capacity = 0;
+    bool current = false;
+    for (int k = 0; k < count; k++) {
+        const int32_t i = past_indices[k];
+        if (i < 0 || i > FRAMES_MAX_CAPACITY) return fail(REXSIM_ERR_INVALID, "past indices must lie in 0..64");
+        capacity = i > capacity ? i : capacity;
+        current = current || i == 0;
+    }
+    if (count > 0 && !current) return fail(REXSIM_ERR_INVALID, "Past indices should include 0 for the current frame.");
+    if (count > 0 && capacity == 0) return fail(REXSIM_ERR_INVALID, "the largest past index must be positive (it is the ring's capacity)");
+    if (count == 0 && !delta) return REXSIM_OK;
+    Params& P = s->P;
+    const size_t N = P.N;
+    const int O = obs_dim(P.cfg.task, P.cfg.num_motors);
+    if (delta && s->mem.zeroed(&P.fr.last, (size_t)O * N)) return REXSIM_ERR_CUDA;
+    if (count > 0) {
+        int32_t* index = nullptr;
+        if (s->mem.zeroed(&P.fr.ring, (size_t)capacity * O * N) || s->mem.zeroed(&index, count)) return REXSIM_ERR_CUDA;
+        CK(cudaMemcpy(index, past_indices, count * sizeof(int32_t), cudaMemcpyHostToDevice));
+        P.fr.index = index; P.fr.capacity = capacity; P.fr.count = count;
+    }
+    P.out_dim = out_dim(P.cfg.task, P.cfg.num_motors, count);
+    s->mem.drop(s->out);                                              // the host-path staging block takes the new width
+    s->out = nullptr;
+    if (s->mem.zeroed(&s->out, host_block(N, P.out_dim).bytes)) return REXSIM_ERR_CUDA;
+    return REXSIM_OK;
+}
+int rexsim_frame_buffers(RexSim* s, float** ring, int64_t* ring_floats, float** last, int64_t* last_floats) {
+    if (!s || !ring || !ring_floats || !last || !last_floats) return fail(REXSIM_ERR_INVALID, "null argument");
+    const int64_t on = (int64_t)obs_dim(s->P.cfg.task, s->P.cfg.num_motors) * s->P.N;
+    *ring = s->P.fr.ring; *ring_floats = s->P.fr.ring ? (int64_t)s->P.fr.capacity * on : 0;
+    *last = s->P.fr.last; *last_floats = s->P.fr.last ? on : 0;
+    return REXSIM_OK;
 }
 int64_t rexsim_launch_count(const RexSim* s) { return s ? s->launches : 0; }
 int rexsim_last_step_build(const RexSim* s, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor) {

@@ -38,6 +38,11 @@ struct DeviceBuffers {
         CK(cudaMemset(p, 0, count * sizeof(**out)));
         return REXSIM_OK;
     }
+    // free one buffer of the list (a buffer that is reallocated with another size)
+    void drop(void* p) {
+        for (size_t i = 0; i < ptrs.size(); i++)
+            if (ptrs[i] == p) { cudaFree(p); ptrs.erase(ptrs.begin() + i); return; }
+    }
     void release() {
         for (void* p : ptrs) cudaFree(p);
         ptrs.clear();

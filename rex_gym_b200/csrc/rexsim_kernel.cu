@@ -1732,11 +1732,53 @@ __device__ __forceinline__ float map_pi(float a) {   // MapToMinusPiToPi rex.py:
     if (r >= PI_F) r -= TWO_PI; else if (r < -PI_F) r += TWO_PI;
     return r;
 }
+// Word w of env's observation, v, through FrameDelta and FrameHistory into its output row (row null: the wrappers' buffers only).
+// t is FrameHistory's step, LimitDuration's counter after this step; `first` marks a reset, where FrameDelta passes v through
+// and FrameHistory fills every slot with it (wrappers.py:130-134,176-180).
+template <int O>
+__device__ __forceinline__ void put_frame(const Frames& F, size_t N, int env, float* row, int w, float v, int t, bool first) {
+    if (F.last) {                                                     // FrameDelta.step: obs - last, then last = obs
+        float* last = F.last + (size_t)w * N + env;
+        const float x = v;
+        if (!first) v = x - *last;
+        *last = x;
+    }
+    if (!F.ring) { if (row) row[w] = v; return; }
+    const size_t slot = (size_t)O * N;
+    float* ring = F.ring + (size_t)w * N + env;
+    const int cur = t % F.capacity;                                   // FrameHistory.step: buffer[step % capacity] = obs
+    if (first) for (int s = 0; s < F.capacity; s++) ring[s * slot] = v;
+    else ring[cur * slot] = v;
+    if (!row) return;
+#pragma unroll 1
+    for (int k = 0; k < F.count; k++) {                               // _select_frames: buffer[(step - index) % capacity]
+        int s = cur - F.index[k];
+        if (s < 0) s += F.capacity;
+        row[k * O + w] = (first || s == cur) ? v : ring[s * slot];     // index = capacity reads the current slot
+    }
+}
+// The frame wrappers of the words one lane writes (lane 0 the base terms o, every lane its gallop angles a), out of line: where
+// they are off, the observation epilogue keeps only the branch around this call.
+template <int O>
+__device__ __noinline__ void put_frames(const Frames F, size_t N, int env, int leg, float* row, int t, bool first, float o0, float o1,
+                                        float o2, float o3, float a0, float a1, float a2) {
+    if (leg == 0) {
+        put_frame<O>(F, N, env, row, 0, o0, t, first); put_frame<O>(F, N, env, row, 1, o1, t, first);
+        put_frame<O>(F, N, env, row, 2, o2, t, first); put_frame<O>(F, N, env, row, 3, o3, t, first);
+    }
+    if (O > 4) {
+        put_frame<O>(F, N, env, row, 4 + 3 * leg, a0, t, first); put_frame<O>(F, N, env, row, 5 + 3 * leg, a1, t, first);
+        put_frame<O>(F, N, env, row, 6 + 3 * leg, a2, t, first);
+    }
+}
+
 // _get_observation (+ RangeNormalize) for the env; lane 0 writes the 4 base terms, every lane its 3 angles (gallop).
 // Sensor model on: GetBaseRollPitchYaw / GetBaseRollPitchYawRate / GetMotorAngles = delayed row + noise (rex.py:429-442,548-558,457-468)
+// `first`: the observation a reset returns (step 0); the frame wrappers restart on it.
 template <int TASK, bool SENSOR>
 __device__ __forceinline__ bool write_obs(const Params& P, int env, int leg, const Lane& L, float* obs_row,
-                                          const Sensor& S, uint32_t step) {
+                                          const Sensor& S, uint32_t step, bool first) {
+    constexpr int O = obs_dim(TASK, 12);
     float rpy[3];
     float wx = L.w.x, wy = L.w.y;
     float qa[3] = {L.q[0], L.q[1], L.q[2]};
@@ -1765,14 +1807,23 @@ __device__ __forceinline__ bool write_obs(const Params& P, int env, int leg, con
         if (P.cfg.normalize) { float hi = (j < 2) ? ub_ang : ub_rate; v = 2.f * (v + hi) / (2.f * hi) - 1.f; }
         o[j] = v;
     }
-    if (leg == 0) { obs_row[0] = o[0]; obs_row[1] = o[1]; obs_row[2] = o[2]; obs_row[3] = o[3]; }
+    float a[3] = {0.f, 0.f, 0.f};
     if (TASK == REXSIM_TASK_GALLOP) {
 #pragma unroll
         for (int j = 0; j < 3; j++) {
             float v = map_pi(qa[j]);
             finite = finite && isfinite(v);
             if (P.cfg.normalize) v = 2.f * (v + ub_ang) / (2.f * ub_ang) - 1.f;
-            obs_row[4 + 3 * leg + j] = v;
+            a[j] = v;
+        }
+    }
+    if (P.fr.ring || P.fr.last) {
+        put_frames<O>(P.fr, P.N, env, leg, obs_row, (int)step, first, o[0], o[1], o[2], o[3], a[0], a[1], a[2]);
+    } else {
+        if (leg == 0) { obs_row[0] = o[0]; obs_row[1] = o[1]; obs_row[2] = o[2]; obs_row[3] = o[3]; }
+        if (TASK == REXSIM_TASK_GALLOP) {
+#pragma unroll
+            for (int j = 0; j < 3; j++) obs_row[4 + 3 * leg + j] = a[j];
         }
     }
     return finite;
@@ -1808,7 +1859,6 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
     const RexSimConfig& c = P.cfg;
     constexpr int A = task_shape(TASK).act[SIGNAL == REXSIM_SIGNAL_IK ? 0 : 1];
     constexpr float bound = task_shape(TASK).bound[SIGNAL == REXSIM_SIGNAL_IK ? 0 : 1];
-    constexpr int O = obs_dim(TASK, 12);
     constexpr bool REPL = pgs_replicated(OCC, ARM, TERRAIN);
 
     Lane L; Task K; Arm AR;
@@ -1935,8 +1985,8 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
     // ---- non-finite guard (ConvertTo32Bit raises; here: flag + force done) ----------------------------------
     bool finite = isfinite(reward) && isfinite(L.pos.x) && isfinite(L.pos.y) && isfinite(L.pos.z) &&
                   isfinite(L.q[0]) && isfinite(L.q[1]) && isfinite(L.q[2]) && isfinite(L.qd[0]) && isfinite(L.qd[1]) && isfinite(L.qd[2]);
-    float* obs_row = P.obs + (size_t)env * O;
-    if (valid) finite = write_obs<TASK, SENSOR>(P, env, leg, L, obs_row, S, (uint32_t)K.env_step) && finite;
+    float* obs_row = P.obs + (size_t)env * P.out_dim;
+    if (valid) finite = write_obs<TASK, SENSOR>(P, env, leg, L, obs_row, S, (uint32_t)K.env_step, false) && finite;
     finite = (sum4(finite ? 0.f : 1.f) == 0.f);
     if (!finite) { L.err |= REXSIM_FLAG_NONFINITE; done = true; }
     int err = (int)or4((unsigned)L.err);
@@ -1970,7 +2020,7 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
     // ---- auto reset: done envs restart from the settled snapshot; obs = first observation of the new episode --
     if (c.auto_reset && done) {
         reset_from_snapshot<ARM>(P, env, leg, L, K, kp, kd, field, AR, valid, S);
-        if (valid) write_obs<TASK, SENSOR>(P, env, leg, L, obs_row, S, 0u);
+        if (valid) write_obs<TASK, SENSOR>(P, env, leg, L, obs_row, S, 0u, true);
     }
     store_lane(P.sf, P.si, N, env, leg, L, K, valid);
     if (ARM && valid && leg == 0) store_arm(P.sf, P.si, N, env, AR);
@@ -1994,13 +2044,13 @@ __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_o
     const bool inrange = env >= 0 && env < P.N;
     if (!inrange) { if (valid && leg == 0) atomicOr(&P.err[P.N], REXSIM_FLAG_BAD_INDEX); env = 0; }
     const bool wr = valid && inrange;
-    constexpr int O = obs_dim(TASK, 12);
     Lane L; Task K; Arm AR; float kp, kd; int field;
     Sensor S = make_sensor<ARM>(P, P.ring, P.N, env, (uint32_t)env + (uint32_t)P.cfg.env_offset);
     reset_from_snapshot<ARM>(P, env, leg, L, K, kp, kd, field, AR, wr, S);
-    if (wr && obs_out) {
-        if (P.sensor_on) write_obs<TASK, true>(P, env, leg, L, obs_out + (size_t)j * O, S, 0u);
-        else write_obs<TASK, false>(P, env, leg, L, obs_out + (size_t)j * O, S, 0u);
+    if (wr && (obs_out || P.fr.ring || P.fr.last)) {      // the frame wrappers restart even when no observation is asked for
+        float* row = obs_out ? obs_out + (size_t)j * P.out_dim : nullptr;
+        if (P.sensor_on) write_obs<TASK, true>(P, env, leg, L, row, S, 0u, true);
+        else write_obs<TASK, false>(P, env, leg, L, row, S, 0u, true);
     }
     if (wr && leg == 0) {
         P.err[env] = 0;

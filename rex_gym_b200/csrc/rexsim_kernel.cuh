@@ -60,6 +60,10 @@ __host__ __device__ constexpr TaskShape task_shape(int task) {
 }
 // observation width: base roll, pitch and their rates, then (gallop) the motor angles
 __host__ __device__ constexpr int obs_dim(int task, int num_motors) { return 4 + (task_shape(task).angles ? num_motors : 0); }
+// width of the rows the kernels write: obs_dim, repeated once per past index when FrameHistory is on (rexsim_out_dim)
+__host__ __device__ constexpr int out_dim(int task, int num_motors, int history_count) {
+    return obs_dim(task, num_motors) * (history_count > 0 ? history_count : 1);
+}
 
 // Episode statistics (RexSimConfig.episode_stats; every pointer is null when it is off): simulate()'s per-env score and length
 // (rex_gym/agents/tools/simulate.py:57-105) and what its StreamingMeans were handed by the episodes that ended, per env (not per
@@ -76,9 +80,23 @@ struct EpisodeStats {
 // bytes of the per-env block behind EpisodeStats: sum_score | sum_length | score | length | count | nonfinite
 __host__ __device__ constexpr size_t episode_block_bytes(size_t n) { return n * (2 * sizeof(double) + 4 * sizeof(int32_t)); }
 
+// Frame wrappers (rexsim_set_frames; both pointers null when off): the reference's FrameHistory(FrameDelta(observation))
+// (rex_gym/agents/tools/wrappers.py:93-181) in the step and reset kernels' epilogues.  Each lane keeps the words of the
+// observation it writes itself (lane 0 the four base terms, every lane its three gallop angles), so no lane reads another's.
+enum { FRAMES_MAX_INDICES = 16, FRAMES_MAX_CAPACITY = 64 };
+struct Frames {
+    float* ring;                       // [capacity][O][N] FrameHistory's buffer, O = obs_dim; null: no history
+    float* last;                       // [O][N] FrameDelta's last observation; null: no delta
+    const int32_t* index;              // [count] the past indices in the caller's order (duplicates allowed; capacity reads the current slot)
+    int32_t capacity;                  // max(past_indices)
+    int32_t count;                     // number of past indices
+};
+
 struct Params {
     RexSimConfig cfg;
     EpisodeStats ep;
+    Frames fr;
+    int32_t out_dim;                   // words per env of the observation rows the step and reset kernels write (rexsim_out_dim)
     const float* __restrict__ model;   // REXSIM_MT_FLOATS floats, 16-byte aligned
     float* __restrict__ sf;            // [NF][N]
     int32_t* __restrict__ si;          // [NI][N]

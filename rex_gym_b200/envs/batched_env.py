@@ -58,6 +58,39 @@ def summarize_episodes(totals):
                 mean_length=length / count if count else None)
 
 
+MAX_FRAME_INDICES, MAX_FRAME_INDEX = 16, 64      # FRAMES_MAX_INDICES / FRAMES_MAX_CAPACITY of the step kernel
+
+
+def check_frame_history(past_indices):
+    """frame_history keyword -> list of ints (empty: off), refused as FrameHistory.__init__ refuses it (wrappers.py:108-109:
+    KeyError without 0) and beyond what the kernels keep (ValueError), before any CUDA call."""
+    if past_indices is None:
+        return []
+    idx = [int(i) for i in past_indices]
+    if any(i != j for i, j in zip(idx, past_indices)):
+        raise ValueError("frame_history takes integer past indices")
+    if 0 not in idx:
+        raise KeyError('Past indices should include 0 for the current frame.')
+    if min(idx) < 0:
+        raise ValueError("frame_history: past indices must be non-negative, got %r" % (idx,))
+    if max(idx) == 0:
+        raise ValueError("frame_history: the largest past index is the ring's capacity and must be positive")
+    if len(idx) > MAX_FRAME_INDICES or max(idx) > MAX_FRAME_INDEX:
+        raise ValueError("frame_history: at most %d past indices, each at most %d" % (MAX_FRAME_INDICES, MAX_FRAME_INDEX))
+    return idx
+
+
+def frame_space(low, high, past_indices, delta):
+    """(low, high) of the observation Box through FrameDelta (wrappers.py:163-168: low - high, high - low) and FrameHistory
+    (:116-125: the box repeated once per past index, flattened), in the Box's float32."""
+    low, high = np.asarray(low, np.float32), np.asarray(high, np.float32)
+    if delta:
+        low, high = low - high, high - low
+    if past_indices:
+        low, high = np.tile(low, len(past_indices)), np.tile(high, len(past_indices))
+    return low, high
+
+
 class _Info(object):
     """Stand-in for BatchEnv's `tuple(infos)`: info[i] == {'action': motor command of env i} of THE STEP THAT RETURNED IT
     (rex_gym_env.py:414).  The command block lives on the device and is overwritten by the next step, so the host copy is taken
@@ -111,7 +144,19 @@ class BatchedRexEnv(object):
                  normalize=False, max_episode_steps=0, auto_reset=False, seed=1234,
                  motor_kp_range=None, motor_kd_range=None, num_fields=64, solver_iterations=None, env_offset=0,
                  base_y=None, base_z=None, base_roll=None, base_pitch=None, base_yaw=None, gait_clock_scale=1.0,
-                 rebalance_every=8, observation_noise_stdev=SENSOR_NOISE_STDDEV, episode_statistics=False):
+                 rebalance_every=8, observation_noise_stdev=SENSOR_NOISE_STDDEV, episode_statistics=False,
+                 frame_history=None, frame_delta=False):
+        """The reference's task-env keywords, plus the batch's own and the training wrappers fused into the kernels:
+        normalize (RangeNormalize + ClipAction), max_episode_steps (LimitDuration), auto_reset, episode_statistics, and
+
+        frame_history: None, or FrameHistory's past_indices (wrappers.py:93-151, flatten=True): a list of 1 to 16 indices in
+          0..64 that includes 0.  Each observation row becomes the frames t - i for each index i in list order, concatenated
+          ([N, len(frame_history) * O]; `.view(N, K, O)` gives the stacked form).  The ring holds max(frame_history) frames and
+          is filled with the first observation at every reset.  As in the reference, an index equal to that maximum reads the
+          current slot, so [0, 1, 2] returns frames t, t - 1 and t.  Duplicates and any order are allowed.
+        frame_delta: FrameDelta (wrappers.py:154-180) inside the history: a step returns obs - last obs in fp32, a reset (and
+          so an auto-reset step) the observation itself.
+        Both are off by default; with both off nothing is allocated."""
         if urdf_version is not None and urdf_version != DEFAULT_URDF_VERSION:
             raise ValueError("%s is not a supported urdf_version." % urdf_version)     # rex_gym_env.py:317-318
         if task not in TASKS or signal_type not in SIGNALS:
@@ -125,6 +170,7 @@ class BatchedRexEnv(object):
             raise ValueError("control_latency / pd_latency must be >= 0 and observation_noise_stdev five values >= 0")
         if env_randomizer:
             raise ValueError("env_randomizer hooks are Python callbacks; use motor_kp_range / motor_kd_range")
+        frames = check_frame_history(frame_history)
         if not torch.cuda.is_available():
             raise RuntimeError("rex_gym_b200 needs a CUDA device: there is no CPU fallback")
         self._L = _capi.load()
@@ -188,7 +234,12 @@ class BatchedRexEnv(object):
         self._call = functools.partial(_capi.call, self._dev_index)
         rt = np.ascontiguousarray(pack_render_tables(mark))
         self._call(self._L.rexsim_set_render_tables, self._h, rt.ctypes.data, rt.size, stream=False)
-        self.obs_dim = self._L.rexsim_obs_dim(c.task, c.num_motors)
+        env_obs_dim = self._L.rexsim_obs_dim(c.task, c.num_motors)
+        if frames or frame_delta:
+            fi = np.ascontiguousarray(frames or [0], np.int32)
+            self._call(self._L.rexsim_set_frames, self._h, fi.ctypes.data, len(frames), int(bool(frame_delta)), stream=False)
+        self.frame_history, self.frame_delta = (list(frames) if frames else None), bool(frame_delta)
+        self.obs_dim = self._L.rexsim_out_dim(self._h)           # env_obs_dim x len(frame_history)
         self.action_dim = self._L.rexsim_action_dim(c.task, c.signal)
         N, O, A = self.num_envs, self.obs_dim, self.action_dim
         dev = self.device
@@ -218,6 +269,9 @@ class BatchedRexEnv(object):
         nr = C.c_int64()
         _capi.check(self._L.rexsim_history_buffer(self._h, C.byref(p), C.byref(nr)))           # sensor history ring (None: model off)
         self._ring = view(p, (nr.value,), "<f4") if nr.value else None
+        nl = C.c_int64()
+        _capi.check(self._L.rexsim_frame_buffers(self._h, C.byref(p), C.byref(nr), C.byref(q), C.byref(nl)))
+        self._frames = {k: view(ptr, (n.value,), "<f4") for k, ptr, n in (("frame_history", p, nr), ("frame_delta", q, nl)) if n.value}
         self._episode = None
         if episode_statistics:
             o, sm, blk, nb = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int64()
@@ -227,15 +281,18 @@ class BatchedRexEnv(object):
                                  objectives=view(o, (4, N), "<f4") if o.value else None)
         # spaces: raw task spaces, or the wrapper-visible ones when the training wrappers are fused in
         b = ACTION_BOUND[(task, signal_type)]
+        Oe = env_obs_dim
         if normalize:
             self.action_space = Box(-np.inf * np.ones(A, np.float32), np.inf * np.ones(A, np.float32))   # ClipAction wrappers.py:257-260
-            self.observation_space = Box(-np.ones(O, np.float32), np.ones(O, np.float32))                # RangeNormalize :204-209
+            lo, hi = -np.ones(Oe, np.float32), np.ones(Oe, np.float32)                                  # RangeNormalize :204-209
         else:
-            hi = np.full(A, b, np.float32)
-            self.action_space = Box(hi, -hi) if task == "gallop" else Box(-hi, hi)                       # gallop_env.py:128-130
-            ub = np.full(O, 2 * math.pi, np.float32)
+            ha = np.full(A, b, np.float32)
+            self.action_space = Box(ha, -ha) if task == "gallop" else Box(-ha, ha)                       # gallop_env.py:128-130
+            ub = np.full(Oe, 2 * math.pi, np.float32)
             ub[2:4] = 2 * math.pi / self._time_step
-            self.observation_space = Box(-(ub + OBSERVATION_EPS), ub + OBSERVATION_EPS)
+            lo, hi = -(ub + OBSERVATION_EPS), ub + OBSERVATION_EPS
+        self.observation_space = Box(*frame_space(lo, hi, frames, frame_delta))
+        assert self.observation_space.shape == (O,)
         # every `rebalance_every` steps the envs are re-grouped over the warps by solver cost (rexsim_rebalance): a scheduling
         # hint only -- results are bit-identical with 0 (off).  It pays off once the batch is several waves deep (+17-19 % at
         # 16 384 / 65 536 envs); a batch that fits one wave (4096 envs = 128 CTAs on 132 SMs) is bound by its slowest env anyway
@@ -374,6 +431,8 @@ class BatchedRexEnv(object):
             sd["sensor_history"] = self._ring.clone()
         if self._episode is not None:
             sd["episode_statistics"] = self._episode["block"].clone()
+        for k, v in self._frames.items():
+            sd[k] = v.clone()
         return sd
 
     def load_state_dict(self, sd):
@@ -383,6 +442,8 @@ class BatchedRexEnv(object):
             self._ring.copy_(sd["sensor_history"])
         if self._episode is not None:
             self._episode["block"].copy_(sd["episode_statistics"])
+        for k, v in self._frames.items():
+            v.copy_(sd[k])
 
     # ---- episode statistics (episode_statistics=True) ------------------------------------------------
     def _episode_buffer(self, name):
