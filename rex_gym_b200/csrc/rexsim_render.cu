@@ -227,7 +227,10 @@ __device__ __forceinline__ void hit_ground(const RenderArgs& A, const float* h, 
     int ix = min(max((int)floorf(fmaf(ta, dgx, gx0)), 0), 254), iy = min(max((int)floorf(fmaf(ta, dgy, gy0)), 0), 254);
     const int sx = dgx > 0.f ? 1 : -1, sy = dgy > 0.f ? 1 : -1;
     const float ez = o.z + zoff;          // heights are compared uncentred
-    float t = ta;
+    // g = ray height - ground height along the ray is evaluated once at every boundary the ray crosses (cell edges, cell
+    // diagonals) and carried into the next piece, so the march is watertight: a crossing of the ground cannot fall between
+    // two pieces through rounding.  The hit is the crossing piece's triangle plane, its ray parameter clamped into the piece.
+    float t = ta, g = NAN;
     for (;;) {
         const float tx = dgx != 0.f ? ((float)(ix + (sx > 0)) - gx0) / dgx : INFINITY;
         const float ty = dgy != 0.f ? ((float)(iy + (sy > 0)) - gy0) / dgy : INFINITY;
@@ -235,24 +238,24 @@ __device__ __forceinline__ void hit_ground(const RenderArgs& A, const float* h, 
         const float* c = h + iy * 256 + ix;
         const float h00 = __ldg(c), h10 = __ldg(c + 1), h01 = __ldg(c + 256), h11 = __ldg(c + 257);
         const float u0 = gx0 - (float)ix, v0 = gy0 - (float)iy;
-        float th = INFINITY, hx = 0.f, hy = 0.f;
-#pragma unroll
-        for (int tri = 0; tri < 2; tri++) {
+        const float dd = dgy - dgx, td = dd != 0.f ? (u0 - v0) / dd : INFINITY;      // v = u on the ray
+        const bool split = td > t && td < tn;
+        float ts = t;
+        for (int piece = 0; piece <= (int)split; piece++) {
+            const float te = split && piece == 0 ? td : tn, tm = 0.5f * (ts + te);
             // tri 0: v >= u, z = h00 + (h11 - h01) u + (h01 - h00) v;  tri 1: v < u, z = h00 + (h10 - h00) u + (h11 - h10) v
-            const float a = tri == 0 ? h11 - h01 : h10 - h00, b = tri == 0 ? h01 - h00 : h11 - h10;
-            const float f0 = ez - h00 - a * u0 - b * v0, f1 = r.z - a * dgx - b * dgy;
-            if (f1 == 0.f) continue;
-            const float tt = -f0 / f1;
-            if (tt < t || tt > tn || tt >= th) continue;
-            const float u = fmaf(tt, dgx, u0), v = fmaf(tt, dgy, v0);
-            if ((v >= u) != (tri == 0)) continue;
-            th = tt; hx = a; hy = b;
-        }
-        if (th < INFINITY) {
-            best = th;
-            float nx = -hx * 20.f, ny = -hy * 20.f, inv = rsqrtf(nx * nx + ny * ny + 1.f);
-            nrm = mk(nx * inv, ny * inv, inv);
-            return;
+            const bool tri0 = fmaf(tm, dgy, v0) >= fmaf(tm, dgx, u0);
+            const float a = tri0 ? h11 - h01 : h10 - h00, b = tri0 ? h01 - h00 : h11 - h10;
+            if (g != g) g = fmaf(ts, r.z, ez) - (h00 + a * fmaf(ts, dgx, u0) + b * fmaf(ts, dgy, v0));
+            const float ge = fmaf(te, r.z, ez) - (h00 + a * fmaf(te, dgx, u0) + b * fmaf(te, dgy, v0));
+            if (g == 0.f || (g > 0.f) != (ge > 0.f)) {
+                const float f0 = ez - h00 - a * u0 - b * v0, f1 = r.z - a * dgx - b * dgy;
+                best = fminf(fmaxf(f1 != 0.f ? -f0 / f1 : ts, ts), te);
+                float nx = -a * 20.f, ny = -b * 20.f, inv = rsqrtf(nx * nx + ny * ny + 1.f);
+                nrm = mk(nx * inv, ny * inv, inv);
+                return;
+            }
+            g = ge; ts = te;
         }
         if (tn >= tb) return;
         t = tn;

@@ -82,11 +82,14 @@ def camera(target, distance=1.0, yaw=0.0, pitch=-30.0):
     return eye, f, s, u, up
 
 
-def rays(f, s, u, width, height, fov_deg=MT.CAMERA_FOV_DEG):
-    """[H][W][3] pixel rays, f component 1 (the ray parameter of a hit is its view depth)."""
+def rays(f, s, u, width, height, fov_deg=MT.CAMERA_FOV_DEG, dx=0.0, dy=0.0, rows=None, cols=None):
+    """[H][W][3] pixel rays, f component 1 (the ray parameter of a hit is its view depth).  dx, dy: every ray moved by that many
+    pixels (x to the right, y down); rows, cols: ranges of the image's pixels to cast (default all)."""
     th = np.tan(np.radians(fov_deg) / 2)
-    x = (2 * np.arange(width) + 1) / width - 1
-    y = 1 - (2 * np.arange(height) + 1) / height
+    cols = np.arange(width) if cols is None else np.asarray(cols)
+    rows = np.arange(height) if rows is None else np.asarray(rows)
+    x = (2 * (cols + dx) + 1) / width - 1
+    y = 1 - (2 * (rows + dy) + 1) / height
     return f + (x[None, :, None] * th * width / height) * s + (y[:, None, None] * th) * u
 
 
@@ -178,8 +181,9 @@ def _hit_cyl(eye, r, c, a, rad, half):
 GROUND_ID = 1 << 50
 
 
-def _ground(eye, r, best, terrain, heights, zoff, zlo, zhi):
-    """Nearest ground hit below best: t, normal, heightfield triangle id (-1 plane / outside the field)."""
+def _ground(eye, r, best, terrain, heights, zoff, zlo, zhi, normal_scale=20.0):
+    """Nearest ground hit below best: t, normal, heightfield triangle id (-1 plane / outside the field).  normal_scale: cells
+    per metre in the triangle's normal (-dh/du * 20, -dh/dv * 20, 1)."""
     P = len(r)
     t_hit = np.full(P, np.inf)
     nrm = np.tile([0.0, 0.0, 1.0], (P, 1))
@@ -236,7 +240,7 @@ def _ground(eye, r, best, terrain, heights, zoff, zlo, zhi):
         if hit.any():
             i = act[hit]
             t_hit[i] = th[hit]
-            nn = np.stack([-hx[hit] * 20, -hy[hit] * 20, np.ones(hit.sum())], 1)
+            nn = np.stack([-hx[hit] * normal_scale, -hy[hit] * normal_scale, np.ones(hit.sum())], 1)
             nrm[i] = nn / np.linalg.norm(nn, axis=1, keepdims=True)
             tri_id[i] = (iy[hit] * 255 + ix[hit]) * 2 + tri[hit]
         go = ~hit & (tn < tb[act])
@@ -252,9 +256,29 @@ def render(mark, pos, quat, q, width=480, height=360, distance=1.0, yaw=0.0, pit
            draw_robot=True):
     """(rgb uint8 [H][W][3], surface-patch id int64 [H][W]) of one robot.  heights: the env's [256][256] field (terrain 'random').
     draw_robot=False: the same camera over the ground alone."""
+    val, ids = render_values(mark, pos, quat, q, width, height, distance, yaw, pitch, terrain, heights, draw_robot)
+    return np.clip(np.floor(val), 0, 255).astype(np.uint8), ids
+
+
+def render_values(mark, pos, quat, q, width=480, height=360, distance=1.0, yaw=0.0, pitch=-30.0, terrain="plane", heights=None,
+                  draw_robot=True, offset=(0.0, 0.0), rows=None, cols=None, normal_scale=20.0):
+    """The colour before quantisation and the patch id of the pixels rows x cols (ranges; default the whole image): fp64
+    value rgb * 255 + 0.5 [h][w][3] (the pixel's byte is its floor, clipped to 0..255) and id int64 [h][w].  offset: (dx, dy),
+    every ray moved by that many pixels (x to the right, y down), or a [K][2] list of such offsets, which adds a leading axis
+    of K to both results.  normal_scale: the heightfield normal's grid scale (20 cells per metre)."""
+    offs = np.asarray(offset, np.float64)
+    single = offs.ndim == 1
+    offs = offs.reshape(-1, 2)
     table = MT.pack_render_tables(mark).astype(np.float64)
     eye, f, s, u, _ = camera(pos, distance, yaw, pitch)
-    r = rays(f, s, u, width, height, table[MT.RT_CAM]).reshape(-1, 3)
+    r = np.stack([rays(f, s, u, width, height, table[MT.RT_CAM], dx, dy, rows, cols) for dx, dy in offs])
+    shp = r.shape[:-1]
+    val, ids = _cast(mark, pos, quat, q, eye, r.reshape(-1, 3), table, terrain, heights, draw_robot, normal_scale)
+    val, ids = val.reshape(shp + (3,)), ids.reshape(shp)
+    return (val[0], ids[0]) if single else (val, ids)
+
+
+def _cast(mark, pos, quat, q, eye, r, table, terrain, heights, draw_robot, normal_scale):
     P = len(r)
     best = np.full(P, np.inf)
     nrm = np.zeros((P, 3))
@@ -279,7 +303,7 @@ def render(mark, pos, quat, q, width=480, height=360, distance=1.0, yaw=0.0, pit
         hmin, hmax = float(heights.min()), float(heights.max())
         zoff = 0.5 * (hmin + hmax)
         zlo, zhi = hmin - zoff, hmax - zoff
-    tg, ng, tri = _ground(eye, r, best.copy(), terrain, heights, zoff, zlo, zhi)
+    tg, ng, tri = _ground(eye, r, best.copy(), terrain, heights, zoff, zlo, zhi, normal_scale)
     g = tg < best
     best[g], nrm[g] = tg[g], ng[g]
     pg = eye + best[:, None] * r
@@ -301,5 +325,74 @@ def render(mark, pos, quat, q, width=480, height=360, distance=1.0, yaw=0.0, pit
     light = table[MT.RT_LIGHT:MT.RT_LIGHT + 3]
     shade = table[MT.RT_LIGHT + 3] + table[MT.RT_LIGHT + 4] * np.maximum(0.0, nrm @ light)
     rgb = np.where(vis[:, None], base * shade[:, None], base)
-    img = np.clip(np.floor(rgb * 255 + 0.5), 0, 255).astype(np.uint8)
-    return img.reshape(height, width, 3), ids.reshape(height, width)
+    return rgb * 255 + 0.5, ids
+
+
+# ---- the per-pixel criterion the device frames are held to ------------------------------------------------------------
+# fp32 error budget of the kernel against this oracle, at the 480 x 360 reference frame (fov 60 deg: 2.9e-3 rad per pixel;
+# 3.2 mm per pixel at 1 m):
+#   ray directions: the camera basis and the pixel coordinate are a few roundings of values <= 1, ~1e-7 rad = 4e-5 px;
+#   posed geometry and the eye: forward kinematics and the camera offset round each coordinate to ~2 ulp of its size, 3e-8 m
+#     near the origin (1e-5 px at 1 m) and 1.5e-5 m at x = 100 m (5e-3 px at 1 m, 0.05 px at a 4096-row frame: that frame
+#     is only rendered near the origin); the slab / quadric / triangle solves add a few ulp of the ray parameter;
+#   the bounding-sphere test dot(d, d) rr - tc^2 > rad^2 rr cancels: its error is ~4 ulp of |d|^2 rr, which at 8 m moves the
+#     perpendicular distance of a 3 cm sphere by ~0.2 mm = 0.01 px, and it only decides where the sphere touches its box (corners);
+#   shading: the normal, the Lambert dot and the fmaf are ~1e-7 relative, 3e-5 LSB of a value <= 255.5.
+# So the kernel's pixel is the oracle's ray through some point within ~0.01 px of the pixel centre, coloured to within 1e-4
+# LSB.  EPS = 0.02 px covers that with a factor 2 (and stays 25x below a half-pixel error); DELTA = 1e-3 LSB covers the
+# shading with a factor 10 and is 500x below a dropped + 0.5.
+# MIN_ROBUST keeps the criterion from going vacuous.  Robot-only and near-ground frames are above 0.97, but ground seen from
+# afar is legitimately not: the heightfield's 5 cm triangles and the 1 m checker lines near the horizon come closer than EPS to
+# most pixel centres of a 160 x 120 frame there (0.84 is the least of the planned scenes), so the floor sits below that.
+# Frames with a side under 48 pixels are held with no floor (test_gpu_render_rounding.test_image_shapes).
+EPS = 0.02
+DELTA = 1e-3
+MIN_ROBUST = 0.8
+
+
+def jitter(eps=EPS):
+    """The centre ray and 8 rays at eps pixels around it, 45 degrees apart: [9][2] offsets (dx, dy)."""
+    a = np.arange(8) * (np.pi / 4)
+    return np.concatenate([[[0.0, 0.0]], eps * np.stack([np.cos(a), np.sin(a)], 1)])
+
+
+def check_pixels(got, val, ids, delta=DELTA):
+    """Hold device bytes got [..][3] to the oracle's 9 jittered rays: val [9][..][3] (colour before quantisation) and ids [9][..]
+    (any pixel shape: [h][w], or [n] pixels picked out of a frame).  A pixel is robust when its 9 rays see one patch and all 27 values lie in one integer cell at least delta
+    from its ends; there the byte must equal the cell.  Elsewhere the byte triple must lie in the delta-widened box
+    [floor(v - delta), floor(v + delta)] of at least one ray, all three channels of that one ray.
+    Returns (robust fraction, largest |byte - cell| on robust pixels, [n][2] failing pixels)."""
+    got = np.asarray(got).astype(np.int64)
+    assert got.shape == val.shape[1:] and ids.shape == val.shape[:-1]
+    lo = np.clip(np.floor(val - delta), 0, 255).astype(np.int64)
+    hi = np.clip(np.floor(val + delta), 0, 255).astype(np.int64)
+    robust = (ids == ids[:1]).all(0) & (lo == lo[:1]).all(0).all(-1) & (hi == lo[:1]).all(0).all(-1)
+    err = np.abs(got - lo[0]).max(-1)
+    fits = ((got[None] >= lo) & (got[None] <= hi)).all(-1).any(0)
+    bad = np.where(robust, err > 0, ~fits)
+    return float(robust.mean()), int(err[robust].max(initial=0)), np.argwhere(bad)
+
+
+def assert_pixels(got, val, ids, what="", min_robust=MIN_ROBUST, delta=DELTA):
+    frac, err, bad = check_pixels(got, val, ids, delta)
+    assert not len(bad), "%s: %d failing pixels (first %s: device %s, centre ray %s, ids %s)" % (
+        what, len(bad), bad[:3].tolist(), np.asarray(got)[tuple(bad[0])].tolist(), val[(0,) + tuple(bad[0])].tolist(),
+        sorted(set(ids[(slice(None),) + tuple(bad[0])].tolist())))
+    assert frac >= min_robust, "%s: only %.4f of the pixels are robust" % (what, frac)
+    return frac, err
+
+
+def scene(env, i, st=None):
+    """render_values' scene arguments of env i of a BatchedRexEnv: mark, fp64 pose and joint angles, terrain, the env's field."""
+    st = st or env.get_state()
+    heights = None
+    if env.terrain_type == "random":
+        field = int(env._state_i[_layout().I_FIELD, i].item())
+        heights = env._fields[field].cpu().numpy().reshape(256, 256)
+    return dict(mark=env.mark, pos=st["pos"][i].astype(np.float64), quat=st["quat"][i].astype(np.float64),
+                q=st["q"][i].astype(np.float64), terrain=env.terrain_type, heights=heights)
+
+
+def _layout():
+    from twin import LAYOUT
+    return LAYOUT
