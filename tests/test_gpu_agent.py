@@ -7,17 +7,11 @@ import numpy as np
 import pytest
 import torch
 
+from agent_twin import (fitted_filter, ff_net, filters_match, flat_weights, observations,
+                        rollout_graph_equals_the_step_by_step_loop, to_numpy)
 from oracle import agent_oracle as AO
 
 pytestmark = pytest.mark.gpu
-
-
-def _random_weights(rng, O, A, H1=200, H2=100):
-    sh = dict(pW1=(O, H1), pb1=(H1,), pW2=(H1, H2), pb2=(H2,), pW3=(H2, A), pb3=(A,), logstd=(A,),
-              vW1=(O, H1), vb1=(H1,), vW2=(H1, H2), vb2=(H2,), vW3=(H2, 1), vb3=(1,))
-    w = {k: rng.normal(0, 0.15, s).astype(np.float32) for k, s in sh.items()}
-    w["logstd"] = rng.uniform(-1.2, -0.5, A).astype(np.float32)
-    return w
 
 
 @pytest.mark.parametrize("O,A,n", [(4, 2, 4096), (16, 4, 1000), (4, 1, 77), (16, 2, 65536), (8, 3, 300), (4, 5, 129),
@@ -27,19 +21,15 @@ def test_perform_on_the_tensor_cores(O, A, n):
     registers).  Against the fp64 oracle and against the fp32 kernel on the same inputs: mean (after tanh) and value within 5e-3
     (a K = 200 dot product of O(1) terms at 2^-11 relative operand error), sampling noise identical (it does not pass through
     the GEMM)."""
-    from rex_gym_b200.agents import ForwardGaussianPolicy
     rng = np.random.default_rng(O * 100 + A + 7)
-    w = _random_weights(rng, O, A)
-    f = AO.StreamingNormalize((O,), True, True, 5)
-    f.update(rng.normal(0.3, 1.7, (5000, O)))
-    obs = (rng.normal(0.3, 3.0, (n, O))).astype(np.float32)
+    w = flat_weights(rng, O, A)
+    f = fitted_filter(rng, O)
+    obs = observations(rng, n, O)
     x = torch.from_numpy(obs).cuda()
     outs = {}
     for tcore in (False, True):
-        net = ForwardGaussianPolicy(O, A, tensor_cores=tcore)
-        net.set_weights(w)
-        net.set_filters(f.count, f.mean, f.var_sum, 0, 0.0, 0.0)
-        outs[tcore] = {k: t.cpu().numpy() for k, t in net.perform(x, training=True, seed=3, step=2, env_offset=10).items()}
+        net = ff_net(O, A, 200, 100, w, f, tensor_cores=tcore)
+        outs[tcore] = to_numpy(net.perform(x, training=True, seed=3, step=2, env_offset=10))
         outs[tcore]["det"] = net.perform(x, training=False)["action"].cpu().numpy()
         net.close()
     sub = slice(0, min(n, 1024))
@@ -57,22 +47,18 @@ def test_perform_on_the_tensor_cores(O, A, n):
 
 @pytest.mark.parametrize("O,A,n", [(4, 2, 4096), (16, 4, 1000), (4, 1, 64), (4, 8, 77), (16, 2, 65536)])
 def test_perform_matches_the_oracle(O, A, n):
-    from rex_gym_b200.agents import ForwardGaussianPolicy
     rng = np.random.default_rng(O * 100 + A)
-    net = ForwardGaussianPolicy(O, A)
-    w = _random_weights(rng, O, A)
-    net.set_weights(w)
-    f = AO.StreamingNormalize((O,), True, True, 5)
-    f.update(rng.normal(0.3, 1.7, (5000, O)))
-    net.set_filters(f.count, f.mean, f.var_sum, 0, 0.0, 0.0)
-    obs = (rng.normal(0.3, 3.0, (n, O))).astype(np.float32)
+    w = flat_weights(rng, O, A)
+    f = fitted_filter(rng, O)
+    net = ff_net(O, A, 200, 100, w, f)
+    obs = observations(rng, n, O)
     obs[0] = 100.0                                                    # clipped at +-5 after normalisation
     x = torch.from_numpy(obs).cuda()
     sub = slice(0, n) if n <= 4096 else np.r_[0:512, n - 512:n]       # the python oracle draws noise per element
     for training in (False, True):
         out = net.perform(x, training=training, seed=99, step=5, env_offset=1000)
         a, m, lp, v = AO.perform(w, f, obs[sub], training, seed=99, step=5, env_offset=1000 if isinstance(sub, slice) else 0)
-        g = {k: t.cpu().numpy() for k, t in out.items()}
+        g = to_numpy(out)
         np.testing.assert_allclose(g["mean"][sub], m, atol=2e-5)
         np.testing.assert_allclose(g["value"][sub], v, atol=5e-5)
         if isinstance(sub, slice) or not training:
@@ -103,12 +89,7 @@ def test_experience_updates_both_filters_like_the_reference():
         rew = rng.normal(0.1, 0.3, (n,)).astype(np.float32)
         net.experience(torch.from_numpy(obs).cuda(), torch.from_numpy(rew).cuda())
         fo.update(obs); fr.update(rew)
-        g = net.get_filters()
-        assert g["observ_count"] == fo.count and g["reward_count"] == fr.count
-        np.testing.assert_allclose(g["observ_mean"], fo.mean, rtol=2e-5, atol=2e-6)
-        np.testing.assert_allclose(g["observ_var_sum"], fo.var_sum, rtol=5e-5, atol=1e-5)
-        np.testing.assert_allclose(g["reward_mean"], fr.mean, rtol=2e-5, atol=2e-6)
-        np.testing.assert_allclose(g["reward_var_sum"], fr.var_sum, rtol=5e-5, atol=1e-5)
+        filters_match(net.get_filters(), fo, fr)
     r = torch.from_numpy(rng.normal(0, 50, 1000).astype(np.float32)).cuda()
     np.testing.assert_allclose(net.transform_reward(r).cpu().numpy(), fr.transform(r.cpu().numpy()), rtol=1e-5, atol=1e-6)
     # bit-reproducible: same batches -> same statistics
@@ -141,10 +122,7 @@ def test_experience_in_partial_sums_matches_one_batch():
 
     def assert_filters(g, count):
         assert g["observ_count"] == g["reward_count"] == fo.count == fr.count == count
-        np.testing.assert_allclose(g["observ_mean"], fo.mean, rtol=2e-5, atol=2e-6)
-        np.testing.assert_allclose(g["observ_var_sum"], fo.var_sum, rtol=5e-5, atol=1e-5)
-        np.testing.assert_allclose(g["reward_mean"], fr.mean, rtol=2e-5, atol=2e-6)
-        np.testing.assert_allclose(g["reward_var_sum"], fr.var_sum, rtol=5e-5, atol=1e-5)
+        filters_match(g, fo, fr)
 
     obs, rew, x, r = batch(777)                       # a non-zero mean first: the partials are centred on it
     a.experience(x, r); b.experience(x, r); fo.update(obs); fr.update(rew)
@@ -202,47 +180,6 @@ def test_scans_match_the_oracle_in_both_layouts():
 
 def test_rollout_graph_equals_the_step_by_step_loop():
     rollout_graph_equals_the_step_by_step_loop(tensor_cores=False)
-
-
-def rollout_graph_equals_the_step_by_step_loop(tensor_cores):
-    """simulate(): T control steps of perform -> env.step -> experience captured as one CUDA graph; same buffers as the
-    unrolled loop on twin environments, and consistent with stepping the env by hand with the recorded actions.  With
-    tensor_cores=True (test_gpu_agent_rounding.py) the networks run perform_tc_kernel."""
-    import rex_gym_b200 as R
-    from rex_gym_b200.agents import ForwardGaussianPolicy, Rollout
-    n, T = 512, 16
-    kw = dict(task="walk", num_envs=n, signal_type="ik", normalize=True, auto_reset=True, max_episode_steps=25, target_position=2.0, backwards=False)
-    outs = []
-    for use_graph in (False, True):
-        env = R.BatchedRexEnv(**kw)
-        net = ForwardGaussianPolicy(env.obs_dim, env.action_dim, seed=3, tensor_cores=tensor_cores)
-        ro = Rollout(env, net, T, seed=17, training=True, use_graph=use_graph)
-        a = {k: v.clone() for k, v in ro.collect().items()}
-        b = {k: v.clone() for k, v in ro.collect().items()}               # second window: continues the episodes
-        outs.append((a, b, net.get_filters(), net.launch_count + env.launch_count))
-        if use_graph:
-            hand = R.BatchedRexEnv(**kw)
-            o = torch.from_numpy(hand.reset()).cuda()
-            for t in range(T):
-                np.testing.assert_allclose(a["observ"][t].cpu().numpy(), o.cpu().numpy(), atol=1e-6)
-                o2, r2, d2, _ = hand.step(a["action"][t])
-                np.testing.assert_allclose(a["reward"][t].cpu().numpy(), r2.cpu().numpy(), atol=1e-6)
-                np.testing.assert_array_equal(a["done"][t].cpu().numpy(), d2.cpu().numpy())
-                o = o2.clone()
-            hand.close()
-        ret, adv = ro.returns_and_advantages(0.985, 0.95)
-        wr, wa = AO.gae_segments(b["reward"].cpu().numpy(), b["value"].cpu().numpy(), b["done"].cpu().numpy(), 0.985, 0.95)
-        np.testing.assert_allclose(ret.cpu().numpy(), wr, rtol=1e-4, atol=1e-4)
-        np.testing.assert_allclose(adv.cpu().numpy(), wa, rtol=1e-4, atol=2e-4)
-        env.close(); net.close()
-    (a0, b0, f0, _), (a1, b1, f1, _) = outs
-    for k in a0:
-        np.testing.assert_array_equal(a0[k].cpu().numpy(), a1[k].cpu().numpy(), err_msg=k)
-        np.testing.assert_array_equal(b0[k].cpu().numpy(), b1[k].cpu().numpy(), err_msg=k)
-    assert f0["observ_count"] == f1["observ_count"] == 2 * T * n
-    np.testing.assert_array_equal(f0["observ_var_sum"], f1["observ_var_sum"])
-    assert b0["done"].any()                                              # LimitDuration(25) fired inside the second window
-    assert np.abs((a0["action"] - a0["mean"]).cpu().numpy()).max() > 1e-3   # training: sampled actions
 
 
 def test_shipped_policy_runs_on_the_device():

@@ -2,7 +2,7 @@
 arithmetic.  test_gpu_agent.py and test_gpu_agent_shapes.py hold them to the fp64 network (5e-3 for the tensor-core form);
 this file asks what each kernel computes, exactly:
 
-* Exact networks (every row of test_gpu_agent_shapes.ROWS, both kernels on the tf32 rows, every batch size): inputs and
+* Exact networks (every row of agent_twin.FF_ROWS, both kernels on the tf32 rows, every batch size): inputs and
   weights on coarse dyadic grids, so every operand is tf32-representable and every partial sum, in any order, is exact in
   fp32 (both asserted on the arrays).  The value equals the exact value bit for bit, the mean is within tanhf's error of
   the fp64 tanh of the exact argument, the deterministic action equals the mean.  These checks are blind to accumulation
@@ -26,11 +26,12 @@ import pytest
 import torch
 
 import agent_restate as R
+from agent_twin import (FF_ROWS, ff_batch_sizes, ff_id, ff_net, ff_setup, ff_weights, fitted_filter, half_sm, observations,
+                        param_shapes, probe_envs, rollout_graph_equals_the_step_by_step_loop, tiling, to_numpy)
 from oracle import agent_oracle as AO
-from test_gpu_agent_shapes import ROWS, _half, _setup, _weights, batch_sizes, probe_envs, row_id, tiling
 
 F32 = np.float32
-TF32_ROWS = [r for r in ROWS if r[4] == "tf32"]
+TF32_ROWS = [r for r in FF_ROWS if r[4] == "tf32"]
 
 
 # ---- the networks -----------------------------------------------------------------------------------------------------
@@ -117,9 +118,7 @@ def probe_network(O, A, H1, H2, col, case):
     in column col at those ks; the value head one-hot on col, b3 = 0, so value = relu(d_col + 8) = d_col + 8.  The policy
     network is all zeros."""
     a, b = (_from_bits(v) for v in case)
-    w = {k: np.zeros(s, F32) for k, s in dict(pW1=(O, H1), pb1=(H1,), pW2=(H1, H2), pb2=(H2,), pW3=(H2, A), pb3=(A,),
-                                                 logstd=(A,), vW1=(O, H1), vb1=(H1,), vW2=(H1, H2), vb2=(H2,), vW3=(H2, 1),
-                                                 vb3=(1,)).items()}
+    w = {k: np.zeros(s, F32) for k, s in param_shapes(O, A, H1, H2).items()}
     for k in probe_ks(H1):
         w["vb1"][k] = a
         w["vW2"][k, col] = b
@@ -201,15 +200,14 @@ def test_grid_and_significant_bits():
         R.assert_exact_dot(np.full((1, 3), 2.0 ** 22), np.ones((3, 1)), np.array([2.0 ** -2]), "too wide")
 
 
-@pytest.mark.parametrize("row", ROWS[:2] + TF32_ROWS[2:4], ids=row_id)
+@pytest.mark.parametrize("row", FF_ROWS[:2] + TF32_ROWS[2:4], ids=ff_id)
 def test_restatement_matches_the_fp64_oracle(row):
-    """Both restatements against AO.forward_gaussian_policy at fp32 / tf32 distance, on _weights and a fitted filter."""
+    """Both restatements against AO.forward_gaussian_policy at fp32 / tf32 distance, on ff_weights and a fitted filter."""
     O, A, H1, H2, _ = row
     rng = np.random.default_rng(5)
-    w = _weights(rng, O, A, H1, H2)
-    f = AO.StreamingNormalize((O,), True, True, 5)
-    f.update(rng.normal(0.3, 1.7, (5000, O)))
-    obs = rng.normal(0.3, 3.0, (300, O)).astype(F32)
+    w = ff_weights(rng, O, A, H1, H2)
+    f = fitted_filter(rng, O)
+    obs = observations(rng, 300, O)
     obs[0] = 100.0
     want_mean, _, want_value = AO.forward_gaussian_policy(w, f.transform(obs))
     x = R.normalise(obs, *R.normaliser(f.count, f.mean, f.var_sum))
@@ -226,12 +224,12 @@ def test_restatement_matches_the_fp64_oracle(row):
         assert np.abs(got - want).max() < 5e-3 and 0 < bound.max() < 1e-3, (net, np.abs(got - want).max(), bound.max())
 
 
-@pytest.mark.parametrize("row", ROWS, ids=row_id)
+@pytest.mark.parametrize("row", FF_ROWS, ids=ff_id)
 def test_exact_networks_are_exact(row):
     """The exactness conditions of the exact network of every row (at the largest batch of a 132-SM H100) and of every
     rounding probe, asserted on the arrays; the tanh arguments stay O(1), so the mean check is not saturated."""
     O, A, H1, H2, prec = row
-    n = max(batch_sizes(66))
+    n = max(ff_batch_sizes(66))
     w, mean, obs = exact_network(O, A, H1, H2, n)
     z, v = exact_outputs(w, mean, obs)
     assert np.mean(np.abs(z) < 2) > 0.5 and np.all(w["pb3"] != 0) and np.all(w["vb3"] != 0)
@@ -243,29 +241,18 @@ def test_exact_networks_are_exact(row):
 
 
 # ---- GPU ----------------------------------------------------------------------------------------------------------------
-def _net(O, A, H1, H2, tensor_cores):
-    from rex_gym_b200.agents import ForwardGaussianPolicy
-    return ForwardGaussianPolicy(O, A, (H1, H2), (H1, H2), tensor_cores=tensor_cores)
-
-
-def _numpy(out):
-    return {k: t.cpu().numpy() for k, t in out.items()}
-
-
 @pytest.mark.gpu
-@pytest.mark.parametrize("row", ROWS, ids=row_id)
+@pytest.mark.parametrize("row", FF_ROWS, ids=ff_id)
 def test_exact_networks_bit_for_bit(row):
     O, A, H1, H2, prec = row
-    sizes = batch_sizes(_half())
+    sizes = ff_batch_sizes(half_sm())
     w, mean, obs = exact_network(O, A, H1, H2, max(sizes))
     z, v = exact_outputs(w, mean, obs)
     x_all = torch.from_numpy(obs).cuda()
     for tc in ((False, True) if prec == "tf32" else (False,)):
-        net = _net(O, A, H1, H2, tc)
-        net.set_weights(w)
-        net.set_filters(0, mean, np.zeros(O, F32), 0, 0.0, 0.0)
+        net = ff_net(O, A, H1, H2, w, (0, mean, np.zeros(O, F32)), tensor_cores=tc)
         for n in sizes:
-            g = _numpy(net.perform(x_all[:n], training=False))
+            g = to_numpy(net.perform(x_all[:n], training=False))
             bad = np.flatnonzero(g["value"] != v[:n].astype(F32))
             assert bad.size == 0, (tc, n, bad[:5], g["value"][bad[:5]], v[bad[:5]])
             ratio = R.within_tanhf(g["mean"], z[:n])
@@ -275,7 +262,7 @@ def test_exact_networks_bit_for_bit(row):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("row", TF32_ROWS, ids=row_id)
+@pytest.mark.parametrize("row", TF32_ROWS, ids=ff_id)
 def test_tensor_core_rounding_probe(row):
     """Every PROBE_CASES pair at the first and last K-step, read out of the first, last and padded 16-column chunks: the
     value equals the fp32-exact sum of the rna-rounded operands bit for bit, in both tiles of a 129-env batch."""
@@ -283,8 +270,7 @@ def test_tensor_core_rounding_probe(row):
     n = 129
     rng = np.random.default_rng(O + A + H1 + H2)
     x = torch.from_numpy(rng.normal(0, 2, (n, O)).astype(F32)).cuda()
-    net = _net(O, A, H1, H2, True)
-    net.set_filters(0, np.zeros(O, F32), np.zeros(O, F32), 0, 0.0, 0.0)
+    net = ff_net(O, A, H1, H2, f=(0, np.zeros(O, F32), np.zeros(O, F32)), tensor_cores=True)
     fails = []
     for col in probe_columns(H2):
         for case in PROBE_CASES:
@@ -305,14 +291,14 @@ def _restate_rows(w, f, obs):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("row", TF32_ROWS, ids=row_id)
+@pytest.mark.parametrize("row", TF32_ROWS, ids=ff_id)
 def test_tensor_core_accumulation_model(row, capsys):
-    """_weights, with the value head replaced by a one-hot readout of column c (b2[c] = 0, b3 = 0), so value =
+    """ff_weights, with the value head replaced by a one-hot readout of column c (b2[c] = 0, b3 = 0), so value =
     max(d_c, 0) exactly: d_c itself wherever it is positive.  Against D_c of the rna-rounded operands, every column:
     |d_c - D_c| <= (ceil(H1 / 8) + 1) 2^-23 S_c (agent_restate.accumulation_bound).  Prints the largest ratio."""
     O, A, H1, H2, _ = row
     n = 1024
-    w, f, obs, nets = _setup(row, n)
+    w, f, obs, nets = ff_setup(row, n)
     for nt in nets[:-1]:
         nt.close()
     net = nets[-1]
@@ -335,21 +321,21 @@ def test_tensor_core_accumulation_model(row, capsys):
         worst = max(worst, float(ratio.max(initial=0)))
     net.close()
     with capsys.disabled():
-        print("\n%s: accumulation |d - D| / ((ceil(H1/8) + 1) 2^-23 S): largest %.3f over %d accumulators" % (row_id(row), worst, seen))
+        print("\n%s: accumulation |d - D| / ((ceil(H1/8) + 1) 2^-23 S): largest %.3f over %d accumulators" % (ff_id(row), worst, seen))
     assert seen > n * H2 // 4 and worst <= 1, worst
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("row", ROWS, ids=row_id)
+@pytest.mark.parametrize("row", FF_ROWS, ids=ff_id)
 def test_perform_against_the_restatement(row, capsys):
-    """_weights and a fitted filter at every batch size, at the probe envs of test_gpu_agent_shapes and a linspace.  fp32
-    kernel (every row): value bit for bit, mean within tanhf's error of tanh(restated argument), deterministic action = mean.
-    Tensor-core kernel (the tf32 rows): mean and value within the bound agent_restate.head_tf32 propagates from the
-    accumulation model; prints the largest error / bound ratio."""
+    """ff_weights and a fitted filter at every batch size, at agent_twin.probe_envs and a linspace.  fp32 kernel (every
+    row): value bit for bit, mean within tanhf's error of tanh(restated argument), deterministic action = mean.  Tensor-core
+    kernel (the tf32 rows): mean and value within the bound agent_restate.head_tf32 propagates from the accumulation model;
+    prints the largest error / bound ratio."""
     O, A, H1, H2, prec = row
-    half = _half()
-    sizes = batch_sizes(half)
-    w, f, obs, nets = _setup(row, max(sizes))
+    half = half_sm()
+    sizes = ff_batch_sizes(half)
+    w, f, obs, nets = ff_setup(row, max(sizes))
     idx = {}
     for n in sizes:
         for p in set(["fp32", prec]):
@@ -363,7 +349,7 @@ def test_perform_against_the_restatement(row, capsys):
     worst = [0.0, 0.0]
     for n in sizes:
         k = np.array([where[e] for e in idx[n, "fp32"]])
-        g = _numpy(nets[0].perform(x_all[:n], training=False))
+        g = to_numpy(nets[0].perform(x_all[:n], training=False))
         e = idx[n, "fp32"]
         bad = np.flatnonzero(g["value"][e] != zv[k])
         assert bad.size == 0, (n, e[bad[:5]], g["value"][e[bad[:5]]], zv[k[bad[:5]]])
@@ -381,7 +367,7 @@ def test_perform_against_the_restatement(row, capsys):
         for n in sizes:
             k = np.array([where[e] for e in idx[n, "tf32"]])
             e = idx[n, "tf32"]
-            g = _numpy(nets[1].perform(x_all[:n], training=False))
+            g = to_numpy(nets[1].perform(x_all[:n], training=False))
             rm = np.abs(g["mean"][e] - np.tanh(zt[k])) / mb[k]
             rv = np.abs(g["value"][e] - vt[k, 0]) / bv[k, 0]
             worst = [max(worst[0], float(rm.max())), max(worst[1], float(rv.max()))]
@@ -389,7 +375,7 @@ def test_perform_against_the_restatement(row, capsys):
             assert np.array_equal(g["action"], g["mean"]), n
         with capsys.disabled():
             print("\n%s: tensor cores, largest error / bound: mean %.3f, value %.3f (bounds up to %.2e / %.2e)" % (
-                row_id(row), worst[0], worst[1], float(mb.max()), float(bv.max())))
+                ff_id(row), worst[0], worst[1], float(mb.max()), float(bv.max())))
     for nt in nets:
         nt.close()
 
@@ -418,5 +404,4 @@ def test_transform_reward_bit_for_bit(count):
 @pytest.mark.gpu
 def test_tensor_core_rollout_graph_equals_the_step_by_step_loop():
     """test_gpu_agent.py's graph-vs-loop rollout check with the networks' layer 2 on the tensor cores."""
-    from test_gpu_agent import rollout_graph_equals_the_step_by_step_loop
     rollout_graph_equals_the_step_by_step_loop(tensor_cores=True)

@@ -4,19 +4,20 @@
 `rexagent_perform` has two forms.  The fp32 kernel runs `perform_kernel<TM>` on 64-env tiles while ceil(n / 128) is below half
 the SM count and on 128-env tiles above it, on a grid of min(tiles, SMs / 2) persistent CTAs per network; its block has
 16 * H2 / 4 threads, rounded up to TM.  The tf32 kernel (`perform_tc_kernel<O, A>`, eight instances) always uses 128-env tiles.
-ROWS lists one network configuration per code path (shapes, widths, block sizes, tensor-core instances); every row runs at the
-batch sizes around each tiling switch of the device it runs on.  The filter update, the reward transform and the scans are
+agent_twin.FF_ROWS lists one network configuration per code path (shapes, widths, block sizes, tensor-core instances); every
+row runs at the batch sizes around each tiling switch of the device it runs on.  The filter update, the reward transform and the scans are
 checked at the lengths where their loops change shape, and the filter counts across 2^31 and 2^32.
 
 The CPU tests check the table itself against the acceptance rule of `rexagent_create`, which validates a configuration before
 its first CUDA call."""
 import ctypes as C
-import math
 
 import numpy as np
 import pytest
 import torch
 
+from agent_twin import (FF_ROWS, OFFSET, SCAN_LENGTHS, SEED, STEP, experience_split, ff_batch_sizes, ff_id, ff_setup,
+                        filters_match, half_sm, noise, param_shapes, probe_envs, sampled, tiling, to_numpy)
 from oracle import agent_oracle as AO
 
 # ---- the acceptance rule of rexagent_create / rexagent_set_precision (rexsim_agent.cu) --------------------------------
@@ -75,33 +76,6 @@ def tc_instance(O, A):
     return (0, 0)
 
 
-# (O, A, H1, H2, precision).  The block of the fp32 kernel has 16 * H2 / 4 threads, rounded up to the tile's TM.
-ROWS = [
-    (4, 2, 200, 100, "fp32"),      # walk / turn / standup / poses policies
-    (16, 4, 200, 100, "fp32"),     # gallop policies
-    (1, 1, 64, 12, "fp32"),        # 48 threads: rounded up to TM on both tile sizes
-    (32, 8, 64, 4, "fp32"),        # widest input and head, 16 threads, A * H2 / 4 = 8
-    (32, 3, 200, 100, "fp32"),     # O = 32 with the shipped hidden sizes: 227 072 of 232 448 bytes of shared memory
-    (4, 2, 256, 64, "fp32"),       # the largest hidden1
-    (4, 1, 200, 128, "fp32"),      # 512 threads, the launch bound
-    (4, 2, 64, 100, "fp32"),
-    (32, 1, 8, 12, "fp32"),        # hidden1 = 8
-    (4, 2, 100, 36, "fp32"),       # hidden1 = 4 mod 8, 144 threads
-    (4, 2, 200, 100, "tf32"),      # perform_tc_kernel<4, 2>
-    (4, 1, 200, 128, "tf32"),      # <4, 1>; H2 = 128: all eight 16-column chunks
-    (4, 8, 8, 4, "tf32"),          # <4, 8>; hidden1 = 8: a single K-step; H2 = 4 padded to 16
-    (4, 5, 64, 12, "tf32"),        # <4, 0>
-    (16, 2, 200, 100, "tf32"),     # <16, 2>
-    (16, 4, 200, 100, "tf32"),     # <16, 4>
-    (16, 3, 128, 100, "tf32"),     # <16, 0>
-    (1, 3, 64, 12, "tf32"),        # <0, 0>
-]
-
-
-def row_id(r):
-    return "O%d-A%d-%dx%d-%s" % r
-
-
 def _lib():
     from rex_gym_b200 import _capi
     return _capi, _capi.load()
@@ -128,16 +102,16 @@ def _assert_create_follows_the_rule(O, A, H1, H2):
 
 # ---- CPU: the table against the rule ----------------------------------------------------------------------------------
 def test_every_table_row_is_accepted_and_the_table_covers_every_path():
-    for O, A, H1, H2, prec in ROWS:
+    for O, A, H1, H2, prec in FF_ROWS:
         assert create_code(O, A, H1, H2) == OK, (O, A, H1, H2)
         _assert_create_follows_the_rule(O, A, H1, H2)
         if prec == "tf32":
             assert tf32_accepted(O, A, H1, H2), (O, A, H1, H2)
-    fp32 = [r for r in ROWS if r[4] == "fp32"]
-    tf32 = [r for r in ROWS if r[4] == "tf32"]
-    assert {r[:2] for r in ROWS} >= {(4, 2), (16, 4)}
-    assert {r[0] for r in fp32} >= {1, 32} and {r[1] for r in ROWS} >= {1, 8}
-    assert {r[3] for r in ROWS} >= {4, 12, 100, 128} and {r[2] for r in ROWS} >= {8, 64, 200, 256}
+    fp32 = [r for r in FF_ROWS if r[4] == "fp32"]
+    tf32 = [r for r in FF_ROWS if r[4] == "tf32"]
+    assert {r[:2] for r in FF_ROWS} >= {(4, 2), (16, 4)}
+    assert {r[0] for r in fp32} >= {1, 32} and {r[1] for r in FF_ROWS} >= {1, 8}
+    assert {r[3] for r in FF_ROWS} >= {4, 12, 100, 128} and {r[2] for r in FF_ROWS} >= {8, 64, 200, 256}
     assert any(16 * r[3] // 4 == 512 for r in fp32)                                 # the launch bound
     assert any(16 * r[3] // 4 < 64 for r in fp32)                                   # block rounded up on 64-env tiles
     assert any(r[2] == MAX_H1 for r in fp32)                                        # the largest hidden1
@@ -167,10 +141,9 @@ def test_create_refuses_exactly_past_each_limit():
 
 def test_parameter_block_sizes_match_the_oracle_packing():
     _capi, L = _lib()
-    for O, A, H1, H2, _ in ROWS + [(33, 9, 300, 132, "")]:
+    for O, A, H1, H2, _ in FF_ROWS + [(33, 9, 300, 132, "")]:
         cfg = _capi.RexAgentConfig(O, A, H1, H2, 5.0, 10.0)
-        shapes = dict(pW1=(O, H1), pb1=(H1,), pW2=(H1, H2), pb2=(H2,), pW3=(H2, A), pb3=(A,), logstd=(A,),
-                      vW1=(O, H1), vb1=(H1,), vW2=(H1, H2), vb2=(H2,), vW3=(H2, 1), vb3=(1,))
+        shapes = param_shapes(O, A, H1, H2)
         block = AO.pack_params({k: np.zeros(s, np.float32) for k, s in shapes.items()}, O, A, H1, H2)
         npol, nval = L.rexagent_policy_floats(C.byref(cfg)), L.rexagent_value_floats(C.byref(cfg))
         assert (npol, nval) == (policy_floats(O, A, H1, H2), value_floats(O, A, H1, H2))
@@ -182,75 +155,8 @@ def test_parameter_block_sizes_match_the_oracle_packing():
 
 
 # ---- GPU --------------------------------------------------------------------------------------------------------------
-def _half():
-    return max(torch.cuda.get_device_properties(0).multi_processor_count // 2, 1)
-
-
-def batch_sizes(half):
-    """The sizes around every tiling switch of the fp32 kernel on a device with 2 * half SMs."""
-    return [1, 63, 64, 65, 129, 64 * half, 64 * half + 1,       # 64 * half + 1: a second 64-env tile on CTA 0
-            128 * (half - 1), 128 * (half - 1) + 1,              # the last size on 64-env tiles, the first on 128-env tiles
-            128 * half + 1, 65536 + 37]
-
-
-def tiling(n, half, prec):
-    if prec == "tf32":
-        tm = 128
-    else:
-        tm = 128 if (n + 127) // 128 >= half else 64
-    ntiles = (n + tm - 1) // tm
-    return tm, ntiles, min(ntiles, half)
-
-
-def probe_envs(n, tm, ntiles, grid):
-    """First and last env of every CTA's second and last tile, and the last env of the batch."""
-    s = {0, n - 1}
-    for b in range(grid):
-        tiles = list(range(b, ntiles, grid))
-        for t in set(tiles[1:2] + tiles[-1:]):
-            s.update((t * tm, min((t + 1) * tm, n) - 1))
-    return np.array(sorted(s))
-
-
-def _weights(rng, O, A, H1, H2):
-    """Per-layer scale 1 / sqrt(fan_in) (sqrt(2 / fan_in) after a ReLU) keeps every pre-activation O(1) at every width."""
-    def dense(i, o, gain):
-        return (rng.standard_normal((i, o)) * gain / math.sqrt(i)).astype(np.float32)
-
-    def bias(k):
-        return rng.normal(0, 0.1, k).astype(np.float32)
-    return dict(pW1=dense(O, H1, 0.7), pb1=bias(H1), pW2=dense(H1, H2, math.sqrt(2)), pb2=bias(H2), pW3=dense(H2, A, 1.0),
-                pb3=bias(A), logstd=rng.uniform(-1.2, -0.5, A).astype(np.float32),
-                vW1=dense(O, H1, 0.7), vb1=bias(H1), vW2=dense(H1, H2, math.sqrt(2)), vb2=bias(H2), vW3=dense(H2, 1, 1.0), vb3=bias(1))
-
-
-def _noise(seed, step, genv, A):
-    return np.array([[AO.normal_noise(seed, int(g), step, a) for a in range(A)] for g in genv])
-
-
-def _setup(row, n_max):
-    from rex_gym_b200.agents import ForwardGaussianPolicy
-    O, A, H1, H2, prec = row
-    rng = np.random.default_rng(1000 * O + 100 * A + H1 + H2 + (7 if prec == "tf32" else 0))
-    w = _weights(rng, O, A, H1, H2)
-    f = AO.StreamingNormalize((O,), True, True, 5)
-    f.update(rng.normal(0.3, 1.7, (5000, O)))
-    obs = rng.normal(0.3, 3.0, (n_max, O)).astype(np.float32)
-    obs[0], obs[n_max // 3] = 100.0, -100.0                             # clipped at +-5 after normalisation
-    nets = []
-    for tc in ((False, True) if prec == "tf32" else (False,)):
-        net = ForwardGaussianPolicy(O, A, (H1, H2), (H1, H2), seed=1, tensor_cores=tc)
-        net.set_weights(w)
-        net.set_filters(f.count, f.mean, f.var_sum, 0, 0.0, 0.0)
-        nets.append(net)
-    return w, f, obs, nets
-
-
-SEED, STEP, OFFSET = 99, 5, 1000
-
-
 @pytest.mark.gpu
-@pytest.mark.parametrize("row", ROWS, ids=row_id)
+@pytest.mark.parametrize("row", FF_ROWS, ids=ff_id)
 def test_perform_matches_the_oracle_at_every_batch_size(row):
     """fp32: mean 2e-5, value 5e-5, sampled action 5e-5, log-prob 2e-4 (the bounds of test_gpu_agent.py).  tf32: mean and
     value 5e-3 against the oracle and against the fp32 kernel (a K <= 256 dot product of O(1) terms at 2^-11 relative operand
@@ -258,28 +164,26 @@ def test_perform_matches_the_oracle_at_every_batch_size(row):
     bound plus the fp32 action bound, 5e-3 + 5e-5; log-prob 2e-4 as in fp32.  Every output alone equals the all-outputs run
     bit for bit, and observ_copy equals the input."""
     O, A, H1, H2, prec = row
-    half = _half()
-    sizes = batch_sizes(half)
-    w, f, obs, nets = _setup(row, max(sizes))
+    half = half_sm()
+    sizes = ff_batch_sizes(half)
+    w, f, obs, nets = ff_setup(row, max(sizes))
     net = nets[-1]
     want_mean, logstd, want_value = AO.forward_gaussian_policy(w, f.transform(obs))
     x_all = torch.from_numpy(obs).cuda()
     tol = dict(mean=2e-5, value=5e-5, action=5e-5) if prec == "fp32" else dict(mean=5e-3, value=5e-3, action=5e-3 + 5e-5)
     for n in sizes:
         x = x_all[:n]
-        det = {k: t.cpu().numpy() for k, t in net.perform(x, training=False).items()}
+        det = to_numpy(net.perform(x, training=False))
         cp = torch.full_like(x, float("nan"))
         out = net.perform(x, training=True, seed=SEED, step=STEP, env_offset=OFFSET, observ_copy=cp)
-        g = {k: t.cpu().numpy() for k, t in out.items()}
+        g = to_numpy(out)
         assert torch.equal(cp, x), n
         em, ev = np.abs(det["mean"] - want_mean[:n]).max(), np.abs(det["value"] - want_value[:n]).max()
         assert em < tol["mean"] and ev < tol["value"], (n, em, ev)
         assert np.array_equal(det["action"], det["mean"]) and np.array_equal(g["mean"], det["mean"]), n
         assert np.array_equal(g["value"], det["value"]), n
         idx = np.unique(np.r_[probe_envs(n, *tiling(n, half, prec)), np.linspace(0, n - 1, 16).astype(int)])
-        z = _noise(SEED, STEP, OFFSET + idx, A)
-        want_a = want_mean[idx] + np.exp(logstd)[None, :] * z
-        want_lp = (-0.5 * z * z - logstd[None, :] - 0.5 * math.log(2 * math.pi)).sum(1)
+        want_a, want_lp = sampled(want_mean[idx], logstd, noise(SEED, STEP, OFFSET + idx, A))
         ea, elp = np.abs(g["action"][idx] - want_a).max(), np.abs(g["logprob"][idx] - want_lp).max()
         assert ea < tol["action"] and elp < 2e-4, (n, ea, elp)
         for k in ("action", "mean", "logprob", "value"):                  # one output at a time
@@ -290,7 +194,7 @@ def test_perform_matches_the_oracle_at_every_batch_size(row):
         net.perform(x, training=False, out=boot)
         assert np.array_equal(boot["value"].cpu().numpy(), det["value"]), n
         if prec == "tf32":                                               # the same inputs through the fp32 kernel
-            r = {k: t.cpu().numpy() for k, t in nets[0].perform(x, training=True, seed=SEED, step=STEP, env_offset=OFFSET).items()}
+            r = to_numpy(nets[0].perform(x, training=True, seed=SEED, step=STEP, env_offset=OFFSET))
             assert np.abs(g["mean"] - r["mean"]).max() < 5e-3 and np.abs(g["value"] - r["value"]).max() < 5e-3, n
             assert np.abs((g["action"] - g["mean"]) - (r["action"] - r["mean"])).max() < 1e-5, n
     for nt in nets:
@@ -298,17 +202,17 @@ def test_perform_matches_the_oracle_at_every_batch_size(row):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("row", ROWS, ids=row_id)
+@pytest.mark.parametrize("row", FF_ROWS, ids=ff_id)
 def test_perform_does_not_depend_on_the_env_position(row, capsys):
     """Every sum of perform_kernel runs in an order fixed by the code, whatever TM and the env's place in its tile: an env's
     mean, value and noise-free action are bit-identical inside a batch of n, inside a batch of 128 * (half - 1) + 1 (128-env
     tiles) and alone in a batch of 1; so are its sampled action and log-prob when the lone run carries env_offset = env.
     The tensor-core form is held to 1e-6 and reports whether it is bit-identical too."""
     O, A, H1, H2, prec = row
-    half = _half()
+    half = half_sm()
     n_big = 128 * (half - 1) + 1
     sizes = [64 * half + 1, 128 * (half - 1), 65536 + 37]
-    _, _, obs, nets = _setup(row, max(sizes))
+    _, _, obs, nets = ff_setup(row, max(sizes))
     net = nets[-1]
     x_all = torch.from_numpy(obs).cuda()
     worst = 0.0
@@ -316,17 +220,17 @@ def test_perform_does_not_depend_on_the_env_position(row, capsys):
         tm, ntiles, grid = tiling(n, half, prec)
         envs = np.unique(np.r_[probe_envs(n, tm, ntiles, grid)[:6], probe_envs(n, tm, ntiles, grid)[-6:], n // 2, 1])
         x = x_all[:n]
-        det = {k: t.cpu().numpy() for k, t in net.perform(x, training=False).items()}
-        smp = {k: t.cpu().numpy() for k, t in net.perform(x, training=True, seed=SEED, step=STEP).items()}
+        det = to_numpy(net.perform(x, training=False))
+        smp = to_numpy(net.perform(x, training=True, seed=SEED, step=STEP))
         pos = np.linspace(0, n_big - 1, len(envs)).astype(int)            # distinct places in the 128-env-tile batch
         xb = x_all[:n_big].clone()
         xb[torch.from_numpy(pos).cuda()] = x[torch.from_numpy(envs).cuda()]
-        big = {k: t.cpu().numpy() for k, t in net.perform(xb, training=False).items()}
+        big = to_numpy(net.perform(xb, training=False))
         got = [(det, envs, big, pos, ("action", "mean", "value"))]
         for e in envs:
-            one = {k: t.cpu().numpy() for k, t in net.perform(x[e:e + 1], training=True, seed=SEED, step=STEP, env_offset=int(e)).items()}
+            one = to_numpy(net.perform(x[e:e + 1], training=True, seed=SEED, step=STEP, env_offset=int(e)))
             got.append((smp, np.array([e]), one, np.array([0]), ("action", "mean", "logprob", "value")))
-            lone = {k: t.cpu().numpy() for k, t in net.perform(x[e:e + 1], training=False).items()}
+            lone = to_numpy(net.perform(x[e:e + 1], training=False))
             got.append((det, np.array([e]), lone, np.array([0]), ("action", "mean", "value")))
         for ref, ri, other, oi, keys in got:
             for k in keys:
@@ -337,27 +241,10 @@ def test_perform_does_not_depend_on_the_env_position(row, capsys):
                 else:
                     assert d <= 1e-6, (n, k, ri[:4], d)
     with capsys.disabled():
-        print("\n%s: largest difference across batch positions %.3g (%s)" % (row_id(row), worst,
-                                                                              "bit-identical" if worst == 0 else "not bit-identical"))
+        print("\n%s: largest difference across batch positions %.3g (%s)" % (ff_id(row), worst,
+                                                                             "bit-identical" if worst == 0 else "not bit-identical"))
     for nt in nets:
         nt.close()
-
-
-def _filters_match(g, fo, fr):
-    assert g["observ_count"] == fo.count and g["reward_count"] == fr.count, (g["observ_count"], fo.count)
-    np.testing.assert_allclose(g["observ_mean"], fo.mean, rtol=2e-5, atol=2e-6)
-    np.testing.assert_allclose(g["observ_var_sum"], fo.var_sum, rtol=5e-5, atol=1e-5)
-    np.testing.assert_allclose(g["reward_mean"], fr.mean, rtol=2e-5, atol=2e-6)
-    np.testing.assert_allclose(g["reward_var_sum"], fr.var_sum, rtol=5e-5, atol=1e-5)
-
-
-def _experience_split(net, x, r):
-    """The env-sharded form on one rank: partial sums of the whole batch, then finalize."""
-    from rex_gym_b200 import _capi
-    sums = torch.zeros((net.O + 1, 2), dtype=torch.float32, device="cuda")
-    st = net._stream()
-    _capi.check(net._L.rexagent_experience_partial(net._h, x.data_ptr(), r.data_ptr(), x.shape[0], sums.data_ptr(), st))
-    _capi.check(net._L.rexagent_experience_finalize(net._h, sums.data_ptr(), x.shape[0], x.data_ptr(), r.data_ptr(), st))
 
 
 @pytest.mark.gpu
@@ -374,10 +261,10 @@ def test_experience_at_every_reduction_shape(O):
         rew = rng.normal(0.1, 0.3, n).astype(np.float32)
         x, r = torch.from_numpy(obs).cuda(), torch.from_numpy(rew).cuda()
         a.experience(x, r)
-        _experience_split(b, x, r)
+        experience_split(b, x, r)
         fo.update(obs); fr.update(rew)
         for net in (a, b):
-            _filters_match(net.get_filters(), fo, fr)
+            filters_match(net.get_filters(), fo, fr)
         if n == 1:
             np.testing.assert_array_equal(a.get_filters()["observ_mean"], obs[0])
     assert int(a._cnt[2]) == int(b._cnt[2]) == 9 and int(a._cnt[3]) == int(b._cnt[3]) == 0
@@ -426,8 +313,8 @@ def test_filter_counts_go_past_two_to_the_31(start, split):
     net.set_filters(start, m0, v0, start, float(rm0), float(rv0))
     fo.count, fo.mean, fo.var_sum = start, m0.astype(np.float64), v0.astype(np.float64)
     fr.count, fr.mean, fr.var_sum = start, np.float64(rm0), np.float64(rv0)
-    _filters_match(net.get_filters(), fo, fr)
-    def moved(new, old, rtol, atol):               # the update is at least ten times what _filters_match tolerates
+    filters_match(net.get_filters(), fo, fr)
+    def moved(new, old, rtol, atol):               # the update is at least ten times what filters_match tolerates
         return np.all(np.abs(np.asarray(new) - old) > 10 * (rtol * np.abs(new) + atol))
 
     for _ in range(3):
@@ -435,14 +322,14 @@ def test_filter_counts_go_past_two_to_the_31(start, split):
         rew = rng.normal(fr.mean + 1000.0, 0.3, n).astype(np.float32)
         x, r = torch.from_numpy(obs).cuda(), torch.from_numpy(rew).cuda()
         if split:
-            _experience_split(net, x, r)
+            experience_split(net, x, r)
         else:
             net.experience(x, r)
         before = (fo.mean, fo.var_sum, fr.mean, fr.var_sum)
         fo.update(obs); fr.update(rew)
         assert moved(fo.mean, before[0], 2e-5, 2e-6) and moved(fo.var_sum, before[1], 5e-5, 1e-5)
         assert moved(fr.mean, before[2], 2e-5, 2e-6) and moved(fr.var_sum, before[3], 5e-5, 1e-5)
-        _filters_match(net.get_filters(), fo, fr)
+        filters_match(net.get_filters(), fo, fr)
     assert fo.count == start + 3 * n and int(net._cnt[0]) == int(net._cnt[1]) == fo.count and int(net._cnt[2]) == 3
     obs = rng.normal(fo.mean, 1.5 * np.sqrt(fo.var_sum / (fo.count - 1)), (n, O)).astype(np.float32)    # around the filter
     x = torch.from_numpy(obs).cuda()
@@ -464,9 +351,6 @@ def _scan_atol(L, want, *inputs, base=1e-4):
     with discount 1 the sums reach |agg| ~ 100 and the bound is ~3e-2."""
     M = max(float(np.abs(i).max()) for i in inputs)
     return max(base, L * 2.0**-24 * (4 * float(np.abs(want).max()) + 9 * M))
-
-
-SCAN_LENGTHS = [1, 7, 8, 9, 1000]
 
 
 @pytest.mark.gpu

@@ -10,135 +10,56 @@ whose absolute values sum to about 11 with these weights; sequential fp32 accumu
 and sigmoid / tanh do not amplify it.  So the new state, the mean and the sampled action are held to 2e-4, the log-prob to
 2e-4 (as the feed-forward tests) and the value, which is the feed-forward kernel's, to 5e-5.  The cell is contractive (u < 1),
 so the state error must not grow along the sequence: at step 64 it stays within 4x its value at step 8 (or 2^-20)."""
-import math
-
 import numpy as np
 import pytest
 import torch
 
-from oracle import agent_oracle as AO
+from agent_twin import (GRU_ROWS, LIN_ROWS, OFFSET, SEED, fitted_filter, ff_value_twin, gru_batch_sizes, gru_id, gru_net,
+                        gru_weights, lin_id, lin_net, lin_weights, load, noise, observations, sampled, sm_count, tile_probes,
+                        to_numpy)
 from oracle import recurrent_oracle as RO
 
 pytestmark = pytest.mark.gpu
 
-SEED, OFFSET = 99, 1000
 TOL = dict(hidden=2e-4, mean=2e-4, action=2e-4, logprob=2e-4, value=5e-5)
 
-ROWS = [  # (O, A, H1, G, value layers)
-    (4, 2, 200, 100, (200, 100)),     # walk / turn / standup / poses with the shipped sizes
-    (16, 4, 200, 100, (200, 100)),    # gallop
-    (1, 1, 64, 12, (64, 12)),         # O = 1; 48 of the block's 128 threads compute cell columns
-    (32, 3, 64, 32, (64, 12)),        # O = 32
-    (4, 8, 64, 16, (64, 12)),         # A = 8
-    (4, 2, 36, 8, (64, 12)),          # small G, H1 = 4 mod 8: K = 44, a 12-row tail chunk
-    (4, 2, 256, 128, (64, 12)),       # the largest H1 and G: 512 threads, 24 chunks
-]
 
-
-def row_id(r):
-    return "O%d-A%d-%dx%d" % r[:4]
-
-
-def _sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def batch_sizes():
-    sm = _sm()
-    return [1, 63, 64, 65, 64 * sm, 64 * sm + 1, 128 * (sm - 1), 128 * (sm - 1) + 1]
-
-
-def _weights(rng, O, A, H1, G, vl):
-    def dense(i, o, gain):
-        return (rng.standard_normal((i, o)) * gain / math.sqrt(i)).astype(np.float32)
-
-    def bias(k, m=0.0):
-        return (m + rng.normal(0, 0.1, k)).astype(np.float32)
-    H1v, H2v = vl
-    return dict(pW1=dense(O, H1, 0.7), pb1=bias(H1), w_ru=dense(H1 + G, 2 * G, 1.0), b_ru=bias(2 * G, 1.0),
-                w_c=dense(H1 + G, G, 1.0), b_c=bias(G), pW3=dense(G, A, 1.0), pb3=bias(A),
-                logstd=rng.uniform(-1.2, -0.5, A).astype(np.float32),
-                vW1=dense(O, H1v, 0.7), vb1=bias(H1v), vW2=dense(H1v, H2v, math.sqrt(2)), vb2=bias(H2v), vW3=dense(H2v, 1, 1.0),
-                vb3=bias(1))
-
-
-def _filters(rng, O):
-    f = AO.StreamingNormalize((O,), True, True, 5)
-    f.update(rng.normal(0.3, 1.7, (5000, O)))
-    return f
-
-
-def _net(row, n, w, f):
-    from rex_gym_b200.agents import RecurrentGaussianPolicy
-    O, A, H1, G, vl = row
-    net = RecurrentGaussianPolicy(O, A, (H1, 100), vl, seed=1, num_envs=n, cell_size=G)
-    net.set_weights(w)
-    net.set_filters(f.count, f.mean, f.var_sum, 0, 0.0, 0.0)
-    return net
-
-
-def _ff(O, A, vl, w, f, policy=None):
-    from rex_gym_b200.agents import ForwardGaussianPolicy
-    ff = ForwardGaussianPolicy(O, A, vl, vl, seed=1)
-    ffw = ff.get_weights()
-    ffw.update({k: w[k] for k in ("vW1", "vb1", "vW2", "vb2", "vW3", "vb3")})
-    ffw.update(policy or {})
-    ff.set_weights(ffw)
-    ff.set_filters(f.count, f.mean, f.var_sum, 0, 0.0, 0.0)
-    return ff
-
-
-def _np(out):
-    return {k: v.cpu().numpy() for k, v in out.items()}
-
-
-def _probes(n, tm=64):
-    """First and last env of the first, second and last tiles, a spread, and the last env."""
-    s = {0, n - 1}
-    for t in {0, 1, (n - 1) // tm}:
-        s.update((min(t * tm, n - 1), min((t + 1) * tm, n) - 1))
-    s.update(np.linspace(0, n - 1, 24).astype(int).tolist())
-    return np.array(sorted(s))
-
-
-@pytest.mark.parametrize("row", ROWS, ids=row_id)
+@pytest.mark.parametrize("row", GRU_ROWS, ids=gru_id)
 def test_perform_matches_the_oracle_over_a_sequence(row):
     """64 control steps with fresh observations and random episode starts (5 % of the rows per step) at every batch size: the
     mean, sampled action, log-prob, value and new state of probe rows against the oracle; the value is bit-identical to the
     feed-forward network's with the same value weights."""
     O, A, H1, G, vl = row
     rng = np.random.default_rng(100 * O + 10 * A + H1 + G)
-    w, f = _weights(rng, O, A, H1, G, vl), _filters(rng, O)
-    sizes = batch_sizes()
+    w, f = gru_weights(rng, O, A, H1, G, vl), fitted_filter(rng, O)
+    sizes = gru_batch_sizes()
     N = max(sizes)
-    net, ff = _net(row, N, w, f), _ff(O, A, vl, w, f)
+    net, ff = gru_net(row, N, w, f), ff_value_twin(O, A, vl, w, f)
     worst = {k: 0.0 for k in TOL}
     for n in sizes:
         net.load_state_dict(dict(net.state_dict(), hidden=torch.zeros_like(net.state_dict()["hidden"])))
-        idx = _probes(n)
+        idx = tile_probes(n)
         h = np.zeros((len(idx), G))
         err_h = []
         for t in range(64):
-            obs = rng.normal(0.3, 3.0, (n, O)).astype(np.float32)
-            obs[rng.random(n) < 0.01] = 100.0                               # clipped after normalisation
+            obs = observations(rng, n, O, outliers=0.01)                     # clipped after normalisation
             begin = rng.random(n) < 0.05
             x, b = torch.from_numpy(obs).cuda(), torch.from_numpy(begin.astype(np.uint8)).cuda()
-            g = _np(net.perform(x, training=True, seed=SEED, step=t, env_offset=OFFSET, begin=b))
+            g = to_numpy(net.perform(x, training=True, seed=SEED, step=t, env_offset=OFFSET, begin=b))
             hid = net.state_dict()["hidden"][torch.from_numpy(idx).cuda()].cpu().numpy()
             _, mean, _, value, h = RO.perform(w, f, obs[idx], False, state=h, begin=begin[idx])
-            z = np.array([[AO.normal_noise(SEED, OFFSET + int(e), t, a) for a in range(A)] for e in idx])
-            logstd = w["logstd"].astype(np.float64)
+            action, logprob = sampled(mean, w["logstd"], noise(SEED, t, OFFSET + idx, A))
             e = dict(hidden=np.abs(hid - h).max(), mean=np.abs(g["mean"][idx] - mean).max(),
-                     action=np.abs(g["action"][idx] - (mean + np.exp(logstd) * z)).max(), value=np.abs(g["value"][idx] - value).max(),
-                     logprob=np.abs(g["logprob"][idx] - (-0.5 * z * z - logstd - 0.5 * math.log(2 * math.pi)).sum(1)).max())
+                     action=np.abs(g["action"][idx] - action).max(), value=np.abs(g["value"][idx] - value).max(),
+                     logprob=np.abs(g["logprob"][idx] - logprob).max())
             for k in TOL:
                 assert e[k] < TOL[k], (n, t, k, e[k])
                 worst[k] = max(worst[k], e[k])
             err_h.append(e["hidden"])
             if t in (0, 63):
-                assert np.array_equal(_np(ff.perform(x, training=False))["value"], g["value"]), (n, t)
+                assert np.array_equal(to_numpy(ff.perform(x, training=False))["value"], g["value"]), (n, t)
         assert max(err_h[56:]) <= 4 * max(max(err_h[:8]), 2.0 ** -20), (n, err_h[:8], err_h[56:])
-    print("worst errors", row_id(row), worst)
+    print("worst errors", gru_id(row), worst)
     net.close(); ff.close()
 
 
@@ -146,8 +67,8 @@ def _snapshot(row, n, steps=3, seed=5):
     """A network after `steps` steps with random begins, its state S, and the next step's inputs."""
     O, A, H1, G, vl = row
     rng = np.random.default_rng(seed)
-    w, f = _weights(rng, O, A, H1, G, vl), _filters(rng, O)
-    net = _net(row, n, w, f)
+    w, f = gru_weights(rng, O, A, H1, G, vl), fitted_filter(rng, O)
+    net = gru_net(row, n, w, f)
     for t in range(steps):
         x = torch.from_numpy(rng.normal(0.3, 3.0, (n, O)).astype(np.float32)).cuda()
         net.perform(x, training=True, seed=SEED, step=t, env_offset=OFFSET,
@@ -159,7 +80,7 @@ def _snapshot(row, n, steps=3, seed=5):
 
 def _run(net, sd, x, m, **kw):
     net.load_state_dict(sd)
-    out = _np(net.perform(x, begin=m, **kw))
+    out = to_numpy(net.perform(x, begin=m, **kw))
     out["hidden"] = net.state_dict()["hidden"].cpu().numpy()
     return out
 
@@ -171,16 +92,16 @@ def _rows_of(sd, rows):
 KEYS = ("action", "mean", "logprob", "value", "hidden")
 
 
-@pytest.mark.parametrize("row", ROWS[:2] + ROWS[5:6], ids=row_id)
+@pytest.mark.parametrize("row", GRU_ROWS[:2] + GRU_ROWS[5:6], ids=gru_id)
 def test_begin_continue_value_only_position_and_shards_bit_for_bit(row):
-    n = 64 * _sm() + 37                                                # several tiles on some CTAs
+    n = 64 * sm_count() + 37                                           # several tiles on some CTAs
     net, w, f, S, x, m = _snapshot(row, n)
     kw = dict(training=True, seed=SEED, step=7, env_offset=OFFSET)
     ref = _run(net, S, x, m, **kw)
     mb = m.cpu().numpy().astype(bool)
     # a begin row equals a fresh network's output for the same observation
-    fresh = _net(row, n, w, f)
-    fr = _np(fresh.perform(x, **kw))
+    fresh = gru_net(row, n, w, f)
+    fr = to_numpy(fresh.perform(x, **kw))
     fr["hidden"] = fresh.state_dict()["hidden"].cpu().numpy()
     for k in KEYS:
         assert np.array_equal(ref[k][mb], fr[k][mb]), k
@@ -203,7 +124,7 @@ def test_begin_continue_value_only_position_and_shards_bit_for_bit(row):
         assert np.array_equal(pd[k], det[k][p]), k
     # a shard (env_offset = k) reproduces the rows of the whole batch, sampling included; so does a lone env
     for k0, k1 in ((37, n), (0, 1), (n - 1, n), (64, 129)):
-        shard = _net(row, k1 - k0, w, f)
+        shard = gru_net(row, k1 - k0, w, f)
         out = _run(shard, _rows_of(S, slice(k0, k1)), x[k0:k1].contiguous(), m[k0:k1].contiguous(), training=True, seed=SEED,
                    step=7, env_offset=OFFSET + k0)
         for k in KEYS:
@@ -215,50 +136,37 @@ def test_begin_continue_value_only_position_and_shards_bit_for_bit(row):
 def test_sampling_noise_is_the_feed_forward_networks():
     """With zero mean heads both networks sample action = exp(logstd) * eps exactly: the recurrent, linear and feed-forward
     networks draw the same eps for the same (seed, env_offset + env, step), and give the same log-prob."""
-    from rex_gym_b200.agents import LinearGaussianPolicy
-    O, A, H1, G, vl = ROWS[1]
+    O, A, H1, G, vl = GRU_ROWS[1]
     rng = np.random.default_rng(3)
-    w, f = _weights(rng, O, A, H1, G, vl), _filters(rng, O)
+    w, f = gru_weights(rng, O, A, H1, G, vl), fitted_filter(rng, O)
     w.update(pW3=np.zeros((G, A), np.float32), pb3=np.zeros(A, np.float32))
     n = 5000
-    net = _net(ROWS[1], n, w, f)
-    ff = _ff(O, A, vl, w, f, dict(pW3=np.zeros((vl[1], A), np.float32), pb3=np.zeros(A, np.float32), logstd=w["logstd"]))
-    lin = LinearGaussianPolicy(O, A, value_layers=vl, num_envs=n)
-    lin.set_weights(dict(w, pW=np.zeros((O, A), np.float32), pb=np.zeros(A, np.float32)))
-    lin.set_filters(f.count, f.mean, f.var_sum, 0, 0.0, 0.0)
+    net = gru_net(GRU_ROWS[1], n, w, f)
+    ff = ff_value_twin(O, A, vl, w, f, dict(pW3=np.zeros((vl[1], A), np.float32), pb3=np.zeros(A, np.float32), logstd=w["logstd"]))
+    lin = lin_net(O, A, vl, n, dict(w, pW=np.zeros((O, A), np.float32), pb=np.zeros(A, np.float32)), f)
     x = torch.from_numpy(rng.normal(size=(n, O)).astype(np.float32)).cuda()
     kw = dict(training=True, seed=SEED, step=11, env_offset=OFFSET)
-    a, b, c = _np(net.perform(x, **kw)), _np(ff.perform(x, **kw)), _np(lin.perform(x, **kw))
+    a, b, c = to_numpy(net.perform(x, **kw)), to_numpy(ff.perform(x, **kw)), to_numpy(lin.perform(x, **kw))
     for k in ("action", "logprob", "value"):
         assert np.array_equal(a[k], b[k]) and np.array_equal(c[k], b[k]), k
     assert np.abs(a["action"]).max() > 0.1
     net.close(); ff.close(); lin.close()
 
 
-LIN_ROWS = [(4, 2, (200, 100)), (16, 4, (200, 100)), (32, 8, (64, 12)), (1, 1, (64, 12))]
-
-
-@pytest.mark.parametrize("row", LIN_ROWS, ids=lambda r: "O%d-A%d" % r[:2])
+@pytest.mark.parametrize("row", LIN_ROWS, ids=lin_id)
 def test_linear_policy_matches_the_oracle(row):
-    from rex_gym_b200.agents import LinearGaussianPolicy
     O, A, vl = row
     rng = np.random.default_rng(7 * O + A)
-    f = _filters(rng, O)
-    w = _weights(rng, O, A, 4, 4, vl)
-    w.update(pW=(rng.standard_normal((O, A)) / math.sqrt(O)).astype(np.float32), pb=rng.normal(0, 0.1, A).astype(np.float32))
+    f = fitted_filter(rng, O)
+    w = lin_weights(rng, O, A, vl)
     sizes = [1, 127, 128, 129, 65536 + 37]
-    net = LinearGaussianPolicy(O, A, value_layers=vl, num_envs=max(sizes))
-    net.set_weights(w)
-    net.set_filters(f.count, f.mean, f.var_sum, 0, 0.0, 0.0)
-    obs = rng.normal(0.3, 3.0, (max(sizes), O)).astype(np.float32)
+    net = lin_net(O, A, vl, max(sizes), w, f)
+    obs = observations(rng, max(sizes), O)
     for n in sizes:
-        g = _np(net.perform(torch.from_numpy(obs[:n]).cuda(), training=True, seed=SEED, step=3, env_offset=OFFSET))
-        idx = _probes(n, 128)
+        g = to_numpy(net.perform(torch.from_numpy(obs[:n]).cuda(), training=True, seed=SEED, step=3, env_offset=OFFSET))
+        idx = tile_probes(n, 128)
         _, want_m, _, want_v, _ = RO.perform(w, f, obs[idx], False)
-        z = np.array([[AO.normal_noise(SEED, OFFSET + int(e), 3, a) for a in range(A)] for e in idx])
-        logstd = w["logstd"].astype(np.float64)
-        want_a = want_m + np.exp(logstd) * z
-        want_lp = (-0.5 * z * z - logstd - 0.5 * math.log(2 * math.pi)).sum(1)
+        want_a, want_lp = sampled(want_m, w["logstd"], noise(SEED, 3, OFFSET + idx, A))
         assert np.abs(g["mean"][idx] - want_m).max() < 2e-5 and np.abs(g["value"][idx] - want_v).max() < TOL["value"], n
         assert np.abs(g["action"][idx] - want_a).max() < 5e-5 and np.abs(g["logprob"][idx] - want_lp).max() < TOL["logprob"], n
     net.close()
@@ -313,9 +221,8 @@ def test_recurrent_rollout_graph_loop_oracle_and_resume():
     rng = np.random.default_rng(4)
     w = net.get_weights()
     w.update(w_ru=(w["w_ru"] * 2).astype(np.float32), b_ru=rng.normal(0, 1, w["b_ru"].shape).astype(np.float32))
-    net.set_weights(w)
-    f = _filters(rng, env.obs_dim)
-    net.set_filters(f.count, f.mean, f.var_sum, 0, 0.0, 0.0)
+    f = fitted_filter(rng, env.obs_dim)
+    load(net, w, f)
     wins = [{k: v.clone().cpu().numpy() for k, v in ro.collect().items()} for _ in range(2)]
     want, h = _replay(w, f, wins, net.G)
     got = [(win["mean"][t], win["value"][t]) for win in wins for t in range(T)]
@@ -342,8 +249,8 @@ def test_linear_rollout_runs_and_matches_the_oracle():
     n, T = 512, 16
     env, net, ro = _rollout(LinearGaussianPolicy, n, T, True, False)
     rng = np.random.default_rng(6)
-    f = _filters(rng, env.obs_dim)
-    net.set_filters(f.count, f.mean, f.var_sum, 0, 0.0, 0.0)
+    f = fitted_filter(rng, env.obs_dim)
+    load(net, f=f)
     w = net.get_weights()
     win = {k: v.clone().cpu().numpy() for k, v in ro.collect().items()}
     for t in range(T):

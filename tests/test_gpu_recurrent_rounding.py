@@ -13,10 +13,10 @@ test_gpu_recurrent_agent.py holds the cells to the fp64 oracle at 2e-4; this fil
     r gate     u = 0, w_c = [0; I], h = 1: h' = tanhf(sigmoidf(pre_r)) within the composed bound
     blend      the u readout with w_ru's h rows of u zero, the candidate readout, then both at once: h' equals
                                       fmaf(U, h, (1 - U) T) bit for bit, U and T the two readouts' device values
-  Each on realistic weights (test_gpu_recurrent_agent._weights: the restated chains catch any reordering) and on exact
+  Each on realistic weights (agent_twin.gru_weights: the restated chains catch any reordering) and on exact
   networks (dyadic inputs, weights and states, every partial sum exact in fp32, asserted on the arrays: blind to order,
   they catch a wrong row, column or tile; non-zeros in the first and last row of every 16-row chunk, at k = H1 - 1 and H1
-  and in the whole last chunk, in every column).  Every batch size of test_gpu_recurrent_agent.batch_sizes(), random begin
+  and in the whole last chunk, in every column).  Every batch size of agent_twin.gru_batch_sizes(), random begin
   masks, and the state rows n .. num_envs - 1 bit-unchanged.
 * The full cell on realistic weights over 64 steps, free of trajectory divergence: each step is restated from the state
   the device held before it and held to agent_restate.gru_step_bound (its docstring derives it).
@@ -34,14 +34,14 @@ import pytest
 import torch
 
 import agent_restate as R
+from agent_twin import (GRU_ROWS, LIN_ROWS, SEED, fitted_filter, gru_batch_sizes, gru_id, gru_net, gru_weights, lin_head,
+                        lin_id, lin_net, lin_weights, load, observations, sm_count, tile_probes, to_numpy)
 from oracle import agent_oracle as AO
 from oracle import recurrent_oracle as RO
-from test_gpu_recurrent_agent import (LIN_ROWS, ROWS as AGENT_ROWS, SEED, _filters, _net, _probes, _sm, _weights,
-                                      batch_sizes, row_id)
 
 F32 = np.float32
 KC = 16                                     # gru_gemm's rows per streamed chunk (RNN_KC)
-ROWS = AGENT_ROWS + [  # (O, A, H1, G, value layers): the chunk geometry the agent rows miss
+ROWS = GRU_ROWS + [  # (O, A, H1, G, value layers): the chunk geometry the agent rows miss
     (4, 2, 4, 4, (64, 12)),               # K = 8: one partial chunk; 16 of the block's 128 threads compute cell columns
     (4, 2, 20, 4, (64, 12)),              # K = 24: a short last chunk of 8 with the a1 -> h switch inside it
     (4, 2, 252, 8, (64, 12)),             # K = 260: 17 chunks, a last chunk of 4, the switch inside chunk 15
@@ -73,11 +73,11 @@ def exact_gru_network(O, A, H1, G, n, vl, seed=0):
     """(weights, observ mean, observations [n][O], states [n][G]) on dyadic grids, with filter count 0 (inv = 1): observations
     and means on 1/4 (a tenth beyond the clip), W1 in +-{1/16, 1/8}, b1 on 1/8, w_ru and w_c sparse in +-{1/32, 1/16, 1/8}
     with every special_rows row non-zero in every column, states on 1/8 in [-1, 1], W3 on 1/8 with rows 0 and G - 1
-    non-zero, b3 non-zero.  The value network is _weights' (not read out here)."""
+    non-zero, b3 non-zero.  The value network is gru_weights' (not read out here)."""
     rng = np.random.default_rng(seed + 1000 * O + 100 * A + H1 + G)
     K, rows = H1 + G, special_rows(H1, G)
     q = np.array([1, 2, 4]) / 32.0
-    w = {k: v for k, v in _weights(rng, O, A, H1, G, vl).items() if k[0] == "v"}
+    w = {k: v for k, v in gru_weights(rng, O, A, H1, G, vl).items() if k[0] == "v"}
     w.update(pW1=rng.choice([-0.125, -0.0625, 0.0625, 0.125], (O, H1)).astype(F32), pb1=(rng.integers(-8, 9, H1) / 8).astype(F32),
              w_ru=_sparse(rng, (K, 2 * G), np.r_[-q, q], 0.05, rows), b_ru=(rng.integers(-16, 17, 2 * G) / 8).astype(F32),
              w_c=_sparse(rng, (K, G), np.r_[-q, q], 0.05, rows), b_c=(rng.integers(-8, 9, G) / 8).astype(F32),
@@ -280,27 +280,27 @@ def test_extreme_draw_search():
             assert abs(k2 + 0.5 - float(name.split()[1]) * 2 ** 23) < 40
 
 
-@pytest.mark.parametrize("row", ROWS[:2] + ROWS[-3:], ids=row_id)
+@pytest.mark.parametrize("row", ROWS[:2] + ROWS[-3:], ids=gru_id)
 def test_restatements_against_the_fp64_oracle(row):
     """The GRU step (gru_step_bound) and the linear head (fma_chain) against recurrent_oracle in fp64: the new state and the
     mean at fp32 distance, and inside the step bound, which stays far below the 2e-4 of test_gpu_recurrent_agent."""
     O, A, H1, G, vl = row
     rng = np.random.default_rng(O + H1 + G)
-    w, f = _weights(rng, O, A, H1, G, vl), _filters(rng, O)
-    obs = rng.normal(0.3, 3.0, (64, O)).astype(F32)
+    w, f = gru_weights(rng, O, A, H1, G, vl), fitted_filter(rng, O)
+    obs = observations(rng, 64, O)
     h = rng.uniform(-0.9, 0.9, (64, G)).astype(F32)
     x = R.normalise(obs, *R.normaliser(f.count, f.mean, f.var_sum))
     hp, dh, s, es = R.gru_step_bound(w, R.layer1(x, w["pW1"], w["pb1"]), h)
     _, mean, _, _, h2 = RO.perform(w, f, obs, False, state=h)
     assert np.abs(hp - h2).max() < 1e-5 and np.abs(np.tanh(s) - mean).max() < 1e-5
     assert np.all(np.abs(hp - h2) <= dh + 1e-6) and dh.max() < 2e-5, float(dh.max())
-    w.update(pW=(rng.standard_normal((O, A)) / math.sqrt(O)).astype(F32), pb=rng.normal(0, 0.1, A).astype(F32))
+    w.update(lin_head(rng, O, A))
     sl = R.fma_chain(x, w["pW"], w["pb"])
     want, _, _ = RO.linear_gaussian_policy(w, f.transform(obs))
     np.testing.assert_allclose(np.tanh(sl.astype(np.float64)), want, atol=2e-5)
 
 
-@pytest.mark.parametrize("row", ROWS, ids=row_id)
+@pytest.mark.parametrize("row", ROWS, ids=gru_id)
 def test_constructed_networks_are_exact(row):
     """Every exact network (at the largest batch of a 132-SM H100) and its readouts: the chains exact in fp32, the
     saturations in force, the special rows non-zero in every column, the u and r pre-activations spread over +-8."""
@@ -323,7 +323,7 @@ def test_constructed_networks_are_exact(row):
             assert np.mean(np.abs(pre) < 8) > 0.3, kind
 
 
-@pytest.mark.parametrize("row", ROWS[-4:], ids=row_id)
+@pytest.mark.parametrize("row", ROWS[-4:], ids=gru_id)
 def test_new_rows_are_accepted(row):
     import ctypes as C
     from rex_gym_b200 import _capi
@@ -333,47 +333,36 @@ def test_new_rows_are_accepted(row):
 
 
 # ---- GPU -----------------------------------------------------------------------------------------------------------------
-def _rnet(row, n, w, count, mean, var_sum):
-    from rex_gym_b200.agents import RecurrentGaussianPolicy
-    O, A, H1, G, vl = row
-    net = RecurrentGaussianPolicy(O, A, (H1, 100), vl, seed=1, num_envs=n, cell_size=G)
-    net.set_weights(w)
-    net.set_filters(count, mean, var_sum, 0, 0.0, 0.0)
-    return net
-
-
 def _hidden(net):
     return net.state_dict()["hidden"].cpu().numpy()
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind", ["realistic", "exact"])
-@pytest.mark.parametrize("row", ROWS, ids=row_id)
+@pytest.mark.parametrize("row", ROWS, ids=gru_id)
 def test_gate_readouts(row, kind):
     O, A, H1, G, vl = row
-    sizes = batch_sizes()
+    sizes = gru_batch_sizes()
     N = max(sizes)
     rng = np.random.default_rng(10 * O + A + H1 + G)
     if kind == "realistic":
-        w, f = _weights(rng, O, A, H1, G, vl), _filters(rng, O)
+        w, f = gru_weights(rng, O, A, H1, G, vl), fitted_filter(rng, O)
         filt = (f.count, f.mean, f.var_sum)
-        obs = rng.normal(0.3, 3.0, (N, O)).astype(F32)
-        obs[rng.random(N) < 0.01] = 100.0
+        obs = observations(rng, N, O, outliers=0.01)
         hs = rng.uniform(-0.9, 0.9, (N, G)).astype(F32)
     else:
         w, mean, obs, hs = exact_gru_network(O, A, H1, G, N, vl)
         filt = (0, mean, np.zeros(O, F32))
     begin = rng.random(N) < 0.05
-    probes = {n: _probes(n) for n in sizes}
+    probes = {n: tile_probes(n) for n in sizes}
     rows = np.unique(np.concatenate(list(probes.values())))
     where = {e: i for i, e in enumerate(rows)}
     x = R.normalise(obs[rows], *R.normaliser(*filt))
     a1 = assert_exact_inputs(w, x, hs[rows]) if kind == "exact" else R.layer1(x, w["pW1"], w["pb1"])
-    net = _rnet(row, N, w, *filt)
+    net = gru_net(row, N, w, filt)
     xd, bd = torch.from_numpy(obs).cuda(), torch.from_numpy(begin.astype(np.uint8)).cuda()
     sd = net.state_dict()
     ones = np.ones((N, G), F32)
-    device = {}
 
     def run(wr, state, n, steps=1, use_begin=True):
         net.set_weights(wr)
@@ -416,22 +405,21 @@ def test_gate_readouts(row, kind):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("row", ROWS, ids=row_id)
+@pytest.mark.parametrize("row", ROWS, ids=gru_id)
 def test_full_cell_within_the_one_step_bound(row, capsys):
-    """_weights over 64 steps with fresh observations and 5 % episode starts at 64 x SMs + 1 envs: before each step the
+    """gru_weights over 64 steps with fresh observations and 5 % episode starts at 64 x SMs + 1 envs: before each step the
     device's state of the probe rows is read; every step is restated from it (agent_restate.gru_step_bound) and the new
     state and the mean held to the bound.  Prints the largest error / bound ratios and the largest bounds."""
     O, A, H1, G, vl = row
     rng = np.random.default_rng(1000 + O + A + H1 + G)
-    w, f = _weights(rng, O, A, H1, G, vl), _filters(rng, O)
-    n = 64 * _sm() + 1
-    net = _net(row, n, w, f)
-    idx = _probes(n)
+    w, f = gru_weights(rng, O, A, H1, G, vl), fitted_filter(rng, O)
+    n = 64 * sm_count() + 1
+    net = gru_net(row, n, w, f)
+    idx = tile_probes(n)
     idt = torch.from_numpy(idx).cuda()
     rec = {k: [] for k in ("obs", "h0", "h1", "mean")}
     for t in range(64):
-        obs = rng.normal(0.3, 3.0, (n, O)).astype(F32)
-        obs[rng.random(n) < 0.01] = 100.0
+        obs = observations(rng, n, O, outliers=0.01)
         begin = rng.random(n) < 0.05
         before = net.state_dict()["hidden"][idt].cpu().numpy()
         g = net.perform(torch.from_numpy(obs).cuda(), training=False, begin=torch.from_numpy(begin.astype(np.uint8)).cuda())
@@ -447,27 +435,24 @@ def test_full_cell_within_the_one_step_bound(row, capsys):
     rm = np.abs(mean - np.tanh(s)) / bm
     with capsys.disabled():
         print("\n%s: full cell, largest error / bound: state %.3f, mean %.3f (bounds up to %.2e / %.2e)" % (
-            row_id(row), rh.max(), rm.max(), dh.max(), bm.max()))
+            gru_id(row), rh.max(), rm.max(), dh.max(), bm.max()))
     assert rh.max() <= 1 and rm.max() <= 1, (float(rh.max()), float(rm.max()))
     assert dh.max() < 2e-5 and bm.max() < 2e-5
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("row", LIN_ROWS, ids=lambda r: "O%d-A%d" % r[:2])
+@pytest.mark.parametrize("row", LIN_ROWS, ids=lin_id)
 def test_linear_policy_head_and_exact_networks(row):
     """Realistic weights: on every row of every batch size the mean within tanhf's 2 ulp of tanh(fma_chain(x, pW, pb)), the
     deterministic action equal to it.  Exact networks (x on 1/4 with filter count 0, pW on +-{1/8, 1/4, 1/2}, pb on 1/8): the
     same against the exact sum, at every size including both edges of each 128-env tile."""
-    from rex_gym_b200.agents import LinearGaussianPolicy
     O, A, vl = row
     rng = np.random.default_rng(3 * O + A)
-    f = _filters(rng, O)
+    f = fitted_filter(rng, O)
     sizes = [1, 127, 128, 129, 255, 256, 257, 65536 + 37]
     N = max(sizes)
-    w = _weights(rng, O, A, 4, 4, vl)
-    w.update(pW=(rng.standard_normal((O, A)) / math.sqrt(O)).astype(F32), pb=rng.normal(0, 0.1, A).astype(F32))
-    obs = rng.normal(0.3, 3.0, (N, O)).astype(F32)
-    obs[rng.random(N) < 0.01] = 100.0
+    w = lin_weights(rng, O, A, vl)
+    obs = observations(rng, N, O, outliers=0.01)
     s_real = R.fma_chain(R.normalise(obs, *R.normaliser(f.count, f.mean, f.var_sum)), w["pW"], w["pb"])
     we = dict(w, pW=rng.choice([-0.5, -0.25, -0.125, 0.125, 0.25, 0.5], (O, A)).astype(F32),
               pb=rng.choice([-0.375, -0.125, 0.125, 0.375], A).astype(F32))
@@ -475,13 +460,12 @@ def test_linear_policy_head_and_exact_networks(row):
     oe = (rng.integers(-28, 29, (N, O)) / 4).astype(F32)
     s_exact = R.assert_exact_dot(R.normalise(oe, me, np.ones(O, F32)), we["pW"], we["pb"], "linear")
     np.testing.assert_array_equal(R.fma_chain(R.normalise(oe, me, np.ones(O, F32)), we["pW"], we["pb"]), s_exact)
-    net = LinearGaussianPolicy(O, A, value_layers=vl, num_envs=N)
-    for ww, filt, ob, s in ((w, (f.count, f.mean, f.var_sum), obs, s_real), (we, (0, me, np.zeros(O, F32)), oe, s_exact)):
-        net.set_weights(ww)
-        net.set_filters(*filt, 0, 0.0, 0.0)
+    net = lin_net(O, A, vl, N)
+    for ww, filt, ob, s in ((w, f, obs, s_real), (we, (0, me, np.zeros(O, F32)), oe, s_exact)):
+        load(net, ww, filt)
         xd = torch.from_numpy(ob).cuda()
         for n in sizes:
-            g = {k: v.cpu().numpy() for k, v in net.perform(xd[:n], training=False).items()}
+            g = to_numpy(net.perform(xd[:n], training=False))
             ratio = R.within_tanhf(g["mean"], s[:n])
             assert ratio.max() <= 1, (n, float(ratio.max()), np.unravel_index(ratio.argmax(), ratio.shape))
             assert np.array_equal(g["action"], g["mean"]), n
@@ -500,7 +484,7 @@ def test_sampler_at_its_extreme_draws(cell, capsys):
     worst = [0.0, 0.0]
     for (a, name), g in sorted(ex.items()):
         off = max(g - 17, 0)
-        out = {k: v.cpu().numpy() for k, v in net.perform(x, training=True, seed=SEED, step=step, env_offset=off).items()}
+        out = to_numpy(net.perform(x, training=True, seed=SEED, step=step, env_offset=off))
         act, da, lp, dl = sampler_expected(SEED, np.arange(off, off + n, dtype=np.uint64), step, logstd, out["mean"])
         ra, rl = np.abs(out["action"] - act) / da, np.abs(out["logprob"] - lp) / dl
         assert ra.max() <= 1 and rl.max() <= 1, (a, name, g, float(ra.max()), float(rl.max()))
@@ -518,7 +502,7 @@ def test_the_top_draw_is_not_one(cell):
     seed, g, step, a = ONE_DRAW
     net, logstd = _cell(cell, 1)
     x = torch.zeros((1, 4), device="cuda")
-    out = {k: v.cpu().numpy() for k, v in net.perform(x, training=True, seed=seed, step=step, env_offset=g).items()}
+    out = to_numpy(net.perform(x, training=True, seed=seed, step=step, env_offset=g))
     net.close()
     act, da, _, _ = sampler_expected(seed, np.array([g], np.uint64), step, logstd, out["mean"])
     assert out["action"][0, a] != out["mean"][0, a]

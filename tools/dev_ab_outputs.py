@@ -11,9 +11,9 @@ Random actions from reset rarely reach the generic solver path, so every configu
 also runs from that test's start states (body, arm and multi-limit contacts): 4 single sub-steps, then 4 control steps of the
 task configuration, hashing the solver cost as well.  Last, render_batch frames of a few envs of walk-ik on flat ground,
 turn-ik on the random heightfields and standup with the arm, with the default camera and at 97 x 61.  Then the agent kernels:
-every network of tests/test_gpu_agent_shapes.ROWS in its precision at that test's batch sizes (perform's four outputs, noise-free
-and sampled), the filter update (whole batch and partial + finalize: filter state and counters) and the reward transform, and
-the three scans on seeded inputs.
+every network of tests/agent_twin.FF_ROWS in its precision at the feed-forward batch sizes, on agent_twin.ff_setup's inputs
+(perform's four outputs, noise-free and sampled), the filter update (whole batch and partial + finalize: filter state and
+counters) and the reward transform, and the three scans on seeded inputs.
 Every later library is compared with the first: each array that is not bit-identical is reported, and for a frame the number
 of pixels that differ."""
 import hashlib
@@ -102,33 +102,33 @@ def render_cases(R, res, frames):
 
 
 def agent_cases(res):
-    """perform, experience, transform_reward of every tests/test_gpu_agent_shapes row; the three scans."""
+    """perform, experience, transform_reward of every tests/agent_twin.FF_ROWS row; the three scans."""
     import torch
-    import test_gpu_agent_shapes as S
+    import agent_twin as T
     from rex_gym_b200.agents import utility
-    sizes = S.batch_sizes(S._half())
-    for row in S.ROWS:
-        _, _, obs, nets = S._setup(row, max(sizes))
+    sizes = T.ff_batch_sizes(T.half_sm())
+    for row in T.FF_ROWS:
+        _, _, obs, nets = T.ff_setup(row, max(sizes))
         net = nets[-1]
         x_all = torch.from_numpy(obs).cuda()
         rew_all = torch.from_numpy(np.random.default_rng(3).normal(0.1, 0.5, max(sizes)).astype(np.float32)).cuda()
-        rec = res["agent-" + S.row_id(row)] = {}
+        rec = res["agent-" + T.ff_id(row)] = {}
         for n in sizes:
             for training in (False, True):
-                out = net.perform(x_all[:n], training=training, seed=S.SEED, step=S.STEP, env_offset=S.OFFSET)
+                out = net.perform(x_all[:n], training=training, seed=T.SEED, step=T.STEP, env_offset=T.OFFSET)
                 for k, t in out.items():
                     rec[f"n{n}_{'sampled' if training else 'mean'}_{k}"] = digest(t.cpu().numpy())
         for n in sizes:
             net.experience(x_all[:n], rew_all[:n])
             rec[f"n{n}_experience"] = digest(np.r_[net._filt.cpu().numpy().view(np.int32), net._cnt.cpu().numpy().view(np.int32)])
-            S._experience_split(net, x_all[:n], rew_all[:n])
+            T.experience_split(net, x_all[:n], rew_all[:n])
             rec[f"n{n}_partial_finalize"] = digest(np.r_[net._filt.cpu().numpy().view(np.int32), net._cnt.cpu().numpy().view(np.int32)])
             rec[f"n{n}_transform_reward"] = digest(net.transform_reward(rew_all[:n]).cpu().numpy())
         for nt in nets:
             nt.close()
     rng = np.random.default_rng(17)
     rec = res["agent-scans"] = {}
-    for L in S.SCAN_LENGTHS:
+    for L in T.SCAN_LENGTHS:
         r, v = (torch.from_numpy(rng.normal(size=(300, L)).astype(np.float32)).cuda() for _ in range(2))
         length = torch.from_numpy(rng.integers(0, L + 1, 300).astype(np.int32)).cuda()
         rec[f"L{L}_return"] = digest(utility.discounted_return(r, length, 0.985).cpu().numpy())
