@@ -14,6 +14,9 @@
  *   rexsim_step     <- BatchEnv.step(actions) -> RexGymEnv.step: signal -> Rex.Step x action_repeat
  *                      (ApplyAction + stepSimulation + ReceiveObservation) -> reward/termination/obs
  *                      (rex_gym/agents/tools/batch_env.py:63-90; rex_gym/envs/rex_gym_env.py:369-414)
+ *   rexsim_step_final
+ *                   <- the same, plus the terminal observation BatchEnv.step returns and gym TimeLimit's
+ *                      info['TimeLimit.truncated'] (in_graph_batch_env.py:71-92; gym 0.17.1 wrappers/time_limit.py)
  *   rexsim_get_state / rexsim_set_state
  *                   <- getBasePositionAndOrientation / getBaseVelocity / getJointState /
  *                      resetBasePositionAndOrientation / resetJointState (rex_gym/model/rex.py:297-299,
@@ -168,6 +171,24 @@ int rexsim_step(RexSim* sim, const float* actions, float* obs, float* reward, ui
  * and N <= 16384 the kernel addresses the host block directly (zero-copy) and the two bulk copies disappear. */
 int64_t rexsim_host_out_bytes(const RexSim* sim);
 int rexsim_step_host(RexSim* sim, const float* h_actions, void* h_out, void* stream);
+/* rexsim_step plus the two outputs an auto-resetting step would otherwise lose (the reference's BatchEnv.step returns the
+ * terminal observation and resets at the top of the next iteration, simulate.py:67-75, in_graph_batch_env.py:71-113; gym's
+ * TimeLimit tells a time-limit cut from a termination, gym 0.17.1 wrappers/time_limit.py).  Either may be NULL:
+ *   final_obs dev [N][O] f32 (O = rexsim_out_dim): for every env whose step returned done, the observation `obs` would hold with
+ *     auto_reset = 0 (RangeNormalize, the sensor model's delayed noisy reads and the frame wrappers included); rows of the other
+ *     envs are left untouched.
+ *   limit dev [N] u8, written for every env: bit 0 = max_episode_steps was reached at this step; bit 1 = the episode also ended
+ *     for another reason (the task's termination or the non-finite guard).  TimeLimit's info['TimeLimit.truncated'] is present
+ *     iff bit 0 is set, with the value !(bit 1).
+ * rexsim_step launches exactly what it launched before this entry point existed. */
+int rexsim_step_final(RexSim* sim, const float* actions, float* obs, float* reward, uint8_t* done, float* final_obs,
+                      uint8_t* limit, void* stream);
+/* Host-buffer form of rexsim_step_final: h_out as in rexsim_step_host, h_final HOST block of rexsim_host_final_bytes() bytes laid out
+ * as final obs [N][O] f32 | limit [N] u8.  Zero-copy when all three buffers are pinned and N <= 16384; otherwise the kernel writes
+ * a device staging block that is copied out whole, so the rows of envs that did not end hold what that path last wrote there.
+ * Either way a caller that keeps one block and one path gets the bytes rexsim_step_final writes into a device block. */
+int64_t rexsim_host_final_bytes(const RexSim* sim);
+int rexsim_step_host_final(RexSim* sim, const float* h_actions, void* h_out, void* h_final, void* stream);
 /* Re-group the environments over the warps by the solver cost of their last control step (counting sort on the device, three
  * small launches).  The step kernel's cost per env is dominated by its PGS iteration count, and a warp of 8 envs runs as long
  * as its slowest one; in a de-synchronised batch (auto-reset) grouping envs of similar cost recovers most of that loss.
@@ -259,6 +280,16 @@ uint32_t rexsim_rand_u32(uint64_t seed, uint32_t global_env, uint32_t reset_coun
 float rexsim_noise(uint64_t seed, uint32_t global_env, uint32_t reset_count, uint32_t control_step, uint32_t site, uint32_t comp);
 /* rows per env of the sensor history ring this configuration keeps (0: sensor model off) */
 int rexsim_history_depth(const RexSimConfig* cfg);
+/* rexagent_gae_segments (rexsim_agent.h) that bootstraps episodes cut by the time limit instead of treating their last step as terminal (the
+ * reference's PPO never does: it has no final observation).  truncated dev [T][N] u8 (non-zero: truncated), final_value dev
+ * [T][N] f32 (the value of the step's final observation, rexsim_step_final; read only where done and truncated are both set).
+ * At such a step: delta_t = r_t + discount * final_value_t - v_t, adv_t = delta_t, return_t = r_t + discount * final_value_t.
+ * Every other step is computed as rexagent_gae_segments computes it, in the same fp32 order: with truncated all zero the
+ * outputs are bit-identical to it.  Declared here, not in rexsim_agent.h, whose entry-point list is held fixed (the agent ABI
+ * tests pin its 20 functions, so that bindings generated from it stay complete); like rexagent_gae_segments it takes no handle. */
+int rexsim_gae_segments_bootstrap(const float* reward, const float* value, const uint8_t* done, const uint8_t* truncated,
+                                  const float* final_value, int32_t T, int32_t n, float discount, float lambda,
+                                  float* out_return, float* out_advantage, void* stream);
 const char* rexsim_last_error(void);
 
 #ifdef __cplusplus

@@ -100,6 +100,7 @@ int rexagent_lambda_advantage(const float* reward, const float* value, const int
  * return_T = bootstrap value */
 int rexagent_gae_segments(const float* reward, const float* value, const uint8_t* done, int32_t T, int32_t n,
                           float discount, float lambda, float* out_return, float* out_advantage, void* stream);
+/* (its form that bootstraps episodes cut by the time limit, rexsim_gae_segments_bootstrap, is declared in rexsim.h) */
 int64_t rexagent_launch_count(const RexAgent* a);
 
 #ifdef __cplusplus

@@ -57,6 +57,9 @@ SIGNATURES = {
     "rexsim_step": (C.c_int, [_ptr] * 6),
     "rexsim_step_host": (C.c_int, [_ptr] * 4),
     "rexsim_host_out_bytes": (_i64, [_ptr]),
+    "rexsim_step_final": (C.c_int, [_ptr] * 8),
+    "rexsim_host_final_bytes": (_i64, [_ptr]),
+    "rexsim_step_host_final": (C.c_int, [_ptr] * 5),
     "rexsim_rebalance": (C.c_int, [_ptr, _ptr]),
     "rexsim_reset": (C.c_int, [_ptr, _ptr, _i32, _ptr, _ptr]),
     "rexsim_get_state": (C.c_int, [_ptr] * 4),
@@ -99,6 +102,7 @@ SIGNATURES = {
     "rexagent_discounted_return": (C.c_int, [_ptr, _ptr, _i32, _i32, _i64, _i64, _f32, _ptr, _ptr]),
     "rexagent_lambda_advantage": (C.c_int, [_ptr, _ptr, _ptr, _i32, _i32, _i64, _i64, _f32, _ptr, _ptr]),
     "rexagent_gae_segments": (C.c_int, [_ptr, _ptr, _ptr, _i32, _i32, _f32, _f32, _ptr, _ptr, _ptr]),
+    "rexsim_gae_segments_bootstrap": (C.c_int, [_ptr] * 5 + [_i32, _i32, _f32, _f32, _ptr, _ptr, _ptr]),
     "rexagent_launch_count": (_i64, [_ptr]),
     "rexrnn_policy_floats": (_i64, [_agent_cfg, _rnn_cfg]),
     "rexrnn_check": (C.c_int, [_agent_cfg, _rnn_cfg]),

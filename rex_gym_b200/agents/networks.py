@@ -144,6 +144,11 @@ class ForwardGaussianPolicy(object):
                    ptr(out.get("action")), ptr(out.get("mean")), ptr(out.get("logprob")), ptr(out.get("value")), ptr(observ_copy))
         return out
 
+    def value(self, observ, out=None):
+        """The value network alone on observ [n][O] (filtered as perform filters it): CUDA float32 [n]."""
+        out = torch.empty((observ.shape[0],), dtype=torch.float32, device=observ.device) if out is None else out
+        return self.perform(observ, out=dict(value=out))["value"]
+
     def experience(self, observ, reward, group=None):
         """PPOAlgorithm._define_experience's filter updates (algorithm.py:157-161) for one batch; advances the device-side
         step counter that keys the next perform's noise.  With torch.distributed initialised (env-sharded rollout, one rank per

@@ -104,6 +104,10 @@ class _PolicyCell(object):
                    ptr(observ_copy))
         return out
 
+    def value(self, observ, out=None):
+        """The value block alone (the ForwardGaussianPolicy's) on observ [n][O], any n: the cell state is not touched."""
+        return self._ff.value(observ, out)
+
     def experience(self, observ, reward, group=None):
         self._ff.experience(observ, reward, group)
 

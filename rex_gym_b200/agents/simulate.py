@@ -11,6 +11,11 @@ A recurrent network (RecurrentGaussianPolicy) gets the matching episode-start ma
 reset(), else the `done` row of the previous control step -- for the first step of a collect, the last row of the previous
 one, kept in a buffer the captured graph owns.
 The whole T-step loop is captured once into a CUDA graph and replayed: no host round trip per step (SURVEY.md 8(f) row 1).
+
+With final_observation=True the step kernel also writes, into two more [T][N] buffers of the graph, what the auto-reset would
+lose: the final observation of every env that ended (the `nextob` simulate() hands to algo.experience, simulate.py:67-75) and
+its time-limit byte (gym TimeLimit's 'TimeLimit.truncated').  returns_and_advantages(bootstrap_truncated=True) then bootstraps
+the episodes the time limit cut from the value of their final observation instead of treating them as terminal.
 """
 import torch
 
@@ -18,7 +23,7 @@ from . import utility
 
 
 class Rollout(object):
-    def __init__(self, env, network, horizon, seed=0, training=True, use_graph=True):
+    def __init__(self, env, network, horizon, seed=0, training=True, use_graph=True, final_observation=False):
         if not getattr(env._cfg, "auto_reset", 0):
             raise ValueError("Rollout needs an env created with auto_reset=True")
         if network.O != env.obs_dim or network.A != env.action_dim:
@@ -36,6 +41,11 @@ class Rollout(object):
         self.reward = torch.zeros((T, N), **f32)
         self.done = torch.zeros((T, N), dtype=torch.uint8, device=dev)
         self._cur = torch.zeros((N, O), **f32)             # observation the next action is computed from
+        self.final_observ = self.limit = self.truncated = None
+        if final_observation:
+            self.final_observ = torch.zeros((T, N, O), **f32)                     # valid where done
+            self.limit = torch.zeros((T, N), dtype=torch.uint8, device=dev)       # step kernel's time-limit bytes
+            self.truncated = torch.zeros((T, N), dtype=torch.bool, device=dev)    # limit == 1: cut by the time limit alone
         self._recurrent = bool(getattr(network, "recurrent", False))
         self._begin = torch.ones((N,), dtype=torch.uint8, device=dev) if self._recurrent else None    # episode starts of step 0
         self._graph = None
@@ -61,10 +71,15 @@ class Rollout(object):
             if self._recurrent:
                 step["begin"] = self._begin if t == 0 else self.done[t - 1]
             net.perform(self._cur, **step)
-            env.step_into(self.action[t], self._cur, self.reward[t], self.done[t])
+            if self.final_observ is None:
+                env.step_into(self.action[t], self._cur, self.reward[t], self.done[t])
+            else:
+                env.step_into(self.action[t], self._cur, self.reward[t], self.done[t], self.final_observ[t], self.limit[t])
             if self.training:
                 net.experience(self.observ[t], self.reward[t])
         net.perform(self._cur, training=False, out=dict(value=self.value[T]))       # bootstrap value of the last observation
+        if self.limit is not None:
+            torch.eq(self.limit, 1, out=self.truncated)
         if self._recurrent:
             self._begin.copy_(self.done[T - 1])
 
@@ -93,8 +108,11 @@ class Rollout(object):
                 with torch.cuda.graph(self._graph):
                     self._loop()
             self._graph.replay()
-        return dict(observ=self.observ, action=self.action, mean=self.mean, logprob=self.logprob, value=self.value,
-                    reward=self.reward, done=self.done.view(torch.bool))
+        out = dict(observ=self.observ, action=self.action, mean=self.mean, logprob=self.logprob, value=self.value,
+                   reward=self.reward, done=self.done.view(torch.bool))
+        if self.final_observ is not None:
+            out.update(final_observ=self.final_observ, truncated=self.truncated)
+        return out
 
     def summary(self, clear=True):
         """simulate()'s mean_score / mean_length (simulate.py:95-106) over the episodes that ended since the last clear: the step
@@ -102,6 +120,18 @@ class Rollout(object):
         (BatchedRexEnv.episode_summary)."""
         return self.env.episode_summary(clear)
 
-    def returns_and_advantages(self, discount, lam=1.0):
-        """Done-aware discounted return and GAE over the last rollout (utility.gae_segments)."""
-        return utility.gae_segments(self.reward, self.value, self.done, discount, lam)
+    def returns_and_advantages(self, discount, lam=1.0, bootstrap_truncated=False):
+        """Done-aware discounted return and GAE over the last rollout (utility.gae_segments).  bootstrap_truncated=True (needs
+        final_observation=True) bootstraps the steps the time limit cut from the value of their final observation: the value
+        network runs once, value only, on those rows (one host sync for their count).  Off by default, as in the reference,
+        whose PPO has no final observation to bootstrap from."""
+        if not bootstrap_truncated:
+            return utility.gae_segments(self.reward, self.value, self.done, discount, lam)
+        if self.final_observ is None:
+            raise ValueError("bootstrap_truncated needs a Rollout created with final_observation=True")
+        final_value = torch.zeros_like(self.reward)
+        rows = self.final_observ[self.truncated]          # a truncated step is a done step
+        if rows.shape[0]:
+            final_value[self.truncated] = self.net.value(rows)
+        return utility.gae_segments(self.reward, self.value, self.done, discount, lam, truncated=self.truncated,
+                                    final_value=final_value)

@@ -750,29 +750,42 @@ __global__ void __launch_bounds__(256) row_scan_kernel(const float* __restrict__
     }
 }
 
+// BOOT: a done step whose `truncated` byte is set (the episode was cut by the time limit) bootstraps from final_value, the value
+// of its final observation, and cuts the chains there: delta = r + discount * final_value - v, adv = delta, ret = r + discount *
+// final_value.  Every other step is the BOOT = false arithmetic, in the same order.  The two extra arguments come last, so the
+// BOOT = false instance reads its arguments where the kernel always has.
+template <bool BOOT>
 __global__ void __launch_bounds__(256) gae_segments_kernel(const float* __restrict__ reward, const float* __restrict__ value,
                                                            const uint8_t* __restrict__ done, int T, int n, float discount,
-                                                           float lambda, float* __restrict__ out_ret, float* __restrict__ out_adv) {
+                                                           float lambda, float* __restrict__ out_ret, float* __restrict__ out_adv,
+                                                           const uint8_t* __restrict__ truncated, const float* __restrict__ final_value) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n) return;
     float next_v = value[(size_t)T * n + e], ret = next_v, adv = 0.f;
     for (int t1 = T; t1 > 0; t1 -= SCAN_U) {
-        float r[SCAN_U], v[SCAN_U]; uint8_t d[SCAN_U];
+        float r[SCAN_U], v[SCAN_U]; uint8_t d[SCAN_U], tr[SCAN_U];
 #pragma unroll
         for (int u = 0; u < SCAN_U; u++) {
             const int t = t1 - 1 - u;
             const size_t idx = (size_t)(t >= 0 ? t : 0) * n + e;
             r[u] = reward[idx]; v[u] = value[idx]; d[u] = done[idx];
+            tr[u] = BOOT ? truncated[idx] : 0;
         }
 #pragma unroll
         for (int u = 0; u < SCAN_U; u++) {
             const int t = t1 - 1 - u;
             if (t < 0) break;
             const size_t idx = (size_t)t * n + e;
-            const float nd = d[u] ? 0.f : 1.f;
-            const float delta = r[u] + discount * next_v * nd - v[u];
-            adv = delta + discount * lambda * nd * adv;
-            ret = r[u] + discount * nd * ret;
+            if (BOOT && d[u] && tr[u]) {
+                const float boot = discount * final_value[idx];
+                adv = r[u] + boot - v[u];
+                ret = r[u] + boot;
+            } else {
+                const float nd = d[u] ? 0.f : 1.f;
+                const float delta = r[u] + discount * next_v * nd - v[u];
+                adv = delta + discount * lambda * nd * adv;
+                ret = r[u] + discount * nd * ret;
+            }
             if (out_adv) out_adv[idx] = adv;
             if (out_ret) out_ret[idx] = ret;
             next_v = v[u];
@@ -1018,7 +1031,18 @@ int rexagent_gae_segments(const float* reward, const float* value, const uint8_t
                           float lambda, float* out_return, float* out_advantage, void* stream) {
     if (!reward || !value || !done) return fail(REXSIM_ERR_INVALID, "null argument");
     if (T <= 0 || n <= 0) return fail(REXSIM_ERR_INVALID, "agent: empty scan");
-    gae_segments_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(reward, value, done, T, n, discount, lambda, out_return, out_advantage);
+    gae_segments_kernel<false><<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(reward, value, done, T, n, discount, lambda,
+                                                                                   out_return, out_advantage, nullptr, nullptr);
+    CK(cudaGetLastError());
+    return REXSIM_OK;
+}
+int rexsim_gae_segments_bootstrap(const float* reward, const float* value, const uint8_t* done, const uint8_t* truncated,
+                                    const float* final_value, int32_t T, int32_t n, float discount, float lambda, float* out_return,
+                                    float* out_advantage, void* stream) {
+    if (!reward || !value || !done || !truncated || !final_value) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (T <= 0 || n <= 0) return fail(REXSIM_ERR_INVALID, "agent: empty scan");
+    gae_segments_kernel<true><<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(reward, value, done, T, n, discount, lambda,
+                                                                                  out_return, out_advantage, truncated, final_value);
     CK(cudaGetLastError());
     return REXSIM_OK;
 }

@@ -31,6 +31,7 @@ struct RexSim {
     int32_t* hist = nullptr;
     float* act = nullptr;              // staging for rexsim_step_host
     uint8_t* out = nullptr;            // obs | reward | done (same layout as the host block)
+    uint8_t* fin = nullptr;            // final obs | limit staging for rexsim_step_host_final (allocated on its first call)
     int A = 0;
     bool started = false;              // a reset or step has been enqueued: the frame wrappers can no longer be switched on
     int nsnap = 1;
@@ -205,6 +206,18 @@ int rexsim_step(RexSim* s, const float* actions, float* obs, float* reward, uint
     s->started = true;
     return enqueue(s, launch_step(P, (cudaStream_t)stream), "step launch");
 }
+int rexsim_step_final(RexSim* s, const float* actions, float* obs, float* reward, uint8_t* done, float* final_obs,
+                      uint8_t* limit, void* stream) {
+    if (!s || !actions || !obs || !reward || !done) return fail(REXSIM_ERR_INVALID, "null argument");
+    Params P = s->P;
+    P.actions = actions; P.obs = obs; P.reward = reward; P.done = done; P.final_obs = final_obs; P.limit = limit;
+    s->started = true;
+    return enqueue(s, launch_step(P, (cudaStream_t)stream), "step launch");
+}
+
+// bytes of the block rexsim_step_host_final fills besides h_out: final obs [N][O] f32 | limit [N] u8
+static size_t final_block_bytes(size_t N, size_t O) { return N * O * sizeof(float) + N; }
+int64_t rexsim_host_final_bytes(const RexSim* s) { return s ? (int64_t)final_block_bytes(s->P.N, s->P.out_dim) : 0; }
 
 int64_t rexsim_host_out_bytes(const RexSim* s) { return s ? (int64_t)host_block(s->P.N, s->P.out_dim).bytes : 0; }
 int rexsim_out_dim(const RexSim* s) { return s ? s->P.out_dim : 0; }
@@ -214,18 +227,23 @@ static bool device_can_address(const void* p) {
     if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
     return at.type == cudaMemoryTypeHost && at.devicePointer == p;
 }
-int rexsim_step_host(RexSim* s, const float* h_actions, void* h_out, void* stream) {
-    if (!s || !h_actions || !h_out) return fail(REXSIM_ERR_INVALID, "null argument");
+// rexsim_step_host, and rexsim_step_host_final when h_final is not null
+static int step_host(RexSim* s, const float* h_actions, void* h_out, void* h_final, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     const size_t N = s->P.N;
     const HostBlock hb = host_block(N, s->P.out_dim);
+    const size_t fb = final_block_bytes(N, s->P.out_dim);
     Params P = s->P;
+    // the staging block keeps the rows of envs that did not end from one call to the next, as the caller's block does on
+    // the zero-copy path; its width is fixed once stepping has started (rexsim_set_frames)
+    if (h_final && !s->fin && s->mem.zeroed(&s->fin, fb)) return REXSIM_ERR_CUDA;
     s->started = true;
     // Small batches with pinned buffers: the kernel reads the actions from, and writes its results into, the host block
     // directly (zero-copy over PCIe) -- no DMA launches at all: the error bits travel as flag bytes the kernel sets in the
     // block, the device-side aggregate is cleared BEFORE the kernel.  Large batches stage through device buffers so the kernel
     // never waits on PCIe.
-    const bool zero_copy = N <= 16384 && device_can_address(h_actions) && device_can_address(h_out);   // queried per call (~1 us)
+    const bool zero_copy = N <= 16384 && device_can_address(h_actions) && device_can_address(h_out) &&
+                           (!h_final || device_can_address(h_final));                     // queried per call (~1 us)
     int32_t* h_err = reinterpret_cast<int32_t*>((char*)h_out + hb.err);
     uint8_t* h_flags = reinterpret_cast<uint8_t*>(h_err + 1);
     if (zero_copy) {
@@ -239,9 +257,14 @@ int rexsim_step_host(RexSim* s, const float* h_actions, void* h_out, void* strea
     }
     uint8_t* block = zero_copy ? (uint8_t*)h_out : s->out;
     P.obs = (float*)block; P.reward = (float*)(block + hb.reward); P.done = block + hb.done;
+    if (h_final) {
+        uint8_t* fin = zero_copy ? (uint8_t*)h_final : s->fin;
+        P.final_obs = (float*)fin; P.limit = fin + N * s->P.out_dim * sizeof(float);
+    }
     if (int rc = enqueue(s, launch_step(P, st), "step launch")) return rc;
     if (!zero_copy) {
         CK(cudaMemcpyAsync(h_out, s->out, hb.err, cudaMemcpyDeviceToHost, st));
+        if (h_final) CK(cudaMemcpyAsync(h_final, s->fin, fb, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(h_err, P.err + N, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         CK(cudaMemsetAsync(P.err + N, 0, sizeof(int32_t), st));
     }
@@ -252,6 +275,14 @@ int rexsim_step_host(RexSim* s, const float* h_actions, void* h_out, void* strea
         *h_err = bits;
     }
     return REXSIM_OK;
+}
+int rexsim_step_host(RexSim* s, const float* h_actions, void* h_out, void* stream) {
+    if (!s || !h_actions || !h_out) return fail(REXSIM_ERR_INVALID, "null argument");
+    return step_host(s, h_actions, h_out, nullptr, stream);
+}
+int rexsim_step_host_final(RexSim* s, const float* h_actions, void* h_out, void* h_final, void* stream) {
+    if (!s || !h_actions || !h_out || !h_final) return fail(REXSIM_ERR_INVALID, "null argument");
+    return step_host(s, h_actions, h_out, h_final, stream);
 }
 
 int rexsim_rebalance(RexSim* s, void* stream) {

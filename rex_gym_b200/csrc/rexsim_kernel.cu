@@ -1772,6 +1772,21 @@ __device__ __noinline__ void put_frames(const Frames F, size_t N, int env, int l
     }
 }
 
+// The final observation of an env whose step returned done (Params.final_obs): its obs row as the step wrote it, copied before
+// the auto-reset overwrites it.  Each lane copies only the words it wrote itself (lane 0 the base terms, every lane its gallop
+// angles, in every frame slot), as put_frames writes them, so no lane reads another's.  Out of line: where the switch is off,
+// the epilogue keeps only the branch around this call.
+template <int O>
+__device__ __noinline__ void put_final(float* dst, const float* row, int out_dim, int leg) {
+    for (int k = 0; k < out_dim; k += O) {
+        if (leg == 0) { dst[k] = row[k]; dst[k + 1] = row[k + 1]; dst[k + 2] = row[k + 2]; dst[k + 3] = row[k + 3]; }
+        if (O > 4) {
+#pragma unroll
+            for (int j = 0; j < 3; j++) dst[k + 4 + 3 * leg + j] = row[k + 4 + 3 * leg + j];
+        }
+    }
+}
+
 // _get_observation (+ RangeNormalize) for the env; lane 0 writes the 4 base terms, every lane its 3 angles (gallop).
 // Sensor model on: GetBaseRollPitchYaw / GetBaseRollPitchYawRate / GetMotorAngles = delayed row + noise (rex.py:429-442,548-558,457-468)
 // `first`: the observation a reset returns (step 0); the frame wrappers restart on it.
@@ -1981,14 +1996,21 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
         done = (TASK == REXSIM_TASK_STANDUP) ? fallen : (fallen || (K.flags & FL_ENVGOAL) || (L.pos.y > 0.3f));
     }
     K.env_step += 1;
-    if (c.max_episode_steps > 0 && K.env_step >= c.max_episode_steps) done = true;   // LimitDuration
+    const bool at_limit = c.max_episode_steps > 0 && K.env_step >= c.max_episode_steps;
+    // gym's TimeLimit (time_limit.py): info['TimeLimit.truncated'] = not done, done being the task's own termination, so the
+    // byte is taken before the limit joins it (the non-finite guard below adds bit 1)
+    if (P.limit && valid && leg == 0) P.limit[env] = (uint8_t)((at_limit ? 1 : 0) | (done ? 2 : 0));
+    if (at_limit) done = true;   // LimitDuration
     // ---- non-finite guard (ConvertTo32Bit raises; here: flag + force done) ----------------------------------
     bool finite = isfinite(reward) && isfinite(L.pos.x) && isfinite(L.pos.y) && isfinite(L.pos.z) &&
                   isfinite(L.q[0]) && isfinite(L.q[1]) && isfinite(L.q[2]) && isfinite(L.qd[0]) && isfinite(L.qd[1]) && isfinite(L.qd[2]);
     float* obs_row = P.obs + (size_t)env * P.out_dim;
     if (valid) finite = write_obs<TASK, SENSOR>(P, env, leg, L, obs_row, S, (uint32_t)K.env_step, false) && finite;
     finite = (sum4(finite ? 0.f : 1.f) == 0.f);
-    if (!finite) { L.err |= REXSIM_FLAG_NONFINITE; done = true; }
+    if (!finite) {
+        L.err |= REXSIM_FLAG_NONFINITE; done = true;
+        if (P.limit && valid && leg == 0) P.limit[env] |= 2;
+    }
     int err = (int)or4((unsigned)L.err);
     if (valid && leg == 0) {
         if (P.cost) P.cost[env] = L.cost;
@@ -2017,6 +2039,8 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
             P.ep.score[env] = score; P.ep.length[env] = length;
         }
     }
+    // `done` is final here: the final observation is the row write_obs just wrote
+    if (P.final_obs && done && valid) put_final<obs_dim(TASK, 12)>(P.final_obs + (size_t)env * P.out_dim, obs_row, P.out_dim, leg);
     // ---- auto reset: done envs restart from the settled snapshot; obs = first observation of the new episode --
     if (c.auto_reset && done) {
         reset_from_snapshot<ARM>(P, env, leg, L, K, kp, kd, field, AR, valid, S);

@@ -111,6 +111,12 @@ struct Params {
     float* __restrict__ obs;           // [N][O]
     float* __restrict__ reward;        // [N]
     uint8_t* __restrict__ done;        // [N]
+    // step kernel, both nullable (rexsim_step_final): the observation of every env whose step returned done, before the
+    // auto-reset overwrites its obs row ([N][out_dim]; other rows untouched), and every env's time-limit byte ([N]: bit 0 the
+    // fused max_episode_steps was reached at this step, bit 1 the episode also ended by the task's termination or the
+    // non-finite guard)
+    float* final_obs;
+    uint8_t* limit;
     const int32_t* __restrict__ reset_idx; // reset kernel: [k] or null
     int32_t reset_k;
     int32_t settle_snapshot;           // settle kernel: which snapshot this launch produces

@@ -94,10 +94,13 @@ def frame_space(low, high, past_indices, delta):
 class _Info(object):
     """Stand-in for BatchEnv's `tuple(infos)`: info[i] == {'action': motor command of env i} of THE STEP THAT RETURNED IT
     (rex_gym_env.py:414).  The command block lives on the device and is overwritten by the next step, so the host copy is taken
-    on first access; an access after the batch has stepped again raises instead of handing out the later step's commands."""
+    on first access; an access after the batch has stepped again raises instead of handing out the later step's commands.
+    With final_observation=True, info[i] also carries gym TimeLimit's 'TimeLimit.truncated' on the steps where env i reached
+    max_episode_steps, valued `not done` of the task (gym 0.17.1 wrappers/time_limit.py); its limit byte is copied with the
+    commands."""
 
     def __init__(self, env):
-        self._env, self._cmd, self._at = env, None, env._nsteps
+        self._env, self._cmd, self._limit, self._at = env, None, None, env._nsteps
 
     def __len__(self):
         return len(self._env)
@@ -109,10 +112,16 @@ class _Info(object):
                 raise RuntimeError("info of step %d read after the batch advanced to step %d: call info.materialize() (or read "
                                    "info[i]) before the next step()" % (self._at, self._env._nsteps))
             self._cmd = self._env.last_command().t().contiguous().cpu().numpy()
+            if self._env._final is not None:
+                lim = self._env.limit_bytes()
+                self._limit = lim.cpu().numpy() if isinstance(lim, torch.Tensor) else lim.copy()
         return self
 
     def __getitem__(self, i):
-        return {"action": self.materialize()._cmd[i]}
+        info = {"action": self.materialize()._cmd[i]}
+        if self._limit is not None and self._limit[i] & 1:
+            info["TimeLimit.truncated"] = not bool(self._limit[i] & 2)
+        return info
 
 
 class _EnvView(object):
@@ -145,7 +154,7 @@ class BatchedRexEnv(object):
                  motor_kp_range=None, motor_kd_range=None, num_fields=64, solver_iterations=None, env_offset=0,
                  base_y=None, base_z=None, base_roll=None, base_pitch=None, base_yaw=None, gait_clock_scale=1.0,
                  rebalance_every=8, observation_noise_stdev=SENSOR_NOISE_STDDEV, episode_statistics=False,
-                 frame_history=None, frame_delta=False):
+                 frame_history=None, frame_delta=False, final_observation=False):
         """The reference's task-env keywords, plus the batch's own and the training wrappers fused into the kernels:
         normalize (RangeNormalize + ClipAction), max_episode_steps (LimitDuration), auto_reset, episode_statistics, and
 
@@ -156,7 +165,11 @@ class BatchedRexEnv(object):
           current slot, so [0, 1, 2] returns frames t, t - 1 and t.  Duplicates and any order are allowed.
         frame_delta: FrameDelta (wrappers.py:154-180) inside the history: a step returns obs - last obs in fp32, a reset (and
           so an auto-reset step) the observation itself.
-        Both are off by default; with both off nothing is allocated."""
+        Both are off by default; with both off nothing is allocated.
+        final_observation: every step also keeps, for each env whose step returned done, the observation the step produced
+          before the auto-reset replaced it (final_observation(), [N, O] like the observation rows), and every env's time-limit
+          byte (truncated(), info[i]['TimeLimit.truncated'] as gym's TimeLimit adds it).  Off by default: no extra buffer, and
+          info[i] is {'action': ...}."""
         if urdf_version is not None and urdf_version != DEFAULT_URDF_VERSION:
             raise ValueError("%s is not a supported urdf_version." % urdf_version)     # rex_gym_env.py:317-318
         if task not in TASKS or signal_type not in SIGNALS:
@@ -297,6 +310,16 @@ class BatchedRexEnv(object):
         # hint only -- results are bit-identical with 0 (off).  It pays off once the batch is several waves deep (+17-19 % at
         # 16 384 / 65 536 envs); a batch that fits one wave (4096 envs = 128 CTAs on 132 SMs) is bound by its slowest env anyway
         self._rebalance_every = int(rebalance_every) if self.num_envs >= 8192 else 0
+        # final observation and time-limit byte of the last step: device buffers for the device path, one pinned block
+        # (final obs [N][O] f32 | limit [N] u8, rexsim_host_final_bytes) for the numpy path
+        self._final = self._limit = self._h_final = None
+        self._last_on_device = True
+        if final_observation:
+            self._final = torch.zeros((N, O), dtype=torch.float32, device=dev)
+            self._limit = torch.zeros((N,), dtype=torch.uint8, device=dev)
+            self._h_final = torch.zeros((int(self._L.rexsim_host_final_bytes(self._h)),), dtype=torch.uint8).pin_memory()
+            hf = self._h_final.numpy()
+            self._h_final_obs, self._h_limit = hf[:N * O * 4].view(np.float32).reshape(N, O), hf[N * O * 4:]
         self._nsteps = 0
         self._closed = False
 
@@ -323,8 +346,13 @@ class BatchedRexEnv(object):
                 raise ValueError("Invalid action shape %s, expected %s" % (tuple(action.shape), (N, A)))
             if action.dtype != torch.float32 or not action.is_contiguous():
                 action = action.to(torch.float32).contiguous()
-            self._call(self._L.rexsim_step, self._h, action.data_ptr(), self._obs.data_ptr(), self._reward.data_ptr(),
-                       self._done_u8.data_ptr())
+            if self._final is None:
+                self._call(self._L.rexsim_step, self._h, action.data_ptr(), self._obs.data_ptr(), self._reward.data_ptr(),
+                           self._done_u8.data_ptr())
+            else:
+                self._call(self._L.rexsim_step_final, self._h, action.data_ptr(), self._obs.data_ptr(), self._reward.data_ptr(),
+                           self._done_u8.data_ptr(), self._final.data_ptr(), self._limit.data_ptr())
+            self._last_on_device = True
             self._maybe_rebalance()
             return self._obs, self._reward, self._done, _Info(self)
         a = np.asarray(action, dtype=np.float32)
@@ -333,16 +361,28 @@ class BatchedRexEnv(object):
         if not np.isfinite(a).all():
             raise ValueError("Invalid action: non-finite values")
         np.copyto(self._h_act_np, a)
-        self._call(self._L.rexsim_step_host, self._h, self._h_act_ptr, self._h_out_ptr)
+        if self._final is None:
+            self._call(self._L.rexsim_step_host, self._h, self._h_act_ptr, self._h_out_ptr)
+        else:
+            self._call(self._L.rexsim_step_host_final, self._h, self._h_act_ptr, self._h_out_ptr, self._h_final.data_ptr())
+        self._last_on_device = False
         self._maybe_rebalance()
         if self._h_err[0] & ERR_NONFINITE:        # the aggregate word is per step on this path (rexsim_step_host clears it)
             raise ValueError("Infinite observation encountered.")          # ConvertTo32Bit wrappers.py:522-523,542-543
         return self._h_obs.copy(), self._h_reward.copy(), self._h_done.copy(), _Info(self)
 
-    def step_into(self, action, obs, reward, done_u8):
+    def step_into(self, action, obs, reward, done_u8, final_obs=None, limit=None):
         """Raw device form of step(): CUDA float32 action [N][A] in; obs [N][O], reward [N] (float32) and done [N] (uint8) are
-        written into the caller's contiguous CUDA buffers (e.g. slices of a rollout).  One asynchronous kernel launch."""
-        self._call(self._L.rexsim_step, self._h, action.data_ptr(), obs.data_ptr(), reward.data_ptr(), done_u8.data_ptr())
+        written into the caller's contiguous CUDA buffers (e.g. slices of a rollout).  One asynchronous kernel launch.
+        final_obs [N][O] float32 / limit [N] uint8 (either may be None; any env, whatever its final_observation switch): the
+        rows of the envs that returned done get their final observation, the others are left untouched; every env gets its
+        time-limit byte (bit 0 max_episode_steps reached, bit 1 the episode also ended otherwise; truncated = limit == 1)."""
+        if final_obs is None and limit is None:
+            self._call(self._L.rexsim_step, self._h, action.data_ptr(), obs.data_ptr(), reward.data_ptr(), done_u8.data_ptr())
+        else:
+            ptr = lambda t: None if t is None else t.data_ptr()
+            self._call(self._L.rexsim_step_final, self._h, action.data_ptr(), obs.data_ptr(), reward.data_ptr(), done_u8.data_ptr(),
+                       ptr(final_obs), ptr(limit))
         self._maybe_rebalance()
 
     def _indices(self, indices, what):
@@ -403,6 +443,27 @@ class BatchedRexEnv(object):
         t = torch.from_numpy(np.ascontiguousarray(f)).to(self.device)
         self._call(self._L.rexsim_set_state, self._h, t.data_ptr())
         torch.cuda.current_stream(self.device).synchronize()
+
+    def _final_buffers(self):
+        if self._final is None:
+            raise ValueError("final observations are off: create the env with final_observation=True")
+        return (self._final, self._limit) if self._last_on_device else (self._h_final_obs, self._h_limit)
+
+    def final_observation(self):
+        """[N, O] observations of the last step before the auto-reset replaced them (what `obs` holds with auto_reset=False):
+        valid in the rows where that step returned done; the other rows keep older values.  A CUDA view after a step with a
+        CUDA action, a numpy copy after a numpy step; both are overwritten by the next step."""
+        f = self._final_buffers()[0]
+        return f if self._last_on_device else f.copy()
+
+    def limit_bytes(self):
+        """[N] uint8 time-limit bytes of the last step: bit 0 max_episode_steps was reached, bit 1 the episode also ended by the
+        task's termination or a non-finite observation (CUDA view or numpy view, as final_observation())."""
+        return self._final_buffers()[1]
+
+    def truncated(self):
+        """[N] bool: the last step ended the episode by the time limit alone (gym's info['TimeLimit.truncated'] is True)."""
+        return self.limit_bytes() == 1
 
     def last_command(self):
         """[num_motors, N] motor commands of the last step (info['action'], rex_gym_env.py:414)."""

@@ -13,7 +13,9 @@ except Exception:
 
 
 class SingleRexEnv(_Base):
-    """gym.Env surface: reset() -> obs[O]; step(a[A]) -> (obs[O], reward, done, {'action': cmd[nm]})."""
+    """gym.Env surface: reset() -> obs[O]; step(a[A]) -> (obs[O], reward, done, {'action': cmd[nm]}).  With
+    final_observation=True the info also carries gym TimeLimit's 'TimeLimit.truncated' on the step that reaches
+    max_episode_steps (BatchedRexEnv)."""
     metadata = {"render.modes": ["human", "rgb_array"], "video.frames_per_second": 66}
     _task = "walk"
 
