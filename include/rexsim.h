@@ -155,7 +155,7 @@ int rexsim_action_dim(int32_t task, int32_t signal);
 int rexsim_state_words(const RexSimConfig* cfg, int32_t* n_float, int32_t* n_int);
 
 /* model_tables: HOST pointer to REXSIM_MT_FLOATS (12 motors) or REXSIM_MT_FLOATS_ARM (18 motors) floats.  Allocates device state, computes the settled
- * reset snapshot(s) (600 physics sub-steps, rex.py:314-323) and synchronises.
+ * reset snapshot(s) (600 physics sub-steps, rex.py:314-323; one launch, one snapshot per field) and synchronises.
  * Returns REXSIM_ERR_UNSUPPORTED when floor(1 / sim_dt_d) >= 1023: the overheat protection (rex.py:601-608) switches a motor off
  * once it has been hot for more than floor(1 / sim_dt) sub-steps, and its per-motor counter is a 10-bit field that stops at 1023.
  * Time steps of 1/1023 s and below are refused; every configuration of the reference (1 ms) is accepted. */
@@ -265,6 +265,38 @@ int rexsim_out_dim(const RexSim* sim);
 /* the frame wrappers' device buffers, part of an exact checkpoint together with the state buffers: ring dev [C][obs_dim][N] f32
  * (FrameHistory, NULL and 0 floats when off), last dev [obs_dim][N] f32 (FrameDelta, NULL and 0 floats when off) */
 int rexsim_frame_buffers(RexSim* sim, float** ring, int64_t* ring_floats, float** last, int64_t* last_floats);
+/* Per-env task-constructor values: what BatchEnv([ctor_0, ctor_1, ...]) gives the reference, each env built with its own
+ * keywords (rex_gym/agents/tools/batch_env.py:21-42).  The value block is [REXSIM_VALUE_BLOCK_ROWS][N] f32; row r of env e
+ * means for e exactly what the RexSimConfig field of the same name means for the batch (NaN = draw per reset; backwards -1, 0
+ * or 1; the five pose values follow pose_values' rule env by env).  The last row is the kernels' own: the backwards value the
+ * env's running episode started with (walk's reward flips on it, rex_gym_env.py:506). */
+enum {
+    REXSIM_VALUE_TARGET_POSITION = 0, REXSIM_VALUE_BACKWARDS = 1, REXSIM_VALUE_TARGET_ORIENT = 2, REXSIM_VALUE_INIT_ORIENT = 3,
+    REXSIM_VALUE_POSE = 4,            /* 5 rows: base_y, base_z, base_roll, base_pitch, base_yaw */
+    REXSIM_VALUE_ROWS = 9,            /* rows a caller writes */
+    REXSIM_VALUE_EPISODE_BACKWARDS = 9,
+    REXSIM_VALUE_BLOCK_ROWS = 10,
+    REXSIM_MAX_GAIN_PAIRS = 64        /* distinct (motor_kp, motor_kd) pairs: the settle runs once per pair and field */
+};
+/* row of the value block that the constructor keyword `keyword` fills ("target_position", "backwards", "target_orient",
+ * "init_orient", "base_y", "base_z", "base_roll", "base_pitch", "base_yaw"); -1 for any other name */
+int rexsim_value_row(const char* keyword);
+/* Switch the per-env values on.  values HOST [REXSIM_VALUE_ROWS][N]; kp, kd HOST [N] each, or both NULL (every env takes
+ * RexSimConfig.motor_kp / motor_kd).  Per-env gains are refused with a motor_kp / motor_kd range, when negative or non-finite,
+ * and beyond REXSIM_MAX_GAIN_PAIRS distinct pairs; with them the reset hold is settled again, once per (pair, field), each env
+ * resetting from its own pair's snapshot (Rex.Reset holds at the env's gains, rex.py:314-323).  Accepted only before the
+ * handle's first reset or step and only once (REXSIM_ERR_INVALID otherwise); synchronous.  Off: nothing is allocated and
+ * every launch is what it is without it. */
+int rexsim_set_env_values(RexSim* sim, const float* values, const float* kp, const float* kd);
+/* Scatter new values into rows of the block: idx dev [k] int32 (NULL: every env, k ignored), values dev [REXSIM_VALUE_ROWS][k]
+ * f32 of which only the rows whose bit is set in `rows` are read.  Each env takes them at its next reset, explicit or
+ * automatic.  One launch on `stream`, no host synchronisation; an index outside [0, N) is skipped and sets
+ * REXSIM_FLAG_BAD_INDEX in the aggregate word.  REXSIM_ERR_INVALID when the per-env values are off. */
+int rexsim_set_task_values(RexSim* sim, const int32_t* idx, int32_t k, const float* values, uint32_t rows, void* stream);
+/* the per-env values' device buffers, part of an exact checkpoint together with the state buffers: values dev
+ * [REXSIM_VALUE_BLOCK_ROWS][N] f32, pair dev [N] int32 (each env's gain pair), gains dev [npairs][2] f32 (kp, kd).
+ * REXSIM_ERR_INVALID when the per-env values are off. */
+int rexsim_env_value_buffers(RexSim* sim, float** values, int32_t** pair, float** gains, int32_t* npairs);
 /* kernels launched by this handle since create (the bench reports it) */
 int64_t rexsim_launch_count(const RexSim* sim);
 /* which build of the step kernel the last rexsim_step / rexsim_step_host launched (all 0 before the first step): CTA size,

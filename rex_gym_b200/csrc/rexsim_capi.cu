@@ -8,7 +8,8 @@
 namespace rexsim {
 cudaError_t launch_step(const Params& P, cudaStream_t st);
 cudaError_t launch_reset(const Params& P, float* obs_out, cudaStream_t st);
-cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, cudaStream_t st);
+cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, int npairs, cudaStream_t st);
+cudaError_t launch_set_task_values(const Params& P, const int32_t* idx, int k, const float* values, uint32_t rows, cudaStream_t st);
 cudaError_t launch_get_state(const Params& P, float* out_f, int32_t* out_i, cudaStream_t st);
 cudaError_t launch_set_state(const Params& P, const float* in_f, cudaStream_t st);
 cudaError_t launch_rebalance(const int32_t* cost, int n, int32_t* hist, int32_t* perm, cudaStream_t st);
@@ -34,7 +35,8 @@ struct RexSim {
     uint8_t* fin = nullptr;            // final obs | limit staging for rexsim_step_host_final (allocated on its first call)
     int A = 0;
     bool started = false;              // a reset or step has been enqueued: the frame wrappers can no longer be switched on
-    int nsnap = 1;
+    int nsnap = 1;                     // reset snapshots per gain pair (one per field)
+    int npairs = 0;                    // gain pairs of the per-env values (0: off)
     int64_t launches = 0;
     int32_t launched[3] = {0, 0, 0};   // step_kernel instance of the last step launch: BLOCK, OCC, SENSOR
 };
@@ -128,7 +130,7 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
         CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         P.sm_count = sms;
     }
-    s->nsnap = cfg->terrain == REXSIM_TERRAIN_RANDOM ? cfg->nfields : 1;
+    s->nsnap = snapshots_per_pair(*cfg);
     s->A = rexsim_action_dim(cfg->task, cfg->signal);
     P.out_dim = out_dim(cfg->task, cfg->num_motors, 0);
     // the kernels read these through pointers to const; create fills them
@@ -183,10 +185,7 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
     P.model = model; P.snap_f = snap_f; P.snap_i = snap_i; P.field_zoff = zoff;
     P.launched = s->launched;
     // settled reset snapshots: Rex.Reset's 100 + 0.5/dt holding sub-steps (rex.py:314-323), once per field
-    for (int f = 0; f < s->nsnap; f++) {
-        P.settle_snapshot = f;
-        if ((rc = enqueue(s, launch_settle(P, snap_f, snap_i, 0), "settle launch"))) return rc;
-    }
+    if ((rc = enqueue(s, launch_settle(P, snap_f, snap_i, 1, 0), "settle launch"))) return rc;
     CK(cudaDeviceSynchronize());
     guard.s = nullptr;
     *out = s;
@@ -414,6 +413,95 @@ int rexsim_frame_buffers(RexSim* s, float** ring, int64_t* ring_floats, float** 
     const int64_t on = (int64_t)obs_dim(s->P.cfg.task, s->P.cfg.num_motors) * s->P.N;
     *ring = s->P.fr.ring; *ring_floats = s->P.fr.ring ? (int64_t)s->P.fr.capacity * on : 0;
     *last = s->P.fr.last; *last_floats = s->P.fr.last ? on : 0;
+    return REXSIM_OK;
+}
+static const char* const c_value_keywords[REXSIM_VALUE_ROWS] = {
+    "target_position", "backwards", "target_orient", "init_orient", "base_y", "base_z", "base_roll", "base_pitch", "base_yaw"};
+static_assert(REXSIM_VALUE_POSE == 4 && REXSIM_VALUE_ROWS == REXSIM_VALUE_POSE + 5, "keyword table follows the row enum");
+int rexsim_value_row(const char* keyword) {
+    for (int r = 0; keyword && r < REXSIM_VALUE_ROWS; r++)
+        if (!strcmp(keyword, c_value_keywords[r])) return r;
+    return -1;
+}
+int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const float* kd) {
+    if (!s || !values || !kp != !kd) return fail(REXSIM_ERR_INVALID, "null argument (kp and kd are given together or not at all)");
+    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env values must be set before the first reset or step");
+    if (s->npairs) return fail(REXSIM_ERR_INVALID, "per-env values are already set");
+    Params& P = s->P;
+    const RexSimConfig& c = P.cfg;
+    const size_t N = P.N;
+    for (size_t e = 0; e < N; e++) {
+        const float b = values[REXSIM_VALUE_BACKWARDS * N + e];
+        if (b != -1.f && b != 0.f && b != 1.f) return fail(REXSIM_ERR_INVALID, "backwards values must be -1, 0 or 1");
+    }
+    // the gain pairs in order of first appearance, and each env's index into them
+    std::vector<float> gains;
+    std::vector<int32_t> pair(N, 0);
+    if (kp) {
+        if (c.kp_lo != c.kp_hi || c.kd_lo != c.kd_hi)
+            return fail(REXSIM_ERR_INVALID, "per-env gains cannot be combined with a motor_kp / motor_kd range");
+        for (size_t e = 0; e < N; e++) {
+            if (!(kp[e] >= 0.f) || !(kd[e] >= 0.f) || std::isinf(kp[e]) || std::isinf(kd[e]))
+                return fail(REXSIM_ERR_INVALID, "gains must be finite and non-negative");
+            size_t p = 0;
+            while (p < gains.size() / 2 && !(gains[2 * p] == kp[e] && gains[2 * p + 1] == kd[e])) p++;
+            if (p == gains.size() / 2) {
+                if ((int)p == REXSIM_MAX_GAIN_PAIRS) return fail(REXSIM_ERR_INVALID, "more than 64 distinct (motor_kp, motor_kd) pairs");
+                gains.push_back(kp[e]); gains.push_back(kd[e]);
+            }
+            pair[e] = (int32_t)p;
+        }
+    } else {
+        gains = {c.motor_kp, c.motor_kd};
+    }
+    const int npairs = (int)gains.size() / 2;
+    float* block = nullptr;
+    int32_t* dpair = nullptr;
+    float* dgains = nullptr;
+    if (s->mem.zeroed(&block, (size_t)REXSIM_VALUE_BLOCK_ROWS * N) || s->mem.zeroed(&dpair, N) || s->mem.zeroed(&dgains, gains.size()))
+        return REXSIM_ERR_CUDA;
+    CK(cudaMemcpy(block, values, (size_t)REXSIM_VALUE_ROWS * N * sizeof(float), cudaMemcpyHostToDevice));
+    // the running episodes (none yet) start with the constructor's direction
+    CK(cudaMemcpy(block + (size_t)REXSIM_VALUE_EPISODE_BACKWARDS * N, values + (size_t)REXSIM_VALUE_BACKWARDS * N, N * sizeof(float),
+                  cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(dpair, pair.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(dgains, gains.data(), gains.size() * sizeof(float), cudaMemcpyHostToDevice));
+    P.ev.values = block; P.ev.pair = dpair; P.ev.gains = dgains;
+    s->npairs = npairs;
+    if (kp) {
+        // the reset hold again, once per (pair, field): snapshots and their sensor history rows grow with the pairs
+        float* snap_f = nullptr;
+        int32_t* snap_i = nullptr;
+        const size_t nsettle = (size_t)npairs * s->nsnap;
+        if (s->mem.zeroed(&snap_f, (size_t)NF * nsettle) || s->mem.zeroed(&snap_i, (size_t)NI * nsettle)) return REXSIM_ERR_CUDA;
+        s->mem.drop((void*)P.snap_f); s->mem.drop((void*)P.snap_i);
+        P.snap_f = snap_f; P.snap_i = snap_i;
+        if (P.sensor_on) {
+            const SensorCfg sc = sensor_cfg(&c);
+            s->mem.drop(P.snap_ring);
+            P.snap_ring = nullptr;
+            if (s->mem.zeroed(&P.snap_ring, nsettle * sc.depth * sc.words)) return REXSIM_ERR_CUDA;
+        }
+        if (int rc = enqueue(s, launch_settle(P, snap_f, snap_i, npairs, 0), "settle launch")) return rc;
+        CK(cudaDeviceSynchronize());
+    }
+    return REXSIM_OK;
+}
+int rexsim_set_task_values(RexSim* s, const int32_t* idx, int32_t k, const float* values, uint32_t rows, void* stream) {
+    if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
+    if (!s->npairs) return fail(REXSIM_ERR_INVALID, "per-env values are off (rexsim_set_env_values)");
+    if (rows >> REXSIM_VALUE_ROWS) return fail(REXSIM_ERR_INVALID, "rows names a row past REXSIM_VALUE_ROWS");
+    if (idx && k < 0) return fail(REXSIM_ERR_INVALID, "negative count");
+    if (!idx) k = s->P.N;
+    if (k == 0 || rows == 0) return REXSIM_OK;
+    if (!values) return fail(REXSIM_ERR_INVALID, "null values");
+    return enqueue(s, launch_set_task_values(s->P, idx, k, values, rows, (cudaStream_t)stream), "set_task_values launch");
+}
+int rexsim_env_value_buffers(RexSim* s, float** values, int32_t** pair, float** gains, int32_t* npairs) {
+    if (!s || !values || !pair || !gains || !npairs) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (!s->npairs) return fail(REXSIM_ERR_INVALID, "per-env values are off (rexsim_set_env_values)");
+    *values = s->P.ev.values; *pair = const_cast<int32_t*>(s->P.ev.pair); *gains = const_cast<float*>(s->P.ev.gains);
+    *npairs = s->npairs;
     return REXSIM_OK;
 }
 int64_t rexsim_launch_count(const RexSim* s) { return s ? s->launches : 0; }

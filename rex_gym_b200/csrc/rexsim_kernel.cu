@@ -1659,8 +1659,13 @@ __device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, in
     uint32_t rc = (uint32_t)P.si[I_RESETCNT * (size_t)N + env] + 1u;
     const uint32_t genv = (uint32_t)env + (uint32_t)c.env_offset;   // global env id: draws do not depend on the sharding
     field = (c.terrain == REXSIM_TERRAIN_RANDOM) ? (int)((genv + rc) % (uint32_t)c.nfields) : 0;
-    const float* sf = P.snap_f + (size_t)field * NF;
-    const int32_t* si = P.snap_i + (size_t)field * NI;
+    // the env's own constructor values when the batch has them (rexsim_set_env_values), the config's otherwise
+    const float* ev = P.ev.values ? P.ev.values + env : nullptr;
+    auto value = [&](int row, float scalar) { return ev ? ev[(size_t)row * N] : scalar; };
+    const int pair = ev ? P.ev.pair[env] : 0;
+    const int snap = pair * snapshots_per_pair(c) + field;
+    const float* sf = P.snap_f + (size_t)snap * NF;
+    const int32_t* si = P.snap_i + (size_t)snap * NI;
     load_lane(sf, si, 1, 0, leg, L);
     load_task(sf, si, 1, 0, K);
     if (ARM && leg == 0) load_arm(sf, si, 1, 0, AR);
@@ -1668,18 +1673,22 @@ __device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, in
     K.flags = K.flags & ~((1 << FL_ENABLED_SHIFT) - 1);
     K.G.phi = 0.0; K.G.last_step = 0; K.G.alpha = 0.f;
     K.target = 0.f; K.torient = 0.f; K.iorient = 0.f;
-    kp = (c.kp_lo == c.kp_hi) ? c.motor_kp : (float)rand_uniform(c.seed, genv, rc,4, c.kp_lo, c.kp_hi);
-    kd = (c.kd_lo == c.kd_hi) ? c.motor_kd : (float)rand_uniform(c.seed, genv, rc,5, c.kd_lo, c.kd_hi);
+    kp = (c.kp_lo == c.kp_hi) ? (ev ? P.ev.gains[2 * pair] : c.motor_kp) : (float)rand_uniform(c.seed, genv, rc,4, c.kp_lo, c.kp_hi);
+    kd = (c.kd_lo == c.kd_hi) ? (ev ? P.ev.gains[2 * pair + 1] : c.motor_kd) : (float)rand_uniform(c.seed, genv, rc,5, c.kd_lo, c.kd_hi);
+    const int backwards = ev ? (int)ev[(size_t)REXSIM_VALUE_BACKWARDS * N] : c.backwards;
+    const float target_position = value(REXSIM_VALUE_TARGET_POSITION, c.target_position);
     if (c.task == REXSIM_TASK_WALK) {
-        int bw = (c.backwards < 0) ? (int)(rand_u32(c.seed, genv, rc,0) >> 31) : c.backwards;
+        int bw = (backwards < 0) ? (int)(rand_u32(c.seed, genv, rc,0) >> 31) : backwards;
         if (bw) K.flags |= FL_BACKWARDS;
-        if (isnan(c.target_position)) K.target = (float)rand_uniform(c.seed, genv, rc,1, bw ? -2.0 : 1.0, bw ? -3.0 : 3.0);
-        else K.target = c.target_position;
+        if (isnan(target_position)) K.target = (float)rand_uniform(c.seed, genv, rc,1, bw ? -2.0 : 1.0, bw ? -3.0 : 3.0);
+        else K.target = target_position;
     } else if (c.task == REXSIM_TASK_GALLOP) {
-        K.target = isnan(c.target_position) ? (float)rand_uniform(c.seed, genv, rc,1, 1.0, 3.0) : c.target_position;
+        K.target = isnan(target_position) ? (float)rand_uniform(c.seed, genv, rc,1, 1.0, 3.0) : target_position;
     } else if (c.task == REXSIM_TASK_TURN) {
-        double to = isnan(c.target_orient) ? rand_uniform(c.seed, genv, rc,2, 0.2, 6.0) : (double)c.target_orient;
-        double io = isnan(c.init_orient) ? rand_uniform(c.seed, genv, rc,3, 0.2, 6.0) : (double)c.init_orient;
+        const float target_orient = value(REXSIM_VALUE_TARGET_ORIENT, c.target_orient);
+        const float init_orient = value(REXSIM_VALUE_INIT_ORIENT, c.init_orient);
+        double to = isnan(target_orient) ? rand_uniform(c.seed, genv, rc,2, 0.2, 6.0) : (double)target_orient;
+        double io = isnan(init_orient) ? rand_uniform(c.seed, genv, rc,3, 0.2, 6.0) : (double)init_orient;
         K.torient = (float)to; K.iorient = (float)io;
         double diff = fabs(io - to);
         bool cw = false;
@@ -1689,15 +1698,16 @@ __device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, in
         float hy = (float)(io * 0.5);
         L.qx = 0.f; L.qy = 0.f; L.qz = sinf(hy); L.qw = cosf(hy);
     } else if (c.task == REXSIM_TASK_POSES) {                         // poses_env.py:148-176
+        float pv[5];
         bool any = false;
 #pragma unroll
-        for (int k = 0; k < 5; k++) any = any || !isnan(c.pose_values[k]);
+        for (int k = 0; k < 5; k++) { pv[k] = value(REXSIM_VALUE_POSE + k, c.pose_values[k]); any = any || !isnan(pv[k]); }
         int pose;
         if (any) {                      // fill_next_pose_and_target (a None argument counts as 0.0)
             pose = 4;
 #pragma unroll
-            for (int k = 3; k >= 0; k--) if (!isnan(c.pose_values[k]) && c.pose_values[k] != 0.f) pose = k;
-            float v = c.pose_values[pose];
+            for (int k = 3; k >= 0; k--) if (!isnan(pv[k]) && pv[k] != 0.f) pose = k;
+            float v = pv[pose];
             K.target = isnan(v) ? 0.f : v;
         } else {                        // deque rotation; the constructor's own reset() consumed 'base_y'
             pose = (int)(rc % 5u);
@@ -1712,7 +1722,7 @@ __device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, in
         const int words = S.words, depth = S.depth;
         S.push = si[I_HPUSH]; S.rc = rc;
         if (valid) {
-            const float* src = P.snap_ring + (size_t)field * depth * words;
+            const float* src = P.snap_ring + (size_t)snap * depth * words;
             for (int t = leg; t < depth * words; t += 4) S.ring[(size_t)t * N + env] = src[t];
         }
         __syncwarp(env_mask());
@@ -1723,6 +1733,7 @@ __device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, in
         if (P.sensor_on) P.si[I_HPUSH * (size_t)N + env] = S.push;
         P.sf[F_KP * (size_t)N + env] = kp; P.sf[F_KD * (size_t)N + env] = kd;
         P.sf[F_TORIENT * (size_t)N + env] = K.torient; P.sf[F_IORIENT * (size_t)N + env] = K.iorient;
+        if (ev) P.ev.values[(size_t)REXSIM_VALUE_EPISODE_BACKWARDS * N + env] = (float)backwards;
     }
 }
 
@@ -1935,7 +1946,9 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
         float cx = -L.pos.x;
         // the reference flips on the CONSTRUCTOR argument only (rex_gym_env.py:269,506 `self._backwards`): a direction drawn
         // at reset (walk_env.py:133-136, `self.backwards`) leaves the forward objective unflipped -- restated as is
-        if (c.backwards == 1) cx = -cx;
+        // (per-env values: the one the env's running episode was started with)
+        const int backwards = P.ev.values ? (int)P.ev.values[(size_t)REXSIM_VALUE_EPISODE_BACKWARDS * N + env] : c.backwards;
+        if (backwards == 1) cx = -cx;
         K.target = fabsf(K.target);
         float tp = K.target, fwd;
         if (cx > tp + 0.15f) fwd = tp - cx;
@@ -2085,17 +2098,22 @@ __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_o
 }
 
 // -------------------------------------------------------------------------------------------------
-// settle kernel: Rex.Reset (rex.py:296-324) for one snapshot, 4 lanes: 100 sub-steps holding 'stand'
-// then reset_time/dt holding the task's init pose; writes the snapshot row
+// settle kernel: Rex.Reset (rex.py:296-324) for every snapshot, one per 4-lane group: 100 sub-steps holding 'stand'
+// then reset_time/dt holding the task's init pose; writes the snapshot row.  Snapshot s = pair * fields + field holds at
+// the gains of its pair.
 // -------------------------------------------------------------------------------------------------
 template <int TERRAIN, bool ARM, bool SENSOR>
-__global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_f, int32_t* snap_i, int signal, int task) {
+__global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_f, int32_t* snap_i, int nsettle, int signal, int task) {
     __shared__ __align__(16) float sm[ARM ? REXSIM_MT_FLOATS_ARM : REXSIM_MT_FLOATS];
     __shared__ __align__(8) uint64_t bar;
     __shared__ float tiles[TERRAIN == REXSIM_TERRAIN_RANDOM ? 8 * TILE_FLOATS : 1];
     tma_load_tables(sm, P.model, (ARM ? REXSIM_MT_FLOATS_ARM : REXSIM_MT_FLOATS) * 4, &bar);
     const int leg = threadIdx.x & 3;
-    const int field = P.settle_snapshot;
+    const int snap = (blockIdx.x * blockDim.x + threadIdx.x) >> 2;
+    if (snap >= nsettle) return;      // whole 4-lane groups leave: no shuffle or barrier spans groups after the table load
+    const int nfield = snapshots_per_pair(P.cfg);
+    const int field = snap % nfield, pair = snap / nfield;
+    const float kp = P.ev.gains ? P.ev.gains[2 * pair] : P.cfg.motor_kp, kd = P.ev.gains ? P.ev.gains[2 * pair + 1] : P.cfg.motor_kd;
     Lane L; Task K;
     L.pos = mk(0.f, 0.f, 0.21f); L.qx = 0.f; L.qy = 0.f; L.qz = 0.f; L.qw = 1.f;
     L.vl = mk(0, 0, 0); L.w = mk(0, 0, 0);
@@ -2117,25 +2135,25 @@ __global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_
     else init_pose(signal, leg, ip);
     // RexPosesEnv.reset -> RexGymEnv.reset(initial_motor_angles=None): Rex.Reset skips both holding phases (rex.py:307)
     // sensor history of the reset hold: _observation_history.clear() (rex.py:303), one ReceiveObservation before the hold
-    // (:313), one per sub-step, one after it (:324).  The 8 replicas of the warp write identical rows to the same addresses.
+    // (:313), one per sub-step, one after it (:324).
     Sensor S = make_sensor<ARM>(P, nullptr, 1, 0, 0u);
-    if (SENSOR) S.ring = P.snap_ring + (size_t)field * S.depth * S.words;
+    if (SENSOR) S.ring = P.snap_ring + (size_t)snap * S.depth * S.words;
     const int n1 = (task == REXSIM_TASK_POSES) ? 0 : 100;
     if (SENSOR && n1) sensor_push<ARM>(S, leg, L, AR, true);
-    for (int it = 0; it < n1; it++) apply_action_and_step<TERRAIN, ARM, SENSOR, false>(P, sm, L, leg, stand, P.cfg.motor_kp, P.cfg.motor_kd, G, AR, S, true, nullptr);
+    for (int it = 0; it < n1; it++) apply_action_and_step<TERRAIN, ARM, SENSOR, false>(P, sm, L, leg, stand, kp, kd, G, AR, S, true, nullptr);
     const int n2 = (task == REXSIM_TASK_POSES) ? 0 : (int)(0.5 / P.cfg.sim_dt_d);
-    for (int it = 0; it < n2; it++) apply_action_and_step<TERRAIN, ARM, SENSOR, false>(P, sm, L, leg, ip, P.cfg.motor_kp, P.cfg.motor_kd, G, AR, S, true, nullptr);
+    for (int it = 0; it < n2; it++) apply_action_and_step<TERRAIN, ARM, SENSOR, false>(P, sm, L, leg, ip, kp, kd, G, AR, S, true, nullptr);
     if (SENSOR) sensor_push<ARM>(S, leg, L, AR, true);
     {
-        float* qf = snap_f + (size_t)field * NF; int32_t* qi = snap_i + (size_t)field * NI;
-        // snapshot rows are [NF] / [NI] with N = 1; the 8 replicas computed the same thing, the first one stores
-        store_lane(qf, qi, 1, 0, leg, L, K, threadIdx.x < 4);
-        if (ARM && threadIdx.x == 0) store_arm(qf, qi, 1, 0, AR);
+        float* qf = snap_f + (size_t)snap * NF; int32_t* qi = snap_i + (size_t)snap * NI;
+        // snapshot rows are [NF] / [NI] with N = 1
+        store_lane(qf, qi, 1, 0, leg, L, K, true);
+        if (ARM && leg == 0) store_arm(qf, qi, 1, 0, AR);
         int err = (int)or4((unsigned)L.err);
-        if (threadIdx.x == 0) {
-            qf[F_KP] = P.cfg.motor_kp; qf[F_KD] = P.cfg.motor_kd; qf[F_TORIENT] = 0.f; qf[F_IORIENT] = 0.f;
+        if (leg == 0) {
+            qf[F_KP] = kp; qf[F_KD] = kd; qf[F_TORIENT] = 0.f; qf[F_IORIENT] = 0.f;
             qi[I_RESETCNT] = 0; qi[I_FIELD] = field; qi[I_HPUSH] = S.push;
-            if (err) { P.err[0] |= err; atomicOr(&P.err[P.N], err); }
+            if (err) { atomicOr(&P.err[0], err); atomicOr(&P.err[P.N], err); }
         }
     }
 }
@@ -2326,19 +2344,35 @@ cudaError_t launch_reset(const Params& P, float* obs_out, cudaStream_t st) {
     return cudaGetLastError();
 }
 template <int TERRAIN, bool ARM>
-static void launch_settle_ta(const Params& P, float* snap_f, int32_t* snap_i, cudaStream_t st) {
-    if (P.sensor_on) settle_kernel<TERRAIN, ARM, true><<<1, 32, 0, st>>>(P, snap_f, snap_i, P.cfg.signal, P.cfg.task);
-    else settle_kernel<TERRAIN, ARM, false><<<1, 32, 0, st>>>(P, snap_f, snap_i, P.cfg.signal, P.cfg.task);
+static void launch_settle_ta(const Params& P, float* snap_f, int32_t* snap_i, int nsettle, cudaStream_t st) {
+    const int blocks = (nsettle + 7) / 8;                 // 8 snapshots per 32-thread CTA
+    if (P.sensor_on) settle_kernel<TERRAIN, ARM, true><<<blocks, 32, 0, st>>>(P, snap_f, snap_i, nsettle, P.cfg.signal, P.cfg.task);
+    else settle_kernel<TERRAIN, ARM, false><<<blocks, 32, 0, st>>>(P, snap_f, snap_i, nsettle, P.cfg.signal, P.cfg.task);
 }
-cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, cudaStream_t st) {
+cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, int npairs, cudaStream_t st) {
     const bool arm = P.cfg.num_motors == 18;
+    const int nsettle = npairs * snapshots_per_pair(P.cfg);
     if (P.cfg.terrain == REXSIM_TERRAIN_PLANE) {
-        if (arm) launch_settle_ta<REXSIM_TERRAIN_PLANE, true>(P, snap_f, snap_i, st);
-        else launch_settle_ta<REXSIM_TERRAIN_PLANE, false>(P, snap_f, snap_i, st);
+        if (arm) launch_settle_ta<REXSIM_TERRAIN_PLANE, true>(P, snap_f, snap_i, nsettle, st);
+        else launch_settle_ta<REXSIM_TERRAIN_PLANE, false>(P, snap_f, snap_i, nsettle, st);
     } else {
-        if (arm) launch_settle_ta<REXSIM_TERRAIN_RANDOM, true>(P, snap_f, snap_i, st);
-        else launch_settle_ta<REXSIM_TERRAIN_RANDOM, false>(P, snap_f, snap_i, st);
+        if (arm) launch_settle_ta<REXSIM_TERRAIN_RANDOM, true>(P, snap_f, snap_i, nsettle, st);
+        else launch_settle_ta<REXSIM_TERRAIN_RANDOM, false>(P, snap_f, snap_i, nsettle, st);
     }
+    return cudaGetLastError();
+}
+
+// rexsim_set_task_values: rows `rows` of values [REXSIM_VALUE_ROWS][k] into the block, column j to env idx[j] (or j)
+__global__ void set_task_values_kernel(const Params P, const int32_t* idx, int k, const float* values, uint32_t rows) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= k) return;
+    const int env = idx ? idx[j] : j;
+    if (env < 0 || env >= P.N) { atomicOr(&P.err[P.N], REXSIM_FLAG_BAD_INDEX); return; }
+    for (int r = 0; r < REXSIM_VALUE_ROWS; r++)
+        if ((rows >> r) & 1u) P.ev.values[(size_t)r * P.N + env] = values[(size_t)r * k + j];
+}
+cudaError_t launch_set_task_values(const Params& P, const int32_t* idx, int k, const float* values, uint32_t rows, cudaStream_t st) {
+    set_task_values_kernel<<<(k + 127) / 128, 128, 0, st>>>(P, idx, k, values, rows);
     return cudaGetLastError();
 }
 cudaError_t launch_get_state(const Params& P, float* out_f, int32_t* out_i, cudaStream_t st) {

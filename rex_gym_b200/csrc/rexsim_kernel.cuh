@@ -92,16 +92,29 @@ struct Frames {
     int32_t count;                     // number of past indices
 };
 
+// Per-env task-constructor values (rexsim_set_env_values; every pointer null when off).  The reset reads the env's values and
+// gain pair instead of the config's scalars; the step reads the backwards value its episode started with.
+struct EnvValues {
+    float* values;                     // [REXSIM_VALUE_BLOCK_ROWS][N]
+    const int32_t* pair;               // [N] gain pair of each env: it resets from snapshot pair * fields + field
+    const float* gains;                // [npairs][2] motor_kp, motor_kd
+};
+// reset snapshots per gain pair: one per field of the heightfield bank
+__host__ __device__ __forceinline__ int snapshots_per_pair(const RexSimConfig& c) {
+    return c.terrain == REXSIM_TERRAIN_RANDOM ? c.nfields : 1;
+}
+
 struct Params {
     RexSimConfig cfg;
     EpisodeStats ep;
     Frames fr;
+    EnvValues ev;
     int32_t out_dim;                   // words per env of the observation rows the step and reset kernels write (rexsim_out_dim)
     const float* __restrict__ model;   // REXSIM_MT_FLOATS floats, 16-byte aligned
     float* __restrict__ sf;            // [NF][N]
     int32_t* __restrict__ si;          // [NI][N]
-    const float* __restrict__ snap_f;  // [nsnap][NF] settled reset snapshots
-    const int32_t* __restrict__ snap_i;// [nsnap][NI]
+    const float* __restrict__ snap_f;  // [npairs * fields][NF] settled reset snapshots, pair-major
+    const int32_t* __restrict__ snap_i;// [npairs * fields][NI]
     const float* __restrict__ field_zoff; // [nfields]
     int32_t* __restrict__ err;         // [N] per-env bits of the most recent step, [N] = OR of all since last cleared
     uint8_t* err_host;                 // host-buffer step with zero-copy buffers: 8 flag bytes in the caller's block, byte b = 1 when an
@@ -119,7 +132,6 @@ struct Params {
     uint8_t* limit;
     const int32_t* __restrict__ reset_idx; // reset kernel: [k] or null
     int32_t reset_k;
-    int32_t settle_snapshot;           // settle kernel: which snapshot this launch produces
     int32_t N;
     int32_t sm_count;                  // SMs of the device (kernel variant choice)
     int32_t* launched;                 // host: {BLOCK, OCC, SENSOR} of the step_kernel instance the last step launched (never read on the device)
@@ -129,7 +141,7 @@ struct Params {
     int32_t sensor_on;
     int32_t ring_depth;                // D rows kept per env: max(n_ctl, n_pd) + 2 (100 = the deque's maxlen when a latency reaches it)
     float* ring;                       // [D][HW_WORDS(_ARM)][N]; NOT __restrict__: lanes of an env read what lane 0 wrote
-    float* snap_ring;                  // [nsnap][D][HW_WORDS(_ARM)] history the reset hold leaves behind, per field
+    float* snap_ring;                  // [npairs * fields][D][HW_WORDS(_ARM)] history the reset hold leaves behind, per snapshot
     int32_t n_ctl, n_pd;               // int(latency / dt)
     float a_ctl, a_pd;                 // blend weight (latency - n dt) / dt of the older sample
     float lat_ctl, lat_pd;             // the latencies themselves (only their sign is used on the device)

@@ -91,6 +91,79 @@ def frame_space(low, high, past_indices, delta):
     return low, high
 
 
+# constructor keywords that also take one value per env (BatchEnv over separately built envs, batch_env.py:21-42); the block's
+# row of each is the library's (rexsim_value_row)
+TASK_VALUE_KEYWORDS = ("target_position", "backwards", "target_orient", "init_orient",
+                       "base_y", "base_z", "base_roll", "base_pitch", "base_yaw")
+MAX_GAIN_PAIRS = 64              # REXSIM_MAX_GAIN_PAIRS: the reset hold is settled once per distinct (motor_kp, motor_kd)
+
+
+def is_per_env(value):
+    """A keyword value given per env: a list, tuple, numpy array or tensor with at least one dimension."""
+    if isinstance(value, (np.ndarray, torch.Tensor)):
+        return value.ndim > 0
+    return isinstance(value, (list, tuple))
+
+
+def task_value(name, value):
+    """What the scalar keyword `name` means to the kernels (RexSimConfig): NaN = draw per reset, backwards -1 / 0 / 1."""
+    if name == "target_position":            # `if not self._target_position` (walk_env.py:144, gallop_env.py:150)
+        return float("nan") if not value else float(value)
+    if name == "backwards":
+        return -1 if value is None else int(bool(value))
+    return float("nan") if value is None else float(value)
+
+
+def _entries(name, value, n):
+    """A per-env keyword -> float64 [n] on the host (None entries as NaN), its length checked."""
+    if isinstance(value, torch.Tensor):
+        value = value.detach().cpu().numpy()
+    a = np.asarray([np.nan if v is None else v for v in value] if isinstance(value, (list, tuple)) else value, dtype=np.float64)
+    if a.shape != (n,):
+        raise ValueError("%s: expected one value per env (%d), got shape %s" % (name, n, a.shape))
+    return a
+
+
+def task_value_entries(name, value, n):
+    """Per-env values of keyword `name` -> float32 [n], each entry meaning what the scalar means: NaN (or None) draws per reset
+    (target_position 0 too, as the scalar), backwards entries are -1 (draw), 0 or 1."""
+    a = _entries(name, value, n)
+    if name == "target_position":
+        a = np.where(a == 0, np.nan, a)
+    elif name == "backwards":
+        a = np.where(np.isnan(a), -1.0, a)
+        if not np.isin(a, (-1.0, 0.0, 1.0)).all():
+            raise ValueError("backwards: per-env entries must be -1 (draw), 0 or 1")
+    return a.astype(np.float32)
+
+
+def check_env_values(num_envs, values, motor_kp, motor_kd, motor_kp_range=None, motor_kd_range=None):
+    """The per-env constructor keywords, checked before any CUDA call.
+    values: {keyword of TASK_VALUE_KEYWORDS: scalar or per-env}.  -> (None, None) when every keyword is a scalar; otherwise
+    ({keyword: float32 [num_envs]} for all nine keywords (scalars repeated) or None, (kp, kd) float32 [num_envs] each or None)."""
+    n = int(num_envs)
+    per_env = {k: task_value_entries(k, v, n) for k, v in values.items() if is_per_env(v)}
+    rows = None
+    if per_env:
+        rows = {k: per_env[k] if k in per_env else np.full(n, task_value(k, values.get(k)), np.float32) for k in TASK_VALUE_KEYWORDS}
+    gains = None
+    if is_per_env(motor_kp) or is_per_env(motor_kd):
+        if motor_kp_range is not None or motor_kd_range is not None:
+            raise ValueError("per-env motor_kp / motor_kd cannot be combined with motor_kp_range / motor_kd_range")
+        kp, kd = (_entries(k, v, n) if is_per_env(v) else np.full(n, float(v)) for k, v in (("motor_kp", motor_kp), ("motor_kd", motor_kd)))
+        kp, kd = kp.astype(np.float32), kd.astype(np.float32)
+        if not (np.isfinite(kp).all() and np.isfinite(kd).all() and (kp >= 0).all() and (kd >= 0).all()):
+            raise ValueError("motor_kp / motor_kd: per-env gains must be finite and non-negative")
+        pairs = len(set(zip(kp.tolist(), kd.tolist())))
+        if pairs > MAX_GAIN_PAIRS:
+            raise ValueError("motor_kp / motor_kd: %d distinct (kp, kd) pairs, at most %d (the reset hold is settled once per "
+                             "pair; motor_kp_range / motor_kd_range draw continuous gains)" % (pairs, MAX_GAIN_PAIRS))
+        gains = (np.ascontiguousarray(kp), np.ascontiguousarray(kd))
+    if gains is not None and rows is None:
+        rows = {k: np.full(n, task_value(k, values.get(k)), np.float32) for k in TASK_VALUE_KEYWORDS}
+    return rows, gains
+
+
 class _Info(object):
     """Stand-in for BatchEnv's `tuple(infos)`: info[i] == {'action': motor command of env i} of THE STEP THAT RETURNED IT
     (rex_gym_env.py:414).  The command block lives on the device and is overwritten by the next step, so the host copy is taken
@@ -184,6 +257,12 @@ class BatchedRexEnv(object):
         if env_randomizer:
             raise ValueError("env_randomizer hooks are Python callbacks; use motor_kp_range / motor_kd_range")
         frames = check_frame_history(frame_history)
+        ctor_values = dict(target_position=target_position, backwards=backwards, target_orient=target_orient,
+                           init_orient=init_orient, base_y=base_y, base_z=base_z, base_roll=base_roll, base_pitch=base_pitch,
+                           base_yaw=base_yaw)
+        env_values, env_gains = check_env_values(num_envs, ctor_values, motor_kp, motor_kd, motor_kp_range, motor_kd_range)
+        if env_gains is not None:            # the handle's own gains only settle the snapshot rexsim_set_env_values replaces
+            motor_kp, motor_kd = float(env_gains[0][0]), float(env_gains[1][0])
         if not torch.cuda.is_available():
             raise RuntimeError("rex_gym_b200 needs a CUDA device: there is no CPU fallback")
         self._L = _capi.load()
@@ -207,17 +286,18 @@ class BatchedRexEnv(object):
         c.motor_kp, c.motor_kd = motor_kp, motor_kd
         c.kp_lo, c.kp_hi = motor_kp_range or (motor_kp, motor_kp)
         c.kd_lo, c.kd_hi = motor_kd_range or (motor_kd, motor_kd)
-        # `if not self._target_position` (walk_env.py:144, gallop_env.py:150): None AND 0 mean "draw one per reset"
-        c.target_position = float("nan") if not target_position else target_position
-        c.backwards = -1 if backwards is None else int(bool(backwards))
-        c.target_orient = float("nan") if target_orient is None else target_orient
-        c.init_orient = float("nan") if init_orient is None else init_orient
+        # per-env keywords leave the scalar "draw" in the config: the kernels read the value block instead
+        scalar = {k: (None if is_per_env(v) else v) for k, v in ctor_values.items()}
+        c.target_position = task_value("target_position", scalar["target_position"])
+        c.backwards = task_value("backwards", scalar["backwards"])
+        c.target_orient = task_value("target_orient", scalar["target_orient"])
+        c.init_orient = task_value("init_orient", scalar["init_orient"])
         c.w_distance, c.w_drift, c.w_shake = 1.0, 2.0, 0.005                            # rex_gym_env.py:56-59
         c.w_energy = energy_weight if energy_weight is not None else (0.005 if task == "gallop" else 0.0005)
         c.normalize, c.max_episode_steps, c.auto_reset, c.seed = int(normalize), int(max_episode_steps), int(auto_reset), seed
         c.gait_clock_scale = float(gait_clock_scale)     # GaitPlanner clock / simulation clock (the reference reads the wall clock)
-        for k, v in enumerate((base_y, base_z, base_roll, base_pitch, base_yaw)):      # poses_env.py:49-53 (None = rotate per reset)
-            c.pose_values[k] = float("nan") if v is None else float(v)
+        for k, name in enumerate(("base_y", "base_z", "base_roll", "base_pitch", "base_yaw")):   # poses_env.py:49-53 (None = rotate)
+            c.pose_values[k] = task_value(name, scalar[name])
         # sensor model (rex_gym_env.py:61,70-71 -> Rex(control_latency, pd_latency, observation_noise_stdev), rex.py:726-769)
         c.control_latency, c.pd_latency = float(control_latency), float(pd_latency)
         for k, v in enumerate(observation_noise_stdev):
@@ -252,6 +332,14 @@ class BatchedRexEnv(object):
             fi = np.ascontiguousarray(frames or [0], np.int32)
             self._call(self._L.rexsim_set_frames, self._h, fi.ctypes.data, len(frames), int(bool(frame_delta)), stream=False)
         self.frame_history, self.frame_delta = (list(frames) if frames else None), bool(frame_delta)
+        self._values = None
+        if env_values is not None:
+            block = np.full((len(TASK_VALUE_KEYWORDS), self.num_envs), np.nan, np.float32)
+            for k, v in env_values.items():
+                block[self._L.rexsim_value_row(k.encode())] = v
+            kp, kd = env_gains if env_gains is not None else (None, None)
+            self._call(self._L.rexsim_set_env_values, self._h, block.ctypes.data, None if kp is None else kp.ctypes.data,
+                       None if kd is None else kd.ctypes.data, stream=False)
         self.obs_dim = self._L.rexsim_out_dim(self._h)           # env_obs_dim x len(frame_history)
         self.action_dim = self._L.rexsim_action_dim(c.task, c.signal)
         N, O, A = self.num_envs, self.obs_dim, self.action_dim
@@ -285,6 +373,11 @@ class BatchedRexEnv(object):
         nl = C.c_int64()
         _capi.check(self._L.rexsim_frame_buffers(self._h, C.byref(p), C.byref(nr), C.byref(q), C.byref(nl)))
         self._frames = {k: view(ptr, (n.value,), "<f4") for k, ptr, n in (("frame_history", p, nr), ("frame_delta", q, nl)) if n.value}
+        if env_values is not None:
+            g, npairs = C.c_void_p(), C.c_int32()
+            _capi.check(self._L.rexsim_env_value_buffers(self._h, C.byref(p), C.byref(q), C.byref(g), C.byref(npairs)))
+            self._values = dict(values=view(p, (len(TASK_VALUE_KEYWORDS) + 1, N), "<f4"), pair=view(q, (N,), "<i4"),
+                                gains=view(g, (npairs.value, 2), "<f4"))
         self._episode = None
         if episode_statistics:
             o, sm, blk, nb = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int64()
@@ -494,9 +587,19 @@ class BatchedRexEnv(object):
             sd["episode_statistics"] = self._episode["block"].clone()
         for k, v in self._frames.items():
             sd[k] = v.clone()
+        if self._values is not None:
+            sd.update(("env_" + k, v.clone()) for k, v in self._values.items())
         return sd
 
     def load_state_dict(self, sd):
+        if (self._values is None) != ("env_values" not in sd):
+            raise ValueError("per-env values: the checkpoint %s them, this batch %s" %
+                             (("has", "does not") if self._values is None else ("lacks", "has")))
+        if self._values is not None:
+            for k in ("gains", "pair"):       # the settled snapshots belong to this handle's pairs
+                if not torch.equal(self._values[k], sd["env_" + k].to(self._values[k].device)):
+                    raise ValueError("per-env gains: the checkpoint's gain pairs differ from this batch's")
+            self._values["values"].copy_(sd["env_values"])
         self._state_f.copy_(sd["state_f"])
         self._state_i.copy_(sd["state_i"])
         if self._ring is not None:
@@ -505,6 +608,50 @@ class BatchedRexEnv(object):
             self._episode["block"].copy_(sd["episode_statistics"])
         for k, v in self._frames.items():
             v.copy_(sd[k])
+
+    # ---- per-env task values ------------------------------------------------------------------------------
+    def set_task_values(self, indices=None, **values):
+        """Give the envs `indices` (default: all) new constructor values, e.g. set_task_values([0, 3], target_position=2.5)
+        or a curriculum between Rollout.collect() calls.  Keywords: those of TASK_VALUE_KEYWORDS (the gains are fixed at
+        construction), each a scalar or one value per index, meaning what it means to the constructor.  Each env starts using
+        them at its next reset, explicit or automatic.  Enqueued on the current stream without a host sync; host values are
+        checked here, device tensors are not inspected.  Needs a batch built with per-env values (any of these keywords, or
+        motor_kp / motor_kd, given one value per env)."""
+        if self._values is None:
+            raise ValueError("per-env values are off: build the batch with one value per env for a task keyword")
+        bad = sorted(set(values) - set(TASK_VALUE_KEYWORDS))
+        if bad:
+            raise ValueError("set_task_values takes %s; not %s (the gains are fixed at construction)" % (TASK_VALUE_KEYWORDS, bad))
+        idx = None if indices is None else self._indices(indices, "set_task_values")
+        k = self.num_envs if idx is None else int(idx.numel())
+        if k == 0 or not values:
+            return
+        block = torch.empty((len(TASK_VALUE_KEYWORDS), k), dtype=torch.float32, device=self.device)
+        rows = 0
+        for name, v in values.items():
+            r = self._L.rexsim_value_row(name.encode())
+            rows |= 1 << r
+            if isinstance(v, torch.Tensor) and v.is_cuda:
+                t = v.to(device=self.device, dtype=torch.float32).reshape(-1).expand(k)
+                if name == "target_position":
+                    t = torch.where(t == 0, torch.full_like(t, float("nan")), t)
+                elif name == "backwards":
+                    t = torch.where(torch.isnan(t), torch.full_like(t, -1.0), t)
+                block[r] = t
+            else:
+                a = task_value_entries(name, v, k) if is_per_env(v) else np.full(k, task_value(name, v), np.float32)
+                block[r] = torch.from_numpy(a).to(self.device, non_blocking=False)
+        self._call(self._L.rexsim_set_task_values, self._h, None if idx is None else idx.data_ptr(), k, block.data_ptr(), rows)
+
+    def task_values(self):
+        """{keyword: CUDA view [N]} of every env's constructor values (what its next reset uses), plus 'episode_backwards'
+        (the direction its running episode started with); None when the batch has no per-env values."""
+        if self._values is None:
+            return None
+        v = self._values["values"]
+        out = {k: v[self._L.rexsim_value_row(k.encode())] for k in TASK_VALUE_KEYWORDS}
+        out["episode_backwards"] = v[len(TASK_VALUE_KEYWORDS)]
+        return out
 
     # ---- episode statistics (episode_statistics=True) ------------------------------------------------
     def _episode_buffer(self, name):

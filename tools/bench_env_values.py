@@ -1,0 +1,120 @@
+#!/usr/bin/env python3
+"""What per-env constructor values cost.  Step time: walk-ik at 4096 and 65 536 envs and C5 (standup with the arm), the batch
+built with scalars (off) and with one value per env (on), alternately in one process, medians over rounds.  On: walk cycles
+its envs through targets 1.5 / 2.0 / 2.5 / drawn and directions -1 / 0 / 1 plus three gain pairs; C5 through three gain pairs.
+Same workload as tools/bench_final_observation.py (normalized actions, auto-reset, staggered episodes); CUDA events around
+`steps` device-path steps.  Creation time (host clock around the constructor, which ends in a device synchronise): walk-ik
+at 4096 envs with 1 gain pair through the scalar keywords, and 1, 8 and 64 pairs through per-env gains, on flat ground and
+on the 64-field heightfield.  Prints the card and its power limit from the same run, then one JSON line per row.
+
+Also an "equal values" column: every scalar given as an array of equal entries, the same physics through the value block.
+
+Usage: python tools/bench_env_values.py [--steps 200] [--rounds 3]"""
+import argparse
+import json
+import os
+import sys
+import time
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+from bench import stagger_episodes  # noqa: E402
+from bench_configs import CONFIGS  # noqa: E402
+from bench_final_observation import median, timed  # noqa: E402
+from bench_render import card  # noqa: E402
+
+NAMES = ("C2 ", "C2' ", "C5 ")                # walk-ik 4096, walk-ik 65536, standup arm 16384
+GAINS = [(1.0, 0.02), (1.2, 0.025), (0.8, 0.015)]
+
+
+def same_values(kw):
+    """The config with every scalar given as one equal value per env: the same physics as the scalars, through the block."""
+    n, kw = kw["num_envs"], dict(kw)
+    for k in ("target_position", "backwards"):
+        if k in kw:
+            kw[k] = [kw[k]] * n
+    kw["motor_kp"], kw["motor_kd"] = np.full(n, 1.0, np.float32), np.full(n, 0.02, np.float32)
+    return kw
+
+
+def per_env(kw):
+    """The config with one value per env: targets, directions and gain pairs cycling over the envs."""
+    n, kw = kw["num_envs"], dict(kw)
+    i = np.arange(n)
+    if kw["task"] == "walk":
+        kw["target_position"] = np.array([1.5, 2.0, 2.5, np.nan], np.float32)[i % 4]
+        kw["backwards"] = (i % 3) - 1
+    kw["motor_kp"] = np.array([g[0] for g in GAINS], np.float32)[i % 3]
+    kw["motor_kd"] = np.array([g[1] for g in GAINS], np.float32)[i % 3]
+    return kw
+
+
+def ms_per_step(kw, steps):
+    import rex_gym_b200 as R
+    env = R.BatchedRexEnv(normalize=True, auto_reset=True, max_episode_steps=2000, **kw)
+    env.reset()
+    g = torch.Generator(device="cuda"); g.manual_seed(3)
+    acts = torch.rand((30, env.num_envs, env.action_dim), device="cuda", generator=g) * 2 - 1
+    stagger_episodes(env, acts)
+    for k in range(20):
+        env.step(acts[k % 30])
+    k = [0]
+
+    def step():
+        env.step(acts[k[0] % 30]); k[0] += 1
+    ms = timed(step, steps)
+    env.close()
+    return ms
+
+
+def create_ms(kw):
+    import rex_gym_b200 as R
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    env = R.BatchedRexEnv(**kw)
+    torch.cuda.synchronize()
+    ms = 1e3 * (time.perf_counter() - t0)
+    env.close()
+    return ms
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--rounds", type=int, default=3, help="step rounds; creation rows take the median of 2 x rounds + 1")
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_env_values needs a CUDA device")
+    print("card: name, power limit, max SM clock =", card(), flush=True)
+    for prefix in NAMES:
+        name, kw = next(c for c in CONFIGS if c[0].startswith(prefix))
+        off, same, on = [], [], []
+        for _ in range(a.rounds):
+            off.append(ms_per_step(kw, a.steps))
+            same.append(ms_per_step(same_values(kw), a.steps))
+            on.append(ms_per_step(per_env(kw), a.steps))
+        # same: the feature's own cost (identical physics); on: a mixed batch, whose envs also walk, fall and reset differently
+        print(json.dumps(dict(config=name, envs=kw["num_envs"], steps=a.steps, ms_off=[round(x, 4) for x in off],
+                              ms_same=[round(x, 4) for x in same], ms_on=[round(x, 4) for x in on],
+                              same_cost_pct=round(100 * (median(same) / median(off) - 1), 2),
+                              mixed_cost_pct=round(100 * (median(on) / median(off) - 1), 2))), flush=True)
+    n = 4096
+    base = dict(task="walk", num_envs=n, signal_type="ik", target_position=2.0, backwards=False)
+    create_ms(base)                                          # module load and first-launch costs out of the timed rows
+    for terrain in ("plane", "random"):
+        kw = dict(base, terrain_type=terrain, num_fields=64)
+        rows = {"scalar": []}
+        for _ in range(2 * a.rounds + 1):
+            rows["scalar"].append(create_ms(kw))
+            for pairs in (1, 8, 64):
+                kp = (1.0 + 0.005 * (np.arange(n) % pairs)).astype(np.float32)
+                rows.setdefault(pairs, []).append(create_ms(dict(kw, motor_kp=kp)))
+        print(json.dumps(dict(config="create walk-ik %d envs, %s" % (n, terrain),
+                              **{("ms_%s" % k if k == "scalar" else "ms_%d_pairs" % k): round(median(v), 1) for k, v in rows.items()})),
+              flush=True)
+
+
+if __name__ == "__main__":
+    main()
