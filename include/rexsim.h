@@ -276,7 +276,8 @@ enum {
     REXSIM_VALUE_ROWS = 9,            /* rows a caller writes */
     REXSIM_VALUE_EPISODE_BACKWARDS = 9,
     REXSIM_VALUE_BLOCK_ROWS = 10,
-    REXSIM_MAX_GAIN_PAIRS = 64        /* distinct (motor_kp, motor_kd) pairs: the settle runs once per pair and field */
+    REXSIM_MAX_GAIN_PAIRS = 64        /* distinct hold settings (motor_kp, motor_kd, pd_latency): the settle runs once per
+                                         setting and field */
 };
 /* row of the value block that the constructor keyword `keyword` fills ("target_position", "backwards", "target_orient",
  * "init_orient", "base_y", "base_z", "base_roll", "base_pitch", "base_yaw"); -1 for any other name */
@@ -294,9 +295,26 @@ int rexsim_set_env_values(RexSim* sim, const float* values, const float* kp, con
  * REXSIM_FLAG_BAD_INDEX in the aggregate word.  REXSIM_ERR_INVALID when the per-env values are off. */
 int rexsim_set_task_values(RexSim* sim, const int32_t* idx, int32_t k, const float* values, uint32_t rows, void* stream);
 /* the per-env values' device buffers, part of an exact checkpoint together with the state buffers: values dev
- * [REXSIM_VALUE_BLOCK_ROWS][N] f32, pair dev [N] int32 (each env's gain pair), gains dev [npairs][2] f32 (kp, kd).
+ * [REXSIM_VALUE_BLOCK_ROWS][N] f32, pair dev [N] int32 (each env's gain pair; its hold setting with per-env latencies), gains
+ * dev [npairs][2] f32 (kp, kd of each pair or setting).
  * REXSIM_ERR_INVALID when the per-env values are off. */
 int rexsim_env_value_buffers(RexSim* sim, float** values, int32_t** pair, float** gains, int32_t* npairs);
+/* Per-env sensor latencies: the control_latency and pd_latency keywords of BatchEnv([ctor_0, ctor_1, ...]) (the latencies do
+ * not change the spaces, batch_env.py:36-43).  control_latency, pd_latency HOST [N] seconds each in fp64, as the config's
+ * scalars are, NULL: every env takes the RexSimConfig scalar.  Env e then runs as a batch built with (control_latency[e], pd_latency[e]) as scalars: the PD loop
+ * reads q, qd pd_latency[e] ago, reward, termination, observation and the turn goal check read the row control_latency[e]
+ * ago; an env whose latencies are both 0 in a batch without noise reads the true state, as the scalar build does.  The ring
+ * keeps the batch's deepest history; a non-zero latency switches the sensor model on.  The reset hold reads the PD
+ * observation (rex.py:303-323), so it is settled again once per hold setting (motor_kp, motor_kd, pd_latency) and field,
+ * at most REXSIM_MAX_GAIN_PAIRS settings, each env resetting from its own setting's snapshot; with a motor_kp / motor_kd
+ * range the settings hold at the config's gains.  Refused (REXSIM_ERR_INVALID) for a negative or non-finite latency, more
+ * settings than the cap, after the handle's first reset or step, and on a second call.  Composes with
+ * rexsim_set_env_values in either order; synchronous.  Off: nothing is allocated and every launch is what it is without it. */
+int rexsim_set_env_latencies(RexSim* sim, const double* control_latency, const double* pd_latency);
+/* the per-env latencies' device buffer, part of an exact checkpoint: latency dev [2][N] f64 (row 0 control_latency, row 1
+ * pd_latency), and the rows per env of the history ring.  With per-env values the hold settings are rexsim_env_value_buffers'
+ * pair index and gains table, one row per setting.  REXSIM_ERR_INVALID when the per-env latencies are off. */
+int rexsim_env_latency_buffers(RexSim* sim, double** latency, int32_t* depth);
 /* kernels launched by this handle since create (the bench reports it) */
 int64_t rexsim_launch_count(const RexSim* sim);
 /* which build of the step kernel the last rexsim_step / rexsim_step_host launched (all 0 before the first step): CTA size,

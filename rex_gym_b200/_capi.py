@@ -73,6 +73,8 @@ SIGNATURES = {
     "rexsim_set_env_values": (C.c_int, [_ptr] * 4),
     "rexsim_set_task_values": (C.c_int, [_ptr, _ptr, _i32, _ptr, _u32, _ptr]),
     "rexsim_env_value_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_ptr), _out(_ptr), _out(_i32)]),
+    "rexsim_set_env_latencies": (C.c_int, [_ptr] * 3),
+    "rexsim_env_latency_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_i32)]),
     "rexsim_launch_count": (_i64, [_ptr]),
     "rexsim_last_step_build": (C.c_int, [_ptr] + [_out(_i32)] * 3),
     "rexsim_last_error": (C.c_char_p, []),

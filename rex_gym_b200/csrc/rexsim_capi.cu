@@ -35,8 +35,12 @@ struct RexSim {
     uint8_t* fin = nullptr;            // final obs | limit staging for rexsim_step_host_final (allocated on its first call)
     int A = 0;
     bool started = false;              // a reset or step has been enqueued: the frame wrappers can no longer be switched on
-    int nsnap = 1;                     // reset snapshots per gain pair (one per field)
-    int npairs = 0;                    // gain pairs of the per-env values (0: off)
+    int nsnap = 1;                     // reset snapshots per hold setting (one per field)
+    int nholds = 0;                    // hold settings (motor_kp, motor_kd, pd_latency) of P.ev.gains / P.el.hold (0: no table)
+    bool values_on = false;            // rexsim_set_env_values was called
+    std::vector<float> kp, kd;         // per-env gains given to rexsim_set_env_values (empty: the config's)
+    std::vector<double> pd;            // per-env pd latencies given to rexsim_set_env_latencies (empty: the config's)
+    double* latency = nullptr;         // [2][N] per-env control and pd latencies (rexsim_set_env_latencies; null: off)
     int64_t launches = 0;
     int32_t launched[3] = {0, 0, 0};   // step_kernel instance of the last step launch: BLOCK, OCC, SENSOR
 };
@@ -53,20 +57,28 @@ static HostBlock host_block(size_t N, size_t O) {
     return b;
 }
 
-// the sensor model a config asks for (all zero but `words` when it is off)
-struct SensorCfg { int on, depth, n_ctl, n_pd; float a_ctl, a_pd; int words; };
+// Rex._GetDelayedObservation reads history[n] and history[n + 1], n = int(latency / dt), blended by a = (latency - n dt) / dt,
+// in fp64 as the reference computes them
+static Delay delay_terms(double latency, double dt) {
+    Delay d;
+    d.n = (int)(latency / dt);
+    d.a = (float)((latency - d.n * dt) / dt);
+    d.lat = (float)latency;
+    return d;
+}
+// the sensor model a config asks for (all zero but `words` when it is off).  Per-env latencies run each env through this with
+// the env's latencies in the config, so every env's terms are the scalar construction's.
+struct SensorCfg { int on, depth; Delay ctl, pd; int words; };
 static SensorCfg sensor_cfg(const RexSimConfig* c) {
     SensorCfg sc = {};
     sc.words = c->num_motors == 18 ? HW_WORDS_ARM : HW_WORDS;
     sc.on = c->control_latency > 0 || c->pd_latency > 0;
     for (int k = 0; k < 5; k++) sc.on = sc.on || c->noise_stdev[k] > 0;
     if (!sc.on) return sc;
-    // Rex._GetDelayedObservation reads history[n] and history[n + 1], n = int(latency / dt); once n + 1 reaches the deque's
-    // length (maxlen 100, rex.py:122) it reads the oldest row instead
-    const double dt = c->sim_dt_d;
-    sc.n_ctl = (int)(c->control_latency / dt); sc.n_pd = (int)(c->pd_latency / dt);
-    sc.a_ctl = (float)((c->control_latency - sc.n_ctl * dt) / dt); sc.a_pd = (float)((c->pd_latency - sc.n_pd * dt) / dt);
-    const int n = sc.n_ctl > sc.n_pd ? sc.n_ctl : sc.n_pd;
+    sc.ctl = delay_terms(c->control_latency, c->sim_dt_d);
+    sc.pd = delay_terms(c->pd_latency, c->sim_dt_d);
+    // rows read: n + 1 at most; once n + 1 reaches the deque's length (maxlen 100, rex.py:122) it reads the oldest row instead
+    const int n = sc.ctl.n > sc.pd.n ? sc.ctl.n : sc.pd.n;
     sc.depth = n + 1 >= HIST_MAXLEN ? (int)HIST_MAXLEN : n + 2;
     return sc;
 }
@@ -148,8 +160,7 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
     if (sc.on) {
         P.sensor_on = 1;
         P.ring_depth = sc.depth;
-        P.n_ctl = sc.n_ctl; P.n_pd = sc.n_pd; P.a_ctl = sc.a_ctl; P.a_pd = sc.a_pd;
-        P.lat_ctl = (float)cfg->control_latency; P.lat_pd = (float)cfg->pd_latency;
+        P.ctl = sc.ctl; P.pd = sc.pd;
         for (int k = 0; k < 5; k++) P.noise_sd[k] = (float)cfg->noise_stdev[k];
         if (mem.zeroed(&P.ring, (size_t)sc.depth * sc.words * N) || mem.zeroed(&P.snap_ring, (size_t)s->nsnap * sc.depth * sc.words))
             return REXSIM_ERR_CUDA;
@@ -318,7 +329,7 @@ int rexsim_history_buffer(RexSim* s, float** ring, int64_t* n_floats) {
     if (!s || !ring || !n_floats) return fail(REXSIM_ERR_INVALID, "null argument");
     const SensorCfg sc = sensor_cfg(&s->P.cfg);
     *ring = s->P.ring;
-    *n_floats = (int64_t)sc.depth * sc.words * s->P.N;       // depth 0: the sensor model is off
+    *n_floats = (int64_t)s->P.ring_depth * sc.words * s->P.N;       // depth 0: the sensor model is off
     return REXSIM_OK;
 }
 int rexsim_error_flags(RexSim* s, int32_t** err_flags) {
@@ -423,10 +434,69 @@ int rexsim_value_row(const char* keyword) {
         if (!strcmp(keyword, c_value_keywords[r])) return r;
     return -1;
 }
+// The reset hold's settings: each env's (motor_kp, motor_kd, pd_latency), distinct ones in order of first appearance, and each
+// env's index into them.  Rex.Reset clears the history and holds through ApplyAction (rex.py:303-323), so the settled state
+// depends on the gains and on the PD observation's latency.  kp, kd, pd: per env, or empty for the config's scalar.
+struct HoldTable { std::vector<float> gains; std::vector<double> pd; std::vector<int32_t> index; };
+static int hold_table(const RexSimConfig& c, size_t N, const std::vector<float>& kp, const std::vector<float>& kd,
+                      const std::vector<double>& pd, HoldTable& t) {
+    t.index.assign(N, 0);
+    for (size_t e = 0; e < N; e++) {
+        const float k = kp.empty() ? c.motor_kp : kp[e], d = kd.empty() ? c.motor_kd : kd[e];
+        const double l = pd.empty() ? c.pd_latency : pd[e];
+        size_t h = 0;
+        while (h < t.pd.size() && !(t.gains[2 * h] == k && t.gains[2 * h + 1] == d && t.pd[h] == l)) h++;
+        if (h == t.pd.size()) {
+            if ((int)h == REXSIM_MAX_GAIN_PAIRS)
+                return fail(REXSIM_ERR_INVALID, "more than 64 distinct reset-hold settings (motor_kp, motor_kd, pd_latency)");
+            t.gains.push_back(k); t.gains.push_back(d); t.pd.push_back(l);
+        }
+        t.index[e] = (int32_t)h;
+    }
+    return REXSIM_OK;
+}
+// Install a hold table (P.ev.pair, P.ev.gains and, with per-env latencies, P.el.hold), and with `settle` run the reset hold
+// again: one launch over every (setting, field) snapshot, its sensor history rows at the handle's ring depth.  Synchronous.
+static int apply_holds(RexSim* s, const HoldTable& t, bool settle) {
+    Params& P = s->P;
+    const size_t N = P.N, nh = t.pd.size();
+    int32_t* dpair = nullptr;
+    float* dgains = nullptr;
+    if (s->mem.zeroed(&dpair, N) || s->mem.zeroed(&dgains, t.gains.size())) return REXSIM_ERR_CUDA;
+    CK(cudaMemcpy(dpair, t.index.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(dgains, t.gains.data(), t.gains.size() * sizeof(float), cudaMemcpyHostToDevice));
+    s->mem.drop((void*)P.ev.pair); s->mem.drop((void*)P.ev.gains);
+    P.ev.pair = dpair; P.ev.gains = dgains;
+    if (s->latency) {
+        std::vector<Delay> hold(nh);
+        for (size_t h = 0; h < nh; h++) hold[h] = delay_terms(t.pd[h], P.cfg.sim_dt_d);
+        Delay* dhold = nullptr;
+        if (s->mem.zeroed(&dhold, nh)) return REXSIM_ERR_CUDA;
+        CK(cudaMemcpy(dhold, hold.data(), nh * sizeof(Delay), cudaMemcpyHostToDevice));
+        s->mem.drop((void*)P.el.hold);
+        P.el.hold = dhold;
+    }
+    s->nholds = (int)nh;
+    if (!settle) return REXSIM_OK;
+    float* snap_f = nullptr;
+    int32_t* snap_i = nullptr;
+    const size_t nsettle = nh * s->nsnap;
+    if (s->mem.zeroed(&snap_f, (size_t)NF * nsettle) || s->mem.zeroed(&snap_i, (size_t)NI * nsettle)) return REXSIM_ERR_CUDA;
+    s->mem.drop((void*)P.snap_f); s->mem.drop((void*)P.snap_i);
+    P.snap_f = snap_f; P.snap_i = snap_i;
+    if (P.sensor_on) {
+        s->mem.drop(P.snap_ring);
+        P.snap_ring = nullptr;
+        if (s->mem.zeroed(&P.snap_ring, nsettle * P.ring_depth * sensor_cfg(&P.cfg).words)) return REXSIM_ERR_CUDA;
+    }
+    if (int rc = enqueue(s, launch_settle(P, snap_f, snap_i, (int)nh, 0), "settle launch")) return rc;
+    CK(cudaDeviceSynchronize());
+    return REXSIM_OK;
+}
 int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const float* kd) {
     if (!s || !values || !kp != !kd) return fail(REXSIM_ERR_INVALID, "null argument (kp and kd are given together or not at all)");
     if (s->started) return fail(REXSIM_ERR_INVALID, "per-env values must be set before the first reset or step");
-    if (s->npairs) return fail(REXSIM_ERR_INVALID, "per-env values are already set");
+    if (s->values_on) return fail(REXSIM_ERR_INVALID, "per-env values are already set");
     Params& P = s->P;
     const RexSimConfig& c = P.cfg;
     const size_t N = P.N;
@@ -434,62 +504,84 @@ int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const
         const float b = values[REXSIM_VALUE_BACKWARDS * N + e];
         if (b != -1.f && b != 0.f && b != 1.f) return fail(REXSIM_ERR_INVALID, "backwards values must be -1, 0 or 1");
     }
-    // the gain pairs in order of first appearance, and each env's index into them
-    std::vector<float> gains;
-    std::vector<int32_t> pair(N, 0);
+    HoldTable t;
     if (kp) {
         if (c.kp_lo != c.kp_hi || c.kd_lo != c.kd_hi)
             return fail(REXSIM_ERR_INVALID, "per-env gains cannot be combined with a motor_kp / motor_kd range");
-        for (size_t e = 0; e < N; e++) {
+        for (size_t e = 0; e < N; e++)
             if (!(kp[e] >= 0.f) || !(kd[e] >= 0.f) || std::isinf(kp[e]) || std::isinf(kd[e]))
                 return fail(REXSIM_ERR_INVALID, "gains must be finite and non-negative");
-            size_t p = 0;
-            while (p < gains.size() / 2 && !(gains[2 * p] == kp[e] && gains[2 * p + 1] == kd[e])) p++;
-            if (p == gains.size() / 2) {
-                if ((int)p == REXSIM_MAX_GAIN_PAIRS) return fail(REXSIM_ERR_INVALID, "more than 64 distinct (motor_kp, motor_kd) pairs");
-                gains.push_back(kp[e]); gains.push_back(kd[e]);
-            }
-            pair[e] = (int32_t)p;
-        }
-    } else {
-        gains = {c.motor_kp, c.motor_kd};
+        if (int rc = hold_table(c, N, std::vector<float>(kp, kp + N), std::vector<float>(kd, kd + N), s->pd, t)) return rc;
+    } else if (!P.ev.pair) {
+        if (int rc = hold_table(c, N, s->kp, s->kd, s->pd, t)) return rc;          // the config's one setting
     }
-    const int npairs = (int)gains.size() / 2;
     float* block = nullptr;
-    int32_t* dpair = nullptr;
-    float* dgains = nullptr;
-    if (s->mem.zeroed(&block, (size_t)REXSIM_VALUE_BLOCK_ROWS * N) || s->mem.zeroed(&dpair, N) || s->mem.zeroed(&dgains, gains.size()))
-        return REXSIM_ERR_CUDA;
+    if (s->mem.zeroed(&block, (size_t)REXSIM_VALUE_BLOCK_ROWS * N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(block, values, (size_t)REXSIM_VALUE_ROWS * N * sizeof(float), cudaMemcpyHostToDevice));
     // the running episodes (none yet) start with the constructor's direction
     CK(cudaMemcpy(block + (size_t)REXSIM_VALUE_EPISODE_BACKWARDS * N, values + (size_t)REXSIM_VALUE_BACKWARDS * N, N * sizeof(float),
                   cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(dpair, pair.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(dgains, gains.data(), gains.size() * sizeof(float), cudaMemcpyHostToDevice));
-    P.ev.values = block; P.ev.pair = dpair; P.ev.gains = dgains;
-    s->npairs = npairs;
-    if (kp) {
-        // the reset hold again, once per (pair, field): snapshots and their sensor history rows grow with the pairs
-        float* snap_f = nullptr;
-        int32_t* snap_i = nullptr;
-        const size_t nsettle = (size_t)npairs * s->nsnap;
-        if (s->mem.zeroed(&snap_f, (size_t)NF * nsettle) || s->mem.zeroed(&snap_i, (size_t)NI * nsettle)) return REXSIM_ERR_CUDA;
-        s->mem.drop((void*)P.snap_f); s->mem.drop((void*)P.snap_i);
-        P.snap_f = snap_f; P.snap_i = snap_i;
-        if (P.sensor_on) {
-            const SensorCfg sc = sensor_cfg(&c);
-            s->mem.drop(P.snap_ring);
-            P.snap_ring = nullptr;
-            if (s->mem.zeroed(&P.snap_ring, nsettle * sc.depth * sc.words)) return REXSIM_ERR_CUDA;
-        }
-        if (int rc = enqueue(s, launch_settle(P, snap_f, snap_i, npairs, 0), "settle launch")) return rc;
-        CK(cudaDeviceSynchronize());
+    P.ev.values = block;
+    s->values_on = true;
+    if (kp) { s->kp.assign(kp, kp + N); s->kd.assign(kd, kd + N); }
+    // per-env gains: the reset hold again, once per (setting, field); without them the table (if new) is the config's one
+    // setting, whose snapshot rexsim_create settled
+    return t.index.empty() ? REXSIM_OK : apply_holds(s, t, kp != nullptr);
+}
+int rexsim_set_env_latencies(RexSim* s, const double* control_latency, const double* pd_latency) {
+    if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
+    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env latencies must be set before the first reset or step");
+    if (s->latency) return fail(REXSIM_ERR_INVALID, "per-env latencies are already set");
+    Params& P = s->P;
+    const RexSimConfig& c = P.cfg;
+    const size_t N = P.N;
+    std::vector<double> lat(2 * N);
+    for (size_t e = 0; e < N; e++) {
+        lat[e] = control_latency ? control_latency[e] : c.control_latency;
+        lat[N + e] = pd_latency ? pd_latency[e] : c.pd_latency;
+        if (!(lat[e] >= 0) || !(lat[N + e] >= 0) || std::isinf(lat[e]) || std::isinf(lat[N + e]))
+            return fail(REXSIM_ERR_INVALID, "latencies must be finite and non-negative");
     }
+    // each env's terms as a batch built with its latencies as scalars would have them; the ring keeps the deepest history
+    std::vector<EnvDelay> env(N);
+    int depth = 0, on = 0;
+    for (size_t e = 0; e < N; e++) {
+        RexSimConfig ce = c;
+        ce.control_latency = lat[e]; ce.pd_latency = lat[N + e];
+        const SensorCfg sc = sensor_cfg(&ce);
+        env[e] = EnvDelay{sc.ctl, sc.pd, sc.on, 0};
+        depth = sc.depth > depth ? sc.depth : depth;
+        on = on || sc.on;
+    }
+    HoldTable t;
+    const std::vector<double> pd(lat.begin() + N, lat.end());
+    if (int rc = hold_table(c, N, s->kp, s->kd, pd, t)) return rc;
+    double* dlat = nullptr;
+    EnvDelay* denv = nullptr;
+    if (s->mem.zeroed(&dlat, 2 * N) || s->mem.zeroed(&denv, N)) return REXSIM_ERR_CUDA;
+    CK(cudaMemcpy(dlat, lat.data(), 2 * N * sizeof(double), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(denv, env.data(), N * sizeof(EnvDelay), cudaMemcpyHostToDevice));
+    s->latency = dlat; s->pd = pd;
+    P.el.env = denv;
+    if (on && depth != P.ring_depth) {          // a latency switches the sensor model on, exactly as a scalar one does
+        s->mem.drop(P.ring);
+        P.ring = nullptr;
+        if (s->mem.zeroed(&P.ring, (size_t)depth * sensor_cfg(&c).words * N)) return REXSIM_ERR_CUDA;
+        P.sensor_on = 1;
+        P.ring_depth = depth;
+        for (int k = 0; k < 5; k++) P.noise_sd[k] = (float)c.noise_stdev[k];
+    }
+    return apply_holds(s, t, true);
+}
+int rexsim_env_latency_buffers(RexSim* s, double** latency, int32_t* depth) {
+    if (!s || !latency || !depth) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (!s->latency) return fail(REXSIM_ERR_INVALID, "per-env latencies are off (rexsim_set_env_latencies)");
+    *latency = s->latency; *depth = s->P.ring_depth;
     return REXSIM_OK;
 }
 int rexsim_set_task_values(RexSim* s, const int32_t* idx, int32_t k, const float* values, uint32_t rows, void* stream) {
     if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
-    if (!s->npairs) return fail(REXSIM_ERR_INVALID, "per-env values are off (rexsim_set_env_values)");
+    if (!s->values_on) return fail(REXSIM_ERR_INVALID, "per-env values are off (rexsim_set_env_values)");
     if (rows >> REXSIM_VALUE_ROWS) return fail(REXSIM_ERR_INVALID, "rows names a row past REXSIM_VALUE_ROWS");
     if (idx && k < 0) return fail(REXSIM_ERR_INVALID, "negative count");
     if (!idx) k = s->P.N;
@@ -499,9 +591,9 @@ int rexsim_set_task_values(RexSim* s, const int32_t* idx, int32_t k, const float
 }
 int rexsim_env_value_buffers(RexSim* s, float** values, int32_t** pair, float** gains, int32_t* npairs) {
     if (!s || !values || !pair || !gains || !npairs) return fail(REXSIM_ERR_INVALID, "null argument");
-    if (!s->npairs) return fail(REXSIM_ERR_INVALID, "per-env values are off (rexsim_set_env_values)");
+    if (!s->values_on) return fail(REXSIM_ERR_INVALID, "per-env values are off (rexsim_set_env_values)");
     *values = s->P.ev.values; *pair = const_cast<int32_t*>(s->P.ev.pair); *gains = const_cast<float*>(s->P.ev.gains);
-    *npairs = s->npairs;
+    *npairs = s->nholds;
     return REXSIM_OK;
 }
 int64_t rexsim_launch_count(const RexSim* s) { return s ? s->launches : 0; }

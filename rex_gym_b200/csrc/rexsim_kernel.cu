@@ -95,10 +95,18 @@ __device__ __forceinline__ void euler_to_quat(const float* rpy, float* q) {     
 // since Rex.Reset cleared the deque (I_HPUSH), so history[k] (k = 0 newest) sits in slot (push - 1 - k) mod depth and the
 // deque's length is min(push, 100).  Every lane writes / reads the 9 words of its own leg; lane 0 writes the 7 base words
 // (and the arm's 18), which the other lanes read after a __syncwarp over the env's 4 lanes.
-struct Sensor { float* ring; int N, env, depth, words, push; uint32_t genv, rc; };
+// ctl / pd are the env's control and PD latency terms (the config's, or its own with per-env latencies); `on` is false for an
+// env whose latencies are both 0 in a batch without noise: it pushes no rows and reads the true state, as the build without
+// the sensor model does.
+struct Sensor { float* ring; int N, env, depth, words, push; uint32_t genv, rc; Delay ctl, pd; bool on; };
 template <bool ARM>
 __device__ __forceinline__ Sensor make_sensor(const Params& P, float* ring, int N, int env, uint32_t genv) {   // no rows pushed yet
-    return Sensor{ring, N, env, P.ring_depth, ARM ? HW_WORDS_ARM : HW_WORDS, 0, genv, 0u};
+    Sensor S{ring, N, env, P.ring_depth, ARM ? HW_WORDS_ARM : HW_WORDS, 0, genv, 0u, P.ctl, P.pd, true};
+    if (P.el.env) {
+        const EnvDelay d = P.el.env[env];
+        S.ctl = d.ctl; S.pd = d.pd; S.on = d.sensed != 0;
+    }
+    return S;
 }
 
 template <bool ARM>
@@ -124,15 +132,15 @@ __device__ __forceinline__ void sensor_push(Sensor& S, int leg, const Lane& L, c
     S.push++;
     __syncwarp(env_mask());          // the base words of lane 0 are visible to the env's other lanes from here on
 }
-// Rex._GetDelayedObservation (rex.py:735-753) for one word of the row: n = int(latency / dt), a = (latency - n dt) / dt
-__device__ __forceinline__ float sensor_delayed(const Sensor& S, float latency, int n, float a, int word) {
+// Rex._GetDelayedObservation (rex.py:735-753) for one word of the row, d = S.ctl or S.pd
+__device__ __forceinline__ float sensor_delayed(const Sensor& S, const Delay& d, int word) {
     const int len = min(S.push, (int)HIST_MAXLEN);
     const float* base = S.ring + (size_t)word * S.N + S.env;
     const size_t row = (size_t)S.words * S.N;
     auto at = [&](int k) { return base[(size_t)((S.push - 1 - k) % S.depth) * row]; };
-    if (latency <= 0.f || len == 1) return at(0);
-    if (n + 1 >= len) return at(len - 1);
-    return (1.0f - a) * at(n) + a * at(n + 1);
+    if (d.lat <= 0.f || len == 1) return at(0);
+    if (d.n + 1 >= len) return at(len - 1);
+    return (1.0f - d.a) * at(d.n) + d.a * at(d.n + 1);
 }
 __device__ __forceinline__ float sensor_noise(const Params& P, const Sensor& S, uint32_t step, int group, uint32_t site, uint32_t comp) {
     const float sd = P.noise_sd[group];
@@ -143,7 +151,7 @@ __device__ __forceinline__ float sensor_noise(const Params& P, const Sensor& S, 
 __device__ __forceinline__ void sensed_quat(const Params& P, const Sensor& S, uint32_t step, uint32_t site, float* q4) {
     float d4[4], rpy[3];
 #pragma unroll
-    for (int a = 0; a < 4; a++) d4[a] = sensor_delayed(S, P.lat_ctl, P.n_ctl, P.a_ctl, HW_BASE + a);
+    for (int a = 0; a < 4; a++) d4[a] = sensor_delayed(S, S.ctl, HW_BASE + a);
     quat_to_euler(d4[0], d4[1], d4[2], d4[3], rpy);
 #pragma unroll
     for (int a = 0; a < 3; a++) rpy[a] += sensor_noise(P, S, step, 3, site, a);
@@ -342,8 +350,8 @@ __device__ __forceinline__ float motor_step(const Params& P, const Sensor& S, bo
                                             uint32_t& enabled, int bit, float& tau_obs) {
     float qo = q, qdo = qd;
     if (pd_delayed) {
-        qo = sensor_delayed(S, P.lat_pd, P.n_pd, P.a_pd, wq);
-        qdo = sensor_delayed(S, P.lat_pd, P.n_pd, P.a_pd, wqd);
+        qo = sensor_delayed(S, S.pd, wq);
+        qdo = sensor_delayed(S, S.pd, wqd);
     }
     const float ta = motor_torque(cmd, qo, qdo, qd, kp, kd, tau_obs);
     uint32_t c = (ovh >> shift) & 1023u;
@@ -1291,7 +1299,7 @@ __device__ __forceinline__ void apply_action_and_step(const Params& P, const flo
                                                       Sensor& S, bool valid, float* pgs) {
     float tau[3];
     float tauA[ARM_NJ];
-    const bool pd_delayed = SENSOR && P.lat_pd > 0.f;        // _GetPDObservation (rex.py:755-759): q, qd as they were pd_latency ago
+    const bool pd_delayed = SENSOR && S.pd.lat > 0.f;        // _GetPDObservation (rex.py:755-759): q, qd as they were pd_latency ago
     const uint32_t limit = (uint32_t)(1.0 / P.cfg.sim_dt_d);   // OVERHEAT_SHUTDOWN_TIME / time_step
     if (ARM) {
 #pragma unroll
@@ -1308,7 +1316,7 @@ __device__ __forceinline__ void apply_action_and_step(const Params& P, const flo
         tau[j] = motor_step(P, S, pd_delayed, 9 * leg + j, 9 * leg + 3 + j, cmd[j], L.q[j], L.qd[j], kp, kd, limit, L.ovh, 10 * j,
                             L.enabled, j, L.tau_obs[j]);
     physics_substep<TERRAIN, ARM, REPL>(P, sm, L, leg, tau, G, AR, tauA, pgs);
-    if (SENSOR) sensor_push<ARM>(S, leg, L, AR, valid);         // Rex.ReceiveObservation (rex.py:162,726-733)
+    if (SENSOR && S.on) sensor_push<ARM>(S, leg, L, AR, valid);  // Rex.ReceiveObservation (rex.py:162,726-733)
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1662,7 +1670,7 @@ __device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, in
     // the env's own constructor values when the batch has them (rexsim_set_env_values), the config's otherwise
     const float* ev = P.ev.values ? P.ev.values + env : nullptr;
     auto value = [&](int row, float scalar) { return ev ? ev[(size_t)row * N] : scalar; };
-    const int pair = ev ? P.ev.pair[env] : 0;
+    const int pair = P.ev.pair ? P.ev.pair[env] : 0;         // the env's hold setting (gain pair, with per-env latencies its PD latency)
     const int snap = pair * snapshots_per_pair(c) + field;
     const float* sf = P.snap_f + (size_t)snap * NF;
     const int32_t* si = P.snap_i + (size_t)snap * NI;
@@ -1673,8 +1681,8 @@ __device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, in
     K.flags = K.flags & ~((1 << FL_ENABLED_SHIFT) - 1);
     K.G.phi = 0.0; K.G.last_step = 0; K.G.alpha = 0.f;
     K.target = 0.f; K.torient = 0.f; K.iorient = 0.f;
-    kp = (c.kp_lo == c.kp_hi) ? (ev ? P.ev.gains[2 * pair] : c.motor_kp) : (float)rand_uniform(c.seed, genv, rc,4, c.kp_lo, c.kp_hi);
-    kd = (c.kd_lo == c.kd_hi) ? (ev ? P.ev.gains[2 * pair + 1] : c.motor_kd) : (float)rand_uniform(c.seed, genv, rc,5, c.kd_lo, c.kd_hi);
+    kp = (c.kp_lo == c.kp_hi) ? (P.ev.gains ? P.ev.gains[2 * pair] : c.motor_kp) : (float)rand_uniform(c.seed, genv, rc,4, c.kp_lo, c.kp_hi);
+    kd = (c.kd_lo == c.kd_hi) ? (P.ev.gains ? P.ev.gains[2 * pair + 1] : c.motor_kd) : (float)rand_uniform(c.seed, genv, rc,5, c.kd_lo, c.kd_hi);
     const int backwards = ev ? (int)ev[(size_t)REXSIM_VALUE_BACKWARDS * N] : c.backwards;
     const float target_position = value(REXSIM_VALUE_TARGET_POSITION, c.target_position);
     if (c.task == REXSIM_TASK_WALK) {
@@ -1716,9 +1724,10 @@ __device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, in
         }
         K.flags = (K.flags & ~(7 << FL_POSE_SHIFT)) | (pose << FL_POSE_SHIFT);
     }
-    if (P.sensor_on) {
-        // the history the reset hold left behind only depends on the field, like the settled state: copy the snapshot's rows
-        // (same slots: the push count is copied with them).  Written by the env's own 4 lanes, read after the __syncwarp.
+    if (P.sensor_on && S.on) {
+        // the history the reset hold left behind only depends on the field and hold setting, like the settled state: copy the
+        // snapshot's rows (same slots: the push count is copied with them).  Written by the env's own 4 lanes, read after the
+        // __syncwarp.
         const int words = S.words, depth = S.depth;
         S.push = si[I_HPUSH]; S.rc = rc;
         if (valid) {
@@ -1808,18 +1817,18 @@ __device__ __forceinline__ bool write_obs(const Params& P, int env, int leg, con
     float rpy[3];
     float wx = L.w.x, wy = L.w.y;
     float qa[3] = {L.q[0], L.q[1], L.q[2]};
-    if (SENSOR) {
+    if (SENSOR && S.on) {
         float d4[4];
 #pragma unroll
-        for (int a = 0; a < 4; a++) d4[a] = sensor_delayed(S, P.lat_ctl, P.n_ctl, P.a_ctl, HW_BASE + a);
+        for (int a = 0; a < 4; a++) d4[a] = sensor_delayed(S, S.ctl, HW_BASE + a);
         quat_to_euler(d4[0], d4[1], d4[2], d4[3], rpy);
         rpy[0] += sensor_noise(P, S, step, 3, 0, 0); rpy[1] += sensor_noise(P, S, step, 3, 0, 1);
-        wx = sensor_delayed(S, P.lat_ctl, P.n_ctl, P.a_ctl, HW_BASE + 4) + sensor_noise(P, S, step, 4, 1, 0);
-        wy = sensor_delayed(S, P.lat_ctl, P.n_ctl, P.a_ctl, HW_BASE + 5) + sensor_noise(P, S, step, 4, 1, 1);
+        wx = sensor_delayed(S, S.ctl, HW_BASE + 4) + sensor_noise(P, S, step, 4, 1, 0);
+        wy = sensor_delayed(S, S.ctl, HW_BASE + 5) + sensor_noise(P, S, step, 4, 1, 1);
         if (TASK == REXSIM_TASK_GALLOP) {
 #pragma unroll
             for (int j = 0; j < 3; j++)
-                qa[j] = sensor_delayed(S, P.lat_ctl, P.n_ctl, P.a_ctl, 9 * leg + j) + sensor_noise(P, S, step, 0, 2, 3 * leg + j);
+                qa[j] = sensor_delayed(S, S.ctl, 9 * leg + j) + sensor_noise(P, S, step, 0, 2, 3 * leg + j);
         }
     } else quat_to_euler(L.qx, L.qy, L.qz, L.qw, rpy);
     const float two_pi = 6.283185307179586f;
@@ -1910,7 +1919,7 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
         act[j] = v;
     }
     float cmd[3];
-    if (SENSOR && TASK == REXSIM_TASK_TURN) {
+    if (SENSOR && TASK == REXSIM_TASK_TURN && S.on) {
         float sq[4]; sensed_quat(P, S, (uint32_t)K.env_step, 7, sq);
         task_command<TASK, SIGNAL>(P, K, L, leg, act, cmd, sq);
     } else task_command<TASK, SIGNAL>(P, K, L, leg, act, cmd);
@@ -1957,7 +1966,7 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
         else fwd = cx / tp;
         float drift = -fabsf(L.pos.y);
         float shake, e;
-        if (SENSOR) {
+        if (SENSOR && S.on) {
             // rex.GetBaseOrientation() / GetMotorTorques() . GetMotorVelocities() (rex_gym_env.py:530-537): delayed row + noise
             float sq[4]; sensed_quat(P, S, ctl_step, 3, sq);
             M3 Rs = quat_to_mat(sq[0], sq[1], sq[2], sq[3]);
@@ -1965,15 +1974,15 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
             e = 0.f;
 #pragma unroll
             for (int j = 0; j < 3; j++) {
-                const float to = sensor_delayed(S, P.lat_ctl, P.n_ctl, P.a_ctl, 9 * leg + 6 + j) + sensor_noise(P, S, ctl_step, 2, 4, 3 * leg + j);
-                const float vo = sensor_delayed(S, P.lat_ctl, P.n_ctl, P.a_ctl, 9 * leg + 3 + j) + sensor_noise(P, S, ctl_step, 1, 5, 3 * leg + j);
+                const float to = sensor_delayed(S, S.ctl, 9 * leg + 6 + j) + sensor_noise(P, S, ctl_step, 2, 4, 3 * leg + j);
+                const float vo = sensor_delayed(S, S.ctl, 9 * leg + 3 + j) + sensor_noise(P, S, ctl_step, 1, 5, 3 * leg + j);
                 e = fmaf(to, vo, e);
             }
             if (ARM && leg == 0) {
 #pragma unroll
                 for (int j = 0; j < ARM_NJ; j++) {
-                    const float to = sensor_delayed(S, P.lat_ctl, P.n_ctl, P.a_ctl, HW_ARM + 12 + j) + sensor_noise(P, S, ctl_step, 2, 4, 12 + j);
-                    const float vo = sensor_delayed(S, P.lat_ctl, P.n_ctl, P.a_ctl, HW_ARM + 6 + j) + sensor_noise(P, S, ctl_step, 1, 5, 12 + j);
+                    const float to = sensor_delayed(S, S.ctl, HW_ARM + 12 + j) + sensor_noise(P, S, ctl_step, 2, 4, 12 + j);
+                    const float vo = sensor_delayed(S, S.ctl, HW_ARM + 6 + j) + sensor_noise(P, S, ctl_step, 1, 5, 12 + j);
                     e = fmaf(to, vo, e);
                 }
             }
@@ -1996,7 +2005,7 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
     bool done;
     if (TASK == REXSIM_TASK_WALK || TASK == REXSIM_TASK_TURN) {
         float up = R.c2.z;
-        if (SENSOR) {                                   // is_fallen reads rex.GetBaseOrientation(): delayed + noisy (rex_gym_env.py:485-488)
+        if (SENSOR && S.on) {                           // is_fallen reads rex.GetBaseOrientation(): delayed + noisy (rex_gym_env.py:485-488)
             float sq[4]; sensed_quat(P, S, ctl_step, 6, sq);
             up = quat_to_mat(sq[0], sq[1], sq[2], sq[3]).c2.z;
         }
@@ -2100,7 +2109,7 @@ __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_o
 // -------------------------------------------------------------------------------------------------
 // settle kernel: Rex.Reset (rex.py:296-324) for every snapshot, one per 4-lane group: 100 sub-steps holding 'stand'
 // then reset_time/dt holding the task's init pose; writes the snapshot row.  Snapshot s = pair * fields + field holds at
-// the gains of its pair.
+// the gains of its pair, and with per-env latencies reads the PD observation at its setting's pd_latency.
 // -------------------------------------------------------------------------------------------------
 template <int TERRAIN, bool ARM, bool SENSOR>
 __global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_f, int32_t* snap_i, int nsettle, int signal, int task) {
@@ -2136,7 +2145,9 @@ __global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_
     // RexPosesEnv.reset -> RexGymEnv.reset(initial_motor_angles=None): Rex.Reset skips both holding phases (rex.py:307)
     // sensor history of the reset hold: _observation_history.clear() (rex.py:303), one ReceiveObservation before the hold
     // (:313), one per sub-step, one after it (:324).
-    Sensor S = make_sensor<ARM>(P, nullptr, 1, 0, 0u);
+    // With per-env latencies the hold reads the PD observation at its setting's latency; its rows serve every env of the setting.
+    Sensor S{nullptr, 1, 0, P.ring_depth, ARM ? HW_WORDS_ARM : HW_WORDS, 0, 0u, 0u, P.ctl, P.pd, true};
+    if (SENSOR && P.el.hold) S.pd = P.el.hold[pair];
     if (SENSOR) S.ring = P.snap_ring + (size_t)snap * S.depth * S.words;
     const int n1 = (task == REXSIM_TASK_POSES) ? 0 : 100;
     if (SENSOR && n1) sensor_push<ARM>(S, leg, L, AR, true);

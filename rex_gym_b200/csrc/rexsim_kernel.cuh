@@ -99,6 +99,16 @@ struct EnvValues {
     const int32_t* pair;               // [N] gain pair of each env: it resets from snapshot pair * fields + field
     const float* gains;                // [npairs][2] motor_kp, motor_kd
 };
+// One latency of Rex._GetDelayedObservation (rex.py:735-753): the latency (only its sign is used on the device), n = int(latency
+// / dt) and the blend weight a = (latency - n dt) / dt of the older row, computed on the host in fp64 (delay_terms)
+struct Delay { float lat; int32_t n; float a; };
+// Per-env sensor latencies (rexsim_set_env_latencies; both pointers null when off).  Each env reads its own terms, by env
+// (not by slot: rexsim_rebalance permutes the slots); the settle reads the PD term of its hold setting.
+struct EnvDelay { Delay ctl, pd; int32_t sensed; int32_t pad; };   // sensed: latency or noise; 0 reads the true state
+struct EnvLatencies {
+    const EnvDelay* __restrict__ env;  // [N]
+    const Delay* __restrict__ hold;    // [settings] PD term of each hold setting (EnvValues.pair indexes it)
+};
 // reset snapshots per gain pair: one per field of the heightfield bank
 __host__ __device__ __forceinline__ int snapshots_per_pair(const RexSimConfig& c) {
     return c.terrain == REXSIM_TERRAIN_RANDOM ? c.nfields : 1;
@@ -109,6 +119,7 @@ struct Params {
     EpisodeStats ep;
     Frames fr;
     EnvValues ev;
+    EnvLatencies el;
     int32_t out_dim;                   // words per env of the observation rows the step and reset kernels write (rexsim_out_dim)
     const float* __restrict__ model;   // REXSIM_MT_FLOATS floats, 16-byte aligned
     float* __restrict__ sf;            // [NF][N]
@@ -139,12 +150,10 @@ struct Params {
     int32_t* __restrict__ cost;        // [N] solver iterations of the last control step
     // sensor model (control / PD latency, observation noise: rex.py:735-769); all unused when sensor_on == 0
     int32_t sensor_on;
-    int32_t ring_depth;                // D rows kept per env: max(n_ctl, n_pd) + 2 (100 = the deque's maxlen when a latency reaches it)
+    int32_t ring_depth;                // D rows kept per env: the batch's largest n + 2 (100 = the deque's maxlen when a latency reaches it)
     float* ring;                       // [D][HW_WORDS(_ARM)][N]; NOT __restrict__: lanes of an env read what lane 0 wrote
     float* snap_ring;                  // [npairs * fields][D][HW_WORDS(_ARM)] history the reset hold leaves behind, per snapshot
-    int32_t n_ctl, n_pd;               // int(latency / dt)
-    float a_ctl, a_pd;                 // blend weight (latency - n dt) / dt of the older sample
-    float lat_ctl, lat_pd;             // the latencies themselves (only their sign is used on the device)
+    Delay ctl, pd;                     // the config's control and PD latency (per env: EnvLatencies)
     float noise_sd[5];                 // SENSOR_NOISE_STDDEV order: motor angle, motor velocity, motor torque, base rpy, base rpy rate
 };
 

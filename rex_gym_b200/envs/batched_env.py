@@ -95,7 +95,8 @@ def frame_space(low, high, past_indices, delta):
 # row of each is the library's (rexsim_value_row)
 TASK_VALUE_KEYWORDS = ("target_position", "backwards", "target_orient", "init_orient",
                        "base_y", "base_z", "base_roll", "base_pitch", "base_yaw")
-MAX_GAIN_PAIRS = 64              # REXSIM_MAX_GAIN_PAIRS: the reset hold is settled once per distinct (motor_kp, motor_kd)
+MAX_GAIN_PAIRS = 64              # REXSIM_MAX_GAIN_PAIRS: the reset hold is settled once per distinct (motor_kp, motor_kd, pd_latency)
+LATENCY_KEYWORDS = ("control_latency", "pd_latency")     # sensor latencies that also take one value per env
 
 
 def is_per_env(value):
@@ -162,6 +163,27 @@ def check_env_values(num_envs, values, motor_kp, motor_kd, motor_kp_range=None, 
     if gains is not None and rows is None:
         rows = {k: np.full(n, task_value(k, values.get(k)), np.float32) for k in TASK_VALUE_KEYWORDS}
     return rows, gains
+
+
+def check_env_latencies(num_envs, control_latency, pd_latency, motor_kp=1.0, motor_kd=0.02, gains=None):
+    """The per-env latency keywords, checked before any CUDA call.  gains: check_env_values' per-env (kp, kd) or None.
+    -> None when both latencies are scalars; otherwise (control, pd) float64 [num_envs] each (a scalar repeated), the values
+    rexsim_set_env_latencies takes (fp64, as the config's scalars: every env's terms are the scalar construction's)."""
+    n = int(num_envs)
+    if not (is_per_env(control_latency) or is_per_env(pd_latency)):
+        return None
+    lat = []
+    for name, v in (("control_latency", control_latency), ("pd_latency", pd_latency)):
+        a = _entries(name, v, n) if is_per_env(v) else np.full(n, float(v))
+        if not (np.isfinite(a).all() and (a >= 0).all()):
+            raise ValueError("%s: per-env latencies must be finite and non-negative" % name)
+        lat.append(np.ascontiguousarray(a, np.float64))
+    kp, kd = gains if gains is not None else (np.full(n, motor_kp, np.float32), np.full(n, motor_kd, np.float32))
+    settings = len(set(zip(kp.tolist(), kd.tolist(), lat[1].tolist())))
+    if settings > MAX_GAIN_PAIRS:
+        raise ValueError("pd_latency: %d distinct reset-hold settings (motor_kp, motor_kd, pd_latency), at most %d (the reset "
+                         "hold reads the PD observation and is settled once per setting)" % (settings, MAX_GAIN_PAIRS))
+    return tuple(lat)
 
 
 class _Info(object):
@@ -252,7 +274,8 @@ class BatchedRexEnv(object):
                              "pybullet_data pip package)" % terrain_type)
         if render or on_rack:
             raise ValueError("render / on_rack are GUI debugging modes of the reference; not part of the batched path")
-        if control_latency < 0 or pd_latency < 0 or len(observation_noise_stdev) != 5 or min(observation_noise_stdev) < 0:
+        scalar_lat = [0.0 if is_per_env(v) else v for v in (control_latency, pd_latency)]
+        if min(scalar_lat) < 0 or len(observation_noise_stdev) != 5 or min(observation_noise_stdev) < 0:
             raise ValueError("control_latency / pd_latency must be >= 0 and observation_noise_stdev five values >= 0")
         if env_randomizer:
             raise ValueError("env_randomizer hooks are Python callbacks; use motor_kp_range / motor_kd_range")
@@ -263,6 +286,8 @@ class BatchedRexEnv(object):
         env_values, env_gains = check_env_values(num_envs, ctor_values, motor_kp, motor_kd, motor_kp_range, motor_kd_range)
         if env_gains is not None:            # the handle's own gains only settle the snapshot rexsim_set_env_values replaces
             motor_kp, motor_kd = float(env_gains[0][0]), float(env_gains[1][0])
+        # per-env latencies: the scalar gains of a motor_kp / motor_kd range hold the reset at each distinct pd_latency
+        env_latency = check_env_latencies(num_envs, control_latency, pd_latency, motor_kp, motor_kd, env_gains)
         if not torch.cuda.is_available():
             raise RuntimeError("rex_gym_b200 needs a CUDA device: there is no CPU fallback")
         self._L = _capi.load()
@@ -299,7 +324,8 @@ class BatchedRexEnv(object):
         for k, name in enumerate(("base_y", "base_z", "base_roll", "base_pitch", "base_yaw")):   # poses_env.py:49-53 (None = rotate)
             c.pose_values[k] = task_value(name, scalar[name])
         # sensor model (rex_gym_env.py:61,70-71 -> Rex(control_latency, pd_latency, observation_noise_stdev), rex.py:726-769)
-        c.control_latency, c.pd_latency = float(control_latency), float(pd_latency)
+        # (per-env latencies leave 0 in the config: rexsim_set_env_latencies gives every env its own)
+        c.control_latency, c.pd_latency = (float(v) for v in scalar_lat)
         for k, v in enumerate(observation_noise_stdev):
             c.noise_stdev[k] = float(v)
         c.episode_stats = int(bool(episode_statistics))       # simulate()'s score / length bookkeeping on the device
@@ -340,6 +366,9 @@ class BatchedRexEnv(object):
             kp, kd = env_gains if env_gains is not None else (None, None)
             self._call(self._L.rexsim_set_env_values, self._h, block.ctypes.data, None if kp is None else kp.ctypes.data,
                        None if kd is None else kd.ctypes.data, stream=False)
+        if env_latency is not None:
+            self._call(self._L.rexsim_set_env_latencies, self._h, env_latency[0].ctypes.data, env_latency[1].ctypes.data,
+                       stream=False)
         self.obs_dim = self._L.rexsim_out_dim(self._h)           # env_obs_dim x len(frame_history)
         self.action_dim = self._L.rexsim_action_dim(c.task, c.signal)
         N, O, A = self.num_envs, self.obs_dim, self.action_dim
@@ -378,6 +407,11 @@ class BatchedRexEnv(object):
             _capi.check(self._L.rexsim_env_value_buffers(self._h, C.byref(p), C.byref(q), C.byref(g), C.byref(npairs)))
             self._values = dict(values=view(p, (len(TASK_VALUE_KEYWORDS) + 1, N), "<f4"), pair=view(q, (N,), "<i4"),
                                 gains=view(g, (npairs.value, 2), "<f4"))
+        self._latency = None                 # [2][N] f64: each env's control_latency, pd_latency (per-env latencies only)
+        if env_latency is not None:
+            depth = C.c_int32()
+            _capi.check(self._L.rexsim_env_latency_buffers(self._h, C.byref(p), C.byref(depth)))
+            self._latency = view(p, (2, N), "<f8")
         self._episode = None
         if episode_statistics:
             o, sm, blk, nb = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int64()
@@ -589,9 +623,16 @@ class BatchedRexEnv(object):
             sd[k] = v.clone()
         if self._values is not None:
             sd.update(("env_" + k, v.clone()) for k, v in self._values.items())
+        if self._latency is not None:
+            sd["env_latency"] = self._latency.clone()
         return sd
 
     def load_state_dict(self, sd):
+        if (self._latency is None) != ("env_latency" not in sd):
+            raise ValueError("per-env latencies: the checkpoint %s them, this batch %s" %
+                             (("has", "does not") if self._latency is None else ("lacks", "has")))
+        if self._latency is not None and not torch.equal(self._latency, sd["env_latency"].to(self._latency.device)):
+            raise ValueError("per-env latencies: the checkpoint's latencies differ from this batch's")
         if (self._values is None) != ("env_values" not in sd):
             raise ValueError("per-env values: the checkpoint %s them, this batch %s" %
                              (("has", "does not") if self._values is None else ("lacks", "has")))
@@ -612,16 +653,17 @@ class BatchedRexEnv(object):
     # ---- per-env task values ------------------------------------------------------------------------------
     def set_task_values(self, indices=None, **values):
         """Give the envs `indices` (default: all) new constructor values, e.g. set_task_values([0, 3], target_position=2.5)
-        or a curriculum between Rollout.collect() calls.  Keywords: those of TASK_VALUE_KEYWORDS (the gains are fixed at
-        construction), each a scalar or one value per index, meaning what it means to the constructor.  Each env starts using
+        or a curriculum between Rollout.collect() calls.  Keywords: those of TASK_VALUE_KEYWORDS (the gains and latencies are
+        fixed at construction), each a scalar or one value per index, meaning what it means to the constructor.  Each env starts using
         them at its next reset, explicit or automatic.  Enqueued on the current stream without a host sync; host values are
         checked here, device tensors are not inspected.  Needs a batch built with per-env values (any of these keywords, or
         motor_kp / motor_kd, given one value per env)."""
-        if self._values is None:
-            raise ValueError("per-env values are off: build the batch with one value per env for a task keyword")
         bad = sorted(set(values) - set(TASK_VALUE_KEYWORDS))
         if bad:
-            raise ValueError("set_task_values takes %s; not %s (the gains are fixed at construction)" % (TASK_VALUE_KEYWORDS, bad))
+            raise ValueError("set_task_values takes %s; not %s (the gains and latencies are fixed at construction)" %
+                             (TASK_VALUE_KEYWORDS, bad))
+        if self._values is None:
+            raise ValueError("per-env values are off: build the batch with one value per env for a task keyword")
         idx = None if indices is None else self._indices(indices, "set_task_values")
         k = self.num_envs if idx is None else int(idx.numel())
         if k == 0 or not values:

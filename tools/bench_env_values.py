@@ -9,7 +9,11 @@ on the 64-field heightfield.  Prints the card and its power limit from the same 
 
 Also an "equal values" column: every scalar given as an array of equal entries, the same physics through the value block.
 
-Usage: python tools/bench_env_values.py [--steps 200] [--rounds 3]"""
+Latencies (--workload latencies): walk-ik at 16 384 and 65 536 envs with control_latency 20 ms and pd_latency 1 ms as scalars
+against a mixed batch cycling its envs through control latencies 0 / 10.5 / 20 ms and pd latencies 0 / 0.5 / 1 ms (the same
+deepest history row), alternately in one process.
+
+Usage: python tools/bench_env_values.py [--steps 200] [--rounds 3] [--workload all|values|latencies]"""
 import argparse
 import json
 import os
@@ -51,6 +55,12 @@ def per_env(kw):
     return kw
 
 
+def mixed_latencies(kw):
+    """The config with each env's (control_latency, pd_latency) one of nine, the deepest the scalar row's."""
+    i = np.arange(kw["num_envs"])
+    return dict(kw, control_latency=np.array([0.0, 0.0105, 0.02])[i % 3], pd_latency=np.array([0.0, 0.0005, 0.001])[(i // 3) % 3])
+
+
 def ms_per_step(kw, steps):
     import rex_gym_b200 as R
     env = R.BatchedRexEnv(normalize=True, auto_reset=True, max_episode_steps=2000, **kw)
@@ -84,10 +94,24 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=3, help="step rounds; creation rows take the median of 2 x rounds + 1")
+    ap.add_argument("--workload", choices=("all", "values", "latencies"), default="all")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_env_values needs a CUDA device")
     print("card: name, power limit, max SM clock =", card(), flush=True)
+    if a.workload in ("all", "latencies"):
+        name, c2 = next(c for c in CONFIGS if c[0].startswith("C2 "))
+        for n in (16384, 65536):
+            kw = dict(c2, num_envs=n, control_latency=0.02, pd_latency=0.001)
+            scalar, mixed = [], []
+            for _ in range(a.rounds):
+                scalar.append(ms_per_step(kw, a.steps))
+                mixed.append(ms_per_step(mixed_latencies(kw), a.steps))
+            print(json.dumps(dict(config="walk-ik latencies", envs=n, steps=a.steps, ms_scalar=[round(x, 4) for x in scalar],
+                                  ms_mixed=[round(x, 4) for x in mixed],
+                                  mixed_cost_pct=round(100 * (median(mixed) / median(scalar) - 1), 2))), flush=True)
+    if a.workload == "latencies":
+        return
     for prefix in NAMES:
         name, kw = next(c for c in CONFIGS if c[0].startswith(prefix))
         off, same, on = [], [], []
