@@ -315,11 +315,34 @@ int rexsim_set_env_latencies(RexSim* sim, const double* control_latency, const d
  * pd_latency), and the rows per env of the history ring.  With per-env values the hold settings are rexsim_env_value_buffers'
  * pair index and gains table, one row per setting.  REXSIM_ERR_INVALID when the per-env latencies are off. */
 int rexsim_env_latency_buffers(RexSim* sim, double** latency, int32_t* depth);
-/* kernels launched by this handle since create (the bench reports it) */
+/* Per-env terrains: the terrain_type keyword of BatchEnv([ctor_0, ctor_1, ...]) (the terrain does not change the spaces,
+ * batch_env.py:36-43), so that one batch holds envs on the plane and envs on the heightfield.  terrain HOST [N] int32, each
+ * REXSIM_TERRAIN_PLANE or REXSIM_TERRAIN_RANDOM.  The handle must have been created with terrain RANDOM (the heightfield bank
+ * and the heightfield's friction); plane_friction is the friction of the plane envs.  Env e then runs exactly as env e of a
+ * batch created with terrain[e] as its terrain and that terrain's friction: a heightfield env resets on field
+ * (global env + reset count) mod nfields of the one bank, a plane env on the plane with field word 0.
+ * Each step launches the step kernel's build for each terrain that has envs, over that terrain's slots (plane envs in slots
+ * [0, nplane), heightfield envs after them; rexsim_rebalance keeps the partition), each launch choosing its build from its
+ * own size; both launches are on the stream.  The reset hold is settled once per hold setting on the plane and once per
+ * setting and field on the heightfield, each terrain's snapshots by one launch of its own build at its own friction.
+ * Refused (REXSIM_ERR_INVALID) for an entry that is neither terrain, a negative or non-finite friction, a handle created on
+ * the plane, after the handle's first reset or step, and on a second call.  Composes with rexsim_set_env_values and
+ * rexsim_set_env_latencies in any order; synchronous.  Off: nothing is allocated and every launch is what it is without it. */
+int rexsim_set_env_terrains(RexSim* sim, const int32_t* terrain, float plane_friction);
+/* the per-env terrains' device buffer, part of a checkpoint's identity: terrain dev [N] u8 (REXSIM_TERRAIN_* of each env),
+ * and the number of envs on the plane.  REXSIM_ERR_INVALID when the per-env terrains are off. */
+int rexsim_env_terrain_buffers(RexSim* sim, uint8_t** terrain, int32_t* nplane);
+/* kernels launched by this handle since create (the bench reports it); a step of a batch with envs on both terrains counts
+ * two launches */
 int64_t rexsim_launch_count(const RexSim* sim);
 /* which build of the step kernel the last rexsim_step / rexsim_step_host launched (all 0 before the first step): CTA size,
- * resident CTAs per SM it is compiled for (1: 255 registers, 4: 128 registers), 1 if the sensor model is compiled in */
+ * resident CTAs per SM it is compiled for (1: 255 registers, 4: 128 registers), 1 if the sensor model is compiled in.
+ * With per-env terrains: the build of that step's last launch, the heightfield envs' when it has any (the plane envs' are
+ * rexsim_last_terrain_build's) */
 int rexsim_last_step_build(const RexSim* sim, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor);
+/* the same for the last launch over the envs on `terrain`: with per-env terrains that terrain's launch; otherwise the
+ * batch's launch for its own terrain, all 0 for the other */
+int rexsim_last_terrain_build(const RexSim* sim, int32_t terrain, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor);
 /* the counter-based generator behind every reset draw (replaces Python's unseeded `random`,
  * walk_env.py:133-147, gallop_env.py:151, turn_env.py:138,147); host-callable so tests can pin it */
 uint32_t rexsim_rand_u32(uint64_t seed, uint32_t global_env, uint32_t reset_count, uint32_t slot);

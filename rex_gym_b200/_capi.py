@@ -75,8 +75,11 @@ SIGNATURES = {
     "rexsim_env_value_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_ptr), _out(_ptr), _out(_i32)]),
     "rexsim_set_env_latencies": (C.c_int, [_ptr] * 3),
     "rexsim_env_latency_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_i32)]),
+    "rexsim_set_env_terrains": (C.c_int, [_ptr, _ptr, _f32]),
+    "rexsim_env_terrain_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_i32)]),
     "rexsim_launch_count": (_i64, [_ptr]),
     "rexsim_last_step_build": (C.c_int, [_ptr] + [_out(_i32)] * 3),
+    "rexsim_last_terrain_build": (C.c_int, [_ptr, _i32] + [_out(_i32)] * 3),
     "rexsim_last_error": (C.c_char_p, []),
     "rexsim_rand_u32": (_u32, [_u64, _u32, _u32, _u32]),
     "rexsim_noise": (_f32, [_u64] + [_u32] * 5),

@@ -12,7 +12,7 @@ cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, int n
 cudaError_t launch_set_task_values(const Params& P, const int32_t* idx, int k, const float* values, uint32_t rows, cudaStream_t st);
 cudaError_t launch_get_state(const Params& P, float* out_f, int32_t* out_i, cudaStream_t st);
 cudaError_t launch_set_state(const Params& P, const float* in_f, cudaStream_t st);
-cudaError_t launch_rebalance(const int32_t* cost, int n, int32_t* hist, int32_t* perm, cudaStream_t st);
+cudaError_t launch_rebalance(const int32_t* cost, const uint8_t* terrain, int n, int32_t* hist, int32_t* perm, cudaStream_t st);
 cudaError_t launch_episode_summary(const Params& P, int clear, double* out, cudaStream_t st);
 cudaError_t launch_render(const Params& P, const float* rt, const float* zrange, const int32_t* idx, int k, int W, int H,
                           float distance, float yaw_deg, float pitch_deg, uint8_t* rgb, cudaStream_t st, int* launches);
@@ -28,22 +28,54 @@ struct RexSim {
     uint8_t* ep_block = nullptr;       // episode statistics: the per-env block behind P.ep (episode_block_bytes)
     double* ep_summary = nullptr;      // [4] count, nonfinite, sum of scores, sum of lengths (rexsim_episode_summary)
     bool rt_set = false;
-    int32_t* perm = nullptr;           // slot -> env, sorted by solver cost; P.perm points here after rexsim_rebalance
-    int32_t* hist = nullptr;
+    int32_t* perm = nullptr;           // slot -> env, sorted by solver cost; P.perm points here after rexsim_rebalance (at once with
+                                       // per-env terrains: plane envs in slots [0, nplane), heightfield envs after them)
+    int32_t* hist = nullptr;           // rexsim_rebalance's bins: 256, 512 with per-env terrains (terrain-major)
     float* act = nullptr;              // staging for rexsim_step_host
     uint8_t* out = nullptr;            // obs | reward | done (same layout as the host block)
     uint8_t* fin = nullptr;            // final obs | limit staging for rexsim_step_host_final (allocated on its first call)
     int A = 0;
     bool started = false;              // a reset or step has been enqueued: the frame wrappers can no longer be switched on
-    int nsnap = 1;                     // reset snapshots per hold setting (one per field)
     int nholds = 0;                    // hold settings (motor_kp, motor_kd, pd_latency) of P.ev.gains / P.el.hold (0: no table)
     bool values_on = false;            // rexsim_set_env_values was called
     std::vector<float> kp, kd;         // per-env gains given to rexsim_set_env_values (empty: the config's)
     std::vector<double> pd;            // per-env pd latencies given to rexsim_set_env_latencies (empty: the config's)
     double* latency = nullptr;         // [2][N] per-env control and pd latencies (rexsim_set_env_latencies; null: off)
+    uint8_t* terrain = nullptr;        // [N] per-env terrains (rexsim_set_env_terrains; null: off); P.env_terrain points here
+    int nplane = 0;                    // envs on the plane (per-env terrains)
+    float friction[2] = {0.f, 0.f};    // per-env terrains: friction of each terrain's envs, plane and heightfield
     int64_t launches = 0;
     int32_t launched[3] = {0, 0, 0};   // step_kernel instance of the last step launch: BLOCK, OCC, SENSOR
+    int32_t group_launched[2][3] = {}; // per-env terrains: the same of the last launch over each terrain's slot range
 };
+
+// The handle's Params for the launches over one terrain's envs: the config's terrain and friction are that terrain's
+static Params terrain_params(const RexSim* s, Params P, int terrain) {
+    if (s->terrain) { P.cfg.terrain = terrain; P.cfg.friction = s->friction[terrain]; }
+    return P;
+}
+// envs on each terrain (every env on the config's terrain without per-env terrains)
+static void terrain_counts(const RexSim* s, int count[2]) {
+    count[0] = count[1] = 0;
+    if (s->terrain) { count[REXSIM_TERRAIN_PLANE] = s->nplane; count[REXSIM_TERRAIN_RANDOM] = s->P.N - s->nplane; }
+    else count[s->P.cfg.terrain] = s->P.N;
+}
+// One control step of every env: one launch over every slot, or with per-env terrains one launch per terrain over its slot
+// range of the permutation (plane [0, nplane), heightfield [nplane, N)), each choosing its build from its own size; a range
+// with no envs launches nothing.  Both on `st`, so a captured graph holds both.
+static int step_launches(RexSim* s, const Params& P, cudaStream_t st) {
+    if (!s->terrain) return enqueue(s, launch_step(P, st), "step launch");
+    int count[2];
+    terrain_counts(s, count);
+    for (int t = 0, first = 0; t < 2; first += count[t], t++) {
+        if (!count[t]) continue;
+        Params G = terrain_params(s, P, t);
+        G.perm = P.perm + first; G.nslots = count[t]; G.launched = s->group_launched[t];
+        if (int rc = enqueue(s, launch_step(G, st), "step launch")) return rc;
+        memcpy(s->launched, s->group_launched[t], sizeof(s->launched));
+    }
+    return REXSIM_OK;
+}
 
 // byte offsets of the block rexsim_step_host fills: obs [N][O] at 0 | reward [N] | done [N] | pad to 4 | int32 error bits |
 // 8 flag bytes the kernel sets directly on the zero-copy path
@@ -136,20 +168,22 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
     P.cfg.sim_dt = (float)cfg->sim_dt_d;
     const size_t N = cfg->num_envs;
     P.N = cfg->num_envs;
+    P.nslots = cfg->num_envs;
     {
         int dev = 0, sms = 132;
         CK(cudaGetDevice(&dev));
         CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         P.sm_count = sms;
     }
-    s->nsnap = snapshots_per_pair(*cfg);
+    P.snaps = snap_layout(cfg->terrain == REXSIM_TERRAIN_PLANE, cfg->terrain == REXSIM_TERRAIN_RANDOM, cfg->nfields);
+    const size_t nsnap = P.snaps.per_setting;
     s->A = rexsim_action_dim(cfg->task, cfg->signal);
     P.out_dim = out_dim(cfg->task, cfg->num_motors, 0);
     // the kernels read these through pointers to const; create fills them
     float *model = nullptr, *snap_f = nullptr, *zoff = nullptr;
     int32_t* snap_i = nullptr;
     if (mem.zeroed(&model, mt_floats) || mem.zeroed(&P.sf, NF * N) || mem.zeroed(&P.si, NI * N) ||
-        mem.zeroed(&snap_f, (size_t)NF * s->nsnap) || mem.zeroed(&snap_i, (size_t)NI * s->nsnap) ||
+        mem.zeroed(&snap_f, (size_t)NF * nsnap) || mem.zeroed(&snap_i, (size_t)NI * nsnap) ||
         mem.zeroed(&P.err, N + 1) ||                                    // [N] per-env bits + 1 word: OR of all
         mem.zeroed(&P.cmd_out, cfg->num_motors * N) || mem.zeroed(&P.cost, N) || mem.zeroed(&s->perm, N) ||
         mem.zeroed(&s->hist, 256) || mem.zeroed(&s->rt, REXSIM_RT_FLOATS) || mem.zeroed(&s->act, N * s->A) ||
@@ -162,7 +196,7 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
         P.ring_depth = sc.depth;
         P.ctl = sc.ctl; P.pd = sc.pd;
         for (int k = 0; k < 5; k++) P.noise_sd[k] = (float)cfg->noise_stdev[k];
-        if (mem.zeroed(&P.ring, (size_t)sc.depth * sc.words * N) || mem.zeroed(&P.snap_ring, (size_t)s->nsnap * sc.depth * sc.words))
+        if (mem.zeroed(&P.ring, (size_t)sc.depth * sc.words * N) || mem.zeroed(&P.snap_ring, nsnap * sc.depth * sc.words))
             return REXSIM_ERR_CUDA;
     }
     if (cfg->episode_stats) {
@@ -214,7 +248,7 @@ int rexsim_step(RexSim* s, const float* actions, float* obs, float* reward, uint
     Params P = s->P;
     P.actions = actions; P.obs = obs; P.reward = reward; P.done = done;
     s->started = true;
-    return enqueue(s, launch_step(P, (cudaStream_t)stream), "step launch");
+    return step_launches(s, P, (cudaStream_t)stream);
 }
 int rexsim_step_final(RexSim* s, const float* actions, float* obs, float* reward, uint8_t* done, float* final_obs,
                       uint8_t* limit, void* stream) {
@@ -222,7 +256,7 @@ int rexsim_step_final(RexSim* s, const float* actions, float* obs, float* reward
     Params P = s->P;
     P.actions = actions; P.obs = obs; P.reward = reward; P.done = done; P.final_obs = final_obs; P.limit = limit;
     s->started = true;
-    return enqueue(s, launch_step(P, (cudaStream_t)stream), "step launch");
+    return step_launches(s, P, (cudaStream_t)stream);
 }
 
 // bytes of the block rexsim_step_host_final fills besides h_out: final obs [N][O] f32 | limit [N] u8
@@ -271,7 +305,7 @@ static int step_host(RexSim* s, const float* h_actions, void* h_out, void* h_fin
         uint8_t* fin = zero_copy ? (uint8_t*)h_final : s->fin;
         P.final_obs = (float*)fin; P.limit = fin + N * s->P.out_dim * sizeof(float);
     }
-    if (int rc = enqueue(s, launch_step(P, st), "step launch")) return rc;
+    if (int rc = step_launches(s, P, st)) return rc;
     if (!zero_copy) {
         CK(cudaMemcpyAsync(h_out, s->out, hb.err, cudaMemcpyDeviceToHost, st));
         if (h_final) CK(cudaMemcpyAsync(h_final, s->fin, fb, cudaMemcpyDeviceToHost, st));
@@ -297,7 +331,8 @@ int rexsim_step_host_final(RexSim* s, const float* h_actions, void* h_out, void*
 
 int rexsim_rebalance(RexSim* s, void* stream) {
     if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
-    const int rc = enqueue(s, launch_rebalance(s->P.cost, s->P.N, s->hist, s->perm, (cudaStream_t)stream), "rebalance launch", 3);
+    const int rc = enqueue(s, launch_rebalance(s->P.cost, s->terrain, s->P.N, s->hist, s->perm, (cudaStream_t)stream),
+                           "rebalance launch", 3);
     if (rc == REXSIM_OK) s->P.perm = s->perm;   // steps enqueued after this call use the new grouping
     return rc;
 }
@@ -455,8 +490,33 @@ static int hold_table(const RexSimConfig& c, size_t N, const std::vector<float>&
     }
     return REXSIM_OK;
 }
+// Run the reset hold again for every snapshot of the layout P.snaps, at the handle's hold settings (the config's one without a
+// table), its sensor history rows at the handle's ring depth: one launch per terrain the batch has, each at that terrain's
+// friction, over all its (setting, field) snapshots.  Synchronous.
+static int settle_snapshots(RexSim* s) {
+    Params& P = s->P;
+    const int nh = s->nholds > 0 ? s->nholds : 1;
+    const size_t nsettle = (size_t)nh * P.snaps.per_setting;
+    float* snap_f = nullptr;
+    int32_t* snap_i = nullptr;
+    if (s->mem.zeroed(&snap_f, (size_t)NF * nsettle) || s->mem.zeroed(&snap_i, (size_t)NI * nsettle)) return REXSIM_ERR_CUDA;
+    s->mem.drop((void*)P.snap_f); s->mem.drop((void*)P.snap_i);
+    P.snap_f = snap_f; P.snap_i = snap_i;
+    if (P.sensor_on) {
+        s->mem.drop(P.snap_ring);
+        P.snap_ring = nullptr;
+        if (s->mem.zeroed(&P.snap_ring, nsettle * P.ring_depth * sensor_cfg(&P.cfg).words)) return REXSIM_ERR_CUDA;
+    }
+    int count[2];
+    terrain_counts(s, count);
+    for (int t = 0; t < 2; t++)
+        if (count[t])
+            if (int rc = enqueue(s, launch_settle(terrain_params(s, P, t), snap_f, snap_i, nh, 0), "settle launch")) return rc;
+    CK(cudaDeviceSynchronize());
+    return REXSIM_OK;
+}
 // Install a hold table (P.ev.pair, P.ev.gains and, with per-env latencies, P.el.hold), and with `settle` run the reset hold
-// again: one launch over every (setting, field) snapshot, its sensor history rows at the handle's ring depth.  Synchronous.
+// again (settle_snapshots).  Synchronous.
 static int apply_holds(RexSim* s, const HoldTable& t, bool settle) {
     Params& P = s->P;
     const size_t N = P.N, nh = t.pd.size();
@@ -477,21 +537,7 @@ static int apply_holds(RexSim* s, const HoldTable& t, bool settle) {
         P.el.hold = dhold;
     }
     s->nholds = (int)nh;
-    if (!settle) return REXSIM_OK;
-    float* snap_f = nullptr;
-    int32_t* snap_i = nullptr;
-    const size_t nsettle = nh * s->nsnap;
-    if (s->mem.zeroed(&snap_f, (size_t)NF * nsettle) || s->mem.zeroed(&snap_i, (size_t)NI * nsettle)) return REXSIM_ERR_CUDA;
-    s->mem.drop((void*)P.snap_f); s->mem.drop((void*)P.snap_i);
-    P.snap_f = snap_f; P.snap_i = snap_i;
-    if (P.sensor_on) {
-        s->mem.drop(P.snap_ring);
-        P.snap_ring = nullptr;
-        if (s->mem.zeroed(&P.snap_ring, nsettle * P.ring_depth * sensor_cfg(&P.cfg).words)) return REXSIM_ERR_CUDA;
-    }
-    if (int rc = enqueue(s, launch_settle(P, snap_f, snap_i, (int)nh, 0), "settle launch")) return rc;
-    CK(cudaDeviceSynchronize());
-    return REXSIM_OK;
+    return settle ? settle_snapshots(s) : REXSIM_OK;
 }
 int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const float* kd) {
     if (!s || !values || !kp != !kd) return fail(REXSIM_ERR_INVALID, "null argument (kp and kd are given together or not at all)");
@@ -577,6 +623,54 @@ int rexsim_env_latency_buffers(RexSim* s, double** latency, int32_t* depth) {
     if (!s || !latency || !depth) return fail(REXSIM_ERR_INVALID, "null argument");
     if (!s->latency) return fail(REXSIM_ERR_INVALID, "per-env latencies are off (rexsim_set_env_latencies)");
     *latency = s->latency; *depth = s->P.ring_depth;
+    return REXSIM_OK;
+}
+int rexsim_set_env_terrains(RexSim* s, const int32_t* terrain, float plane_friction) {
+    if (!s || !terrain) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env terrains must be set before the first reset or step");
+    if (s->terrain) return fail(REXSIM_ERR_INVALID, "per-env terrains are already set");
+    Params& P = s->P;
+    if (P.cfg.terrain != REXSIM_TERRAIN_RANDOM)
+        return fail(REXSIM_ERR_INVALID, "per-env terrains need a handle created on the random terrain (its heightfield bank)");
+    if (!(plane_friction >= 0.f) || std::isinf(plane_friction)) return fail(REXSIM_ERR_INVALID, "plane friction must be finite and non-negative");
+    const size_t N = P.N;
+    std::vector<uint8_t> bytes(N);
+    std::vector<int32_t> perm;
+    perm.reserve(N);
+    for (size_t e = 0; e < N; e++) {
+        if (terrain[e] != REXSIM_TERRAIN_PLANE && terrain[e] != REXSIM_TERRAIN_RANDOM)
+            return fail(REXSIM_ERR_INVALID, "terrain entries must be REXSIM_TERRAIN_PLANE or REXSIM_TERRAIN_RANDOM");
+        bytes[e] = (uint8_t)terrain[e];
+        if (terrain[e] == REXSIM_TERRAIN_PLANE) perm.push_back((int32_t)e);
+    }
+    const int nplane = (int)perm.size();
+    for (size_t e = 0; e < N; e++) if (bytes[e] == REXSIM_TERRAIN_RANDOM) perm.push_back((int32_t)e);
+    uint8_t* dterrain = nullptr;
+    int32_t* hist = nullptr;
+    if (s->mem.zeroed(&dterrain, N) || s->mem.zeroed(&hist, 512)) return REXSIM_ERR_CUDA;
+    CK(cudaMemcpy(dterrain, bytes.data(), N, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(s->perm, perm.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
+    s->mem.drop(s->hist);
+    s->hist = hist;
+    s->terrain = dterrain; s->nplane = nplane;
+    s->friction[REXSIM_TERRAIN_PLANE] = plane_friction; s->friction[REXSIM_TERRAIN_RANDOM] = P.cfg.friction;
+    P.env_terrain = dterrain;
+    P.perm = s->perm;                          // the partition holds from the first step on
+    P.snaps = snap_layout(nplane > 0, nplane < (int)N, P.cfg.nfields);
+    return settle_snapshots(s);
+}
+int rexsim_env_terrain_buffers(RexSim* s, uint8_t** terrain, int32_t* nplane) {
+    if (!s || !terrain || !nplane) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (!s->terrain) return fail(REXSIM_ERR_INVALID, "per-env terrains are off (rexsim_set_env_terrains)");
+    *terrain = s->terrain; *nplane = s->nplane;
+    return REXSIM_OK;
+}
+int rexsim_last_terrain_build(const RexSim* s, int32_t terrain, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor) {
+    if (!s || !cta_threads || !ctas_per_sm || !sensor) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (terrain != REXSIM_TERRAIN_PLANE && terrain != REXSIM_TERRAIN_RANDOM) return fail(REXSIM_ERR_INVALID, "terrain type");
+    static const int32_t none[3] = {0, 0, 0};
+    const int32_t* b = s->terrain ? s->group_launched[terrain] : terrain == s->P.cfg.terrain ? s->launched : none;
+    *cta_threads = b[0]; *ctas_per_sm = b[1]; *sensor = b[2];
     return REXSIM_OK;
 }
 int rexsim_set_task_values(RexSim* s, const int32_t* idx, int32_t k, const float* values, uint32_t rows, void* stream) {

@@ -1659,19 +1659,19 @@ __device__ __forceinline__ void store_arm(float* sf, int32_t* si, int N, int env
 // reset one env from the settled snapshot + task draws (BatchEnv.reset -> <task>.reset; rex.py:255-324)
 template <bool ARM>
 // `valid` is false on the padding lanes that replicate the last env to keep warps whole: they compute, but never write
-// (a replica that re-read the counter after the real lane's write would otherwise bump it twice)
-__device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, int leg, Lane& L, Task& K, float& kp, float& kd, int& field, Arm& AR, bool valid,
-                                                    Sensor& S) {
+// (a replica that re-read the counter after the real lane's write would otherwise bump it twice).  `terrain`: the env's own.
+__device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, int terrain, int leg, Lane& L, Task& K, float& kp, float& kd, int& field,
+                                                    Arm& AR, bool valid, Sensor& S) {
     const RexSimConfig& c = P.cfg;
     const int N = P.N;
     uint32_t rc = (uint32_t)P.si[I_RESETCNT * (size_t)N + env] + 1u;
     const uint32_t genv = (uint32_t)env + (uint32_t)c.env_offset;   // global env id: draws do not depend on the sharding
-    field = (c.terrain == REXSIM_TERRAIN_RANDOM) ? (int)((genv + rc) % (uint32_t)c.nfields) : 0;
+    field = (terrain == REXSIM_TERRAIN_RANDOM) ? (int)((genv + rc) % (uint32_t)c.nfields) : 0;
     // the env's own constructor values when the batch has them (rexsim_set_env_values), the config's otherwise
     const float* ev = P.ev.values ? P.ev.values + env : nullptr;
     auto value = [&](int row, float scalar) { return ev ? ev[(size_t)row * N] : scalar; };
     const int pair = P.ev.pair ? P.ev.pair[env] : 0;         // the env's hold setting (gain pair, with per-env latencies its PD latency)
-    const int snap = pair * snapshots_per_pair(c) + field;
+    const int snap = snapshot_index(P.snaps, pair, terrain, field);
     const float* sf = P.snap_f + (size_t)snap * NF;
     const int32_t* si = P.snap_i + (size_t)snap * NI;
     load_lane(sf, si, 1, 0, leg, L);
@@ -1871,9 +1871,12 @@ __device__ __forceinline__ bool write_obs(const Params& P, int env, int leg, con
 // 4 -> 128 registers (16 warps/SM hide the serial PGS / ABA chains, large batches)
 // SENSOR: the observation-history / latency / noise model of Rex (rex.py:726-769) is compiled in (any latency or noise > 0);
 // the default build reads the true state and keeps no history.
+// RANGE: the launch covers one terrain's slot range of a batch of both terrains, perm[0, nslots) (rexsim_set_env_terrains);
+// otherwise every slot of the batch.  A bound read in the single-terrain builds re-schedules their sub-step (6.5 % slower on the
+// headline build, H100), so it is compiled in only where it is needed.
 // heightfield tiles, (BLOCK / 4) x TILE_FLOATS floats (random terrain only), then (BLOCK / 4) x PGS_ENV_FLOATS (replicated PGS only)
 extern __shared__ __align__(16) float dyn_smem[];
-template <int TASK, int SIGNAL, int TERRAIN, int OCC, bool ARM, bool SENSOR, int BLOCK>
+template <int TASK, int SIGNAL, int TERRAIN, int OCC, bool ARM, bool SENSOR, int BLOCK, bool RANGE>
 __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const Params P) {
     __shared__ __align__(16) float sm[ARM ? REXSIM_MT_FLOATS_ARM : REXSIM_MT_FLOATS];
     __shared__ __align__(8) uint64_t bar;
@@ -1885,11 +1888,13 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
     const int gid = blockIdx.x * blockDim.x + threadIdx.x;
     int slot = gid >> 2;
     const int leg = gid & 3;
-    const bool valid = slot < N;
-    if (!valid) slot = N - 1;         // keep the warp converged for the shuffles; stores are masked
+    const int nslots = RANGE ? P.nslots : N;
+    const bool valid = slot < nslots;
+    if (!valid) slot = nslots - 1;    // keep the warp converged for the shuffles; stores are masked
     // Warp re-grouping: slot -> env through a permutation sorted by last step's solver cost (rexsim_rebalance), so the 8
     // envs of a warp need about the same number of PGS iterations.  Every env's arithmetic is independent of the
-    // permutation (bit-identical results); the scattered state accesses stay in L2.
+    // permutation (bit-identical results); the scattered state accesses stay in L2.  In a batch of both terrains each
+    // launch gets its terrain's range of the permutation, so padding lanes replicate an env of the launch's own terrain.
     const int env = P.perm ? P.perm[slot] : slot;
     const RexSimConfig& c = P.cfg;
     constexpr int A = task_shape(TASK).act[SIGNAL == REXSIM_SIGNAL_IK ? 0 : 1];
@@ -2065,7 +2070,7 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
     if (P.final_obs && done && valid) put_final<obs_dim(TASK, 12)>(P.final_obs + (size_t)env * P.out_dim, obs_row, P.out_dim, leg);
     // ---- auto reset: done envs restart from the settled snapshot; obs = first observation of the new episode --
     if (c.auto_reset && done) {
-        reset_from_snapshot<ARM>(P, env, leg, L, K, kp, kd, field, AR, valid, S);
+        reset_from_snapshot<ARM>(P, env, TERRAIN, leg, L, K, kp, kd, field, AR, valid, S);     // the launch's terrain is the env's
         if (valid) write_obs<TASK, SENSOR>(P, env, leg, L, obs_row, S, 0u, true);
     }
     store_lane(P.sf, P.si, N, env, leg, L, K, valid);
@@ -2092,7 +2097,8 @@ __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_o
     const bool wr = valid && inrange;
     Lane L; Task K; Arm AR; float kp, kd; int field;
     Sensor S = make_sensor<ARM>(P, P.ring, P.N, env, (uint32_t)env + (uint32_t)P.cfg.env_offset);
-    reset_from_snapshot<ARM>(P, env, leg, L, K, kp, kd, field, AR, wr, S);
+    const int terrain = P.env_terrain ? (int)P.env_terrain[env] : P.cfg.terrain;
+    reset_from_snapshot<ARM>(P, env, terrain, leg, L, K, kp, kd, field, AR, wr, S);
     if (wr && (obs_out || P.fr.ring || P.fr.last)) {      // the frame wrappers restart even when no observation is asked for
         float* row = obs_out ? obs_out + (size_t)j * P.out_dim : nullptr;
         if (P.sensor_on) write_obs<TASK, true>(P, env, leg, L, row, S, 0u, true);
@@ -2108,8 +2114,9 @@ __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_o
 
 // -------------------------------------------------------------------------------------------------
 // settle kernel: Rex.Reset (rex.py:296-324) for every snapshot, one per 4-lane group: 100 sub-steps holding 'stand'
-// then reset_time/dt holding the task's init pose; writes the snapshot row.  Snapshot s = pair * fields + field holds at
-// the gains of its pair, and with per-env latencies reads the PD observation at its setting's pd_latency.
+// then reset_time/dt holding the task's init pose; writes the snapshot row.  Group j of a launch settles the TERRAIN
+// snapshot (pair = j / fields, field = j % fields) of the layout P.snaps; it holds at the gains of its pair, and with per-env
+// latencies reads the PD observation at its setting's pd_latency.  P.cfg's friction is the terrain's.
 // -------------------------------------------------------------------------------------------------
 template <int TERRAIN, bool ARM, bool SENSOR>
 __global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_f, int32_t* snap_i, int nsettle, int signal, int task) {
@@ -2118,10 +2125,11 @@ __global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_
     __shared__ float tiles[TERRAIN == REXSIM_TERRAIN_RANDOM ? 8 * TILE_FLOATS : 1];
     tma_load_tables(sm, P.model, (ARM ? REXSIM_MT_FLOATS_ARM : REXSIM_MT_FLOATS) * 4, &bar);
     const int leg = threadIdx.x & 3;
-    const int snap = (blockIdx.x * blockDim.x + threadIdx.x) >> 2;
-    if (snap >= nsettle) return;      // whole 4-lane groups leave: no shuffle or barrier spans groups after the table load
-    const int nfield = snapshots_per_pair(P.cfg);
-    const int field = snap % nfield, pair = snap / nfield;
+    const int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 2;
+    if (j >= nsettle) return;         // whole 4-lane groups leave: no shuffle or barrier spans groups after the table load
+    const int nfield = terrain_snapshots(TERRAIN, P.cfg.nfields);
+    const int field = j % nfield, pair = j / nfield;
+    const int snap = snapshot_index(P.snaps, pair, TERRAIN, field);
     const float kp = P.ev.gains ? P.ev.gains[2 * pair] : P.cfg.motor_kp, kd = P.ev.gains ? P.ev.gains[2 * pair + 1] : P.cfg.motor_kd;
     Lane L; Task K;
     L.pos = mk(0.f, 0.f, 0.21f); L.qx = 0.f; L.qy = 0.f; L.qz = 0.f; L.qw = 1.f;
@@ -2192,10 +2200,10 @@ constexpr bool unit_of_inverts_c_units(int u = 0) {
 static_assert(unit_of_inverts_c_units(), "unit_of must map every (task, signal) of c_units to its own unit");
 template <int U> cudaError_t launch_step_unit(const Params& P, cudaStream_t st);
 #if !defined(REXSIM_UNIT) || REXSIM_UNIT < 100
-template <int TASK, int SIGNAL, int TERRAIN, int OCC, bool ARM, bool SENSOR, int BLOCK>
-static cudaError_t launch_step_variant(const Params& P, cudaStream_t st) {
-    auto kern = step_kernel<TASK, SIGNAL, TERRAIN, OCC, ARM, SENSOR, BLOCK>;
-    const int blocks = (P.N * 4 + BLOCK - 1) / BLOCK;
+template <int TASK, int SIGNAL, int TERRAIN, int OCC, bool ARM, bool SENSOR, int BLOCK, bool RANGE>
+static cudaError_t launch_step_range(const Params& P, cudaStream_t st) {
+    auto kern = step_kernel<TASK, SIGNAL, TERRAIN, OCC, ARM, SENSOR, BLOCK, RANGE>;
+    const int blocks = (P.nslots * 4 + BLOCK - 1) / BLOCK;
     const size_t smem = ((TERRAIN == REXSIM_TERRAIN_RANDOM ? (size_t)(BLOCK / 4) * TILE_FLOATS : 0) +
                          (pgs_replicated(OCC, ARM, TERRAIN) ? (size_t)(BLOCK / 4) * PGS_ENV_FLOATS : 0)) * sizeof(float);
     if (smem > 48 * 1024) {        // opt in once per kernel (the attribute is sticky)
@@ -2210,6 +2218,11 @@ static cudaError_t launch_step_variant(const Params& P, cudaStream_t st) {
     if (P.launched) { P.launched[0] = BLOCK; P.launched[1] = OCC; P.launched[2] = SENSOR; }
     return cudaGetLastError();
 }
+template <int TASK, int SIGNAL, int TERRAIN, int OCC, bool ARM, bool SENSOR, int BLOCK>
+static cudaError_t launch_step_variant(const Params& P, cudaStream_t st) {
+    if (P.nslots < P.N) return launch_step_range<TASK, SIGNAL, TERRAIN, OCC, ARM, SENSOR, BLOCK, true>(P, st);
+    return launch_step_range<TASK, SIGNAL, TERRAIN, OCC, ARM, SENSOR, BLOCK, false>(P, st);
+}
 template <int TASK, int SIGNAL, int TERRAIN, bool ARM>
 static cudaError_t launch_step_tsta(const Params& P, cudaStream_t st) {
     // sensor model compiled in: one (255-register) build per terrain
@@ -2217,7 +2230,8 @@ static cudaError_t launch_step_tsta(const Params& P, cudaStream_t st) {
     // Beyond one wave of 2-CTA/SM residency (128-thread CTAs; two waves on heightfields): the 128-register build (16 warps/SM
     // hide the serial ABA / PGS chains) in larger CTAs; below that the 255-register build, lowest single-wave latency
     // (DESIGN.md section 5).  Arm batches stay on the 255-register build: at 128 registers the arm's working set spills 4 KB.
-    bool big = !ARM && (P.N * 4 + 127) / 128 > (TERRAIN == REXSIM_TERRAIN_PLANE ? 2 : 4) * P.sm_count;
+    // A batch of both terrains chooses per launch, from the size of that terrain's slot range.
+    bool big = !ARM && (P.nslots * 4 + 127) / 128 > (TERRAIN == REXSIM_TERRAIN_PLANE ? 2 : 4) * P.sm_count;
     if (const char* f = getenv("REXSIM_FORCE_BUILD")) big = !ARM && f[0] == 'b';      // developer A/B: "big" / "small"
     if (big) return launch_step_variant<TASK, SIGNAL, TERRAIN, ARM ? 1 : REXSIM_OCC_BIG, ARM, false, ARM ? REXSIM_BLOCK : REXSIM_BLOCK_BIG>(P, st);
     return launch_step_variant<TASK, SIGNAL, TERRAIN, 1, ARM, false, REXSIM_BLOCK>(P, st);
@@ -2277,28 +2291,36 @@ __global__ void set_state_kernel(const Params P, const float* in_f) {
 }
 
 // ---- warp re-grouping: counting sort of the envs by solver cost, most expensive first (they start first: LPT order) ----
-__global__ void rebalance_hist_kernel(const int32_t* __restrict__ cost, int n, int32_t* __restrict__ hist) {
-    int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e < n) atomicAdd(&hist[255 - min(cost[e] >> 1, 255)], 1);
+// With per-env terrains the key is (terrain, cost bin): the plane envs keep slots [0, Np), the heightfield envs [Np, N).
+__device__ __forceinline__ int rebalance_bin(const int32_t* __restrict__ cost, const uint8_t* __restrict__ terrain, int e) {
+    const int b = 255 - min(cost[e] >> 1, 255);
+    return terrain ? (int)terrain[e] * 256 + b : b;
 }
-__global__ void rebalance_scan_kernel(int32_t* hist) {          // 1 block, 256 threads: exclusive prefix sum in place
-    __shared__ int32_t s[256];
+__global__ void rebalance_hist_kernel(const int32_t* __restrict__ cost, const uint8_t* __restrict__ terrain, int n, int32_t* __restrict__ hist) {
+    int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < n) atomicAdd(&hist[rebalance_bin(cost, terrain, e)], 1);
+}
+__global__ void rebalance_scan_kernel(int32_t* hist) {          // 1 block, one thread per bin (256 or 512): exclusive prefix sum in place
+    __shared__ int32_t s[512];
     const int t = threadIdx.x;
     s[t] = hist[t];
     __syncthreads();
-    for (int o = 1; o < 256; o <<= 1) { int v = t >= o ? s[t - o] : 0; __syncthreads(); s[t] += v; __syncthreads(); }
+    for (int o = 1; o < (int)blockDim.x; o <<= 1) { int v = t >= o ? s[t - o] : 0; __syncthreads(); s[t] += v; __syncthreads(); }
     hist[t] = s[t] - hist[t];
 }
-__global__ void rebalance_scatter_kernel(const int32_t* __restrict__ cost, int n, int32_t* __restrict__ offs, int32_t* __restrict__ perm) {
+__global__ void rebalance_scatter_kernel(const int32_t* __restrict__ cost, const uint8_t* __restrict__ terrain, int n,
+                                         int32_t* __restrict__ offs, int32_t* __restrict__ perm) {
     int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e < n) perm[atomicAdd(&offs[255 - min(cost[e] >> 1, 255)], 1)] = e;
+    if (e < n) perm[atomicAdd(&offs[rebalance_bin(cost, terrain, e)], 1)] = e;
 }
-cudaError_t launch_rebalance(const int32_t* cost, int n, int32_t* hist, int32_t* perm, cudaStream_t st) {
-    cudaError_t e = cudaMemsetAsync(hist, 0, 256 * sizeof(int32_t), st);
+// hist: [256] bins, [512] with per-env terrains (terrain not null)
+cudaError_t launch_rebalance(const int32_t* cost, const uint8_t* terrain, int n, int32_t* hist, int32_t* perm, cudaStream_t st) {
+    const int bins = terrain ? 512 : 256;
+    cudaError_t e = cudaMemsetAsync(hist, 0, bins * sizeof(int32_t), st);
     if (e != cudaSuccess) return e;
-    rebalance_hist_kernel<<<(n + 255) / 256, 256, 0, st>>>(cost, n, hist);
-    rebalance_scan_kernel<<<1, 256, 0, st>>>(hist);
-    rebalance_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(cost, n, hist, perm);
+    rebalance_hist_kernel<<<(n + 255) / 256, 256, 0, st>>>(cost, terrain, n, hist);
+    rebalance_scan_kernel<<<1, bins, 0, st>>>(hist);
+    rebalance_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(cost, terrain, n, hist, perm);
     return cudaGetLastError();
 }
 
@@ -2360,9 +2382,10 @@ static void launch_settle_ta(const Params& P, float* snap_f, int32_t* snap_i, in
     if (P.sensor_on) settle_kernel<TERRAIN, ARM, true><<<blocks, 32, 0, st>>>(P, snap_f, snap_i, nsettle, P.cfg.signal, P.cfg.task);
     else settle_kernel<TERRAIN, ARM, false><<<blocks, 32, 0, st>>>(P, snap_f, snap_i, nsettle, P.cfg.signal, P.cfg.task);
 }
+// the snapshots of `npairs` hold settings on P.cfg.terrain (one terrain per launch)
 cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, int npairs, cudaStream_t st) {
     const bool arm = P.cfg.num_motors == 18;
-    const int nsettle = npairs * snapshots_per_pair(P.cfg);
+    const int nsettle = npairs * terrain_snapshots(P.cfg.terrain, P.cfg.nfields);
     if (P.cfg.terrain == REXSIM_TERRAIN_PLANE) {
         if (arm) launch_settle_ta<REXSIM_TERRAIN_PLANE, true>(P, snap_f, snap_i, nsettle, st);
         else launch_settle_ta<REXSIM_TERRAIN_PLANE, false>(P, snap_f, snap_i, nsettle, st);

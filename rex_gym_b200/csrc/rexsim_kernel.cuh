@@ -109,9 +109,20 @@ struct EnvLatencies {
     const EnvDelay* __restrict__ env;  // [N]
     const Delay* __restrict__ hold;    // [settings] PD term of each hold setting (EnvValues.pair indexes it)
 };
-// reset snapshots per gain pair: one per field of the heightfield bank
-__host__ __device__ __forceinline__ int snapshots_per_pair(const RexSimConfig& c) {
-    return c.terrain == REXSIM_TERRAIN_RANDOM ? c.nfields : 1;
+// Settled reset snapshots of one hold setting on one terrain: one per field of the heightfield bank, one on the plane
+__host__ __device__ __forceinline__ int terrain_snapshots(int terrain, int nfields) {
+    return terrain == REXSIM_TERRAIN_RANDOM ? nfields : 1;
+}
+// The snapshot layout, its one owner (the settle writes it, reset_from_snapshot and the auto-reset read it): hold setting h
+// owns snapshots [h * per_setting, (h + 1) * per_setting), the plane's first when the batch has plane envs, then one per
+// field from `field0` on when it has heightfield envs.  A single-terrain batch: per_setting = terrain_snapshots, field0 0
+// on the heightfield (1 on the plane, where it is never read).
+struct SnapLayout { int32_t per_setting, field0; };
+__host__ __device__ __forceinline__ SnapLayout snap_layout(bool plane, bool random, int nfields) {
+    return SnapLayout{(plane ? 1 : 0) + (random ? nfields : 0), plane ? 1 : 0};
+}
+__host__ __device__ __forceinline__ int snapshot_index(const SnapLayout& s, int setting, int terrain, int field) {
+    return setting * s.per_setting + (terrain == REXSIM_TERRAIN_RANDOM ? s.field0 + field : 0);
 }
 
 struct Params {
@@ -124,8 +135,12 @@ struct Params {
     const float* __restrict__ model;   // REXSIM_MT_FLOATS floats, 16-byte aligned
     float* __restrict__ sf;            // [NF][N]
     int32_t* __restrict__ si;          // [NI][N]
-    const float* __restrict__ snap_f;  // [npairs * fields][NF] settled reset snapshots, pair-major
-    const int32_t* __restrict__ snap_i;// [npairs * fields][NI]
+    const float* __restrict__ snap_f;  // [settings * snaps.per_setting][NF] settled reset snapshots, setting-major
+    const int32_t* __restrict__ snap_i;// [settings * snaps.per_setting][NI]
+    SnapLayout snaps;
+    // per-env terrains (rexsim_set_env_terrains; null: every env on cfg.terrain): [N] REXSIM_TERRAIN_* by env.  The step
+    // kernel never reads it: each of its launches covers one terrain's slot range, with that terrain in cfg.terrain.
+    const uint8_t* __restrict__ env_terrain;
     const float* __restrict__ field_zoff; // [nfields]
     int32_t* __restrict__ err;         // [N] per-env bits of the most recent step, [N] = OR of all since last cleared
     uint8_t* err_host;                 // host-buffer step with zero-copy buffers: 8 flag bytes in the caller's block, byte b = 1 when an
@@ -143,10 +158,11 @@ struct Params {
     uint8_t* limit;
     const int32_t* __restrict__ reset_idx; // reset kernel: [k] or null
     int32_t reset_k;
-    int32_t N;
+    int32_t N;                         // envs: the stride of every per-env array
+    int32_t nslots;                    // step kernel: slots it covers, perm[0, nslots) (N, or one terrain's range of a mixed batch)
     int32_t sm_count;                  // SMs of the device (kernel variant choice)
     int32_t* launched;                 // host: {BLOCK, OCC, SENSOR} of the step_kernel instance the last step launched (never read on the device)
-    const int32_t* __restrict__ perm;  // [N] slot -> env (null: identity); see rexsim_rebalance
+    const int32_t* __restrict__ perm;  // [nslots] slot -> env (null: identity); see rexsim_rebalance
     int32_t* __restrict__ cost;        // [N] solver iterations of the last control step
     // sensor model (control / PD latency, observation noise: rex.py:735-769); all unused when sensor_on == 0
     int32_t sensor_on;

@@ -28,6 +28,7 @@ struct RenderArgs {
     const int32_t* __restrict__ idx;    // [k] env of each image
     uint8_t* __restrict__ rgb;          // [k][H][W][3]
     int32_t* __restrict__ err;          // [N + 1]: word N = aggregate error bits
+    const uint8_t* __restrict__ env_terrain;   // [N] terrain of each env (per-env terrains), else null: `terrain` for all
     int N, terrain, arm, toe_npts;
     int W, H, tiles_x, image0;
     float dist, yaw, pitch;             // radians
@@ -200,13 +201,13 @@ __device__ __forceinline__ void hit_cylinder(const float* rec, V3 o, V3 r, float
     }
 }
 
-// ground: the plane z = 0, or the env's heightfield (rexsim_kernel.cu ground_query: vertex (ix, iy) at x = (ix - 127.5) * 0.05,
+// ground: the plane z = 0 (h null), or the env's heightfield h (rexsim_kernel.cu ground_query: vertex (ix, iy) at x = (ix - 127.5) * 0.05,
 // height h[iy][ix] - zoff, cell split v >= u).  The ray is marched cell by cell (2-D DDA) over the part of it that lies inside
 // the field's square and inside the slab of the field's heights.  Outside the square the ground is the horizontal plane at
 // the field's lowest centred height (the physics clamps its queries to the border cells instead; DESIGN.md section 5).
 __device__ __forceinline__ void hit_ground(const RenderArgs& A, const float* h, float zoff, float zlo, float zhi, V3 o, V3 r,
                                            float& best, V3& nrm) {
-    if (A.terrain != REXSIM_TERRAIN_RANDOM) {
+    if (!h) {                  // the plane
         if (r.z < 0.f) { float t = -o.z / r.z; if (t > 0.f && t < best) { best = t; nrm = mk(0.f, 0.f, 1.f); } }
         return;
     }
@@ -334,7 +335,7 @@ __global__ void __launch_bounds__(RT_TILE * RT_TILE) render_kernel(const RenderA
             else hit_cylinder(rec, o, r, best, nrm);
             if (best < prev) who = s;
         }
-        if (A.terrain == REXSIM_TERRAIN_RANDOM) {
+        if ((A.env_terrain ? (int)A.env_terrain[env] : A.terrain) == REXSIM_TERRAIN_RANDOM) {      // the env's own ground
             const int field = A.si[I_FIELD * (size_t)A.N + env];
             const float prev = best;
             hit_ground(A, A.fields + (size_t)field * 65536, A.zoff[field], A.zrange[2 * field], A.zrange[2 * field + 1], o, r, best, nrm);
@@ -368,7 +369,7 @@ cudaError_t launch_render(const Params& P, const float* rt, const float* zrange,
                           float distance, float yaw_deg, float pitch_deg, uint8_t* rgb, cudaStream_t st, int* launches) {
     RenderArgs A;
     A.sf = P.sf; A.si = P.si; A.model = P.model; A.rt = rt; A.fields = P.cfg.fields; A.zoff = P.field_zoff; A.zrange = zrange;
-    A.idx = idx; A.err = P.err; A.N = P.N; A.terrain = P.cfg.terrain; A.arm = P.cfg.num_motors == 18; A.toe_npts = P.cfg.toe_npts;
+    A.idx = idx; A.err = P.err; A.N = P.N; A.terrain = P.cfg.terrain; A.env_terrain = P.env_terrain; A.arm = P.cfg.num_motors == 18; A.toe_npts = P.cfg.toe_npts;
     A.W = W; A.H = H; A.dist = distance;
     A.yaw = yaw_deg * (float)(3.14159265358979323846 / 180.0); A.pitch = pitch_deg * (float)(3.14159265358979323846 / 180.0);
     const int tiles_y = (H + RT_TILE - 1) / RT_TILE;

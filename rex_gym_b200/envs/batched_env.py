@@ -186,6 +186,33 @@ def check_env_latencies(num_envs, control_latency, pd_latency, motor_kp=1.0, mot
     return tuple(lat)
 
 
+def check_terrain(terrain_type):
+    """One terrain_type value, refused before any CUDA call unless it is a built terrain."""
+    if not isinstance(terrain_type, str) or terrain_type not in TERRAINS:
+        raise ValueError("terrain_type %r: only 'plane' and 'random' are built (csv/png assets live in the "
+                         "pybullet_data pip package)" % (terrain_type,))
+
+
+def check_env_terrains(num_envs, terrain_type):
+    """The terrain_type keyword, checked before any CUDA call: a scalar, or one entry per env (a list, tuple or ndarray), each
+    'plane' or 'random'.  -> (scalar, None) for a scalar or an array whose entries are all equal (the scalar construction);
+    (None, int32 [num_envs] of TERRAINS ids) for a batch of both terrains."""
+    if not is_per_env(terrain_type):
+        check_terrain(terrain_type)
+        return terrain_type, None
+    if isinstance(terrain_type, torch.Tensor):
+        raise ValueError("terrain_type: per-env entries are the strings 'plane' / 'random', not a tensor")
+    a = np.asarray(list(terrain_type) if isinstance(terrain_type, (list, tuple)) else terrain_type, dtype=object)
+    if a.shape != (int(num_envs),):
+        raise ValueError("terrain_type: expected one entry per env (%d), got shape %s" % (int(num_envs), a.shape))
+    entries = [str(t) if isinstance(t, str) else t for t in a]
+    for t in entries:
+        check_terrain(t)
+    if len(set(entries)) == 1:
+        return entries[0], None
+    return None, np.ascontiguousarray([TERRAINS[t] for t in entries], np.int32)
+
+
 class _Info(object):
     """Stand-in for BatchEnv's `tuple(infos)`: info[i] == {'action': motor command of env i} of THE STEP THAT RETURNED IT
     (rex_gym_env.py:414).  The command block lives on the device and is overwritten by the next step, so the host copy is taken
@@ -264,14 +291,18 @@ class BatchedRexEnv(object):
         final_observation: every step also keeps, for each env whose step returned done, the observation the step produced
           before the auto-reset replaced it (final_observation(), [N, O] like the observation rows), and every env's time-limit
           byte (truncated(), info[i]['TimeLimit.truncated'] as gym's TimeLimit adds it).  Off by default: no extra buffer, and
-          info[i] is {'action': ...}."""
+          info[i] is {'action': ...}.
+
+        terrain_type: 'plane', 'random', or one of them per env (a list, tuple or ndarray of num_envs entries).  Env e of a
+          batch of both runs exactly as env e of the batch built with its entry as the scalar: its own ground, friction and
+          field sequence from the one num_fields bank.  Each step launches the plane envs and the heightfield envs as two slot
+          ranges of the batch, each with its terrain's kernel build.  All-equal entries build the scalar construction."""
         if urdf_version is not None and urdf_version != DEFAULT_URDF_VERSION:
             raise ValueError("%s is not a supported urdf_version." % urdf_version)     # rex_gym_env.py:317-318
         if task not in TASKS or signal_type not in SIGNALS:
             raise ValueError("unknown task/signal_type %r/%r" % (task, signal_type))
-        if terrain_type not in TERRAINS:
-            raise ValueError("terrain_type %r: only 'plane' and 'random' are built (csv/png assets live in the "
-                             "pybullet_data pip package)" % terrain_type)
+        # per-env terrains: a batch of both is created on the heightfield (its bank), then told which envs are on the plane
+        terrain_scalar, env_terrain = check_env_terrains(num_envs, terrain_type)
         if render or on_rack:
             raise ValueError("render / on_rack are GUI debugging modes of the reference; not part of the batched path")
         scalar_lat = [0.0 if is_per_env(v) else v for v in (control_latency, pd_latency)]
@@ -292,7 +323,9 @@ class BatchedRexEnv(object):
             raise RuntimeError("rex_gym_b200 needs a CUDA device: there is no CPU fallback")
         self._L = _capi.load()
         self._debug = bool(debug)
-        self.task, self.signal_type, self.terrain_type, self.mark = task, signal_type, terrain_type, mark
+        self.task, self.signal_type, self.mark = task, signal_type, mark
+        # the scalar for a scalar construction (an array of equal entries is one), else the N entries
+        self.terrain_type = terrain_scalar if env_terrain is None else tuple(str(t) for t in terrain_type)
         self.device = torch.device(device)
         self.num_envs = int(num_envs)
         self.num_motors = 12 if mark == "base" else 18
@@ -304,7 +337,8 @@ class BatchedRexEnv(object):
             raise ValueError("mark must be 'base' or 'arm'")          # mark_constants.py:1
         tables, toe_npts = pack_model_tables(mark)
         c = _capi.RexSimConfig()
-        c.num_envs, c.task, c.signal, c.terrain = self.num_envs, TASKS[task], SIGNALS[signal_type], TERRAINS[terrain_type]
+        c.num_envs, c.task, c.signal = self.num_envs, TASKS[task], SIGNALS[signal_type]
+        c.terrain = TERRAINS[terrain_scalar or "random"]
         c.num_motors, c.action_repeat = self.num_motors, rep
         c.solver_iterations = solver_iterations or int(300 / rep)                      # rex_gym_env.py:25,184
         c.sim_dt, c.sim_dt_d = self._time_step, self._time_step
@@ -330,14 +364,16 @@ class BatchedRexEnv(object):
             c.noise_stdev[k] = float(v)
         c.episode_stats = int(bool(episode_statistics))       # simulate()'s score / length bookkeeping on the device
         self._fields = None
+        friction = {"random": 0.5 * 0.5,      # URDF link default 0.5 x createMultiBody default 0.5
+                    "plane": 0.5 * 1.0}       # x plane.urdf lateral_friction 1
         with torch.cuda.device(self.device):
-            if terrain_type == "random":
+            if c.terrain == TERRAINS["random"]:
                 self._fields = torch.from_numpy(make_random_fields(num_fields)).to(self.device).contiguous()
                 c.nfields, c.fields = num_fields, self._fields.data_ptr()
-                c.friction = 0.5 * 0.5          # URDF link default 0.5 x createMultiBody default 0.5
+                c.friction = friction["random"]
             else:
                 c.nfields, c.fields = 0, None
-                c.friction = 0.5 * 1.0          # x plane.urdf lateral_friction 1
+                c.friction = friction["plane"]
             c.residual_threshold, c.erp_contact, c.erp_joint = 1e-7, 0.08, 0.2
             c.toe_npts, c.toe_margin = toe_npts, TOE_MARGIN
             c.contact_breaking = contact_breaking_distance(mark)
@@ -358,6 +394,8 @@ class BatchedRexEnv(object):
             fi = np.ascontiguousarray(frames or [0], np.int32)
             self._call(self._L.rexsim_set_frames, self._h, fi.ctypes.data, len(frames), int(bool(frame_delta)), stream=False)
         self.frame_history, self.frame_delta = (list(frames) if frames else None), bool(frame_delta)
+        if env_terrain is not None:
+            self._call(self._L.rexsim_set_env_terrains, self._h, env_terrain.ctypes.data, friction["plane"], stream=False)
         self._values = None
         if env_values is not None:
             block = np.full((len(TASK_VALUE_KEYWORDS), self.num_envs), np.nan, np.float32)
@@ -407,6 +445,11 @@ class BatchedRexEnv(object):
             _capi.check(self._L.rexsim_env_value_buffers(self._h, C.byref(p), C.byref(q), C.byref(g), C.byref(npairs)))
             self._values = dict(values=view(p, (len(TASK_VALUE_KEYWORDS) + 1, N), "<f4"), pair=view(q, (N,), "<i4"),
                                 gains=view(g, (npairs.value, 2), "<f4"))
+        self._terrain = None                 # [N] u8: each env's TERRAINS id (per-env terrains only)
+        if env_terrain is not None:
+            nplane = C.c_int32()
+            _capi.check(self._L.rexsim_env_terrain_buffers(self._h, C.byref(p), C.byref(nplane)))
+            self._terrain = view(p, (N,), "|u1")
         self._latency = None                 # [2][N] f64: each env's control_latency, pd_latency (per-env latencies only)
         if env_latency is not None:
             depth = C.c_int32()
@@ -625,9 +668,16 @@ class BatchedRexEnv(object):
             sd.update(("env_" + k, v.clone()) for k, v in self._values.items())
         if self._latency is not None:
             sd["env_latency"] = self._latency.clone()
+        if self._terrain is not None:
+            sd["env_terrain"] = self._terrain.clone()
         return sd
 
     def load_state_dict(self, sd):
+        if (self._terrain is None) != ("env_terrain" not in sd):
+            raise ValueError("per-env terrains: the checkpoint %s them, this batch %s" %
+                             (("has", "does not") if self._terrain is None else ("lacks", "has")))
+        if self._terrain is not None and not torch.equal(self._terrain, sd["env_terrain"].to(self._terrain.device)):
+            raise ValueError("per-env terrains: the checkpoint's terrains differ from this batch's")
         if (self._latency is None) != ("env_latency" not in sd):
             raise ValueError("per-env latencies: the checkpoint %s them, this batch %s" %
                              (("has", "does not") if self._latency is None else ("lacks", "has")))
@@ -653,14 +703,14 @@ class BatchedRexEnv(object):
     # ---- per-env task values ------------------------------------------------------------------------------
     def set_task_values(self, indices=None, **values):
         """Give the envs `indices` (default: all) new constructor values, e.g. set_task_values([0, 3], target_position=2.5)
-        or a curriculum between Rollout.collect() calls.  Keywords: those of TASK_VALUE_KEYWORDS (the gains and latencies are
-        fixed at construction), each a scalar or one value per index, meaning what it means to the constructor.  Each env starts using
-        them at its next reset, explicit or automatic.  Enqueued on the current stream without a host sync; host values are
+        or a curriculum between Rollout.collect() calls.  Keywords: those of TASK_VALUE_KEYWORDS (the gains, latencies and
+        terrains are fixed at construction), each a scalar or one value per index, meaning what it means to the constructor.
+        Each env starts using them at its next reset, explicit or automatic.  Enqueued on the current stream without a host sync; host values are
         checked here, device tensors are not inspected.  Needs a batch built with per-env values (any of these keywords, or
         motor_kp / motor_kd, given one value per env)."""
         bad = sorted(set(values) - set(TASK_VALUE_KEYWORDS))
         if bad:
-            raise ValueError("set_task_values takes %s; not %s (the gains and latencies are fixed at construction)" %
+            raise ValueError("set_task_values takes %s; not %s (the gains, latencies and terrains are fixed at construction)" %
                              (TASK_VALUE_KEYWORDS, bad))
         if self._values is None:
             raise ValueError("per-env values are off: build the batch with one value per env for a task keyword")

@@ -13,7 +13,11 @@ Latencies (--workload latencies): walk-ik at 16 384 and 65 536 envs with control
 against a mixed batch cycling its envs through control latencies 0 / 10.5 / 20 ms and pd latencies 0 / 0.5 / 1 ms (the same
 deepest history row), alternately in one process.
 
-Usage: python tools/bench_env_values.py [--steps 200] [--rounds 3] [--workload all|values|latencies]"""
+Terrains (--workload terrains): walk-ik and turn-ik at 16 384 and 65 536 envs on the 64-field bank, all on the plane, all on
+the heightfield, a 50/50 mix (every other env) stepped as two slot ranges of one batch, and the sum of an all-plane and an
+all-heightfield batch of N/2 each, alternately in one process.
+
+Usage: python tools/bench_env_values.py [--steps 200] [--rounds 3] [--workload all|values|latencies|terrains]"""
 import argparse
 import json
 import os
@@ -94,7 +98,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=3, help="step rounds; creation rows take the median of 2 x rounds + 1")
-    ap.add_argument("--workload", choices=("all", "values", "latencies"), default="all")
+    ap.add_argument("--workload", choices=("all", "values", "latencies", "terrains"), default="all")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_env_values needs a CUDA device")
@@ -110,7 +114,25 @@ def main():
             print(json.dumps(dict(config="walk-ik latencies", envs=n, steps=a.steps, ms_scalar=[round(x, 4) for x in scalar],
                                   ms_mixed=[round(x, 4) for x in mixed],
                                   mixed_cost_pct=round(100 * (median(mixed) / median(scalar) - 1), 2))), flush=True)
-    if a.workload == "latencies":
+    if a.workload in ("all", "terrains"):
+        for task in ("walk", "turn"):
+            for n in (16384, 65536):
+                kw = dict(task=task, signal_type="ik", num_fields=64)
+                mix = ["plane", "random"] * (n // 2)
+                rows = {}
+                for _ in range(a.rounds):
+                    for name, k in (("plane", dict(kw, num_envs=n, terrain_type="plane")),
+                                    ("random", dict(kw, num_envs=n, terrain_type="random")),
+                                    ("mixed", dict(kw, num_envs=n, terrain_type=mix)),
+                                    ("half_plane", dict(kw, num_envs=n // 2, terrain_type="plane")),
+                                    ("half_random", dict(kw, num_envs=n // 2, terrain_type="random"))):
+                        rows.setdefault(name, []).append(ms_per_step(k, a.steps))
+                halves = median(rows["half_plane"]) + median(rows["half_random"])
+                print(json.dumps(dict(config="%s-ik terrains" % task, envs=n, steps=a.steps,
+                                      **{"ms_" + k: [round(x, 4) for x in v] for k, v in rows.items()},
+                                      ms_halves_sum=round(halves, 4),
+                                      mixed_vs_halves_pct=round(100 * (median(rows["mixed"]) / halves - 1), 2))), flush=True)
+    if a.workload in ("latencies", "terrains"):
         return
     for prefix in NAMES:
         name, kw = next(c for c in CONFIGS if c[0].startswith(prefix))
