@@ -276,8 +276,10 @@ enum {
     REXSIM_VALUE_ROWS = 9,            /* rows a caller writes */
     REXSIM_VALUE_EPISODE_BACKWARDS = 9,
     REXSIM_VALUE_BLOCK_ROWS = 10,
-    REXSIM_MAX_GAIN_PAIRS = 64        /* distinct hold settings (motor_kp, motor_kd, pd_latency): the settle runs once per
-                                         setting and field */
+    REXSIM_MAX_GAIN_PAIRS = 64,       /* distinct hold settings (motor_kp, motor_kd, pd_latency, solver_iterations): the settle
+                                         runs once per setting and field */
+    REXSIM_MAX_REPEAT_PAIRS = 8,      /* distinct (action_repeat, solver_iterations) pairs of rexsim_set_env_repeats */
+    REXSIM_GROUP_WORDS = 8            /* int32 words rexsim_launch_group writes */
 };
 /* row of the value block that the constructor keyword `keyword` fills ("target_position", "backwards", "target_orient",
  * "init_orient", "base_y", "base_z", "base_roll", "base_pitch", "base_yaw"); -1 for any other name */
@@ -332,16 +334,44 @@ int rexsim_set_env_terrains(RexSim* sim, const int32_t* terrain, float plane_fri
 /* the per-env terrains' device buffer, part of a checkpoint's identity: terrain dev [N] u8 (REXSIM_TERRAIN_* of each env),
  * and the number of envs on the plane.  REXSIM_ERR_INVALID when the per-env terrains are off. */
 int rexsim_env_terrain_buffers(RexSim* sim, uint8_t** terrain, int32_t* nplane);
-/* kernels launched by this handle since create (the bench reports it); a step of a batch with envs on both terrains counts
- * two launches */
+/* Per-env control rates: the control_time_step and action_repeat keywords of BatchEnv([ctor_0, ctor_1, ...]) over envs that
+ * share the simulation time step control_time_step / action_repeat (rex_gym_env.py:170-173), which the observation space
+ * depends on; the action space depends on neither (batch_env.py:36-43).  action_repeat, solver_iterations HOST [N] int32
+ * each, NULL: every env takes the RexSimConfig scalar.  Env e then runs exactly as a batch created with action_repeat[e] and
+ * solver_iterations[e] as its scalars: action_repeat[e] physics sub-steps per control step, each PGS solve capped at
+ * solver_iterations[e] iterations, and its reset hold settled at that cap.  Everything derived from sim_dt (sensor delays,
+ * overheat limit, gait clock, hold length, rate bounds, energy) stays the batch's.
+ * The batch's envs fall into launch groups (terrain, action_repeat, solver_iterations), terrain-major (plane first) and in
+ * order of first appearance; group g owns a contiguous slot range of the permutation (rexsim_rebalance keeps the
+ * partition), and each step launches the step kernel once per group over its range with the group's values, each launch
+ * choosing its build from its own size, all on the stream.  The hold settings become (motor_kp, motor_kd, pd_latency,
+ * solver_iterations), each count's settings contiguous, settled once per (terrain, count).
+ * Refused (REXSIM_ERR_INVALID) for an entry <= 0, more than REXSIM_MAX_REPEAT_PAIRS distinct (action_repeat,
+ * solver_iterations) pairs, more hold settings than REXSIM_MAX_GAIN_PAIRS, after the handle's first reset or step, and on a
+ * second call.  Composes with rexsim_set_env_values, rexsim_set_env_latencies and rexsim_set_env_terrains in any order;
+ * synchronous.  Off: nothing is allocated and every launch is what it is without it. */
+int rexsim_set_env_repeats(RexSim* sim, const int32_t* action_repeat, const int32_t* solver_iterations);
+/* the per-env control rates' device buffer, part of a checkpoint's identity: repeats dev [2][N] int32 (row 0 action_repeat,
+ * row 1 solver_iterations).  REXSIM_ERR_INVALID when the per-env repeats are off. */
+int rexsim_env_repeat_buffers(RexSim* sim, int32_t** repeats);
+/* launch groups of the batch: 1 unless per-env terrains or repeats split it (0 for a null handle) */
+int rexsim_launch_groups(const RexSim* sim);
+/* launch group g: info[REXSIM_GROUP_WORDS] = terrain, action_repeat, solver_iterations, first slot, slot count, and the
+ * build its last step launch used (CTA size, CTAs per SM, sensor; all 0 before the first step).  A batch of one group
+ * reports the config's values over slots [0, N).  REXSIM_ERR_INVALID for g outside [0, rexsim_launch_groups). */
+int rexsim_launch_group(const RexSim* sim, int32_t g, int32_t* info);
+/* the permutation the step launches read and each env's launch group: perm dev [N] int32 (slot -> env; group g's envs in
+ * slots [first_g, first_g + count_g) of rexsim_launch_group), NULL until rexsim_rebalance or a per-env setter that splits
+ * the batch (the identity); group dev [N] u8, NULL for a batch of one launch group */
+int rexsim_slot_buffers(RexSim* sim, int32_t** perm, uint8_t** group);
+/* kernels launched by this handle since create (the bench reports it); a step counts one launch per launch group */
 int64_t rexsim_launch_count(const RexSim* sim);
 /* which build of the step kernel the last rexsim_step / rexsim_step_host launched (all 0 before the first step): CTA size,
  * resident CTAs per SM it is compiled for (1: 255 registers, 4: 128 registers), 1 if the sensor model is compiled in.
- * With per-env terrains: the build of that step's last launch, the heightfield envs' when it has any (the plane envs' are
- * rexsim_last_terrain_build's) */
+ * With several launch groups: the build of that step's last launch (rexsim_launch_group has each group's) */
 int rexsim_last_step_build(const RexSim* sim, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor);
-/* the same for the last launch over the envs on `terrain`: with per-env terrains that terrain's launch; otherwise the
- * batch's launch for its own terrain, all 0 for the other */
+/* the same for the last launch over the envs on `terrain`: the last launch group on that terrain; all 0 when the batch has no
+ * env on it */
 int rexsim_last_terrain_build(const RexSim* sim, int32_t terrain, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor);
 /* the counter-based generator behind every reset draw (replaces Python's unseeded `random`,
  * walk_env.py:133-147, gallop_env.py:151, turn_env.py:138,147); host-callable so tests can pin it */

@@ -77,6 +77,11 @@ SIGNATURES = {
     "rexsim_env_latency_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_i32)]),
     "rexsim_set_env_terrains": (C.c_int, [_ptr, _ptr, _f32]),
     "rexsim_env_terrain_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_i32)]),
+    "rexsim_set_env_repeats": (C.c_int, [_ptr] * 3),
+    "rexsim_env_repeat_buffers": (C.c_int, [_ptr, _out(_ptr)]),
+    "rexsim_launch_groups": (C.c_int, [_ptr]),
+    "rexsim_launch_group": (C.c_int, [_ptr, _i32, _ptr]),
+    "rexsim_slot_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_ptr)]),
     "rexsim_launch_count": (_i64, [_ptr]),
     "rexsim_last_step_build": (C.c_int, [_ptr] + [_out(_i32)] * 3),
     "rexsim_last_terrain_build": (C.c_int, [_ptr, _i32] + [_out(_i32)] * 3),

@@ -1,6 +1,7 @@
 // rexsim_capi.cu -- the C ABI declared in include/rexsim.h (plain pointers and sizes, no torch types).
 #include "rexsim_kernel.cuh"
 #include "rexsim_host.h"
+#include <algorithm>
 #include <cstring>
 #include <cmath>
 #include <vector>
@@ -8,17 +9,25 @@
 namespace rexsim {
 cudaError_t launch_step(const Params& P, cudaStream_t st);
 cudaError_t launch_reset(const Params& P, float* obs_out, cudaStream_t st);
-cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, int npairs, cudaStream_t st);
+cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, int first, int npairs, cudaStream_t st);
 cudaError_t launch_set_task_values(const Params& P, const int32_t* idx, int k, const float* values, uint32_t rows, cudaStream_t st);
 cudaError_t launch_get_state(const Params& P, float* out_f, int32_t* out_i, cudaStream_t st);
 cudaError_t launch_set_state(const Params& P, const float* in_f, cudaStream_t st);
-cudaError_t launch_rebalance(const int32_t* cost, const uint8_t* terrain, int n, int32_t* hist, int32_t* perm, cudaStream_t st);
+cudaError_t launch_rebalance(const int32_t* cost, const uint8_t* group, int ngroups, int n, int32_t* hist, int32_t* perm,
+                             cudaStream_t st);
 cudaError_t launch_episode_summary(const Params& P, int clear, double* out, cudaStream_t st);
 cudaError_t launch_render(const Params& P, const float* rt, const float* zrange, const int32_t* idx, int k, int W, int H,
                           float distance, float yaw_deg, float pitch_deg, uint8_t* rgb, cudaStream_t st, int* launches);
 }  // namespace rexsim
 
 using namespace rexsim;
+
+// One launch of the step kernel per control step: the envs of one (terrain, action_repeat, solver_iterations), which own slots
+// perm[first, first + count)
+struct LaunchGroup {
+    int32_t terrain, repeat, iters, first, count;
+    int32_t launched[3];               // step_kernel instance of the group's last launch: BLOCK, OCC, SENSOR
+};
 
 struct RexSim {
     Params P;                          // the handle's buffers are P's pointer fields, allocated from `mem`
@@ -29,50 +38,52 @@ struct RexSim {
     double* ep_summary = nullptr;      // [4] count, nonfinite, sum of scores, sum of lengths (rexsim_episode_summary)
     bool rt_set = false;
     int32_t* perm = nullptr;           // slot -> env, sorted by solver cost; P.perm points here after rexsim_rebalance (at once with
-                                       // per-env terrains: plane envs in slots [0, nplane), heightfield envs after them)
-    int32_t* hist = nullptr;           // rexsim_rebalance's bins: 256, 512 with per-env terrains (terrain-major)
+                                       // several launch groups: each group's envs in its slot range)
+    int32_t* hist = nullptr;           // rexsim_rebalance's bins: 256 per launch group (group-major)
     float* act = nullptr;              // staging for rexsim_step_host
     uint8_t* out = nullptr;            // obs | reward | done (same layout as the host block)
     uint8_t* fin = nullptr;            // final obs | limit staging for rexsim_step_host_final (allocated on its first call)
     int A = 0;
     bool started = false;              // a reset or step has been enqueued: the frame wrappers can no longer be switched on
-    int nholds = 0;                    // hold settings (motor_kp, motor_kd, pd_latency) of P.ev.gains / P.el.hold (0: no table)
+    int nholds = 0;                    // hold settings (motor_kp, motor_kd, pd_latency, solver_iterations) of P.ev.gains /
+                                       // P.el.hold (0: no table)
+    std::vector<int32_t> hold_iters;   // [nholds] PGS cap of each hold setting, each cap's settings contiguous
     bool values_on = false;            // rexsim_set_env_values was called
     std::vector<float> kp, kd;         // per-env gains given to rexsim_set_env_values (empty: the config's)
     std::vector<double> pd;            // per-env pd latencies given to rexsim_set_env_latencies (empty: the config's)
     double* latency = nullptr;         // [2][N] per-env control and pd latencies (rexsim_set_env_latencies; null: off)
     uint8_t* terrain = nullptr;        // [N] per-env terrains (rexsim_set_env_terrains; null: off); P.env_terrain points here
-    int nplane = 0;                    // envs on the plane (per-env terrains)
+    std::vector<uint8_t> terr;         // the same on the host (empty: the config's)
     float friction[2] = {0.f, 0.f};    // per-env terrains: friction of each terrain's envs, plane and heightfield
+    int32_t* repeats = nullptr;        // [2][N] per-env action_repeat, solver_iterations (rexsim_set_env_repeats; null: off)
+    std::vector<int32_t> rep, iters;   // the same on the host (empty: the config's)
+    // The launch groups (empty: one launch over every slot with the config's values), terrain-major, plane first, then in
+    // order of first appearance; group g owns slots perm[first_g, first_g + count_g).  `group` is each env's group, the key
+    // rexsim_rebalance sorts on: its own [N] bytes with per-env repeats; the terrain bytes without them, as the groups are then
+    // the two terrains; null for a batch of one group.
+    std::vector<LaunchGroup> groups;
+    const uint8_t* group = nullptr;
+    uint8_t* group_bytes = nullptr;
     int64_t launches = 0;
     int32_t launched[3] = {0, 0, 0};   // step_kernel instance of the last step launch: BLOCK, OCC, SENSOR
-    int32_t group_launched[2][3] = {}; // per-env terrains: the same of the last launch over each terrain's slot range
 };
 
-// The handle's Params for the launches over one terrain's envs: the config's terrain and friction are that terrain's
-static Params terrain_params(const RexSim* s, Params P, int terrain) {
-    if (s->terrain) { P.cfg.terrain = terrain; P.cfg.friction = s->friction[terrain]; }
+// The handle's Params for the launches over one group's envs: its terrain with that terrain's friction, its sub-steps per
+// control step and its PGS cap
+static Params group_params(const RexSim* s, Params P, const LaunchGroup& g) {
+    if (s->terrain) P.cfg.friction = s->friction[g.terrain];
+    P.cfg.terrain = g.terrain; P.cfg.action_repeat = g.repeat; P.cfg.solver_iterations = g.iters;
     return P;
 }
-// envs on each terrain (every env on the config's terrain without per-env terrains)
-static void terrain_counts(const RexSim* s, int count[2]) {
-    count[0] = count[1] = 0;
-    if (s->terrain) { count[REXSIM_TERRAIN_PLANE] = s->nplane; count[REXSIM_TERRAIN_RANDOM] = s->P.N - s->nplane; }
-    else count[s->P.cfg.terrain] = s->P.N;
-}
-// One control step of every env: one launch over every slot, or with per-env terrains one launch per terrain over its slot
-// range of the permutation (plane [0, nplane), heightfield [nplane, N)), each choosing its build from its own size; a range
-// with no envs launches nothing.  Both on `st`, so a captured graph holds both.
+// One control step of every env: one launch over every slot, or one launch per launch group over its slot range of the
+// permutation, each choosing its build from its own size.  All on `st`, so a captured graph holds them all.
 static int step_launches(RexSim* s, const Params& P, cudaStream_t st) {
-    if (!s->terrain) return enqueue(s, launch_step(P, st), "step launch");
-    int count[2];
-    terrain_counts(s, count);
-    for (int t = 0, first = 0; t < 2; first += count[t], t++) {
-        if (!count[t]) continue;
-        Params G = terrain_params(s, P, t);
-        G.perm = P.perm + first; G.nslots = count[t]; G.launched = s->group_launched[t];
+    if (s->groups.empty()) return enqueue(s, launch_step(P, st), "step launch");
+    for (LaunchGroup& g : s->groups) {
+        Params G = group_params(s, P, g);
+        G.perm = P.perm + g.first; G.nslots = g.count; G.launched = g.launched;
         if (int rc = enqueue(s, launch_step(G, st), "step launch")) return rc;
-        memcpy(s->launched, s->group_launched[t], sizeof(s->launched));
+        memcpy(s->launched, g.launched, sizeof(s->launched));
     }
     return REXSIM_OK;
 }
@@ -230,7 +241,7 @@ int rexsim_create(const RexSimConfig* cfg, const float* model_tables, int32_t n_
     P.model = model; P.snap_f = snap_f; P.snap_i = snap_i; P.field_zoff = zoff;
     P.launched = s->launched;
     // settled reset snapshots: Rex.Reset's 100 + 0.5/dt holding sub-steps (rex.py:314-323), once per field
-    if ((rc = enqueue(s, launch_settle(P, snap_f, snap_i, 1, 0), "settle launch"))) return rc;
+    if ((rc = enqueue(s, launch_settle(P, snap_f, snap_i, 0, 1, 0), "settle launch"))) return rc;
     CK(cudaDeviceSynchronize());
     guard.s = nullptr;
     *out = s;
@@ -331,8 +342,8 @@ int rexsim_step_host_final(RexSim* s, const float* h_actions, void* h_out, void*
 
 int rexsim_rebalance(RexSim* s, void* stream) {
     if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
-    const int rc = enqueue(s, launch_rebalance(s->P.cost, s->terrain, s->P.N, s->hist, s->perm, (cudaStream_t)stream),
-                           "rebalance launch", 3);
+    const int rc = enqueue(s, launch_rebalance(s->P.cost, s->group, (int)s->groups.size(), s->P.N, s->hist, s->perm,
+                                               (cudaStream_t)stream), "rebalance launch", 3);
     if (rc == REXSIM_OK) s->P.perm = s->perm;   // steps enqueued after this call use the new grouping
     return rc;
 }
@@ -469,30 +480,89 @@ int rexsim_value_row(const char* keyword) {
         if (!strcmp(keyword, c_value_keywords[r])) return r;
     return -1;
 }
-// The reset hold's settings: each env's (motor_kp, motor_kd, pd_latency), distinct ones in order of first appearance, and each
-// env's index into them.  Rex.Reset clears the history and holds through ApplyAction (rex.py:303-323), so the settled state
-// depends on the gains and on the PD observation's latency.  kp, kd, pd: per env, or empty for the config's scalar.
-struct HoldTable { std::vector<float> gains; std::vector<double> pd; std::vector<int32_t> index; };
+// The reset hold's settings: each env's (motor_kp, motor_kd, pd_latency, solver_iterations), distinct ones in order of first
+// appearance within each PGS cap, the caps in order of first appearance (each cap's settings contiguous), and each env's index
+// into them.  Rex.Reset clears the history and holds through ApplyAction (rex.py:303-323), so the settled state depends on the
+// gains, on the PD observation's latency and on the solver's cap.  kp, kd, pd, iters: per env, or empty for the config's scalar.
+struct HoldTable { std::vector<float> gains; std::vector<double> pd; std::vector<int32_t> iters, index; };
 static int hold_table(const RexSimConfig& c, size_t N, const std::vector<float>& kp, const std::vector<float>& kd,
-                      const std::vector<double>& pd, HoldTable& t) {
+                      const std::vector<double>& pd, const std::vector<int32_t>& iters, HoldTable& t) {
     t.index.assign(N, 0);
+    std::vector<int32_t> caps;
     for (size_t e = 0; e < N; e++) {
-        const float k = kp.empty() ? c.motor_kp : kp[e], d = kd.empty() ? c.motor_kd : kd[e];
-        const double l = pd.empty() ? c.pd_latency : pd[e];
-        size_t h = 0;
-        while (h < t.pd.size() && !(t.gains[2 * h] == k && t.gains[2 * h + 1] == d && t.pd[h] == l)) h++;
-        if (h == t.pd.size()) {
-            if ((int)h == REXSIM_MAX_GAIN_PAIRS)
-                return fail(REXSIM_ERR_INVALID, "more than 64 distinct reset-hold settings (motor_kp, motor_kd, pd_latency)");
-            t.gains.push_back(k); t.gains.push_back(d); t.pd.push_back(l);
-        }
-        t.index[e] = (int32_t)h;
+        const int32_t it = iters.empty() ? c.solver_iterations : iters[e];
+        if (std::find(caps.begin(), caps.end(), it) == caps.end()) caps.push_back(it);
     }
+    for (const int32_t cap : caps)
+        for (size_t e = 0; e < N; e++) {
+            const int32_t it = iters.empty() ? c.solver_iterations : iters[e];
+            if (it != cap) continue;
+            const float k = kp.empty() ? c.motor_kp : kp[e], d = kd.empty() ? c.motor_kd : kd[e];
+            const double l = pd.empty() ? c.pd_latency : pd[e];
+            size_t h = 0;
+            while (h < t.pd.size() && !(t.gains[2 * h] == k && t.gains[2 * h + 1] == d && t.pd[h] == l && t.iters[h] == it)) h++;
+            if (h == t.pd.size()) {
+                if ((int)h == REXSIM_MAX_GAIN_PAIRS)
+                    return fail(REXSIM_ERR_INVALID, "more than 64 distinct reset-hold settings (motor_kp, motor_kd, pd_latency, solver_iterations)");
+                t.gains.push_back(k); t.gains.push_back(d); t.pd.push_back(l); t.iters.push_back(it);
+            }
+            t.index[e] = (int32_t)h;
+        }
+    return REXSIM_OK;
+}
+static int terrain_of(const RexSim* s, size_t e) { return s->terr.empty() ? s->P.cfg.terrain : s->terr[e]; }
+// the launch groups a step launches: the table, or for a batch without one its single group over every slot
+static std::vector<LaunchGroup> launch_groups(const RexSim* s) {
+    if (!s->groups.empty()) return s->groups;
+    const RexSimConfig& c = s->P.cfg;
+    return {LaunchGroup{c.terrain, c.action_repeat, c.solver_iterations, 0, s->P.N, {s->launched[0], s->launched[1], s->launched[2]}}};
+}
+// Rebuild the launch groups from each env's terrain and control rate: put each group's envs in its slot range, in env order,
+// and give rexsim_rebalance the group key.  Synchronous.
+static int build_groups(RexSim* s) {
+    Params& P = s->P;
+    const size_t N = P.N;
+    std::vector<LaunchGroup> gs;
+    std::vector<uint8_t> key(N);
+    for (const int t : {REXSIM_TERRAIN_PLANE, REXSIM_TERRAIN_RANDOM})
+        for (size_t e = 0; e < N; e++) {
+            if (terrain_of(s, e) != t) continue;
+            const int32_t r = s->rep.empty() ? P.cfg.action_repeat : s->rep[e];
+            const int32_t it = s->iters.empty() ? P.cfg.solver_iterations : s->iters[e];
+            size_t g = 0;
+            while (g < gs.size() && !(gs[g].terrain == t && gs[g].repeat == r && gs[g].iters == it)) g++;
+            if (g == gs.size()) gs.push_back(LaunchGroup{t, r, it, 0, 0, {0, 0, 0}});
+            gs[g].count++;
+            key[e] = (uint8_t)g;
+        }
+    std::vector<int32_t> at(gs.size()), perm(N);
+    for (size_t g = 1; g < gs.size(); g++) gs[g].first = gs[g - 1].first + gs[g - 1].count;
+    for (size_t g = 0; g < gs.size(); g++) at[g] = gs[g].first;
+    for (size_t e = 0; e < N; e++) perm[at[key[e]]++] = (int32_t)e;
+    CK(cudaMemcpy(s->perm, perm.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
+    P.perm = s->perm;                          // the partition holds from the first step on
+    s->mem.drop(s->group_bytes);
+    s->group_bytes = nullptr;
+    s->group = nullptr;
+    if (gs.size() > 1) {
+        int32_t* hist = nullptr;
+        if (s->mem.zeroed(&hist, 256 * gs.size())) return REXSIM_ERR_CUDA;
+        s->mem.drop(s->hist);
+        s->hist = hist;
+        if (!s->repeats) {
+            s->group = s->terrain;             // the groups are the two terrains: group g is terrain g
+        } else {
+            if (s->mem.zeroed(&s->group_bytes, N)) return REXSIM_ERR_CUDA;
+            CK(cudaMemcpy(s->group_bytes, key.data(), N, cudaMemcpyHostToDevice));
+            s->group = s->group_bytes;
+        }
+    }
+    s->groups = gs;
     return REXSIM_OK;
 }
 // Run the reset hold again for every snapshot of the layout P.snaps, at the handle's hold settings (the config's one without a
-// table), its sensor history rows at the handle's ring depth: one launch per terrain the batch has, each at that terrain's
-// friction, over all its (setting, field) snapshots.  Synchronous.
+// table), its sensor history rows at the handle's ring depth: one launch per (terrain, PGS cap) the launch groups hold, each
+// at that terrain's friction and with that cap, over all the cap's (setting, field) snapshots.  Synchronous.
 static int settle_snapshots(RexSim* s) {
     Params& P = s->P;
     const int nh = s->nholds > 0 ? s->nholds : 1;
@@ -507,11 +577,17 @@ static int settle_snapshots(RexSim* s) {
         P.snap_ring = nullptr;
         if (s->mem.zeroed(&P.snap_ring, nsettle * P.ring_depth * sensor_cfg(&P.cfg).words)) return REXSIM_ERR_CUDA;
     }
-    int count[2];
-    terrain_counts(s, count);
-    for (int t = 0; t < 2; t++)
-        if (count[t])
-            if (int rc = enqueue(s, launch_settle(terrain_params(s, P, t), snap_f, snap_i, nh, 0), "settle launch")) return rc;
+    const std::vector<int32_t> caps = s->nholds > 0 ? s->hold_iters : std::vector<int32_t>{P.cfg.solver_iterations};
+    const std::vector<LaunchGroup> gs = launch_groups(s);
+    for (size_t g = 0; g < gs.size(); g++) {
+        bool settled = false;                  // an earlier group on the same terrain with the same cap
+        for (size_t h = 0; h < g; h++) settled = settled || (gs[h].terrain == gs[g].terrain && gs[h].iters == gs[g].iters);
+        if (settled) continue;
+        const int first = (int)(std::find(caps.begin(), caps.end(), gs[g].iters) - caps.begin());
+        const int count = (int)std::count(caps.begin(), caps.end(), gs[g].iters);
+        const Params G = group_params(s, P, gs[g]);
+        if (int rc = enqueue(s, launch_settle(G, snap_f, snap_i, first, count, 0), "settle launch")) return rc;
+    }
     CK(cudaDeviceSynchronize());
     return REXSIM_OK;
 }
@@ -537,6 +613,7 @@ static int apply_holds(RexSim* s, const HoldTable& t, bool settle) {
         P.el.hold = dhold;
     }
     s->nholds = (int)nh;
+    s->hold_iters = t.iters;
     return settle ? settle_snapshots(s) : REXSIM_OK;
 }
 int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const float* kd) {
@@ -557,9 +634,9 @@ int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const
         for (size_t e = 0; e < N; e++)
             if (!(kp[e] >= 0.f) || !(kd[e] >= 0.f) || std::isinf(kp[e]) || std::isinf(kd[e]))
                 return fail(REXSIM_ERR_INVALID, "gains must be finite and non-negative");
-        if (int rc = hold_table(c, N, std::vector<float>(kp, kp + N), std::vector<float>(kd, kd + N), s->pd, t)) return rc;
+        if (int rc = hold_table(c, N, std::vector<float>(kp, kp + N), std::vector<float>(kd, kd + N), s->pd, s->iters, t)) return rc;
     } else if (!P.ev.pair) {
-        if (int rc = hold_table(c, N, s->kp, s->kd, s->pd, t)) return rc;          // the config's one setting
+        if (int rc = hold_table(c, N, s->kp, s->kd, s->pd, s->iters, t)) return rc;          // the config's one setting
     }
     float* block = nullptr;
     if (s->mem.zeroed(&block, (size_t)REXSIM_VALUE_BLOCK_ROWS * N)) return REXSIM_ERR_CUDA;
@@ -601,7 +678,7 @@ int rexsim_set_env_latencies(RexSim* s, const double* control_latency, const dou
     }
     HoldTable t;
     const std::vector<double> pd(lat.begin() + N, lat.end());
-    if (int rc = hold_table(c, N, s->kp, s->kd, pd, t)) return rc;
+    if (int rc = hold_table(c, N, s->kp, s->kd, pd, s->iters, t)) return rc;
     double* dlat = nullptr;
     EnvDelay* denv = nullptr;
     if (s->mem.zeroed(&dlat, 2 * N) || s->mem.zeroed(&denv, N)) return REXSIM_ERR_CUDA;
@@ -635,41 +712,86 @@ int rexsim_set_env_terrains(RexSim* s, const int32_t* terrain, float plane_frict
     if (!(plane_friction >= 0.f) || std::isinf(plane_friction)) return fail(REXSIM_ERR_INVALID, "plane friction must be finite and non-negative");
     const size_t N = P.N;
     std::vector<uint8_t> bytes(N);
-    std::vector<int32_t> perm;
-    perm.reserve(N);
+    size_t nplane = 0;
     for (size_t e = 0; e < N; e++) {
         if (terrain[e] != REXSIM_TERRAIN_PLANE && terrain[e] != REXSIM_TERRAIN_RANDOM)
             return fail(REXSIM_ERR_INVALID, "terrain entries must be REXSIM_TERRAIN_PLANE or REXSIM_TERRAIN_RANDOM");
         bytes[e] = (uint8_t)terrain[e];
-        if (terrain[e] == REXSIM_TERRAIN_PLANE) perm.push_back((int32_t)e);
+        nplane += terrain[e] == REXSIM_TERRAIN_PLANE;
     }
-    const int nplane = (int)perm.size();
-    for (size_t e = 0; e < N; e++) if (bytes[e] == REXSIM_TERRAIN_RANDOM) perm.push_back((int32_t)e);
     uint8_t* dterrain = nullptr;
-    int32_t* hist = nullptr;
-    if (s->mem.zeroed(&dterrain, N) || s->mem.zeroed(&hist, 512)) return REXSIM_ERR_CUDA;
+    if (s->mem.zeroed(&dterrain, N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(dterrain, bytes.data(), N, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(s->perm, perm.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
-    s->mem.drop(s->hist);
-    s->hist = hist;
-    s->terrain = dterrain; s->nplane = nplane;
+    s->terrain = dterrain; s->terr = bytes;
     s->friction[REXSIM_TERRAIN_PLANE] = plane_friction; s->friction[REXSIM_TERRAIN_RANDOM] = P.cfg.friction;
     P.env_terrain = dterrain;
-    P.perm = s->perm;                          // the partition holds from the first step on
-    P.snaps = snap_layout(nplane > 0, nplane < (int)N, P.cfg.nfields);
+    P.snaps = snap_layout(nplane > 0, nplane < N, P.cfg.nfields);
+    if (int rc = build_groups(s)) return rc;
     return settle_snapshots(s);
 }
 int rexsim_env_terrain_buffers(RexSim* s, uint8_t** terrain, int32_t* nplane) {
     if (!s || !terrain || !nplane) return fail(REXSIM_ERR_INVALID, "null argument");
     if (!s->terrain) return fail(REXSIM_ERR_INVALID, "per-env terrains are off (rexsim_set_env_terrains)");
-    *terrain = s->terrain; *nplane = s->nplane;
+    *terrain = s->terrain;
+    *nplane = 0;
+    for (const LaunchGroup& g : s->groups) if (g.terrain == REXSIM_TERRAIN_PLANE) *nplane += g.count;
+    return REXSIM_OK;
+}
+int rexsim_set_env_repeats(RexSim* s, const int32_t* action_repeat, const int32_t* solver_iterations) {
+    if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
+    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env repeats must be set before the first reset or step");
+    if (s->repeats) return fail(REXSIM_ERR_INVALID, "per-env repeats are already set");
+    Params& P = s->P;
+    const RexSimConfig& c = P.cfg;
+    const size_t N = P.N;
+    std::vector<int32_t> rep(N), iters(N);
+    std::vector<std::pair<int32_t, int32_t>> pairs;
+    for (size_t e = 0; e < N; e++) {
+        rep[e] = action_repeat ? action_repeat[e] : c.action_repeat;
+        iters[e] = solver_iterations ? solver_iterations[e] : c.solver_iterations;
+        if (rep[e] <= 0 || iters[e] <= 0) return fail(REXSIM_ERR_INVALID, "action_repeat and solver_iterations must be positive");
+        if (std::find(pairs.begin(), pairs.end(), std::make_pair(rep[e], iters[e])) == pairs.end()) {
+            if ((int)pairs.size() == REXSIM_MAX_REPEAT_PAIRS)
+                return fail(REXSIM_ERR_INVALID, "more than 8 distinct (action_repeat, solver_iterations) pairs");
+            pairs.push_back(std::make_pair(rep[e], iters[e]));
+        }
+    }
+    HoldTable t;
+    if (int rc = hold_table(c, N, s->kp, s->kd, s->pd, iters, t)) return rc;
+    int32_t* d = nullptr;
+    if (s->mem.zeroed(&d, 2 * N)) return REXSIM_ERR_CUDA;
+    CK(cudaMemcpy(d, rep.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d + N, iters.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
+    s->repeats = d; s->rep = rep; s->iters = iters;
+    if (int rc = build_groups(s)) return rc;
+    return apply_holds(s, t, true);
+}
+int rexsim_env_repeat_buffers(RexSim* s, int32_t** repeats) {
+    if (!s || !repeats) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (!s->repeats) return fail(REXSIM_ERR_INVALID, "per-env repeats are off (rexsim_set_env_repeats)");
+    *repeats = s->repeats;
+    return REXSIM_OK;
+}
+int rexsim_launch_groups(const RexSim* s) { return s ? (int)launch_groups(s).size() : 0; }
+int rexsim_launch_group(const RexSim* s, int32_t g, int32_t* info) {
+    if (!s || !info) return fail(REXSIM_ERR_INVALID, "null argument");
+    const std::vector<LaunchGroup> gs = launch_groups(s);
+    if (g < 0 || g >= (int32_t)gs.size()) return fail(REXSIM_ERR_INVALID, "no such launch group");
+    const LaunchGroup& G = gs[g];
+    const int32_t w[REXSIM_GROUP_WORDS] = {G.terrain, G.repeat, G.iters, G.first, G.count, G.launched[0], G.launched[1], G.launched[2]};
+    memcpy(info, w, sizeof(w));
+    return REXSIM_OK;
+}
+int rexsim_slot_buffers(RexSim* s, int32_t** perm, uint8_t** group) {
+    if (!s || !perm || !group) return fail(REXSIM_ERR_INVALID, "null argument");
+    *perm = const_cast<int32_t*>(s->P.perm); *group = const_cast<uint8_t*>(s->group);
     return REXSIM_OK;
 }
 int rexsim_last_terrain_build(const RexSim* s, int32_t terrain, int32_t* cta_threads, int32_t* ctas_per_sm, int32_t* sensor) {
     if (!s || !cta_threads || !ctas_per_sm || !sensor) return fail(REXSIM_ERR_INVALID, "null argument");
     if (terrain != REXSIM_TERRAIN_PLANE && terrain != REXSIM_TERRAIN_RANDOM) return fail(REXSIM_ERR_INVALID, "terrain type");
-    static const int32_t none[3] = {0, 0, 0};
-    const int32_t* b = s->terrain ? s->group_launched[terrain] : terrain == s->P.cfg.terrain ? s->launched : none;
+    int32_t b[3] = {0, 0, 0};
+    for (const LaunchGroup& g : launch_groups(s)) if (g.terrain == terrain) memcpy(b, g.launched, sizeof(b));
     *cta_threads = b[0]; *ctas_per_sm = b[1]; *sensor = b[2];
     return REXSIM_OK;
 }

@@ -1871,7 +1871,7 @@ __device__ __forceinline__ bool write_obs(const Params& P, int env, int leg, con
 // 4 -> 128 registers (16 warps/SM hide the serial PGS / ABA chains, large batches)
 // SENSOR: the observation-history / latency / noise model of Rex (rex.py:726-769) is compiled in (any latency or noise > 0);
 // the default build reads the true state and keeps no history.
-// RANGE: the launch covers one terrain's slot range of a batch of both terrains, perm[0, nslots) (rexsim_set_env_terrains);
+// RANGE: the launch covers one launch group's slot range of a split batch, perm[0, nslots) (per-env terrains or rates);
 // otherwise every slot of the batch.  A bound read in the single-terrain builds re-schedules their sub-step (6.5 % slower on the
 // headline build, H100), so it is compiled in only where it is needed.
 // heightfield tiles, (BLOCK / 4) x TILE_FLOATS floats (random terrain only), then (BLOCK / 4) x PGS_ENV_FLOATS (replicated PGS only)
@@ -2115,11 +2115,12 @@ __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_o
 // -------------------------------------------------------------------------------------------------
 // settle kernel: Rex.Reset (rex.py:296-324) for every snapshot, one per 4-lane group: 100 sub-steps holding 'stand'
 // then reset_time/dt holding the task's init pose; writes the snapshot row.  Group j of a launch settles the TERRAIN
-// snapshot (pair = j / fields, field = j % fields) of the layout P.snaps; it holds at the gains of its pair, and with per-env
-// latencies reads the PD observation at its setting's pd_latency.  P.cfg's friction is the terrain's.
+// snapshot (pair = first + j / fields, field = j % fields) of the layout P.snaps; it holds at the gains of its pair, and with
+// per-env latencies reads the PD observation at its setting's pd_latency.  P.cfg's friction and PGS cap are the launch's.
 // -------------------------------------------------------------------------------------------------
 template <int TERRAIN, bool ARM, bool SENSOR>
-__global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_f, int32_t* snap_i, int nsettle, int signal, int task) {
+__global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_f, int32_t* snap_i, int first, int nsettle, int signal,
+                                                     int task) {
     __shared__ __align__(16) float sm[ARM ? REXSIM_MT_FLOATS_ARM : REXSIM_MT_FLOATS];
     __shared__ __align__(8) uint64_t bar;
     __shared__ float tiles[TERRAIN == REXSIM_TERRAIN_RANDOM ? 8 * TILE_FLOATS : 1];
@@ -2128,7 +2129,7 @@ __global__ void __launch_bounds__(32) settle_kernel(const Params P, float* snap_
     const int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 2;
     if (j >= nsettle) return;         // whole 4-lane groups leave: no shuffle or barrier spans groups after the table load
     const int nfield = terrain_snapshots(TERRAIN, P.cfg.nfields);
-    const int field = j % nfield, pair = j / nfield;
+    const int field = j % nfield, pair = first + j / nfield;
     const int snap = snapshot_index(P.snaps, pair, TERRAIN, field);
     const float kp = P.ev.gains ? P.ev.gains[2 * pair] : P.cfg.motor_kp, kd = P.ev.gains ? P.ev.gains[2 * pair + 1] : P.cfg.motor_kd;
     Lane L; Task K;
@@ -2230,7 +2231,7 @@ static cudaError_t launch_step_tsta(const Params& P, cudaStream_t st) {
     // Beyond one wave of 2-CTA/SM residency (128-thread CTAs; two waves on heightfields): the 128-register build (16 warps/SM
     // hide the serial ABA / PGS chains) in larger CTAs; below that the 255-register build, lowest single-wave latency
     // (DESIGN.md section 5).  Arm batches stay on the 255-register build: at 128 registers the arm's working set spills 4 KB.
-    // A batch of both terrains chooses per launch, from the size of that terrain's slot range.
+    // A batch of several launch groups chooses per launch, from the size of that group's slot range.
     bool big = !ARM && (P.nslots * 4 + 127) / 128 > (TERRAIN == REXSIM_TERRAIN_PLANE ? 2 : 4) * P.sm_count;
     if (const char* f = getenv("REXSIM_FORCE_BUILD")) big = !ARM && f[0] == 'b';      // developer A/B: "big" / "small"
     if (big) return launch_step_variant<TASK, SIGNAL, TERRAIN, ARM ? 1 : REXSIM_OCC_BIG, ARM, false, ARM ? REXSIM_BLOCK : REXSIM_BLOCK_BIG>(P, st);
@@ -2291,36 +2292,45 @@ __global__ void set_state_kernel(const Params P, const float* in_f) {
 }
 
 // ---- warp re-grouping: counting sort of the envs by solver cost, most expensive first (they start first: LPT order) ----
-// With per-env terrains the key is (terrain, cost bin): the plane envs keep slots [0, Np), the heightfield envs [Np, N).
-__device__ __forceinline__ int rebalance_bin(const int32_t* __restrict__ cost, const uint8_t* __restrict__ terrain, int e) {
+// With several launch groups the key is (group, cost bin): group g keeps its slot range [first_g, first_g + count_g).
+__device__ __forceinline__ int rebalance_bin(const int32_t* __restrict__ cost, const uint8_t* __restrict__ group, int e) {
     const int b = 255 - min(cost[e] >> 1, 255);
-    return terrain ? (int)terrain[e] * 256 + b : b;
+    return group ? (int)group[e] * 256 + b : b;
 }
-__global__ void rebalance_hist_kernel(const int32_t* __restrict__ cost, const uint8_t* __restrict__ terrain, int n, int32_t* __restrict__ hist) {
+__global__ void rebalance_hist_kernel(const int32_t* __restrict__ cost, const uint8_t* __restrict__ group, int n, int32_t* __restrict__ hist) {
     int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e < n) atomicAdd(&hist[rebalance_bin(cost, terrain, e)], 1);
+    if (e < n) atomicAdd(&hist[rebalance_bin(cost, group, e)], 1);
 }
-__global__ void rebalance_scan_kernel(int32_t* hist) {          // 1 block, one thread per bin (256 or 512): exclusive prefix sum in place
-    __shared__ int32_t s[512];
-    const int t = threadIdx.x;
-    s[t] = hist[t];
+constexpr int REBALANCE_MAX_BINS = 4096, REBALANCE_SCAN_THREADS = 1024;
+// 1 block: exclusive prefix sum of `bins` bins in place, thread t owning bins [t * per, (t + 1) * per).  Up to 1024 bins it is
+// one thread per bin (per = 1).
+__global__ void rebalance_scan_kernel(int32_t* hist, int bins, int per) {
+    __shared__ int32_t s[REBALANCE_SCAN_THREADS];
+    const int t = threadIdx.x, b0 = t * per;
+    int32_t own = 0;
+    for (int i = 0; i < per; i++) own += b0 + i < bins ? hist[b0 + i] : 0;
+    s[t] = own;
     __syncthreads();
     for (int o = 1; o < (int)blockDim.x; o <<= 1) { int v = t >= o ? s[t - o] : 0; __syncthreads(); s[t] += v; __syncthreads(); }
-    hist[t] = s[t] - hist[t];
+    int32_t at = s[t] - own;
+    for (int i = 0; i < per && b0 + i < bins; i++) { const int32_t h = hist[b0 + i]; hist[b0 + i] = at; at += h; }
 }
-__global__ void rebalance_scatter_kernel(const int32_t* __restrict__ cost, const uint8_t* __restrict__ terrain, int n,
+__global__ void rebalance_scatter_kernel(const int32_t* __restrict__ cost, const uint8_t* __restrict__ group, int n,
                                          int32_t* __restrict__ offs, int32_t* __restrict__ perm) {
     int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e < n) perm[atomicAdd(&offs[rebalance_bin(cost, terrain, e)], 1)] = e;
+    if (e < n) perm[atomicAdd(&offs[rebalance_bin(cost, group, e)], 1)] = e;
 }
-// hist: [256] bins, [512] with per-env terrains (terrain not null)
-cudaError_t launch_rebalance(const int32_t* cost, const uint8_t* terrain, int n, int32_t* hist, int32_t* perm, cudaStream_t st) {
-    const int bins = terrain ? 512 : 256;
+// group: [n] launch group of each env, null for a batch of one group; hist: [ngroups * 256] bins
+cudaError_t launch_rebalance(const int32_t* cost, const uint8_t* group, int ngroups, int n, int32_t* hist, int32_t* perm,
+                             cudaStream_t st) {
+    const int bins = (group ? ngroups : 1) * 256;
+    if (bins > REBALANCE_MAX_BINS) return cudaErrorInvalidValue;
+    const int per = (bins + REBALANCE_SCAN_THREADS - 1) / REBALANCE_SCAN_THREADS, threads = (bins + per - 1) / per;
     cudaError_t e = cudaMemsetAsync(hist, 0, bins * sizeof(int32_t), st);
     if (e != cudaSuccess) return e;
-    rebalance_hist_kernel<<<(n + 255) / 256, 256, 0, st>>>(cost, terrain, n, hist);
-    rebalance_scan_kernel<<<1, bins, 0, st>>>(hist);
-    rebalance_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(cost, terrain, n, hist, perm);
+    rebalance_hist_kernel<<<(n + 255) / 256, 256, 0, st>>>(cost, group, n, hist);
+    rebalance_scan_kernel<<<1, threads, 0, st>>>(hist, bins, per);
+    rebalance_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(cost, group, n, hist, perm);
     return cudaGetLastError();
 }
 
@@ -2377,21 +2387,21 @@ cudaError_t launch_reset(const Params& P, float* obs_out, cudaStream_t st) {
     return cudaGetLastError();
 }
 template <int TERRAIN, bool ARM>
-static void launch_settle_ta(const Params& P, float* snap_f, int32_t* snap_i, int nsettle, cudaStream_t st) {
+static void launch_settle_ta(const Params& P, float* snap_f, int32_t* snap_i, int first, int nsettle, cudaStream_t st) {
     const int blocks = (nsettle + 7) / 8;                 // 8 snapshots per 32-thread CTA
-    if (P.sensor_on) settle_kernel<TERRAIN, ARM, true><<<blocks, 32, 0, st>>>(P, snap_f, snap_i, nsettle, P.cfg.signal, P.cfg.task);
-    else settle_kernel<TERRAIN, ARM, false><<<blocks, 32, 0, st>>>(P, snap_f, snap_i, nsettle, P.cfg.signal, P.cfg.task);
+    if (P.sensor_on) settle_kernel<TERRAIN, ARM, true><<<blocks, 32, 0, st>>>(P, snap_f, snap_i, first, nsettle, P.cfg.signal, P.cfg.task);
+    else settle_kernel<TERRAIN, ARM, false><<<blocks, 32, 0, st>>>(P, snap_f, snap_i, first, nsettle, P.cfg.signal, P.cfg.task);
 }
-// the snapshots of `npairs` hold settings on P.cfg.terrain (one terrain per launch)
-cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, int npairs, cudaStream_t st) {
+// the snapshots of hold settings [first, first + npairs) on P.cfg.terrain (one terrain per launch), at P.cfg's PGS cap
+cudaError_t launch_settle(const Params& P, float* snap_f, int32_t* snap_i, int first, int npairs, cudaStream_t st) {
     const bool arm = P.cfg.num_motors == 18;
     const int nsettle = npairs * terrain_snapshots(P.cfg.terrain, P.cfg.nfields);
     if (P.cfg.terrain == REXSIM_TERRAIN_PLANE) {
-        if (arm) launch_settle_ta<REXSIM_TERRAIN_PLANE, true>(P, snap_f, snap_i, nsettle, st);
-        else launch_settle_ta<REXSIM_TERRAIN_PLANE, false>(P, snap_f, snap_i, nsettle, st);
+        if (arm) launch_settle_ta<REXSIM_TERRAIN_PLANE, true>(P, snap_f, snap_i, first, nsettle, st);
+        else launch_settle_ta<REXSIM_TERRAIN_PLANE, false>(P, snap_f, snap_i, first, nsettle, st);
     } else {
-        if (arm) launch_settle_ta<REXSIM_TERRAIN_RANDOM, true>(P, snap_f, snap_i, nsettle, st);
-        else launch_settle_ta<REXSIM_TERRAIN_RANDOM, false>(P, snap_f, snap_i, nsettle, st);
+        if (arm) launch_settle_ta<REXSIM_TERRAIN_RANDOM, true>(P, snap_f, snap_i, first, nsettle, st);
+        else launch_settle_ta<REXSIM_TERRAIN_RANDOM, false>(P, snap_f, snap_i, first, nsettle, st);
     }
     return cudaGetLastError();
 }

@@ -139,7 +139,7 @@ struct Params {
     const int32_t* __restrict__ snap_i;// [settings * snaps.per_setting][NI]
     SnapLayout snaps;
     // per-env terrains (rexsim_set_env_terrains; null: every env on cfg.terrain): [N] REXSIM_TERRAIN_* by env.  The step
-    // kernel never reads it: each of its launches covers one terrain's slot range, with that terrain in cfg.terrain.
+    // kernel never reads it: each of its launches covers one launch group's slots, with the group's terrain in cfg.terrain.
     const uint8_t* __restrict__ env_terrain;
     const float* __restrict__ field_zoff; // [nfields]
     int32_t* __restrict__ err;         // [N] per-env bits of the most recent step, [N] = OR of all since last cleared
@@ -159,7 +159,7 @@ struct Params {
     const int32_t* __restrict__ reset_idx; // reset kernel: [k] or null
     int32_t reset_k;
     int32_t N;                         // envs: the stride of every per-env array
-    int32_t nslots;                    // step kernel: slots it covers, perm[0, nslots) (N, or one terrain's range of a mixed batch)
+    int32_t nslots;                    // step kernel: slots it covers, perm[0, nslots) (N, or one launch group's range)
     int32_t sm_count;                  // SMs of the device (kernel variant choice)
     int32_t* launched;                 // host: {BLOCK, OCC, SENSOR} of the step_kernel instance the last step launched (never read on the device)
     const int32_t* __restrict__ perm;  // [nslots] slot -> env (null: identity); see rexsim_rebalance

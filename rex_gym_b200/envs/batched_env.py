@@ -10,6 +10,7 @@ One call = one kernel launch for all N environments; there is no CPU fallback.
 import ctypes as C
 import functools
 import math
+import numbers
 
 import numpy as np
 import torch
@@ -97,6 +98,8 @@ TASK_VALUE_KEYWORDS = ("target_position", "backwards", "target_orient", "init_or
                        "base_y", "base_z", "base_roll", "base_pitch", "base_yaw")
 MAX_GAIN_PAIRS = 64              # REXSIM_MAX_GAIN_PAIRS: the reset hold is settled once per distinct (motor_kp, motor_kd, pd_latency)
 LATENCY_KEYWORDS = ("control_latency", "pd_latency")     # sensor latencies that also take one value per env
+RATE_KEYWORDS = ("control_time_step", "action_repeat")   # the control rate, one value per env over one simulation time step
+MAX_REPEAT_PAIRS = 8             # REXSIM_MAX_REPEAT_PAIRS: distinct (action_repeat, solver_iterations) pairs, one launch each
 
 
 def is_per_env(value):
@@ -213,6 +216,58 @@ def check_env_terrains(num_envs, terrain_type):
     return None, np.ascontiguousarray([TERRAINS[t] for t in entries], np.int32)
 
 
+def _rate_entries(name, value, n):
+    """A control_time_step / action_repeat value, scalar or per env -> a list of n Python numbers, each checked: action_repeat
+    a positive integer, control_time_step positive and finite."""
+    if is_per_env(value):
+        if isinstance(value, torch.Tensor):
+            value = value.detach().cpu().numpy()
+        a = np.asarray(list(value) if isinstance(value, (list, tuple)) else value, dtype=object)
+        if a.shape != (n,):
+            raise ValueError("%s: expected one entry per env (%d), got shape %s" % (name, n, a.shape))
+        entries = list(a)
+    else:
+        entries = [value] * n
+    for v in entries:
+        if name == "action_repeat":
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Integral) or v <= 0:
+                raise ValueError("action_repeat: %r is not a positive integer" % (v,))
+        elif isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Real) or not (math.isfinite(v) and v > 0):
+            raise ValueError("control_time_step: %r is not a positive finite number of seconds" % (v,))
+    return [int(v) if name == "action_repeat" else float(v) for v in entries]
+
+
+def check_env_repeats(num_envs, task, control_time_step, action_repeat, solver_iterations=None):
+    """The control-rate keywords, checked before any CUDA call.  control_time_step and action_repeat: a scalar (None: the
+    task's default) or one entry per env (a list, tuple or ndarray).  Env e is built as if (control_time_step[e],
+    action_repeat[e]) were the scalars, so every control_time_step[e] / action_repeat[e], in fp64 as rex_gym_env.py:173
+    computes it, must be the one simulation time step: the observation space's rate bounds are 2 pi / time step, and the
+    reference's BatchEnv refuses envs whose spaces differ.  solver_iterations: None (each env int(300 / action_repeat[e]),
+    rex_gym_env.py:184) or a scalar for every env.
+    -> (control_time_step, action_repeat, time step, None) for a scalar construction (all-equal arrays are one), else
+    (control_time_step tuple, action_repeat tuple, time step, (action_repeat, solver_iterations) int32 [num_envs] each)."""
+    n = int(num_envs)
+    if is_per_env(solver_iterations):
+        raise ValueError("solver_iterations takes one value for the batch (None: int(300 / action_repeat) per env)")
+    long_step = task in ("gallop", "poses")
+    default = lambda v, d: v if is_per_env(v) else (v or d)                  # a scalar None (or 0) takes the task's default
+    cts = _rate_entries("control_time_step", default(control_time_step, 0.006 if long_step else 0.005), n)
+    rep = _rate_entries("action_repeat", default(action_repeat, 6 if long_step else 5), n)
+    steps = sorted({c / r for c, r in zip(cts, rep)})
+    if len(steps) > 1:
+        raise ValueError("control_time_step / action_repeat: the envs' simulation time steps differ (%s s); the observation "
+                         "space's rate bounds are 2 pi / time step, so the spaces differ and the reference's BatchEnv refuses "
+                         "the mix" % ", ".join(repr(t) for t in steps[:4]))
+    if len(set(zip(cts, rep))) == 1:
+        return cts[0], rep[0], steps[0], None
+    iters = [solver_iterations or int(300 / r) for r in rep]                     # rex_gym_env.py:25,184
+    pairs = len(set(zip(rep, iters)))
+    if pairs > MAX_REPEAT_PAIRS:
+        raise ValueError("action_repeat: %d distinct (action_repeat, solver_iterations) pairs, at most %d (each is one step "
+                         "launch)" % (pairs, MAX_REPEAT_PAIRS))
+    return tuple(cts), tuple(rep), steps[0], (np.ascontiguousarray(rep, np.int32), np.ascontiguousarray(iters, np.int32))
+
+
 class _Info(object):
     """Stand-in for BatchEnv's `tuple(infos)`: info[i] == {'action': motor command of env i} of THE STEP THAT RETURNED IT
     (rex_gym_env.py:414).  The command block lives on the device and is overwritten by the next step, so the host copy is taken
@@ -296,7 +351,14 @@ class BatchedRexEnv(object):
         terrain_type: 'plane', 'random', or one of them per env (a list, tuple or ndarray of num_envs entries).  Env e of a
           batch of both runs exactly as env e of the batch built with its entry as the scalar: its own ground, friction and
           field sequence from the one num_fields bank.  Each step launches the plane envs and the heightfield envs as two slot
-          ranges of the batch, each with its terrain's kernel build.  All-equal entries build the scalar construction."""
+          ranges of the batch, each with its terrain's kernel build.  All-equal entries build the scalar construction.
+
+        control_time_step, action_repeat: each a scalar or one entry per env.  Env e runs exactly as the batch built with
+          (control_time_step[e], action_repeat[e]) as scalars: action_repeat[e] sub-steps per control step, each PGS solve
+          capped at solver_iterations (None: int(300 / action_repeat[e])).  Every control_time_step[e] / action_repeat[e]
+          must be the same simulation time step, which the observation space depends on.  Each (terrain, action_repeat,
+          solver_iterations) group of envs is one slot range of the batch, launched with its own values; at most 8 distinct
+          rates.  All-equal entries build the scalar construction."""
         if urdf_version is not None and urdf_version != DEFAULT_URDF_VERSION:
             raise ValueError("%s is not a supported urdf_version." % urdf_version)     # rex_gym_env.py:317-318
         if task not in TASKS or signal_type not in SIGNALS:
@@ -319,6 +381,7 @@ class BatchedRexEnv(object):
             motor_kp, motor_kd = float(env_gains[0][0]), float(env_gains[1][0])
         # per-env latencies: the scalar gains of a motor_kp / motor_kd range hold the reset at each distinct pd_latency
         env_latency = check_env_latencies(num_envs, control_latency, pd_latency, motor_kp, motor_kd, env_gains)
+        cts, rep, time_step, env_repeats = check_env_repeats(num_envs, task, control_time_step, action_repeat, solver_iterations)
         if not torch.cuda.is_available():
             raise RuntimeError("rex_gym_b200 needs a CUDA device: there is no CPU fallback")
         self._L = _capi.load()
@@ -329,18 +392,20 @@ class BatchedRexEnv(object):
         self.device = torch.device(device)
         self.num_envs = int(num_envs)
         self.num_motors = 12 if mark == "base" else 18
-        rep = action_repeat or (6 if task in ("gallop", "poses") else 5)
-        cts = control_time_step or (0.006 if task in ("gallop", "poses") else 0.005)
+        # the scalars for a scalar construction, else the N entries; the simulation time step is the batch's
         self.control_time_step, self._action_repeat = cts, rep
-        self._time_step = cts / rep
+        self._time_step = time_step
         if mark not in ("base", "arm"):
             raise ValueError("mark must be 'base' or 'arm'")          # mark_constants.py:1
         tables, toe_npts = pack_model_tables(mark)
         c = _capi.RexSimConfig()
         c.num_envs, c.task, c.signal = self.num_envs, TASKS[task], SIGNALS[signal_type]
         c.terrain = TERRAINS[terrain_scalar or "random"]
-        c.num_motors, c.action_repeat = self.num_motors, rep
-        c.solver_iterations = solver_iterations or int(300 / rep)                      # rex_gym_env.py:25,184
+        if env_repeats is None:
+            c.num_motors, c.action_repeat = self.num_motors, rep
+            c.solver_iterations = solver_iterations or int(300 / rep)                  # rex_gym_env.py:25,184
+        else:                                # env 0's rate in the config; rexsim_set_env_repeats gives every env its own
+            c.num_motors, c.action_repeat, c.solver_iterations = self.num_motors, int(env_repeats[0][0]), int(env_repeats[1][0])
         c.sim_dt, c.sim_dt_d = self._time_step, self._time_step
         c.motor_kp, c.motor_kd = motor_kp, motor_kd
         c.kp_lo, c.kp_hi = motor_kp_range or (motor_kp, motor_kp)
@@ -396,6 +461,9 @@ class BatchedRexEnv(object):
         self.frame_history, self.frame_delta = (list(frames) if frames else None), bool(frame_delta)
         if env_terrain is not None:
             self._call(self._L.rexsim_set_env_terrains, self._h, env_terrain.ctypes.data, friction["plane"], stream=False)
+        if env_repeats is not None:
+            self._call(self._L.rexsim_set_env_repeats, self._h, env_repeats[0].ctypes.data, env_repeats[1].ctypes.data,
+                       stream=False)
         self._values = None
         if env_values is not None:
             block = np.full((len(TASK_VALUE_KEYWORDS), self.num_envs), np.nan, np.float32)
@@ -450,6 +518,10 @@ class BatchedRexEnv(object):
             nplane = C.c_int32()
             _capi.check(self._L.rexsim_env_terrain_buffers(self._h, C.byref(p), C.byref(nplane)))
             self._terrain = view(p, (N,), "|u1")
+        self._repeats = None                 # [2][N] i32: each env's action_repeat, solver_iterations (per-env rates only)
+        if env_repeats is not None:
+            _capi.check(self._L.rexsim_env_repeat_buffers(self._h, C.byref(p)))
+            self._repeats = view(p, (2, N), "<i4")
         self._latency = None                 # [2][N] f64: each env's control_latency, pd_latency (per-env latencies only)
         if env_latency is not None:
             depth = C.c_int32()
@@ -670,9 +742,16 @@ class BatchedRexEnv(object):
             sd["env_latency"] = self._latency.clone()
         if self._terrain is not None:
             sd["env_terrain"] = self._terrain.clone()
+        if self._repeats is not None:
+            sd["env_repeats"] = self._repeats.clone()
         return sd
 
     def load_state_dict(self, sd):
+        if (self._repeats is None) != ("env_repeats" not in sd):
+            raise ValueError("per-env control rates: the checkpoint %s them, this batch %s" %
+                             (("has", "does not") if self._repeats is None else ("lacks", "has")))
+        if self._repeats is not None and not torch.equal(self._repeats, sd["env_repeats"].to(self._repeats.device)):
+            raise ValueError("per-env control rates: the checkpoint's action repeats or solver iterations differ from this batch's")
         if (self._terrain is None) != ("env_terrain" not in sd):
             raise ValueError("per-env terrains: the checkpoint %s them, this batch %s" %
                              (("has", "does not") if self._terrain is None else ("lacks", "has")))
@@ -703,14 +782,16 @@ class BatchedRexEnv(object):
     # ---- per-env task values ------------------------------------------------------------------------------
     def set_task_values(self, indices=None, **values):
         """Give the envs `indices` (default: all) new constructor values, e.g. set_task_values([0, 3], target_position=2.5)
-        or a curriculum between Rollout.collect() calls.  Keywords: those of TASK_VALUE_KEYWORDS (the gains, latencies and
-        terrains are fixed at construction), each a scalar or one value per index, meaning what it means to the constructor.
+        or a curriculum between Rollout.collect() calls.  Keywords: those of TASK_VALUE_KEYWORDS (the gains, latencies, control
+        rates and terrains are fixed at construction), each a scalar or one value per index, meaning what it means to the
+        constructor.
         Each env starts using them at its next reset, explicit or automatic.  Enqueued on the current stream without a host sync; host values are
         checked here, device tensors are not inspected.  Needs a batch built with per-env values (any of these keywords, or
         motor_kp / motor_kd, given one value per env)."""
         bad = sorted(set(values) - set(TASK_VALUE_KEYWORDS))
         if bad:
-            raise ValueError("set_task_values takes %s; not %s (the gains, latencies and terrains are fixed at construction)" %
+            raise ValueError("set_task_values takes %s; not %s (the gains, latencies, control rates and terrains are fixed at "
+                             "construction)" %
                              (TASK_VALUE_KEYWORDS, bad))
         if self._values is None:
             raise ValueError("per-env values are off: build the batch with one value per env for a task keyword")

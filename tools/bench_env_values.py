@@ -17,7 +17,13 @@ Terrains (--workload terrains): walk-ik and turn-ik at 16 384 and 65 536 envs on
 the heightfield, a 50/50 mix (every other env) stepped as two slot ranges of one batch, and the sum of an all-plane and an
 all-heightfield batch of N/2 each, alternately in one process.
 
-Usage: python tools/bench_env_values.py [--steps 200] [--rounds 3] [--workload all|values|latencies|terrains]"""
+Repeats (--workload repeats): walk-ik at 16 384 and 65 536 envs, the scalar 5 ms / 5 sub-step batch, a 50/50 mix (every
+other env) of (5 ms, 5) and (10 ms, 10) stepped as two slot ranges of one batch, the same mix with each rate on one
+contiguous half of the envs ("blocked"), and the sum of a (5 ms, 5) and a (10 ms, 10)
+batch of N/2 each, alternately in one process; ms per control step and env-steps/s.  Creation time of walk-ik at 4096 envs
+with 1 rate (scalar) and with 8 rates (r ms, r sub-steps for r = 1..8: 8 settle caps).
+
+Usage: python tools/bench_env_values.py [--steps 200] [--rounds 3] [--workload all|values|latencies|terrains|repeats]"""
 import argparse
 import json
 import os
@@ -98,7 +104,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=3, help="step rounds; creation rows take the median of 2 x rounds + 1")
-    ap.add_argument("--workload", choices=("all", "values", "latencies", "terrains"), default="all")
+    ap.add_argument("--workload", choices=("all", "values", "latencies", "terrains", "repeats"), default="all")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_env_values needs a CUDA device")
@@ -132,7 +138,40 @@ def main():
                                       **{"ms_" + k: [round(x, 4) for x in v] for k, v in rows.items()},
                                       ms_halves_sum=round(halves, 4),
                                       mixed_vs_halves_pct=round(100 * (median(rows["mixed"]) / halves - 1), 2))), flush=True)
-    if a.workload in ("latencies", "terrains"):
+    if a.workload in ("all", "repeats"):
+        for n in (16384, 65536):
+            kw = dict(task="walk", signal_type="ik")
+            mix = [(0.005, 5), (0.010, 10)] * (n // 2)
+            rows = {}
+            for _ in range(a.rounds):
+                for name, k in (("scalar", dict(kw, num_envs=n, control_time_step=0.005, action_repeat=5)),
+                                ("mixed", dict(kw, num_envs=n, control_time_step=[c for c, _ in mix],
+                                               action_repeat=[r for _, r in mix])),
+                                ("mixed_blocked", dict(kw, num_envs=n, control_time_step=[0.005] * (n // 2) + [0.010] * (n // 2),
+                                                       action_repeat=[5] * (n // 2) + [10] * (n // 2))),
+                                ("half_5", dict(kw, num_envs=n // 2, control_time_step=0.005, action_repeat=5)),
+                                ("half_10", dict(kw, num_envs=n // 2, control_time_step=0.010, action_repeat=10))):
+                    rows.setdefault(name, []).append(ms_per_step(k, a.steps))
+            halves = median(rows["half_5"]) + median(rows["half_10"])
+            print(json.dumps(dict(config="walk-ik repeats", envs=n, steps=a.steps,
+                                  **{"ms_" + k: [round(x, 4) for x in v] for k, v in rows.items()},
+                                  ms_halves_sum=round(halves, 4),
+                                  env_steps_per_s={"scalar": round(n / median(rows["scalar"]) * 1e3),
+                                                   "mixed": round(n / median(rows["mixed"]) * 1e3),
+                                                   "halves": round(n / halves * 1e3)},
+                                  mixed_vs_halves_pct=round(100 * (median(rows["mixed"]) / halves - 1), 2))), flush=True)
+        n = 4096
+        base = dict(task="walk", num_envs=n, signal_type="ik", target_position=2.0, backwards=False)
+        create_ms(base)                                      # module load and first-launch costs out of the timed rows
+        rates = [(r / 1000, r) for r in range(1, 9)]
+        eight = dict(base, control_time_step=[rates[e % 8][0] for e in range(n)], action_repeat=[rates[e % 8][1] for e in range(n)])
+        rows = {"1_rate": [], "8_rates": []}
+        for _ in range(2 * a.rounds + 1):
+            rows["1_rate"].append(create_ms(base))
+            rows["8_rates"].append(create_ms(eight))
+        print(json.dumps(dict(config="create walk-ik %d envs, plane" % n, **{"ms_" + k: round(median(v), 1) for k, v in rows.items()})),
+              flush=True)
+    if a.workload in ("latencies", "terrains", "repeats"):
         return
     for prefix in NAMES:
         name, kw = next(c for c in CONFIGS if c[0].startswith(prefix))
