@@ -279,7 +279,9 @@ enum {
     REXSIM_MAX_GAIN_PAIRS = 64,       /* distinct hold settings (motor_kp, motor_kd, pd_latency, solver_iterations): the settle
                                          runs once per setting and field */
     REXSIM_MAX_REPEAT_PAIRS = 8,      /* distinct (action_repeat, solver_iterations) pairs of rexsim_set_env_repeats */
-    REXSIM_GROUP_WORDS = 8            /* int32 words rexsim_launch_group writes */
+    REXSIM_GROUP_WORDS = 8,           /* int32 words rexsim_launch_group writes */
+    REXSIM_MAX_LAUNCH_GROUPS = 16     /* launch groups of one batch: rexsim_rebalance sorts on (group, 256 cost bins) in one
+                                         block of its scan, 4096 bins at most */
 };
 /* row of the value block that the constructor keyword `keyword` fills ("target_position", "backwards", "target_orient",
  * "init_orient", "base_y", "base_z", "base_roll", "base_pitch", "base_yaw"); -1 for any other name */
@@ -354,7 +356,29 @@ int rexsim_set_env_repeats(RexSim* sim, const int32_t* action_repeat, const int3
 /* the per-env control rates' device buffer, part of a checkpoint's identity: repeats dev [2][N] int32 (row 0 action_repeat,
  * row 1 solver_iterations).  REXSIM_ERR_INVALID when the per-env repeats are off. */
 int rexsim_env_repeat_buffers(RexSim* sim, int32_t** repeats);
-/* launch groups of the batch: 1 unless per-env terrains or repeats split it (0 for a null handle) */
+/* Per-env tasks and signals: the task and signal_type of BatchEnv([ctor_0, ctor_1, ...]) over envs whose spaces agree
+ * (batch_env.py:36-43), e.g. turn ik with turn ol, standup with poses, or with RexSimConfig.normalize walk ik with turn.
+ * task, signal HOST [N] int32 each (REXSIM_TASK_*, REXSIM_SIGNAL_*).  Env e then runs exactly as a batch created with
+ * (task[e], signal[e]) as its scalars: its reset draws, its reset hold, its step kernel, reward and termination.
+ * The step kernel's compile unit (standup and poses ignore the signal) becomes one more key of the launch groups, which are
+ * (terrain, unit, action_repeat, solver_iterations), terrain-major, then in order of first appearance.  The hold settings
+ * become (start, motor_kp, motor_kd, pd_latency, solver_iterations), the start being the pose the hold ends in: the IK stand,
+ * the open-loop stand, standup's fold, or none (poses skips the hold); each (count, start)'s settings are contiguous and
+ * settled once per terrain.  With episode statistics the objectives are kept when any env is walk or gallop; the columns of
+ * the other envs are NaN.
+ * Refused (REXSIM_ERR_INVALID) for an entry that is no task or signal, an env whose rexsim_action_dim or rexsim_obs_dim
+ * differs from the handle's, with normalize = 0 an env whose raw action bound differs from the handle's, gallop with the
+ * 18-motor arm, more than REXSIM_MAX_LAUNCH_GROUPS launch groups or REXSIM_MAX_GAIN_PAIRS hold settings, after the handle's
+ * first reset or step, and on a second call.  Composes with the other per-env setters in any order (each refuses a batch
+ * past the group cap); synchronous.  Off: nothing is allocated and every launch is what it is without it. */
+int rexsim_set_env_tasks(RexSim* sim, const int32_t* task, const int32_t* signal);
+/* the per-env tasks' device buffer, part of a checkpoint's identity: task dev [2][N] u8 (row 0 REXSIM_TASK_*, row 1
+ * REXSIM_SIGNAL_*, as given).  REXSIM_ERR_INVALID when the per-env tasks are off. */
+int rexsim_env_task_buffers(RexSim* sim, uint8_t** task);
+/* the task and signal of launch group g's step launches: its first env's (the config's for a batch of one group).
+ * REXSIM_ERR_INVALID for g outside [0, rexsim_launch_groups). */
+int rexsim_launch_group_task(const RexSim* sim, int32_t g, int32_t* task, int32_t* signal);
+/* launch groups of the batch: 1 unless per-env terrains, repeats or tasks split it (0 for a null handle) */
 int rexsim_launch_groups(const RexSim* sim);
 /* launch group g: info[REXSIM_GROUP_WORDS] = terrain, action_repeat, solver_iterations, first slot, slot count, and the
  * build its last step launch used (CTA size, CTAs per SM, sensor; all 0 before the first step).  A batch of one group

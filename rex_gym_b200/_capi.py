@@ -79,6 +79,9 @@ SIGNATURES = {
     "rexsim_env_terrain_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_i32)]),
     "rexsim_set_env_repeats": (C.c_int, [_ptr] * 3),
     "rexsim_env_repeat_buffers": (C.c_int, [_ptr, _out(_ptr)]),
+    "rexsim_set_env_tasks": (C.c_int, [_ptr] * 3),
+    "rexsim_env_task_buffers": (C.c_int, [_ptr, _out(_ptr)]),
+    "rexsim_launch_group_task": (C.c_int, [_ptr, _i32, _out(_i32), _out(_i32)]),
     "rexsim_launch_groups": (C.c_int, [_ptr]),
     "rexsim_launch_group": (C.c_int, [_ptr, _i32, _ptr]),
     "rexsim_slot_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_ptr)]),

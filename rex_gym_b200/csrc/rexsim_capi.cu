@@ -22,10 +22,10 @@ cudaError_t launch_render(const Params& P, const float* rt, const float* zrange,
 
 using namespace rexsim;
 
-// One launch of the step kernel per control step: the envs of one (terrain, action_repeat, solver_iterations), which own slots
-// perm[first, first + count)
+// One launch of the step kernel per control step: the envs of one (terrain, step unit, action_repeat, solver_iterations), which
+// own slots perm[first, first + count); task, signal: the group's first env's, whose unit_of is the group's unit
 struct LaunchGroup {
-    int32_t terrain, repeat, iters, first, count;
+    int32_t terrain, task, signal, repeat, iters, first, count;
     int32_t launched[3];               // step_kernel instance of the group's last launch: BLOCK, OCC, SENSOR
 };
 
@@ -45,9 +45,10 @@ struct RexSim {
     uint8_t* fin = nullptr;            // final obs | limit staging for rexsim_step_host_final (allocated on its first call)
     int A = 0;
     bool started = false;              // a reset or step has been enqueued: the frame wrappers can no longer be switched on
-    int nholds = 0;                    // hold settings (motor_kp, motor_kd, pd_latency, solver_iterations) of P.ev.gains /
+    int nholds = 0;                    // hold settings (start, motor_kp, motor_kd, pd_latency, solver_iterations) of P.ev.gains /
                                        // P.el.hold (0: no table)
     std::vector<int32_t> hold_iters;   // [nholds] PGS cap of each hold setting, each cap's settings contiguous
+    std::vector<int32_t> hold_start;   // [nholds] start pose of each (hold_start), each (cap, start)'s settings contiguous
     bool values_on = false;            // rexsim_set_env_values was called
     std::vector<float> kp, kd;         // per-env gains given to rexsim_set_env_values (empty: the config's)
     std::vector<double> pd;            // per-env pd latencies given to rexsim_set_env_latencies (empty: the config's)
@@ -57,10 +58,12 @@ struct RexSim {
     float friction[2] = {0.f, 0.f};    // per-env terrains: friction of each terrain's envs, plane and heightfield
     int32_t* repeats = nullptr;        // [2][N] per-env action_repeat, solver_iterations (rexsim_set_env_repeats; null: off)
     std::vector<int32_t> rep, iters;   // the same on the host (empty: the config's)
+    uint8_t* tasks = nullptr;          // [2][N] per-env task, signal (rexsim_set_env_tasks; null: off); P.env_task points here
+    std::vector<uint8_t> task, signal; // the same on the host (empty: the config's)
     // The launch groups (empty: one launch over every slot with the config's values), terrain-major, plane first, then in
     // order of first appearance; group g owns slots perm[first_g, first_g + count_g).  `group` is each env's group, the key
-    // rexsim_rebalance sorts on: its own [N] bytes with per-env repeats; the terrain bytes without them, as the groups are then
-    // the two terrains; null for a batch of one group.
+    // rexsim_rebalance sorts on: the terrain bytes when the groups are exactly the two terrains, its own [N] bytes otherwise;
+    // null for a batch of one group.
     std::vector<LaunchGroup> groups;
     const uint8_t* group = nullptr;
     uint8_t* group_bytes = nullptr;
@@ -68,11 +71,12 @@ struct RexSim {
     int32_t launched[3] = {0, 0, 0};   // step_kernel instance of the last step launch: BLOCK, OCC, SENSOR
 };
 
-// The handle's Params for the launches over one group's envs: its terrain with that terrain's friction, its sub-steps per
-// control step and its PGS cap
+// The handle's Params for the launches over one group's envs: its terrain with that terrain's friction, its task and signal
+// (launch_step's unit, the auto-reset's draws, the settle's start pose), its sub-steps per control step and its PGS cap
 static Params group_params(const RexSim* s, Params P, const LaunchGroup& g) {
     if (s->terrain) P.cfg.friction = s->friction[g.terrain];
-    P.cfg.terrain = g.terrain; P.cfg.action_repeat = g.repeat; P.cfg.solver_iterations = g.iters;
+    P.cfg.terrain = g.terrain; P.cfg.task = g.task; P.cfg.signal = g.signal;
+    P.cfg.action_repeat = g.repeat; P.cfg.solver_iterations = g.iters;
     return P;
 }
 // One control step of every env: one launch over every slot, or one launch per launch group over its slot range of the
@@ -480,61 +484,103 @@ int rexsim_value_row(const char* keyword) {
         if (!strcmp(keyword, c_value_keywords[r])) return r;
     return -1;
 }
-// The reset hold's settings: each env's (motor_kp, motor_kd, pd_latency, solver_iterations), distinct ones in order of first
-// appearance within each PGS cap, the caps in order of first appearance (each cap's settings contiguous), and each env's index
-// into them.  Rex.Reset clears the history and holds through ApplyAction (rex.py:303-323), so the settled state depends on the
-// gains, on the PD observation's latency and on the solver's cap.  kp, kd, pd, iters: per env, or empty for the config's scalar.
-struct HoldTable { std::vector<float> gains; std::vector<double> pd; std::vector<int32_t> iters, index; };
-static int hold_table(const RexSimConfig& c, size_t N, const std::vector<float>& kp, const std::vector<float>& kd,
-                      const std::vector<double>& pd, const std::vector<int32_t>& iters, HoldTable& t) {
+// The pose the reset hold of a (task, signal) ends in (settle_kernel): the IK stand, the open-loop stand (c_pose_stand_ol),
+// standup's fold, or none (poses skips both holding phases)
+enum { START_IK = 0, START_OL = 1, START_FOLD = 2, START_NONE = 3 };
+static int32_t hold_start(int task, int signal) {
+    return task == REXSIM_TASK_STANDUP ? START_FOLD : task == REXSIM_TASK_POSES ? START_NONE
+         : signal == REXSIM_SIGNAL_OL ? START_OL : START_IK;
+}
+// The reset hold's settings: each env's (start, motor_kp, motor_kd, pd_latency, solver_iterations), distinct ones in order of
+// first appearance within each (PGS cap, start), the starts in order of first appearance within each cap and the caps in order
+// of first appearance (each cap's and each (cap, start)'s settings contiguous), and each env's index into them.  Rex.Reset
+// clears the history and holds through ApplyAction (rex.py:303-323), so the settled state depends on the pose held, the gains,
+// the PD observation's latency and the solver's cap.  start, kp, kd, pd, iters: per env, or empty for the config's scalar.
+struct HoldTable { std::vector<float> gains; std::vector<double> pd; std::vector<int32_t> iters, start, index; };
+static int hold_table(const RexSimConfig& c, size_t N, const std::vector<int32_t>& start, const std::vector<float>& kp,
+                      const std::vector<float>& kd, const std::vector<double>& pd, const std::vector<int32_t>& iters, HoldTable& t) {
     t.index.assign(N, 0);
+    auto cap_of = [&](size_t e) { return iters.empty() ? c.solver_iterations : iters[e]; };
+    auto start_of = [&](size_t e) { return start.empty() ? hold_start(c.task, c.signal) : start[e]; };
     std::vector<int32_t> caps;
-    for (size_t e = 0; e < N; e++) {
-        const int32_t it = iters.empty() ? c.solver_iterations : iters[e];
-        if (std::find(caps.begin(), caps.end(), it) == caps.end()) caps.push_back(it);
-    }
+    for (size_t e = 0; e < N; e++)
+        if (std::find(caps.begin(), caps.end(), cap_of(e)) == caps.end()) caps.push_back(cap_of(e));
+    std::vector<std::pair<int32_t, int32_t>> keys;             // (cap, start): each cap's starts in order of first appearance
     for (const int32_t cap : caps)
         for (size_t e = 0; e < N; e++) {
-            const int32_t it = iters.empty() ? c.solver_iterations : iters[e];
-            if (it != cap) continue;
+            const std::pair<int32_t, int32_t> k(cap, start_of(e));
+            if (cap_of(e) == cap && std::find(keys.begin(), keys.end(), k) == keys.end()) keys.push_back(k);
+        }
+    for (const std::pair<int32_t, int32_t>& key : keys)
+        for (size_t e = 0; e < N; e++) {
+            const int32_t it = cap_of(e), st = start_of(e);
+            if (it != key.first || st != key.second) continue;
             const float k = kp.empty() ? c.motor_kp : kp[e], d = kd.empty() ? c.motor_kd : kd[e];
             const double l = pd.empty() ? c.pd_latency : pd[e];
             size_t h = 0;
-            while (h < t.pd.size() && !(t.gains[2 * h] == k && t.gains[2 * h + 1] == d && t.pd[h] == l && t.iters[h] == it)) h++;
+            while (h < t.pd.size() && !(t.gains[2 * h] == k && t.gains[2 * h + 1] == d && t.pd[h] == l && t.iters[h] == it &&
+                                        t.start[h] == st)) h++;
             if (h == t.pd.size()) {
                 if ((int)h == REXSIM_MAX_GAIN_PAIRS)
-                    return fail(REXSIM_ERR_INVALID, "more than 64 distinct reset-hold settings (motor_kp, motor_kd, pd_latency, solver_iterations)");
-                t.gains.push_back(k); t.gains.push_back(d); t.pd.push_back(l); t.iters.push_back(it);
+                    return fail(REXSIM_ERR_INVALID, "more than 64 distinct reset-hold settings (start pose, motor_kp, motor_kd, pd_latency, solver_iterations)");
+                t.gains.push_back(k); t.gains.push_back(d); t.pd.push_back(l); t.iters.push_back(it); t.start.push_back(st);
             }
             t.index[e] = (int32_t)h;
         }
     return REXSIM_OK;
 }
-static int terrain_of(const RexSim* s, size_t e) { return s->terr.empty() ? s->P.cfg.terrain : s->terr[e]; }
+// each env's hold start under per-env tasks (empty without them: the config's)
+static std::vector<int32_t> env_starts(const std::vector<uint8_t>& task, const std::vector<uint8_t>& signal) {
+    std::vector<int32_t> st(task.size());
+    for (size_t e = 0; e < task.size(); e++) st[e] = hold_start(task[e], signal[e]);
+    return st;
+}
 // the launch groups a step launches: the table, or for a batch without one its single group over every slot
 static std::vector<LaunchGroup> launch_groups(const RexSim* s) {
     if (!s->groups.empty()) return s->groups;
     const RexSimConfig& c = s->P.cfg;
-    return {LaunchGroup{c.terrain, c.action_repeat, c.solver_iterations, 0, s->P.N, {s->launched[0], s->launched[1], s->launched[2]}}};
+    return {LaunchGroup{c.terrain, c.task, c.signal, c.action_repeat, c.solver_iterations, 0, s->P.N,
+                        {s->launched[0], s->launched[1], s->launched[2]}}};
 }
-// Rebuild the launch groups from each env's terrain and control rate: put each group's envs in its slot range, in env order,
-// and give rexsim_rebalance the group key.  Synchronous.
+// Each env's launch group: the groups (terrain, step unit, action_repeat, solver_iterations), terrain-major, plane first, then
+// in order of first appearance, from the per-env terrains, repeats, iteration counts, tasks and signals given (each empty for
+// the config's).  Refused past REXSIM_MAX_LAUNCH_GROUPS groups.
+struct GroupPlan { std::vector<LaunchGroup> gs; std::vector<uint8_t> key; };
+static int plan_groups(const RexSim* s, const std::vector<uint8_t>& terr, const std::vector<int32_t>& rep,
+                       const std::vector<int32_t>& iters, const std::vector<uint8_t>& task, const std::vector<uint8_t>& signal,
+                       GroupPlan& p) {
+    const RexSimConfig& c = s->P.cfg;
+    const size_t N = s->P.N;
+    p.gs.clear();
+    p.key.assign(N, 0);
+    for (const int t : {REXSIM_TERRAIN_PLANE, REXSIM_TERRAIN_RANDOM})
+        for (size_t e = 0; e < N; e++) {
+            if ((terr.empty() ? c.terrain : terr[e]) != t) continue;
+            const int32_t r = rep.empty() ? c.action_repeat : rep[e];
+            const int32_t it = iters.empty() ? c.solver_iterations : iters[e];
+            const int32_t k = task.empty() ? c.task : task[e], sg = signal.empty() ? c.signal : signal[e];
+            size_t g = 0;
+            while (g < p.gs.size() && !(p.gs[g].terrain == t && unit_of(p.gs[g].task, p.gs[g].signal) == unit_of(k, sg) &&
+                                        p.gs[g].repeat == r && p.gs[g].iters == it)) g++;
+            if (g == p.gs.size()) {
+                if ((int)g == REXSIM_MAX_LAUNCH_GROUPS)
+                    return fail(REXSIM_ERR_INVALID, "more than 16 launch groups (terrain, task unit, action_repeat, solver_iterations)");
+                p.gs.push_back(LaunchGroup{t, k, sg, r, it, 0, 0, {0, 0, 0}});
+            }
+            p.gs[g].count++;
+            p.key[e] = (uint8_t)g;
+        }
+    return REXSIM_OK;
+}
+// Install the launch groups of the handle's per-env values (plan_groups): put each group's envs in its slot range, in env
+// order, and give rexsim_rebalance the group key.  Synchronous.
 static int build_groups(RexSim* s) {
     Params& P = s->P;
     const size_t N = P.N;
-    std::vector<LaunchGroup> gs;
-    std::vector<uint8_t> key(N);
-    for (const int t : {REXSIM_TERRAIN_PLANE, REXSIM_TERRAIN_RANDOM})
-        for (size_t e = 0; e < N; e++) {
-            if (terrain_of(s, e) != t) continue;
-            const int32_t r = s->rep.empty() ? P.cfg.action_repeat : s->rep[e];
-            const int32_t it = s->iters.empty() ? P.cfg.solver_iterations : s->iters[e];
-            size_t g = 0;
-            while (g < gs.size() && !(gs[g].terrain == t && gs[g].repeat == r && gs[g].iters == it)) g++;
-            if (g == gs.size()) gs.push_back(LaunchGroup{t, r, it, 0, 0, {0, 0, 0}});
-            gs[g].count++;
-            key[e] = (uint8_t)g;
-        }
+    GroupPlan plan;
+    if (int rc = plan_groups(s, s->terr, s->rep, s->iters, s->task, s->signal, plan)) return rc;
+    std::vector<LaunchGroup>& gs = plan.gs;
+    const std::vector<uint8_t>& key = plan.key;
     std::vector<int32_t> at(gs.size()), perm(N);
     for (size_t g = 1; g < gs.size(); g++) gs[g].first = gs[g - 1].first + gs[g - 1].count;
     for (size_t g = 0; g < gs.size(); g++) at[g] = gs[g].first;
@@ -549,8 +595,8 @@ static int build_groups(RexSim* s) {
         if (s->mem.zeroed(&hist, 256 * gs.size())) return REXSIM_ERR_CUDA;
         s->mem.drop(s->hist);
         s->hist = hist;
-        if (!s->repeats) {
-            s->group = s->terrain;             // the groups are the two terrains: group g is terrain g
+        if (gs.size() == 2 && gs[0].terrain == REXSIM_TERRAIN_PLANE && gs[1].terrain == REXSIM_TERRAIN_RANDOM) {
+            s->group = s->terrain;             // the groups are exactly the two terrains: group g is terrain g
         } else {
             if (s->mem.zeroed(&s->group_bytes, N)) return REXSIM_ERR_CUDA;
             CK(cudaMemcpy(s->group_bytes, key.data(), N, cudaMemcpyHostToDevice));
@@ -561,8 +607,9 @@ static int build_groups(RexSim* s) {
     return REXSIM_OK;
 }
 // Run the reset hold again for every snapshot of the layout P.snaps, at the handle's hold settings (the config's one without a
-// table), its sensor history rows at the handle's ring depth: one launch per (terrain, PGS cap) the launch groups hold, each
-// at that terrain's friction and with that cap, over all the cap's (setting, field) snapshots.  Synchronous.
+// table), its sensor history rows at the handle's ring depth: one launch per (terrain, PGS cap, start pose) the launch groups
+// hold, each at that terrain's friction, with that cap and with a task and signal of that start, over all the (cap, start)'s
+// (setting, field) snapshots.  Synchronous.
 static int settle_snapshots(RexSim* s) {
     Params& P = s->P;
     const int nh = s->nholds > 0 ? s->nholds : 1;
@@ -578,13 +625,19 @@ static int settle_snapshots(RexSim* s) {
         if (s->mem.zeroed(&P.snap_ring, nsettle * P.ring_depth * sensor_cfg(&P.cfg).words)) return REXSIM_ERR_CUDA;
     }
     const std::vector<int32_t> caps = s->nholds > 0 ? s->hold_iters : std::vector<int32_t>{P.cfg.solver_iterations};
+    const std::vector<int32_t> starts = s->nholds > 0 ? s->hold_start : std::vector<int32_t>{hold_start(P.cfg.task, P.cfg.signal)};
     const std::vector<LaunchGroup> gs = launch_groups(s);
+    auto same_hold = [](const LaunchGroup& a, const LaunchGroup& b) {
+        return a.terrain == b.terrain && a.iters == b.iters && hold_start(a.task, a.signal) == hold_start(b.task, b.signal);
+    };
     for (size_t g = 0; g < gs.size(); g++) {
-        bool settled = false;                  // an earlier group on the same terrain with the same cap
-        for (size_t h = 0; h < g; h++) settled = settled || (gs[h].terrain == gs[g].terrain && gs[h].iters == gs[g].iters);
+        bool settled = false;                  // an earlier group on the same terrain with the same cap and start
+        for (size_t h = 0; h < g; h++) settled = settled || same_hold(gs[h], gs[g]);
         if (settled) continue;
-        const int first = (int)(std::find(caps.begin(), caps.end(), gs[g].iters) - caps.begin());
-        const int count = (int)std::count(caps.begin(), caps.end(), gs[g].iters);
+        const int32_t st = hold_start(gs[g].task, gs[g].signal);
+        int first = -1, count = 0;             // the (cap, start)'s settings are contiguous
+        for (size_t h = 0; h < caps.size(); h++)
+            if (caps[h] == gs[g].iters && starts[h] == st) { first = first < 0 ? (int)h : first; count++; }
         const Params G = group_params(s, P, gs[g]);
         if (int rc = enqueue(s, launch_settle(G, snap_f, snap_i, first, count, 0), "settle launch")) return rc;
     }
@@ -614,6 +667,7 @@ static int apply_holds(RexSim* s, const HoldTable& t, bool settle) {
     }
     s->nholds = (int)nh;
     s->hold_iters = t.iters;
+    s->hold_start = t.start;
     return settle ? settle_snapshots(s) : REXSIM_OK;
 }
 int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const float* kd) {
@@ -634,9 +688,9 @@ int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const
         for (size_t e = 0; e < N; e++)
             if (!(kp[e] >= 0.f) || !(kd[e] >= 0.f) || std::isinf(kp[e]) || std::isinf(kd[e]))
                 return fail(REXSIM_ERR_INVALID, "gains must be finite and non-negative");
-        if (int rc = hold_table(c, N, std::vector<float>(kp, kp + N), std::vector<float>(kd, kd + N), s->pd, s->iters, t)) return rc;
+        if (int rc = hold_table(c, N, env_starts(s->task, s->signal), std::vector<float>(kp, kp + N), std::vector<float>(kd, kd + N), s->pd, s->iters, t)) return rc;
     } else if (!P.ev.pair) {
-        if (int rc = hold_table(c, N, s->kp, s->kd, s->pd, s->iters, t)) return rc;          // the config's one setting
+        if (int rc = hold_table(c, N, env_starts(s->task, s->signal), s->kp, s->kd, s->pd, s->iters, t)) return rc;          // the config's one setting
     }
     float* block = nullptr;
     if (s->mem.zeroed(&block, (size_t)REXSIM_VALUE_BLOCK_ROWS * N)) return REXSIM_ERR_CUDA;
@@ -678,7 +732,7 @@ int rexsim_set_env_latencies(RexSim* s, const double* control_latency, const dou
     }
     HoldTable t;
     const std::vector<double> pd(lat.begin() + N, lat.end());
-    if (int rc = hold_table(c, N, s->kp, s->kd, pd, s->iters, t)) return rc;
+    if (int rc = hold_table(c, N, env_starts(s->task, s->signal), s->kp, s->kd, pd, s->iters, t)) return rc;
     double* dlat = nullptr;
     EnvDelay* denv = nullptr;
     if (s->mem.zeroed(&dlat, 2 * N) || s->mem.zeroed(&denv, N)) return REXSIM_ERR_CUDA;
@@ -719,6 +773,8 @@ int rexsim_set_env_terrains(RexSim* s, const int32_t* terrain, float plane_frict
         bytes[e] = (uint8_t)terrain[e];
         nplane += terrain[e] == REXSIM_TERRAIN_PLANE;
     }
+    GroupPlan plan;
+    if (int rc = plan_groups(s, bytes, s->rep, s->iters, s->task, s->signal, plan)) return rc;
     uint8_t* dterrain = nullptr;
     if (s->mem.zeroed(&dterrain, N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(dterrain, bytes.data(), N, cudaMemcpyHostToDevice));
@@ -756,8 +812,10 @@ int rexsim_set_env_repeats(RexSim* s, const int32_t* action_repeat, const int32_
             pairs.push_back(std::make_pair(rep[e], iters[e]));
         }
     }
+    GroupPlan plan;
+    if (int rc = plan_groups(s, s->terr, rep, iters, s->task, s->signal, plan)) return rc;
     HoldTable t;
-    if (int rc = hold_table(c, N, s->kp, s->kd, s->pd, iters, t)) return rc;
+    if (int rc = hold_table(c, N, env_starts(s->task, s->signal), s->kp, s->kd, s->pd, iters, t)) return rc;
     int32_t* d = nullptr;
     if (s->mem.zeroed(&d, 2 * N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(d, rep.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
@@ -770,6 +828,66 @@ int rexsim_env_repeat_buffers(RexSim* s, int32_t** repeats) {
     if (!s || !repeats) return fail(REXSIM_ERR_INVALID, "null argument");
     if (!s->repeats) return fail(REXSIM_ERR_INVALID, "per-env repeats are off (rexsim_set_env_repeats)");
     *repeats = s->repeats;
+    return REXSIM_OK;
+}
+int rexsim_set_env_tasks(RexSim* s, const int32_t* task, const int32_t* signal) {
+    if (!s || !task || !signal) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env tasks must be set before the first reset or step");
+    if (s->tasks) return fail(REXSIM_ERR_INVALID, "per-env tasks are already set");
+    Params& P = s->P;
+    const RexSimConfig& c = P.cfg;
+    const size_t N = P.N;
+    // the reference's BatchEnv refuses envs whose spaces differ (batch_env.py:36-43): the widths always, the raw action bound
+    // unless ClipAction and RangeNormalize replace both boxes (the observation bounds depend on the time step alone)
+    const TaskShape own = task_shape(c.task);
+    std::vector<uint8_t> tk(N), sg(N);
+    bool objectives = false;
+    for (size_t e = 0; e < N; e++) {
+        const int32_t k = task[e], g = signal[e];
+        if (k < REXSIM_TASK_WALK || k > REXSIM_TASK_POSES || (g != REXSIM_SIGNAL_IK && g != REXSIM_SIGNAL_OL))
+            return fail(REXSIM_ERR_INVALID, "task entries must be REXSIM_TASK_* and signal entries REXSIM_SIGNAL_*");
+        if (k == REXSIM_TASK_GALLOP && c.num_motors == 18)
+            return fail(REXSIM_ERR_INVALID, "mark='arm' is built for every task but gallop");
+        if (rexsim_action_dim(k, g) != s->A || obs_dim(k, c.num_motors) != obs_dim(c.task, c.num_motors))
+            return fail(REXSIM_ERR_INVALID, "All environments must use the same observation space (action or observation width differs)");
+        if (!c.normalize && task_shape(k).bound[g] != own.bound[c.signal])
+            return fail(REXSIM_ERR_INVALID, "All environments must use the same observation space (raw action bound differs)");
+        tk[e] = (uint8_t)k; sg[e] = (uint8_t)g;
+        objectives = objectives || k == REXSIM_TASK_WALK || k == REXSIM_TASK_GALLOP;
+    }
+    GroupPlan plan;
+    if (int rc = plan_groups(s, s->terr, s->rep, s->iters, tk, sg, plan)) return rc;
+    HoldTable t;
+    if (int rc = hold_table(c, N, env_starts(tk, sg), s->kp, s->kd, s->pd, s->iters, t)) return rc;
+    uint8_t* d = nullptr;
+    if (s->mem.zeroed(&d, 2 * N)) return REXSIM_ERR_CUDA;
+    CK(cudaMemcpy(d, tk.data(), N, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d + N, sg.data(), N, cudaMemcpyHostToDevice));
+    s->tasks = d; s->task = tk; s->signal = sg;
+    P.env_task = d;
+    if (s->ep_block && objectives) {
+        // walk and gallop record the objectives of every step; the other envs' columns are NaN and stay NaN
+        std::vector<float> o(4 * N, 0.f);
+        for (size_t e = 0; e < N; e++)
+            if (tk[e] != REXSIM_TASK_WALK && tk[e] != REXSIM_TASK_GALLOP)
+                for (int r = 0; r < 4; r++) o[r * N + e] = NAN;
+        if (!P.ep.objectives && s->mem.zeroed(&P.ep.objectives, 4 * N)) return REXSIM_ERR_CUDA;
+        CK(cudaMemcpy(P.ep.objectives, o.data(), 4 * N * sizeof(float), cudaMemcpyHostToDevice));
+    }
+    if (int rc = build_groups(s)) return rc;
+    return apply_holds(s, t, true);
+}
+int rexsim_env_task_buffers(RexSim* s, uint8_t** task) {
+    if (!s || !task) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (!s->tasks) return fail(REXSIM_ERR_INVALID, "per-env tasks are off (rexsim_set_env_tasks)");
+    *task = s->tasks;
+    return REXSIM_OK;
+}
+int rexsim_launch_group_task(const RexSim* s, int32_t g, int32_t* task, int32_t* signal) {
+    if (!s || !task || !signal) return fail(REXSIM_ERR_INVALID, "null argument");
+    const std::vector<LaunchGroup> gs = launch_groups(s);
+    if (g < 0 || g >= (int32_t)gs.size()) return fail(REXSIM_ERR_INVALID, "no such launch group");
+    *task = gs[g].task; *signal = gs[g].signal;
     return REXSIM_OK;
 }
 int rexsim_launch_groups(const RexSim* s) { return s ? (int)launch_groups(s).size() : 0; }

@@ -1657,9 +1657,11 @@ __device__ __forceinline__ void store_arm(float* sf, int32_t* si, int N, int env
 }
 
 // reset one env from the settled snapshot + task draws (BatchEnv.reset -> <task>.reset; rex.py:255-324)
-template <bool ARM>
+template <bool ARM, bool ENV_TASK = false>
 // `valid` is false on the padding lanes that replicate the last env to keep warps whole: they compute, but never write
 // (a replica that re-read the counter after the real lane's write would otherwise bump it twice).  `terrain`: the env's own.
+// ENV_TASK: the draws follow the env's task in P.env_task when the batch has per-env tasks (the reset kernel); without it they
+// follow cfg.task, the launch group's (the step kernel's auto-reset).
 __device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, int terrain, int leg, Lane& L, Task& K, float& kp, float& kd, int& field,
                                                     Arm& AR, bool valid, Sensor& S) {
     const RexSimConfig& c = P.cfg;
@@ -1685,14 +1687,15 @@ __device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, in
     kd = (c.kd_lo == c.kd_hi) ? (P.ev.gains ? P.ev.gains[2 * pair + 1] : c.motor_kd) : (float)rand_uniform(c.seed, genv, rc,5, c.kd_lo, c.kd_hi);
     const int backwards = ev ? (int)ev[(size_t)REXSIM_VALUE_BACKWARDS * N] : c.backwards;
     const float target_position = value(REXSIM_VALUE_TARGET_POSITION, c.target_position);
-    if (c.task == REXSIM_TASK_WALK) {
+    const int task = ENV_TASK && P.env_task ? (int)P.env_task[env] : c.task;
+    if (task == REXSIM_TASK_WALK) {
         int bw = (backwards < 0) ? (int)(rand_u32(c.seed, genv, rc,0) >> 31) : backwards;
         if (bw) K.flags |= FL_BACKWARDS;
         if (isnan(target_position)) K.target = (float)rand_uniform(c.seed, genv, rc,1, bw ? -2.0 : 1.0, bw ? -3.0 : 3.0);
         else K.target = target_position;
-    } else if (c.task == REXSIM_TASK_GALLOP) {
+    } else if (task == REXSIM_TASK_GALLOP) {
         K.target = isnan(target_position) ? (float)rand_uniform(c.seed, genv, rc,1, 1.0, 3.0) : target_position;
-    } else if (c.task == REXSIM_TASK_TURN) {
+    } else if (task == REXSIM_TASK_TURN) {
         const float target_orient = value(REXSIM_VALUE_TARGET_ORIENT, c.target_orient);
         const float init_orient = value(REXSIM_VALUE_INIT_ORIENT, c.init_orient);
         double to = isnan(target_orient) ? rand_uniform(c.seed, genv, rc,2, 0.2, 6.0) : (double)target_orient;
@@ -1705,7 +1708,7 @@ __device__ __forceinline__ void reset_from_snapshot(const Params& P, int env, in
         L.pos = mk(0.f, 0.f, 0.21f);
         float hy = (float)(io * 0.5);
         L.qx = 0.f; L.qy = 0.f; L.qz = sinf(hy); L.qw = cosf(hy);
-    } else if (c.task == REXSIM_TASK_POSES) {                         // poses_env.py:148-176
+    } else if (task == REXSIM_TASK_POSES) {                         // poses_env.py:148-176
         float pv[5];
         bool any = false;
 #pragma unroll
@@ -2070,7 +2073,7 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
     if (P.final_obs && done && valid) put_final<obs_dim(TASK, 12)>(P.final_obs + (size_t)env * P.out_dim, obs_row, P.out_dim, leg);
     // ---- auto reset: done envs restart from the settled snapshot; obs = first observation of the new episode --
     if (c.auto_reset && done) {
-        reset_from_snapshot<ARM>(P, env, TERRAIN, leg, L, K, kp, kd, field, AR, valid, S);     // the launch's terrain is the env's
+        reset_from_snapshot<ARM>(P, env, TERRAIN, leg, L, K, kp, kd, field, AR, valid, S);     // the launch's terrain and task are the env's
         if (valid) write_obs<TASK, SENSOR>(P, env, leg, L, obs_row, S, 0u, true);
     }
     store_lane(P.sf, P.si, N, env, leg, L, K, valid);
@@ -2079,7 +2082,8 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
 }
 
 // -------------------------------------------------------------------------------------------------
-// reset kernel: BatchEnv.reset(indices)
+// reset kernel: BatchEnv.reset(indices).  The WALK instance serves every task but gallop (their observations are the same
+// four base terms); each env's draws follow its own task (P.env_task), so one launch resets envs of several tasks.
 // -------------------------------------------------------------------------------------------------
 template <int TASK, bool ARM>
 __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_out) {
@@ -2098,7 +2102,7 @@ __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_o
     Lane L; Task K; Arm AR; float kp, kd; int field;
     Sensor S = make_sensor<ARM>(P, P.ring, P.N, env, (uint32_t)env + (uint32_t)P.cfg.env_offset);
     const int terrain = P.env_terrain ? (int)P.env_terrain[env] : P.cfg.terrain;
-    reset_from_snapshot<ARM>(P, env, terrain, leg, L, K, kp, kd, field, AR, wr, S);
+    reset_from_snapshot<ARM, true>(P, env, terrain, leg, L, K, kp, kd, field, AR, wr, S);
     if (wr && (obs_out || P.fr.ring || P.fr.last)) {      // the frame wrappers restart even when no observation is asked for
         float* row = obs_out ? obs_out + (size_t)j * P.out_dim : nullptr;
         if (P.sensor_on) write_obs<TASK, true>(P, env, leg, L, row, S, 0u, true);
@@ -2191,10 +2195,7 @@ constexpr StepUnit c_units[8] = {{REXSIM_TASK_WALK, REXSIM_SIGNAL_IK}, {REXSIM_T
                                  {REXSIM_TASK_GALLOP, REXSIM_SIGNAL_IK}, {REXSIM_TASK_GALLOP, REXSIM_SIGNAL_OL},
                                  {REXSIM_TASK_TURN, REXSIM_SIGNAL_IK}, {REXSIM_TASK_TURN, REXSIM_SIGNAL_OL},
                                  {REXSIM_TASK_STANDUP, REXSIM_SIGNAL_OL}, {REXSIM_TASK_POSES, REXSIM_SIGNAL_IK}};
-// the unit launch_step takes for a (task, signal) pair; standup and poses ignore the signal, an unknown task takes unit 6
-constexpr int unit_of(int task, int signal) {
-    return task == REXSIM_TASK_POSES ? 7 : (task >= 0 && task < REXSIM_TASK_STANDUP) ? 2 * task + (signal != REXSIM_SIGNAL_IK) : 6;
-}
+// launch_step takes unit unit_of(task, signal) (rexsim_kernel.cuh)
 constexpr bool unit_of_inverts_c_units(int u = 0) {
     return u == 8 || (unit_of(c_units[u].task, c_units[u].signal) == u && unit_of_inverts_c_units(u + 1));
 }
@@ -2302,6 +2303,7 @@ __global__ void rebalance_hist_kernel(const int32_t* __restrict__ cost, const ui
     if (e < n) atomicAdd(&hist[rebalance_bin(cost, group, e)], 1);
 }
 constexpr int REBALANCE_MAX_BINS = 4096, REBALANCE_SCAN_THREADS = 1024;
+static_assert(REXSIM_MAX_LAUNCH_GROUPS * 256 <= REBALANCE_MAX_BINS, "the scan holds every group's bins");
 // 1 block: exclusive prefix sum of `bins` bins in place, thread t owning bins [t * per, (t + 1) * per).  Up to 1024 bins it is
 // one thread per bin (per = 1).
 __global__ void rebalance_scan_kernel(int32_t* hist, int bins, int per) {

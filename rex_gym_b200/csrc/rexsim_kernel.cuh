@@ -58,6 +58,11 @@ __host__ __device__ constexpr TaskShape task_shape(int task) {
          : task == REXSIM_TASK_TURN   ? TaskShape{{2, 2}, false, {0.01f, 0.01f}}      // turn_env.py:104-108
          : TaskShape{{1, 1}, false, {0.1f, 0.1f}};                                   // standup_env.py:99, poses_env.py:118
 }
+// the step-kernel compile unit (rexsim_kernel.cu c_units) of a (task, signal) pair: walk, gallop and turn per signal, then
+// standup and poses, which ignore the signal; an unknown task takes unit 6
+__host__ __device__ constexpr int unit_of(int task, int signal) {
+    return task == REXSIM_TASK_POSES ? 7 : (task >= 0 && task < REXSIM_TASK_STANDUP) ? 2 * task + (signal != REXSIM_SIGNAL_IK) : 6;
+}
 // observation width: base roll, pitch and their rates, then (gallop) the motor angles
 __host__ __device__ constexpr int obs_dim(int task, int num_motors) { return 4 + (task_shape(task).angles ? num_motors : 0); }
 // width of the rows the kernels write: obs_dim, repeated once per past index when FrameHistory is on (rexsim_out_dim)
@@ -171,6 +176,9 @@ struct Params {
     float* snap_ring;                  // [npairs * fields][D][HW_WORDS(_ARM)] history the reset hold leaves behind, per snapshot
     Delay ctl, pd;                     // the config's control and PD latency (per env: EnvLatencies)
     float noise_sd[5];                 // SENSOR_NOISE_STDDEV order: motor angle, motor velocity, motor torque, base rpy, base rpy rate
+    // per-env tasks (rexsim_set_env_tasks; null: every env runs cfg.task): [2][N] REXSIM_TASK_* row, REXSIM_SIGNAL_* row, by
+    // env.  Only the reset kernel reads it: each step launch covers one launch group, with the group's task in cfg.task.
+    const uint8_t* __restrict__ env_task;
 };
 
 // ----- tiny vector algebra ---------------------------------------------------------------------------

@@ -29,6 +29,10 @@ OBSERVATION_EPS = 0.01          # rex_gym/envs/rex_gym_env.py:19
 ACTION_BOUND = {("walk", "ik"): 0.4, ("walk", "ol"): 0.01, ("gallop", "ik"): 0.4, ("gallop", "ol"): 0.3,
                 ("turn", "ik"): 0.01, ("turn", "ol"): 0.01, ("standup", "ol"): 0.1, ("standup", "ik"): 0.1,
                 ("poses", "ik"): 0.1, ("poses", "ol"): 0.1}
+# action width per signal (ik, ol) and whether the observation carries the motor angles (the library's task_shape, which
+# rexsim_action_dim / rexsim_obs_dim report; the constructor checks the two agree)
+ACTION_DIM = {"walk": (2, 8), "gallop": (2, 4), "turn": (2, 2), "standup": (1, 1), "poses": (1, 1)}
+OBSERVES_ANGLES = {"gallop"}
 
 ERR_NONFINITE, ERR_JOINT_LIMIT, ERR_BODY_CONTACT, ERR_TILE_MISS, ERR_BAD_INDEX = 1, 2, 4, 8, 16
 SENSOR_NOISE_STDDEV = (0.0, 0.0, 0.0, 0.0, 0.0)      # rex_gym/model/rex.py:22, default of rex_gym_env.py:61
@@ -238,8 +242,9 @@ def _rate_entries(name, value, n):
 
 
 def check_env_repeats(num_envs, task, control_time_step, action_repeat, solver_iterations=None):
-    """The control-rate keywords, checked before any CUDA call.  control_time_step and action_repeat: a scalar (None: the
-    task's default) or one entry per env (a list, tuple or ndarray).  Env e is built as if (control_time_step[e],
+    """The control-rate keywords, checked before any CUDA call.  task: the task name, or one per env.  control_time_step and
+    action_repeat: a scalar (None: each env's task's default, 6 ms / 6 for gallop and poses, 5 ms / 5 otherwise) or one entry
+    per env (a list, tuple or ndarray).  Env e is built as if (control_time_step[e],
     action_repeat[e]) were the scalars, so every control_time_step[e] / action_repeat[e], in fp64 as rex_gym_env.py:173
     computes it, must be the one simulation time step: the observation space's rate bounds are 2 pi / time step, and the
     reference's BatchEnv refuses envs whose spaces differ.  solver_iterations: None (each env int(300 / action_repeat[e]),
@@ -249,10 +254,14 @@ def check_env_repeats(num_envs, task, control_time_step, action_repeat, solver_i
     n = int(num_envs)
     if is_per_env(solver_iterations):
         raise ValueError("solver_iterations takes one value for the batch (None: int(300 / action_repeat) per env)")
-    long_step = task in ("gallop", "poses")
-    default = lambda v, d: v if is_per_env(v) else (v or d)                  # a scalar None (or 0) takes the task's default
-    cts = _rate_entries("control_time_step", default(control_time_step, 0.006 if long_step else 0.005), n)
-    rep = _rate_entries("action_repeat", default(action_repeat, 6 if long_step else 5), n)
+    long_step = [t in ("gallop", "poses") for t in (list(task) if is_per_env(task) else [task] * n)]
+
+    def default(v, long, short):                 # a scalar None (or 0) takes each env's task's default
+        if is_per_env(v) or v:
+            return v
+        return long if all(long_step) else short if not any(long_step) else [long if ls else short for ls in long_step]
+    cts = _rate_entries("control_time_step", default(control_time_step, 0.006, 0.005), n)
+    rep = _rate_entries("action_repeat", default(action_repeat, 6, 5), n)
     steps = sorted({c / r for c, r in zip(cts, rep)})
     if len(steps) > 1:
         raise ValueError("control_time_step / action_repeat: the envs' simulation time steps differ (%s s); the observation "
@@ -266,6 +275,70 @@ def check_env_repeats(num_envs, task, control_time_step, action_repeat, solver_i
         raise ValueError("action_repeat: %d distinct (action_repeat, solver_iterations) pairs, at most %d (each is one step "
                          "launch)" % (pairs, MAX_REPEAT_PAIRS))
     return tuple(cts), tuple(rep), steps[0], (np.ascontiguousarray(rep, np.int32), np.ascontiguousarray(iters, np.int32))
+
+
+def task_spaces(task, signal_type, normalize, time_step, frames=None, frame_delta=False, num_motors=12):
+    """(action_space, observation_space) of one (task, signal_type) env: the raw task spaces, or the wrapper-visible ones when
+    the training wrappers are fused in, through the frame wrappers."""
+    A = ACTION_DIM[task][SIGNALS[signal_type]]
+    O = 4 + (num_motors if task in OBSERVES_ANGLES else 0)
+    if normalize:
+        action_space = Box(-np.inf * np.ones(A, np.float32), np.inf * np.ones(A, np.float32))   # ClipAction wrappers.py:257-260
+        lo, hi = -np.ones(O, np.float32), np.ones(O, np.float32)                               # RangeNormalize :204-209
+    else:
+        ha = np.full(A, ACTION_BOUND[(task, signal_type)], np.float32)
+        action_space = Box(ha, -ha) if task == "gallop" else Box(-ha, ha)                         # gallop_env.py:128-130
+        ub = np.full(O, 2 * math.pi, np.float32)
+        ub[2:4] = 2 * math.pi / time_step
+        lo, hi = -(ub + OBSERVATION_EPS), ub + OBSERVATION_EPS
+    return action_space, Box(*frame_space(lo, hi, frames, frame_delta))
+
+
+def _same_box(a, b):
+    """Exactly the same Box: shapes first (Box.__eq__ compares bounds by broadcasting only), then every bound."""
+    return a.low.shape == b.low.shape and np.array_equal(a.low, b.low) and np.array_equal(a.high, b.high)
+
+
+def _name_entries(name, value, names, n):
+    """A task / signal_type keyword, scalar or per env -> a list of n names, each one of `names`."""
+    if is_per_env(value):
+        if isinstance(value, torch.Tensor):
+            raise ValueError("%s: per-env entries are names, not a tensor" % name)
+        a = np.asarray(list(value) if isinstance(value, (list, tuple)) else value, dtype=object)
+        if a.shape != (n,):
+            raise ValueError("%s: expected one entry per env (%d), got shape %s" % (name, n, a.shape))
+        entries = [str(v) if isinstance(v, str) else v for v in a]
+    else:
+        entries = [value] * n
+    for v in entries:
+        if not isinstance(v, str) or v not in names:
+            raise ValueError("unknown %s %r (have %s)" % (name, v, sorted(names)))
+    return entries
+
+
+def check_env_tasks(num_envs, task, signal_type, time_step=0.001, normalize=False, frames=None, frame_delta=False, mark="base"):
+    """The task and signal_type keywords, checked before any CUDA call: each a scalar or one entry per env (a list, tuple or
+    ndarray).  Envs of several (task, signal_type) pairs are one batch only when their spaces (task_spaces) are the same, as
+    the reference's BatchEnv requires (batch_env.py:36-43): e.g. turn ik with turn ol, standup with poses, and under normalize
+    walk ik with turn.  -> (task, signal_type, None) for a scalar construction (all-equal pairs are one), else (tasks tuple,
+    signals tuple, (task ids, signal ids) int32 [num_envs] each)."""
+    n = int(num_envs)
+    tasks = _name_entries("task", task, TASKS, n)
+    signals = _name_entries("signal_type", signal_type, SIGNALS, n)
+    pairs = list(dict.fromkeys(zip(tasks, signals)))
+    if len(pairs) == 1:
+        return pairs[0][0], pairs[0][1], None
+    nm = 12 if mark == "base" else 18
+    spaces = {p: task_spaces(p[0], p[1], normalize, time_step, frames, frame_delta, nm) for p in pairs}
+    a0, o0 = spaces[pairs[0]]
+    for p in pairs[1:]:
+        a, o = spaces[p]
+        if not (_same_box(o, o0) and _same_box(a, a0)):
+            raise ValueError("All environments must use the same observation space. (%s/%s: action %s, observation %s; %s/%s: "
+                             "action %s, observation %s%s)" % (pairs[0] + (a0, o0) + p + (a, o, "" if normalize else
+                                                               "; normalize=True gives every task the same bounds")))
+    ids = (np.ascontiguousarray([TASKS[t] for t in tasks], np.int32), np.ascontiguousarray([SIGNALS[g] for g in signals], np.int32))
+    return tuple(tasks), tuple(signals), ids
 
 
 class _Info(object):
@@ -358,11 +431,19 @@ class BatchedRexEnv(object):
           capped at solver_iterations (None: int(300 / action_repeat[e])).  Every control_time_step[e] / action_repeat[e]
           must be the same simulation time step, which the observation space depends on.  Each (terrain, action_repeat,
           solver_iterations) group of envs is one slot range of the batch, launched with its own values; at most 8 distinct
-          rates.  All-equal entries build the scalar construction."""
+          rates.  All-equal entries build the scalar construction.
+
+        task, signal_type: each a scalar or one entry per env.  Env e runs exactly as the batch built with (task[e],
+          signal_type[e]) as scalars, its defaults included (a default control rate of 6 ms / 6 for gallop and poses, 5 ms / 5
+          otherwise).  The envs' spaces must be the same, as the reference's BatchEnv requires: turn ik with turn ol, standup
+          with poses, and under normalize walk ik with turn.  Each (terrain, step-kernel unit, rate) group of envs is one
+          slot range of the batch, launched with its own task; at most 16 groups.  All-equal entries build the scalar
+          construction."""
         if urdf_version is not None and urdf_version != DEFAULT_URDF_VERSION:
             raise ValueError("%s is not a supported urdf_version." % urdf_version)     # rex_gym_env.py:317-318
-        if task not in TASKS or signal_type not in SIGNALS:
-            raise ValueError("unknown task/signal_type %r/%r" % (task, signal_type))
+        n_envs = int(num_envs)
+        task_list = _name_entries("task", task, TASKS, n_envs)
+        _name_entries("signal_type", signal_type, SIGNALS, n_envs)
         # per-env terrains: a batch of both is created on the heightfield (its bank), then told which envs are on the plane
         terrain_scalar, env_terrain = check_env_terrains(num_envs, terrain_type)
         if render or on_rack:
@@ -381,11 +462,15 @@ class BatchedRexEnv(object):
             motor_kp, motor_kd = float(env_gains[0][0]), float(env_gains[1][0])
         # per-env latencies: the scalar gains of a motor_kp / motor_kd range hold the reset at each distinct pd_latency
         env_latency = check_env_latencies(num_envs, control_latency, pd_latency, motor_kp, motor_kd, env_gains)
-        cts, rep, time_step, env_repeats = check_env_repeats(num_envs, task, control_time_step, action_repeat, solver_iterations)
+        cts, rep, time_step, env_repeats = check_env_repeats(num_envs, task_list, control_time_step, action_repeat, solver_iterations)
+        task, signal_type, env_tasks = check_env_tasks(num_envs, task, signal_type, time_step, normalize, frames, frame_delta, mark)
+        # env 0's task and signal in the config, as its rate; rexsim_set_env_tasks gives every env its own
+        task0, signal0 = (task, signal_type) if env_tasks is None else (task[0], signal_type[0])
         if not torch.cuda.is_available():
             raise RuntimeError("rex_gym_b200 needs a CUDA device: there is no CPU fallback")
         self._L = _capi.load()
         self._debug = bool(debug)
+        # the scalars for a scalar construction (an array of equal pairs is one), else the N entries
         self.task, self.signal_type, self.mark = task, signal_type, mark
         # the scalar for a scalar construction (an array of equal entries is one), else the N entries
         self.terrain_type = terrain_scalar if env_terrain is None else tuple(str(t) for t in terrain_type)
@@ -399,7 +484,7 @@ class BatchedRexEnv(object):
             raise ValueError("mark must be 'base' or 'arm'")          # mark_constants.py:1
         tables, toe_npts = pack_model_tables(mark)
         c = _capi.RexSimConfig()
-        c.num_envs, c.task, c.signal = self.num_envs, TASKS[task], SIGNALS[signal_type]
+        c.num_envs, c.task, c.signal = self.num_envs, TASKS[task0], SIGNALS[signal0]
         c.terrain = TERRAINS[terrain_scalar or "random"]
         if env_repeats is None:
             c.num_motors, c.action_repeat = self.num_motors, rep
@@ -417,7 +502,7 @@ class BatchedRexEnv(object):
         c.target_orient = task_value("target_orient", scalar["target_orient"])
         c.init_orient = task_value("init_orient", scalar["init_orient"])
         c.w_distance, c.w_drift, c.w_shake = 1.0, 2.0, 0.005                            # rex_gym_env.py:56-59
-        c.w_energy = energy_weight if energy_weight is not None else (0.005 if task == "gallop" else 0.0005)
+        c.w_energy = energy_weight if energy_weight is not None else (0.005 if task0 == "gallop" else 0.0005)
         c.normalize, c.max_episode_steps, c.auto_reset, c.seed = int(normalize), int(max_episode_steps), int(auto_reset), seed
         c.gait_clock_scale = float(gait_clock_scale)     # GaitPlanner clock / simulation clock (the reference reads the wall clock)
         for k, name in enumerate(("base_y", "base_z", "base_roll", "base_pitch", "base_yaw")):   # poses_env.py:49-53 (None = rotate)
@@ -464,6 +549,8 @@ class BatchedRexEnv(object):
         if env_repeats is not None:
             self._call(self._L.rexsim_set_env_repeats, self._h, env_repeats[0].ctypes.data, env_repeats[1].ctypes.data,
                        stream=False)
+        if env_tasks is not None:
+            self._call(self._L.rexsim_set_env_tasks, self._h, env_tasks[0].ctypes.data, env_tasks[1].ctypes.data, stream=False)
         self._values = None
         if env_values is not None:
             block = np.full((len(TASK_VALUE_KEYWORDS), self.num_envs), np.nan, np.float32)
@@ -522,6 +609,10 @@ class BatchedRexEnv(object):
         if env_repeats is not None:
             _capi.check(self._L.rexsim_env_repeat_buffers(self._h, C.byref(p)))
             self._repeats = view(p, (2, N), "<i4")
+        self._tasks = None                   # [2][N] u8: each env's TASKS and SIGNALS id (per-env tasks only)
+        if env_tasks is not None:
+            _capi.check(self._L.rexsim_env_task_buffers(self._h, C.byref(p)))
+            self._tasks = view(p, (2, N), "|u1")
         self._latency = None                 # [2][N] f64: each env's control_latency, pd_latency (per-env latencies only)
         if env_latency is not None:
             depth = C.c_int32()
@@ -534,20 +625,10 @@ class BatchedRexEnv(object):
             self._episode = dict(score=view(p, (N,), "<f4"), length=view(q, (N,), "<i4"), summary=view(sm, (4,), "<f8"),
                                  block=view(blk, (nb.value,), "|u1"),
                                  objectives=view(o, (4, N), "<f4") if o.value else None)
-        # spaces: raw task spaces, or the wrapper-visible ones when the training wrappers are fused in
-        b = ACTION_BOUND[(task, signal_type)]
-        Oe = env_obs_dim
-        if normalize:
-            self.action_space = Box(-np.inf * np.ones(A, np.float32), np.inf * np.ones(A, np.float32))   # ClipAction wrappers.py:257-260
-            lo, hi = -np.ones(Oe, np.float32), np.ones(Oe, np.float32)                                  # RangeNormalize :204-209
-        else:
-            ha = np.full(A, b, np.float32)
-            self.action_space = Box(ha, -ha) if task == "gallop" else Box(-ha, ha)                       # gallop_env.py:128-130
-            ub = np.full(Oe, 2 * math.pi, np.float32)
-            ub[2:4] = 2 * math.pi / self._time_step
-            lo, hi = -(ub + OBSERVATION_EPS), ub + OBSERVATION_EPS
-        self.observation_space = Box(*frame_space(lo, hi, frames, frame_delta))
-        assert self.observation_space.shape == (O,)
+        # spaces: raw task spaces, or the wrapper-visible ones when the training wrappers are fused in (every env's are these)
+        self.action_space, self.observation_space = task_spaces(task0, signal0, normalize, self._time_step, frames, frame_delta,
+                                                                self.num_motors)
+        assert self.observation_space.shape == (O,) and self.action_space.shape == (A,) and env_obs_dim * max(len(frames), 1) == O
         # every `rebalance_every` steps the envs are re-grouped over the warps by solver cost (rexsim_rebalance): a scheduling
         # hint only -- results are bit-identical with 0 (off).  It pays off once the batch is several waves deep (+17-19 % at
         # 16 384 / 65 536 envs); a batch that fits one wave (4096 envs = 128 CTAs on 132 SMs) is bound by its slowest env anyway
@@ -744,9 +825,16 @@ class BatchedRexEnv(object):
             sd["env_terrain"] = self._terrain.clone()
         if self._repeats is not None:
             sd["env_repeats"] = self._repeats.clone()
+        if self._tasks is not None:
+            sd["env_tasks"] = self._tasks.clone()
         return sd
 
     def load_state_dict(self, sd):
+        if (self._tasks is None) != ("env_tasks" not in sd):
+            raise ValueError("per-env tasks: the checkpoint %s them, this batch %s" %
+                             (("has", "does not") if self._tasks is None else ("lacks", "has")))
+        if self._tasks is not None and not torch.equal(self._tasks, sd["env_tasks"].to(self._tasks.device)):
+            raise ValueError("per-env tasks: the checkpoint's tasks or signals differ from this batch's")
         if (self._repeats is None) != ("env_repeats" not in sd):
             raise ValueError("per-env control rates: the checkpoint %s them, this batch %s" %
                              (("has", "does not") if self._repeats is None else ("lacks", "has")))
@@ -840,10 +928,11 @@ class BatchedRexEnv(object):
 
     def objectives(self):
         """RexGymEnv.get_objectives of the last step for every env: CUDA view [N, 4] of forward, energy, drift, shake before
-        the weights, overwritten by the next step.  Walk and gallop only: the other tasks' rewards have no objectives."""
+        the weights, overwritten by the next step.  Walk and gallop only: the other tasks' rewards have no objectives (in a
+        batch of several tasks with a walking env, their rows are NaN)."""
         o = self._episode_buffer("objectives")
         if o is None:
-            raise ValueError("the %s task records no objectives (its _reward replaces RexGymEnv's)" % self.task)
+            raise ValueError("the %s task records no objectives (its _reward replaces RexGymEnv's)" % (self.task,))
         return o.t()
 
     def episode_score(self):

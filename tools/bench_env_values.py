@@ -23,7 +23,11 @@ contiguous half of the envs ("blocked"), and the sum of a (5 ms, 5) and a (10 ms
 batch of N/2 each, alternately in one process; ms per control step and env-steps/s.  Creation time of walk-ik at 4096 envs
 with 1 rate (scalar) and with 8 rates (r ms, r sub-steps for r = 1..8: 8 settle caps).
 
-Usage: python tools/bench_env_values.py [--steps 200] [--rounds 3] [--workload all|values|latencies|terrains|repeats]"""
+Tasks (--workload tasks): normalized walk-ik and turn-ik at 16 384 and 65 536 envs, all walk, all turn, a 50/50 mix (every
+other env) stepped as two slot ranges of one batch, and the sum of an all-walk and an all-turn batch of N/2 each, alternately
+in one process.
+
+Usage: python tools/bench_env_values.py [--steps 200] [--rounds 3] [--workload all|values|latencies|terrains|repeats|tasks]"""
 import argparse
 import json
 import os
@@ -104,7 +108,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=3, help="step rounds; creation rows take the median of 2 x rounds + 1")
-    ap.add_argument("--workload", choices=("all", "values", "latencies", "terrains", "repeats"), default="all")
+    ap.add_argument("--workload", choices=("all", "values", "latencies", "terrains", "repeats", "tasks"), default="all")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_env_values needs a CUDA device")
@@ -171,7 +175,23 @@ def main():
             rows["8_rates"].append(create_ms(eight))
         print(json.dumps(dict(config="create walk-ik %d envs, plane" % n, **{"ms_" + k: round(median(v), 1) for k, v in rows.items()})),
               flush=True)
-    if a.workload in ("latencies", "terrains", "repeats"):
+    if a.workload in ("all", "tasks"):
+        for n in (16384, 65536):
+            kw = dict(signal_type="ik")
+            rows = {}
+            for _ in range(a.rounds):
+                for name, k in (("walk", dict(kw, num_envs=n, task="walk")),
+                                ("turn", dict(kw, num_envs=n, task="turn")),
+                                ("mixed", dict(kw, num_envs=n, task=["walk", "turn"] * (n // 2))),
+                                ("half_walk", dict(kw, num_envs=n // 2, task="walk")),
+                                ("half_turn", dict(kw, num_envs=n // 2, task="turn"))):
+                    rows.setdefault(name, []).append(ms_per_step(k, a.steps))
+            halves = median(rows["half_walk"]) + median(rows["half_turn"])
+            print(json.dumps(dict(config="walk-ik + turn-ik tasks, normalized", envs=n, steps=a.steps,
+                                  **{"ms_" + k: [round(x, 4) for x in v] for k, v in rows.items()},
+                                  ms_halves_sum=round(halves, 4),
+                                  mixed_vs_halves_pct=round(100 * (median(rows["mixed"]) / halves - 1), 2))), flush=True)
+    if a.workload in ("latencies", "terrains", "repeats", "tasks"):
         return
     for prefix in NAMES:
         name, kw = next(c for c in CONFIGS if c[0].startswith(prefix))
