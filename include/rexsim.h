@@ -378,7 +378,28 @@ int rexsim_env_task_buffers(RexSim* sim, uint8_t** task);
 /* the task and signal of launch group g's step launches: its first env's (the config's for a batch of one group).
  * REXSIM_ERR_INVALID for g outside [0, rexsim_launch_groups). */
 int rexsim_launch_group_task(const RexSim* sim, int32_t g, int32_t* task, int32_t* signal);
-/* launch groups of the batch: 1 unless per-env terrains, repeats or tasks split it (0 for a null handle) */
+/* Per-env marks: the mark of BatchEnv([ctor_0, ctor_1, ...]) over envs with and without the arm, whose spaces agree for every
+ * task but gallop.  num_motors HOST [N] int32, 12 (base) or 18 (arm).  The handle must have been created with 18 motors: the
+ * arm's model table starts with the base's REXSIM_MT_FLOATS floats, its render table draws the base's shapes, and each row of
+ * its sensor history ring holds the base's HW_WORDS words first, so the arm's buffers serve both marks.  Env e then runs
+ * exactly as a batch created with num_motors[e]: its reset hold, its step kernel build, its sensor history (a base env uses
+ * the first 43 words of each 61-word ring row, the rest stay untouched), its renderer shapes.  The mark becomes one more key
+ * of the launch groups, which are (terrain, mark, unit, action_repeat, solver_iterations), terrain-major, then in order of
+ * first appearance, and of the hold settings, (mark, start, motor_kp, motor_kd, pd_latency, solver_iterations), each
+ * (count, start, mark)'s settings contiguous and settled once per terrain.  The command block stays [18][N]: rows 12..17 of
+ * a base env's column are NaN.
+ * Refused (REXSIM_ERR_INVALID) for a handle created with 12 motors, an entry other than 12 or 18, 18 for a gallop env (the
+ * config's task or its per-env task), more than REXSIM_MAX_LAUNCH_GROUPS launch groups or REXSIM_MAX_GAIN_PAIRS hold
+ * settings, after the handle's first reset or step, and on a second call.  Composes with the other per-env setters in any
+ * order; synchronous.  Off: nothing is allocated and every launch is what it is without it. */
+int rexsim_set_env_marks(RexSim* sim, const int32_t* num_motors);
+/* the per-env marks' device buffer, part of a checkpoint's identity: mark dev [N] u8, 1 for the arm, 0 for the base.
+ * REXSIM_ERR_INVALID when the per-env marks are off. */
+int rexsim_env_mark_buffers(RexSim* sim, uint8_t** mark);
+/* the motor count (12 or 18) of launch group g's step launches (the config's for a batch of one group).
+ * REXSIM_ERR_INVALID for g outside [0, rexsim_launch_groups). */
+int rexsim_launch_group_mark(const RexSim* sim, int32_t g, int32_t* num_motors);
+/* launch groups of the batch: 1 unless per-env terrains, repeats, tasks or marks split it (0 for a null handle) */
 int rexsim_launch_groups(const RexSim* sim);
 /* launch group g: info[REXSIM_GROUP_WORDS] = terrain, action_repeat, solver_iterations, first slot, slot count, and the
  * build its last step launch used (CTA size, CTAs per SM, sensor; all 0 before the first step).  A batch of one group

@@ -82,6 +82,9 @@ SIGNATURES = {
     "rexsim_set_env_tasks": (C.c_int, [_ptr] * 3),
     "rexsim_env_task_buffers": (C.c_int, [_ptr, _out(_ptr)]),
     "rexsim_launch_group_task": (C.c_int, [_ptr, _i32, _out(_i32), _out(_i32)]),
+    "rexsim_set_env_marks": (C.c_int, [_ptr] * 2),
+    "rexsim_env_mark_buffers": (C.c_int, [_ptr, _out(_ptr)]),
+    "rexsim_launch_group_mark": (C.c_int, [_ptr, _i32, _out(_i32)]),
     "rexsim_launch_groups": (C.c_int, [_ptr]),
     "rexsim_launch_group": (C.c_int, [_ptr, _i32, _ptr]),
     "rexsim_slot_buffers": (C.c_int, [_ptr, _out(_ptr), _out(_ptr)]),

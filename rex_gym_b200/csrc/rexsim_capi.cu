@@ -22,10 +22,11 @@ cudaError_t launch_render(const Params& P, const float* rt, const float* zrange,
 
 using namespace rexsim;
 
-// One launch of the step kernel per control step: the envs of one (terrain, step unit, action_repeat, solver_iterations), which
-// own slots perm[first, first + count); task, signal: the group's first env's, whose unit_of is the group's unit
+// One launch of the step kernel per control step: the envs of one (terrain, mark, step unit, action_repeat, solver_iterations),
+// which own slots perm[first, first + count); task, signal: the group's first env's, whose unit_of is the group's unit;
+// motors: the mark's motor count, 12 or 18
 struct LaunchGroup {
-    int32_t terrain, task, signal, repeat, iters, first, count;
+    int32_t terrain, motors, task, signal, repeat, iters, first, count;
     int32_t launched[3];               // step_kernel instance of the group's last launch: BLOCK, OCC, SENSOR
 };
 
@@ -49,6 +50,7 @@ struct RexSim {
                                        // P.el.hold (0: no table)
     std::vector<int32_t> hold_iters;   // [nholds] PGS cap of each hold setting, each cap's settings contiguous
     std::vector<int32_t> hold_start;   // [nholds] start pose of each (hold_start), each (cap, start)'s settings contiguous
+    std::vector<int32_t> hold_motors;  // [nholds] motor count of each, each (cap, start, motors)'s settings contiguous
     bool values_on = false;            // rexsim_set_env_values was called
     std::vector<float> kp, kd;         // per-env gains given to rexsim_set_env_values (empty: the config's)
     std::vector<double> pd;            // per-env pd latencies given to rexsim_set_env_latencies (empty: the config's)
@@ -60,6 +62,10 @@ struct RexSim {
     std::vector<int32_t> rep, iters;   // the same on the host (empty: the config's)
     uint8_t* tasks = nullptr;          // [2][N] per-env task, signal (rexsim_set_env_tasks; null: off); P.env_task points here
     std::vector<uint8_t> task, signal; // the same on the host (empty: the config's)
+    uint8_t* marks = nullptr;          // [N] per-env marks, 1 arm / 0 base (rexsim_set_env_marks; null: off); P.env_mark points here
+    std::vector<int32_t> motors;       // each env's motor count, 12 or 18, on the host (empty: the config's)
+    float* snap_ring_base = nullptr;   // per-env marks with the sensor model: the base envs' snapshot ring, [settings * fields][D]
+                                       // [HW_WORDS] (P.snap_ring is the arm's); the base launches read it as their P.snap_ring
     // The launch groups (empty: one launch over every slot with the config's values), terrain-major, plane first, then in
     // order of first appearance; group g owns slots perm[first_g, first_g + count_g).  `group` is each env's group, the key
     // rexsim_rebalance sorts on: the terrain bytes when the groups are exactly the two terrains, its own [N] bytes otherwise;
@@ -71,11 +77,13 @@ struct RexSim {
     int32_t launched[3] = {0, 0, 0};   // step_kernel instance of the last step launch: BLOCK, OCC, SENSOR
 };
 
-// The handle's Params for the launches over one group's envs: its terrain with that terrain's friction, its task and signal
-// (launch_step's unit, the auto-reset's draws, the settle's start pose), its sub-steps per control step and its PGS cap
+// The handle's Params for the launches over one group's envs: its terrain with that terrain's friction, its mark (the base or
+// arm build of the step and settle kernels), its task and signal (launch_step's unit, the auto-reset's draws, the settle's
+// start pose), its sub-steps per control step and its PGS cap
 static Params group_params(const RexSim* s, Params P, const LaunchGroup& g) {
     if (s->terrain) P.cfg.friction = s->friction[g.terrain];
-    P.cfg.terrain = g.terrain; P.cfg.task = g.task; P.cfg.signal = g.signal;
+    if (s->marks && g.motors == 12) P.snap_ring = s->snap_ring_base;
+    P.cfg.terrain = g.terrain; P.cfg.num_motors = g.motors; P.cfg.task = g.task; P.cfg.signal = g.signal;
     P.cfg.action_repeat = g.repeat; P.cfg.solver_iterations = g.iters;
     return P;
 }
@@ -358,6 +366,13 @@ int rexsim_reset(RexSim* s, const int32_t* idx, int32_t k, float* obs_out, void*
     Params P = s->P;
     P.reset_idx = idx; P.reset_k = k;
     s->started = true;
+    if (s->marks) {
+        // a batch of both marks: the base instance, on the base envs' snapshot ring, then the arm instance; each writes only
+        // the envs of its own mark (P.env_mark)
+        Params B = P;
+        B.cfg.num_motors = 12; B.snap_ring = s->snap_ring_base;
+        if (int rc = enqueue(s, launch_reset(B, obs_out, (cudaStream_t)stream), "reset launch", !idx || k > 0)) return rc;
+    }
     return enqueue(s, launch_reset(P, obs_out, (cudaStream_t)stream), "reset launch", !idx || k > 0);
 }
 
@@ -491,39 +506,50 @@ static int32_t hold_start(int task, int signal) {
     return task == REXSIM_TASK_STANDUP ? START_FOLD : task == REXSIM_TASK_POSES ? START_NONE
          : signal == REXSIM_SIGNAL_OL ? START_OL : START_IK;
 }
-// The reset hold's settings: each env's (start, motor_kp, motor_kd, pd_latency, solver_iterations), distinct ones in order of
-// first appearance within each (PGS cap, start), the starts in order of first appearance within each cap and the caps in order
-// of first appearance (each cap's and each (cap, start)'s settings contiguous), and each env's index into them.  Rex.Reset
-// clears the history and holds through ApplyAction (rex.py:303-323), so the settled state depends on the pose held, the gains,
-// the PD observation's latency and the solver's cap.  start, kp, kd, pd, iters: per env, or empty for the config's scalar.
-struct HoldTable { std::vector<float> gains; std::vector<double> pd; std::vector<int32_t> iters, start, index; };
-static int hold_table(const RexSimConfig& c, size_t N, const std::vector<int32_t>& start, const std::vector<float>& kp,
-                      const std::vector<float>& kd, const std::vector<double>& pd, const std::vector<int32_t>& iters, HoldTable& t) {
+// The reset hold's settings: each env's (mark, start, motor_kp, motor_kd, pd_latency, solver_iterations), distinct ones in
+// order of first appearance within each (PGS cap, start, mark), the marks in order of first appearance within each (cap,
+// start), the starts within each cap and the caps in order of first appearance (each cap's, (cap, start)'s and (cap, start,
+// mark)'s settings contiguous), and each env's index into them.  Rex.Reset clears the history and holds through ApplyAction
+// (rex.py:303-323), so the settled state depends on the robot held, the pose held, the gains, the PD observation's latency
+// and the solver's cap.  motors, start, kp, kd, pd, iters: per env, or empty for the config's scalar.
+struct HoldTable { std::vector<float> gains; std::vector<double> pd; std::vector<int32_t> iters, start, motors, index; };
+static int hold_table(const RexSimConfig& c, size_t N, const std::vector<int32_t>& motors, const std::vector<int32_t>& start,
+                      const std::vector<float>& kp, const std::vector<float>& kd, const std::vector<double>& pd,
+                      const std::vector<int32_t>& iters, HoldTable& t) {
     t.index.assign(N, 0);
     auto cap_of = [&](size_t e) { return iters.empty() ? c.solver_iterations : iters[e]; };
     auto start_of = [&](size_t e) { return start.empty() ? hold_start(c.task, c.signal) : start[e]; };
+    auto motors_of = [&](size_t e) { return motors.empty() ? c.num_motors : motors[e]; };
     std::vector<int32_t> caps;
     for (size_t e = 0; e < N; e++)
         if (std::find(caps.begin(), caps.end(), cap_of(e)) == caps.end()) caps.push_back(cap_of(e));
-    std::vector<std::pair<int32_t, int32_t>> keys;             // (cap, start): each cap's starts in order of first appearance
+    std::vector<std::pair<int32_t, int32_t>> starts;           // (cap, start): each cap's starts in order of first appearance
     for (const int32_t cap : caps)
         for (size_t e = 0; e < N; e++) {
             const std::pair<int32_t, int32_t> k(cap, start_of(e));
-            if (cap_of(e) == cap && std::find(keys.begin(), keys.end(), k) == keys.end()) keys.push_back(k);
+            if (cap_of(e) == cap && std::find(starts.begin(), starts.end(), k) == starts.end()) starts.push_back(k);
         }
-    for (const std::pair<int32_t, int32_t>& key : keys)
+    std::vector<std::pair<std::pair<int32_t, int32_t>, int32_t>> keys;   // ((cap, start), motors), marks by first appearance
+    for (const std::pair<int32_t, int32_t>& cs : starts)
         for (size_t e = 0; e < N; e++) {
-            const int32_t it = cap_of(e), st = start_of(e);
-            if (it != key.first || st != key.second) continue;
+            const std::pair<std::pair<int32_t, int32_t>, int32_t> k(cs, motors_of(e));
+            if (cap_of(e) == cs.first && start_of(e) == cs.second && std::find(keys.begin(), keys.end(), k) == keys.end())
+                keys.push_back(k);
+        }
+    for (const std::pair<std::pair<int32_t, int32_t>, int32_t>& key : keys)
+        for (size_t e = 0; e < N; e++) {
+            const int32_t it = cap_of(e), st = start_of(e), nm = motors_of(e);
+            if (it != key.first.first || st != key.first.second || nm != key.second) continue;
             const float k = kp.empty() ? c.motor_kp : kp[e], d = kd.empty() ? c.motor_kd : kd[e];
             const double l = pd.empty() ? c.pd_latency : pd[e];
             size_t h = 0;
             while (h < t.pd.size() && !(t.gains[2 * h] == k && t.gains[2 * h + 1] == d && t.pd[h] == l && t.iters[h] == it &&
-                                        t.start[h] == st)) h++;
+                                        t.start[h] == st && t.motors[h] == nm)) h++;
             if (h == t.pd.size()) {
                 if ((int)h == REXSIM_MAX_GAIN_PAIRS)
-                    return fail(REXSIM_ERR_INVALID, "more than 64 distinct reset-hold settings (start pose, motor_kp, motor_kd, pd_latency, solver_iterations)");
+                    return fail(REXSIM_ERR_INVALID, "more than 64 distinct reset-hold settings (mark, start pose, motor_kp, motor_kd, pd_latency, solver_iterations)");
                 t.gains.push_back(k); t.gains.push_back(d); t.pd.push_back(l); t.iters.push_back(it); t.start.push_back(st);
+                t.motors.push_back(nm);
             }
             t.index[e] = (int32_t)h;
         }
@@ -539,16 +565,16 @@ static std::vector<int32_t> env_starts(const std::vector<uint8_t>& task, const s
 static std::vector<LaunchGroup> launch_groups(const RexSim* s) {
     if (!s->groups.empty()) return s->groups;
     const RexSimConfig& c = s->P.cfg;
-    return {LaunchGroup{c.terrain, c.task, c.signal, c.action_repeat, c.solver_iterations, 0, s->P.N,
+    return {LaunchGroup{c.terrain, c.num_motors, c.task, c.signal, c.action_repeat, c.solver_iterations, 0, s->P.N,
                         {s->launched[0], s->launched[1], s->launched[2]}}};
 }
-// Each env's launch group: the groups (terrain, step unit, action_repeat, solver_iterations), terrain-major, plane first, then
-// in order of first appearance, from the per-env terrains, repeats, iteration counts, tasks and signals given (each empty for
-// the config's).  Refused past REXSIM_MAX_LAUNCH_GROUPS groups.
+// Each env's launch group: the groups (terrain, mark, step unit, action_repeat, solver_iterations), terrain-major, plane first,
+// then in order of first appearance, from the per-env terrains, repeats, iteration counts, tasks, signals and motor counts
+// given (each empty for the config's).  Refused past REXSIM_MAX_LAUNCH_GROUPS groups.
 struct GroupPlan { std::vector<LaunchGroup> gs; std::vector<uint8_t> key; };
 static int plan_groups(const RexSim* s, const std::vector<uint8_t>& terr, const std::vector<int32_t>& rep,
                        const std::vector<int32_t>& iters, const std::vector<uint8_t>& task, const std::vector<uint8_t>& signal,
-                       GroupPlan& p) {
+                       const std::vector<int32_t>& motors, GroupPlan& p) {
     const RexSimConfig& c = s->P.cfg;
     const size_t N = s->P.N;
     p.gs.clear();
@@ -559,13 +585,15 @@ static int plan_groups(const RexSim* s, const std::vector<uint8_t>& terr, const 
             const int32_t r = rep.empty() ? c.action_repeat : rep[e];
             const int32_t it = iters.empty() ? c.solver_iterations : iters[e];
             const int32_t k = task.empty() ? c.task : task[e], sg = signal.empty() ? c.signal : signal[e];
+            const int32_t nm = motors.empty() ? c.num_motors : motors[e];
             size_t g = 0;
-            while (g < p.gs.size() && !(p.gs[g].terrain == t && unit_of(p.gs[g].task, p.gs[g].signal) == unit_of(k, sg) &&
+            while (g < p.gs.size() && !(p.gs[g].terrain == t && p.gs[g].motors == nm &&
+                                        unit_of(p.gs[g].task, p.gs[g].signal) == unit_of(k, sg) &&
                                         p.gs[g].repeat == r && p.gs[g].iters == it)) g++;
             if (g == p.gs.size()) {
                 if ((int)g == REXSIM_MAX_LAUNCH_GROUPS)
-                    return fail(REXSIM_ERR_INVALID, "more than 16 launch groups (terrain, task unit, action_repeat, solver_iterations)");
-                p.gs.push_back(LaunchGroup{t, k, sg, r, it, 0, 0, {0, 0, 0}});
+                    return fail(REXSIM_ERR_INVALID, "more than 16 launch groups (terrain, mark, task unit, action_repeat, solver_iterations)");
+                p.gs.push_back(LaunchGroup{t, nm, k, sg, r, it, 0, 0, {0, 0, 0}});
             }
             p.gs[g].count++;
             p.key[e] = (uint8_t)g;
@@ -578,7 +606,7 @@ static int build_groups(RexSim* s) {
     Params& P = s->P;
     const size_t N = P.N;
     GroupPlan plan;
-    if (int rc = plan_groups(s, s->terr, s->rep, s->iters, s->task, s->signal, plan)) return rc;
+    if (int rc = plan_groups(s, s->terr, s->rep, s->iters, s->task, s->signal, s->motors, plan)) return rc;
     std::vector<LaunchGroup>& gs = plan.gs;
     const std::vector<uint8_t>& key = plan.key;
     std::vector<int32_t> at(gs.size()), perm(N);
@@ -607,9 +635,9 @@ static int build_groups(RexSim* s) {
     return REXSIM_OK;
 }
 // Run the reset hold again for every snapshot of the layout P.snaps, at the handle's hold settings (the config's one without a
-// table), its sensor history rows at the handle's ring depth: one launch per (terrain, PGS cap, start pose) the launch groups
-// hold, each at that terrain's friction, with that cap and with a task and signal of that start, over all the (cap, start)'s
-// (setting, field) snapshots.  Synchronous.
+// table), its sensor history rows at the handle's ring depth and row width: one launch per (terrain, PGS cap, start pose, mark)
+// the launch groups hold, each at that terrain's friction, with that cap, with a task and signal of that start and with that
+// mark's build, over all the (cap, start, mark)'s (setting, field) snapshots.  Synchronous.
 static int settle_snapshots(RexSim* s) {
     Params& P = s->P;
     const int nh = s->nholds > 0 ? s->nholds : 1;
@@ -623,21 +651,28 @@ static int settle_snapshots(RexSim* s) {
         s->mem.drop(P.snap_ring);
         P.snap_ring = nullptr;
         if (s->mem.zeroed(&P.snap_ring, nsettle * P.ring_depth * sensor_cfg(&P.cfg).words)) return REXSIM_ERR_CUDA;
+        if (s->marks) {                        // the base envs' snapshots, at the base's row width
+            s->mem.drop(s->snap_ring_base);
+            s->snap_ring_base = nullptr;
+            if (s->mem.zeroed(&s->snap_ring_base, nsettle * P.ring_depth * HW_WORDS)) return REXSIM_ERR_CUDA;
+        }
     }
     const std::vector<int32_t> caps = s->nholds > 0 ? s->hold_iters : std::vector<int32_t>{P.cfg.solver_iterations};
     const std::vector<int32_t> starts = s->nholds > 0 ? s->hold_start : std::vector<int32_t>{hold_start(P.cfg.task, P.cfg.signal)};
+    const std::vector<int32_t> motors = s->nholds > 0 ? s->hold_motors : std::vector<int32_t>{P.cfg.num_motors};
     const std::vector<LaunchGroup> gs = launch_groups(s);
     auto same_hold = [](const LaunchGroup& a, const LaunchGroup& b) {
-        return a.terrain == b.terrain && a.iters == b.iters && hold_start(a.task, a.signal) == hold_start(b.task, b.signal);
+        return a.terrain == b.terrain && a.iters == b.iters && hold_start(a.task, a.signal) == hold_start(b.task, b.signal) &&
+               a.motors == b.motors;
     };
     for (size_t g = 0; g < gs.size(); g++) {
-        bool settled = false;                  // an earlier group on the same terrain with the same cap and start
+        bool settled = false;                  // an earlier group on the same terrain with the same cap, start and mark
         for (size_t h = 0; h < g; h++) settled = settled || same_hold(gs[h], gs[g]);
         if (settled) continue;
         const int32_t st = hold_start(gs[g].task, gs[g].signal);
-        int first = -1, count = 0;             // the (cap, start)'s settings are contiguous
+        int first = -1, count = 0;             // the (cap, start, mark)'s settings are contiguous
         for (size_t h = 0; h < caps.size(); h++)
-            if (caps[h] == gs[g].iters && starts[h] == st) { first = first < 0 ? (int)h : first; count++; }
+            if (caps[h] == gs[g].iters && starts[h] == st && motors[h] == gs[g].motors) { first = first < 0 ? (int)h : first; count++; }
         const Params G = group_params(s, P, gs[g]);
         if (int rc = enqueue(s, launch_settle(G, snap_f, snap_i, first, count, 0), "settle launch")) return rc;
     }
@@ -668,6 +703,7 @@ static int apply_holds(RexSim* s, const HoldTable& t, bool settle) {
     s->nholds = (int)nh;
     s->hold_iters = t.iters;
     s->hold_start = t.start;
+    s->hold_motors = t.motors;
     return settle ? settle_snapshots(s) : REXSIM_OK;
 }
 int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const float* kd) {
@@ -688,9 +724,9 @@ int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const
         for (size_t e = 0; e < N; e++)
             if (!(kp[e] >= 0.f) || !(kd[e] >= 0.f) || std::isinf(kp[e]) || std::isinf(kd[e]))
                 return fail(REXSIM_ERR_INVALID, "gains must be finite and non-negative");
-        if (int rc = hold_table(c, N, env_starts(s->task, s->signal), std::vector<float>(kp, kp + N), std::vector<float>(kd, kd + N), s->pd, s->iters, t)) return rc;
+        if (int rc = hold_table(c, N, s->motors, env_starts(s->task, s->signal), std::vector<float>(kp, kp + N), std::vector<float>(kd, kd + N), s->pd, s->iters, t)) return rc;
     } else if (!P.ev.pair) {
-        if (int rc = hold_table(c, N, env_starts(s->task, s->signal), s->kp, s->kd, s->pd, s->iters, t)) return rc;          // the config's one setting
+        if (int rc = hold_table(c, N, s->motors, env_starts(s->task, s->signal), s->kp, s->kd, s->pd, s->iters, t)) return rc;          // the config's one setting
     }
     float* block = nullptr;
     if (s->mem.zeroed(&block, (size_t)REXSIM_VALUE_BLOCK_ROWS * N)) return REXSIM_ERR_CUDA;
@@ -732,7 +768,7 @@ int rexsim_set_env_latencies(RexSim* s, const double* control_latency, const dou
     }
     HoldTable t;
     const std::vector<double> pd(lat.begin() + N, lat.end());
-    if (int rc = hold_table(c, N, env_starts(s->task, s->signal), s->kp, s->kd, pd, s->iters, t)) return rc;
+    if (int rc = hold_table(c, N, s->motors, env_starts(s->task, s->signal), s->kp, s->kd, pd, s->iters, t)) return rc;
     double* dlat = nullptr;
     EnvDelay* denv = nullptr;
     if (s->mem.zeroed(&dlat, 2 * N) || s->mem.zeroed(&denv, N)) return REXSIM_ERR_CUDA;
@@ -774,7 +810,7 @@ int rexsim_set_env_terrains(RexSim* s, const int32_t* terrain, float plane_frict
         nplane += terrain[e] == REXSIM_TERRAIN_PLANE;
     }
     GroupPlan plan;
-    if (int rc = plan_groups(s, bytes, s->rep, s->iters, s->task, s->signal, plan)) return rc;
+    if (int rc = plan_groups(s, bytes, s->rep, s->iters, s->task, s->signal, s->motors, plan)) return rc;
     uint8_t* dterrain = nullptr;
     if (s->mem.zeroed(&dterrain, N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(dterrain, bytes.data(), N, cudaMemcpyHostToDevice));
@@ -813,9 +849,9 @@ int rexsim_set_env_repeats(RexSim* s, const int32_t* action_repeat, const int32_
         }
     }
     GroupPlan plan;
-    if (int rc = plan_groups(s, s->terr, rep, iters, s->task, s->signal, plan)) return rc;
+    if (int rc = plan_groups(s, s->terr, rep, iters, s->task, s->signal, s->motors, plan)) return rc;
     HoldTable t;
-    if (int rc = hold_table(c, N, env_starts(s->task, s->signal), s->kp, s->kd, s->pd, iters, t)) return rc;
+    if (int rc = hold_table(c, N, s->motors, env_starts(s->task, s->signal), s->kp, s->kd, s->pd, iters, t)) return rc;
     int32_t* d = nullptr;
     if (s->mem.zeroed(&d, 2 * N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(d, rep.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
@@ -856,9 +892,9 @@ int rexsim_set_env_tasks(RexSim* s, const int32_t* task, const int32_t* signal) 
         objectives = objectives || k == REXSIM_TASK_WALK || k == REXSIM_TASK_GALLOP;
     }
     GroupPlan plan;
-    if (int rc = plan_groups(s, s->terr, s->rep, s->iters, tk, sg, plan)) return rc;
+    if (int rc = plan_groups(s, s->terr, s->rep, s->iters, tk, sg, s->motors, plan)) return rc;
     HoldTable t;
-    if (int rc = hold_table(c, N, env_starts(tk, sg), s->kp, s->kd, s->pd, s->iters, t)) return rc;
+    if (int rc = hold_table(c, N, s->motors, env_starts(tk, sg), s->kp, s->kd, s->pd, s->iters, t)) return rc;
     uint8_t* d = nullptr;
     if (s->mem.zeroed(&d, 2 * N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(d, tk.data(), N, cudaMemcpyHostToDevice));
@@ -888,6 +924,57 @@ int rexsim_launch_group_task(const RexSim* s, int32_t g, int32_t* task, int32_t*
     const std::vector<LaunchGroup> gs = launch_groups(s);
     if (g < 0 || g >= (int32_t)gs.size()) return fail(REXSIM_ERR_INVALID, "no such launch group");
     *task = gs[g].task; *signal = gs[g].signal;
+    return REXSIM_OK;
+}
+int rexsim_set_env_marks(RexSim* s, const int32_t* num_motors) {
+    if (!s || !num_motors) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env marks must be set before the first reset or step");
+    if (s->marks) return fail(REXSIM_ERR_INVALID, "per-env marks are already set");
+    Params& P = s->P;
+    const RexSimConfig& c = P.cfg;
+    const size_t N = P.N;
+    // the arm's model table starts with the base's (REXSIM_MT_FLOATS), its render table draws the base's shapes, its ring rows
+    // hold the base's words first: a handle built for the arm serves base envs, not the other way round
+    if (c.num_motors != 18) return fail(REXSIM_ERR_INVALID, "per-env marks need a handle created with the arm (num_motors 18)");
+    std::vector<int32_t> nm(N);
+    std::vector<uint8_t> bytes(N);
+    for (size_t e = 0; e < N; e++) {
+        if (num_motors[e] != 12 && num_motors[e] != 18) return fail(REXSIM_ERR_INVALID, "mark entries must be 12 (base) or 18 (arm)");
+        const int32_t task = s->task.empty() ? c.task : s->task[e];
+        if (num_motors[e] == 18 && task == REXSIM_TASK_GALLOP)
+            return fail(REXSIM_ERR_INVALID, "mark='arm' is built for every task but gallop");
+        nm[e] = num_motors[e];
+        bytes[e] = (uint8_t)(num_motors[e] == 18);
+    }
+    GroupPlan plan;
+    if (int rc = plan_groups(s, s->terr, s->rep, s->iters, s->task, s->signal, nm, plan)) return rc;
+    HoldTable t;
+    if (int rc = hold_table(c, N, nm, env_starts(s->task, s->signal), s->kp, s->kd, s->pd, s->iters, t)) return rc;
+    uint8_t* d = nullptr;
+    if (s->mem.zeroed(&d, N)) return REXSIM_ERR_CUDA;
+    CK(cudaMemcpy(d, bytes.data(), N, cudaMemcpyHostToDevice));
+    // rows 12..17 of the [18][N] command block (still zero: nothing has stepped): NaN in a base env's column, which the base
+    // build never writes
+    std::vector<float> arm_rows(6 * N, 0.f);
+    for (size_t e = 0; e < N; e++)
+        if (!bytes[e]) for (int j = 0; j < 6; j++) arm_rows[j * N + e] = NAN;
+    CK(cudaMemcpy(P.cmd_out + 12 * N, arm_rows.data(), 6 * N * sizeof(float), cudaMemcpyHostToDevice));
+    s->marks = d; s->motors = nm;
+    P.env_mark = d;
+    if (int rc = build_groups(s)) return rc;
+    return apply_holds(s, t, true);
+}
+int rexsim_env_mark_buffers(RexSim* s, uint8_t** mark) {
+    if (!s || !mark) return fail(REXSIM_ERR_INVALID, "null argument");
+    if (!s->marks) return fail(REXSIM_ERR_INVALID, "per-env marks are off (rexsim_set_env_marks)");
+    *mark = s->marks;
+    return REXSIM_OK;
+}
+int rexsim_launch_group_mark(const RexSim* s, int32_t g, int32_t* num_motors) {
+    if (!s || !num_motors) return fail(REXSIM_ERR_INVALID, "null argument");
+    const std::vector<LaunchGroup> gs = launch_groups(s);
+    if (g < 0 || g >= (int32_t)gs.size()) return fail(REXSIM_ERR_INVALID, "no such launch group");
+    *num_motors = gs[g].motors;
     return REXSIM_OK;
 }
 int rexsim_launch_groups(const RexSim* s) { return s ? (int)launch_groups(s).size() : 0; }

@@ -2083,7 +2083,9 @@ __global__ void __launch_bounds__(BLOCK, (OCC * 128) / BLOCK) step_kernel(const 
 
 // -------------------------------------------------------------------------------------------------
 // reset kernel: BatchEnv.reset(indices).  The WALK instance serves every task but gallop (their observations are the same
-// four base terms); each env's draws follow its own task (P.env_task), so one launch resets envs of several tasks.
+// four base terms); each env's draws follow its own task (P.env_task), so one launch resets envs of several tasks.  A batch of
+// both marks (P.env_mark) launches the base and the arm instance, each writing only the envs of its own mark: an env's sensor
+// history column is addressed with its mark's row width, and read from its mark's snapshot ring (P.snap_ring of the launch).
 // -------------------------------------------------------------------------------------------------
 template <int TASK, bool ARM>
 __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_out) {
@@ -2098,7 +2100,7 @@ __global__ void __launch_bounds__(128) reset_kernel(const Params P, float* obs_o
     // error word gets REXSIM_FLAG_BAD_INDEX (the Python mirror raises IndexError like BatchEnv.reset would)
     const bool inrange = env >= 0 && env < P.N;
     if (!inrange) { if (valid && leg == 0) atomicOr(&P.err[P.N], REXSIM_FLAG_BAD_INDEX); env = 0; }
-    const bool wr = valid && inrange;
+    const bool wr = valid && inrange && (!P.env_mark || (P.env_mark[env] != 0) == ARM);      // the other mark's launch writes it
     Lane L; Task K; Arm AR; float kp, kd; int field;
     Sensor S = make_sensor<ARM>(P, P.ring, P.N, env, (uint32_t)env + (uint32_t)P.cfg.env_offset);
     const int terrain = P.env_terrain ? (int)P.env_terrain[env] : P.cfg.terrain;

@@ -172,13 +172,21 @@ struct Params {
     // sensor model (control / PD latency, observation noise: rex.py:735-769); all unused when sensor_on == 0
     int32_t sensor_on;
     int32_t ring_depth;                // D rows kept per env: the batch's largest n + 2 (100 = the deque's maxlen when a latency reaches it)
-    float* ring;                       // [D][HW_WORDS(_ARM)][N]; NOT __restrict__: lanes of an env read what lane 0 wrote
+    // [D][HW_WORDS(_ARM)][N]; NOT __restrict__: lanes of an env read what lane 0 wrote.  In a batch of both marks it is
+    // [D][HW_WORDS_ARM][N] words and a base env's column holds its [D][HW_WORDS] rows in its first D * HW_WORDS words: only
+    // launches of the env's own mark address it
+    float* ring;
     float* snap_ring;                  // [npairs * fields][D][HW_WORDS(_ARM)] history the reset hold leaves behind, per snapshot
+                                       // (a batch of both marks: one ring per mark, the launch's)
     Delay ctl, pd;                     // the config's control and PD latency (per env: EnvLatencies)
     float noise_sd[5];                 // SENSOR_NOISE_STDDEV order: motor angle, motor velocity, motor torque, base rpy, base rpy rate
     // per-env tasks (rexsim_set_env_tasks; null: every env runs cfg.task): [2][N] REXSIM_TASK_* row, REXSIM_SIGNAL_* row, by
     // env.  Only the reset kernel reads it: each step launch covers one launch group, with the group's task in cfg.task.
     const uint8_t* __restrict__ env_task;
+    // per-env marks (rexsim_set_env_marks; null: every env carries cfg.num_motors): [N] by env, 1 for the arm, 0 for the base.
+    // The reset kernel (one launch per mark, each skipping the other mark's envs) and the renderer read it; each step and
+    // settle launch covers one mark, the launch group's cfg.num_motors.
+    const uint8_t* __restrict__ env_mark;
 };
 
 // ----- tiny vector algebra ---------------------------------------------------------------------------

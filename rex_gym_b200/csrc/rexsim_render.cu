@@ -29,6 +29,7 @@ struct RenderArgs {
     uint8_t* __restrict__ rgb;          // [k][H][W][3]
     int32_t* __restrict__ err;          // [N + 1]: word N = aggregate error bits
     const uint8_t* __restrict__ env_terrain;   // [N] terrain of each env (per-env terrains), else null: `terrain` for all
+    const uint8_t* __restrict__ env_mark;      // [N] 1 for an arm env (per-env marks), else null: `arm` for all
     int N, terrain, arm, toe_npts;
     int W, H, tiles_x, image0;
     float dist, yaw, pitch;             // radians
@@ -91,8 +92,8 @@ __device__ __forceinline__ void write_sphere(float* rec, V3 c, float r) {
 }
 __device__ __forceinline__ V3 ld3(const float* p) { return mk(p[0], p[1], p[2]); }
 
-// warp 0: pose every shape of env `env` into `shapes` (world frame)
-__device__ void pose_shapes(const RenderArgs& A, int env, float* shapes, int lane) {
+// warp 0: pose every shape of env `env` into `shapes` (world frame); `arm`: the env carries the arm
+__device__ void pose_shapes(const RenderArgs& A, int env, bool arm, float* shapes, int lane) {
     const size_t N = A.N;
     const float* sf = A.sf;
     const V3 pos = mk(sf[(F_POS + 0) * N + env], sf[(F_POS + 1) * N + env], sf[(F_POS + 2) * N + env]);
@@ -115,7 +116,7 @@ __device__ void pose_shapes(const RenderArgs& A, int env, float* shapes, int lan
         write_sphere(toe, p3 + mul(R3, mk(ts[0], 0.f, ts[1])), ts[2]);
     } else if (lane < 7) {     // base and chassis boxes
         write_box(shapes + (lane - 4) * SHAPE_FLOATS, mt + REXSIM_MT_BASEBOX + 24 * (lane - 4), R0, pos);
-    } else if (lane == 7 && A.arm) {   // the arm: one serial chain with general joint frames (rexsim_arm.cuh layout)
+    } else if (lane == 7 && arm) {   // the arm: one serial chain with general joint frames (rexsim_arm.cuh layout)
         M3 Rp = R0; V3 pp = pos;
         for (int j = 0; j < ARM_NJ; j++) {
             M3 Rj; V3 pj;
@@ -277,13 +278,14 @@ __global__ void __launch_bounds__(RT_TILE * RT_TILE) render_kernel(const RenderA
     const int tile = blockIdx.x, c0 = (tile % A.tiles_x) * RT_TILE, r0 = (tile / A.tiles_x) * RT_TILE;
     const float tan_half = tanf(0.5f * A.rt[REXSIM_RT_CAM] * (3.14159265358979323846f / 180.f)), aspect = (float)A.W / (float)A.H;
     const float inv_w = 1.f / (float)A.W, inv_h = 1.f / (float)A.H;
-    const int nshapes = A.arm ? REXSIM_RT_NSHAPES : 19;
+    const bool arm = valid && (A.env_mark ? A.env_mark[env] != 0 : A.arm != 0);      // the env's own mark
+    const int nshapes = arm ? REXSIM_RT_NSHAPES : 19;
     Camera C;
     if (valid) C = make_camera(mk(A.sf[(F_POS + 0) * (size_t)A.N + env], A.sf[(F_POS + 1) * (size_t)A.N + env],
                                   A.sf[(F_POS + 2) * (size_t)A.N + env]), A.dist, A.yaw, A.pitch, tan_half, aspect);
     if (tid < 32) {
         if (valid) {
-            pose_shapes(A, env, shapes, tid);
+            pose_shapes(A, env, arm, shapes, tid);
             __syncwarp();
             // frustum of the tile: the four planes through the eye spanned by its extreme pixel rays
             const int c1 = min(c0 + RT_TILE, A.W) - 1, r1 = min(r0 + RT_TILE, A.H) - 1;
@@ -369,7 +371,8 @@ cudaError_t launch_render(const Params& P, const float* rt, const float* zrange,
                           float distance, float yaw_deg, float pitch_deg, uint8_t* rgb, cudaStream_t st, int* launches) {
     RenderArgs A;
     A.sf = P.sf; A.si = P.si; A.model = P.model; A.rt = rt; A.fields = P.cfg.fields; A.zoff = P.field_zoff; A.zrange = zrange;
-    A.idx = idx; A.err = P.err; A.N = P.N; A.terrain = P.cfg.terrain; A.env_terrain = P.env_terrain; A.arm = P.cfg.num_motors == 18; A.toe_npts = P.cfg.toe_npts;
+    A.idx = idx; A.err = P.err; A.N = P.N; A.terrain = P.cfg.terrain; A.env_terrain = P.env_terrain; A.env_mark = P.env_mark;
+    A.arm = P.cfg.num_motors == 18; A.toe_npts = P.cfg.toe_npts;
     A.W = W; A.H = H; A.dist = distance;
     A.yaw = yaw_deg * (float)(3.14159265358979323846 / 180.0); A.pitch = pitch_deg * (float)(3.14159265358979323846 / 180.0);
     const int tiles_y = (H + RT_TILE - 1) / RT_TILE;

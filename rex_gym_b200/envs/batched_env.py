@@ -24,6 +24,7 @@ from .spaces import Box
 TASKS = {"walk": 0, "gallop": 1, "turn": 2, "standup": 3, "poses": 4}
 SIGNALS = {"ik": 0, "ol": 1}
 TERRAINS = {"plane": 0, "random": 1}
+MARKS = {"base": 12, "arm": 18}     # mark -> motors the robot carries (mark_constants.py:1; the arm adds six)
 DEFAULT_URDF_VERSION = "default"
 OBSERVATION_EPS = 0.01          # rex_gym/envs/rex_gym_env.py:19
 ACTION_BOUND = {("walk", "ik"): 0.4, ("walk", "ol"): 0.01, ("gallop", "ik"): 0.4, ("gallop", "ol"): 0.3,
@@ -316,27 +317,54 @@ def _name_entries(name, value, names, n):
     return entries
 
 
+def check_env_marks(num_envs, mark):
+    """The mark keyword, checked before any CUDA call: a scalar, or one entry per env (a list, tuple or ndarray), each 'base'
+    or 'arm'.  -> (scalar, None) for a scalar or an array whose entries are all equal (the scalar construction); (None,
+    int32 [num_envs] of each env's motor count, 12 or 18) for a batch of both marks."""
+    n = int(num_envs)
+    if is_per_env(mark):
+        if isinstance(mark, torch.Tensor):
+            raise ValueError("mark: per-env entries are the strings 'base' / 'arm', not a tensor")
+        a = np.asarray(list(mark) if isinstance(mark, (list, tuple)) else mark, dtype=object)
+        if a.shape != (n,):
+            raise ValueError("mark: expected one entry per env (%d), got shape %s" % (n, a.shape))
+        entries = [str(m) if isinstance(m, str) else m for m in a]
+    else:
+        entries = [mark]
+    if any(not isinstance(m, str) or m not in MARKS for m in entries):
+        raise ValueError("mark must be 'base' or 'arm'")          # mark_constants.py:1
+    if len(set(entries)) == 1:
+        return entries[0], None
+    return None, np.ascontiguousarray([MARKS[m] for m in entries], np.int32)
+
+
 def check_env_tasks(num_envs, task, signal_type, time_step=0.001, normalize=False, frames=None, frame_delta=False, mark="base"):
     """The task and signal_type keywords, checked before any CUDA call: each a scalar or one entry per env (a list, tuple or
-    ndarray).  Envs of several (task, signal_type) pairs are one batch only when their spaces (task_spaces) are the same, as
-    the reference's BatchEnv requires (batch_env.py:36-43): e.g. turn ik with turn ol, standup with poses, and under normalize
-    walk ik with turn.  -> (task, signal_type, None) for a scalar construction (all-equal pairs are one), else (tasks tuple,
-    signals tuple, (task ids, signal ids) int32 [num_envs] each)."""
+    ndarray).  Envs of several (task, signal_type) pairs, or of both marks (`mark`: a scalar or one entry per env), are one
+    batch only when their spaces (task_spaces, at each env's own motor count) are the same, as the reference's BatchEnv
+    requires (batch_env.py:36-43): e.g. turn ik with turn ol, standup with poses, under normalize walk ik with turn, and any
+    task but gallop with and without the arm.  A gallop env with the arm in a batch of both marks is refused with the
+    library's message.  -> (task, signal_type, None) for a scalar construction of the pair (all-equal pairs are one), else
+    (tasks tuple, signals tuple, (task ids, signal ids) int32 [num_envs] each)."""
     n = int(num_envs)
     tasks = _name_entries("task", task, TASKS, n)
     signals = _name_entries("signal_type", signal_type, SIGNALS, n)
+    marks = list(mark) if is_per_env(mark) else [mark] * n
     pairs = list(dict.fromkeys(zip(tasks, signals)))
-    if len(pairs) == 1:
-        return pairs[0][0], pairs[0][1], None
-    nm = 12 if mark == "base" else 18
-    spaces = {p: task_spaces(p[0], p[1], normalize, time_step, frames, frame_delta, nm) for p in pairs}
-    a0, o0 = spaces[pairs[0]]
-    for p in pairs[1:]:
+    envs = list(dict.fromkeys(zip(tasks, signals, marks)))         # the distinct (task, signal_type, mark) of the batch
+    if len(set(marks)) > 1 and any(t == "gallop" and m == "arm" for t, _, m in envs):
+        raise ValueError("mark='arm' is built for every task but gallop (its observation would carry the 18 motor angles)")
+    spaces = {p: task_spaces(p[0], p[1], normalize, time_step, frames, frame_delta, MARKS[p[2]]) for p in envs}
+    name = lambda p: "/".join(p if len(set(marks)) > 1 else p[:2])
+    a0, o0 = spaces[envs[0]]
+    for p in envs[1:]:
         a, o = spaces[p]
         if not (_same_box(o, o0) and _same_box(a, a0)):
-            raise ValueError("All environments must use the same observation space. (%s/%s: action %s, observation %s; %s/%s: "
-                             "action %s, observation %s%s)" % (pairs[0] + (a0, o0) + p + (a, o, "" if normalize else
-                                                               "; normalize=True gives every task the same bounds")))
+            raise ValueError("All environments must use the same observation space. (%s: action %s, observation %s; %s: "
+                             "action %s, observation %s%s)" % (name(envs[0]), a0, o0, name(p), a, o, "" if normalize else
+                                                              "; normalize=True gives every task the same bounds"))
+    if len(pairs) == 1:
+        return pairs[0][0], pairs[0][1], None
     ids = (np.ascontiguousarray([TASKS[t] for t in tasks], np.int32), np.ascontiguousarray([SIGNALS[g] for g in signals], np.int32))
     return tuple(tasks), tuple(signals), ids
 
@@ -368,7 +396,9 @@ class _Info(object):
         return self
 
     def __getitem__(self, i):
-        info = {"action": self.materialize()._cmd[i]}
+        cmd = self.materialize()._cmd[i]
+        motors = getattr(self._env, "_env_motors", None)       # [N] motors of each env, per-env marks only
+        info = {"action": cmd if motors is None else cmd[:motors[i]]}      # a base env of a batch of both marks: its 12
         if self._limit is not None and self._limit[i] & 1:
             info["TimeLimit.truncated"] = not bool(self._limit[i] & 2)
         return info
@@ -438,10 +468,19 @@ class BatchedRexEnv(object):
           otherwise).  The envs' spaces must be the same, as the reference's BatchEnv requires: turn ik with turn ol, standup
           with poses, and under normalize walk ik with turn.  Each (terrain, step-kernel unit, rate) group of envs is one
           slot range of the batch, launched with its own task; at most 16 groups.  All-equal entries build the scalar
-          construction."""
+          construction.
+
+        mark: 'base', 'arm', or one of them per env.  Env e of a batch of both runs exactly as env e of the batch built with
+          its entry as the scalar: its own robot, reset hold and sensor history.  The spaces agree for every task but gallop,
+          which the arm is not built for.  A batch of both is built on the arm's tables, which serve the base envs too; each
+          (terrain, mark, step-kernel unit, rate) group of envs is one slot range of the batch, launched with its mark's
+          build.  num_motors is 18 there, the width of last_command(); a base env's rows 12..17 are NaN, and its
+          info[i]['action'] has its own 12 entries.  All-equal entries build the scalar construction."""
         if urdf_version is not None and urdf_version != DEFAULT_URDF_VERSION:
             raise ValueError("%s is not a supported urdf_version." % urdf_version)     # rex_gym_env.py:317-318
         n_envs = int(num_envs)
+        # per-env marks: a batch of both is created with the arm, then told which envs are base
+        mark_scalar, env_marks = check_env_marks(num_envs, mark)
         task_list = _name_entries("task", task, TASKS, n_envs)
         _name_entries("signal_type", signal_type, SIGNALS, n_envs)
         # per-env terrains: a batch of both is created on the heightfield (its bank), then told which envs are on the plane
@@ -463,7 +502,8 @@ class BatchedRexEnv(object):
         # per-env latencies: the scalar gains of a motor_kp / motor_kd range hold the reset at each distinct pd_latency
         env_latency = check_env_latencies(num_envs, control_latency, pd_latency, motor_kp, motor_kd, env_gains)
         cts, rep, time_step, env_repeats = check_env_repeats(num_envs, task_list, control_time_step, action_repeat, solver_iterations)
-        task, signal_type, env_tasks = check_env_tasks(num_envs, task, signal_type, time_step, normalize, frames, frame_delta, mark)
+        marks = mark_scalar if env_marks is None else tuple(str(m) for m in mark)
+        task, signal_type, env_tasks = check_env_tasks(num_envs, task, signal_type, time_step, normalize, frames, frame_delta, marks)
         # env 0's task and signal in the config, as its rate; rexsim_set_env_tasks gives every env its own
         task0, signal0 = (task, signal_type) if env_tasks is None else (task[0], signal_type[0])
         if not torch.cuda.is_available():
@@ -471,18 +511,18 @@ class BatchedRexEnv(object):
         self._L = _capi.load()
         self._debug = bool(debug)
         # the scalars for a scalar construction (an array of equal pairs is one), else the N entries
-        self.task, self.signal_type, self.mark = task, signal_type, mark
+        self.task, self.signal_type, self.mark = task, signal_type, marks
         # the scalar for a scalar construction (an array of equal entries is one), else the N entries
         self.terrain_type = terrain_scalar if env_terrain is None else tuple(str(t) for t in terrain_type)
         self.device = torch.device(device)
         self.num_envs = int(num_envs)
-        self.num_motors = 12 if mark == "base" else 18
+        # the command block's width: the scalar mark's motors, 18 for a batch of both marks
+        self.num_motors = MARKS[mark_scalar or "arm"]
         # the scalars for a scalar construction, else the N entries; the simulation time step is the batch's
         self.control_time_step, self._action_repeat = cts, rep
         self._time_step = time_step
-        if mark not in ("base", "arm"):
-            raise ValueError("mark must be 'base' or 'arm'")          # mark_constants.py:1
-        tables, toe_npts = pack_model_tables(mark)
+        table_mark = mark_scalar or "arm"
+        tables, toe_npts = pack_model_tables(table_mark)
         c = _capi.RexSimConfig()
         c.num_envs, c.task, c.signal = self.num_envs, TASKS[task0], SIGNALS[signal0]
         c.terrain = TERRAINS[terrain_scalar or "random"]
@@ -526,7 +566,7 @@ class BatchedRexEnv(object):
                 c.friction = friction["plane"]
             c.residual_threshold, c.erp_contact, c.erp_joint = 1e-7, 0.08, 0.2
             c.toe_npts, c.toe_margin = toe_npts, TOE_MARGIN
-            c.contact_breaking = contact_breaking_distance(mark)
+            c.contact_breaking = contact_breaking_distance(table_mark)
             c.link_damping, c.max_coordinate_velocity = LINK_DAMPING, MAX_COORDINATE_VELOCITY
             c.env_offset = int(env_offset)
             self._cfg = c
@@ -537,7 +577,7 @@ class BatchedRexEnv(object):
         self._dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
         # every library call: on this env's device and torch's current stream there, a non-zero status raised (_capi.call)
         self._call = functools.partial(_capi.call, self._dev_index)
-        rt = np.ascontiguousarray(pack_render_tables(mark))
+        rt = np.ascontiguousarray(pack_render_tables(table_mark))
         self._call(self._L.rexsim_set_render_tables, self._h, rt.ctypes.data, rt.size, stream=False)
         env_obs_dim = self._L.rexsim_obs_dim(c.task, c.num_motors)
         if frames or frame_delta:
@@ -551,6 +591,9 @@ class BatchedRexEnv(object):
                        stream=False)
         if env_tasks is not None:
             self._call(self._L.rexsim_set_env_tasks, self._h, env_tasks[0].ctypes.data, env_tasks[1].ctypes.data, stream=False)
+        if env_marks is not None:
+            self._call(self._L.rexsim_set_env_marks, self._h, env_marks.ctypes.data, stream=False)
+        self._env_motors = env_marks         # [N] motors of each env on the host (per-env marks only): info[i]['action'] width
         self._values = None
         if env_values is not None:
             block = np.full((len(TASK_VALUE_KEYWORDS), self.num_envs), np.nan, np.float32)
@@ -613,6 +656,10 @@ class BatchedRexEnv(object):
         if env_tasks is not None:
             _capi.check(self._L.rexsim_env_task_buffers(self._h, C.byref(p)))
             self._tasks = view(p, (2, N), "|u1")
+        self._marks = None                   # [N] u8: 1 for each arm env, 0 for each base env (per-env marks only)
+        if env_marks is not None:
+            _capi.check(self._L.rexsim_env_mark_buffers(self._h, C.byref(p)))
+            self._marks = view(p, (N,), "|u1")
         self._latency = None                 # [2][N] f64: each env's control_latency, pd_latency (per-env latencies only)
         if env_latency is not None:
             depth = C.c_int32()
@@ -789,7 +836,8 @@ class BatchedRexEnv(object):
         return self.limit_bytes() == 1
 
     def last_command(self):
-        """[num_motors, N] motor commands of the last step (info['action'], rex_gym_env.py:414)."""
+        """[num_motors, N] motor commands of the last step (info['action'], rex_gym_env.py:414).  In a batch of both marks
+        num_motors is 18 and a base env's rows 12..17 are NaN."""
         return self._cmd
 
     def error_flags(self):
@@ -827,9 +875,16 @@ class BatchedRexEnv(object):
             sd["env_repeats"] = self._repeats.clone()
         if self._tasks is not None:
             sd["env_tasks"] = self._tasks.clone()
+        if self._marks is not None:
+            sd["env_marks"] = self._marks.clone()
         return sd
 
     def load_state_dict(self, sd):
+        if (self._marks is None) != ("env_marks" not in sd):
+            raise ValueError("per-env marks: the checkpoint %s them, this batch %s" %
+                             (("has", "does not") if self._marks is None else ("lacks", "has")))
+        if self._marks is not None and not torch.equal(self._marks, sd["env_marks"].to(self._marks.device)):
+            raise ValueError("per-env marks: the checkpoint's marks differ from this batch's")
         if (self._tasks is None) != ("env_tasks" not in sd):
             raise ValueError("per-env tasks: the checkpoint %s them, this batch %s" %
                              (("has", "does not") if self._tasks is None else ("lacks", "has")))

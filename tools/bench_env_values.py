@@ -27,7 +27,11 @@ Tasks (--workload tasks): normalized walk-ik and turn-ik at 16 384 and 65 536 en
 other env) stepped as two slot ranges of one batch, and the sum of an all-walk and an all-turn batch of N/2 each, alternately
 in one process.
 
-Usage: python tools/bench_env_values.py [--steps 200] [--rounds 3] [--workload all|values|latencies|terrains|repeats|tasks]"""
+Marks (--workload marks): normalized walk-ik at 16 384 and 65 536 envs, all base, all arm, a 50/50 mix (every other env)
+stepped as two slot ranges of one batch, and the sum of an all-base and an all-arm batch of N/2 each, alternately in one
+process.  Creation time of walk-ik at 4096 envs, all base, all arm and the 50/50 mix.
+
+Usage: python tools/bench_env_values.py [--steps 200] [--rounds 3] [--workload all|values|latencies|terrains|repeats|tasks|marks]"""
 import argparse
 import json
 import os
@@ -108,7 +112,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=3, help="step rounds; creation rows take the median of 2 x rounds + 1")
-    ap.add_argument("--workload", choices=("all", "values", "latencies", "terrains", "repeats", "tasks"), default="all")
+    ap.add_argument("--workload", choices=("all", "values", "latencies", "terrains", "repeats", "tasks", "marks"), default="all")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_env_values needs a CUDA device")
@@ -191,7 +195,33 @@ def main():
                                   **{"ms_" + k: [round(x, 4) for x in v] for k, v in rows.items()},
                                   ms_halves_sum=round(halves, 4),
                                   mixed_vs_halves_pct=round(100 * (median(rows["mixed"]) / halves - 1), 2))), flush=True)
-    if a.workload in ("latencies", "terrains", "repeats", "tasks"):
+    if a.workload in ("all", "marks"):
+        for n in (16384, 65536):
+            kw = dict(task="walk", signal_type="ik")
+            rows = {}
+            for _ in range(a.rounds):
+                for name, k in (("base", dict(kw, num_envs=n, mark="base")),
+                                ("arm", dict(kw, num_envs=n, mark="arm")),
+                                ("mixed", dict(kw, num_envs=n, mark=["base", "arm"] * (n // 2))),
+                                ("half_base", dict(kw, num_envs=n // 2, mark="base")),
+                                ("half_arm", dict(kw, num_envs=n // 2, mark="arm"))):
+                    rows.setdefault(name, []).append(ms_per_step(k, a.steps))
+            halves = median(rows["half_base"]) + median(rows["half_arm"])
+            print(json.dumps(dict(config="walk-ik marks, normalized", envs=n, steps=a.steps,
+                                  **{"ms_" + k: [round(x, 4) for x in v] for k, v in rows.items()},
+                                  ms_halves_sum=round(halves, 4),
+                                  mixed_vs_halves_pct=round(100 * (median(rows["mixed"]) / halves - 1), 2))), flush=True)
+        n = 4096
+        base = dict(task="walk", num_envs=n, signal_type="ik", target_position=2.0, backwards=False)
+        create_ms(base)                                      # module load and first-launch costs out of the timed rows
+        rows = {"base": [], "arm": [], "mixed": []}
+        for _ in range(2 * a.rounds + 1):
+            rows["base"].append(create_ms(dict(base, mark="base")))
+            rows["arm"].append(create_ms(dict(base, mark="arm")))
+            rows["mixed"].append(create_ms(dict(base, mark=["base", "arm"] * (n // 2))))
+        print(json.dumps(dict(config="create walk-ik %d envs, marks" % n, **{"ms_" + k: round(median(v), 1) for k, v in rows.items()})),
+              flush=True)
+    if a.workload in ("latencies", "terrains", "repeats", "tasks", "marks"):
         return
     for prefix in NAMES:
         name, kw = next(c for c in CONFIGS if c[0].startswith(prefix))
