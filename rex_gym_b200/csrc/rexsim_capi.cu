@@ -2,8 +2,10 @@
 #include "rexsim_kernel.cuh"
 #include "rexsim_host.h"
 #include <algorithm>
+#include <array>
 #include <cstring>
 #include <cmath>
+#include <tuple>
 #include <vector>
 
 namespace rexsim {
@@ -29,6 +31,23 @@ struct LaunchGroup {
     int32_t terrain, motors, task, signal, repeat, iters, first, count;
     int32_t launched[3];               // step_kernel instance of the group's last launch: BLOCK, OCC, SENSOR
 };
+// One env's construction values, as the per-env setters give them (the config's otherwise)
+struct EnvRecord {
+    uint8_t terrain, task, signal;
+    int32_t motors, repeat, iters;     // motor count (12 or 18), action_repeat, solver_iterations
+    float kp, kd;                      // motor_kp, motor_kd
+    double pd;                         // pd_latency
+};
+// One setting of the reset hold.  Rex.Reset clears the history and holds through ApplyAction (rex.py:303-323), so the settled
+// state depends on the solver's cap, the pose held (hold_start), the robot held, the gains and the PD observation's latency.
+struct HoldSetting {
+    int32_t iters, start, motors;
+    float kp, kd;
+    double pd;
+    bool operator==(const HoldSetting& o) const {
+        return iters == o.iters && start == o.start && motors == o.motors && kp == o.kp && kd == o.kd && pd == o.pd;
+    }
+};
 
 struct RexSim {
     Params P;                          // the handle's buffers are P's pointer fields, allocated from `mem`
@@ -46,24 +65,15 @@ struct RexSim {
     uint8_t* fin = nullptr;            // final obs | limit staging for rexsim_step_host_final (allocated on its first call)
     int A = 0;
     bool started = false;              // a reset or step has been enqueued: the frame wrappers can no longer be switched on
-    int nholds = 0;                    // hold settings (start, motor_kp, motor_kd, pd_latency, solver_iterations) of P.ev.gains /
-                                       // P.el.hold (0: no table)
-    std::vector<int32_t> hold_iters;   // [nholds] PGS cap of each hold setting, each cap's settings contiguous
-    std::vector<int32_t> hold_start;   // [nholds] start pose of each (hold_start), each (cap, start)'s settings contiguous
-    std::vector<int32_t> hold_motors;  // [nholds] motor count of each, each (cap, start, motors)'s settings contiguous
+    std::vector<EnvRecord> env;        // each env's construction values (empty before the first per-env setter: the config's)
+    std::vector<HoldSetting> holds;    // the hold settings of P.ev.gains / P.el.hold, in plan()'s order (empty: no table)
     bool values_on = false;            // rexsim_set_env_values was called
-    std::vector<float> kp, kd;         // per-env gains given to rexsim_set_env_values (empty: the config's)
-    std::vector<double> pd;            // per-env pd latencies given to rexsim_set_env_latencies (empty: the config's)
     double* latency = nullptr;         // [2][N] per-env control and pd latencies (rexsim_set_env_latencies; null: off)
     uint8_t* terrain = nullptr;        // [N] per-env terrains (rexsim_set_env_terrains; null: off); P.env_terrain points here
-    std::vector<uint8_t> terr;         // the same on the host (empty: the config's)
     float friction[2] = {0.f, 0.f};    // per-env terrains: friction of each terrain's envs, plane and heightfield
     int32_t* repeats = nullptr;        // [2][N] per-env action_repeat, solver_iterations (rexsim_set_env_repeats; null: off)
-    std::vector<int32_t> rep, iters;   // the same on the host (empty: the config's)
     uint8_t* tasks = nullptr;          // [2][N] per-env task, signal (rexsim_set_env_tasks; null: off); P.env_task points here
-    std::vector<uint8_t> task, signal; // the same on the host (empty: the config's)
     uint8_t* marks = nullptr;          // [N] per-env marks, 1 arm / 0 base (rexsim_set_env_marks; null: off); P.env_mark points here
-    std::vector<int32_t> motors;       // each env's motor count, 12 or 18, on the host (empty: the config's)
     float* snap_ring_base = nullptr;   // per-env marks with the sensor model: the base envs' snapshot ring, [settings * fields][D]
                                        // [HW_WORDS] (P.snap_ring is the arm's); the base launches read it as their P.snap_ring
     // The launch groups (empty: one launch over every slot with the config's values), terrain-major, plane first, then in
@@ -506,60 +516,77 @@ static int32_t hold_start(int task, int signal) {
     return task == REXSIM_TASK_STANDUP ? START_FOLD : task == REXSIM_TASK_POSES ? START_NONE
          : signal == REXSIM_SIGNAL_OL ? START_OL : START_IK;
 }
-// The reset hold's settings: each env's (mark, start, motor_kp, motor_kd, pd_latency, solver_iterations), distinct ones in
-// order of first appearance within each (PGS cap, start, mark), the marks in order of first appearance within each (cap,
-// start), the starts within each cap and the caps in order of first appearance (each cap's, (cap, start)'s and (cap, start,
-// mark)'s settings contiguous), and each env's index into them.  Rex.Reset clears the history and holds through ApplyAction
-// (rex.py:303-323), so the settled state depends on the robot held, the pose held, the gains, the PD observation's latency
-// and the solver's cap.  motors, start, kp, kd, pd, iters: per env, or empty for the config's scalar.
-struct HoldTable { std::vector<float> gains; std::vector<double> pd; std::vector<int32_t> iters, start, motors, index; };
-static int hold_table(const RexSimConfig& c, size_t N, const std::vector<int32_t>& motors, const std::vector<int32_t>& start,
-                      const std::vector<float>& kp, const std::vector<float>& kd, const std::vector<double>& pd,
-                      const std::vector<int32_t>& iters, HoldTable& t) {
-    t.index.assign(N, 0);
-    auto cap_of = [&](size_t e) { return iters.empty() ? c.solver_iterations : iters[e]; };
-    auto start_of = [&](size_t e) { return start.empty() ? hold_start(c.task, c.signal) : start[e]; };
-    auto motors_of = [&](size_t e) { return motors.empty() ? c.num_motors : motors[e]; };
-    std::vector<int32_t> caps;
-    for (size_t e = 0; e < N; e++)
-        if (std::find(caps.begin(), caps.end(), cap_of(e)) == caps.end()) caps.push_back(cap_of(e));
-    std::vector<std::pair<int32_t, int32_t>> starts;           // (cap, start): each cap's starts in order of first appearance
-    for (const int32_t cap : caps)
-        for (size_t e = 0; e < N; e++) {
-            const std::pair<int32_t, int32_t> k(cap, start_of(e));
-            if (cap_of(e) == cap && std::find(starts.begin(), starts.end(), k) == starts.end()) starts.push_back(k);
-        }
-    std::vector<std::pair<std::pair<int32_t, int32_t>, int32_t>> keys;   // ((cap, start), motors), marks by first appearance
-    for (const std::pair<int32_t, int32_t>& cs : starts)
-        for (size_t e = 0; e < N; e++) {
-            const std::pair<std::pair<int32_t, int32_t>, int32_t> k(cs, motors_of(e));
-            if (cap_of(e) == cs.first && start_of(e) == cs.second && std::find(keys.begin(), keys.end(), k) == keys.end())
-                keys.push_back(k);
-        }
-    for (const std::pair<std::pair<int32_t, int32_t>, int32_t>& key : keys)
-        for (size_t e = 0; e < N; e++) {
-            const int32_t it = cap_of(e), st = start_of(e), nm = motors_of(e);
-            if (it != key.first.first || st != key.first.second || nm != key.second) continue;
-            const float k = kp.empty() ? c.motor_kp : kp[e], d = kd.empty() ? c.motor_kd : kd[e];
-            const double l = pd.empty() ? c.pd_latency : pd[e];
-            size_t h = 0;
-            while (h < t.pd.size() && !(t.gains[2 * h] == k && t.gains[2 * h + 1] == d && t.pd[h] == l && t.iters[h] == it &&
-                                        t.start[h] == st && t.motors[h] == nm)) h++;
-            if (h == t.pd.size()) {
-                if ((int)h == REXSIM_MAX_GAIN_PAIRS)
-                    return fail(REXSIM_ERR_INVALID, "more than 64 distinct reset-hold settings (mark, start pose, motor_kp, motor_kd, pd_latency, solver_iterations)");
-                t.gains.push_back(k); t.gains.push_back(d); t.pd.push_back(l); t.iters.push_back(it); t.start.push_back(st);
-                t.motors.push_back(nm);
-            }
-            t.index[e] = (int32_t)h;
-        }
-    return REXSIM_OK;
+static EnvRecord config_record(const RexSimConfig& c) {
+    return EnvRecord{(uint8_t)c.terrain, (uint8_t)c.task, (uint8_t)c.signal, c.num_motors, c.action_repeat, c.solver_iterations,
+                     c.motor_kp, c.motor_kd, c.pd_latency};
 }
-// each env's hold start under per-env tasks (empty without them: the config's)
-static std::vector<int32_t> env_starts(const std::vector<uint8_t>& task, const std::vector<uint8_t>& signal) {
-    std::vector<int32_t> st(task.size());
-    for (size_t e = 0; e < task.size(); e++) st[e] = hold_start(task[e], signal[e]);
-    return st;
+// the handle's per-env records, or N copies of the config's values before the first per-env setter
+static std::vector<EnvRecord> records(const RexSim* s) {
+    return s->env.empty() ? std::vector<EnvRecord>(s->P.N, config_record(s->P.cfg)) : s->env;
+}
+static HoldSetting hold_of(const EnvRecord& r) { return HoldSetting{r.iters, hold_start(r.task, r.signal), r.motors, r.kp, r.kd, r.pd}; }
+
+// What a record vector asks the step and the reset hold for.  groups: the launch groups (terrain, mark, step unit,
+// action_repeat, solver_iterations), terrain-major, plane first, then in order of first appearance, with their slot ranges;
+// group: each env's.  holds: the distinct hold settings, ordered by the env at which each one's PGS cap first appears, then
+// its (cap, start), then its (cap, start, mark), then the setting itself, so that each cap's, (cap, start)'s and (cap, start,
+// mark)'s settings are contiguous (settle_snapshots settles each (cap, start, mark) in one launch); hold: each env's.
+struct Plan { std::vector<LaunchGroup> groups; std::vector<uint8_t> group; std::vector<HoldSetting> holds; std::vector<int32_t> hold; };
+static int plan(const std::vector<EnvRecord>& r, Plan& p) {
+    const size_t N = r.size();
+    p.group.assign(N, 0);
+    for (const int t : {REXSIM_TERRAIN_PLANE, REXSIM_TERRAIN_RANDOM})
+        for (size_t e = 0; e < N; e++) {
+            if (r[e].terrain != t) continue;
+            size_t g = 0;
+            while (g < p.groups.size() && !(p.groups[g].terrain == t && p.groups[g].motors == r[e].motors &&
+                                             unit_of(p.groups[g].task, p.groups[g].signal) == unit_of(r[e].task, r[e].signal) &&
+                                             p.groups[g].repeat == r[e].repeat && p.groups[g].iters == r[e].iters)) g++;
+            if (g == p.groups.size()) {
+                if ((int)g == REXSIM_MAX_LAUNCH_GROUPS)
+                    return fail(REXSIM_ERR_INVALID, "more than 16 launch groups (terrain, mark, task unit, action_repeat, solver_iterations)");
+                p.groups.push_back(LaunchGroup{t, r[e].motors, r[e].task, r[e].signal, r[e].repeat, r[e].iters, 0, 0, {0, 0, 0}});
+            }
+            p.groups[g].count++;
+            p.group[e] = (uint8_t)g;
+        }
+    for (size_t g = 1; g < p.groups.size(); g++) p.groups[g].first = p.groups[g - 1].first + p.groups[g - 1].count;
+    std::vector<HoldSetting> seen;                 // the distinct settings in order of first appearance
+    std::vector<size_t> at;                        // the env each first appears at
+    std::vector<int32_t> idx(N);
+    for (size_t e = 0; e < N; e++) {
+        const HoldSetting h = hold_of(r[e]);
+        const size_t k = std::find(seen.begin(), seen.end(), h) - seen.begin();
+        if (k == seen.size()) {
+            if ((int)k == REXSIM_MAX_GAIN_PAIRS)
+                return fail(REXSIM_ERR_INVALID, "more than 64 distinct reset-hold settings (mark, start pose, motor_kp, motor_kd, pd_latency, solver_iterations)");
+            seen.push_back(h);
+            at.push_back(e);
+        }
+        idx[e] = (int32_t)k;
+    }
+    // the sort key of setting k: the first appearance of its cap, (cap, start), (cap, start, mark) and of itself -- the first
+    // setting sharing a prefix is the one that appears first
+    auto prefix = [](const HoldSetting& h, int level) {
+        return std::make_tuple(h.iters, level > 0 ? h.start : 0, level > 1 ? h.motors : 0);
+    };
+    std::vector<std::array<size_t, 4>> key(seen.size());
+    for (size_t k = 0; k < seen.size(); k++) {
+        for (int level = 0; level < 3; level++) {
+            size_t j = 0;
+            while (prefix(seen[j], level) != prefix(seen[k], level)) j++;
+            key[k][level] = at[j];
+        }
+        key[k][3] = at[k];
+    }
+    std::vector<int32_t> order(seen.size()), rank(seen.size());
+    for (size_t k = 0; k < seen.size(); k++) order[k] = (int32_t)k;
+    std::sort(order.begin(), order.end(), [&](int32_t a, int32_t b) { return key[a] < key[b]; });
+    p.holds.resize(seen.size());
+    for (size_t i = 0; i < order.size(); i++) { p.holds[i] = seen[order[i]]; rank[order[i]] = (int32_t)i; }
+    p.hold.resize(N);
+    for (size_t e = 0; e < N; e++) p.hold[e] = rank[idx[e]];
+    return REXSIM_OK;
 }
 // the launch groups a step launches: the table, or for a batch without one its single group over every slot
 static std::vector<LaunchGroup> launch_groups(const RexSim* s) {
@@ -568,51 +595,15 @@ static std::vector<LaunchGroup> launch_groups(const RexSim* s) {
     return {LaunchGroup{c.terrain, c.num_motors, c.task, c.signal, c.action_repeat, c.solver_iterations, 0, s->P.N,
                         {s->launched[0], s->launched[1], s->launched[2]}}};
 }
-// Each env's launch group: the groups (terrain, mark, step unit, action_repeat, solver_iterations), terrain-major, plane first,
-// then in order of first appearance, from the per-env terrains, repeats, iteration counts, tasks, signals and motor counts
-// given (each empty for the config's).  Refused past REXSIM_MAX_LAUNCH_GROUPS groups.
-struct GroupPlan { std::vector<LaunchGroup> gs; std::vector<uint8_t> key; };
-static int plan_groups(const RexSim* s, const std::vector<uint8_t>& terr, const std::vector<int32_t>& rep,
-                       const std::vector<int32_t>& iters, const std::vector<uint8_t>& task, const std::vector<uint8_t>& signal,
-                       const std::vector<int32_t>& motors, GroupPlan& p) {
-    const RexSimConfig& c = s->P.cfg;
-    const size_t N = s->P.N;
-    p.gs.clear();
-    p.key.assign(N, 0);
-    for (const int t : {REXSIM_TERRAIN_PLANE, REXSIM_TERRAIN_RANDOM})
-        for (size_t e = 0; e < N; e++) {
-            if ((terr.empty() ? c.terrain : terr[e]) != t) continue;
-            const int32_t r = rep.empty() ? c.action_repeat : rep[e];
-            const int32_t it = iters.empty() ? c.solver_iterations : iters[e];
-            const int32_t k = task.empty() ? c.task : task[e], sg = signal.empty() ? c.signal : signal[e];
-            const int32_t nm = motors.empty() ? c.num_motors : motors[e];
-            size_t g = 0;
-            while (g < p.gs.size() && !(p.gs[g].terrain == t && p.gs[g].motors == nm &&
-                                        unit_of(p.gs[g].task, p.gs[g].signal) == unit_of(k, sg) &&
-                                        p.gs[g].repeat == r && p.gs[g].iters == it)) g++;
-            if (g == p.gs.size()) {
-                if ((int)g == REXSIM_MAX_LAUNCH_GROUPS)
-                    return fail(REXSIM_ERR_INVALID, "more than 16 launch groups (terrain, mark, task unit, action_repeat, solver_iterations)");
-                p.gs.push_back(LaunchGroup{t, nm, k, sg, r, it, 0, 0, {0, 0, 0}});
-            }
-            p.gs[g].count++;
-            p.key[e] = (uint8_t)g;
-        }
-    return REXSIM_OK;
-}
-// Install the launch groups of the handle's per-env values (plan_groups): put each group's envs in its slot range, in env
-// order, and give rexsim_rebalance the group key.  Synchronous.
-static int build_groups(RexSim* s) {
+// Install a plan's launch groups: put each group's envs in its slot range, in env order, and give rexsim_rebalance the group
+// key.  Synchronous.
+static int build_groups(RexSim* s, const Plan& p) {
     Params& P = s->P;
     const size_t N = P.N;
-    GroupPlan plan;
-    if (int rc = plan_groups(s, s->terr, s->rep, s->iters, s->task, s->signal, s->motors, plan)) return rc;
-    std::vector<LaunchGroup>& gs = plan.gs;
-    const std::vector<uint8_t>& key = plan.key;
+    const std::vector<LaunchGroup>& gs = p.groups;
     std::vector<int32_t> at(gs.size()), perm(N);
-    for (size_t g = 1; g < gs.size(); g++) gs[g].first = gs[g - 1].first + gs[g - 1].count;
     for (size_t g = 0; g < gs.size(); g++) at[g] = gs[g].first;
-    for (size_t e = 0; e < N; e++) perm[at[key[e]]++] = (int32_t)e;
+    for (size_t e = 0; e < N; e++) perm[at[p.group[e]]++] = (int32_t)e;
     CK(cudaMemcpy(s->perm, perm.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
     P.perm = s->perm;                          // the partition holds from the first step on
     s->mem.drop(s->group_bytes);
@@ -627,11 +618,36 @@ static int build_groups(RexSim* s) {
             s->group = s->terrain;             // the groups are exactly the two terrains: group g is terrain g
         } else {
             if (s->mem.zeroed(&s->group_bytes, N)) return REXSIM_ERR_CUDA;
-            CK(cudaMemcpy(s->group_bytes, key.data(), N, cudaMemcpyHostToDevice));
+            CK(cudaMemcpy(s->group_bytes, p.group.data(), N, cudaMemcpyHostToDevice));
             s->group = s->group_bytes;
         }
     }
     s->groups = gs;
+    return REXSIM_OK;
+}
+// Install a plan's hold table: P.ev.pair, P.ev.gains and, with per-env latencies, P.el.hold.  Synchronous.
+static int apply_holds(RexSim* s, const Plan& p) {
+    Params& P = s->P;
+    const size_t N = P.N, nh = p.holds.size();
+    std::vector<float> gains(2 * nh);
+    for (size_t h = 0; h < nh; h++) { gains[2 * h] = p.holds[h].kp; gains[2 * h + 1] = p.holds[h].kd; }
+    int32_t* dpair = nullptr;
+    float* dgains = nullptr;
+    if (s->mem.zeroed(&dpair, N) || s->mem.zeroed(&dgains, gains.size())) return REXSIM_ERR_CUDA;
+    CK(cudaMemcpy(dpair, p.hold.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(dgains, gains.data(), gains.size() * sizeof(float), cudaMemcpyHostToDevice));
+    s->mem.drop((void*)P.ev.pair); s->mem.drop((void*)P.ev.gains);
+    P.ev.pair = dpair; P.ev.gains = dgains;
+    if (s->latency) {
+        std::vector<Delay> hold(nh);
+        for (size_t h = 0; h < nh; h++) hold[h] = delay_terms(p.holds[h].pd, P.cfg.sim_dt_d);
+        Delay* dhold = nullptr;
+        if (s->mem.zeroed(&dhold, nh)) return REXSIM_ERR_CUDA;
+        CK(cudaMemcpy(dhold, hold.data(), nh * sizeof(Delay), cudaMemcpyHostToDevice));
+        s->mem.drop((void*)P.el.hold);
+        P.el.hold = dhold;
+    }
+    s->holds = p.holds;
     return REXSIM_OK;
 }
 // Run the reset hold again for every snapshot of the layout P.snaps, at the handle's hold settings (the config's one without a
@@ -640,8 +656,8 @@ static int build_groups(RexSim* s) {
 // mark's build, over all the (cap, start, mark)'s (setting, field) snapshots.  Synchronous.
 static int settle_snapshots(RexSim* s) {
     Params& P = s->P;
-    const int nh = s->nholds > 0 ? s->nholds : 1;
-    const size_t nsettle = (size_t)nh * P.snaps.per_setting;
+    const std::vector<HoldSetting> holds = s->holds.empty() ? std::vector<HoldSetting>{hold_of(config_record(P.cfg))} : s->holds;
+    const size_t nsettle = holds.size() * P.snaps.per_setting;
     float* snap_f = nullptr;
     int32_t* snap_i = nullptr;
     if (s->mem.zeroed(&snap_f, (size_t)NF * nsettle) || s->mem.zeroed(&snap_i, (size_t)NI * nsettle)) return REXSIM_ERR_CUDA;
@@ -657,9 +673,6 @@ static int settle_snapshots(RexSim* s) {
             if (s->mem.zeroed(&s->snap_ring_base, nsettle * P.ring_depth * HW_WORDS)) return REXSIM_ERR_CUDA;
         }
     }
-    const std::vector<int32_t> caps = s->nholds > 0 ? s->hold_iters : std::vector<int32_t>{P.cfg.solver_iterations};
-    const std::vector<int32_t> starts = s->nholds > 0 ? s->hold_start : std::vector<int32_t>{hold_start(P.cfg.task, P.cfg.signal)};
-    const std::vector<int32_t> motors = s->nholds > 0 ? s->hold_motors : std::vector<int32_t>{P.cfg.num_motors};
     const std::vector<LaunchGroup> gs = launch_groups(s);
     auto same_hold = [](const LaunchGroup& a, const LaunchGroup& b) {
         return a.terrain == b.terrain && a.iters == b.iters && hold_start(a.task, a.signal) == hold_start(b.task, b.signal) &&
@@ -671,45 +684,45 @@ static int settle_snapshots(RexSim* s) {
         if (settled) continue;
         const int32_t st = hold_start(gs[g].task, gs[g].signal);
         int first = -1, count = 0;             // the (cap, start, mark)'s settings are contiguous
-        for (size_t h = 0; h < caps.size(); h++)
-            if (caps[h] == gs[g].iters && starts[h] == st && motors[h] == gs[g].motors) { first = first < 0 ? (int)h : first; count++; }
+        for (size_t h = 0; h < holds.size(); h++)
+            if (holds[h].iters == gs[g].iters && holds[h].start == st && holds[h].motors == gs[g].motors) {
+                first = first < 0 ? (int)h : first;
+                count++;
+            }
         const Params G = group_params(s, P, gs[g]);
         if (int rc = enqueue(s, launch_settle(G, snap_f, snap_i, first, count, 0), "settle launch")) return rc;
     }
     CK(cudaDeviceSynchronize());
     return REXSIM_OK;
 }
-// Install a hold table (P.ev.pair, P.ev.gains and, with per-env latencies, P.el.hold), and with `settle` run the reset hold
-// again (settle_snapshots).  Synchronous.
-static int apply_holds(RexSim* s, const HoldTable& t, bool settle) {
-    Params& P = s->P;
-    const size_t N = P.N, nh = t.pd.size();
-    int32_t* dpair = nullptr;
-    float* dgains = nullptr;
-    if (s->mem.zeroed(&dpair, N) || s->mem.zeroed(&dgains, t.gains.size())) return REXSIM_ERR_CUDA;
-    CK(cudaMemcpy(dpair, t.index.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(dgains, t.gains.data(), t.gains.size() * sizeof(float), cudaMemcpyHostToDevice));
-    s->mem.drop((void*)P.ev.pair); s->mem.drop((void*)P.ev.gains);
-    P.ev.pair = dpair; P.ev.gains = dgains;
-    if (s->latency) {
-        std::vector<Delay> hold(nh);
-        for (size_t h = 0; h < nh; h++) hold[h] = delay_terms(t.pd[h], P.cfg.sim_dt_d);
-        Delay* dhold = nullptr;
-        if (s->mem.zeroed(&dhold, nh)) return REXSIM_ERR_CUDA;
-        CK(cudaMemcpy(dhold, hold.data(), nh * sizeof(Delay), cudaMemcpyHostToDevice));
-        s->mem.drop((void*)P.el.hold);
-        P.el.hold = dhold;
+// What a per-env setter installs of its plan, after its own device bytes (install)
+enum { GROUPS = 1, HOLDS = 2, SETTLE = 4 };
+// Take a setter's records, and install the parts `what` of their plan: the launch groups (build_groups), the hold table
+// (apply_holds), and the reset hold run again (settle_snapshots).  Synchronous.
+static int install(RexSim* s, std::vector<EnvRecord>&& rec, const Plan& p, int what) {
+    s->env = std::move(rec);
+    if (what & GROUPS) if (int rc = build_groups(s, p)) return rc;
+    if (what & HOLDS) if (int rc = apply_holds(s, p)) return rc;
+    return what & SETTLE ? settle_snapshots(s) : REXSIM_OK;
+}
+// The per-env setters' common refusals, each before anything changes: a null argument (null_msg), a handle already reset or
+// stepped, and the setter's block already set (`set`)
+static int setter_prelude(const RexSim* s, bool null_args, const char* null_msg, const char* what, bool set) {
+    if (!s || null_args) return fail(REXSIM_ERR_INVALID, null_msg);
+    char msg[96];
+    if (s->started) {
+        snprintf(msg, sizeof(msg), "per-env %s must be set before the first reset or step", what);
+        return fail(REXSIM_ERR_INVALID, msg);
     }
-    s->nholds = (int)nh;
-    s->hold_iters = t.iters;
-    s->hold_start = t.start;
-    s->hold_motors = t.motors;
-    return settle ? settle_snapshots(s) : REXSIM_OK;
+    if (set) {
+        snprintf(msg, sizeof(msg), "per-env %s are already set", what);
+        return fail(REXSIM_ERR_INVALID, msg);
+    }
+    return REXSIM_OK;
 }
 int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const float* kd) {
-    if (!s || !values || !kp != !kd) return fail(REXSIM_ERR_INVALID, "null argument (kp and kd are given together or not at all)");
-    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env values must be set before the first reset or step");
-    if (s->values_on) return fail(REXSIM_ERR_INVALID, "per-env values are already set");
+    if (int rc = setter_prelude(s, !values || !kp != !kd, "null argument (kp and kd are given together or not at all)", "values",
+                                s && s->values_on)) return rc;
     Params& P = s->P;
     const RexSimConfig& c = P.cfg;
     const size_t N = P.N;
@@ -717,17 +730,18 @@ int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const
         const float b = values[REXSIM_VALUE_BACKWARDS * N + e];
         if (b != -1.f && b != 0.f && b != 1.f) return fail(REXSIM_ERR_INVALID, "backwards values must be -1, 0 or 1");
     }
-    HoldTable t;
+    std::vector<EnvRecord> rec = records(s);
     if (kp) {
         if (c.kp_lo != c.kp_hi || c.kd_lo != c.kd_hi)
             return fail(REXSIM_ERR_INVALID, "per-env gains cannot be combined with a motor_kp / motor_kd range");
-        for (size_t e = 0; e < N; e++)
+        for (size_t e = 0; e < N; e++) {
             if (!(kp[e] >= 0.f) || !(kd[e] >= 0.f) || std::isinf(kp[e]) || std::isinf(kd[e]))
                 return fail(REXSIM_ERR_INVALID, "gains must be finite and non-negative");
-        if (int rc = hold_table(c, N, s->motors, env_starts(s->task, s->signal), std::vector<float>(kp, kp + N), std::vector<float>(kd, kd + N), s->pd, s->iters, t)) return rc;
-    } else if (!P.ev.pair) {
-        if (int rc = hold_table(c, N, s->motors, env_starts(s->task, s->signal), s->kp, s->kd, s->pd, s->iters, t)) return rc;          // the config's one setting
+            rec[e].kp = kp[e]; rec[e].kd = kd[e];
+        }
     }
+    Plan p;
+    if (int rc = plan(rec, p)) return rc;
     float* block = nullptr;
     if (s->mem.zeroed(&block, (size_t)REXSIM_VALUE_BLOCK_ROWS * N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(block, values, (size_t)REXSIM_VALUE_ROWS * N * sizeof(float), cudaMemcpyHostToDevice));
@@ -736,24 +750,23 @@ int rexsim_set_env_values(RexSim* s, const float* values, const float* kp, const
                   cudaMemcpyHostToDevice));
     P.ev.values = block;
     s->values_on = true;
-    if (kp) { s->kp.assign(kp, kp + N); s->kd.assign(kd, kd + N); }
-    // per-env gains: the reset hold again, once per (setting, field); without them the table (if new) is the config's one
-    // setting, whose snapshot rexsim_create settled
-    return t.index.empty() ? REXSIM_OK : apply_holds(s, t, kp != nullptr);
+    // per-env gains: the reset hold again, once per (setting, field); without them a new table is the config's one setting,
+    // whose snapshot rexsim_create settled
+    return install(s, std::move(rec), p, kp ? HOLDS | SETTLE : P.ev.pair ? 0 : HOLDS);
 }
 int rexsim_set_env_latencies(RexSim* s, const double* control_latency, const double* pd_latency) {
-    if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
-    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env latencies must be set before the first reset or step");
-    if (s->latency) return fail(REXSIM_ERR_INVALID, "per-env latencies are already set");
+    if (int rc = setter_prelude(s, false, "null handle", "latencies", s && s->latency)) return rc;
     Params& P = s->P;
     const RexSimConfig& c = P.cfg;
     const size_t N = P.N;
     std::vector<double> lat(2 * N);
+    std::vector<EnvRecord> rec = records(s);
     for (size_t e = 0; e < N; e++) {
         lat[e] = control_latency ? control_latency[e] : c.control_latency;
         lat[N + e] = pd_latency ? pd_latency[e] : c.pd_latency;
         if (!(lat[e] >= 0) || !(lat[N + e] >= 0) || std::isinf(lat[e]) || std::isinf(lat[N + e]))
             return fail(REXSIM_ERR_INVALID, "latencies must be finite and non-negative");
+        rec[e].pd = lat[N + e];
     }
     // each env's terms as a batch built with its latencies as scalars would have them; the ring keeps the deepest history
     std::vector<EnvDelay> env(N);
@@ -766,15 +779,14 @@ int rexsim_set_env_latencies(RexSim* s, const double* control_latency, const dou
         depth = sc.depth > depth ? sc.depth : depth;
         on = on || sc.on;
     }
-    HoldTable t;
-    const std::vector<double> pd(lat.begin() + N, lat.end());
-    if (int rc = hold_table(c, N, s->motors, env_starts(s->task, s->signal), s->kp, s->kd, pd, s->iters, t)) return rc;
+    Plan p;
+    if (int rc = plan(rec, p)) return rc;
     double* dlat = nullptr;
     EnvDelay* denv = nullptr;
     if (s->mem.zeroed(&dlat, 2 * N) || s->mem.zeroed(&denv, N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(dlat, lat.data(), 2 * N * sizeof(double), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(denv, env.data(), N * sizeof(EnvDelay), cudaMemcpyHostToDevice));
-    s->latency = dlat; s->pd = pd;
+    s->latency = dlat;
     P.el.env = denv;
     if (on && depth != P.ring_depth) {          // a latency switches the sensor model on, exactly as a scalar one does
         s->mem.drop(P.ring);
@@ -784,7 +796,7 @@ int rexsim_set_env_latencies(RexSim* s, const double* control_latency, const dou
         P.ring_depth = depth;
         for (int k = 0; k < 5; k++) P.noise_sd[k] = (float)c.noise_stdev[k];
     }
-    return apply_holds(s, t, true);
+    return install(s, std::move(rec), p, HOLDS | SETTLE);
 }
 int rexsim_env_latency_buffers(RexSim* s, double** latency, int32_t* depth) {
     if (!s || !latency || !depth) return fail(REXSIM_ERR_INVALID, "null argument");
@@ -793,33 +805,31 @@ int rexsim_env_latency_buffers(RexSim* s, double** latency, int32_t* depth) {
     return REXSIM_OK;
 }
 int rexsim_set_env_terrains(RexSim* s, const int32_t* terrain, float plane_friction) {
-    if (!s || !terrain) return fail(REXSIM_ERR_INVALID, "null argument");
-    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env terrains must be set before the first reset or step");
-    if (s->terrain) return fail(REXSIM_ERR_INVALID, "per-env terrains are already set");
+    if (int rc = setter_prelude(s, !terrain, "null argument", "terrains", s && s->terrain)) return rc;
     Params& P = s->P;
     if (P.cfg.terrain != REXSIM_TERRAIN_RANDOM)
         return fail(REXSIM_ERR_INVALID, "per-env terrains need a handle created on the random terrain (its heightfield bank)");
     if (!(plane_friction >= 0.f) || std::isinf(plane_friction)) return fail(REXSIM_ERR_INVALID, "plane friction must be finite and non-negative");
     const size_t N = P.N;
+    std::vector<EnvRecord> rec = records(s);
     std::vector<uint8_t> bytes(N);
     size_t nplane = 0;
     for (size_t e = 0; e < N; e++) {
         if (terrain[e] != REXSIM_TERRAIN_PLANE && terrain[e] != REXSIM_TERRAIN_RANDOM)
             return fail(REXSIM_ERR_INVALID, "terrain entries must be REXSIM_TERRAIN_PLANE or REXSIM_TERRAIN_RANDOM");
-        bytes[e] = (uint8_t)terrain[e];
+        bytes[e] = rec[e].terrain = (uint8_t)terrain[e];
         nplane += terrain[e] == REXSIM_TERRAIN_PLANE;
     }
-    GroupPlan plan;
-    if (int rc = plan_groups(s, bytes, s->rep, s->iters, s->task, s->signal, s->motors, plan)) return rc;
+    Plan p;
+    if (int rc = plan(rec, p)) return rc;
     uint8_t* dterrain = nullptr;
     if (s->mem.zeroed(&dterrain, N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(dterrain, bytes.data(), N, cudaMemcpyHostToDevice));
-    s->terrain = dterrain; s->terr = bytes;
+    s->terrain = dterrain;
     s->friction[REXSIM_TERRAIN_PLANE] = plane_friction; s->friction[REXSIM_TERRAIN_RANDOM] = P.cfg.friction;
     P.env_terrain = dterrain;
     P.snaps = snap_layout(nplane > 0, nplane < N, P.cfg.nfields);
-    if (int rc = build_groups(s)) return rc;
-    return settle_snapshots(s);
+    return install(s, std::move(rec), p, GROUPS | SETTLE);     // the terrain is no part of a hold setting
 }
 int rexsim_env_terrain_buffers(RexSim* s, uint8_t** terrain, int32_t* nplane) {
     if (!s || !terrain || !nplane) return fail(REXSIM_ERR_INVALID, "null argument");
@@ -830,12 +840,11 @@ int rexsim_env_terrain_buffers(RexSim* s, uint8_t** terrain, int32_t* nplane) {
     return REXSIM_OK;
 }
 int rexsim_set_env_repeats(RexSim* s, const int32_t* action_repeat, const int32_t* solver_iterations) {
-    if (!s) return fail(REXSIM_ERR_INVALID, "null handle");
-    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env repeats must be set before the first reset or step");
-    if (s->repeats) return fail(REXSIM_ERR_INVALID, "per-env repeats are already set");
+    if (int rc = setter_prelude(s, false, "null handle", "repeats", s && s->repeats)) return rc;
     Params& P = s->P;
     const RexSimConfig& c = P.cfg;
     const size_t N = P.N;
+    std::vector<EnvRecord> rec = records(s);
     std::vector<int32_t> rep(N), iters(N);
     std::vector<std::pair<int32_t, int32_t>> pairs;
     for (size_t e = 0; e < N; e++) {
@@ -847,18 +856,16 @@ int rexsim_set_env_repeats(RexSim* s, const int32_t* action_repeat, const int32_
                 return fail(REXSIM_ERR_INVALID, "more than 8 distinct (action_repeat, solver_iterations) pairs");
             pairs.push_back(std::make_pair(rep[e], iters[e]));
         }
+        rec[e].repeat = rep[e]; rec[e].iters = iters[e];
     }
-    GroupPlan plan;
-    if (int rc = plan_groups(s, s->terr, rep, iters, s->task, s->signal, s->motors, plan)) return rc;
-    HoldTable t;
-    if (int rc = hold_table(c, N, s->motors, env_starts(s->task, s->signal), s->kp, s->kd, s->pd, iters, t)) return rc;
+    Plan p;
+    if (int rc = plan(rec, p)) return rc;
     int32_t* d = nullptr;
     if (s->mem.zeroed(&d, 2 * N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(d, rep.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(d + N, iters.data(), N * sizeof(int32_t), cudaMemcpyHostToDevice));
-    s->repeats = d; s->rep = rep; s->iters = iters;
-    if (int rc = build_groups(s)) return rc;
-    return apply_holds(s, t, true);
+    s->repeats = d;
+    return install(s, std::move(rec), p, GROUPS | HOLDS | SETTLE);
 }
 int rexsim_env_repeat_buffers(RexSim* s, int32_t** repeats) {
     if (!s || !repeats) return fail(REXSIM_ERR_INVALID, "null argument");
@@ -867,15 +874,14 @@ int rexsim_env_repeat_buffers(RexSim* s, int32_t** repeats) {
     return REXSIM_OK;
 }
 int rexsim_set_env_tasks(RexSim* s, const int32_t* task, const int32_t* signal) {
-    if (!s || !task || !signal) return fail(REXSIM_ERR_INVALID, "null argument");
-    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env tasks must be set before the first reset or step");
-    if (s->tasks) return fail(REXSIM_ERR_INVALID, "per-env tasks are already set");
+    if (int rc = setter_prelude(s, !task || !signal, "null argument", "tasks", s && s->tasks)) return rc;
     Params& P = s->P;
     const RexSimConfig& c = P.cfg;
     const size_t N = P.N;
     // the reference's BatchEnv refuses envs whose spaces differ (batch_env.py:36-43): the widths always, the raw action bound
     // unless ClipAction and RangeNormalize replace both boxes (the observation bounds depend on the time step alone)
     const TaskShape own = task_shape(c.task);
+    std::vector<EnvRecord> rec = records(s);
     std::vector<uint8_t> tk(N), sg(N);
     bool objectives = false;
     for (size_t e = 0; e < N; e++) {
@@ -888,18 +894,16 @@ int rexsim_set_env_tasks(RexSim* s, const int32_t* task, const int32_t* signal) 
             return fail(REXSIM_ERR_INVALID, "All environments must use the same observation space (action or observation width differs)");
         if (!c.normalize && task_shape(k).bound[g] != own.bound[c.signal])
             return fail(REXSIM_ERR_INVALID, "All environments must use the same observation space (raw action bound differs)");
-        tk[e] = (uint8_t)k; sg[e] = (uint8_t)g;
+        tk[e] = rec[e].task = (uint8_t)k; sg[e] = rec[e].signal = (uint8_t)g;
         objectives = objectives || k == REXSIM_TASK_WALK || k == REXSIM_TASK_GALLOP;
     }
-    GroupPlan plan;
-    if (int rc = plan_groups(s, s->terr, s->rep, s->iters, tk, sg, s->motors, plan)) return rc;
-    HoldTable t;
-    if (int rc = hold_table(c, N, s->motors, env_starts(tk, sg), s->kp, s->kd, s->pd, s->iters, t)) return rc;
+    Plan p;
+    if (int rc = plan(rec, p)) return rc;
     uint8_t* d = nullptr;
     if (s->mem.zeroed(&d, 2 * N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(d, tk.data(), N, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(d + N, sg.data(), N, cudaMemcpyHostToDevice));
-    s->tasks = d; s->task = tk; s->signal = sg;
+    s->tasks = d;
     P.env_task = d;
     if (s->ep_block && objectives) {
         // walk and gallop record the objectives of every step; the other envs' columns are NaN and stay NaN
@@ -910,8 +914,7 @@ int rexsim_set_env_tasks(RexSim* s, const int32_t* task, const int32_t* signal) 
         if (!P.ep.objectives && s->mem.zeroed(&P.ep.objectives, 4 * N)) return REXSIM_ERR_CUDA;
         CK(cudaMemcpy(P.ep.objectives, o.data(), 4 * N * sizeof(float), cudaMemcpyHostToDevice));
     }
-    if (int rc = build_groups(s)) return rc;
-    return apply_holds(s, t, true);
+    return install(s, std::move(rec), p, GROUPS | HOLDS | SETTLE);
 }
 int rexsim_env_task_buffers(RexSim* s, uint8_t** task) {
     if (!s || !task) return fail(REXSIM_ERR_INVALID, "null argument");
@@ -927,29 +930,23 @@ int rexsim_launch_group_task(const RexSim* s, int32_t g, int32_t* task, int32_t*
     return REXSIM_OK;
 }
 int rexsim_set_env_marks(RexSim* s, const int32_t* num_motors) {
-    if (!s || !num_motors) return fail(REXSIM_ERR_INVALID, "null argument");
-    if (s->started) return fail(REXSIM_ERR_INVALID, "per-env marks must be set before the first reset or step");
-    if (s->marks) return fail(REXSIM_ERR_INVALID, "per-env marks are already set");
+    if (int rc = setter_prelude(s, !num_motors, "null argument", "marks", s && s->marks)) return rc;
     Params& P = s->P;
-    const RexSimConfig& c = P.cfg;
     const size_t N = P.N;
     // the arm's model table starts with the base's (REXSIM_MT_FLOATS), its render table draws the base's shapes, its ring rows
     // hold the base's words first: a handle built for the arm serves base envs, not the other way round
-    if (c.num_motors != 18) return fail(REXSIM_ERR_INVALID, "per-env marks need a handle created with the arm (num_motors 18)");
-    std::vector<int32_t> nm(N);
+    if (P.cfg.num_motors != 18) return fail(REXSIM_ERR_INVALID, "per-env marks need a handle created with the arm (num_motors 18)");
+    std::vector<EnvRecord> rec = records(s);
     std::vector<uint8_t> bytes(N);
     for (size_t e = 0; e < N; e++) {
         if (num_motors[e] != 12 && num_motors[e] != 18) return fail(REXSIM_ERR_INVALID, "mark entries must be 12 (base) or 18 (arm)");
-        const int32_t task = s->task.empty() ? c.task : s->task[e];
-        if (num_motors[e] == 18 && task == REXSIM_TASK_GALLOP)
+        if (num_motors[e] == 18 && rec[e].task == REXSIM_TASK_GALLOP)
             return fail(REXSIM_ERR_INVALID, "mark='arm' is built for every task but gallop");
-        nm[e] = num_motors[e];
+        rec[e].motors = num_motors[e];
         bytes[e] = (uint8_t)(num_motors[e] == 18);
     }
-    GroupPlan plan;
-    if (int rc = plan_groups(s, s->terr, s->rep, s->iters, s->task, s->signal, nm, plan)) return rc;
-    HoldTable t;
-    if (int rc = hold_table(c, N, nm, env_starts(s->task, s->signal), s->kp, s->kd, s->pd, s->iters, t)) return rc;
+    Plan p;
+    if (int rc = plan(rec, p)) return rc;
     uint8_t* d = nullptr;
     if (s->mem.zeroed(&d, N)) return REXSIM_ERR_CUDA;
     CK(cudaMemcpy(d, bytes.data(), N, cudaMemcpyHostToDevice));
@@ -959,10 +956,9 @@ int rexsim_set_env_marks(RexSim* s, const int32_t* num_motors) {
     for (size_t e = 0; e < N; e++)
         if (!bytes[e]) for (int j = 0; j < 6; j++) arm_rows[j * N + e] = NAN;
     CK(cudaMemcpy(P.cmd_out + 12 * N, arm_rows.data(), 6 * N * sizeof(float), cudaMemcpyHostToDevice));
-    s->marks = d; s->motors = nm;
+    s->marks = d;
     P.env_mark = d;
-    if (int rc = build_groups(s)) return rc;
-    return apply_holds(s, t, true);
+    return install(s, std::move(rec), p, GROUPS | HOLDS | SETTLE);
 }
 int rexsim_env_mark_buffers(RexSim* s, uint8_t** mark) {
     if (!s || !mark) return fail(REXSIM_ERR_INVALID, "null argument");
@@ -1014,7 +1010,7 @@ int rexsim_env_value_buffers(RexSim* s, float** values, int32_t** pair, float** 
     if (!s || !values || !pair || !gains || !npairs) return fail(REXSIM_ERR_INVALID, "null argument");
     if (!s->values_on) return fail(REXSIM_ERR_INVALID, "per-env values are off (rexsim_set_env_values)");
     *values = s->P.ev.values; *pair = const_cast<int32_t*>(s->P.ev.pair); *gains = const_cast<float*>(s->P.ev.gains);
-    *npairs = s->nholds;
+    *npairs = (int32_t)s->holds.size();
     return REXSIM_OK;
 }
 int64_t rexsim_launch_count(const RexSim* s) { return s ? s->launches : 0; }

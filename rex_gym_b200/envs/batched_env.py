@@ -7,6 +7,7 @@ Reference interface mirrored (same names, argument meaning, error behaviour):
   * gym ids RexWalk-v0 ... rex_gym/playground/__init__.py:17-57 via make()
 One call = one kernel launch for all N environments; there is no CPU fallback.
 """
+import collections
 import ctypes as C
 import functools
 import math
@@ -105,6 +106,9 @@ MAX_GAIN_PAIRS = 64              # REXSIM_MAX_GAIN_PAIRS: the reset hold is sett
 LATENCY_KEYWORDS = ("control_latency", "pd_latency")     # sensor latencies that also take one value per env
 RATE_KEYWORDS = ("control_time_step", "action_repeat")   # the control rate, one value per env over one simulation time step
 MAX_REPEAT_PAIRS = 8             # REXSIM_MAX_REPEAT_PAIRS: distinct (action_repeat, solver_iterations) pairs, one launch each
+# every constructor keyword that takes one value per env
+PER_ENV_KEYWORDS = (TASK_VALUE_KEYWORDS + ("motor_kp", "motor_kd") + LATENCY_KEYWORDS + RATE_KEYWORDS +
+                    ("terrain_type", "task", "signal_type", "mark"))
 
 
 def is_per_env(value):
@@ -123,20 +127,30 @@ def task_value(name, value):
     return float("nan") if value is None else float(value)
 
 
-def _entries(name, value, n):
-    """A per-env keyword -> float64 [n] on the host (None entries as NaN), its length checked."""
+def env_entries(name, value, n, numeric=False, names=None):
+    """The value of keyword `name`, a scalar or one entry per env (is_per_env) -> its n entries: the scalar repeated, or the
+    per-env value with its shape checked.  numeric: float64 [n] on the host, None entries as NaN; otherwise a list, str
+    entries as Python str.  A tensor is read on the host, unless the entries are names (`names`: what they are, for the
+    refusal)."""
+    if not is_per_env(value):
+        return np.full(n, float(value)) if numeric else [value] * n
     if isinstance(value, torch.Tensor):
+        if names:
+            raise ValueError("%s: per-env entries are %s, not a tensor" % (name, names))
         value = value.detach().cpu().numpy()
-    a = np.asarray([np.nan if v is None else v for v in value] if isinstance(value, (list, tuple)) else value, dtype=np.float64)
+    if numeric:
+        a = np.asarray([np.nan if v is None else v for v in value] if isinstance(value, (list, tuple)) else value, np.float64)
+    else:
+        a = np.asarray(list(value) if isinstance(value, (list, tuple)) else value, dtype=object)
     if a.shape != (n,):
-        raise ValueError("%s: expected one value per env (%d), got shape %s" % (name, n, a.shape))
-    return a
+        raise ValueError("%s: expected one %s per env (%d), got shape %s" % (name, "value" if numeric else "entry", n, a.shape))
+    return a if numeric else [str(v) if isinstance(v, str) else v for v in a]
 
 
 def task_value_entries(name, value, n):
     """Per-env values of keyword `name` -> float32 [n], each entry meaning what the scalar means: NaN (or None) draws per reset
     (target_position 0 too, as the scalar), backwards entries are -1 (draw), 0 or 1."""
-    a = _entries(name, value, n)
+    a = env_entries(name, value, n, numeric=True)
     if name == "target_position":
         a = np.where(a == 0, np.nan, a)
     elif name == "backwards":
@@ -159,7 +173,7 @@ def check_env_values(num_envs, values, motor_kp, motor_kd, motor_kp_range=None, 
     if is_per_env(motor_kp) or is_per_env(motor_kd):
         if motor_kp_range is not None or motor_kd_range is not None:
             raise ValueError("per-env motor_kp / motor_kd cannot be combined with motor_kp_range / motor_kd_range")
-        kp, kd = (_entries(k, v, n) if is_per_env(v) else np.full(n, float(v)) for k, v in (("motor_kp", motor_kp), ("motor_kd", motor_kd)))
+        kp, kd = (env_entries(k, v, n, numeric=True) for k, v in (("motor_kp", motor_kp), ("motor_kd", motor_kd)))
         kp, kd = kp.astype(np.float32), kd.astype(np.float32)
         if not (np.isfinite(kp).all() and np.isfinite(kd).all() and (kp >= 0).all() and (kd >= 0).all()):
             raise ValueError("motor_kp / motor_kd: per-env gains must be finite and non-negative")
@@ -182,7 +196,7 @@ def check_env_latencies(num_envs, control_latency, pd_latency, motor_kp=1.0, mot
         return None
     lat = []
     for name, v in (("control_latency", control_latency), ("pd_latency", pd_latency)):
-        a = _entries(name, v, n) if is_per_env(v) else np.full(n, float(v))
+        a = env_entries(name, v, n, numeric=True)
         if not (np.isfinite(a).all() and (a >= 0).all()):
             raise ValueError("%s: per-env latencies must be finite and non-negative" % name)
         lat.append(np.ascontiguousarray(a, np.float64))
@@ -205,41 +219,12 @@ def check_env_terrains(num_envs, terrain_type):
     """The terrain_type keyword, checked before any CUDA call: a scalar, or one entry per env (a list, tuple or ndarray), each
     'plane' or 'random'.  -> (scalar, None) for a scalar or an array whose entries are all equal (the scalar construction);
     (None, int32 [num_envs] of TERRAINS ids) for a batch of both terrains."""
-    if not is_per_env(terrain_type):
-        check_terrain(terrain_type)
-        return terrain_type, None
-    if isinstance(terrain_type, torch.Tensor):
-        raise ValueError("terrain_type: per-env entries are the strings 'plane' / 'random', not a tensor")
-    a = np.asarray(list(terrain_type) if isinstance(terrain_type, (list, tuple)) else terrain_type, dtype=object)
-    if a.shape != (int(num_envs),):
-        raise ValueError("terrain_type: expected one entry per env (%d), got shape %s" % (int(num_envs), a.shape))
-    entries = [str(t) if isinstance(t, str) else t for t in a]
+    entries = env_entries("terrain_type", terrain_type, int(num_envs), names="the strings 'plane' / 'random'")
     for t in entries:
         check_terrain(t)
     if len(set(entries)) == 1:
         return entries[0], None
     return None, np.ascontiguousarray([TERRAINS[t] for t in entries], np.int32)
-
-
-def _rate_entries(name, value, n):
-    """A control_time_step / action_repeat value, scalar or per env -> a list of n Python numbers, each checked: action_repeat
-    a positive integer, control_time_step positive and finite."""
-    if is_per_env(value):
-        if isinstance(value, torch.Tensor):
-            value = value.detach().cpu().numpy()
-        a = np.asarray(list(value) if isinstance(value, (list, tuple)) else value, dtype=object)
-        if a.shape != (n,):
-            raise ValueError("%s: expected one entry per env (%d), got shape %s" % (name, n, a.shape))
-        entries = list(a)
-    else:
-        entries = [value] * n
-    for v in entries:
-        if name == "action_repeat":
-            if isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Integral) or v <= 0:
-                raise ValueError("action_repeat: %r is not a positive integer" % (v,))
-        elif isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Real) or not (math.isfinite(v) and v > 0):
-            raise ValueError("control_time_step: %r is not a positive finite number of seconds" % (v,))
-    return [int(v) if name == "action_repeat" else float(v) for v in entries]
 
 
 def check_env_repeats(num_envs, task, control_time_step, action_repeat, solver_iterations=None):
@@ -261,8 +246,15 @@ def check_env_repeats(num_envs, task, control_time_step, action_repeat, solver_i
         if is_per_env(v) or v:
             return v
         return long if all(long_step) else short if not any(long_step) else [long if ls else short for ls in long_step]
-    cts = _rate_entries("control_time_step", default(control_time_step, 0.006, 0.005), n)
-    rep = _rate_entries("action_repeat", default(action_repeat, 6, 5), n)
+    cts = env_entries("control_time_step", default(control_time_step, 0.006, 0.005), n)
+    for v in cts:
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Real) or not (math.isfinite(v) and v > 0):
+            raise ValueError("control_time_step: %r is not a positive finite number of seconds" % (v,))
+    rep = env_entries("action_repeat", default(action_repeat, 6, 5), n)
+    for v in rep:
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Integral) or v <= 0:
+            raise ValueError("action_repeat: %r is not a positive integer" % (v,))
+    cts, rep = [float(v) for v in cts], [int(v) for v in rep]
     steps = sorted({c / r for c, r in zip(cts, rep)})
     if len(steps) > 1:
         raise ValueError("control_time_step / action_repeat: the envs' simulation time steps differ (%s s); the observation "
@@ -302,15 +294,7 @@ def _same_box(a, b):
 
 def _name_entries(name, value, names, n):
     """A task / signal_type keyword, scalar or per env -> a list of n names, each one of `names`."""
-    if is_per_env(value):
-        if isinstance(value, torch.Tensor):
-            raise ValueError("%s: per-env entries are names, not a tensor" % name)
-        a = np.asarray(list(value) if isinstance(value, (list, tuple)) else value, dtype=object)
-        if a.shape != (n,):
-            raise ValueError("%s: expected one entry per env (%d), got shape %s" % (name, n, a.shape))
-        entries = [str(v) if isinstance(v, str) else v for v in a]
-    else:
-        entries = [value] * n
+    entries = env_entries(name, value, n, names="names")
     for v in entries:
         if not isinstance(v, str) or v not in names:
             raise ValueError("unknown %s %r (have %s)" % (name, v, sorted(names)))
@@ -321,16 +305,7 @@ def check_env_marks(num_envs, mark):
     """The mark keyword, checked before any CUDA call: a scalar, or one entry per env (a list, tuple or ndarray), each 'base'
     or 'arm'.  -> (scalar, None) for a scalar or an array whose entries are all equal (the scalar construction); (None,
     int32 [num_envs] of each env's motor count, 12 or 18) for a batch of both marks."""
-    n = int(num_envs)
-    if is_per_env(mark):
-        if isinstance(mark, torch.Tensor):
-            raise ValueError("mark: per-env entries are the strings 'base' / 'arm', not a tensor")
-        a = np.asarray(list(mark) if isinstance(mark, (list, tuple)) else mark, dtype=object)
-        if a.shape != (n,):
-            raise ValueError("mark: expected one entry per env (%d), got shape %s" % (n, a.shape))
-        entries = [str(m) if isinstance(m, str) else m for m in a]
-    else:
-        entries = [mark]
+    entries = env_entries("mark", mark, int(num_envs), names="the strings 'base' / 'arm'")
     if any(not isinstance(m, str) or m not in MARKS for m in entries):
         raise ValueError("mark must be 'base' or 'arm'")          # mark_constants.py:1
     if len(set(entries)) == 1:
@@ -367,6 +342,20 @@ def check_env_tasks(num_envs, task, signal_type, time_step=0.001, normalize=Fals
         return pairs[0][0], pairs[0][1], None
     ids = (np.ascontiguousarray([TASKS[t] for t in tasks], np.int32), np.ascontiguousarray([SIGNALS[g] for g in signals], np.int32))
     return tuple(tasks), tuple(signals), ids
+
+
+# The optional per-env device blocks besides the values block: the attribute that views it, its state_dict key, the noun and
+# the entries named when a checkpoint's differ, the library call that hands it out (`depth`: it also reports an int32) and
+# the view's rows and element type.  Checkpoints compare them in this order.
+_EnvBlock = collections.namedtuple("_EnvBlock", "attr key noun entries call depth rows typestr")
+_ENV_BLOCKS = (
+    _EnvBlock("_marks", "env_marks", "marks", "marks", "rexsim_env_mark_buffers", False, 1, "|u1"),
+    _EnvBlock("_tasks", "env_tasks", "tasks", "tasks or signals", "rexsim_env_task_buffers", False, 2, "|u1"),
+    _EnvBlock("_repeats", "env_repeats", "control rates", "action repeats or solver iterations", "rexsim_env_repeat_buffers",
+              False, 2, "<i4"),
+    _EnvBlock("_terrain", "env_terrain", "terrains", "terrains", "rexsim_env_terrain_buffers", True, 1, "|u1"),
+    _EnvBlock("_latency", "env_latency", "latencies", "latencies", "rexsim_env_latency_buffers", True, 2, "<f8"),
+)
 
 
 class _Info(object):
@@ -451,31 +440,24 @@ class BatchedRexEnv(object):
           byte (truncated(), info[i]['TimeLimit.truncated'] as gym's TimeLimit adds it).  Off by default: no extra buffer, and
           info[i] is {'action': ...}.
 
-        terrain_type: 'plane', 'random', or one of them per env (a list, tuple or ndarray of num_envs entries).  Env e of a
-          batch of both runs exactly as env e of the batch built with its entry as the scalar: its own ground, friction and
-          field sequence from the one num_fields bank.  Each step launches the plane envs and the heightfield envs as two slot
-          ranges of the batch, each with its terrain's kernel build.  All-equal entries build the scalar construction.
-
-        control_time_step, action_repeat: each a scalar or one entry per env.  Env e runs exactly as the batch built with
-          (control_time_step[e], action_repeat[e]) as scalars: action_repeat[e] sub-steps per control step, each PGS solve
-          capped at solver_iterations (None: int(300 / action_repeat[e])).  Every control_time_step[e] / action_repeat[e]
-          must be the same simulation time step, which the observation space depends on.  Each (terrain, action_repeat,
-          solver_iterations) group of envs is one slot range of the batch, launched with its own values; at most 8 distinct
-          rates.  All-equal entries build the scalar construction.
-
-        task, signal_type: each a scalar or one entry per env.  Env e runs exactly as the batch built with (task[e],
-          signal_type[e]) as scalars, its defaults included (a default control rate of 6 ms / 6 for gallop and poses, 5 ms / 5
-          otherwise).  The envs' spaces must be the same, as the reference's BatchEnv requires: turn ik with turn ol, standup
-          with poses, and under normalize walk ik with turn.  Each (terrain, step-kernel unit, rate) group of envs is one
-          slot range of the batch, launched with its own task; at most 16 groups.  All-equal entries build the scalar
-          construction.
-
-        mark: 'base', 'arm', or one of them per env.  Env e of a batch of both runs exactly as env e of the batch built with
-          its entry as the scalar: its own robot, reset hold and sensor history.  The spaces agree for every task but gallop,
-          which the arm is not built for.  A batch of both is built on the arm's tables, which serve the base envs too; each
-          (terrain, mark, step-kernel unit, rate) group of envs is one slot range of the batch, launched with its mark's
-          build.  num_motors is 18 there, the width of last_command(); a base env's rows 12..17 are NaN, and its
-          info[i]['action'] has its own 12 entries.  All-equal entries build the scalar construction."""
+        The keywords of PER_ENV_KEYWORDS take a scalar or one entry per env (a list, tuple or ndarray of num_envs entries).
+        Entry e builds env e exactly as the batch built with that entry as the scalar would, and entries that are all equal
+        build the scalar construction.  Each step launches every (terrain, mark, step-kernel unit, rate) group of envs as one
+        slot range of the batch with its own values and kernel build, at most 16 groups; the reset hold is settled once per
+        distinct hold setting, at most 64.
+        target_position ... base_yaw: the task values, which set_task_values changes later.
+        motor_kp, motor_kd: the gains; not with motor_kp_range / motor_kd_range.
+        control_latency, pd_latency: the sensor latencies.
+        terrain_type: 'plane' or 'random': the env's ground, friction and field sequence from the one num_fields bank.
+        control_time_step, action_repeat: every control_time_step[e] / action_repeat[e] must be the one simulation time step,
+          which the observation space depends on; each PGS solve is capped at solver_iterations (None: int(300 /
+          action_repeat[e])); at most 8 distinct rates.
+        task, signal_type: the env's defaults included (a control rate of 6 ms / 6 for gallop and poses, 5 ms / 5 otherwise).
+          The envs' spaces must be the same, as the reference's BatchEnv requires: turn ik with turn ol, standup with poses,
+          and under normalize walk ik with turn.
+        mark: 'base' or 'arm': the env's robot, reset hold and sensor history; every task but gallop, which the arm is not
+          built for.  A batch of both is built on the arm's tables, which serve the base envs too: num_motors is 18, the
+          width of last_command(), a base env's rows 12..17 are NaN, and its info[i]['action'] has its own 12 entries."""
         if urdf_version is not None and urdf_version != DEFAULT_URDF_VERSION:
             raise ValueError("%s is not a supported urdf_version." % urdf_version)     # rex_gym_env.py:317-318
         n_envs = int(num_envs)
@@ -643,28 +625,15 @@ class BatchedRexEnv(object):
             _capi.check(self._L.rexsim_env_value_buffers(self._h, C.byref(p), C.byref(q), C.byref(g), C.byref(npairs)))
             self._values = dict(values=view(p, (len(TASK_VALUE_KEYWORDS) + 1, N), "<f4"), pair=view(q, (N,), "<i4"),
                                 gains=view(g, (npairs.value, 2), "<f4"))
-        self._terrain = None                 # [N] u8: each env's TERRAINS id (per-env terrains only)
-        if env_terrain is not None:
-            nplane = C.c_int32()
-            _capi.check(self._L.rexsim_env_terrain_buffers(self._h, C.byref(p), C.byref(nplane)))
-            self._terrain = view(p, (N,), "|u1")
-        self._repeats = None                 # [2][N] i32: each env's action_repeat, solver_iterations (per-env rates only)
-        if env_repeats is not None:
-            _capi.check(self._L.rexsim_env_repeat_buffers(self._h, C.byref(p)))
-            self._repeats = view(p, (2, N), "<i4")
-        self._tasks = None                   # [2][N] u8: each env's TASKS and SIGNALS id (per-env tasks only)
-        if env_tasks is not None:
-            _capi.check(self._L.rexsim_env_task_buffers(self._h, C.byref(p)))
-            self._tasks = view(p, (2, N), "|u1")
-        self._marks = None                   # [N] u8: 1 for each arm env, 0 for each base env (per-env marks only)
-        if env_marks is not None:
-            _capi.check(self._L.rexsim_env_mark_buffers(self._h, C.byref(p)))
-            self._marks = view(p, (N,), "|u1")
-        self._latency = None                 # [2][N] f64: each env's control_latency, pd_latency (per-env latencies only)
-        if env_latency is not None:
-            depth = C.c_int32()
-            _capi.check(self._L.rexsim_env_latency_buffers(self._h, C.byref(p), C.byref(depth)))
-            self._latency = view(p, (2, N), "<f8")
+        # _marks [N] u8: 1 for each arm env, 0 for each base env; _tasks [2][N] u8: each env's TASKS and SIGNALS id; _repeats
+        # [2][N] i32: each env's action_repeat, solver_iterations; _terrain [N] u8: each env's TERRAINS id; _latency [2][N]
+        # f64: each env's control_latency, pd_latency.  None when the keyword is not per env.
+        given = dict(_marks=env_marks, _tasks=env_tasks, _repeats=env_repeats, _terrain=env_terrain, _latency=env_latency)
+        for b in _ENV_BLOCKS:
+            setattr(self, b.attr, None)
+            if given[b.attr] is not None:
+                _capi.check(getattr(self._L, b.call)(self._h, C.byref(p), *((C.byref(C.c_int32()),) if b.depth else ())))
+                setattr(self, b.attr, view(p, (N,) if b.rows == 1 else (b.rows, N), b.typestr))
         self._episode = None
         if episode_statistics:
             o, sm, blk, nb = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int64()
@@ -867,47 +836,22 @@ class BatchedRexEnv(object):
             sd[k] = v.clone()
         if self._values is not None:
             sd.update(("env_" + k, v.clone()) for k, v in self._values.items())
-        if self._latency is not None:
-            sd["env_latency"] = self._latency.clone()
-        if self._terrain is not None:
-            sd["env_terrain"] = self._terrain.clone()
-        if self._repeats is not None:
-            sd["env_repeats"] = self._repeats.clone()
-        if self._tasks is not None:
-            sd["env_tasks"] = self._tasks.clone()
-        if self._marks is not None:
-            sd["env_marks"] = self._marks.clone()
+        for b in _ENV_BLOCKS:
+            if getattr(self, b.attr) is not None:
+                sd[b.key] = getattr(self, b.attr).clone()
         return sd
 
     def load_state_dict(self, sd):
-        if (self._marks is None) != ("env_marks" not in sd):
-            raise ValueError("per-env marks: the checkpoint %s them, this batch %s" %
-                             (("has", "does not") if self._marks is None else ("lacks", "has")))
-        if self._marks is not None and not torch.equal(self._marks, sd["env_marks"].to(self._marks.device)):
-            raise ValueError("per-env marks: the checkpoint's marks differ from this batch's")
-        if (self._tasks is None) != ("env_tasks" not in sd):
-            raise ValueError("per-env tasks: the checkpoint %s them, this batch %s" %
-                             (("has", "does not") if self._tasks is None else ("lacks", "has")))
-        if self._tasks is not None and not torch.equal(self._tasks, sd["env_tasks"].to(self._tasks.device)):
-            raise ValueError("per-env tasks: the checkpoint's tasks or signals differ from this batch's")
-        if (self._repeats is None) != ("env_repeats" not in sd):
-            raise ValueError("per-env control rates: the checkpoint %s them, this batch %s" %
-                             (("has", "does not") if self._repeats is None else ("lacks", "has")))
-        if self._repeats is not None and not torch.equal(self._repeats, sd["env_repeats"].to(self._repeats.device)):
-            raise ValueError("per-env control rates: the checkpoint's action repeats or solver iterations differ from this batch's")
-        if (self._terrain is None) != ("env_terrain" not in sd):
-            raise ValueError("per-env terrains: the checkpoint %s them, this batch %s" %
-                             (("has", "does not") if self._terrain is None else ("lacks", "has")))
-        if self._terrain is not None and not torch.equal(self._terrain, sd["env_terrain"].to(self._terrain.device)):
-            raise ValueError("per-env terrains: the checkpoint's terrains differ from this batch's")
-        if (self._latency is None) != ("env_latency" not in sd):
-            raise ValueError("per-env latencies: the checkpoint %s them, this batch %s" %
-                             (("has", "does not") if self._latency is None else ("lacks", "has")))
-        if self._latency is not None and not torch.equal(self._latency, sd["env_latency"].to(self._latency.device)):
-            raise ValueError("per-env latencies: the checkpoint's latencies differ from this batch's")
-        if (self._values is None) != ("env_values" not in sd):
-            raise ValueError("per-env values: the checkpoint %s them, this batch %s" %
-                             (("has", "does not") if self._values is None else ("lacks", "has")))
+        def present(noun, block, key):
+            if (block is None) != (key not in sd):
+                raise ValueError("per-env %s: the checkpoint %s them, this batch %s" %
+                                 ((noun,) + (("has", "does not") if block is None else ("lacks", "has"))))
+        for b in _ENV_BLOCKS:
+            block = getattr(self, b.attr)
+            present(b.noun, block, b.key)
+            if block is not None and not torch.equal(block, sd[b.key].to(block.device)):
+                raise ValueError("per-env %s: the checkpoint's %s differ from this batch's" % (b.noun, b.entries))
+        present("values", self._values, "env_values")
         if self._values is not None:
             for k in ("gains", "pair"):       # the settled snapshots belong to this handle's pairs
                 if not torch.equal(self._values[k], sd["env_" + k].to(self._values[k].device)):
@@ -933,9 +877,9 @@ class BatchedRexEnv(object):
         motor_kp / motor_kd, given one value per env)."""
         bad = sorted(set(values) - set(TASK_VALUE_KEYWORDS))
         if bad:
-            raise ValueError("set_task_values takes %s; not %s (the gains, latencies, control rates and terrains are fixed at "
-                             "construction)" %
-                             (TASK_VALUE_KEYWORDS, bad))
+            fixed = tuple(k for k in PER_ENV_KEYWORDS if k not in TASK_VALUE_KEYWORDS)
+            raise ValueError("set_task_values takes %s; not %s (the gains, latencies, tasks, marks, control rates and terrains "
+                             "are fixed at construction: %s)" % (TASK_VALUE_KEYWORDS, bad, fixed))
         if self._values is None:
             raise ValueError("per-env values are off: build the batch with one value per env for a task keyword")
         idx = None if indices is None else self._indices(indices, "set_task_values")

@@ -55,10 +55,10 @@ def make_sharded_env(global_envs, rank=None, world=None, **kwargs):
         rank = dist.get_rank() if dist.is_initialized() else 0
     if world is None:
         world = dist.get_world_size() if dist.is_initialized() else 1
-    from .envs.batched_env import LATENCY_KEYWORDS, RATE_KEYWORDS, TASK_VALUE_KEYWORDS, is_per_env
+    from .envs.batched_env import PER_ENV_KEYWORDS, is_per_env
     off, n = shard_range(global_envs, rank, world)
     # per-env constructor values of the whole batch: this rank's slice
-    for k in TASK_VALUE_KEYWORDS + ("motor_kp", "motor_kd", "terrain_type", "task", "signal_type", "mark") + LATENCY_KEYWORDS + RATE_KEYWORDS:
+    for k in PER_ENV_KEYWORDS:
         if k in kwargs and is_per_env(kwargs[k]) and len(kwargs[k]) == global_envs:
             kwargs[k] = kwargs[k][off:off + n]
     return BatchedRexEnv(num_envs=n, env_offset=off, **kwargs)

@@ -14,6 +14,9 @@ turn-ik on the random heightfields and standup with the arm, with the default ca
 every network of tests/agent_twin.FF_ROWS in its precision at the feed-forward batch sizes, on agent_twin.ff_setup's inputs
 (perform's four outputs, noise-free and sampled), the filter update (whole batch and partial + finalize: filter state and
 counters) and the reward transform, and the three scans on seeded inputs.
+Then the mixed batches of the per-env keywords (mixed_cases, as tests/test_gpu_env_*.py build them, up to the 16-group and
+64-setting caps): the launch groups' words, the slot buffers, the hold table, the latency buffer and the launch count after
+construction, then every output of 30 steps after a full reset and the state and ring words after them.
 Every later library is compared with the first: each array that is not bit-identical is reported, and for a frame the number
 of pixels that differ."""
 import hashlib
@@ -37,6 +40,80 @@ def cases():
     out.append(("turn-ik-random-n16897", "turn", None, 16897,
                 dict(signal_type="ik", seed=13, max_episode_steps=15, terrain_type="random", num_fields=64)))
     return out
+
+
+def mixed_cases():
+    """(case id, task, n, action bound, keywords) of mixed batches: each per-env keyword alone, then together, at the caps."""
+    gains = [(1.0, 0.02), (1.3, 0.03), (0.8, 0.015)]
+    cyc = lambda vals, n, k=1: [vals[(e // k) % len(vals)] for e in range(n)]
+    cfg = dict(seed=13, max_episode_steps=15, num_fields=4)
+    out = [("mixed-values", "walk", 24, 0.4, dict(cfg, target_position=cyc([None, 1.5, 3.0], 24), backwards=cyc([None, 0, 1], 24, 2),
+                                                   motor_kp=[g[0] for g in cyc(gains, 24, 3)], motor_kd=[g[1] for g in cyc(gains, 24, 3)])),
+           ("mixed-latencies", "walk", 27, 0.4, dict(cfg, control_latency=cyc([0.0, 0.0105, 0.02], 27), pd_latency=cyc([0.0, 0.0005, 0.001], 27, 3),
+                                                      motor_kp=[g[0] for g in cyc(gains, 27, 9)], motor_kd=[g[1] for g in cyc(gains, 27, 9)])),
+           ("mixed-terrains", "walk", 27, 0.4, dict(cfg, terrain_type=cyc(["plane", "random", "random"], 27), pd_latency=cyc([0.0, 0.001], 27))),
+           ("mixed-repeats", "gallop", 24, 0.3, dict(cfg, signal_type="ol", control_time_step=cyc([0.005, 0.006, 0.010], 24),
+                                                      action_repeat=cyc([5, 6, 10], 24), terrain_type=cyc(["plane", "random"], 24, 4))),
+           ("mixed-tasks-turn", "turn", 24, 0.01, dict(cfg, signal_type=cyc(["ik", "ol"], 24), terrain_type=cyc(["plane", "random"], 24, 3))),
+           ("mixed-tasks-walk-turn", None, 24, 1.0, dict(cfg, normalize=True, task=cyc(["walk", "turn", "turn"], 24),
+                                                          signal_type=cyc(["ik", "ik", "ol"], 24))),
+           ("mixed-tasks-standup-poses", None, 24, 0.1, dict(cfg, task=cyc(["standup", "poses", "standup"], 24), signal_type=cyc(["ol", "ik", "ik"], 24),
+                                                              motor_kp=[g[0] for g in cyc(gains, 24, 2)], motor_kd=[g[1] for g in cyc(gains, 24, 2)])),
+           ("mixed-marks", "walk", 24, 0.4, dict(cfg, mark=cyc(["base", "arm"], 24, 5), pd_latency=cyc([0.0, 0.001], 24, 3),
+                                                  observation_noise_stdev=(0.01, 0.01, 0.01, 0.01, 0.01)))]
+    # the 16 groups of the cap: 2 terrains x 2 marks x 2 rates x 2 step units
+    combos = [(t, m, r, sg) for t in ("plane", "random") for m in ("base", "arm") for r in ((0.005, 5), (0.010, 10)) for sg in ("ik", "ol")]
+    labels = [combos[(i + i // 16) % 16] for i in range(64)]
+    out.append(("mixed-16-groups", "turn", 64, 0.01, dict(cfg, terrain_type=[l[0] for l in labels], mark=[l[1] for l in labels],
+                                                          control_time_step=[l[2][0] for l in labels],
+                                                          action_repeat=[l[2][1] for l in labels], signal_type=[l[3] for l in labels])))
+    # the 64 hold settings of the cap: 8 gains x 2 marks x 2 PD latencies x 2 start poses, on both terrains
+    out.append(("mixed-64-settings", None, 128, 0.1, dict(cfg, task=cyc(["standup", "poses"], 128, 64), signal_type="ol",
+                                                          motor_kp=cyc([1.0 + 0.01 * k for k in range(8)], 128),
+                                                          mark=cyc(["base", "arm"], 128, 16), pd_latency=cyc([0.0, 0.001], 128, 32),
+                                                          terrain_type=cyc(["plane", "random"], 128, 3))))
+    return out
+
+
+def mixed_run(R, res):
+    """mixed_cases: what the handle holds after construction, then 30 steps after a full reset."""
+    import ctypes as C
+    import torch
+    from rex_gym_b200 import _capi
+    _force_build(None)
+    for cid, task, n, b, kw in mixed_cases():
+        env = R.BatchedRexEnv(num_envs=n, auto_reset=True, **(dict(task=task) if task else {}), **kw)
+        L, h = env._L, env._h
+        view = lambda p, shape, typestr: _capi.device_view(p.value, shape, typestr, env, "cuda").cpu().numpy()
+        rec = res[cid] = {"launch_count": str(env.launch_count)}
+
+        def groups(when):
+            words = []
+            for g in range(L.rexsim_launch_groups(h)):
+                info, t, sg, m = np.zeros(8, np.int32), C.c_int32(), C.c_int32(), C.c_int32()
+                assert L.rexsim_launch_group(h, g, info.ctypes.data) == 0
+                assert L.rexsim_launch_group_task(h, g, C.byref(t), C.byref(sg)) == 0
+                assert L.rexsim_launch_group_mark(h, g, C.byref(m)) == 0
+                words.append(info.tolist() + [t.value, sg.value, m.value])
+            rec[when + "_groups"] = digest(np.array(words, np.int32))
+        groups("built")
+        p, q, g, k = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_int32()
+        assert L.rexsim_slot_buffers(h, C.byref(p), C.byref(q)) == 0
+        rec["perm"] = digest(view(p, (n,), "<i4")) if p.value else "identity"
+        rec["group"] = digest(view(q, (n,), "|u1")) if q.value else "one group"
+        if env._values is not None:
+            assert L.rexsim_env_value_buffers(h, C.byref(p), C.byref(q), C.byref(g), C.byref(k)) == 0
+            rec["pair"], rec["gains"], rec["npairs"] = digest(view(q, (n,), "<i4")), digest(view(g, (k.value, 2), "<f4")), str(k.value)
+        if env._latency is not None:
+            assert L.rexsim_env_latency_buffers(h, C.byref(p), C.byref(k)) == 0
+            rec["latency"], rec["depth"] = digest(view(p, (2, n), "<f8")), str(k.value)
+        env.reset()
+        rng = np.random.default_rng(11)
+        for s in range(30):
+            ret = env.step(torch.as_tensor(rng.uniform(-b, b, size=(n, env.action_dim)).astype(np.float32), device="cuda"))
+            _record(env, rec, s, ret)
+        groups("stepped")
+        env.close()
 
 
 def digest(a):
@@ -158,6 +235,7 @@ def run(out):
             _record(env, rec, k, ret)
         env.close()
     generic_cases(res)
+    mixed_run(R, res)
     frames = {}
     render_cases(R, res, frames)
     agent_cases(res)
